@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- chunks/s and real-time factor of the full encode -> stage 1 -> stage 2 -> vocode path.
 
-  python bench.py --gpus 1 --steps K --warmup W            (driver; N > 1 via torch.distributed.run)
+  python bench.py --gpus 1 --steps K --warmup W [--dump-outputs DIR]   (N > 1 via torch.distributed.run)
   python bench.py --impl reference ...                      (the CPU implementation of the same path)
 
 A "step" is one 0.3 s @ 24 kHz chunk of one audio stream pushed through the device-resident session
@@ -11,6 +11,8 @@ stage-1 / stage-2 U-Nets at base width 64 with seeded synthetic weights; synthet
           (ryk_session_push_device), K consecutive chunks, CUDA events, max over ranks
   e2e   : the same K chunks through ryk_session_push with HOST buffers (H2D + kernels + D2H per step)
 Multi-GPU: one independent stream per rank ("weak"); NCCL only broadcasts the weights at init.
+--dump-outputs DIR writes what the last timed step returned (the output audio of every stream) as DIR/*.npy; inputs and weights
+are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -39,7 +41,7 @@ WORKLOAD = ('single stream per GPU, buffer_time=0.3 s, extras (0,0.5,0), frame_p
             'stage-2 2-D U-Net base 64 on 384x512 (54.4 M params, 142 GFLOP/chunk), WORLD DIO+StoneMask/CheapTrick/D4C + realtime synthesis')
 
 
-# algorithmic work of the stage-2 k4 layers (the tcgen05 kernel launches) for one 384x512 forward, base 64
+# algorithmic work of the stage-2 k4 layers (the wgmma kernel launches) for one 384x512 forward, base 64
 STAGE2_TC_FLOP = None
 
 
@@ -60,7 +62,7 @@ def stage2_tc_flop(Tp=384, base=64):
 # short device-resident legs of BASELINE configs 3 and 5 plus 4 grouped streams of the headline chunk size (buffer_time, streams per GPU, steps)
 EXTRA_LEGS = ((0.1, 1, 20), (1.0, 1, 12), (1.0, 8, 8), (0.3, 4, 12))
 
-DTYPE = ('f64 (WORLD analysis / synthesis, SPTK), f16 operands / f32 accumulate: stage-2 k4 layers on tcgen05, stage-1 k4 layers on mma.sync '
+DTYPE = ('f64 (WORLD analysis / synthesis, SPTK), f16 operands / f32 accumulate: stage-2 k4 layers on wgmma, stage-1 k4 layers on mma.sync '
          'inside the one-launch cluster kernel; f32 CUDA cores (3x3 / k3 edge layers)')
 
 
@@ -71,18 +73,8 @@ def bench_config(workload, B=1):
         timing='CUDA events on the engine stream (forked to / joined from the session streams) around the K pushes, max over ranks',
         pipeline='gate | analysis (2 chunks in flight) | stage 1 | stage 2 | synthesis of consecutive chunks overlap on 6 CUDA streams per audio '
                  'stream, each stage a CUDA graph (the reference overlaps its 3 worker processes); e2e keeps 4 steps in flight',
-        l2='per-step footprint (109 MB fp16 stage-2 weights + 54 MB stage-1 weights + ~100 MB activations) exceeds the 126 MB L2; no explicit flush',
+        l2='per-step footprint (109 MB fp16 stage-2 weights + 54 MB stage-1 weights + ~100 MB activations) exceeds the 50 MB L2; no explicit flush',
         streams_per_gpu=B, silence_threshold_db=THRESHOLD_DB)
-
-
-def stage2_traffic():
-    """DRAM bytes of one stage-2 k4 block from THIS round's ncu capture (tools/ncu_stage2_traffic.py writes the file from the
-    --set full report); None when the capture is absent."""
-    f = ROOT / 'profiles' / 'r02b_stage2_traffic.json'      # this round's latest `--set full` capture (tools/gpu_r02b_final.sh)
-    if not f.exists():
-        return None, None
-    d = json.loads(f.read_text())
-    return float(d['dram_bytes_per_forward']), d.get('source')
 
 
 def measured_peaks():
@@ -94,7 +86,8 @@ def measured_peaks():
         return dict(tflops=float(d['bf16_tflops']), hbm=float(d['hbm_gbs']), burst=float(d['bf16_tflops']),
                     sustained=float(d.get('bf16_tflops_sustained') or d['bf16_tflops']),
                     source='measured (MEASURED_PEAKS.json, cuBLAS bf16 burst; sustained figure in peak_sustained)')
-    return dict(tflops=1590.0, hbm=6650.0, burst=1590.0, sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    return dict(tflops=989.0, hbm=3350.0, burst=989.0, sustained=989.0,
+                source='H100 SXM data sheet, dense FP16 at up to 700 W (not a measured figure)')
 
 
 class ClockSampler(threading.Thread):
@@ -366,6 +359,8 @@ def run_gpu(args):
         clocks = sampler.stop()
         launches = eng.launch_count - launches0
         res = dict(T=T, B=B, Tw=Tw, Tp=Tp, n=n, t_dev=max_over_ranks(t_dev), t_host=t_host, s2_ms=s2_ms, s2_sum=s2_sum, s2_runs=s2_runs, launches=launches, clocks=clocks)
+        r_last = (total - 1) % RING                  # output slots of the last timed step
+        res['last_out'] = [d_out[r_last, j, :int(d_n[r_last, j])].cpu().numpy() for j in range(B)]
 
         # ---- sustained: the same K-step block repeated back to back for >= sustain_s seconds (thermal / power steady state) ----
         if sustain_s > 0:
@@ -444,6 +439,8 @@ def run_gpu(args):
         import torch.distributed as dist
         dist.barrier()
         dist.destroy_process_group()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, main['last_out'], rank)
     if rank != 0:
         return
     peaks = measured_peaks()
@@ -468,7 +465,6 @@ def run_gpu(args):
                 f', buffer_time={T_:g} s, extras (0,0.5,0), frame_period 5 ms, 24 kHz in/out, convert window {Tw_} -> {Tp_} frames, '
                 f'stage-2 input ({B_},1,{Tp_},512), same models as the default workload; one step = one chunk of every stream')
     workload = WORKLOAD if default_workload else workload_of(T, B, Tw, Tp)
-    traffic, traffic_src = stage2_traffic() if default_workload else (None, None)
     line = dict(
         metric=metric, value=value, unit='chunks/s', rtf=value * T, n_gpus=world, steps=args.steps, warmup=args.warmup,
         ms_per_step=1000.0 * main['t_dev'] / args.steps, higher_is_better=True, scaling='weak', vs_baseline=None,
@@ -478,10 +474,8 @@ def run_gpu(args):
                  d2h_bytes_per_step=int(main['produced'] / max(1, args.steps)) * 8 + B * (4 + 8)),
         gpu_launches=int(main['launches']), host_enqueue_ms_per_step=1000.0 * main['t_host'] / args.steps,
         clocks=main['clocks'],
-        roofline=dict(bound='tensor', kernel=('stage-2 k4 layers 1..14: k_conv_tc (tcgen05, one tile per CTA) + k_splitk_reduce for c3-d3' if B == 1 else
-                                              'stage-2 k4 layers 1..14: k_conv_halo (persistent tcgen05, c1-c3 / d3-d6) + k_conv_tc / k_splitk_reduce (c4-d2)'
-                                              ' + the two 3x3 edge layers (group forward timed as a whole)'), achieved=ach, peak=peaks['tflops'],
-                      unit='TFLOP/s', frac=(ach / peaks['tflops']) if ach else None, traffic=traffic, traffic_source=traffic_src,
+        roofline=dict(bound='tensor', kernel='stage-2 k4 layers 1..14: k_conv_tc (TMA + wgmma, one tile per CTA) + k_splitk_reduce for split-K layers',
+                      achieved=ach, peak=peaks['tflops'], unit='TFLOP/s', frac=(ach / peaks['tflops']) if ach else None,
                       peak_source=peaks['source'], peak_burst=peaks['burst'], peak_sustained=peaks['sustained'],
                       flop_per_step=fl, ms_per_step_in_kernel=(main['s2_ms'] / main['s2_runs']) if main['s2_runs'] else None,
                       ms_per_forward_wall=(main['s2_sum'] / main['s2_runs']) if main['s2_runs'] else None,
@@ -518,6 +512,14 @@ def run_gpu(args):
     print(json.dumps(line), flush=True)
 
 
+def dump_outputs(d, outs, rank):
+    """The output audio (float64 samples at 24 kHz) of every stream of this rank's last timed step: DIR/audio_r<rank>_s<stream>.npy."""
+    d = Path(d)
+    d.mkdir(parents=True, exist_ok=True)
+    for j, y in enumerate(outs):
+        np.save(d / f'audio_r{rank}_s{j}.npy', np.asarray(y, dtype=np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
@@ -530,6 +532,7 @@ def main():
     ap.add_argument('--buffer-time', type=float, default=BUFFER_TIME, help='seconds per chunk (default workload: 0.3)')
     ap.add_argument('--sustain', type=float, default=2.0, help='seconds of back-to-back K-step blocks for the `sustained` key (0 = skip)')
     ap.add_argument('--no-extra', action='store_true', help='skip the short BASELINE config 3 / 5 legs (`extra_configs`)')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR', help='write the outputs of the last timed step as DIR/*.npy')
     args = ap.parse_args()
     if args.steps is None:
         args.steps = 20 if args.impl == 'b200' else 6

@@ -1,5 +1,5 @@
 /*
- * ryk.h -- C ABI of libryk.so: the B200-native per-chunk hot path of realtime-yukarin
+ * ryk.h -- C ABI of libryk.so: the H100-native per-chunk hot path of realtime-yukarin
  *          (encode -> stage 1 -> stage 2 -> vocode).  Plain pointers and sizes only.
  *
  * Every entry point replaces one call the reference makes into an un-vendored third-party library
@@ -45,7 +45,7 @@ const char* ryk_last_error(void);
 int ryk_engine_create(int device, ryk_engine** out);
 int ryk_engine_destroy(ryk_engine* e);
 /* 0: FP32 CUDA-core convolutions everywhere (bisecting / numerics reference)
- * 1: FP16 operands + FP32 accumulate on tcgen05 tensor cores for the stage-2 k4 layers (default) */
+ * 1: FP16 operands + FP32 accumulate on the tensor cores (wgmma) for the stage-2 k4 layers (default) */
 int ryk_engine_set_precision(ryk_engine* e, int mode);
 int ryk_engine_get_precision(ryk_engine* e);
 /* FP16 mode: run the stage-1 1-D U-Net (AcousticConverter.convert_from_feature, voice_changer.py:36) as ONE thread-block-cluster
@@ -54,7 +54,7 @@ int ryk_engine_get_precision(ryk_engine* e);
 int ryk_engine_set_stage1_fused(ryk_engine* e, int enable);
 long long ryk_engine_launch_count(ryk_engine* e);        /* kernels launched by this engine so far */
 int ryk_engine_synchronize(ryk_engine* e);
-/* CUDA-event timing of the stage-2 k4-layer block (layers 1..14, the tcgen05 kernels) on the engine's stream */
+/* CUDA-event timing of the stage-2 k4-layer block (layers 1..14, the wgmma kernel) on the engine's stream */
 int ryk_engine_timer_start(ryk_engine* e);                    /* cudaEventRecord on the engine's stream */
 int ryk_engine_timer_stop(ryk_engine* e, float* elapsed_ms);  /* record + synchronize + elapsed */
 int ryk_engine_profile(ryk_engine* e, int enable);
@@ -251,7 +251,7 @@ int ryk_debug_harvest(ryk_engine* e, int n, int fs, double frame_period_ms, doub
  * kernel's phase timeline (31 doubles, us). */
 int ryk_debug_stage1_bench(ryk_engine* e, int Tp, int iters, float* ms_fused, float* ms_layered, double* timeline_us);
 /* One conv (transposed = 0) or transposed-conv layer of the U-Nets in isolation, host fp32 NHWC tensors in and
- * out, weights in the Chainer layout; use_tc selects the FP16 tcgen05 kernel (1) or the FP32 CUDA-core kernel (0).
+ * out, weights in the Chainer layout; use_tc selects the FP16 wgmma kernel (1) or the FP32 CUDA-core kernel (0).
  * `repeat` extra timed runs report the mean device time per run (ms) -- used by the unit parity tests and ncu. */
 int ryk_test_conv_layer(ryk_engine* e, int transposed, int k, int stride, int pad, int B, int Hin, int Win, int C0, int C1, int Cout,
                         const float* in0, const float* in1, const float* W, const float* scale, const float* shift, int act,

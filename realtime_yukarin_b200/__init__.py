@@ -1,5 +1,5 @@
 """realtime_yukarin_b200: the per-chunk hot path of realtime-yukarin (encode -> stage 1 -> stage 2 -> vocode)
-on NVIDIA B200 (sm_100a), behind the reference's Stream / SegmentMethod plugin API and its
+on NVIDIA H100 (sm_90a), behind the reference's Stream / SegmentMethod plugin API and its
 Vocoder / VoiceChanger / AcousticConverter / SuperResolution call surface.  See DESIGN.md.
 
 `import realtime_yukarin_b200.dropin; realtime_yukarin_b200.dropin.install()` registers

@@ -1,4 +1,4 @@
-"""CREPE f0 front-end on the B200: the host mirror of `crepe.predict` / `crepe.predict_voicing` as the reference uses them in
+"""CREPE f0 front-end on the H100: the host mirror of `crepe.predict` / `crepe.predict_voicing` as the reference uses them in
 realtime_voice_conversion/yukarin_wrapper/acoustic_feature_wrapper.py:65-80 (CrepeAcousticFeatureWrapper.extract_f0).
 
     t, f0, confidence, _ = crepe.predict(x, fs, viterbi=True, model_capacity='full', step_size=frame_period, verbose=0)

@@ -144,8 +144,7 @@ const char* ryk_last_error(void) { return g_err.c_str(); }
 int ryk_engine_create(int device, ryk_engine** out) {
   RYK_CHECK(out != nullptr, "null out pointer");
   // A session drives 7 streams and a group of 8 sessions 57: with the default 8 hardware work queues independent streams share a queue
-  // and a stream that waits on an event holds up its queue-mates (measured: the steps of a group of 8 ran strictly one after another,
-  // 1280 chunks/s; with 32 queues they overlap, 1678; profiles/r02b_max_connections_groups.txt).  Read by the driver when the CUDA
+  // and a stream that waits on an event holds up its queue-mates, so the steps of a group run one after another.  Read by the driver when the CUDA
   // context is created, so it only takes effect if nothing initialised CUDA earlier in this process; never overrides the user's value.
   setenv("CUDA_DEVICE_MAX_CONNECTIONS", "32", 0);
   int count = 0;
@@ -154,7 +153,7 @@ int ryk_engine_create(int device, ryk_engine** out) {
   RYK_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   RYK_CUDA(cudaGetDeviceProperties(&prop, device));
-  RYK_CHECK(prop.major == 10, "libryk is built for sm_100a (B200) only");
+  RYK_CHECK(prop.major == 9 && prop.minor == 0, "libryk is built for sm_90a (H100) only");
   ryk_engine* h = new ryk_engine();
   Engine* e = &h->impl;
   e->device = device;
@@ -757,7 +756,7 @@ int ryk_debug_dio(ryk_engine* h, int n, int fs, double fp, double f0_floor, doub
 
 // ---- diagnostics: one conv / transposed-conv layer in isolation (unit parity + profiling) -------
 // in0/in1: host fp32 NHWC [B][Hin][Win][C0|C1]; W: Chainer layout; out: host fp32 NHWC [B][Hout][Wout][Cout].
-// use_tc = 1 runs the FP16 tcgen05 kernel (activations rounded to fp16), 0 the FP32 CUDA-core kernel.
+// use_tc = 1 runs the FP16 wgmma kernel (activations rounded to fp16), 0 the FP32 CUDA-core kernel.
 int ryk_test_conv_layer(ryk_engine* h, int transposed, int k, int stride, int pad, int B, int Hin, int Win, int C0, int C1, int Cout,
                         const float* in0, const float* in1, const float* W, const float* scale, const float* shift, int act,
                         int use_tc, int repeat, float* out, float* ms_per_run) {
@@ -814,11 +813,10 @@ int ryk_test_conv_layer(ryk_engine* h, int transposed, int k, int stride, int pa
     if (n1) k_f32_to_f16<<<1184, 256, 0, st>>>(d_in1, d_h1, n1);
     L.in0 = d_h0; L.in1 = n1 ? d_h1 : nullptr; L.in_dtype = DT_F16; L.out = d_ho; L.out_dtype = DT_F16; L.w_tc = d_wt;
     RYK_CHECK(tc_layer_eligible(L), "layer shape is not eligible for the tensor-core kernel");
-    int num_sms = 148;
+    int num_sms = 132;
     cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, e->device);
     size_t ws = tc_splitk_ws_bytes(L, num_sms);
     if (ws) L.splitk_ws = (float*)A(ws);
-    if (tc_layer_wants_counter(L, num_sms)) { L.t3_ctr = (int*)A(16); RYK_CUDA(cudaMemsetAsync(L.t3_ctr, 0, 16, st)); }
     if (tc_layer_prepare(L, num_sms)) return -1;
     rc = conv_tc_run(L, st);
     if (!rc && repeat > 0) rc = timed_graph([&]() { return conv_tc_run(L, st); });

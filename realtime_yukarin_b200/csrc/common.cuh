@@ -1,4 +1,4 @@
-// common.cuh -- shared declarations for libryk (B200 / sm_100a hot path of realtime-yukarin).
+// common.cuh -- shared declarations for libryk (H100 / sm_90a hot path of realtime-yukarin).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>

@@ -6,7 +6,7 @@
 //   * the first (Cin = 1) and last (Cout = 1) 3x3 layers of the stage-2 2-D U-Net, whose GEMM shape
 //     has nothing for a tensor core to chew on;
 //   * all layers when the engine runs in FP32 "bisect" precision (the numerics reference for the
-//     tcgen05 path in conv_tc.cu).
+//     wgmma path in conv_tc.cu).
 // Tiling: 64 output pixels x 64 output channels per CTA, 16-channel K steps through shared memory,
 // 4x4 register micro-tiles (classic SGEMM shape).  Transposed convs are evaluated per output-parity
 // class so that every pixel of a tile shares the same set of contributing taps.

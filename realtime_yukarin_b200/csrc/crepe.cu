@@ -1,4 +1,4 @@
-// crepe.cu -- the CREPE f0 front-end on the B200 (SURVEY 8(f) rank 4; realtime_voice_conversion/yukarin_wrapper/
+// crepe.cu -- the CREPE f0 front-end on the H100 (SURVEY 8(f) rank 4; realtime_voice_conversion/yukarin_wrapper/
 // acoustic_feature_wrapper.py:65-80: crepe.predict(x, fs, viterbi=True, model_capacity='full', step_size=frame_period) followed by
 // crepe.predict_voicing).  Input is the 16 kHz signal (the caller resamples with ryk_resample_poly); output is the per-frame
 // frequency, confidence and voicing state, plus the 360-bin activation.

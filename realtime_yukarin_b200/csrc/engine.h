@@ -21,7 +21,7 @@ struct Reblock;
 struct Engine {
   int device = 0;
   cudaStream_t stream = nullptr;
-  int precision = 1;                 // 0: FP32 CUDA-core convs everywhere, 1: FP16 tcgen05 tensor-core convs where eligible
+  int precision = 1;                 // 0: FP32 CUDA-core convs everywhere, 1: FP16 wgmma tensor-core convs where eligible
   int f0_method = 0;                 // 0: DIO + StoneMask, 1: Harvest + StoneMask (world_harvest.cu)
   bool s1_fused = true;              // FP16 mode: stage 1 as ONE cluster kernel (s1_fused.cu) instead of 16 layer launches
   // FFT twiddles

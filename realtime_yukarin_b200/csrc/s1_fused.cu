@@ -7,7 +7,7 @@
 //     co-scheduled by the hardware, so there is no software grid barrier that could dead-lock on a full GPU, and the kernel occupies
 //     only `cluster size` SMs next to the stage-2 tensor-core kernels of the neighbouring chunks;
 //   * each k4 layer is a skinny GEMM out[m][n] = sum_k A[m][k] W[n][k] (s1_map.h) on mma.sync m16n8k16 (FP16 in, FP32 accumulate:
-//     same operand precision as the tcgen05 path it replaces; M is 3..320 rows, far below a 128-row UMMA tile);
+//     same operand precision as the wgmma path it replaces; M is 3..320 rows, far below a 128-row tile);
 //   * weights are pre-packed in B-fragment order, so a warp streams its share with coalesced 16-byte loads straight into the mma
 //     operands, every weight byte exactly once per M slab; the blocks a CTA will need three layers later are requested into L2 with
 //     cp.async.bulk.prefetch.L2, which keeps HBM busy across the layer barriers;

@@ -14,7 +14,7 @@
 // Pipelining = what run.py does with three OS processes and queues (run.py:58-93), done with streams and events:
 //   stream E: slide wave, silence gate (needs only the samples), DIO/StoneMask/CheapTrick/D4C          of chunk k+1
 //   stream C: slide features, stage-1 U-Net (+f0 map), mc2sp                                          of chunk k
-//   stream C2: stage-2 U-Net (the tcgen05 layers)                                                     of chunk k-1
+//   stream C2: stage-2 U-Net (the wgmma layers)                                                     of chunk k-1
 //   stream D: slide converted features, synthesizer add/plan/pulse/overlap-add, NaN scrub             of chunk k-2
 // Inter-stage buffers are double-buffered (index = step parity); events order producer/consumer and guard reuse.
 // The only host<->device handshake inside a step is the 8-byte effective-frame count that selects the stage-1
@@ -307,7 +307,7 @@ int session_streams_join(Engine* e) {
 // padded effective length), so each variant is stream-captured once and replayed: a step costs ~6 graph launches on
 // the host instead of ~90 kernel launches (the host was the bottleneck at 0.75 ms of launch overhead per 0.78 ms step).
 // RYK_SESSION_SKIP (timing experiments only; results are garbage): bit 0 analysis (E2), 1 stage 1, 2 stage-2 layers 1..14, 3 synthesis
-// Compiled in only with -DRYK_DIAG (tools/gpu_skip_sweep.sh builds a separate diagnostics library): a release libryk.so has no
+// Compiled in only with -DRYK_DIAG (RYK_NVCC_EXTRA=-DRYK_DIAG builds a separate diagnostics library): a release libryk.so has no
 // knob that can turn the timed path into a partial one.
 static int session_skip_mask() {
 #ifdef RYK_DIAG
@@ -540,7 +540,7 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
   return 0;
 }
 
-// single session: stage-2 layers 1..14 (the tcgen05 layers) on the session's own stream
+// single session: stage-2 layers 1..14 (the wgmma layers) on the session's own stream
 static int session_mid_single(Engine* e, Session* s, bool was_profiling) {
   STEP_LOCALS
   S2_LOCALS

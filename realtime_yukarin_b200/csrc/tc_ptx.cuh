@@ -1,5 +1,5 @@
-// tc_ptx.cuh -- inline-PTX wrappers shared by the tcgen05 convolution kernels (conv_tc.cu: one CTA per tile;
-// conv_tc2.cu: CTA pairs, cta_group::2): mbarriers, TMA loads, UMMA issue / commit, smem descriptors, PDL.
+// tc_ptx.cuh -- inline-PTX wrappers of the Hopper (sm_90a) tensor-core convolution kernel (conv_tc.cu): mbarriers, TMA loads,
+// warpgroup MMA (wgmma) issue / commit / wait, shared-memory matrix descriptors, thread-block clusters, PDL.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -8,23 +8,22 @@ namespace ryk {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;          // fp16 elements = 128 bytes = one swizzle row
-constexpr int kUmmaK = 16;
-constexpr int kTcThreads = 192;
+constexpr int kMmaK = 16;           // K of one wgmma.m64nNk16
+constexpr int kTcConsumers = 256;   // two consumer warpgroups, 64 accumulator rows (pixels) each
+constexpr int kTcThreads = kTcConsumers + 32;   // + one TMA producer warp
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // Programmatic dependent launch: every kernel of a U-Net forward is a dependent of the one before it in the stream.
 // pdl_trigger() lets the NEXT kernel's CTAs be scheduled as soon as all CTAs of this grid have started (they run their
-// prologue -- barrier init, TMEM allocation, tensor-map prefetch, scale/shift staging -- in the shadow of this grid's
+// prologue -- barrier init, tensor-map prefetch, scale/shift staging -- in the shadow of this grid's
 // tail); pdl_wait() blocks until the PREVIOUS grid has completed and its memory is visible, and must precede every
 // access to activations / workspaces.  Both are no-ops for launches without the programmatic attribute.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// One elected lane of a fully active warp.  The TMA / MMA issuing warps run their loops WARP-UNIFORMLY (all 32 lanes compute the same
-// coordinates and descriptors) and guard only the issuing instruction with elect_one(): ptxas then keeps the operands in uniform
-// registers.  Issuing from an `if (lane == 0)` region instead makes it wrap EVERY UTCHMMA / UTMALDG in an ELECT + 5 x R2UR.BROADCAST +
-// BRA.U.ANY loop (~100 clocks per instruction: the tensor pipe then runs at ~60 % behind its issuer -- profiles/r02_halo_timeline.txt).
+// One elected lane of a fully active warp.  The TMA producer warp runs its loop WARP-UNIFORMLY (all 32 lanes compute the same
+// coordinates) and guards only the issuing instructions with elect_one(), so ptxas keeps the coordinates in uniform registers.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
@@ -36,6 +35,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
@@ -58,16 +60,45 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// ---- warpgroup MMA (sm_90a): D[64 x N] (fp32 registers of the 128 threads of a warpgroup) += A[64 x 16] * B[16 x N]^T, both operands
+// fp16 K-major in shared memory.  Accumulator fragment of thread t (warp w = t / 32, lane l), register i:
+//   row = 16 w + l / 4 + 8 ((i >> 1) & 1),  column = 8 (i >> 2) + 2 (l % 4) + (i & 1).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R> __device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(1));
+}
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(1));
+}
+// the same 2-D box into the same shared-memory offset of every CTA of the cluster in `mask`; each CTA's mbarrier at `bar`'s offset
+// receives the transaction bytes of its copy
+__device__ __forceinline__ void tma_load_2d_multicast(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask) : "memory");
+}
+// arrive on an mbarrier of another CTA of the cluster (shared::cluster address from cluster_map_rank)
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
 // thread-block clusters: shared::cluster address of a CTA-local shared address in CTA `rank`, cluster rank, cluster-wide barrier
 __device__ __forceinline__ uint32_t cluster_map_rank(uint32_t smem_addr, uint32_t rank) {
@@ -86,13 +117,14 @@ __device__ __forceinline__ float4 ld_cluster_f4(uint32_t addr) {
   return v;
 }
 
-// K-major, 128B-swizzled operand: 8-row atoms of 1024 B (SBO), LBO unused, descriptor version 1 (sm_100)
+// K-major, 128B-swizzled operand (the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_128B): 8-row atoms of 1024 B (stride byte
+// offset), leading byte offset unused, layout type 1 = 128B swizzle.  Advancing K by 16 fp16 inside the atom adds 32 B (+2).
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+  d |= (uint64_t)1 << 16;
   d |= (uint64_t)((1024u >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
 

@@ -98,7 +98,7 @@ int unet_set_layer(Engine* e, UNet* n, int idx, const float* W, const float* sca
   return 0;
 }
 
-// Plan for a (batch, H, W) input; H = 1 for 1-D nets. precision: 0 = FP32 everywhere, 1 = FP16 activations + tcgen05.
+// Plan for a (batch, H, W) input; H = 1 for 1-D nets. precision: 0 = FP32 everywhere, 1 = FP16 activations + wgmma.
 int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPlan** out, int owner) {
   for (auto& L : n->layers) RYK_CHECK(L.loaded, "U-Net layer weights not loaded");
   auto key = std::make_tuple(B, H, W, precision, owner);
@@ -107,7 +107,7 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
   RYK_CHECK(W % 128 == 0 && (n->ndim == 1 || H % 128 == 0), "U-Net input extent must be a multiple of 128");
   UNetPlan* p = new UNetPlan();
   p->B = B; p->H = H; p->W = W; p->precision = precision;
-  int num_sms = 148;
+  int num_sms = 132;
   cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, e->device);
   const int act_dt = precision ? DT_F16 : DT_F32;
   const size_t esz = precision ? 2 : 4;
@@ -157,7 +157,6 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
     if (precision == 1 && L.w_tc && tc_layer_eligible(L)) {
       size_t ws = tc_splitk_ws_bytes(L, num_sms);
       if (ws) { void* w = nullptr; if (alloc(ws, &w)) return -1; L.splitk_ws = (float*)w; }
-      if (tc_layer_wants_counter(L, num_sms)) { void* c = nullptr; if (alloc(16, &c)) return -1; L.t3_ctr = (int*)c; }
       if (tc_layer_prepare(L, num_sms)) return -1;
     }
   }

@@ -1,4 +1,4 @@
-// world_analysis.cu -- WORLD analysis on the B200: DIO + StoneMask (f0), CheapTrick (spectral
+// world_analysis.cu -- WORLD analysis on the H100: DIO + StoneMask (f0), CheapTrick (spectral
 // envelope, fused with SPTK sp2mc), D4C (aperiodicity).  Replaces the CPU pyworld/pysptk calls
 // reached from realtime_voice_conversion/yukarin_wrapper/vocoder.py:26-48 ->
 // acoustic_feature_wrapper.py:28-33 -> yukarin.AcousticFeature.extract (SURVEY rows a6, A-E).

@@ -1,4 +1,4 @@
-// world_harvest.cu -- WORLD Harvest f0 extraction on the B200 (pyworld.harvest; the f0 hook of yukarin.AcousticFeature.extract reached
+// world_harvest.cu -- WORLD Harvest f0 extraction on the H100 (pyworld.harvest; the f0 hook of yukarin.AcousticFeature.extract reached
 // from realtime_voice_conversion/yukarin_wrapper/acoustic_feature_wrapper.py:28-33; f0_estimating_method='harvest', SURVEY A.2 / A.7).
 // Selected with ryk_engine_set_f0_method(e, 1); the result feeds StoneMask exactly like DIO's does (DESIGN, DECIDE H3).
 //

@@ -1,4 +1,4 @@
-// world_synth.cu -- WORLD realtime synthesizer on the B200 (SURVEY row a14, component J).
+// world_synth.cu -- WORLD realtime synthesizer on the H100 (SURVEY row a14, component J).
 // Replaces world4py's _InitializeSynthesizer / _AddParameters / _Synthesis2 (call sites:
 // realtime_voice_conversion/yukarin_wrapper/vocoder.py:79-103) with a device-resident state machine:
 //   k_synth_add     one CTA : append frames to the device ring, sample-rate f0/vuv interpolation,
@@ -240,7 +240,7 @@ __global__ void k_synth_plan(SynthDev S, int max_blocks) {
 }
 
 // ------------------------------------------------------------------------------------ per-pulse response
-constexpr int kPulseGrid = 296;      // 2 CTAs x 148 SMs; more pulses than that in one drain are handled by the grid-stride loop
+constexpr int kPulseGrid = 264;      // 2 CTAs x 132 SMs; more pulses than that in one drain are handled by the grid-stride loop
 __global__ void __launch_bounds__(256) k_synth_pulse(SynthDev S, const double2* __restrict__ tw) {
   extern __shared__ double2 sm2[];
   SynthState* st = S.state;

@@ -1,6 +1,6 @@
 """ctypes binding of libryk.so (include/ryk.h): the only door between the Python host layer and
 the CUDA hot path.  There is NO CPU fallback: if the shared object is missing, cannot be loaded, or
-no B200 is visible, every call raises.
+no H100 is visible, every call raises.
 """
 import os as _os
 
@@ -69,7 +69,7 @@ def load_library() -> ctypes.CDLL:
             if not _LIB_PATH.exists():
                 raise RykError(f'{_LIB_PATH} is missing: run `python -c "import __graft_entry__ as g; g.build()"` '
                                f'(the hot path has no CPU fallback)')
-            # RYK_LIB: a diagnostics build of the same library (e.g. -DRYK_TC_TIMELINE); never a different implementation
+            # RYK_LIB: a diagnostics build of the same library (e.g. -DRYK_DIAG); never a different implementation
             lib = ctypes.CDLL(os.environ.get('RYK_LIB') or str(_LIB_PATH))
             lib.ryk_last_error.restype = ctypes.c_char_p
             lib.ryk_engine_launch_count.restype = ctypes.c_longlong

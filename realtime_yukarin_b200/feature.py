@@ -118,7 +118,7 @@ class AcousticFeature(object):
     # ---- WORLD analysis (SURVEY a6; vocoder.py:28-37 -> acoustic_feature_wrapper.py:28-33) ----
     @classmethod
     def extract_f0(cls, x: numpy.ndarray, fs: int, frame_period: int, f0_floor: float, f0_ceil: float):
-        """DIO + StoneMask on the B200 (hook kept so that subclasses can swap the f0 front-end,
+        """DIO + StoneMask on the H100 (hook kept so that subclasses can swap the f0 front-end,
         as acoustic_feature_wrapper.py:66-80 does)."""
         from .engine import default_engine
         return default_engine().world_f0(x, fs, frame_period, f0_floor, f0_ceil)

@@ -134,7 +134,7 @@ def load_stage1_stats(params: Dict[str, numpy.ndarray], model_path, in_ch: int, 
 
 class AcousticConverter(object):
     """Stage 1.  `gpu` is accepted for signature compatibility (converter/yukarin_converter.py:44);
-    the engine always runs on the process's B200."""
+    the engine always runs on the process's H100."""
 
     def __init__(self, config: Config, model_path: Path, gpu: int = None, f0_converter: F0Converter = None,
                  out_sampling_rate: int = None, engine: Optional[Engine] = None, feature_stats=None) -> None:

@@ -1,4 +1,4 @@
-"""`python -m realtime_yukarin_b200.run --config_path config.yaml` -- the reference's run.py (run.py:22-199) on one B200.
+"""`python -m realtime_yukarin_b200.run --config_path config.yaml` -- the reference's run.py (run.py:22-199) on one H100.
 
 Same config file (config.yaml), same model loading (YukarinConverter.make_yukarin_converter) and the same audio loop; the
 three worker processes and their queues (run.py:58-93) are one device-resident session (worker.RealtimePipeline).

@@ -1,4 +1,4 @@
-"""Vocoder / RealtimeVocoder: WORLD analysis and realtime synthesis on the B200.
+"""Vocoder / RealtimeVocoder: WORLD analysis and realtime synthesis on the H100.
 
 Same constructor and methods as realtime_voice_conversion/yukarin_wrapper/vocoder.py:15-126; the
 pyworld / world4py calls are replaced by libryk entry points (include/ryk.h).

@@ -11,7 +11,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a B200 (run with -m gpu on the GPU box)')
+    config.addinivalue_line('markers', 'gpu: needs an H100 (sm_90a)')
 
 
 def _has_gpu() -> bool:

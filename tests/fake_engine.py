@@ -1,6 +1,6 @@
 """A CPU stand-in for realtime_yukarin_b200.engine.Engine built on the oracle -- TESTS ONLY.
 It lets the host-side Stream/VoiceChanger/Vocoder logic be checked end to end without a GPU
-(the product never uses it; the product path raises when libryk / a B200 is missing)."""
+(the product never uses it; the product path raises when libryk / an H100 is missing)."""
 import numpy as np
 
 from oracle import nets as onets

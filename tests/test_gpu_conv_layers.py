@@ -1,5 +1,5 @@
 """Unit parity of the two convolution kernels against torch's CPU conv on the same data:
-FP32 CUDA-core kernel (conv_direct.cu) and FP16 tcgen05 kernel (conv_tc.cu, TMA + UMMA + TMEM)."""
+FP32 CUDA-core kernel (conv_direct.cu) and FP16 wgmma kernel (conv_tc.cu, TMA + mbarrier pipeline + warpgroup MMA)."""
 import numpy as np
 import pytest
 import torch
@@ -64,7 +64,7 @@ def test_conv_kernels(engine, case):
     if k == 4 and C0 % 64 == 0 and C1 % 64 == 0 and Cout % 64 == 0:
         got16, ms = engine.test_conv_layer(in0, in1, Wt, scale, shift, tr, k, s, p, act, use_tc=1, repeat=3)
         err16 = np.abs(got16 - ref).max()
-        print('tcgen05', case, 'max err', err16, 'ms', ms)
+        print('wgmma', case, 'max err', err16, 'ms', ms)
         assert err16 < 3e-2, err16
 
 
@@ -118,7 +118,7 @@ def test_stage1_last_layer_kernel(engine, case):
 
 
 PAIR_CASES = [
-    # CTA-pair kernel (conv_tc2.cu, cta_group::2), forced with RYK_TC2=2: transposed, B, H, W, C0, C1, Cout, act
+    # CTA-pair kernel (conv_tc.cu, 2-CTA clusters multicasting the weight tiles), forced with RYK_TC2=2: transposed, B, H, W, C0, C1, Cout, act
     (0, 1, 32, 64, 64, 0, 128, 1),       # conv, N = 128, 4 pixel tiles (2 pairs)
     (0, 2, 16, 16, 128, 0, 256, 1),      # conv, two N tiles, batch 2, 64-pixel images (tile covers two batch rows? no: 1 tile per image)
     (0, 1, 48, 80, 64, 64, 128, 1),      # conv, two sources, ragged tile edges (24 x 40 outputs)
@@ -132,7 +132,8 @@ PAIR_CASES = [
 
 @pytest.mark.parametrize('case', PAIR_CASES)
 def test_pair_kernel(engine, case):
-    """k_conv_tc2: UMMA M = 256 over a CTA pair, class-fused transposed convs; same tolerance as the one-CTA tcgen05 kernel."""
+    """k_conv_tc<..., kPair = true>: 256 pixels x N per CTA pair, each CTA fetching half of every weight tile and multicasting it to
+    both; same tolerance as the one-CTA kernel."""
     import os
     tr, B, H, W, C0, C1, Cout, act = case
     rng = np.random.default_rng(abs(hash(case)) % (2 ** 31))
@@ -191,7 +192,7 @@ def _ref32(in0, in1, W, scale, shift, transposed, act):
 
 @pytest.mark.parametrize('case', PRODUCTION_LAYERS, ids=[c[0] for c in PRODUCTION_LAYERS])
 def test_production_layer_shapes(engine, case):
-    """tcgen05 kernel (and, with RYK_TC_HALO default on, the halo kernel) on the shapes bench.py runs; inputs are fp16-representable
+    """wgmma kernel on the shapes bench.py runs; inputs are fp16-representable
     so that the only differences from the float32 reference are accumulation order and the fp16 output rounding."""
     name, tr, H, W, C0, C1, Cout, act = case
     B = 2 if name.endswith('_b2_512') else 1
@@ -225,7 +226,7 @@ HALO_CASES = [
     (1, 2, 32, 16, 64, 64, 256, 2, 2, 8),       # deconv, batch 2, two sources, two N tiles, M = 256
     (1, 1, 24, 32, 128, 128, 128, 2, 1, 16),    # deconv, d3-like class grid 24 x 32 with 8 x 16 tiles
     (1, 1, 12, 24, 64, 0, 128, 2, 2, 8),        # deconv, ragged (12 rows in 32-row CTA tiles)
-    (1, 1, 16, 32, 128, 128, 64, 2, 1, 8),      # deconv Cout = 64: fused column classes (d6 family)
+    (1, 1, 16, 32, 128, 128, 64, 2, 1, 8),      # deconv Cout = 64 (d6 family)
     (1, 1, 32, 16, 64, 64, 64, 2, 2, 8),        # fused classes, M = 256
     (1, 2, 20, 24, 64, 0, 64, 2, 2, 8),         # fused classes, ragged rows, batch 2
     (1, 1, 16, 32, 64, 0, 64, 2, 1, 16),        # fused classes, 8 x 16 tiles
@@ -234,8 +235,8 @@ HALO_CASES = [
 
 @pytest.mark.parametrize('case', HALO_CASES)
 def test_halo_kernel(engine, case):
-    """k_conv_halo: shared halo rows (two taps per A box), M = 128 / 256 per CTA, fused column classes, dynamic tile scheduler.
-    Same tolerance as the per-tap tcgen05 kernel, and the result must agree with it (same fp16 operands, fp32 accumulation)."""
+    """k_conv_halo: shared halo rows (two taps per A box), M = 128 / 256 per CTA, persistent or one tile per CTA.
+    Same tolerance as the per-tap wgmma kernel, and the result must agree with it (same fp16 operands, fp32 accumulation)."""
     import os
     tr, B, H, W, C0, C1, Cout, act, mt, tw = case
     rng = np.random.default_rng(sum(case) * 104729 + 7)
@@ -253,7 +254,7 @@ def test_halo_kernel(engine, case):
         os.environ['RYK_TC3'] = '0'
         base, _ = engine.test_conv_layer(in0, in1, Wt, scale, shift, tr, 4, 2, 1, act, use_tc=1)
         os.environ.update(RYK_TC3='2', RYK_TC3_MT=str(mt), RYK_TC3_TW=str(tw), RYK_TC3_ONE='0')
-        # depth 1 / 0: persistent CTAs with 3 / 2 stages; 'one': one tile per CTA, two CTAs per SM, staging aliased to stage 0
+        # depth 1 / 0: persistent CTAs with 3 / 2 stages (where 3 fit); 'one': one tile per CTA
         for depth in (1, 0, 'one'):
             if depth == 'one':
                 os.environ.update(RYK_TC3='1', RYK_TC3_ONE='2')

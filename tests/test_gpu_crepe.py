@@ -1,4 +1,4 @@
-"""CREPE f0 mode on the B200 (csrc/crepe.cu, realtime_yukarin_b200/crepe.py) against the restatement in oracle/crepe.py, with seeded
+"""CREPE f0 mode on the H100 (csrc/crepe.cu, realtime_yukarin_b200/crepe.py) against the restatement in oracle/crepe.py, with seeded
 synthetic weights: (1) the network -- activations within FP32 accumulation tolerance; (2) the decoders -- Viterbi pitch path, local
 cents average and the voicing HMM applied by the oracle to the SAME activations must reproduce the device decisions exactly;
 (3) end to end through CrepeAcousticFeatureWrapper / Vocoder(extract_f0_mode=CREPE)."""

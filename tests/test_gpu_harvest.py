@@ -1,4 +1,4 @@
-"""Harvest f0 on the B200 (csrc/world_harvest.cu, ryk_engine_set_f0_method) against the oracle's Harvest restatement, stage by stage:
+"""Harvest f0 on the H100 (csrc/world_harvest.cu, ryk_engine_set_f0_method) against the oracle's Harvest restatement, stage by stage:
 decimated waveform, raw per-channel candidates, refined candidates / scores, tracked contour, smoothed 1 ms contour, 5 ms output, then
 Harvest + StoneMask through ryk_world_f0 / ryk_world_analyze and a device session in Harvest mode against the oracle stream."""
 import dataclasses

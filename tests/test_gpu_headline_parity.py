@@ -1,4 +1,4 @@
-"""GPU parity AT THE BENCHMARKED CONFIGURATION: full-width models (base 64), FP16 operands on tcgen05, the pipelined session
+"""GPU parity AT THE BENCHMARKED CONFIGURATION: full-width models (base 64), FP16 operands on wgmma, the pipelined session
 (`ryk_session_submit / collect`, `ryk_group_submit / collect`) -- the exact path `bench.py` times -- against the CPU oracle stream.
 
 BASELINE.json configs covered: [1] single stream 0.3 s, extras (0,0.5,0) (Tw 260 -> Tp 384); [2] the buffer sweep 0.1 / 0.3 / 1.0 s

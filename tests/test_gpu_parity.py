@@ -283,7 +283,7 @@ def test_pipelined_submit_collect_equals_sequential(engine, small_models):
 def test_group_batched_stage2_matches_oracle_streams(engine, small_models):
     """BASELINE config 5 shape: several streams on one GPU share ONE batched stage-2 forward per step (ryk_group_*).
     Each member must still reproduce the oracle's chunked stream for ITS audio (fp32), with chunks kept in flight,
-    and the fp16 (tcgen05) group must stay within the end-to-end tolerance."""
+    and the fp16 (wgmma) group must stay within the end-to-end tolerance."""
     from realtime_yukarin_b200.engine import SessionConfig
     ac, sr, f0c = _load(engine, small_models)
     p1, p2 = onets.load_npz(small_models['stage1_model_path']), onets.load_npz(small_models['stage2_model_path'])

@@ -1,4 +1,4 @@
-"""Fused stage-1 kernel (csrc/s1_fused.cu: the whole 1-D U-Net as one cluster launch) against the 16-layer tcgen05 sequence it replaces
+"""Fused stage-1 kernel (csrc/s1_fused.cu: the whole 1-D U-Net as one cluster launch) against the 16-layer wgmma sequence it replaces
 and against the oracle (oracle/nets.py), base-64 model, every padded-length bucket the BASELINE configurations reach."""
 import numpy as np
 import pytest

@@ -18,7 +18,7 @@ from oracle import world as W
 from realtime_yukarin_b200 import synthetic
 
 CFG = opipe.PathConfig()
-AUDIO_A = Path('/root/reference/tests/data/audioA.wav')        # the reference's own fixture; read in place when the checkout is present
+AUDIO_A = Path(__file__).resolve().parent / 'golden' / 'audioA_24k_4s.wav'     # the original project's tests/data/audioA.wav: first 4 s at 24 kHz
 
 
 def _resynth(feat, canonical, chunk=60, skip=0):
@@ -71,7 +71,6 @@ def test_decide_10_11_on_synthetic_speech():
     assert r['shifted'] < 1e-12 * max(1.0, r[3][3])
 
 
-@pytest.mark.skipif(not AUDIO_A.exists(), reason='reference checkout (tests/data/audioA.wav) not present on this machine')
 def test_decide_10_11_on_the_reference_recording():
     from realtime_yukarin_b200 import wave_io
     import scipy.signal

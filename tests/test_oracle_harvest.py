@@ -103,12 +103,11 @@ def test_harvest_golden_fixture():
     assert np.allclose(f0, g['f0'], rtol=1e-9, atol=0)
 
 
-AUDIO_A = Path('/root/reference/tests/data/audioA.wav')        # the reference's own fixture; read in place when the checkout is present
+AUDIO_A = Path(__file__).resolve().parent / 'golden' / 'audioA_24k_4s.wav'     # the original project's tests/data/audioA.wav: first 4 s at 24 kHz
 
 
-@pytest.mark.skipif(not AUDIO_A.exists(), reason='reference checkout (tests/data/audioA.wav) not present on this machine')
 def test_harvest_on_the_reference_recording():
-    """Real speech (the reference's tests/data/audioA.wav at 24 kHz, 4 s): Harvest and DIO + StoneMask -- two different published
+    """Real speech (the original project's tests/data/audioA.wav at 24 kHz, 4 s): Harvest and DIO + StoneMask -- two different published
     extractors restated independently of each other -- agree on the pitch where both are voiced, Harvest's contour is the smoother
     one and covers more of the voiced speech, and every value is inside [f0_floor, f0_ceil]."""
     from realtime_yukarin_b200 import wave_io

@@ -1,105 +1,86 @@
-"""The reference's REAL glue classes on top of this package's third-party replacements (CPU, reference checkout required).
+"""The original project's glue classes on top of this package's third-party replacements, pinned by stored outputs (CPU).
 
-`realtime_voice_conversion/{stream,segment}/*.py`, `yukarin_wrapper/voice_changer.py` and
-`yukarin_wrapper/acoustic_feature_wrapper.py` are pure Python over `yukarin` / `become_yukarin` / the vocoder; here they are
-imported from the read-only checkout with `yukarin`, `become_yukarin` resolved by `dropin` and `yukarin_wrapper.vocoder` (the
-module that binds pyworld / world4py) replaced by ours.  Driving the reference's EncodeStream -> ConvertStream(VoiceChanger) ->
-DecodeStream chain the way its workers do must give exactly what this package's own classes give on the same engine."""
-import importlib
-import sys
+`realtime_voice_conversion/{stream,segment}/*.py`, `yukarin_wrapper/voice_changer.py`, `worker/*.py` and `config.py` of the
+original (Hiroshiba/realtime-yukarin) are pure Python over `yukarin` / `become_yukarin` / the vocoder.  tests/golden/
+make_reference_golden.py drove them over this package's replacements (the oracle-backed engine of tests/fake_engine.py) the way
+the original's workers do and stored what they returned (tests/golden/reference_golden.npz); this package's own classes must give
+the same on the same engine."""
+import json
 from pathlib import Path
 
 import numpy as np
 import pytest
 
-REF_ROOT = Path('/root/reference')
-pytestmark = pytest.mark.skipif(not (REF_ROOT / 'realtime_voice_conversion').exists(), reason='reference checkout not present (GPU box)')
+from tests.golden.make_reference_golden import check_digest
+
+GOLDEN = Path(__file__).resolve().parent / 'golden'
+# the stored outputs come from torch-CPU float32 convolutions on another machine: its kernels may round differently
+RTOL = 1e-5
+STREAM_CASES = [(0.3, (0.0, 0.5, 0.0)), (0.1, (0.1, 0.2, 0.1))]
+WORKER_T, WORKER_EXTRA = 0.3, (0.0, 0.5, 0.0)
 
 
-class _RealReferencePackage:
-    """Context manager: `realtime_voice_conversion` resolves to the real checkout (except yukarin_wrapper.vocoder = ours)."""
-
-    def __enter__(self):
-        from realtime_yukarin_b200 import dropin, vocoder
-        import types
-        dropin.install()                                   # yukarin / become_yukarin / librosa aliases
-        self.saved = {k: v for k, v in sys.modules.items() if k == 'realtime_voice_conversion' or k.startswith('realtime_voice_conversion.')}
-        for k in self.saved:
-            del sys.modules[k]
-        pkg = types.ModuleType('realtime_voice_conversion')
-        pkg.__path__ = [str(REF_ROOT / 'realtime_voice_conversion')]      # real files for every submodule ...
-        sys.modules['realtime_voice_conversion'] = pkg
-        yw = types.ModuleType('realtime_voice_conversion.yukarin_wrapper')
-        yw.__path__ = [str(REF_ROOT / 'realtime_voice_conversion' / 'yukarin_wrapper')]
-        sys.modules['realtime_voice_conversion.yukarin_wrapper'] = yw
-        voc = types.ModuleType('realtime_voice_conversion.yukarin_wrapper.vocoder')    # ... except the pyworld / world4py binding
-        voc.Vocoder, voc.RealtimeVocoder = vocoder.Vocoder, vocoder.RealtimeVocoder
-        sys.modules['realtime_voice_conversion.yukarin_wrapper.vocoder'] = voc
-        return self
-
-    def load(self, name):
-        return importlib.import_module(f'realtime_voice_conversion.{name}')
-
-    def __exit__(self, *exc):
-        for k in [k for k in sys.modules if k == 'realtime_voice_conversion' or k.startswith('realtime_voice_conversion.')]:
-            del sys.modules[k]
-        sys.modules.update(self.saved)
-        return False
+@pytest.fixture(scope='module')
+def golden():
+    return dict(np.load(GOLDEN / 'reference_golden.npz'))
 
 
-@pytest.mark.parametrize('T,extra', [(0.3, (0.0, 0.5, 0.0)), (0.1, (0.1, 0.2, 0.1))])
-def test_reference_streams_and_voice_changer_over_our_replacements(small_models, T, extra):
-    from realtime_yukarin_b200 import engine as eng_mod
-    from realtime_yukarin_b200 import stream as our_stream
+def stream_tag(T, extra):
+    return f'streams_T{T:g}_extra' + '_'.join(f'{e:g}' for e in extra)
+
+
+def run_stream_chain(models, fake, T, extra, EncodeStream, ConvertStream, DecodeStream, StreamWrapper, VoiceChanger):
+    """EncodeStream -> ConvertStream(VoiceChanger) -> DecodeStream over 1.5 s of synthetic speech in chunks of T seconds;
+    per chunk: (encoded f0, converted f0, converted sp, decoded wave)"""
     from realtime_yukarin_b200 import synthetic
-    from realtime_yukarin_b200 import voice_changer as our_vc
     from realtime_yukarin_b200.config import VocodeMode
     from realtime_yukarin_b200.models import AcousticConverter, F0Converter, SuperResolution
     from realtime_yukarin_b200.params import create_from_json, create_sr_from_json
     from realtime_yukarin_b200.vocoder import RealtimeVocoder
+    f0c = F0Converter(models['input_statistics_path'], models['target_statistics_path'])
+    ac = AcousticConverter(create_from_json(models['stage1_config_path']), models['stage1_model_path'], f0_converter=f0c, engine=fake)
+    sr = SuperResolution(create_sr_from_json(models['stage2_config_path']), models['stage2_model_path'], engine=fake)
+    acp = create_from_json(models['stage1_config_path']).dataset.acoustic_param
+    voc = RealtimeVocoder(acoustic_param=acp, out_sampling_rate=24000, extract_f0_mode=VocodeMode.WORLD)
+    voc.create_synthesizer(buffer_size=1024, number_of_pointers=16)
+    es, cs, ds = EncodeStream(vocoder=voc), ConvertStream(voice_changer=VoiceChanger(acoustic_converter=ac, super_resolution=sr, threshold=60)), DecodeStream(vocoder=voc)
+    ws = [StreamWrapper(stream=es, extra_time=extra[0]), StreamWrapper(stream=cs, extra_time=extra[1]), StreamWrapper(stream=ds, extra_time=extra[2])]
+    x = synthetic.synthetic_speech(1.5, 31)
+    n = round(T * 24000)
+    outs = []
+    for k in range(len(x) // n):
+        es.add(start_time=extra[0] + k * T, data=x[k * n:(k + 1) * n])
+        f = ws[0].process_next(time_length=T)
+        cs.add(start_time=extra[1] + k * T, data=f)
+        c = ws[1].process_next(time_length=T)
+        ds.add(start_time=extra[2] + k * T, data=c)
+        y = ws[2].process_next(time_length=T)
+        outs.append((np.asarray(f.f0).copy(), np.asarray(c.f0).copy(), np.asarray(c.sp).copy(), np.asarray(y.wave if hasattr(y, 'wave') else y).copy()))
+    return outs
+
+
+@pytest.mark.parametrize('T,extra', STREAM_CASES)
+def test_reference_streams_and_voice_changer_over_our_replacements(small_models, golden, T, extra):
+    from realtime_yukarin_b200 import engine as eng_mod
+    from realtime_yukarin_b200 import stream as our_stream
+    from realtime_yukarin_b200 import voice_changer as our_vc
     from tests.fake_engine import OracleEngine
     fake = OracleEngine(small_models['stage1_model_path'], small_models['stage2_model_path'])
     eng_mod.set_default_engine(fake)
     try:
-        f0c = F0Converter(small_models['input_statistics_path'], small_models['target_statistics_path'])
-        ac = AcousticConverter(create_from_json(small_models['stage1_config_path']), small_models['stage1_model_path'], f0_converter=f0c, engine=fake)
-        sr = SuperResolution(create_sr_from_json(small_models['stage2_config_path']), small_models['stage2_model_path'], engine=fake)
-        acp = create_from_json(small_models['stage1_config_path']).dataset.acoustic_param
-
-        def chain(EncodeStream, ConvertStream, DecodeStream, StreamWrapper, VoiceChanger):
-            voc = RealtimeVocoder(acoustic_param=acp, out_sampling_rate=24000, extract_f0_mode=VocodeMode.WORLD)
-            voc.create_synthesizer(buffer_size=1024, number_of_pointers=16)
-            es, cs, ds = EncodeStream(vocoder=voc), ConvertStream(voice_changer=VoiceChanger(acoustic_converter=ac, super_resolution=sr, threshold=60)), DecodeStream(vocoder=voc)
-            ws = [StreamWrapper(stream=es, extra_time=extra[0]), StreamWrapper(stream=cs, extra_time=extra[1]), StreamWrapper(stream=ds, extra_time=extra[2])]
-            x = synthetic.synthetic_speech(1.5, 31)
-            n = round(T * 24000)
-            outs = []
-            for k in range(len(x) // n):
-                es.add(start_time=extra[0] + k * T, data=x[k * n:(k + 1) * n])
-                f = ws[0].process_next(time_length=T)
-                cs.add(start_time=extra[1] + k * T, data=f)
-                c = ws[1].process_next(time_length=T)
-                ds.add(start_time=extra[2] + k * T, data=c)
-                y = ws[2].process_next(time_length=T)
-                outs.append((np.asarray(f.f0).copy(), np.asarray(c.f0).copy(), np.asarray(c.sp).copy(), np.asarray(y.wave if hasattr(y, 'wave') else y).copy()))
-            return outs
-
-        with _RealReferencePackage() as ref:
-            rs = ref.load('stream')
-            rvc = ref.load('yukarin_wrapper.voice_changer')
-            assert Path(rs.__file__).is_relative_to(REF_ROOT) and Path(rvc.__file__).is_relative_to(REF_ROOT)      # really the checkout's code
-            got_ref = chain(rs.EncodeStream, rs.ConvertStream, rs.DecodeStream, rs.StreamWrapper, rvc.VoiceChanger)
-        got_ours = chain(our_stream.EncodeStream, our_stream.ConvertStream, our_stream.DecodeStream, our_stream.StreamWrapper, our_vc.VoiceChanger)
-        assert len(got_ref) == len(got_ours) > 0
-        for k, (a, b) in enumerate(zip(got_ref, got_ours)):
-            for u, v in zip(a, b):
-                assert u.shape == v.shape and np.array_equal(u, v, equal_nan=True), k
+        got = run_stream_chain(small_models, fake, T, extra, our_stream.EncodeStream, our_stream.ConvertStream, our_stream.DecodeStream,
+                               our_stream.StreamWrapper, our_vc.VoiceChanger)
+        tag = stream_tag(T, extra)
+        assert len(got) == int(golden[tag + '/chunks']) > 0
+        for i, arrs in enumerate(got):
+            for j, a in enumerate(arrs):
+                check_digest(golden, f'{tag}/{i}/{j}', a, rtol=RTOL)
     finally:
         eng_mod.set_default_engine(None)
 
 
-def _test_librosa_module():
-    """`librosa.stft` / `librosa.core.power_to_db` for the reference's decode worker (decode_worker.py:56), written here in numpy
+def librosa_module():
+    """`librosa.stft` / `librosa.core.power_to_db` for the original's decode worker (decode_worker.py:56), written here in numpy
     (librosa 0.6/0.7 defaults: n_fft 2048, hop 512, periodic Hann, reflect-centred; ref 1, amin 1e-10, top_db 80).  Test harness only."""
     import types
     import scipy.signal as ss
@@ -121,151 +102,96 @@ def _test_librosa_module():
     return lib, core
 
 
-def test_reference_workers_over_our_replacements_match_realtime_pipeline(small_models, tmp_path, monkeypatch):
-    """SURVEY 8(f) ranks 1 / 2 against the REAL worker code: the reference's encode_worker / convert_worker / decode_worker
-    (worker/*.py, imported from the checkout, each in a thread with queue.Queue standing in for multiprocessing.Queue) over this
-    package's replacements, versus worker.RealtimePipeline on the same engine: the same Items in the same order -- chunk played,
-    or None (not enough samples yet / gated as silent)."""
-    import queue
-    import threading
-    import types
-    from realtime_yukarin_b200 import engine as eng_mod
-    from realtime_yukarin_b200 import synthetic
-    from realtime_yukarin_b200.config import Config, VocodeMode
+def worker_models(models, fake):
+    from realtime_yukarin_b200.config import VocodeMode
     from realtime_yukarin_b200.models import AcousticConverter, F0Converter, SuperResolution
     from realtime_yukarin_b200.params import create_from_json, create_sr_from_json
     from realtime_yukarin_b200.vocoder import RealtimeVocoder
+    f0c = F0Converter(models['input_statistics_path'], models['target_statistics_path'])
+    ac = AcousticConverter(create_from_json(models['stage1_config_path']), models['stage1_model_path'], f0_converter=f0c, engine=fake)
+    sr = SuperResolution(create_sr_from_json(models['stage2_config_path']), models['stage2_model_path'], engine=fake)
+    acp = create_from_json(models['stage1_config_path']).dataset.acoustic_param
+    return ac, sr, acp, RealtimeVocoder(acoustic_param=acp, out_sampling_rate=24000, extract_f0_mode=VocodeMode.WORLD)
+
+
+def worker_setup(models, fake):
+    """-> (config whose output threshold gates some chunks and keeps others, input audio, chunk count, chunks that pass ungated)"""
+    from realtime_yukarin_b200 import synthetic
+    from realtime_yukarin_b200.config import Config, VocodeMode
     from realtime_yukarin_b200.worker import Item, RealtimePipeline
-    from tests.fake_engine import OracleEngine
-    monkeypatch.chdir(tmp_path)                      # the reference's init_logger writes ./log.txt
-    fake = OracleEngine(small_models['stage1_model_path'], small_models['stage2_model_path'])
-    eng_mod.set_default_engine(fake)
-    T, extra = 0.3, (0.0, 0.5, 0.0)
+    T, extra = WORKER_T, WORKER_EXTRA
     x = synthetic.synthetic_speech(3.0, stream=37)
     x[int(1.2 * 24000):int(2.1 * 24000)] *= 1e-4
     n = round(T * 24000)
     K = len(x) // n
-    saved_mods = {k: sys.modules.get(k) for k in ('librosa', 'librosa.core', 'chainer')}
-    try:
-        f0c = F0Converter(small_models['input_statistics_path'], small_models['target_statistics_path'])
-        ac = AcousticConverter(create_from_json(small_models['stage1_config_path']), small_models['stage1_model_path'], f0_converter=f0c, engine=fake)
-        sr = SuperResolution(create_sr_from_json(small_models['stage2_config_path']), small_models['stage2_model_path'], engine=fake)
-        acp = create_from_json(small_models['stage1_config_path']).dataset.acoustic_param
-        def make_cfg(out_thr):
-            return Config(input_device_name=None, output_device_name=None, input_rate=24000, output_rate=24000, frame_period=5.0, buffer_time=T,
-                          extract_f0_mode=VocodeMode.WORLD, vocoder_buffer_size=1024, input_scale=1.0, output_scale=1.0,
-                          input_silent_threshold=60.0, output_silent_threshold=out_thr, encode_extra_time=extra[0],
-                          convert_extra_time=extra[1], decode_extra_time=extra[2],
-                          **{k: small_models[k] for k in ('input_statistics_path', 'target_statistics_path', 'stage1_model_path',
-                                                          'stage1_config_path', 'stage2_model_path', 'stage2_config_path')})
+    acp = worker_models(models, fake)[2]
 
-        # a threshold that gates some chunks and keeps others: powers of the ungated chunks, split at their widest gap
-        lib_probe, core_probe = _test_librosa_module()
-        probe = RealtimePipeline(make_cfg(1e9), acoustic_param=acp, engine=fake, depth=1)
-        powers = []
-        for k in range(K):
-            probe.put(Item(item=x[k * n:(k + 1) * n].copy(), index=k))
-            it = probe.get()
-            if it.item is not None:
-                powers.append(float(core_probe.power_to_db(np.abs(lib_probe.stft(it.item)) ** 2).mean()))
-        probe.close()
-        ps = np.sort(np.asarray(powers))
-        gi = int(np.argmax(np.diff(ps)))
-        assert ps[gi + 1] - ps[gi] > 1e-3
-        cfg = make_cfg(-float(0.5 * (ps[gi] + ps[gi + 1])))
-        with _RealReferencePackage() as ref:
-            lib, core = _test_librosa_module()
-            sys.modules['librosa'], sys.modules['librosa.core'] = lib, core
-            chainer = types.ModuleType('chainer')
-            chainer.global_config = types.SimpleNamespace(enable_backprop=True, train=True)
-            sys.modules['chainer'] = chainer
-            workers = ref.load('worker')
-            assert Path(workers.__file__).is_relative_to(REF_ROOT)
-            q_in, q_feat, q_conv, q_out = queue.Queue(), queue.Queue(), queue.Queue(), queue.Queue()
-            locks = [threading.Lock() for _ in range(3)]
-            for lk in locks:
-                lk.acquire()
-            voc = RealtimeVocoder(acoustic_param=acp, out_sampling_rate=24000, extract_f0_mode=VocodeMode.WORLD)
-            threads = [
-                threading.Thread(target=workers.encode_worker, daemon=True, kwargs=dict(
-                    realtime_vocoder=voc, time_length=T, extra_time=extra[0], queue_input=q_in, queue_output=q_feat, acquired_lock=locks[0])),
-                threading.Thread(target=workers.convert_worker, daemon=True, kwargs=dict(
-                    acoustic_converter=ac, super_resolution=sr, time_length=T, extra_time=extra[1], input_silent_threshold=cfg.input_silent_threshold,
-                    queue_input=q_feat, queue_output=q_conv, acquired_lock=locks[1])),
-                threading.Thread(target=workers.decode_worker, daemon=True, kwargs=dict(
-                    realtime_vocoder=voc, time_length=T, extra_time=extra[2], vocoder_buffer_size=1024, out_audio_chunk=cfg.out_audio_chunk,
-                    output_silent_threshold=cfg.output_silent_threshold, queue_input=q_conv, queue_output=q_out, acquired_lock=locks[2])),
-            ]
-            for th in threads:
-                th.start()
-            for lk in locks:                             # run.py:95-96: wait until every worker is ready
-                assert lk.acquire(timeout=30)
-            ref_items = []
-            for k in range(K):
-                q_in.put(workers.utility.Item(item=x[k * n:(k + 1) * n].copy(), index=k) if hasattr(workers, 'utility')
-                         else ref.load('worker.utility').Item(item=x[k * n:(k + 1) * n].copy(), index=k))
-                ref_items.append(q_out.get(timeout=120))
-            assert chainer.global_config.train is False and chainer.global_config.enable_backprop is False      # convert_worker.py:33-34 ran
+    def make_cfg(out_thr):
+        return Config(input_device_name=None, output_device_name=None, input_rate=24000, output_rate=24000, frame_period=5.0, buffer_time=T,
+                      extract_f0_mode=VocodeMode.WORLD, vocoder_buffer_size=1024, input_scale=1.0, output_scale=1.0,
+                      input_silent_threshold=60.0, output_silent_threshold=out_thr, encode_extra_time=extra[0],
+                      convert_extra_time=extra[1], decode_extra_time=extra[2],
+                      **{k: models[k] for k in ('input_statistics_path', 'target_statistics_path', 'stage1_model_path',
+                                                'stage1_config_path', 'stage2_model_path', 'stage2_config_path')})
+
+    # a threshold that gates some chunks and keeps others: powers of the ungated chunks, split at their widest gap
+    lib, core = librosa_module()
+    probe = RealtimePipeline(make_cfg(1e9), acoustic_param=acp, engine=fake, depth=1)
+    powers = []
+    for k in range(K):
+        probe.put(Item(item=x[k * n:(k + 1) * n].copy(), index=k))
+        it = probe.get()
+        if it.item is not None:
+            powers.append(float(core.power_to_db(np.abs(lib.stft(it.item)) ** 2).mean()))
+    probe.close()
+    ps = np.sort(np.asarray(powers))
+    gi = int(np.argmax(np.diff(ps)))
+    assert ps[gi + 1] - ps[gi] > 1e-3
+    return make_cfg(-float(0.5 * (ps[gi] + ps[gi + 1]))), x, K, len(powers)
+
+
+def test_reference_workers_over_our_replacements_match_realtime_pipeline(small_models, golden):
+    """SURVEY 8(f) ranks 1 / 2 against the original's worker code: its encode_worker / convert_worker / decode_worker (each in a
+    thread, queue.Queue standing in for multiprocessing.Queue) over this package's replacements, stored, versus
+    worker.RealtimePipeline on the same engine: the same Items in the same order -- chunk played, or None (not enough samples
+    yet / gated as silent)."""
+    from realtime_yukarin_b200 import engine as eng_mod
+    from realtime_yukarin_b200.worker import Item, RealtimePipeline
+    from tests.fake_engine import OracleEngine
+    fake = OracleEngine(small_models['stage1_model_path'], small_models['stage2_model_path'])
+    eng_mod.set_default_engine(fake)
+    try:
+        cfg, x, K, n_powers = worker_setup(small_models, fake)
+        assert abs(cfg.output_silent_threshold - float(golden['workers/output_silent_threshold'])) <= RTOL * abs(cfg.output_silent_threshold)
+        acp = worker_models(small_models, fake)[2]
+        n = round(WORKER_T * 24000)
         pipe = RealtimePipeline(cfg, acoustic_param=acp, engine=fake, depth=1)
         ours = []
         for k in range(K):
             pipe.put(Item(item=x[k * n:(k + 1) * n].copy(), index=k))
             ours.append(pipe.get())
         pipe.close()
-        assert [it.index for it in ref_items] == [it.index for it in ours] == list(range(K))
-        played = silent = 0
-        for a, b in zip(ref_items, ours):
-            assert (a.item is None) == (b.item is None), a.index
-            if a.item is not None:
+        assert list(golden['workers/index']) == [it.index for it in ours] == list(range(K))
+        played = 0
+        for k, (ref_played, b) in enumerate(zip(golden['workers/played'], ours)):
+            assert bool(ref_played) == (b.item is not None), k
+            if b.item is not None:
                 played += 1
-                assert len(a.item) == len(b.item) == cfg.out_audio_chunk
-                assert np.abs(np.asarray(a.item) - b.item).max() < 1e-9
-        assert 0 < played < len(powers)                   # the gate kept some chunks and dropped others, identically on both sides
+                assert len(b.item) == cfg.out_audio_chunk
+                check_digest(golden, f'workers/{k}', b.item, atol=1e-9, rtol=RTOL)
+        assert 0 < played < n_powers                     # the gate kept some chunks and dropped others, identically on both sides
     finally:
-        for k, v in saved_mods.items():
-            if v is None:
-                sys.modules.pop(k, None)
-            else:
-                sys.modules[k] = v
         eng_mod.set_default_engine(None)
 
 
-def test_reference_converter_and_config_modules_over_our_replacements(small_models):
-    """The reference's real converter/yukarin_converter.py and config.py: model loading through the reference's own call site
-    (kwargs gpu=0, out_sampling_rate=24000, F0Converter(input_statistics=...)) lands in this package's classes, and its Config reads
-    the same values from config.yaml as ours."""
-    from realtime_yukarin_b200 import engine as eng_mod
+def test_reference_converter_and_config_modules_over_our_replacements():
+    """The original's config.py reads its config.yaml (stored) into the values in reference_config_fields.json; this package's
+    Config reads the same values from the same file."""
     from realtime_yukarin_b200 import config as our_config
-    from realtime_yukarin_b200.models import AcousticConverter, SuperResolution
-    from tests.fake_engine import OracleEngine
-    fake = OracleEngine(small_models['stage1_model_path'], small_models['stage2_model_path'])
-    eng_mod.set_default_engine(fake)
-    try:
-        saved_mods = {k: sys.modules.get(k) for k in ('librosa', 'librosa.core', 'chainer')}
-        with _RealReferencePackage() as ref:
-            import types
-            lib, core = _test_librosa_module()             # worker/__init__ (pulled in by yukarin_converter.py:10) imports librosa and chainer
-            sys.modules['librosa'], sys.modules['librosa.core'] = lib, core
-            chainer = types.ModuleType('chainer'); chainer.global_config = types.SimpleNamespace()
-            sys.modules['chainer'] = chainer
-            yc = ref.load('converter.yukarin_converter')
-            assert Path(yc.__file__).is_relative_to(REF_ROOT)
-            conv = yc.YukarinConverter.make_yukarin_converter(**{k: small_models[k] for k in (
-                'input_statistics_path', 'target_statistics_path', 'stage1_model_path', 'stage1_config_path', 'stage2_model_path',
-                'stage2_config_path')})
-            assert isinstance(conv.acoustic_converter, AcousticConverter) and isinstance(conv.super_resolution, SuperResolution)
-            assert fake.stats is not None
-            rc = ref.load('config')
-            a = rc.Config.from_yaml(REF_ROOT / 'config.yaml')
-        b = our_config.Config.from_yaml(REF_ROOT / 'config.yaml')
-        for name in a._fields:
-            va, vb = getattr(a, name), getattr(b, name)
-            assert (va.value if hasattr(va, 'value') else va) == (vb.value if hasattr(vb, 'value') else vb), name
-        assert a.in_audio_chunk == b.in_audio_chunk and a.out_audio_chunk == b.out_audio_chunk
-    finally:
-        for k, v in locals().get('saved_mods', {}).items():
-            if v is None:
-                sys.modules.pop(k, None)
-            else:
-                sys.modules[k] = v
-        eng_mod.set_default_engine(None)
+    want = json.loads((GOLDEN / 'reference_config_fields.json').read_text())
+    b = our_config.Config.from_yaml(GOLDEN / 'reference_config.yaml')
+    for name in set(want) - {'in_audio_chunk', 'out_audio_chunk'}:
+        vb = getattr(b, name)
+        vb = vb.value if hasattr(vb, 'value') else vb
+        assert (str(vb) if isinstance(vb, Path) else vb) == want[name], name
+    assert b.in_audio_chunk == want['in_audio_chunk'] and b.out_audio_chunk == want['out_audio_chunk']
