@@ -165,7 +165,6 @@ int ryk_engine_create(int device, ryk_engine** out) {
   if (analysis_kernels_init()) return -1;
   if (tc_init()) return -1;
   if (s1_fused_init()) return -1;
-  { const char* ev = getenv("RYK_S1_FUSED"); e->s1_fused = !(ev && atoi(ev) == 0); }
   RYK_CUDA(cudaMalloc(&e->d_colmin, sizeof(float) * 64 * 512));   // stage-2 prologue scratch (never allocated inside a graph capture)
   *out = h;
   return 0;

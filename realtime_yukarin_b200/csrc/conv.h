@@ -2,7 +2,6 @@
 // FP16 wgmma tensor-core path (conv_tc.cu) and the U-Net scheduler (unet.cu).
 #pragma once
 #include <cuda.h>
-#include <cudaTypedefs.h>
 
 #include "common.cuh"
 
@@ -36,11 +35,6 @@ struct ConvLayer {
   int tile_w = 0, tile_h = 0;             // pixel tile = tile_w x tile_h = 128
   int block_n = 0;
   bool tc_ready = false;
-  bool tc2 = false;                       // CTA-pair kernel: 2-CTA clusters share (multicast) the weight tiles
-  CUtensorMap tmB2;                       // weights, box of block_n / 2 rows (each CTA of a pair fetches one half)
-  bool tc3 = false;                       // halo kernel (conv_tc3.cu)
-  struct Halo { int tile_w = 0, tile_h = 0, mt = 1, stages = 2; bool one = false; } t3;
-  CUtensorMap t3A0, t3A1, t3O;            // halo boxes of the inputs, output tile of one M tile
 };
 
 // Weight repacking from the Chainer layouts the model files use:
@@ -55,14 +49,6 @@ int tc_init();                                           // resolves cuTensorMap
 int tc_layer_prepare(ConvLayer& L, int num_sms);         // builds tensor maps, picks tiles / split-K (needs final pointers)
 int conv_tc_run(const ConvLayer& L, cudaStream_t st);
 size_t tc_splitk_ws_bytes(const ConvLayer& L, int num_sms);
-bool tc_layer_clusterk(const ConvLayer& L);                 // split-K layer whose partial sums are reduced inside the kernel (no reduce launch)
-void tc_force_pdl(int v);                                // -1 environment default, 0 / 1 forced
-
-// conv_tc3.cu: halo kernel for the k4 s2 p1 2-D layers
-int tc3_init();
-bool tc3_layer_config(const ConvLayer& L, int num_sms, ConvLayer::Halo* cfg);    // cfg may be null
-int tc3_layer_prepare(ConvLayer& L, PFN_cuTensorMapEncodeTiled_v12000 encode);
-int conv_tc3_run(const ConvLayer& L, cudaStream_t st, bool pdl);
 
 // s1_fused.cu: the whole 1-D U-Net as one cluster kernel
 int s1_pack_weights(const float* d_w_chainer, int transposed, int Cin, int Cout, __half* d_out, cudaStream_t st);

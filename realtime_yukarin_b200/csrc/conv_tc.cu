@@ -19,13 +19,8 @@
 //                                       FP16 staging in the idle stage buffers, TMA store)
 // * Small-M bottleneck layers are weight-bandwidth bound: split-K over blockIdx.z spreads the weight
 //   stream over all SMs; partial sums meet in an FP32 workspace and a reduce kernel applies the epilogue.
-// * CTA pairs (kPair, RYK_TC2): the two CTAs of a 2-CTA cluster compute neighbouring pixel tiles with the same weights; each
-//   fetches HALF of every weight tile and multicasts it into both CTAs' shared memory (TMA .multicast::cluster), halving the
-//   weight bytes each SM pulls from L2.  A stage is refilled only after the consumers of BOTH CTAs released it (every consumer
-//   warp arrives on its own and on the peer's `empty` barrier).
 #include <cuda.h>
 #include <cudaTypedefs.h>
-#include <stdlib.h>
 
 #include "conv.h"
 #include "tc_ptx.cuh"
@@ -43,11 +38,8 @@ struct TcParams {
   int ksplit, chunks_per_split;
   int act;
   const float* scale; const float* shift;
-  __half* out;
   float* ws;                     // split-K workspace [ksplit][pixels][Cout] or nullptr
   size_t out_pixels;             // B * Hout * Wout
-  int cluster_k;                 // split-K partial sums are reduced INSIDE the kernel: the ksplit CTAs of a tile form a thread-block cluster
-                                 // (cluster rank == split) and read each other's FP32 partial tiles through distributed shared memory
 };
 
 template <int BLOCK_N>
@@ -56,17 +48,15 @@ __device__ __forceinline__ void wgmma_tile(float (&acc)[BLOCK_N / 2], uint64_t a
   else wgmma_m64n64(acc, adesc, bdesc);
 }
 
-template <int BLOCK_N, int kStages, int kMinBlocks, bool kPair>
+template <int BLOCK_N, int kStages, int kMinBlocks>
 __global__ void __launch_bounds__(kTcThreads, kMinBlocks)
 k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
           const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmW,
-          const __grid_constant__ CUtensorMap tmB2, const TcParams p) {
+          const TcParams p) {
   static_assert(BLOCK_N == 64 || BLOCK_N == 128, "BLOCK_N");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   constexpr uint32_t kABytes = kBlockM * kBlockK * 2;
   constexpr uint32_t kBBytes = BLOCK_N * kBlockK * 2;
-  constexpr uint32_t kCkPitch = BLOCK_N * 4 + 16;          // row pitch of the FP32 partial tile of the in-cluster split-K reduction
-  constexpr bool kCkOk = (size_t)kBlockM * kCkPitch <= (size_t)kStages * (kABytes + kBBytes);      // partial tile fits the stage buffers
   static_assert((size_t)kBlockM * BLOCK_N * 4 <= (size_t)kStages * (kABytes + kBBytes), "epilogue staging must fit the stage buffers");
   // carve: 1024-aligned stage buffers first, barriers after
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -102,16 +92,14 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
     if (p.chunks1 > 0) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA1) : "memory");
     if (!p.ws) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
     else asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW) : "memory");
-    for (int i = 0; i < kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], (kPair ? 2 : 1) * kTcConsumers / 32); }
+    for (int i = 0; i < kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kTcConsumers / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (threadIdx.x < kTcConsumers && !p.ws) {
     for (int i = threadIdx.x; i < BLOCK_N; i += kTcConsumers) { s_scale[i] = __ldg(p.scale + n0 + i); s_shift[i] = __ldg(p.shift + n0 + i); }
   }
   __syncthreads();
-  const uint32_t peer = kPair ? (cluster_rank() ^ 1u) : 0u;
-  if (kPair) cluster_barrier();     // the peer's barriers are initialised before any multicast or remote arrive reaches them
-  pdl_wait();                       // the previous layer's outputs (our A operand) are complete from here on
+  pdl_wait();                      // the previous layer's outputs (our A operand) are complete from here on
 
   if (warp == kTcConsumers / 32) {
     // ===== TMA producer (warp-uniform loop, one elected lane issues: see elect_one() in tc_ptx.cuh) =====
@@ -133,12 +121,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
         mbar_expect_tx(&full_bar[s], kABytes + kBBytes);
         if (cc < p.chunks0) tma_load_4d(smem_a + s * kABytes, &tmA0, &full_bar[s], cc * kBlockK, ix, iy, b);
         else tma_load_4d(smem_a + s * kABytes, &tmA1, &full_bar[s], (cc - p.chunks0) * kBlockK, ix, iy, b);
-        if (kPair) {
-          const int half = (int)(peer ^ 1u) * (BLOCK_N / 2);        // this CTA's half of the weight tile, multicast to both CTAs
-          tma_load_2d_multicast(smem_b + s * kBBytes + half * 128, &tmB2, &full_bar[s], kc * kBlockK, cls * p.Cout + n0 + half, 0x3);
-        } else {
-          tma_load_2d(smem_b + s * kBBytes, &tmB, &full_bar[s], kc * kBlockK, cls * p.Cout + n0);
-        }
+        tma_load_2d(smem_b + s * kBBytes, &tmB, &full_bar[s], kc * kBlockK, cls * p.Cout + n0);
       }
     }
   } else if (warp < kTcConsumers / 32) {
@@ -162,10 +145,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
       wgmma_fence_acc(acc);
       if (i > 0) {
         __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(&empty_bar[(i - 1) % kStages]);
-          if (kPair) mbar_arrive_cluster(cluster_map_rank(smem_u32(&empty_bar[(i - 1) % kStages]), peer));
-        }
+        if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % kStages]);
       }
     }
     wgmma_wait<0>();
@@ -180,10 +160,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
       const int row = rbase + 8 * ((i >> 1) & 1);
       const int col = 8 * (i >> 2) + cq;
       const float a0 = acc[i], a1 = acc[i + 1];
-      if (kCkOk && p.cluster_k) {
-        // raw FP32 partial sums -> plain [pixel][channel] tile in the (idle) stage buffers, row pitch kCkPitch; the cluster reduces below
-        *reinterpret_cast<float2*>(smem + (size_t)row * kCkPitch + col * 4) = make_float2(a0, a1);
-      } else if (p.ws) {
+      if (p.ws) {
         // split-K partial tile (raw FP32 sums) -> 128B-swizzled [128 pixels][32 channels] blocks, stored below by TMA into this
         // split's slice of the workspace; k_splitk_reduce sums the slices
         uint8_t* blk = smem + (col >> 5) * (kBlockM * 128) + row * 128;
@@ -199,7 +176,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
         *reinterpret_cast<__half2*>(blk + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2) = __floats2half2_rn(v0, v1);
       }
     }
-    if (!p.cluster_k && my_chunks > 0) {
+    if (my_chunks > 0) {
       // generic-proxy smem writes -> visible to the async proxy; one thread hands the tile to the TMA unit
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       asm volatile("bar.sync 1, %0;" ::"n"(kTcConsumers) : "memory");
@@ -222,43 +199,6 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
       }
     }
   }
-  if (kCkOk && p.cluster_k) {
-    // ===== in-cluster split-K reduction (replaces the FP32 workspace round trip + k_splitk_reduce launch) =====
-    // CTA r of the cluster (= split r) owns tile rows r, r + ksplit, ...; it sums the ksplit partial rows in split order (fixed:
-    // deterministic), applies scale / shift / activation and writes FP16 NHWC directly.  All threads take both cluster barriers.
-    cluster_barrier();                                   // every split's partial tile is in its CTA's shared memory
-    if (threadIdx.x < kTcConsumers) {
-      constexpr int kTpr = BLOCK_N / 4;                  // threads per row (one float4 each)
-      constexpr int kRpp = kTcConsumers / kTpr;          // rows per pass
-      const int sub = threadIdx.x / kTpr, c4 = threadIdx.x % kTpr;
-      const uint32_t my_base = smem_u32(smem);
-      const float4 sc = *reinterpret_cast<const float4*>(s_scale + c4 * 4), sh = *reinterpret_cast<const float4*>(s_shift + c4 * 4);
-      for (int i = sub; ; i += kRpp) {
-        const int row = split + i * p.ksplit;
-        if (row >= kBlockM) break;
-        const int hl = row / p.tile_w, wl = row - hl * p.tile_w;
-        const int my = oy0 + hl, mx = ox0 + wl;
-        if (my >= p.Hc || mx >= p.Wc) continue;
-        const uint32_t off = (uint32_t)row * kCkPitch + (uint32_t)c4 * 16u;
-        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int q = 0; q < p.ksplit; ++q) {
-          const float4 v = ld_cluster_f4(cluster_map_rank(my_base + off, (uint32_t)q));
-          a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
-        }
-        float v4[4] = {fmaf(a.x, sc.x, sh.x), fmaf(a.y, sc.y, sh.y), fmaf(a.z, sc.z, sh.z), fmaf(a.w, sc.w, sh.w)};
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          if (p.act == ACT_LEAKY) v4[j] = v4[j] > 0.f ? v4[j] : 0.2f * v4[j]; else if (p.act == ACT_RELU) v4[j] = fmaxf(v4[j], 0.f);
-        }
-        const int oy = p.transposed ? my * p.sh + py : my, ox = p.transposed ? mx * p.sw + px : mx;
-        __half2 h0 = __floats2half2_rn(v4[0], v4[1]), h1 = __floats2half2_rn(v4[2], v4[3]);
-        __half* dst = p.out + ((size_t)(b * p.Hout + oy) * p.Wout + ox) * p.Cout + n0 + c4 * 4;
-        *reinterpret_cast<uint2*>(dst) = make_uint2(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1));
-      }
-    }
-    cluster_barrier();                                   // nobody exits (and frees its shared memory) while a peer may still read it
-  }
-  if (kPair) cluster_barrier();                          // nor while the peer may still arrive on its barriers
 }
 
 // split-K reduce + epilogue: out = act((sum over splits of ws[s]) * scale + shift) as fp16, 4 channels per thread.
@@ -331,10 +271,8 @@ template <int BN, int ST> static constexpr size_t tc_smem_bytes() {
 }
 // Kernel configurations (BLOCK_N, stages, CTAs/SM): two co-resident CTAs per SM let one tile's epilogue overlap the other's main
 // loop; both fit 2 x ~98 KB of an H100 SM's 228 KB of shared memory and its 64 K registers (2 x 288 threads x <= 112).
-#define RYK_TC_N128 k_conv_tc<128, 3, 2, false>
-#define RYK_TC_N64 k_conv_tc<64, 4, 2, false>
-#define RYK_TC_PAIR_N128 k_conv_tc<128, 3, 2, true>
-#define RYK_TC_PAIR_N64 k_conv_tc<64, 4, 2, true>
+#define RYK_TC_N128 k_conv_tc<128, 3, 2>
+#define RYK_TC_N64 k_conv_tc<64, 4, 2>
 
 int tc_init() {
   if (!g_encode) {
@@ -346,9 +284,6 @@ int tc_init() {
   }
   RYK_CUDA(cudaFuncSetAttribute(RYK_TC_N128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<128, 3>()));
   RYK_CUDA(cudaFuncSetAttribute(RYK_TC_N64, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<64, 4>()));
-  RYK_CUDA(cudaFuncSetAttribute(RYK_TC_PAIR_N128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<128, 3>()));
-  RYK_CUDA(cudaFuncSetAttribute(RYK_TC_PAIR_N64, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<64, 4>()));
-  if (tc3_init()) return -1;
   return 0;
 }
 
@@ -362,29 +297,7 @@ bool tc_layer_eligible(const ConvLayer& L) {
   return true;
 }
 
-// RYK_TC_CLUSTERK: 1 = split-K layers reduce their partial sums inside the kernel (thread-block cluster + distributed shared memory),
-// 0 (default) = FP32 workspace + k_splitk_reduce launch.
-static bool tc_clusterk() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("RYK_TC_CLUSTERK"); v = (e && atoi(e) != 0) ? 1 : 0; }
-  return v != 0;
-}
-bool tc_layer_clusterk(const ConvLayer& L) { return tc_clusterk() && L.ksplit > 1 && !L.tc2 && !L.tc3; }
-
 static int pow2_floor(int v) { int p = 1; while (p * 2 <= v) p *= 2; return p; }
-
-// RYK_TC2: 0 (default) = never, 1 = CTA pairs where the layer has at least two tiles per CTA slot, 2 = wherever the shape allows
-// (tests).  Read at every plan so that a test can switch it.  Off by default: not measured to be faster on H100.
-static bool tc2_layer_config(const ConvLayer& L, int num_sms) {
-  const char* e = getenv("RYK_TC2");
-  const int mode = e ? atoi(e) : 0;
-  if (mode <= 0 || !tc_layer_eligible(L)) return false;
-  if (mode >= 2) return true;
-  const int Wc = L.transposed ? L.Win : L.Wout, Hc = L.transposed ? L.Hin : L.Hout;
-  const int tw = pow2_floor(Wc < kBlockM ? Wc : kBlockM), th = kBlockM / tw;
-  const int tiles = L.B * ((Wc + tw - 1) / tw) * ((Hc + th - 1) / th) * (L.Cout / (L.Cout >= 128 ? 128 : 64)) * (L.transposed ? L.SH * L.SW : 1);
-  return tiles >= 4 * num_sms;
-}
 
 static int make_act_map(CUtensorMap* m, const void* ptr, int C, int W, int H, int B, int box_w, int box_h, int stride_w, int stride_h) {
   cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
@@ -437,23 +350,20 @@ static void tc_geometry(const ConvLayer& L, int num_sms, int* tile_w, int* tile_
   int ks = 1;
   int slots = num_sms * 2;                            // two co-resident CTAs per SM
   if (tiles < slots) {
+    constexpr int kMinChunks = 8;                       // at least this many K chunks per split
     ks = slots / tiles;
-    static int min_chunks = -1;
-    if (min_chunks < 0) { const char* v = getenv("RYK_TC_MIN_CHUNKS"); min_chunks = v ? atoi(v) : 8; if (min_chunks < 1) min_chunks = 1; }
-    if (ks > total_chunks / min_chunks) ks = total_chunks / min_chunks;   // at least min_chunks chunks per split
+    if (ks > total_chunks / kMinChunks) ks = total_chunks / kMinChunks;
     if (ks < 1) ks = 1;
-    if (tc_clusterk() && ks > 8) ks = 8;                // in-cluster reduction: the splits of a tile form one (portable-size) cluster
     int cps = (total_chunks + ks - 1) / ks;
     ks = (total_chunks + cps - 1) / cps;                // every split owns at least one chunk
   }
-  if (tc2_layer_config(L, num_sms) || tc3_layer_config(L, num_sms, nullptr)) ks = 1;       // pair / halo kernels: no split-K
   *tile_w = tw; *tile_h = th; *block_n = bn; *ksplit = ks;
 }
 
 size_t tc_splitk_ws_bytes(const ConvLayer& L, int num_sms) {
   int tw, th, bn, ks;
   tc_geometry(L, num_sms, &tw, &th, &bn, &ks);
-  return (ks > 1 && !tc_clusterk()) ? (size_t)ks * L.B * L.Hout * L.Wout * L.Cout * sizeof(float) : 0;
+  return ks > 1 ? (size_t)ks * L.B * L.Hout * L.Wout * L.Cout * sizeof(float) : 0;
 }
 
 int tc_layer_prepare(ConvLayer& L, int num_sms) {
@@ -469,50 +379,29 @@ int tc_layer_prepare(ConvLayer& L, int num_sms) {
   size_t K = (size_t)ntaps * (L.C0 + L.C1);
   size_t rows = (size_t)classes * L.Cout;
   if (make_weight_map(&L.tmB, L.w_tc, K, rows, L.block_n)) return -1;
-  L.tc2 = tc2_layer_config(L, num_sms);
-  if (L.tc2) { if (make_weight_map(&L.tmB2, L.w_tc, K, rows, L.block_n / 2)) return -1; }
-  else L.tmB2 = L.tmB;
-  L.tc3 = !L.tc2 && tc3_layer_config(L, num_sms, &L.t3);
-  if (L.tc3 && tc3_layer_prepare(L, g_encode)) return -1;
   // output map for the TMA-store epilogue: deconv classes write every other pixel (element strides = conv strides)
   if (make_act_map(&L.tmO, L.out, L.Cout, L.Wout, L.Hout, L.B, L.tile_w, L.tile_h, L.transposed ? L.SW : 1, L.transposed ? L.SH : 1)) return -1;
-  RYK_CHECK(L.ksplit == 1 || tc_layer_clusterk(L) || L.splitk_ws != nullptr, "split-K layer without a workspace");
-  if (L.ksplit > 1 && !tc_layer_clusterk(L)) {
+  RYK_CHECK(L.ksplit == 1 || L.splitk_ws != nullptr, "split-K layer without a workspace");
+  if (L.ksplit > 1) {
     if (make_ws_map(&L.tmW, L.splitk_ws, L.Cout, L.Wout, L.Hout, L.B, L.ksplit, L.tile_w, L.tile_h, L.transposed ? L.SW : 1, L.transposed ? L.SH : 1)) return -1;
   } else L.tmW = L.tmO;
   L.tc_ready = true;
   return 0;
 }
 
-// Launch with the programmatic-stream-serialization attribute (see pdl_trigger / pdl_wait); RYK_NO_PDL=1 falls back to
-// plain stream order (the device-side instructions are then no-ops).
-static int g_pdl_force = -1;                       // -1: environment decides; 0 / 1: forced (captures that must not carry programmatic edges)
-void tc_force_pdl(int v) { g_pdl_force = v; }
-static bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("RYK_NO_PDL"); v = (e && atoi(e) != 0) ? 0 : 1; }
-  return g_pdl_force >= 0 ? g_pdl_force != 0 : v != 0;
-}
-static int g_cluster_z = 1;                        // cluster dimension along grid z of the next launch_pdl (in-cluster split-K)
-static int g_cluster_x = 1;                        // cluster dimension along grid x of the next launch_pdl (CTA pairs)
+// Launch with the programmatic-stream-serialization attribute (see pdl_trigger / pdl_wait).
 template <typename... KArgs, typename... Args>
 static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[3];
-  int n = 0;
-  if (pdl_enabled()) { attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[n].val.programmaticStreamSerializationAllowed = 1; ++n; }
-  if (g_cluster_z > 1 || g_cluster_x > 1) {
-    attr[n].id = cudaLaunchAttributeClusterDimension;
-    attr[n].val.clusterDim.x = (unsigned)g_cluster_x; attr[n].val.clusterDim.y = 1; attr[n].val.clusterDim.z = (unsigned)g_cluster_z; ++n;
-  }
-  cfg.attrs = attr; cfg.numAttrs = n;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
 int conv_tc_run(const ConvLayer& L, cudaStream_t st) {
   RYK_CHECK(L.tc_ready, "tc layer not prepared");
-  if (L.tc3) return conv_tc3_run(L, st, pdl_enabled());
   TcParams p;
   p.transposed = L.transposed; p.B = L.B; p.Hout = L.Hout; p.Wout = L.Wout; p.Cout = L.Cout;
   p.Hc = L.transposed ? L.Hin : L.Hout; p.Wc = L.transposed ? L.Win : L.Wout;
@@ -527,22 +416,13 @@ int conv_tc_run(const ConvLayer& L, cudaStream_t st) {
   p.ksplit = L.ksplit;
   int total_chunks = p.ntaps * (p.chunks0 + p.chunks1);
   p.chunks_per_split = (total_chunks + L.ksplit - 1) / L.ksplit;
-  p.act = L.act; p.scale = L.scale; p.shift = L.shift; p.out = (__half*)L.out;
-  const bool ck = tc_layer_clusterk(L);
-  p.ws = (L.ksplit > 1 && !ck) ? L.splitk_ws : nullptr;
-  p.cluster_k = ck ? 1 : 0;
-  g_cluster_z = ck ? L.ksplit : 1;
+  p.act = L.act; p.scale = L.scale; p.shift = L.shift;
+  p.ws = L.ksplit > 1 ? L.splitk_ws : nullptr;
   p.out_pixels = (size_t)L.B * L.Hout * L.Wout;
   size_t out_elems = (size_t)L.B * L.Hout * L.Wout * L.Cout;
   dim3 grid(L.B * p.tiles_w * p.tiles_h, L.Cout / L.block_n, classes * L.ksplit);
-  if (L.tc2) {
-    grid.x += grid.x & 1;             // whole pairs; the padding CTA's tile lies past the last image: zero-filled loads, clipped stores
-    g_cluster_x = 2;
-    if (L.block_n == 128) RYK_CUDA(launch_pdl(RYK_TC_PAIR_N128, grid, dim3(kTcThreads), tc_smem_bytes<128, 3>(), st, L.tmA0, L.tmA1, L.tmB, L.tmO, L.tmW, L.tmB2, p));
-    else RYK_CUDA(launch_pdl(RYK_TC_PAIR_N64, grid, dim3(kTcThreads), tc_smem_bytes<64, 4>(), st, L.tmA0, L.tmA1, L.tmB, L.tmO, L.tmW, L.tmB2, p));
-  } else if (L.block_n == 128) RYK_CUDA(launch_pdl(RYK_TC_N128, grid, dim3(kTcThreads), tc_smem_bytes<128, 3>(), st, L.tmA0, L.tmA1, L.tmB, L.tmO, L.tmW, L.tmB2, p));
-  else RYK_CUDA(launch_pdl(RYK_TC_N64, grid, dim3(kTcThreads), tc_smem_bytes<64, 4>(), st, L.tmA0, L.tmA1, L.tmB, L.tmO, L.tmW, L.tmB2, p));
-  g_cluster_z = 1; g_cluster_x = 1;
+  if (L.block_n == 128) RYK_CUDA(launch_pdl(RYK_TC_N128, grid, dim3(kTcThreads), tc_smem_bytes<128, 3>(), st, L.tmA0, L.tmA1, L.tmB, L.tmO, L.tmW, p));
+  else RYK_CUDA(launch_pdl(RYK_TC_N64, grid, dim3(kTcThreads), tc_smem_bytes<64, 4>(), st, L.tmA0, L.tmA1, L.tmB, L.tmO, L.tmW, p));
   RYK_CUDA(cudaGetLastError());
   if (p.ws) {
     size_t total4 = out_elems / 4;

@@ -372,8 +372,7 @@ int s1_fused_init() {
   const int smem = kS1ActBytes + kS1PartialBytes;
   if (cudaFuncSetAttribute(k_s1_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) { cudaGetLastError(); g_s1_cluster = -1; return 0; }
   int want = 16;
-  if (const char* ev = getenv("RYK_S1_CLUSTER")) { const int v = atoi(ev); if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16) want = v; }
-  if (want > 8 && cudaFuncSetAttribute(k_s1_fused, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) { cudaGetLastError(); want = 8; }
+  if (cudaFuncSetAttribute(k_s1_fused, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) { cudaGetLastError(); want = 8; }
   for (; want >= 1; want /= 2) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(want); cfg.blockDim = dim3(kS1Threads); cfg.dynamicSmemBytes = smem;

@@ -17,12 +17,9 @@
 //   stream C2: stage-2 U-Net (the wgmma layers)                                                     of chunk k-1
 //   stream D: slide converted features, synthesizer add/plan/pulse/overlap-add, NaN scrub             of chunk k-2
 // Inter-stage buffers are double-buffered (index = step parity); events order producer/consumer and guard reuse.
-// The only host<->device handshake inside a step is the 8-byte effective-frame count that selects the stage-1
-// plan (T_eff + 128 - T_eff % 128); the gate runs first in stream E so the count is on the host long before
-// stream C needs it.
+// The effective-frame count that selects the stage-1 plan (T_eff + 128 - T_eff % 128) is read on the device by a
+// conditional graph node, so the host never waits inside a step.
 #include <math.h>
-#include <stdio.h>
-#include <chrono>
 #include <stdlib.h>
 #include <string.h>
 #include <map>
@@ -53,9 +50,9 @@ struct Session {
   long long step = 0;              // chunks submitted
   long long collected = 0;         // chunks collected through the host API
   cudaStream_t sE = nullptr, sC = nullptr, sD = nullptr;     // gate | stage 1 | decode
-  // stage 2 of even / odd chunks on two streams with two activation plans (RYK_S2_ALT=0: one): the latency-bound bottleneck layers
-  // (c4-d2: 30 % of a forward's time, a few CTAs each) of one chunk overlap the GPU-filling layers of its neighbour
-  cudaStream_t sC2s[2] = {nullptr, nullptr}; bool two_s2 = false;
+  // stage 2 of even / odd chunks on two streams with two activation plans (a group member uses only the first): the latency-bound
+  // bottleneck layers (c4-d2: 30 % of a forward's time, a few CTAs each) of one chunk overlap the GPU-filling layers of its neighbour
+  cudaStream_t sC2s[2] = {nullptr, nullptr};
   cudaStream_t sA[2] = {nullptr, nullptr};   // WORLD analysis of even / odd chunks: two chunks' analyses may be in flight
   cudaEvent_t ev_gate[kRing];
   cudaEvent_t ev_count[kRing], ev_enc[kRing], ev_cslide[kRing], ev_s1[kRing], ev_conv[kRing], ev_dslide[kRing], ev_dec[kRing];
@@ -78,14 +75,10 @@ struct Session {
   float* d_chunk_fixed = nullptr;      // the chunk the (captured) encode graph reads
   double* d_out_fixed[2];              // blocks written by the (captured) decode graph, by parity
   int* d_n_fixed[2];
-  bool use_graphs = true;
-  bool merge_s2 = false;           // this step: stage-2 prologue + 16 layers + epilogue replayed as ONE graph (no profiling events in between)
-  bool host_prof = false; double host_wait_us = 0.0, host_total_us = 0.0; long long host_steps = 0;   // RYK_HOST_PROF=1
   std::map<int, StageGraph> graphs;
   // stage 1 with the padded-length bucket chosen ON THE DEVICE: one graph per chunk parity = {k_set_bucket -> SWITCH conditional node
   // whose body i is the stage-1 sequence for the padded length 128 i (0: no effective frame)}; no host sync on the submit path
   cudaGraphExec_t s1_switch[2] = {nullptr, nullptr}; long long s1_switch_launches[2][16]; int s1_buckets = 0; int last_bucket = 0;
-  bool device_buckets = false;
   Synth* synth = nullptr;
   DioPlan* dio[2] = {nullptr, nullptr};     // one analysis plan per chunk parity
   std::vector<void*> allocs, pinned;
@@ -231,9 +224,6 @@ static Session* get_session(Engine* e, int id) { return (id >= 0 && id < (int)e-
 
 static void session_free(Session* s) {
   if (!s) return;
-  if (s->host_prof && s->host_steps > 0)
-    fprintf(stderr, "[ryk host prof] %lld steps: %.1f us per step on the host, of which %.1f us waiting for the gate count\n", s->host_steps,
-            s->host_total_us / s->host_steps, s->host_wait_us / s->host_steps);
   for (cudaStream_t st : {s->sE, s->sA[0], s->sA[1], s->sC, s->sC2s[0], s->sC2s[1], s->sD}) if (st) { cudaStreamSynchronize(st); cudaStreamDestroy(st); }
   for (int i = 0; i < kRing; ++i)
     for (cudaEvent_t ev : {s->ev_gate[i], s->ev_pro[i], s->ev_count[i], s->ev_enc[i], s->ev_cslide[i], s->ev_s1[i], s->ev_conv[i], s->ev_dslide[i], s->ev_dec[i]}) if (ev) cudaEventDestroy(ev);
@@ -306,26 +296,9 @@ int session_streams_join(Engine* e) {
 // Every stage of a step is a fixed kernel sequence over fixed buffers (selected by chunk parity, and for stage 1 by the
 // padded effective length), so each variant is stream-captured once and replayed: a step costs ~6 graph launches on
 // the host instead of ~90 kernel launches (the host was the bottleneck at 0.75 ms of launch overhead per 0.78 ms step).
-// RYK_SESSION_SKIP (timing experiments only; results are garbage): bit 0 analysis (E2), 1 stage 1, 2 stage-2 layers 1..14, 3 synthesis
-// Compiled in only with -DRYK_DIAG (RYK_NVCC_EXTRA=-DRYK_DIAG builds a separate diagnostics library): a release libryk.so has no
-// knob that can turn the timed path into a partial one.
-static int session_skip_mask() {
-#ifdef RYK_DIAG
-  static int m = -1;
-  if (m < 0) { const char* v = getenv("RYK_SESSION_SKIP"); m = v ? atoi(v) : 0; }
-  return m;
-#else
-  return 0;
-#endif
-}
+// run_graph captures body() on stream st into g on first use and replays g; e->launches counts the kernels of every replay.
 template <typename F>
-static int run_stage(Engine* e, Session* s, int key, cudaStream_t st, F&& body, bool capture_only = false) {
-  if (const int m = session_skip_mask()) {
-    if (((m & 1) && (key == 2 || key == 3)) || ((m & 2) && key >= 4 && key < 40) || ((m & 4) && (key == 42 || key == 43)) || ((m & 8) && key >= 46 && key <= 49))
-      return 0;
-  }
-  if (!s->use_graphs) return body();
-  StageGraph& g = s->graphs[key];
+static int run_graph(Engine* e, StageGraph& g, cudaStream_t st, F&& body) {
   if (!g.exec) {
     long long before = e->launches;
     cudaGraph_t graph = nullptr;
@@ -339,14 +312,13 @@ static int run_stage(Engine* e, Session* s, int key, cudaStream_t st, F&& body, 
     g.launches = e->launches - before;
     e->launches = before;
   }
-  if (capture_only) return 0;
   RYK_CUDA(cudaGraphLaunch(g.exec, st));
   e->launches += g.launches;
   return 0;
 }
 
-enum { G_E1 = 0, G_E2 = 2, G_S1 = 4 /* + 2 * bucket + parity; bucket 0 = no effective frame, else padded length / 128 (1..15) */,
-       G_S2A = 40, G_S2B = 42, G_S2C = 44, G_D = 46, G_D1 = 48, G_S2M = 50 };
+// keys of Session::graphs (+ chunk parity)
+enum { G_E1 = 0, G_E2 = 2, G_S2A = 40, G_S2B = 42, G_S2C = 44, G_D = 46, G_D1 = 48 };
 
 // value of the SWITCH node = padded effective length / 128 (count[1] / 128), 0 when no frame is effective (count[0] == 0)
 __global__ void k_set_bucket(cudaGraphConditionalHandle handle, const int* __restrict__ count, int n_buckets) {
@@ -357,7 +329,7 @@ __global__ void k_set_bucket(cudaGraphConditionalHandle handle, const int* __res
   }
 }
 
-static int stage1_enqueue(Engine* e, Session* s, int b, int tp1, bool capture_only);
+static int stage1_body(Engine* e, Session* s, int b, int tp1);
 
 // Build the per-parity stage-1 graph with a device-side switch over the padded-length buckets (CUDA conditional nodes, 12.8+).
 static int stage1_build_switch(Engine* e, Session* s, int b) {
@@ -386,14 +358,11 @@ static int stage1_build_switch(Engine* e, Session* s, int b) {
   cp.conditional.size = (unsigned)n_buckets;
   cudaGraphNode_t sw = nullptr;
   RYK_CUDA(cudaGraphAddNode(&sw, graph, &set_node, 1, &cp));
-  const bool saved = s->use_graphs;
   for (int i = 0; i < n_buckets; ++i) {
     cudaGraph_t body = cp.conditional.phGraph_out[i];
     const long long before = e->launches;
     RYK_CUDA(cudaStreamBeginCaptureToGraph(s->sC, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-    s->use_graphs = false;                               // run the body's kernels straight into the capture
-    int rc = stage1_enqueue(e, s, b, i * 128, false);
-    s->use_graphs = saved;
+    int rc = stage1_body(e, s, b, i * 128);
     cudaGraph_t out = nullptr;
     cudaError_t err = cudaStreamEndCapture(s->sC, &out);
     if (rc) return rc;
@@ -407,31 +376,30 @@ static int stage1_build_switch(Engine* e, Session* s, int b) {
 }
 
 // Stage 1 of a chunk of parity b: slide the feature window, (gather ->) 1-D U-Net at padded length tp1 (0: no effective frame,
-// voice_changer.py:32-35 skips the net) -> scatter into the silent template + f0 map, mc2sp.  One graph per (tp1 bucket, parity);
-// all of them are captured when the session is created so that no chunk ever pays for a capture in the middle of a stream.
-static int stage1_enqueue(Engine* e, Session* s, int b, int tp1, bool capture_only) {
+// voice_changer.py:32-35 skips the net) -> scatter into the silent template + f0 map, mc2sp.  Enqueued on stream C while it is
+// captured as one body of the parity's SWITCH graph; every body is captured when the session is created so that no chunk ever
+// pays for a capture in the middle of a stream.
+static int stage1_body(Engine* e, Session* s, int b, int tp1) {
   const int f = b, g = b ^ 1, pe = s->e_enc_frames;
   const ryk_session_config& c = s->cfg;
-  return run_stage(e, s, G_S1 + 2 * (tp1 / 128) + b, s->sC, [&]() -> int {
-        SlideBatch sb; sb.n = 0;
-        slide_add<float>(sb, s->cw_f0[f], s->enc_f0[b] + pe, s->cw_f0[g], s->Tw, s->n_feat, 1);
-        slide_add<float>(sb, s->cw_ap[f], s->enc_ap[b] + (size_t)pe * s->nb, s->cw_ap[g], s->Tw, s->n_feat, s->nb);
-        slide_add<float>(sb, s->cw_mc[f], s->enc_mc[b] + (size_t)pe * s->C, s->cw_mc[g], s->Tw, s->n_feat, s->C);
-        slide_add<uint8_t>(sb, s->cw_voiced[f], s->enc_voiced[b] + pe, s->cw_voiced[g], s->Tw, s->n_feat, 1);
-        if (slide_batch(sb, s->sC)) return -1;
-        e->launches += 1;
-        const float* d_y = nullptr;
-        if (tp1 > 0) {
-          UNetPlan* p1 = nullptr;
-          if (unet_get_plan(e, e->stage1, 1, 1, tp1, e->precision, &p1, s->owner)) return -1;
-          if (stage1_prologue_run(e, s->cw_mc[g], s->d_index[b], s->d_count[b], s->C, (float*)p1->d_in, tp1, s->sC)) return -1;
-          if (unet_forward(e, p1, s->sC)) return -1;
-          d_y = (const float*)p1->d_out;
-        }
-        if (stage1_epilogue_run(e, d_y, s->d_index[b], s->d_mask[b], s->d_count[b], s->Tw, s->C, s->cw_f0[g], s->cw_ap[g], s->cw_voiced[g], s->nb,
-                                kSilentMc0, s->cv_mc_out[b], s->cv_f0_out[b], s->cv_ap_out[b], s->cv_voiced_out[b], s->sC)) return -1;
-        return mc2sp_run(e, s->cv_mc_out[b], s->Tw, c.order, c.fft_length, 1e-16, s->cv_sp_mid[b], nullptr, s->sC);
-      }, capture_only);
+  SlideBatch sb; sb.n = 0;
+  slide_add<float>(sb, s->cw_f0[f], s->enc_f0[b] + pe, s->cw_f0[g], s->Tw, s->n_feat, 1);
+  slide_add<float>(sb, s->cw_ap[f], s->enc_ap[b] + (size_t)pe * s->nb, s->cw_ap[g], s->Tw, s->n_feat, s->nb);
+  slide_add<float>(sb, s->cw_mc[f], s->enc_mc[b] + (size_t)pe * s->C, s->cw_mc[g], s->Tw, s->n_feat, s->C);
+  slide_add<uint8_t>(sb, s->cw_voiced[f], s->enc_voiced[b] + pe, s->cw_voiced[g], s->Tw, s->n_feat, 1);
+  if (slide_batch(sb, s->sC)) return -1;
+  e->launches += 1;
+  const float* d_y = nullptr;
+  if (tp1 > 0) {
+    UNetPlan* p1 = nullptr;
+    if (unet_get_plan(e, e->stage1, 1, 1, tp1, e->precision, &p1, s->owner)) return -1;
+    if (stage1_prologue_run(e, s->cw_mc[g], s->d_index[b], s->d_count[b], s->C, (float*)p1->d_in, tp1, s->sC)) return -1;
+    if (unet_forward(e, p1, s->sC)) return -1;
+    d_y = (const float*)p1->d_out;
+  }
+  if (stage1_epilogue_run(e, d_y, s->d_index[b], s->d_mask[b], s->d_count[b], s->Tw, s->C, s->cw_f0[g], s->cw_ap[g], s->cw_voiced[g], s->nb,
+                          kSilentMc0, s->cv_mc_out[b], s->cv_f0_out[b], s->cv_ap_out[b], s->cv_voiced_out[b], s->sC)) return -1;
+  return mc2sp_run(e, s->cv_mc_out[b], s->Tw, c.order, c.fft_length, 1e-16, s->cv_sp_mid[b], nullptr, s->sC);
 }
 
 // Step k = s->step is enqueued in three parts so that a group can interleave its members:
@@ -448,11 +416,12 @@ static int stage1_enqueue(Engine* e, Session* s, int b, int tp1, bool capture_on
 
 #define TSTAMP(stage, which, stream) do { if (s->stage_times) RYK_CUDA(cudaEventRecord(s->tev[stage][which][r], stream)); } while (0)
 
-#define S2_LOCALS cudaStream_t sC2 = s->sC2s[(s->two_s2 && !s->group) ? b : 0]; const int s2_owner = s->owner + ((s->two_s2 && !s->group && b) ? 3000000 : 0); float* d_colmin = s->d_colmin[(s->two_s2 && !s->group) ? b : 0]; (void)s2_owner; (void)d_colmin;
+#define S2_LOCALS cudaStream_t sC2 = s->sC2s[s->group ? 0 : b]; const int s2_owner = s->owner + ((!s->group && b) ? 3000000 : 0); (void)s2_owner;
 
 static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
   STEP_LOCALS
   S2_LOCALS
+  float* d_colmin = s->d_colmin[s->group ? 0 : b];
 
   // ================= stream E: gate + WORLD analysis =================
   RYK_CUDA(cudaMemcpyAsync(s->d_chunk_fixed, d_chunk_user, sizeof(float) * s->n_wave, cudaMemcpyDeviceToDevice, s->sE));
@@ -461,7 +430,7 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
     RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev_enc[(k - 2) % kRing], 0));     // wave_win[g]: last read by the analysis of k-2
   }
   TSTAMP(0, 0, s->sE);
-  if (run_stage(e, s, G_E1 + b, s->sE, [&]() -> int {
+  if (run_graph(e, s->graphs[G_E1 + b], s->sE, [&]() -> int {
         if (slide<float>(s->wave_win[f], s->d_chunk_fixed, s->wave_win[g], s->Lw, s->n_wave, 1, s->sE)) return -1;
         if (slide<float>(s->cw_wave[f], s->wave_win[g] + (size_t)pe * s->hop, s->cw_wave[g], (size_t)s->Tw * s->hop, (size_t)s->n_feat * s->hop, 1, s->sE)) return -1;
         e->launches += 2;
@@ -478,7 +447,7 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
   RYK_CUDA(cudaStreamWaitEvent(sA, s->ev_gate[r], 0));
   if (k >= 2) RYK_CUDA(cudaStreamWaitEvent(sA, s->ev_cslide[(k - 2) % kRing], 0));   // enc_*[b] consumed by stage 1 of k-2
   TSTAMP(1, 0, sA);
-  if (run_stage(e, s, G_E2 + b, sA, [&]() -> int {
+  if (run_graph(e, s->graphs[G_E2 + b], sA, [&]() -> int {
         if (dio_stonemask_run(e, s->dio[b], s->wave_win[g], sA)) return -1;
         const int n_enc = s->Lw / s->hop;
         e->launches += 13;
@@ -495,23 +464,14 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
     RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev_conv[(k - 2) % kRing], 0));     // cv_sp_mid[b] consumed by stage 2 of k-2
   }
   TSTAMP(2, 0, s->sC);
-  if (s->device_buckets) {
-    // launch-count bookkeeping only (never waits): the newest count that has already arrived tells which body ran last
-    for (int back = 1; back <= 3 && k - back >= 0; ++back) {
-      const int rr = (int)((k - back) % kRing);
-      if (cudaEventQuery(s->ev_count[rr]) == cudaSuccess) { s->last_bucket = s->h_count[rr][0] > 0 ? s->h_count[rr][1] / 128 : 0; break; }
-    }
-    if (s->last_bucket < 0 || s->last_bucket >= s->s1_buckets) s->last_bucket = s->s1_buckets - 1;
-    RYK_CUDA(cudaGraphLaunch(s->s1_switch[b], s->sC));
-    e->launches += s->s1_switch_launches[b][s->last_bucket];
-  } else {
-    const auto t0 = std::chrono::steady_clock::now();
-    RYK_CUDA(cudaEventSynchronize(s->ev_count[r]));                            // effective-frame count of THIS step (RYK_NO_GRAPH / RYK_HOST_BUCKETS path)
-    if (s->host_prof) s->host_wait_us += std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();
-    const int t_eff = s->h_count[r][0], tp1 = s->h_count[r][1];
-    RYK_CHECK(tp1 / 128 < 16, "window too long for the stage-1 graph table");
-    if (stage1_enqueue(e, s, b, t_eff > 0 ? tp1 : 0, false)) return -1;
+  // launch-count bookkeeping only (never waits): the newest count that has already arrived tells which body ran last
+  for (int back = 1; back <= 3 && k - back >= 0; ++back) {
+    const int rr = (int)((k - back) % kRing);
+    if (cudaEventQuery(s->ev_count[rr]) == cudaSuccess) { s->last_bucket = s->h_count[rr][0] > 0 ? s->h_count[rr][1] / 128 : 0; break; }
   }
+  if (s->last_bucket < 0 || s->last_bucket >= s->s1_buckets) s->last_bucket = s->s1_buckets - 1;
+  RYK_CUDA(cudaGraphLaunch(s->s1_switch[b], s->sC));
+  e->launches += s->s1_switch_launches[b][s->last_bucket];
   // NB: enc_*[b] may be overwritten by encode k+2 once this stage's slides ran; the stage-1 graph is short, so the
   // guard event is simply the end of the stage.
   TSTAMP(2, 1, s->sC);
@@ -527,12 +487,12 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
     Group* G = s->group;
     if (G->step >= 1) RYK_CUDA(cudaStreamWaitEvent(sC2, G->ev_fwd[(G->step - 1) % kRing], 0));   // batched input read by forward k-1
     float* dst = (float*)G->p2->d_in + (size_t)s->slot * Tp * 512;
-    if (run_stage(e, s, G_S2A + b, sC2, [&]() -> int { return sr_prologue_run(e, s->cv_sp_mid[b], s->Tw, Tp, s->nb, dst, sC2, d_colmin); })) return -1;
+    if (run_graph(e, s->graphs[G_S2A + b], sC2, [&]() -> int { return sr_prologue_run(e, s->cv_sp_mid[b], s->Tw, Tp, s->nb, dst, sC2, d_colmin); })) return -1;
     RYK_CUDA(cudaEventRecord(s->ev_pro[r], sC2));
   } else {
     UNetPlan* p2 = nullptr;
     if (unet_get_plan(e, e->stage2, 1, Tp, 512, e->precision, &p2, s2_owner)) return -1;
-    if (!s->merge_s2 && run_stage(e, s, G_S2A + b, sC2, [&]() -> int {
+    if (run_graph(e, s->graphs[G_S2A + b], sC2, [&]() -> int {
           if (sr_prologue_run(e, s->cv_sp_mid[b], s->Tw, Tp, s->nb, (float*)p2->d_in, sC2, d_colmin)) return -1;
           return unet_forward(e, p2, sC2, 0, 0);
         })) return -1;
@@ -549,15 +509,7 @@ static int session_mid_single(Engine* e, Session* s, bool was_profiling) {
   if (unet_get_plan(e, e->stage2, 1, Tp, 512, e->precision, &p2, s2_owner)) return -1;
   cudaEvent_t pe0 = nullptr, pe1 = nullptr;
   if (was_profiling) { RYK_CUDA(cudaEventCreate(&pe0)); RYK_CUDA(cudaEventCreate(&pe1)); RYK_CUDA(cudaEventRecord(pe0, sC2)); }
-  if (s->merge_s2) {
-    // whole stage 2 as one graph: no launch gaps between prologue, the 16 layers and the epilogue (PDL chains through)
-    return run_stage(e, s, G_S2M + b, sC2, [&]() -> int {
-      if (sr_prologue_run(e, s->cv_sp_mid[b], s->Tw, Tp, s->nb, (float*)p2->d_in, sC2, d_colmin)) return -1;
-      if (unet_forward(e, p2, sC2, 0, 15)) return -1;
-      return sr_epilogue_run(e, (const float*)p2->d_out, s->Tw, s->nb, s->cv_sp_out[b], sC2);
-    });
-  }
-  if (run_stage(e, s, G_S2B + b, sC2, [&]() -> int { return unet_forward(e, p2, sC2, 1, 14); })) return -1;
+  if (run_graph(e, s->graphs[G_S2B + b], sC2, [&]() -> int { return unet_forward(e, p2, sC2, 1, 14); })) return -1;
   if (was_profiling) { RYK_CUDA(cudaEventRecord(pe1, sC2)); e->prof_events.emplace_back(pe0, pe1); }
   return 0;
 }
@@ -570,11 +522,11 @@ static int session_back(Engine* e, Session* s) {
     Group* G = s->group;
     RYK_CUDA(cudaStreamWaitEvent(sC2, G->ev_fwd[G->step % kRing], 0));
     const float* src = (const float*)G->p2->d_out + (size_t)s->slot * Tp * 512;
-    if (run_stage(e, s, G_S2C + b, sC2, [&]() -> int { return sr_epilogue_run(e, src, s->Tw, s->nb, s->cv_sp_out[b], sC2); })) return -1;
+    if (run_graph(e, s->graphs[G_S2C + b], sC2, [&]() -> int { return sr_epilogue_run(e, src, s->Tw, s->nb, s->cv_sp_out[b], sC2); })) return -1;
   } else {
     UNetPlan* p2 = nullptr;
     if (unet_get_plan(e, e->stage2, 1, Tp, 512, e->precision, &p2, s2_owner)) return -1;
-    if (!s->merge_s2 && run_stage(e, s, G_S2C + b, sC2, [&]() -> int {
+    if (run_graph(e, s->graphs[G_S2C + b], sC2, [&]() -> int {
           if (unet_forward(e, p2, sC2, 15, 15)) return -1;
           return sr_epilogue_run(e, (const float*)p2->d_out, s->Tw, s->nb, s->cv_sp_out[b], sC2);
         })) return -1;
@@ -587,7 +539,7 @@ static int session_back(Engine* e, Session* s) {
   TSTAMP(4, 0, s->sD);
   if (synth_host_advance(e, s->synth, s->Td, s->sD)) return -1;
   const int max_blocks = s->max_blocks;
-  if (run_stage(e, s, G_D1 + b, s->sD, [&]() -> int {
+  if (run_graph(e, s->graphs[G_D1 + b], s->sD, [&]() -> int {
         SlideBatch sb; sb.n = 0;
         slide_add<float>(sb, s->dw_f0[f], s->cv_f0_out[b] + pc, s->dw_f0[g], s->Td, s->n_feat, 1);
         slide_add<float>(sb, s->dw_ap[f], s->cv_ap_out[b] + (size_t)pc * s->nb, s->dw_ap[g], s->Td, s->n_feat, s->nb);
@@ -600,7 +552,7 @@ static int session_back(Engine* e, Session* s) {
       })) return -1;
   // the converted features of this parity are free again as soon as they sit in the decode window
   RYK_CUDA(cudaEventRecord(s->ev_dslide[r], s->sD));
-  if (run_stage(e, s, G_D + b, s->sD, [&]() -> int {
+  if (run_graph(e, s->graphs[G_D + b], s->sD, [&]() -> int {
         if (synth_add_kernel(e, s->synth, s->dec_f0_f64, s->Td, s->dw_sp[g], s->dw_ap[g], s->sD)) return -1;
         if (synth_drain_async(e, s->synth, s->d_out_fixed[b], max_blocks, s->sD)) return -1;
         k_scrub<<<8, 256, 0, s->sD>>>(s->d_out_fixed[b], s->synth->dev.state, c.vocoder_buffer_size, max_blocks * c.vocoder_buffer_size, s->d_n_fixed[b]);
@@ -615,14 +567,8 @@ static int session_back(Engine* e, Session* s) {
 }
 
 static int session_enqueue(Engine* e, Session* s, const float* d_chunk_user) {
-  const auto host_t0 = std::chrono::steady_clock::now();
-  struct HostProf { Session* s; std::chrono::steady_clock::time_point t0;
-    ~HostProf() { if (s->host_prof) { s->host_total_us += std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count(); s->host_steps++; } } } host_prof_guard{s, host_t0};
   const bool was_profiling = e->profile;
   e->profile = false;                                      // the session places its own timing events (between graph launches)
-  // RYK_S2_MERGE=1 (experiment, off by default: +1 % end to end): replay stage 2 as one graph on steps without profiling events
-  { static int merge = -1; if (merge < 0) { const char* v = getenv("RYK_S2_MERGE"); merge = v && atoi(v) ? 1 : 0; }
-    s->merge_s2 = merge && !was_profiling && !s->group && s->use_graphs && session_skip_mask() == 0; }
   int rc = session_front(e, s, d_chunk_user);
   if (!rc) rc = session_mid_single(e, s, was_profiling);
   if (!rc) rc = session_back(e, s);
@@ -641,29 +587,7 @@ static int group_enqueue_impl(Engine* e, Group* G, const float* const* d_chunks,
   }
   cudaEvent_t pe0 = nullptr, pe1 = nullptr;
   if (was_profiling) { RYK_CUDA(cudaEventCreate(&pe0)); RYK_CUDA(cudaEventCreate(&pe1)); RYK_CUDA(cudaEventRecord(pe0, G->sG)); }
-  {
-    StageGraph& g = G->fwd_graph;
-    const bool use_graphs = G->members[0]->use_graphs;
-    if (!use_graphs) {
-      if (unet_forward(e, G->p2, G->sG, 0, 15)) return -1;
-    } else {
-      if (!g.exec) {
-        long long before = e->launches;
-        cudaGraph_t graph = nullptr;
-        RYK_CUDA(cudaStreamBeginCapture(G->sG, cudaStreamCaptureModeThreadLocal));
-        int rc = unet_forward(e, G->p2, G->sG, 0, 15);
-        cudaError_t err = cudaStreamEndCapture(G->sG, &graph);
-        if (rc) return rc;
-        RYK_CUDA(err);
-        RYK_CUDA(cudaGraphInstantiate(&g.exec, graph, 0));
-        RYK_CUDA(cudaGraphDestroy(graph));
-        g.launches = e->launches - before;
-        e->launches = before;
-      }
-      RYK_CUDA(cudaGraphLaunch(g.exec, G->sG));
-      e->launches += g.launches;
-    }
-  }
+  if (run_graph(e, G->fwd_graph, G->sG, [&]() -> int { return unet_forward(e, G->p2, G->sG, 0, 15); })) return -1;
   if (was_profiling) { RYK_CUDA(cudaEventRecord(pe1, G->sG)); e->prof_events.emplace_back(pe0, pe1); }
   RYK_CUDA(cudaEventRecord(G->ev_fwd[r], G->sG));
   for (Session* m : G->members)
@@ -714,26 +638,19 @@ int ryk_session_create(ryk_engine* h, const ryk_session_config* cfg, int* sessio
   if (sptk_prepare(e, cfg->order, cfg->alpha, cfg->fft_length)) return -1;
   // The analysis, stage-1 and synthesis stages are chains of small, latency-bound kernels; stage 2 is bulk work that fills
   // every SM.  Higher stream priority for the former lets their CTAs take freed SM slots first, so their latency does not
-  // inflate behind stage-2 waves (the analysis chain is what the host's per-step count sync waits on).
+  // inflate behind stage-2 waves.
   int prio_lo = 0, prio_hi = 0;
   RYK_CUDA(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));      // lo = least (numerically largest), hi = greatest
-  { const char* v = getenv("RYK_NO_PRIORITY"); if (v && atoi(v)) prio_hi = prio_lo; }
-  // RYK_PRIO="E,A,C,C2,D" (tuning experiments): priority level of each stream as steps above the lowest (0 .. lo - hi)
-  int lv[5] = {prio_lo - prio_hi, prio_lo - prio_hi, prio_lo - prio_hi, 0, prio_lo - prio_hi};
-  if (const char* v = getenv("RYK_PRIO")) sscanf(v, "%d,%d,%d,%d,%d", &lv[0], &lv[1], &lv[2], &lv[3], &lv[4]);
-  auto PR = [&](int i) { int l = lv[i] < 0 ? 0 : (lv[i] > prio_lo - prio_hi ? prio_lo - prio_hi : lv[i]); return prio_lo - l; };
-  RYK_CUDA(cudaStreamCreateWithPriority(&s->sE, cudaStreamNonBlocking, PR(0)));
-  for (int i = 0; i < 2; ++i) RYK_CUDA(cudaStreamCreateWithPriority(&s->sA[i], cudaStreamNonBlocking, PR(1)));
-  RYK_CUDA(cudaStreamCreateWithPriority(&s->sC, cudaStreamNonBlocking, PR(2)));
-  for (int i = 0; i < 2; ++i) RYK_CUDA(cudaStreamCreateWithPriority(&s->sC2s[i], cudaStreamNonBlocking, PR(3)));
-  { const char* v = getenv("RYK_S2_ALT"); s->two_s2 = !(v && atoi(v) == 0); }
-  RYK_CUDA(cudaStreamCreateWithPriority(&s->sD, cudaStreamNonBlocking, PR(4)));
+  RYK_CUDA(cudaStreamCreateWithPriority(&s->sE, cudaStreamNonBlocking, prio_hi));
+  for (int i = 0; i < 2; ++i) RYK_CUDA(cudaStreamCreateWithPriority(&s->sA[i], cudaStreamNonBlocking, prio_hi));
+  RYK_CUDA(cudaStreamCreateWithPriority(&s->sC, cudaStreamNonBlocking, prio_hi));
+  for (int i = 0; i < 2; ++i) RYK_CUDA(cudaStreamCreateWithPriority(&s->sC2s[i], cudaStreamNonBlocking, prio_lo));
+  RYK_CUDA(cudaStreamCreateWithPriority(&s->sD, cudaStreamNonBlocking, prio_hi));
   for (int i = 0; i < kRing; ++i) {
     cudaEvent_t* evs[] = {&s->ev_gate[i], &s->ev_pro[i], &s->ev_count[i], &s->ev_enc[i], &s->ev_cslide[i], &s->ev_s1[i], &s->ev_conv[i], &s->ev_dslide[i], &s->ev_dec[i]};
     for (cudaEvent_t* ev : evs) RYK_CUDA(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
   }
   { const char* v = getenv("RYK_STAGE_TIMES"); s->stage_times = v && atoi(v) != 0; }
-  { const char* v = getenv("RYK_HOST_PROF"); s->host_prof = v && atoi(v) != 0; }
   if (s->stage_times) for (int a = 0; a < 5; ++a) for (int w = 0; w < 2; ++w) for (int i = 0; i < kRing; ++i) RYK_CUDA(cudaEventCreate(&s->tev[a][w][i]));
   // zero-fill on the ENGINE stream: the template fill below (k_fill_rows on e->stream, a non-blocking stream) must be ordered after
   // it -- a legacy-default-stream cudaMemset is not, and could land after the fill (seen once as a 4e-3 RMSE mismatch)
@@ -771,7 +688,6 @@ int ryk_session_create(ryk_engine* h, const ryk_session_config* cfg, int* sessio
   for (int i = 0; i < 2; ++i) if (A((void**)&s->d_colmin[i], sizeof(float) * kColminFloats)) return -1;
   if (A((void**)&s->dec_f0_f64, sizeof(double) * s->Td)) return -1;
   if (A((void**)&s->d_chunk_fixed, sizeof(float) * s->n_wave)) return -1;
-  { const char* ng = getenv("RYK_NO_GRAPH"); s->use_graphs = !(ng && atoi(ng) != 0); }
   s->max_blocks = (s->Td * s->hop) / cfg->vocoder_buffer_size + 4;
   const size_t out_samples = (size_t)s->max_blocks * cfg->vocoder_buffer_size;
   for (int i = 0; i < 2; ++i) {
@@ -799,22 +715,7 @@ int ryk_session_create(ryk_engine* h, const ryk_session_config* cfg, int* sessio
   // (the stage-2 plan is created on first use: a session that joins a group never needs its own)
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   RYK_CUDA(cudaDeviceSynchronize());
-  { const char* hb = getenv("RYK_HOST_BUCKETS"); s->device_buckets = s->use_graphs && !(hb && atoi(hb) != 0); }
-  if (s->device_buckets) {
-    const char* sp = getenv("RYK_S1_PDL");
-    const bool pdl_bodies = !(sp && atoi(sp) == 0);
-    if (!pdl_bodies) tc_force_pdl(0);
-    int rc = 0;
-    for (int b = 0; b < 2 && !rc; ++b) rc = stage1_build_switch(e, s, b);
-    if (!pdl_bodies) tc_force_pdl(-1);
-    if (rc) return rc;
-  } else if (s->use_graphs) {
-    const long long before = e->launches;
-    for (int b = 0; b < 2; ++b)
-      for (int tp1 = 0; tp1 <= s->Tw + (128 - s->Tw % 128); tp1 += 128)
-        if (stage1_enqueue(e, s, b, tp1, true)) return -1;
-    e->launches = before;
-  }
+  for (int b = 0; b < 2; ++b) if (stage1_build_switch(e, s, b)) return -1;
   e->sessions.push_back(s);
   *session_id = (int)e->sessions.size() - 1;
   return 0;

@@ -69,7 +69,7 @@ def load_library() -> ctypes.CDLL:
             if not _LIB_PATH.exists():
                 raise RykError(f'{_LIB_PATH} is missing: run `python -c "import __graft_entry__ as g; g.build()"` '
                                f'(the hot path has no CPU fallback)')
-            # RYK_LIB: a diagnostics build of the same library (e.g. -DRYK_DIAG); never a different implementation
+            # RYK_LIB: another build of the same library (e.g. one compiled with extra nvcc flags); never a different implementation
             lib = ctypes.CDLL(os.environ.get('RYK_LIB') or str(_LIB_PATH))
             lib.ryk_last_error.restype = ctypes.c_char_p
             lib.ryk_engine_launch_count.restype = ctypes.c_longlong
