@@ -58,8 +58,8 @@ int ryk_engine_synchronize(ryk_engine* e);
 int ryk_engine_timer_start(ryk_engine* e);                    /* cudaEventRecord on the engine's stream */
 int ryk_engine_timer_stop(ryk_engine* e, float* elapsed_ms);  /* record + synchronize + elapsed */
 int ryk_engine_profile(ryk_engine* e, int enable);
-int ryk_engine_profile_read(ryk_engine* e, double* stage2_ms_total, int* stage2_runs);
-/* as above plus the UNION of the per-forward intervals (a session alternates its stage-2 forwards between two streams, so they overlap) */
+/* Device time (ms) of the stage-2 k4-layer block over all forwards since the last read: the sum of the per-forward durations and
+ * the UNION of the per-forward intervals (a session alternates its stage-2 forwards between two streams, so they overlap) */
 int ryk_engine_profile_read2(ryk_engine* e, double* stage2_ms_total, double* stage2_ms_union, int* stage2_runs);
 
 /* ---- WORLD analysis (encode) -------------------------------------------------------------- */
@@ -233,23 +233,11 @@ int ryk_group_push_device(ryk_engine* e, int group_id, const float* const* waves
                           int out_capacity, int* const* n_outs_dev);
 
 /* ---- diagnostics -------------------------------------------------------------------------------------- */
-/* Synthesizer pulse ring entries [first, first+count) and state {n_pulses, next_pulse, last_location, synthesized_sample,
- * cumulative_frame, rng_generated, blocks_out}. */
-int ryk_debug_synth_pulses(ryk_engine* e, int synth_id, long long first, int count, long long* index, double* time, int* vuv, long long* state7);
-/* Per-sample time base of the last AddParameters call (interpolated f0, vuv, total phase), first n samples. */
-int ryk_debug_synth_timebase(ryk_engine* e, int synth_id, int n, double* if0, double* ivuv, double* tp);
-/* DIO internals (raw contour before StoneMask, per-band candidates [bands][frames], normalised scores, event counts [bands][4])
- * of the most recent analysis that used the (n, fs, frame_period, f0_floor, f0_ceil) plan. */
-int ryk_debug_dio(ryk_engine* e, int n, int fs, double frame_period_ms, double f0_floor, double f0_ceil,
-                  double* f0_raw, double* cand, double* score, int* counts);
 /* Harvest internals of the most recent analysis with this plan (engine in f0 method 1): info = {channels, 1 ms frames, decimated
  * length, fft size, candidate columns, decimation ratio, used columns}; y [info[2]], raw [channels][frames], cand / score
  * [frames][columns] (after refinement and removal), best / basic [frames], f0_raw [n / hop + 1] (before StoneMask).  Any may be NULL. */
 int ryk_debug_harvest(ryk_engine* e, int n, int fs, double frame_period_ms, double f0_floor, double f0_ceil, int* info, double* y,
                       double* raw, double* cand, double* score, double* best, double* basic, double* f0_raw);
-/* Stage-1 forward of padded length Tp stand-alone: ms per forward as one cluster kernel / as 16 layer launches, and the fused
- * kernel's phase timeline (31 doubles, us). */
-int ryk_debug_stage1_bench(ryk_engine* e, int Tp, int iters, float* ms_fused, float* ms_layered, double* timeline_us);
 /* One conv (transposed = 0) or transposed-conv layer of the U-Nets in isolation, host fp32 NHWC tensors in and
  * out, weights in the Chainer layout; use_tc selects the FP16 wgmma kernel (1) or the FP32 CUDA-core kernel (0).
  * `repeat` extra timed runs report the mean device time per run (ms) -- used by the unit parity tests and ncu. */

@@ -231,9 +231,6 @@ int ryk_engine_profile_read2(ryk_engine* h, double* stage2_ms_total, double* sta
   e->prof_events.clear();
   return 0;
 }
-int ryk_engine_profile_read(ryk_engine* h, double* stage2_ms_total, int* stage2_runs) {
-  return ryk_engine_profile_read2(h, stage2_ms_total, nullptr, stage2_runs);
-}
 
 // device-side stopwatch on the engine's stream (bench.py brackets its timed region with it)
 int ryk_engine_timer_start(ryk_engine* h) {
@@ -662,37 +659,6 @@ int ryk_resample_poly(ryk_engine* h, const float* x, int n, int up, int down, co
   return 0;
 }
 
-// ---- diagnostics: the synthesizer's pulse ring (index, time, vuv) and scalar state
-int ryk_debug_synth_pulses(ryk_engine* h, int id, long long first, int count, long long* index, double* time, int* vuv, long long* state7) {
-  Engine* e = E(h);
-  RYK_CUDA(cudaSetDevice(e->device));
-  Synth* s = get_synth(e, id);
-  RYK_CHECK(s != nullptr, "no such synthesizer");
-  RYK_CUDA(cudaStreamSynchronize(e->stream));
-  SynthState st;
-  RYK_CUDA(cudaMemcpy(&st, s->dev.state, sizeof(st), cudaMemcpyDeviceToHost));
-  state7[0] = st.n_pulses; state7[1] = st.next_pulse; state7[2] = st.last_location; state7[3] = st.synthesized_sample;
-  state7[4] = st.cumulative_frame; state7[5] = st.rng_generated; state7[6] = st.blocks_out;
-  for (int i = 0; i < count; ++i) {
-    int slot = (int)((first + i) % s->dev.cap_pulses);
-    RYK_CUDA(cudaMemcpy(index + i, s->dev.p_index + slot, sizeof(long long), cudaMemcpyDeviceToHost));
-    RYK_CUDA(cudaMemcpy(time + i, s->dev.p_time + slot, sizeof(double), cudaMemcpyDeviceToHost));
-    RYK_CUDA(cudaMemcpy(vuv + i, s->dev.p_vuv + slot, sizeof(int), cudaMemcpyDeviceToHost));
-  }
-  return 0;
-}
-
-int ryk_debug_synth_timebase(ryk_engine* h, int id, int n, double* if0, double* ivuv, double* tp) {
-  Engine* e = E(h);
-  Synth* s = get_synth(e, id);
-  RYK_CHECK(s != nullptr, "no such synthesizer");
-  RYK_CUDA(cudaStreamSynchronize(e->stream));
-  RYK_CUDA(cudaMemcpy(if0, s->dev.if0, sizeof(double) * n, cudaMemcpyDeviceToHost));
-  RYK_CUDA(cudaMemcpy(ivuv, s->dev.ivuv, sizeof(double) * n, cudaMemcpyDeviceToHost));
-  RYK_CUDA(cudaMemcpy(tp, s->dev.tp, sizeof(double) * n, cudaMemcpyDeviceToHost));
-  return 0;
-}
-
 // ---- CREPE f0 front-end (acoustic_feature_wrapper.py:65-80): model upload and crepe.predict + predict_voicing on 16 kHz audio
 int ryk_crepe_create(ryk_engine* h, int capacity_multiplier) { RYK_CUDA(cudaSetDevice(E(h)->device)); return crepe_create(E(h), capacity_multiplier); }
 int ryk_crepe_set_conv(ryk_engine* h, int layer, const float* W, const float* bias, const float* gamma, const float* beta, const float* mean,
@@ -731,26 +697,6 @@ int ryk_debug_harvest(ryk_engine* h, int n, int fs, double fp, double f0_floor, 
   if (dio_get_plan(e, n, fs, fp, f0_floor, f0_ceil, &plan)) return -1;
   if (f0_raw) RYK_CUDA(cudaMemcpyAsync(f0_raw, dio_plan_f0_raw(plan), sizeof(double) * dio_plan_frames(plan), cudaMemcpyDeviceToHost, e->stream));
   return harvest_plan_debug_copy(dio_plan_harvest(plan), info, y, raw, cand, score, best, basic, e->stream);
-}
-
-// ---- diagnostics: stage-1 forward of padded length Tp as one cluster kernel vs 16 layer launches (ms per forward, stand-alone),
-// and the fused kernel's phase timeline (31 values in us: start, after layer 0, {tasks done, barrier passed} x 14, end)
-int ryk_debug_stage1_bench(ryk_engine* h, int Tp, int iters, float* ms_fused, float* ms_layered, double* timeline_us) {
-  Engine* e = E(h);
-  RYK_CUDA(cudaSetDevice(e->device));
-  RYK_CHECK(e->precision == 1 && Tp > 0 && Tp % 128 == 0 && iters > 0, "needs FP16 mode and a padded length (multiple of 128)");
-  UNetPlan* plan = nullptr;
-  if (stage1_plan_for(e, Tp, &plan)) return -1;
-  return s1_fused_bench(e, plan, iters, ms_fused, ms_layered, timeline_us);
-}
-
-// ---- diagnostics: DIO internals of the last ryk_world_f0 / ryk_world_analyze call with this (n, fs, ...) plan
-int ryk_debug_dio(ryk_engine* h, int n, int fs, double fp, double f0_floor, double f0_ceil, double* f0_raw, double* cand, double* score, int* counts) {
-  Engine* e = E(h);
-  RYK_CUDA(cudaSetDevice(e->device));
-  DioPlan* plan = nullptr;
-  if (dio_get_plan(e, n, fs, fp, f0_floor, f0_ceil, &plan)) return -1;
-  return dio_plan_debug_copy(plan, f0_raw, cand, score, counts, e->stream);
 }
 
 // ---- diagnostics: one conv / transposed-conv layer in isolation (unit parity + profiling) -------

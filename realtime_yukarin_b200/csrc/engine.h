@@ -52,6 +52,7 @@ struct Engine {
   void* h_pinned = nullptr; size_t pinned_bytes = 0;
   // counters
   long long launches = 0;
+  int plan_owners = 0;               // U-Net plan owner ids handed out to sessions and groups (0 is the engine's own plans)
   // optional device-side timing of the stage-2 tensor-core layers (bench roofline): event pairs per forward
   bool profile = false;
   cudaEvent_t timer_ev[2] = {nullptr, nullptr};
@@ -86,9 +87,6 @@ int crepe_set_dense(Engine* e, const float* W, const float* bias);
 int crepe_set_tables(Engine* e, const double* log_trans, const double* cents_mapping, double log_start, double log_emit_self, double log_emit_other);
 int crepe_num_frames(int n16, double step_ms);
 int crepe_predict(Engine* e, const float* audio16k, int n, double step_ms, double* f0, float* confidence, int* voicing, float* activation, int* path_out);
-// s1_fused.cu diagnostics
-int s1_fused_bench(Engine* e, UNetPlan* p, int iters, float* ms_fused, float* ms_layered, double* timeline_us);
-int dio_plan_debug_copy(DioPlan* p, double* f0_raw, double* cand, double* score, int* counts, cudaStream_t st);
 int spectral_analysis_run(Engine* e, const float* d_x, int n, int fs, double frame_period, const double* d_f0, int n_out,
                           int fft_size, int order, float* d_sp, float* d_ap, float* d_mc, float* d_f0_out, uint8_t* d_voiced,
                           cudaStream_t st);

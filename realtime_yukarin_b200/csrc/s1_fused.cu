@@ -42,7 +42,6 @@ struct S1Params {
   const float* x; const float* w0; const float* sc0; const float* sh0; __half* enc0; int in_ch, base, act0;
   const __half* yin0; const __half* yin1; const float* w15; const float* sc15; const float* sh15; float* y; int yc0, yc1, out_ch, act15;
   int W;
-  unsigned long long* dbg;            // nullable: 31 timestamps (ns) of CTA 0 -- start, after layer 0, {tasks, barrier} x 14, end
 };
 
 __device__ __forceinline__ uint32_t cluster_size() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_nctaid.x;" : "=r"(r)); return r; }
@@ -258,16 +257,12 @@ __device__ __forceinline__ void s1_layer(const S1LayerP& L, int rank, int nc, __
   carry.valid = false;
 }
 
-__device__ __forceinline__ unsigned long long s1_now() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
-
 __global__ void __launch_bounds__(kS1Threads, 1) k_s1_fused(const __grid_constant__ S1Params P) {
   extern __shared__ __align__(128) unsigned char s1_smem[];
   __half* act = reinterpret_cast<__half*>(s1_smem);
   float* partial = reinterpret_cast<float*>(s1_smem + kS1ActBytes);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int rank = (int)cluster_rank(), nc = (int)cluster_size();
-  const bool stamp = P.dbg != nullptr && rank == 0 && tid == 0;      // diagnostics: per-phase timeline of CTA 0 (ns)
-  if (stamp) P.dbg[0] = s1_now();
   for (int l = 0; l < 3; ++l) s1_prefetch_layer(P.L[l], rank, nc);
   // ---- layer 0: conv k3 s1 p1, in_ch -> base, FP32 input, LeakyReLU, FP16 output (input rows and weights staged in smem) ----
   {
@@ -294,15 +289,12 @@ __global__ void __launch_bounds__(kS1Threads, 1) k_s1_fused(const __grid_constan
   cluster_arrive();
   s1_first_of_layer(P.L[0], rank, nc, warp, lane, carry);           // weights do not depend on the activations being exchanged
   cluster_wait();
-  if (stamp) P.dbg[1] = s1_now();
   for (int l = 0; l < 14; ++l) {
     s1_layer(P.L[l], rank, nc, act, partial, carry);
-    if (stamp) P.dbg[2 + 2 * l] = s1_now();
     cluster_arrive();
     if (l + 3 < 14) s1_prefetch_layer(P.L[l + 3], rank, nc);
     if (l + 1 < 14) s1_first_of_layer(P.L[l + 1], rank, nc, warp, lane, carry);
     cluster_wait();
-    if (stamp) P.dbg[3 + 2 * l] = s1_now();
   }
   // ---- layer 15: conv k3 s1 p1 over the concatenation (yc0 + yc1 channels) -> out_ch, FP32 output; one warp per output pixel,
   //      weights staged in shared memory ----
@@ -340,7 +332,6 @@ __global__ void __launch_bounds__(kS1Threads, 1) k_s1_fused(const __grid_constan
       if (lane < P.out_ch) P.y[(size_t)px * P.out_ch + lane] = apply_act(fmaf(mine, __ldg(P.sc15 + lane), __ldg(P.sh15 + lane)), P.act15);
     }
   }
-  if (stamp) P.dbg[30] = s1_now();
 }
 
 // ---- host side -----------------------------------------------------------------------------------------------------------------
@@ -363,7 +354,6 @@ int s1_pack_weights(const float* d_w_chainer, int transposed, int Cin, int Cout,
 }
 
 static int g_s1_cluster = 0;     // 0: not initialised, -1: unavailable, else the cluster size
-static unsigned long long* g_s1_dbg = nullptr;      // device buffer of 32 timestamps while a diagnostic run is active
 
 static bool pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
@@ -428,7 +418,6 @@ int s1_fused_run(Engine* e, const UNetPlan* p, cudaStream_t st) {
   P.yin0 = (const __half*)Z.in0; P.yin1 = (const __half*)Z.in1; P.w15 = Z.w_direct; P.sc15 = Z.scale; P.sh15 = Z.shift; P.y = (float*)Z.out;
   P.yc0 = Z.C0; P.yc1 = Z.C1; P.out_ch = Z.Cout; P.act15 = Z.act;
   P.W = p->W;
-  P.dbg = g_s1_dbg;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(g_s1_cluster); cfg.blockDim = dim3(kS1Threads); cfg.dynamicSmemBytes = kS1ActBytes + kS1PartialBytes; cfg.stream = st;
   cudaLaunchAttribute at[1];
@@ -440,38 +429,5 @@ int s1_fused_run(Engine* e, const UNetPlan* p, cudaStream_t st) {
 }
 
 int s1_fused_cluster_size() { return g_s1_cluster; }
-
-// Diagnostics: `iters` back-to-back forwards of the plan's 16 layers on the engine stream, fused and layered, timed with CUDA events
-// (ms per forward), plus the phase timeline of the last fused forward (31 device timestamps in ns, relative to the first).
-int s1_fused_bench(Engine* e, UNetPlan* p, int iters, float* ms_fused, float* ms_layered, double* timeline_us) {
-  RYK_CHECK(p->fused && g_s1_cluster > 0, "plan cannot run fused");
-  cudaEvent_t ev0, ev1;
-  RYK_CUDA(cudaEventCreate(&ev0)); RYK_CUDA(cudaEventCreate(&ev1));
-  const bool keep = e->s1_fused;
-  for (int mode = 0; mode < 2; ++mode) {
-    e->s1_fused = mode == 0;
-    for (int i = 0; i < 3; ++i) if (unet_forward(e, p, e->stream)) return -1;
-    RYK_CUDA(cudaEventRecord(ev0, e->stream));
-    for (int i = 0; i < iters; ++i) if (unet_forward(e, p, e->stream)) return -1;
-    RYK_CUDA(cudaEventRecord(ev1, e->stream));
-    RYK_CUDA(cudaEventSynchronize(ev1));
-    float ms = 0.f;
-    RYK_CUDA(cudaEventElapsedTime(&ms, ev0, ev1));
-    *(mode == 0 ? ms_fused : ms_layered) = ms / iters;
-  }
-  e->s1_fused = true;
-  RYK_CUDA(cudaMalloc(&g_s1_dbg, sizeof(unsigned long long) * 32));
-  RYK_CUDA(cudaMemsetAsync(g_s1_dbg, 0, sizeof(unsigned long long) * 32, e->stream));
-  int rc = unet_forward(e, p, e->stream);
-  unsigned long long h[32];
-  RYK_CUDA(cudaMemcpyAsync(h, g_s1_dbg, sizeof(h), cudaMemcpyDeviceToHost, e->stream));
-  RYK_CUDA(cudaStreamSynchronize(e->stream));
-  cudaFree(g_s1_dbg); g_s1_dbg = nullptr;
-  e->s1_fused = keep;
-  cudaEventDestroy(ev0); cudaEventDestroy(ev1);
-  if (rc) return rc;
-  for (int i = 0; i < 31; ++i) timeline_us[i] = h[i] >= h[0] ? (double)(h[i] - h[0]) * 1e-3 : -1.0;
-  return 0;
-}
 
 }  // namespace ryk

@@ -22,7 +22,7 @@
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
-#include <map>
+#include <array>
 #include <vector>
 
 #include "../../include/ryk.h"
@@ -35,18 +35,50 @@ namespace ryk {
 
 constexpr int kRing = 8;          // event / output-slot ring (pipeline depth is bounded by the buffer guards below)
 
-struct StageGraph { cudaGraphExec_t exec = nullptr; long long launches = 0; };
+// One captured stage of a step (see run_graph).  Destroying it drops the executable graph.
+struct StageGraph {
+  cudaGraphExec_t exec = nullptr; long long launches = 0;
+  StageGraph() = default;
+  StageGraph(const StageGraph&) = delete;
+  StageGraph& operator=(const StageGraph&) = delete;
+  ~StageGraph() { reset(); }
+  void reset() { if (exec) cudaGraphExecDestroy(exec); exec = nullptr; launches = 0; }
+};
+// The stage graphs of the chunks of one parity, in step order (stage 1 is the separate SWITCH graph Session::s1_switch).
+struct ParityGraphs {
+  StageGraph gate;         // stream E: wave slides + silence gate
+  StageGraph analysis;     // stream A: DIO/Harvest + StoneMask, CheapTrick, D4C
+  StageGraph s2_pro;       // stage-2 prologue (single session: + layer 0; group member: into the group's batched input)
+  StageGraph s2_layers;    // single session: stage-2 layers 1..14
+  StageGraph s2_epi;       // stage-2 epilogue (single session: layer 15 +; group member: from the group's batched output)
+  StageGraph dec_slide;    // stream D: decode-window slides
+  StageGraph synth;        // stream D: synthesizer + NaN scrub
+};
+// Events of one ring slot r = step % kRing.  Null until created, so a partly built session can be freed.
+struct StepEvents {
+  cudaEvent_t gate = nullptr;      // gate of step r done (stream E)
+  cudaEvent_t count = nullptr;     // effective-frame count of step r copied to the host (launch bookkeeping only)
+  cudaEvent_t enc = nullptr;       // analysis of step r done
+  cudaEvent_t cslide = nullptr;    // stage 1 of step r has consumed the analysis outputs
+  cudaEvent_t s1 = nullptr;        // stage 1 of step r done
+  cudaEvent_t pro = nullptr;       // stage-2 prologue of step r done (group members only)
+  cudaEvent_t conv = nullptr;      // stage 2 of step r done
+  cudaEvent_t dslide = nullptr;    // the converted features of step r sit in the decode window
+  cudaEvent_t dec = nullptr;       // output of step r staged (after the copies the entry point appends to stream D)
+  std::array<cudaEvent_t*, 9> all() { return {&gate, &count, &enc, &cslide, &s1, &pro, &conv, &dslide, &dec}; }
+};
 struct Group;
 struct Session {
   // optional per-stage device timing (RYK_STAGE_TIMES=1): [stage E1,E2,S1,S2,D][begin/end][ring]
   cudaEvent_t tev[5][2][kRing]; bool stage_times = false;
-  int owner = 0;                               // plan-cache owner id (activation buffers are private to the session)
+  // plan-cache owner ids (activation buffers are private to the session): stage 1, and stage 2 of even / odd chunks
+  int s1_owner = 0, s2_owner[2] = {0, 0};
   float* d_colmin[2] = {nullptr, nullptr};
   Group* group = nullptr; int slot = 0;        // member of a batched stage-2 group (config 5), else nullptr
-  cudaEvent_t ev_pro[kRing];                   // stage-2 prologue of step r done (group members only)
   ryk_session_config cfg;
   int hop, rate, n_wave, n_feat, e_wave, e_enc_frames, e_conv, e_dec;
   int Lw, Tw, Td, nb, C;
+  int Tp;                          // stage-2 padded length: Tw rounded up to the next multiple of 128 (always > Tw)
   long long step = 0;              // chunks submitted
   long long collected = 0;         // chunks collected through the host API
   cudaStream_t sE = nullptr, sC = nullptr, sD = nullptr;     // gate | stage 1 | decode
@@ -54,8 +86,8 @@ struct Session {
   // bottleneck layers (c4-d2: 30 % of a forward's time, a few CTAs each) of one chunk overlap the GPU-filling layers of its neighbour
   cudaStream_t sC2s[2] = {nullptr, nullptr};
   cudaStream_t sA[2] = {nullptr, nullptr};   // WORLD analysis of even / odd chunks: two chunks' analyses may be in flight
-  cudaEvent_t ev_gate[kRing];
-  cudaEvent_t ev_count[kRing], ev_enc[kRing], ev_cslide[kRing], ev_s1[kRing], ev_conv[kRing], ev_dslide[kRing], ev_dec[kRing];
+  std::array<cudaStream_t, 7> streams() const { return {sE, sA[0], sA[1], sC, sC2s[0], sC2s[1], sD}; }
+  StepEvents ev[kRing];
   // sliding windows, double-buffered by step parity
   float* wave_win[2];
   float *cw_f0[2], *cw_ap[2], *cw_mc[2], *cw_wave[2]; uint8_t* cw_voiced[2];
@@ -75,12 +107,12 @@ struct Session {
   float* d_chunk_fixed = nullptr;      // the chunk the (captured) encode graph reads
   double* d_out_fixed[2];              // blocks written by the (captured) decode graph, by parity
   int* d_n_fixed[2];
-  std::map<int, StageGraph> graphs;
+  ParityGraphs graphs[2];
   // stage 1 with the padded-length bucket chosen ON THE DEVICE: one graph per chunk parity = {k_set_bucket -> SWITCH conditional node
   // whose body i is the stage-1 sequence for the padded length 128 i (0: no effective frame)}; no host sync on the submit path
   cudaGraphExec_t s1_switch[2] = {nullptr, nullptr}; long long s1_switch_launches[2][16]; int s1_buckets = 0; int last_bucket = 0;
   Synth* synth = nullptr;
-  DioPlan* dio[2] = {nullptr, nullptr};     // one analysis plan per chunk parity
+  DioPlan* dio[2] = {nullptr, nullptr};     // one analysis plan per chunk parity (owned)
   std::vector<void*> allocs, pinned;
 };
 
@@ -89,10 +121,10 @@ struct Session {
 // stages carry per-stream state and data-dependent lengths, and they are a small share of the SM time.
 struct Group {
   std::vector<Session*> members;
-  int Tp = 0, owner = 0;
+  int owner = 0;                               // plan-cache owner id of p2
   UNetPlan* p2 = nullptr;                      // stage-2 plan at batch = members.size()
   cudaStream_t sG = nullptr;
-  cudaEvent_t ev_fwd[kRing];                   // batched forward of step r done
+  cudaEvent_t ev_fwd[kRing] = {};              // batched forward of step r done
   long long step = 0, collected = 0;
   StageGraph fwd_graph;
 };
@@ -224,28 +256,27 @@ static Session* get_session(Engine* e, int id) { return (id >= 0 && id < (int)e-
 
 static void session_free(Session* s) {
   if (!s) return;
-  for (cudaStream_t st : {s->sE, s->sA[0], s->sA[1], s->sC, s->sC2s[0], s->sC2s[1], s->sD}) if (st) { cudaStreamSynchronize(st); cudaStreamDestroy(st); }
-  for (int i = 0; i < kRing; ++i)
-    for (cudaEvent_t ev : {s->ev_gate[i], s->ev_pro[i], s->ev_count[i], s->ev_enc[i], s->ev_cslide[i], s->ev_s1[i], s->ev_conv[i], s->ev_dslide[i], s->ev_dec[i]}) if (ev) cudaEventDestroy(ev);
-  for (auto& kv : s->graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+  for (cudaStream_t st : s->streams()) if (st) { cudaStreamSynchronize(st); cudaStreamDestroy(st); }
+  for (StepEvents& ev : s->ev)
+    for (cudaEvent_t* p : ev.all()) if (*p) cudaEventDestroy(*p);
   for (int b = 0; b < 2; ++b) if (s->s1_switch[b]) cudaGraphExecDestroy(s->s1_switch[b]);
   if (s->stage_times) for (int a = 0; a < 5; ++a) for (int w = 0; w < 2; ++w) for (int i = 0; i < kRing; ++i) cudaEventDestroy(s->tev[a][w][i]);
   for (void* p : s->allocs) cudaFree(p);
   for (void* p : s->pinned) cudaFreeHost(p);
+  for (DioPlan* p : s->dio) dio_plan_free(p);
   synth_destroy(s->synth);
-  delete s;
+  delete s;                                       // drops the stage graphs
 }
 
 static void group_free(Group* G) {
   if (!G) return;
   if (G->sG) { cudaStreamSynchronize(G->sG); cudaStreamDestroy(G->sG); }
   for (int i = 0; i < kRing; ++i) if (G->ev_fwd[i]) cudaEventDestroy(G->ev_fwd[i]);
-  if (G->fwd_graph.exec) cudaGraphExecDestroy(G->fwd_graph.exec);
   for (Session* m : G->members) {
     m->group = nullptr;
-    for (int key = 40; key < 46; ++key) {          // the captured stage-2 prologue / epilogue graphs point into the group's plan
-      auto it = m->graphs.find(key);
-      if (it != m->graphs.end()) { if (it->second.exec) cudaGraphExecDestroy(it->second.exec); m->graphs.erase(it); }
+    for (ParityGraphs& pg : m->graphs) {          // the captured stage-2 prologue / epilogue graphs point into the group's plan
+      pg.s2_pro.reset();
+      pg.s2_epi.reset();
     }
   }
   delete G;
@@ -264,7 +295,7 @@ void session_destroy_all(Engine* e) {
 int session_streams_fork(Engine* e, cudaEvent_t ev) {
   for (Session* s : e->sessions) {
     if (!s) continue;
-    for (cudaStream_t st : {s->sE, s->sA[0], s->sA[1], s->sC, s->sC2s[0], s->sC2s[1], s->sD}) RYK_CUDA(cudaStreamWaitEvent(st, ev, 0));
+    for (cudaStream_t st : s->streams()) RYK_CUDA(cudaStreamWaitEvent(st, ev, 0));
   }
   for (Group* G : e->groups) if (G) RYK_CUDA(cudaStreamWaitEvent(G->sG, ev, 0));
   return 0;
@@ -273,7 +304,7 @@ int session_streams_fork(Engine* e, cudaEvent_t ev) {
 int session_streams_join(Engine* e) {
   for (Session* s : e->sessions) {
     if (!s) continue;
-    for (cudaStream_t st : {s->sE, s->sA[0], s->sA[1], s->sC, s->sC2s[0], s->sC2s[1], s->sD}) {
+    for (cudaStream_t st : s->streams()) {
       cudaEvent_t ev;
       RYK_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
       RYK_CUDA(cudaEventRecord(ev, st));
@@ -317,9 +348,6 @@ static int run_graph(Engine* e, StageGraph& g, cudaStream_t st, F&& body) {
   return 0;
 }
 
-// keys of Session::graphs (+ chunk parity)
-enum { G_E1 = 0, G_E2 = 2, G_S2A = 40, G_S2B = 42, G_S2C = 44, G_D = 46, G_D1 = 48 };
-
 // value of the SWITCH node = padded effective length / 128 (count[1] / 128), 0 when no frame is effective (count[0] == 0)
 __global__ void k_set_bucket(cudaGraphConditionalHandle handle, const int* __restrict__ count, int n_buckets) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
@@ -333,7 +361,7 @@ static int stage1_body(Engine* e, Session* s, int b, int tp1);
 
 // Build the per-parity stage-1 graph with a device-side switch over the padded-length buckets (CUDA conditional nodes, 12.8+).
 static int stage1_build_switch(Engine* e, Session* s, int b) {
-  const int n_buckets = (s->Tw + (128 - s->Tw % 128)) / 128 + 1;
+  const int n_buckets = s->Tp / 128 + 1;
   RYK_CHECK(n_buckets <= 16, "window too long for the stage-1 graph table");
   s->s1_buckets = n_buckets;
   cudaGraph_t graph = nullptr;
@@ -392,7 +420,7 @@ static int stage1_body(Engine* e, Session* s, int b, int tp1) {
   const float* d_y = nullptr;
   if (tp1 > 0) {
     UNetPlan* p1 = nullptr;
-    if (unet_get_plan(e, e->stage1, 1, 1, tp1, e->precision, &p1, s->owner)) return -1;
+    if (unet_get_plan(e, e->stage1, 1, 1, tp1, e->precision, &p1, s->s1_owner)) return -1;
     if (stage1_prologue_run(e, s->cw_mc[g], s->d_index[b], s->d_count[b], s->C, (float*)p1->d_in, tp1, s->sC)) return -1;
     if (unet_forward(e, p1, s->sC)) return -1;
     d_y = (const float*)p1->d_out;
@@ -406,94 +434,100 @@ static int stage1_body(Engine* e, Session* s, int b, int tp1) {
 //   front: streams E and C (analysis, gate, stage 1, mc2sp) and the stage-2 prologue
 //   mid:   the stage-2 U-Net forward (single session: on its own stream C2; group: one batched forward on the group stream)
 //   back:  stage-2 epilogue and stream D (synthesizer); results land in s->d_out_fixed[b] / s->d_n_fixed[b]; s->step advances.
-#define STEP_LOCALS                                                                                         \
-  const long long k = s->step;                                                                              \
-  const int b = (int)(k & 1), f = b, g = b ^ 1; /* windows: read [f], write [g]; inter-stage sets: [b] */    \
-  const int r = (int)(k % kRing);                                                                           \
-  const ryk_session_config& c = s->cfg;                                                                     \
-  const int pe = s->e_enc_frames, pc = s->e_conv;                                                           \
-  (void)f; (void)g; (void)r; (void)c; (void)pe; (void)pc;
+// In each part b = k & 1 selects the inter-stage buffer set; the sliding windows are read from [f] = [b] and written to [g] = [b ^ 1];
+// r = k % kRing is the event slot.
 
-#define TSTAMP(stage, which, stream) do { if (s->stage_times) RYK_CUDA(cudaEventRecord(s->tev[stage][which][r], stream)); } while (0)
+// stage 2 of a single session alternates its stream (and plan) by chunk parity; a group member always uses the first stream
+static cudaStream_t s2_stream(const Session* s, int b) { return s->sC2s[s->group ? 0 : b]; }
+static int s2_plan(Engine* e, const Session* s, int b, UNetPlan** p2) {
+  return unet_get_plan(e, e->stage2, 1, s->Tp, 512, e->precision, p2, s->s2_owner[b]);
+}
 
-#define S2_LOCALS cudaStream_t sC2 = s->sC2s[s->group ? 0 : b]; const int s2_owner = s->owner + ((!s->group && b) ? 3000000 : 0); (void)s2_owner;
+// begin (which = 0) / end (1) of a stage in the RYK_STAGE_TIMES timeline
+static int stage_time(Session* s, int stage, int which, int r, cudaStream_t st) {
+  if (s->stage_times) RYK_CUDA(cudaEventRecord(s->tev[stage][which][r], st));
+  return 0;
+}
 
 static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
-  STEP_LOCALS
-  S2_LOCALS
+  const long long k = s->step;
+  const int b = (int)(k & 1), f = b, g = b ^ 1, r = (int)(k % kRing);
+  const ryk_session_config& c = s->cfg;
+  const int pe = s->e_enc_frames;
+  cudaStream_t sC2 = s2_stream(s, b);
   float* d_colmin = s->d_colmin[s->group ? 0 : b];
+  ParityGraphs& pg = s->graphs[b];
 
   // ================= stream E: gate + WORLD analysis =================
   RYK_CUDA(cudaMemcpyAsync(s->d_chunk_fixed, d_chunk_user, sizeof(float) * s->n_wave, cudaMemcpyDeviceToDevice, s->sE));
   if (k >= 2) {
-    RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev_s1[(k - 2) % kRing], 0));      // mask/index/count[b]: last read by stage 1 of k-2
-    RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev_enc[(k - 2) % kRing], 0));     // wave_win[g]: last read by the analysis of k-2
+    RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev[(k - 2) % kRing].s1, 0));      // mask/index/count[b]: last read by stage 1 of k-2
+    RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev[(k - 2) % kRing].enc, 0));     // wave_win[g]: last read by the analysis of k-2
   }
-  TSTAMP(0, 0, s->sE);
-  if (run_graph(e, s->graphs[G_E1 + b], s->sE, [&]() -> int {
+  if (stage_time(s, 0, 0, r, s->sE)) return -1;
+  if (run_graph(e, pg.gate, s->sE, [&]() -> int {
         if (slide<float>(s->wave_win[f], s->d_chunk_fixed, s->wave_win[g], s->Lw, s->n_wave, 1, s->sE)) return -1;
         if (slide<float>(s->cw_wave[f], s->wave_win[g] + (size_t)pe * s->hop, s->cw_wave[g], (size_t)s->Tw * s->hop, (size_t)s->n_feat * s->hop, 1, s->sE)) return -1;
         e->launches += 2;
         return gate_mask_run(e, s->cw_wave[g], s->Tw * s->hop, c.fft_length, s->hop, c.threshold_db, s->Tw, s->d_mse, s->d_mask[b], s->d_index[b],
                              s->d_count[b], s->sE);
       })) return -1;
-  TSTAMP(0, 1, s->sE);
+  if (stage_time(s, 0, 1, r, s->sE)) return -1;
   RYK_CUDA(cudaMemcpyAsync(s->h_count[r], s->d_count[b], sizeof(int) * 2, cudaMemcpyDeviceToHost, s->sE));
-  RYK_CUDA(cudaEventRecord(s->ev_count[r], s->sE));
-  RYK_CUDA(cudaEventRecord(s->ev_gate[r], s->sE));
+  RYK_CUDA(cudaEventRecord(s->ev[r].count, s->sE));
+  RYK_CUDA(cudaEventRecord(s->ev[r].gate, s->sE));
 
   // ================= stream A[b]: WORLD analysis (the chunks of one parity share a plan and a stream) =================
   cudaStream_t sA = s->sA[b];
-  RYK_CUDA(cudaStreamWaitEvent(sA, s->ev_gate[r], 0));
-  if (k >= 2) RYK_CUDA(cudaStreamWaitEvent(sA, s->ev_cslide[(k - 2) % kRing], 0));   // enc_*[b] consumed by stage 1 of k-2
-  TSTAMP(1, 0, sA);
-  if (run_graph(e, s->graphs[G_E2 + b], sA, [&]() -> int {
+  RYK_CUDA(cudaStreamWaitEvent(sA, s->ev[r].gate, 0));
+  if (k >= 2) RYK_CUDA(cudaStreamWaitEvent(sA, s->ev[(k - 2) % kRing].cslide, 0));   // enc_*[b] consumed by stage 1 of k-2
+  if (stage_time(s, 1, 0, r, sA)) return -1;
+  if (run_graph(e, pg.analysis, sA, [&]() -> int {
         if (dio_stonemask_run(e, s->dio[b], s->wave_win[g], sA)) return -1;
         const int n_enc = s->Lw / s->hop;
         e->launches += 13;
         return spectral_analysis_run(e, s->wave_win[g], s->Lw, c.fs, c.frame_period_ms, dio_plan_f0(s->dio[b]), n_enc, c.fft_length, c.order,
                                      s->enc_sp[b], s->enc_ap[b], s->enc_mc[b], s->enc_f0[b], s->enc_voiced[b], sA);
       })) return -1;
-  TSTAMP(1, 1, sA);
-  RYK_CUDA(cudaEventRecord(s->ev_enc[r], sA));
+  if (stage_time(s, 1, 1, r, sA)) return -1;
+  RYK_CUDA(cudaEventRecord(s->ev[r].enc, sA));
 
   // ================= stream C: stage 1 (+ f0 map, mc2sp) =================
-  RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev_enc[r], 0));
+  RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[r].enc, 0));
   if (k >= 2) {
-    RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev_dslide[(k - 2) % kRing], 0));   // cv_{f0,ap,voiced}_out[b] consumed by decode k-2
-    RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev_conv[(k - 2) % kRing], 0));     // cv_sp_mid[b] consumed by stage 2 of k-2
+    RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[(k - 2) % kRing].dslide, 0));   // cv_{f0,ap,voiced}_out[b] consumed by decode k-2
+    RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[(k - 2) % kRing].conv, 0));     // cv_sp_mid[b] consumed by stage 2 of k-2
   }
-  TSTAMP(2, 0, s->sC);
+  if (stage_time(s, 2, 0, r, s->sC)) return -1;
   // launch-count bookkeeping only (never waits): the newest count that has already arrived tells which body ran last
   for (int back = 1; back <= 3 && k - back >= 0; ++back) {
     const int rr = (int)((k - back) % kRing);
-    if (cudaEventQuery(s->ev_count[rr]) == cudaSuccess) { s->last_bucket = s->h_count[rr][0] > 0 ? s->h_count[rr][1] / 128 : 0; break; }
+    if (cudaEventQuery(s->ev[rr].count) == cudaSuccess) { s->last_bucket = s->h_count[rr][0] > 0 ? s->h_count[rr][1] / 128 : 0; break; }
   }
   if (s->last_bucket < 0 || s->last_bucket >= s->s1_buckets) s->last_bucket = s->s1_buckets - 1;
   RYK_CUDA(cudaGraphLaunch(s->s1_switch[b], s->sC));
   e->launches += s->s1_switch_launches[b][s->last_bucket];
   // NB: enc_*[b] may be overwritten by encode k+2 once this stage's slides ran; the stage-1 graph is short, so the
   // guard event is simply the end of the stage.
-  TSTAMP(2, 1, s->sC);
-  RYK_CUDA(cudaEventRecord(s->ev_cslide[r], s->sC));
-  RYK_CUDA(cudaEventRecord(s->ev_s1[r], s->sC));
+  if (stage_time(s, 2, 1, r, s->sC)) return -1;
+  RYK_CUDA(cudaEventRecord(s->ev[r].cslide, s->sC));
+  RYK_CUDA(cudaEventRecord(s->ev[r].s1, s->sC));
 
   // ================= stream C2: stage-2 prologue =================
-  RYK_CUDA(cudaStreamWaitEvent(sC2, s->ev_s1[r], 0));
-  if (k >= 2) RYK_CUDA(cudaStreamWaitEvent(sC2, s->ev_dslide[(k - 2) % kRing], 0));  // cv_sp_out[b] consumed by decode k-2
-  const int Tp = s->Tw + (128 - s->Tw % 128);
-  TSTAMP(3, 0, sC2);
+  RYK_CUDA(cudaStreamWaitEvent(sC2, s->ev[r].s1, 0));
+  if (k >= 2) RYK_CUDA(cudaStreamWaitEvent(sC2, s->ev[(k - 2) % kRing].dslide, 0));  // cv_sp_out[b] consumed by decode k-2
+  if (stage_time(s, 3, 0, r, sC2)) return -1;
   if (s->group) {
     Group* G = s->group;
     if (G->step >= 1) RYK_CUDA(cudaStreamWaitEvent(sC2, G->ev_fwd[(G->step - 1) % kRing], 0));   // batched input read by forward k-1
-    float* dst = (float*)G->p2->d_in + (size_t)s->slot * Tp * 512;
-    if (run_graph(e, s->graphs[G_S2A + b], sC2, [&]() -> int { return sr_prologue_run(e, s->cv_sp_mid[b], s->Tw, Tp, s->nb, dst, sC2, d_colmin); })) return -1;
-    RYK_CUDA(cudaEventRecord(s->ev_pro[r], sC2));
+    float* dst = (float*)G->p2->d_in + (size_t)s->slot * s->Tp * 512;
+    if (run_graph(e, pg.s2_pro, sC2, [&]() -> int { return sr_prologue_run(e, s->cv_sp_mid[b], s->Tw, s->Tp, s->nb, dst, sC2, d_colmin); })) return -1;
+    RYK_CUDA(cudaEventRecord(s->ev[r].pro, sC2));
   } else {
     UNetPlan* p2 = nullptr;
-    if (unet_get_plan(e, e->stage2, 1, Tp, 512, e->precision, &p2, s2_owner)) return -1;
-    if (run_graph(e, s->graphs[G_S2A + b], sC2, [&]() -> int {
-          if (sr_prologue_run(e, s->cv_sp_mid[b], s->Tw, Tp, s->nb, (float*)p2->d_in, sC2, d_colmin)) return -1;
+    if (s2_plan(e, s, b, &p2)) return -1;
+    if (run_graph(e, pg.s2_pro, sC2, [&]() -> int {
+          if (sr_prologue_run(e, s->cv_sp_mid[b], s->Tw, s->Tp, s->nb, (float*)p2->d_in, sC2, d_colmin)) return -1;
           return unet_forward(e, p2, sC2, 0, 0);
         })) return -1;
   }
@@ -502,44 +536,46 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
 
 // single session: stage-2 layers 1..14 (the wgmma layers) on the session's own stream
 static int session_mid_single(Engine* e, Session* s, bool was_profiling) {
-  STEP_LOCALS
-  S2_LOCALS
-  const int Tp = s->Tw + (128 - s->Tw % 128);
+  const int b = (int)(s->step & 1);
+  cudaStream_t sC2 = s2_stream(s, b);
   UNetPlan* p2 = nullptr;
-  if (unet_get_plan(e, e->stage2, 1, Tp, 512, e->precision, &p2, s2_owner)) return -1;
+  if (s2_plan(e, s, b, &p2)) return -1;
   cudaEvent_t pe0 = nullptr, pe1 = nullptr;
   if (was_profiling) { RYK_CUDA(cudaEventCreate(&pe0)); RYK_CUDA(cudaEventCreate(&pe1)); RYK_CUDA(cudaEventRecord(pe0, sC2)); }
-  if (run_graph(e, s->graphs[G_S2B + b], sC2, [&]() -> int { return unet_forward(e, p2, sC2, 1, 14); })) return -1;
+  if (run_graph(e, s->graphs[b].s2_layers, sC2, [&]() -> int { return unet_forward(e, p2, sC2, 1, 14); })) return -1;
   if (was_profiling) { RYK_CUDA(cudaEventRecord(pe1, sC2)); e->prof_events.emplace_back(pe0, pe1); }
   return 0;
 }
 
 static int session_back(Engine* e, Session* s) {
-  STEP_LOCALS
-  S2_LOCALS
-  const int Tp = s->Tw + (128 - s->Tw % 128);
+  const long long k = s->step;
+  const int b = (int)(k & 1), f = b, g = b ^ 1, r = (int)(k % kRing);
+  const ryk_session_config& c = s->cfg;
+  const int pc = s->e_conv;
+  cudaStream_t sC2 = s2_stream(s, b);
+  ParityGraphs& pg = s->graphs[b];
   if (s->group) {
     Group* G = s->group;
     RYK_CUDA(cudaStreamWaitEvent(sC2, G->ev_fwd[G->step % kRing], 0));
-    const float* src = (const float*)G->p2->d_out + (size_t)s->slot * Tp * 512;
-    if (run_graph(e, s->graphs[G_S2C + b], sC2, [&]() -> int { return sr_epilogue_run(e, src, s->Tw, s->nb, s->cv_sp_out[b], sC2); })) return -1;
+    const float* src = (const float*)G->p2->d_out + (size_t)s->slot * s->Tp * 512;
+    if (run_graph(e, pg.s2_epi, sC2, [&]() -> int { return sr_epilogue_run(e, src, s->Tw, s->nb, s->cv_sp_out[b], sC2); })) return -1;
   } else {
     UNetPlan* p2 = nullptr;
-    if (unet_get_plan(e, e->stage2, 1, Tp, 512, e->precision, &p2, s2_owner)) return -1;
-    if (run_graph(e, s->graphs[G_S2C + b], sC2, [&]() -> int {
+    if (s2_plan(e, s, b, &p2)) return -1;
+    if (run_graph(e, pg.s2_epi, sC2, [&]() -> int {
           if (unet_forward(e, p2, sC2, 15, 15)) return -1;
           return sr_epilogue_run(e, (const float*)p2->d_out, s->Tw, s->nb, s->cv_sp_out[b], sC2);
         })) return -1;
   }
-  TSTAMP(3, 1, sC2);
-  RYK_CUDA(cudaEventRecord(s->ev_conv[r], sC2));
+  if (stage_time(s, 3, 1, r, sC2)) return -1;
+  RYK_CUDA(cudaEventRecord(s->ev[r].conv, sC2));
 
   // ================= stream D: realtime synthesizer =================
-  RYK_CUDA(cudaStreamWaitEvent(s->sD, s->ev_conv[r], 0));
-  TSTAMP(4, 0, s->sD);
+  RYK_CUDA(cudaStreamWaitEvent(s->sD, s->ev[r].conv, 0));
+  if (stage_time(s, 4, 0, r, s->sD)) return -1;
   if (synth_host_advance(e, s->synth, s->Td, s->sD)) return -1;
   const int max_blocks = s->max_blocks;
-  if (run_graph(e, s->graphs[G_D1 + b], s->sD, [&]() -> int {
+  if (run_graph(e, pg.dec_slide, s->sD, [&]() -> int {
         SlideBatch sb; sb.n = 0;
         slide_add<float>(sb, s->dw_f0[f], s->cv_f0_out[b] + pc, s->dw_f0[g], s->Td, s->n_feat, 1);
         slide_add<float>(sb, s->dw_ap[f], s->cv_ap_out[b] + (size_t)pc * s->nb, s->dw_ap[g], s->Td, s->n_feat, s->nb);
@@ -551,8 +587,8 @@ static int session_back(Engine* e, Session* s) {
         return 0;
       })) return -1;
   // the converted features of this parity are free again as soon as they sit in the decode window
-  RYK_CUDA(cudaEventRecord(s->ev_dslide[r], s->sD));
-  if (run_graph(e, s->graphs[G_D + b], s->sD, [&]() -> int {
+  RYK_CUDA(cudaEventRecord(s->ev[r].dslide, s->sD));
+  if (run_graph(e, pg.synth, s->sD, [&]() -> int {
         if (synth_add_kernel(e, s->synth, s->dec_f0_f64, s->Td, s->dw_sp[g], s->dw_ap[g], s->sD)) return -1;
         if (synth_drain_async(e, s->synth, s->d_out_fixed[b], max_blocks, s->sD)) return -1;
         k_scrub<<<8, 256, 0, s->sD>>>(s->d_out_fixed[b], s->synth->dev.state, c.vocoder_buffer_size, max_blocks * c.vocoder_buffer_size, s->d_n_fixed[b]);
@@ -560,8 +596,8 @@ static int session_back(Engine* e, Session* s) {
         RYK_CUDA(cudaGetLastError());
         return 0;
       })) return -1;
-  TSTAMP(4, 1, s->sD);
-  // ev_dec[r] is recorded by the caller after the copies it appends to stream D
+  if (stage_time(s, 4, 1, r, s->sD)) return -1;
+  // ev[r].dec is recorded by stage_out after the copies it appends to stream D
   s->step++;
   return 0;
 }
@@ -582,8 +618,8 @@ static int group_enqueue_impl(Engine* e, Group* G, const float* const* d_chunks,
   for (size_t i = 0; i < G->members.size(); ++i)
     if (session_front(e, G->members[i], d_chunks[i])) return -1;
   for (Session* m : G->members) {
-    RYK_CUDA(cudaStreamWaitEvent(G->sG, m->ev_pro[m->step % kRing], 0));
-    if (m->step >= 1) RYK_CUDA(cudaStreamWaitEvent(G->sG, m->ev_conv[(m->step - 1) % kRing], 0));   // batched output read by epilogue k-1
+    RYK_CUDA(cudaStreamWaitEvent(G->sG, m->ev[m->step % kRing].pro, 0));
+    if (m->step >= 1) RYK_CUDA(cudaStreamWaitEvent(G->sG, m->ev[(m->step - 1) % kRing].conv, 0));   // batched output read by epilogue k-1
   }
   cudaEvent_t pe0 = nullptr, pe1 = nullptr;
   if (was_profiling) { RYK_CUDA(cudaEventCreate(&pe0)); RYK_CUDA(cudaEventCreate(&pe1)); RYK_CUDA(cudaEventRecord(pe0, G->sG)); }
@@ -603,6 +639,37 @@ static int group_enqueue(Engine* e, Group* G, const float* const* d_chunks) {
   return rc;
 }
 
+// ---- host-API staging shared by sessions and groups (ring slot r = step % kRing) ----
+// host chunk -> pinned slot -> s->d_chunk[r] on stream E
+static int stage_in(Session* s, int r, const float* wave) {
+  memcpy(s->h_in[r], wave, sizeof(float) * s->n_wave);
+  RYK_CUDA(cudaMemcpyAsync(s->d_chunk[r], s->h_in[r], sizeof(float) * s->n_wave, cudaMemcpyHostToDevice, s->sE));
+  return 0;
+}
+
+// after step k was enqueued: copy its blocks and sample count to out / n_out (kind: to the host ring or to device buffers) behind
+// the decode stream and record ev[r].dec
+static int stage_out(Session* s, long long k, double* out, int* n_out, cudaMemcpyKind kind) {
+  const int b = (int)(k & 1), r = (int)(k % kRing);
+  const size_t cap = (size_t)s->max_blocks * s->cfg.vocoder_buffer_size;
+  RYK_CUDA(cudaMemcpyAsync(n_out, s->d_n_fixed[b], sizeof(int), kind, s->sD));
+  RYK_CUDA(cudaMemcpyAsync(out, s->d_out_fixed[b], sizeof(double) * cap, kind, s->sD));
+  RYK_CUDA(cudaEventRecord(s->ev[r].dec, s->sD));
+  return 0;
+}
+
+// wait for step `ticket` of s and copy its samples out of the host ring
+static int collect_out(Session* s, long long ticket, double* out, int out_capacity, int* n_out) {
+  const int r = (int)(ticket % kRing);
+  RYK_CUDA(cudaEventSynchronize(s->ev[r].dec));
+  const int produced = *s->h_n[r];
+  RYK_CHECK(produced <= out_capacity, "output buffer too small for the produced blocks");
+  memcpy(out, s->h_out[r], sizeof(double) * produced);
+  *n_out = produced;
+  s->collected++;
+  return 0;
+}
+
 }  // namespace ryk
 
 using namespace ryk;
@@ -616,8 +683,6 @@ int ryk_session_create(ryk_engine* h, const ryk_session_config* cfg, int* sessio
   RYK_CHECK(cfg && session_id, "null argument");
   RYK_CHECK(e->stage1 && e->stage2, "load both models before creating a session");
   Session* s = new Session();
-  memset(s->ev_count, 0, sizeof(s->ev_count)); memset(s->ev_enc, 0, sizeof(s->ev_enc)); memset(s->ev_cslide, 0, sizeof(s->ev_cslide));
-  memset(s->ev_s1, 0, sizeof(s->ev_s1)); memset(s->ev_gate, 0, sizeof(s->ev_gate)); memset(s->ev_pro, 0, sizeof(s->ev_pro)); memset(s->ev_conv, 0, sizeof(s->ev_conv)); memset(s->ev_dslide, 0, sizeof(s->ev_dslide)); memset(s->ev_dec, 0, sizeof(s->ev_dec));
   s->cfg = *cfg;
   s->hop = (int)(cfg->fs * cfg->frame_period_ms / 1000.0);
   s->rate = (int)lround(1000.0 / cfg->frame_period_ms);
@@ -630,6 +695,7 @@ int ryk_session_create(ryk_engine* h, const ryk_session_config* cfg, int* sessio
   s->Lw = s->n_wave + 2 * s->e_wave;
   s->Tw = s->n_feat + 2 * s->e_conv;
   s->Td = s->n_feat + 2 * s->e_dec;
+  s->Tp = s->Tw + (128 - s->Tw % 128);
   s->nb = cfg->fft_length / 2 + 1;
   s->C = cfg->order + 1;
   RYK_CHECK(s->n_wave == s->n_feat * s->hop && s->e_wave == s->e_enc_frames * s->hop, "buffer_time / encode_extra_time must be whole frames");
@@ -646,10 +712,8 @@ int ryk_session_create(ryk_engine* h, const ryk_session_config* cfg, int* sessio
   RYK_CUDA(cudaStreamCreateWithPriority(&s->sC, cudaStreamNonBlocking, prio_hi));
   for (int i = 0; i < 2; ++i) RYK_CUDA(cudaStreamCreateWithPriority(&s->sC2s[i], cudaStreamNonBlocking, prio_lo));
   RYK_CUDA(cudaStreamCreateWithPriority(&s->sD, cudaStreamNonBlocking, prio_hi));
-  for (int i = 0; i < kRing; ++i) {
-    cudaEvent_t* evs[] = {&s->ev_gate[i], &s->ev_pro[i], &s->ev_count[i], &s->ev_enc[i], &s->ev_cslide[i], &s->ev_s1[i], &s->ev_conv[i], &s->ev_dslide[i], &s->ev_dec[i]};
-    for (cudaEvent_t* ev : evs) RYK_CUDA(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
-  }
+  for (StepEvents& ev : s->ev)
+    for (cudaEvent_t* p : ev.all()) RYK_CUDA(cudaEventCreateWithFlags(p, cudaEventDisableTiming));
   { const char* v = getenv("RYK_STAGE_TIMES"); s->stage_times = v && atoi(v) != 0; }
   if (s->stage_times) for (int a = 0; a < 5; ++a) for (int w = 0; w < 2; ++w) for (int i = 0; i < kRing; ++i) RYK_CUDA(cudaEventCreate(&s->tev[a][w][i]));
   // zero-fill on the ENGINE stream: the template fill below (k_fill_rows on e->stream, a non-blocking stream) must be ordered after
@@ -703,16 +767,15 @@ int ryk_session_create(ryk_engine* h, const ryk_session_config* cfg, int* sessio
     if (P((void**)&s->h_n[i], sizeof(int))) return -1;
     if (P((void**)&s->h_count[i], sizeof(int) * 2)) return -1;
   }
-  for (int i = 0; i < 2; ++i) {
+  for (int i = 0; i < 2; ++i)
     if (dio_plan_create(e, s->Lw, cfg->fs, cfg->frame_period_ms, cfg->f0_floor, cfg->f0_ceil, &s->dio[i], e->f0_method)) return -1;
-    e->dio_plans[std::make_tuple(-(int)e->sessions.size() - 1, cfg->fs, i, 0, 0)] = s->dio[i];   // owned by the engine's plan table
-  }
   if (synth_create(e, cfg->fs, cfg->frame_period_ms, cheaptrick_fft_size(cfg->fs, 71.0), cfg->vocoder_buffer_size, 4096, &s->synth)) return -1;
   // build the U-Net plans this session can need up front (allocation + tensor maps), not on the first chunk
   UNetPlan* p = nullptr;
-  s->owner = (int)e->sessions.size() + 1;
-  for (int Tp = 128; Tp <= s->Tw + 128; Tp += 128) if (unet_get_plan(e, e->stage1, 1, 1, Tp, e->precision, &p, s->owner)) return -1;
-  // (the stage-2 plan is created on first use: a session that joins a group never needs its own)
+  s->s1_owner = ++e->plan_owners;
+  for (int b = 0; b < 2; ++b) s->s2_owner[b] = ++e->plan_owners;
+  for (int Tp = 128; Tp <= s->Tp; Tp += 128) if (unet_get_plan(e, e->stage1, 1, 1, Tp, e->precision, &p, s->s1_owner)) return -1;
+  // (the stage-2 plans are created on first use: a session that joins a group never needs its own)
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   RYK_CUDA(cudaDeviceSynchronize());
   for (int b = 0; b < 2; ++b) if (stage1_build_switch(e, s, b)) return -1;
@@ -727,11 +790,10 @@ int ryk_session_destroy(ryk_engine* h, int id) {
   RYK_CHECK(s != nullptr, "no such session");
   RYK_CHECK(s->group == nullptr, "session belongs to a group: destroy the group first");
   RYK_CUDA(cudaStreamSynchronize(e->stream));
-  const int owner = s->owner;
+  const int s1_owner = s->s1_owner, s2_owner[2] = {s->s2_owner[0], s->s2_owner[1]};
   session_free(s);                         // synchronises the session's streams
-  unet_release_owner(e->stage1, owner);
-  unet_release_owner(e->stage2, owner);
-  unet_release_owner(e->stage2, owner + 3000000);
+  unet_release_owner(e->stage1, s1_owner);
+  for (int owner : s2_owner) unet_release_owner(e->stage2, owner);
   e->sessions[id] = nullptr;
   return 0;
 }
@@ -747,14 +809,9 @@ int ryk_session_submit(ryk_engine* h, int id, const float* wave, int n, long lon
   RYK_CHECK(s->step - s->collected < kRing - 2, "too many chunks in flight: collect before submitting more");
   const long long k = s->step;
   const int r = (int)(k % kRing);
-  memcpy(s->h_in[r], wave, sizeof(float) * n);
-  RYK_CUDA(cudaMemcpyAsync(s->d_chunk[r], s->h_in[r], sizeof(float) * n, cudaMemcpyHostToDevice, s->sE));
-  const int cap = s->max_blocks * s->cfg.vocoder_buffer_size;
-  const int b = (int)(k & 1);
+  if (stage_in(s, r, wave)) return -1;
   if (session_enqueue(e, s, s->d_chunk[r])) return -1;
-  RYK_CUDA(cudaMemcpyAsync(s->h_n[r], s->d_n_fixed[b], sizeof(int), cudaMemcpyDeviceToHost, s->sD));
-  RYK_CUDA(cudaMemcpyAsync(s->h_out[r], s->d_out_fixed[b], sizeof(double) * (size_t)cap, cudaMemcpyDeviceToHost, s->sD));
-  RYK_CUDA(cudaEventRecord(s->ev_dec[r], s->sD));
+  if (stage_out(s, k, s->h_out[r], s->h_n[r], cudaMemcpyDeviceToHost)) return -1;
   if (ticket) *ticket = k;
   return 0;
 }
@@ -765,14 +822,7 @@ int ryk_session_collect(ryk_engine* h, int id, long long ticket, double* out, in
   Session* s = get_session(e, id);
   RYK_CHECK(s != nullptr, "no such session");
   RYK_CHECK(ticket == s->collected && ticket < s->step, "tickets are collected in submission order");
-  const int r = (int)(ticket % kRing);
-  RYK_CUDA(cudaEventSynchronize(s->ev_dec[r]));
-  int produced = *s->h_n[r];
-  RYK_CHECK(produced <= out_capacity, "output buffer too small for the produced blocks");
-  memcpy(out, s->h_out[r], sizeof(double) * produced);
-  *n_out = produced;
-  s->collected++;
-  return 0;
+  return collect_out(s, ticket, out, out_capacity, n_out);
 }
 
 // Non-blocking completion query (cudaEventQuery of the step's last decode-stream event): *done = 1 when ryk_session_collect would
@@ -782,7 +832,7 @@ int ryk_session_poll(ryk_engine* h, int id, long long ticket, int* done) {
   Session* s = get_session(e, id);
   RYK_CHECK(s != nullptr && done != nullptr, "no such session");
   RYK_CHECK(ticket >= 0 && ticket < s->step && ticket + kRing > s->step, "ticket is not among the last 8 steps");
-  cudaError_t q = cudaEventQuery(s->ev_dec[ticket % kRing]);
+  cudaError_t q = cudaEventQuery(s->ev[ticket % kRing].dec);
   if (q != cudaSuccess && q != cudaErrorNotReady) RYK_CUDA(q);
   *done = q == cudaSuccess ? 1 : 0;
   return 0;
@@ -803,13 +853,10 @@ int ryk_session_push_device(ryk_engine* h, int id, const float* wave_dev, int n,
   RYK_CHECK(s != nullptr, "no such session");
   RYK_CHECK(n == s->n_wave, "chunk length must be round(fs * buffer_time)");
   RYK_CHECK(s->group == nullptr, "session belongs to a group: use ryk_group_push_device");
-  const int r = (int)(s->step % kRing), b = (int)(s->step & 1);
-  const int cap = s->max_blocks * s->cfg.vocoder_buffer_size;
-  RYK_CHECK(out_capacity >= cap, "out_capacity must hold (frames * hop / block + 4) synthesizer blocks");
+  RYK_CHECK(out_capacity >= s->max_blocks * s->cfg.vocoder_buffer_size, "out_capacity must hold (frames * hop / block + 4) synthesizer blocks");
+  const long long k = s->step;
   if (session_enqueue(e, s, wave_dev)) return -1;
-  RYK_CUDA(cudaMemcpyAsync(out_dev, s->d_out_fixed[b], sizeof(double) * (size_t)cap, cudaMemcpyDeviceToDevice, s->sD));
-  RYK_CUDA(cudaMemcpyAsync(n_out_dev, s->d_n_fixed[b], sizeof(int), cudaMemcpyDeviceToDevice, s->sD));
-  RYK_CUDA(cudaEventRecord(s->ev_dec[r], s->sD));
+  if (stage_out(s, k, out_dev, n_out_dev, cudaMemcpyDeviceToDevice)) return -1;
   s->collected = s->step;         // device-resident steps are not collected through the host API
   return 0;
 }
@@ -822,8 +869,7 @@ int ryk_group_create(ryk_engine* h, const int* session_ids, int n_sessions, int*
   RYK_CUDA(cudaSetDevice(e->device));
   RYK_CHECK(session_ids && group_id && n_sessions >= 1 && n_sessions <= 64, "a group holds 1..64 sessions");
   Group* G = new Group();
-  G->owner = 1000000 + (int)e->groups.size();
-  memset(G->ev_fwd, 0, sizeof(G->ev_fwd));
+  G->owner = ++e->plan_owners;
   for (int i = 0; i < n_sessions; ++i) {
     Session* s = get_session(e, session_ids[i]);
     if (!s || s->group || s->step != 0 || (i > 0 && s->Tw != G->members[0]->Tw)) {
@@ -834,8 +880,7 @@ int ryk_group_create(ryk_engine* h, const int* session_ids, int n_sessions, int*
     s->group = G; s->slot = i;
     G->members.push_back(s);
   }
-  G->Tp = G->members[0]->Tw + (128 - G->members[0]->Tw % 128);
-  if (unet_get_plan(e, e->stage2, n_sessions, G->Tp, 512, e->precision, &G->p2, G->owner)) { group_free(G); return -1; }
+  if (unet_get_plan(e, e->stage2, n_sessions, G->members[0]->Tp, 512, e->precision, &G->p2, G->owner)) { group_free(G); return -1; }
   { int lo = 0, hi = 0; RYK_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi)); RYK_CUDA(cudaStreamCreateWithPriority(&G->sG, cudaStreamNonBlocking, lo)); }
   for (int i = 0; i < kRing; ++i) RYK_CUDA(cudaEventCreateWithFlags(&G->ev_fwd[i], cudaEventDisableTiming));
   RYK_CUDA(cudaDeviceSynchronize());
@@ -869,22 +914,17 @@ int ryk_group_submit(ryk_engine* h, int group_id, const float* const* waves, int
   RYK_CHECK(G != nullptr, "no such group");
   RYK_CHECK(G->step - G->collected < kRing - 2, "too many chunks in flight: collect before submitting more");
   const long long k = G->step;
-  const int r = (int)(k % kRing), b = (int)(k & 1);
+  const int r = (int)(k % kRing);
   std::vector<const float*> d_chunks(G->members.size());
   for (size_t i = 0; i < G->members.size(); ++i) {
     Session* s = G->members[i];
     RYK_CHECK(n == s->n_wave, "chunk length must be round(fs * buffer_time)");
-    memcpy(s->h_in[r], waves[i], sizeof(float) * n);
-    RYK_CUDA(cudaMemcpyAsync(s->d_chunk[r], s->h_in[r], sizeof(float) * n, cudaMemcpyHostToDevice, s->sE));
+    if (stage_in(s, r, waves[i])) return -1;
     d_chunks[i] = s->d_chunk[r];
   }
   if (group_enqueue(e, G, d_chunks.data())) return -1;
-  for (Session* s : G->members) {
-    const int cap = s->max_blocks * s->cfg.vocoder_buffer_size;
-    RYK_CUDA(cudaMemcpyAsync(s->h_n[r], s->d_n_fixed[b], sizeof(int), cudaMemcpyDeviceToHost, s->sD));
-    RYK_CUDA(cudaMemcpyAsync(s->h_out[r], s->d_out_fixed[b], sizeof(double) * (size_t)cap, cudaMemcpyDeviceToHost, s->sD));
-    RYK_CUDA(cudaEventRecord(s->ev_dec[r], s->sD));
-  }
+  for (Session* s : G->members)
+    if (stage_out(s, k, s->h_out[r], s->h_n[r], cudaMemcpyDeviceToHost)) return -1;
   if (ticket) *ticket = k;
   return 0;
 }
@@ -895,16 +935,8 @@ int ryk_group_collect(ryk_engine* h, int group_id, long long ticket, double* con
   Group* G = get_group(e, group_id);
   RYK_CHECK(G != nullptr, "no such group");
   RYK_CHECK(ticket == G->collected && ticket < G->step, "tickets are collected in submission order");
-  const int r = (int)(ticket % kRing);
-  for (size_t i = 0; i < G->members.size(); ++i) {
-    Session* s = G->members[i];
-    RYK_CUDA(cudaEventSynchronize(s->ev_dec[r]));
-    const int produced = *s->h_n[r];
-    RYK_CHECK(produced <= out_capacity, "output buffer too small for the produced blocks");
-    memcpy(outs[i], s->h_out[r], sizeof(double) * produced);
-    n_outs[i] = produced;
-    s->collected++;
-  }
+  for (size_t i = 0; i < G->members.size(); ++i)
+    if (collect_out(G->members[i], ticket, outs[i], out_capacity, &n_outs[i])) return -1;
   G->collected++;
   return 0;
 }
@@ -916,18 +948,15 @@ int ryk_group_push_device(ryk_engine* h, int group_id, const float* const* waves
   RYK_CUDA(cudaSetDevice(e->device));
   Group* G = get_group(e, group_id);
   RYK_CHECK(G != nullptr, "no such group");
-  const int r = (int)(G->step % kRing), b = (int)(G->step & 1);
   for (Session* s : G->members) {
     RYK_CHECK(n == s->n_wave, "chunk length must be round(fs * buffer_time)");
     RYK_CHECK(out_capacity >= s->max_blocks * s->cfg.vocoder_buffer_size, "out_capacity must hold (frames * hop / block + 4) synthesizer blocks");
   }
+  const long long k = G->step;
   if (group_enqueue(e, G, waves_dev)) return -1;
   for (size_t i = 0; i < G->members.size(); ++i) {
     Session* s = G->members[i];
-    const int cap = s->max_blocks * s->cfg.vocoder_buffer_size;
-    RYK_CUDA(cudaMemcpyAsync(outs_dev[i], s->d_out_fixed[b], sizeof(double) * (size_t)cap, cudaMemcpyDeviceToDevice, s->sD));
-    RYK_CUDA(cudaMemcpyAsync(n_outs_dev[i], s->d_n_fixed[b], sizeof(int), cudaMemcpyDeviceToDevice, s->sD));
-    RYK_CUDA(cudaEventRecord(s->ev_dec[r], s->sD));
+    if (stage_out(s, k, outs_dev[i], n_outs_dev[i], cudaMemcpyDeviceToDevice)) return -1;
     s->collected = s->step;
   }
   G->collected = G->step;

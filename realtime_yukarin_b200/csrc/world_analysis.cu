@@ -730,14 +730,6 @@ int dio_stonemask_run(Engine* e, DioPlan* p, const float* d_x, cudaStream_t st) 
 }
 
 const double* dio_plan_f0(DioPlan* p) { return p->d_f0r; }
-int dio_plan_debug_copy(DioPlan* p, double* f0_raw, double* cand, double* score, int* counts, cudaStream_t st) {
-  RYK_CUDA(cudaMemcpyAsync(f0_raw, p->d_f0, sizeof(double) * p->f0_length, cudaMemcpyDeviceToHost, st));
-  RYK_CUDA(cudaMemcpyAsync(cand, p->d_cand, sizeof(double) * p->f0_length * p->nbands, cudaMemcpyDeviceToHost, st));
-  RYK_CUDA(cudaMemcpyAsync(score, p->d_score, sizeof(double) * p->f0_length * p->nbands, cudaMemcpyDeviceToHost, st));
-  RYK_CUDA(cudaMemcpyAsync(counts, p->d_counts, sizeof(int) * 4 * p->nbands, cudaMemcpyDeviceToHost, st));
-  RYK_CUDA(cudaStreamSynchronize(st));
-  return 0;
-}
 double* dio_plan_f0_mut(DioPlan* p) { return p->d_f0r; }
 int dio_plan_frames(DioPlan* p) { return p->f0_length; }
 HarvestPlan* dio_plan_harvest(DioPlan* p) { return p->harvest; }

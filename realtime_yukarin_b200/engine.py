@@ -52,11 +52,11 @@ EXPORTED_SYMBOLS = [
     'ryk_stage2_convert', 'ryk_convert_window', 'ryk_synth_create', 'ryk_synth_destroy', 'ryk_synth_add_parameters',
     'ryk_synth_synthesis2', 'ryk_synth_decode', 'ryk_session_create', 'ryk_session_destroy', 'ryk_session_push',
     'ryk_session_push_device', 'ryk_session_submit', 'ryk_session_collect', 'ryk_group_create', 'ryk_group_destroy',
-    'ryk_group_size', 'ryk_session_stage_times', 'ryk_group_submit', 'ryk_group_collect', 'ryk_group_push_device', 'ryk_test_conv_layer', 'ryk_debug_dio', 'ryk_debug_synth_pulses', 'ryk_debug_synth_timebase', 'ryk_engine_profile', 'ryk_engine_profile_read', 'ryk_engine_timer_start', 'ryk_engine_timer_stop',
+    'ryk_group_size', 'ryk_session_stage_times', 'ryk_group_submit', 'ryk_group_collect', 'ryk_group_push_device', 'ryk_test_conv_layer', 'ryk_engine_profile', 'ryk_engine_timer_start', 'ryk_engine_timer_stop',
     'ryk_world_synthesize_length', 'ryk_world_synthesize', 'ryk_output_gate', 'ryk_reblock_create', 'ryk_reblock_destroy',
     'ryk_reblock_push', 'ryk_reblock_push_device', 'ryk_reblock_collect', 'ryk_reblock_result_device', 'ryk_resample_length',
     'ryk_resample_poly', 'ryk_session_poll', 'ryk_reblock_poll', 'ryk_engine_profile_read2', 'ryk_engine_set_stage1_fused',
-    'ryk_engine_set_f0_method', 'ryk_engine_get_f0_method', 'ryk_debug_harvest', 'ryk_debug_stage1_bench',
+    'ryk_engine_set_f0_method', 'ryk_engine_get_f0_method', 'ryk_debug_harvest',
     'ryk_crepe_create', 'ryk_crepe_set_conv', 'ryk_crepe_set_dense', 'ryk_crepe_set_decoder_tables', 'ryk_crepe_num_frames', 'ryk_crepe_predict',
 ]
 
@@ -149,11 +149,6 @@ class Engine(object):
 
     def profile(self, enable: bool):
         self._check(self.lib.ryk_engine_profile(self._h, int(bool(enable))))
-
-    def profile_read(self):
-        ms, runs = ctypes.c_double(), ctypes.c_int()
-        self._check(self.lib.ryk_engine_profile_read(self._h, ctypes.byref(ms), ctypes.byref(runs)))
-        return ms.value, runs.value
 
     def profile_read2(self):
         """(sum of per-forward durations ms, union of the intervals ms, forwards) of the stage-2 k4 block since the last read."""
@@ -378,24 +373,6 @@ class Engine(object):
         self._check(self.lib.ryk_resample_poly(self._h, _fp(x), len(x), int(up), int(down), _dp(taps), len(taps), _fp(y), len(y), ctypes.byref(no)))
         return y[:no.value]
 
-    # ---- diagnostics ----
-    def debug_synth_pulses(self, sid, first=0, count=None):
-        st = numpy.zeros(7, numpy.int64)
-        z = numpy.zeros(1, numpy.int64); zd = numpy.zeros(1); zi = numpy.zeros(1, numpy.int32)
-        self._check(self.lib.ryk_debug_synth_pulses(self._h, sid, ctypes.c_longlong(0), 0, z.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong)),
-                                                    _dp(zd), zi.ctypes.data_as(c_int_p), st.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong))))
-        if count is None:
-            count = int(st[0]) - first
-        idx = numpy.zeros(max(count, 1), numpy.int64); tm = numpy.zeros(max(count, 1)); vuv = numpy.zeros(max(count, 1), numpy.int32)
-        self._check(self.lib.ryk_debug_synth_pulses(self._h, sid, ctypes.c_longlong(first), count, idx.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong)),
-                                                    _dp(tm), vuv.ctypes.data_as(c_int_p), st.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong))))
-        return idx[:count], tm[:count], vuv[:count], st
-
-    def debug_synth_timebase(self, sid, n):
-        a, b, c = numpy.zeros(n), numpy.zeros(n), numpy.zeros(n)
-        self._check(self.lib.ryk_debug_synth_timebase(self._h, sid, int(n), _dp(a), _dp(b), _dp(c)))
-        return a, b, c
-
     F0_METHODS = {'dio': 0, 'harvest': 1}
 
     def set_f0_method(self, method: str):
@@ -424,21 +401,6 @@ class Engine(object):
         assert (info[0], info[1], info[2], info[4]) == (channels, nf1, ylen, maxc), info
         out['nc'] = int(info[6])
         return out
-
-    def stage1_bench(self, Tp: int, iters: int = 50):
-        """(ms per stand-alone stage-1 forward fused, layered, fused-kernel phase timeline in us)."""
-        a, b = ctypes.c_float(), ctypes.c_float()
-        tl = numpy.zeros(31)
-        self._check(self.lib.ryk_debug_stage1_bench(self._h, int(Tp), int(iters), ctypes.byref(a), ctypes.byref(b), _dp(tl)))
-        return float(a.value), float(b.value), tl
-
-    def debug_dio(self, n, fs, frame_period, f0_floor, f0_ceil):
-        nf = dio_num_frames(fs, n, frame_period)
-        nbands = 1 + int(numpy.log(f0_ceil / f0_floor) / 0.69314718055994529 * 2.0)
-        f0 = numpy.empty(nf); cand = numpy.empty((nbands, nf)); score = numpy.empty((nbands, nf)); counts = numpy.empty((nbands, 4), numpy.int32)
-        self._check(self.lib.ryk_debug_dio(self._h, int(n), int(fs), ctypes.c_double(frame_period), ctypes.c_double(f0_floor),
-                                           ctypes.c_double(f0_ceil), _dp(f0), _dp(cand), _dp(score), counts.ctypes.data_as(c_int_p)))
-        return f0, cand, score, counts
 
     def test_conv_layer(self, in0, in1, W, scale, shift, transposed, k, stride, pad, act, use_tc, repeat=0):
         """One conv layer in isolation; in0/in1 NHWC float32, W in the Chainer layout. Returns (out NHWC, ms per run)."""
@@ -529,10 +491,6 @@ class Engine(object):
         n_outs = (ctypes.c_int * len(outs))()
         self._check(self.lib.ryk_group_collect(self._h, gid, ctypes.c_longlong(ticket), ptrs, min(len(o) for o in outs), n_outs))
         return [o[:n] for o, n in zip(outs, n_outs)]
-
-    def group_push(self, gid: int, waves: Sequence) -> List[numpy.ndarray]:
-        outs = [numpy.empty(len(waves[0]) * 2 + 8192, dtype=numpy.float64) for _ in waves]
-        return self.group_collect(gid, self.group_submit(gid, waves), outs)
 
     def group_push_device(self, gid: int, wave_dev_ptrs: Sequence[int], n: int, out_dev_ptrs: Sequence[int], out_capacity: int,
                           n_out_dev_ptrs: Sequence[int]):

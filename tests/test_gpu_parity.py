@@ -280,6 +280,30 @@ def test_pipelined_submit_collect_equals_sequential(engine, small_models):
     engine.set_precision('fp16')
 
 
+def test_session_create_destroy_frees_device_memory(engine, small_models):
+    """A destroyed session returns everything it allocated (buffers, analysis plans, U-Net plans, graphs): creating and
+    destroying sessions on one engine, with a chunk pushed through each, must not grow the device memory in use."""
+    import torch
+    from realtime_yukarin_b200.engine import SessionConfig
+    _load(engine, small_models)
+    T = 0.3
+    cfg = SessionConfig(fs=24000, frame_period_ms=5.0, f0_floor=71.0, f0_ceil=800.0, fft_length=1024, order=8, alpha=0.466,
+                        buffer_time=T, encode_extra_time=0.0, convert_extra_time=0.5, decode_extra_time=0.0,
+                        threshold_db=60.0, vocoder_buffer_size=1024)
+    chunk = _speech(1.0, 5)[:round(T * 24000)]
+    free = {}
+    for cycle in range(1, 51):
+        sid = engine.session_create(cfg)
+        engine.session_push(sid, chunk)
+        engine.session_destroy(sid)
+        if cycle in (5, 50):
+            engine.synchronize()
+            free[cycle] = torch.cuda.mem_get_info()[0]
+    grown = (free[5] - free[50]) / 2**20
+    print(f'device memory in use grew by {grown:.1f} MiB over 45 session create / push / destroy cycles')
+    assert abs(grown) < 4.0
+
+
 def test_group_batched_stage2_matches_oracle_streams(engine, small_models):
     """BASELINE config 5 shape: several streams on one GPU share ONE batched stage-2 forward per step (ryk_group_*).
     Each member must still reproduce the oracle's chunked stream for ITS audio (fp32), with chunks kept in flight,
