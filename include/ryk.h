@@ -75,7 +75,11 @@ int ryk_world_f0(ryk_engine* e, const float* wave_host, int n, int fs, double fr
 int ryk_world_num_frames(int n, int fs, double frame_period_ms);
 /* f0 extractor behind ryk_world_f0 / ryk_world_analyze and sessions created afterwards -- the f0 hook of yukarin's
  * AcousticFeature.extract (acoustic_feature_wrapper.py:28-33; f0_estimating_method, SURVEY A.2 / A.7):
- *   0 = pyworld.dio + pyworld.stonemask (default), 1 = pyworld.harvest + pyworld.stonemask. */
+ *   0 = pyworld.dio + pyworld.stonemask (default), 1 = pyworld.harvest + pyworld.stonemask,
+ *   2 = CREPE (crepe.predict + predict_voicing, no StoneMask) for sessions created afterwards.  Method 2 needs a complete CREPE model,
+ *       its decoder tables and the resampler taps for the session's fs (see below); each step's encode window is analysed on its own.
+ *       ryk_world_f0, and ryk_world_analyze without f0_override, fail in method 2: for a single signal use ryk_crepe_predict and pass
+ *       its f0 as f0_override (CrepeAcousticFeatureWrapper does). */
 int ryk_engine_set_f0_method(ryk_engine* e, int method);
 int ryk_engine_get_f0_method(ryk_engine* e);
 
@@ -92,6 +96,10 @@ int ryk_crepe_set_conv(ryk_engine* e, int block, const float* W, const float* bi
 int ryk_crepe_set_dense(ryk_engine* e, const float* W, const float* bias);
 int ryk_crepe_set_decoder_tables(ryk_engine* e, const double* log_trans, const double* cents_mapping /* [360] */, double log_start,
                                  double log_emit_self, double log_emit_other);
+/* Polyphase filter fs -> 16 kHz for the sessions' CREPE analysis (f0 method 2): up / down = 16000 / fs reduced, taps as for
+ * ryk_resample_poly (realtime_yukarin_b200/wave_io.py: resample_filter(up, down)).  One filter per fs; a new upload replaces it.
+ * ryk_crepe_create / _set_* fail while a session in f0 method 2 exists: its captured graphs point at the model. */
+int ryk_crepe_set_resampler(ryk_engine* e, int fs, int up, int down, const double* taps, int n_taps);
 int ryk_crepe_num_frames(int n16, double step_ms);
 /* f0 / confidence / voicing (HMM state) [frames], activation [frames][360], path [frames] (pitch-bin Viterbi path); any may be NULL */
 int ryk_crepe_predict(ryk_engine* e, const float* audio16k, int n, double step_ms, double* f0, float* confidence, int* voicing,
@@ -244,6 +252,16 @@ int ryk_debug_harvest(ryk_engine* e, int n, int fs, double frame_period_ms, doub
 int ryk_test_conv_layer(ryk_engine* e, int transposed, int k, int stride, int pad, int B, int Hin, int Win, int C0, int C1, int Cout,
                         const float* in0, const float* in1, const float* W, const float* scale, const float* shift, int act,
                         int use_tc, int repeat, float* out, float* ms_per_run);
+/* CREPE convolutions with an explicit back-end: 0 = the FP32 CUDA-core kernel (ryk_crepe_predict, sessions in precision 0),
+ * 1 = the 3xTF32 tensor-core kernel (sessions in precision 1).
+ * ryk_crepe_test_conv: one layer in isolation, x [F][Win][Cin], W (Cout, Cin, k), stride 1, no padding ->
+ *   y = ReLU(conv + bias) [F][Win - k + 1][Cout]; CREPE's first layer is given in its im2col form (Win 256, Cin 512, k 1).
+ * ryk_crepe_test_network: the loaded model and decoders on a host 16 kHz signal (frames as ryk_crepe_predict): activation
+ *   [frames][360], path and voicing [frames] (any may be NULL); repeat > 0 further runs report their mean device time. */
+int ryk_crepe_test_conv(ryk_engine* e, int backend, int F, int Win, int Cin, int Cout, int k, const float* x, const float* W,
+                        const float* bias, float* y);
+int ryk_crepe_test_network(ryk_engine* e, int backend, const float* audio16k, int n, double step_ms, float* activation, int* path,
+                           int* voicing, int repeat, float* ms_per_run);
 
 #ifdef __cplusplus
 }

@@ -10,17 +10,19 @@ and applies the voicing rule.  Weights: an npz {conv<l>.W (cout, cin, k), conv<l
 (360, 64 m), dense.b}; the trained CREPE weights are not redistributable with this repository -- point RYK_CREPE_MODEL (or
 load_crepe_model) at a converted file.  No CPU fallback."""
 import ctypes
+import math
 import os
 from typing import Optional
 
 import numpy
 
 MODEL_SRATE = 16000
+SESSION_RATE = 24000          # the streaming session's rate (config.yaml input_rate); its CREPE analysis resamples from it
 CAPACITY = {'tiny': 4, 'small': 8, 'medium': 16, 'large': 24, 'full': 32}
 _FILTERS = [32, 4, 4, 4, 8, 16]
 _WIDTHS = [512, 64, 64, 64, 64, 64]
 
-_loaded = {'engine': None, 'multiplier': None}
+_loaded = {'engine': None, 'multiplier': None, 'rates': set()}
 
 
 def pitch_hmm_tables():
@@ -36,7 +38,8 @@ def pitch_hmm_tables():
 
 
 def load_crepe_model(path, engine=None) -> int:
-    """Upload an npz weight file; returns the capacity multiplier (4 tiny .. 32 full)."""
+    """Upload an npz weight file and the 24 kHz -> 16 kHz resampler taps that sessions in f0 method 'crepe' use; returns the
+    capacity multiplier (4 tiny .. 32 full)."""
     from .engine import default_engine
     engine = engine or default_engine()
     w = numpy.load(path)
@@ -63,11 +66,27 @@ def load_crepe_model(path, engine=None) -> int:
     engine._check(lib.ryk_crepe_set_decoder_tables(h, lt.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
                                                    cents.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), ctypes.c_double(ls),
                                                    ctypes.c_double(es), ctypes.c_double(eo)))
-    _loaded['engine'], _loaded['multiplier'] = engine, mult
+    _loaded['engine'], _loaded['multiplier'], _loaded['rates'] = engine, mult, set()
+    set_session_rate(SESSION_RATE, engine)
     return mult
 
 
-def _engine_with_model(engine=None):
+def set_session_rate(fs: int, engine) -> None:
+    """Upload the fs -> 16 kHz resampler taps (wave_io.resample_filter) that sessions at `fs` in f0 method 'crepe' need; once per
+    loaded model and rate."""
+    from . import wave_io
+    fs = int(fs)
+    if fs in _loaded.get('rates', ()):
+        return
+    g = math.gcd(fs, MODEL_SRATE)
+    up, down = MODEL_SRATE // g, fs // g
+    taps = numpy.ascontiguousarray(wave_io.resample_filter(up, down), dtype=numpy.float64)
+    engine._check(engine.lib.ryk_crepe_set_resampler(engine._h, fs, up, down, taps.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), len(taps)))
+    _loaded['rates'].add(fs)
+
+
+def engine_with_model(engine=None):
+    """`engine` (default: the process engine) with CREPE weights loaded, from RYK_CREPE_MODEL when none were loaded into it yet."""
     from .engine import default_engine
     engine = engine or default_engine()
     if _loaded['engine'] is not engine:
@@ -82,7 +101,7 @@ def predict(audio: numpy.ndarray, sr: int, step_size: float = 10.0, engine=None,
     """crepe.predict(audio, sr, viterbi=True, step_size=...) -> (time, frequency, confidence, activation); details=True appends
     (voicing states, pitch-bin path)."""
     from . import wave_io
-    engine = _engine_with_model(engine)
+    engine = engine_with_model(engine)
     x = numpy.asarray(audio, dtype=numpy.float32)
     if x.ndim == 2:
         x = x.mean(1)
@@ -108,3 +127,31 @@ def extract_f0(x: numpy.ndarray, fs: int, frame_period: float, engine=None):
     f0 = f0.copy()
     f0[~voiced] = 0
     return f0, t
+
+
+def run_test_conv(engine, backend: int, x, W, bias) -> numpy.ndarray:
+    """One CREPE-shaped conv layer on the device (ryk_crepe_test_conv): x [F][Win][Cin], W (Cout, Cin, k) -> ReLU(conv + bias)
+    [F][Win - k + 1][Cout]; backend 0 = FP32 CUDA cores, 1 = 3xTF32 tensor cores."""
+    x = numpy.ascontiguousarray(x, dtype=numpy.float32)
+    W = numpy.ascontiguousarray(W, dtype=numpy.float32)
+    bias = numpy.ascontiguousarray(bias, dtype=numpy.float32)
+    F, Win, Cin = x.shape
+    Cout, _, k = W.shape
+    y = numpy.empty((F, Win - k + 1, Cout), numpy.float32)
+    fp = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_float))
+    engine._check(engine.lib.ryk_crepe_test_conv(engine._h, int(backend), F, Win, Cin, Cout, k, fp(x), fp(W), fp(bias), fp(y)))
+    return y
+
+
+def run_test_network(engine, backend: int, x16, step_size: float = 5.0, repeat: int = 0):
+    """The loaded network and decoders on a 16 kHz signal with an explicit conv back-end (ryk_crepe_test_network):
+    (activation [F][360], path [F], voicing [F], mean device ms per run over `repeat` timed runs or None)."""
+    x16 = numpy.ascontiguousarray(x16, dtype=numpy.float32)
+    F = int(engine.lib.ryk_crepe_num_frames(len(x16), ctypes.c_double(step_size)))
+    act = numpy.zeros((F, 360), numpy.float32); path = numpy.zeros(F, numpy.int32); voicing = numpy.zeros(F, numpy.int32)
+    ms = ctypes.c_float()
+    engine._check(engine.lib.ryk_crepe_test_network(
+        engine._h, int(backend), x16.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), len(x16), ctypes.c_double(step_size),
+        act.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), path.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
+        voicing.ctypes.data_as(ctypes.POINTER(ctypes.c_int)), int(repeat), ctypes.byref(ms)))
+    return act, path, voicing, (ms.value if repeat > 0 else None)

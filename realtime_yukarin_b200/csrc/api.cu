@@ -177,9 +177,9 @@ int ryk_engine_destroy(ryk_engine* h) {
   cudaStreamSynchronize(e->stream);
   for (auto& kv : e->dio_plans) dio_plan_free(kv.second);
   unet_destroy(e->stage1); unet_destroy(e->stage2);
-  crepe_destroy();
   for (Synth* s : e->synths) synth_destroy(s);
   session_destroy_all(e);
+  crepe_destroy();                                  // after the sessions: their CREPE plans are counted on the model
   void* ptrs[] = {e->d_colmin, e->d_twiddle, e->d_jump, e->d_G, e->d_H, e->d_s1_in_mean, e->d_s1_in_std, e->d_s1_out_mean, e->d_s1_out_std, e->d_scratch};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (e->h_pinned) cudaFreeHost(e->h_pinned);
@@ -257,6 +257,7 @@ int ryk_world_f0(ryk_engine* h, const float* wave, int n, int fs, double fp, dou
   Engine* e = E(h);
   RYK_CUDA(cudaSetDevice(e->device));
   RYK_CHECK(n > 0, "empty wave");
+  RYK_CHECK(e->f0_method != 2, "f0 method 2 (CREPE) runs in sessions only: use the CREPE front-end (ryk_crepe_predict) for a single signal");
   DioPlan* plan = nullptr;
   if (dio_get_plan(e, n, fs, fp, f0_floor, f0_ceil, &plan)) return -1;
   void* scratch = nullptr;
@@ -278,6 +279,7 @@ int ryk_world_analyze(ryk_engine* h, const float* wave, int n, int fs, double fp
   RYK_CUDA(cudaSetDevice(e->device));
   int hop = (int)(fs * fp / 1000.0);
   RYK_CHECK(hop > 0, "bad frame period");
+  RYK_CHECK(f0_override || e->f0_method != 2, "f0 method 2 (CREPE) runs in sessions only: pass the CREPE f0 as f0_override");
   int n_out = n / hop;
   if (n_out <= 0) return 0;
   int nb = fft_length / 2 + 1;
@@ -672,16 +674,31 @@ int ryk_crepe_set_decoder_tables(ryk_engine* h, const double* log_trans, const d
   RYK_CUDA(cudaSetDevice(E(h)->device));
   return crepe_set_tables(E(h), log_trans, cents_mapping, log_start, log_emit_self, log_emit_other);
 }
+int ryk_crepe_set_resampler(ryk_engine* h, int fs, int up, int down, const double* taps, int n_taps) {
+  RYK_CUDA(cudaSetDevice(E(h)->device));
+  return crepe_set_resampler(E(h), fs, up, down, taps, n_taps);
+}
 int ryk_crepe_num_frames(int n16, double step_ms) { return crepe_num_frames(n16, step_ms); }
+int ryk_crepe_test_conv(ryk_engine* h, int backend, int F, int Win, int Cin, int Cout, int k, const float* x, const float* W, const float* bias,
+                        float* y) {
+  RYK_CUDA(cudaSetDevice(E(h)->device));
+  return crepe_test_conv(E(h), backend, F, Win, Cin, Cout, k, x, W, bias, y);
+}
+int ryk_crepe_test_network(ryk_engine* h, int backend, const float* audio16k, int n, double step_ms, float* activation, int* path, int* voicing,
+                           int repeat, float* ms_per_run) {
+  RYK_CUDA(cudaSetDevice(E(h)->device));
+  return crepe_test_network(E(h), backend, audio16k, n, step_ms, activation, path, voicing, repeat, ms_per_run);
+}
 int ryk_crepe_predict(ryk_engine* h, const float* audio16k, int n, double step_ms, double* f0, float* confidence, int* voicing, float* activation,
                       int* path) {
   RYK_CUDA(cudaSetDevice(E(h)->device));
   return crepe_predict(E(h), audio16k, n, step_ms, f0, confidence, voicing, activation, path);
 }
 
-// f0 extractor behind ryk_world_f0 / ryk_world_analyze / new sessions: 0 = DIO + StoneMask (default), 1 = Harvest + StoneMask.
+// f0 extractor behind ryk_world_f0 / ryk_world_analyze / new sessions: 0 = DIO + StoneMask (default), 1 = Harvest + StoneMask,
+// 2 = CREPE (new sessions only).
 int ryk_engine_set_f0_method(ryk_engine* h, int method) {
-  RYK_CHECK(method == 0 || method == 1, "f0 method must be 0 (DIO) or 1 (Harvest)");
+  RYK_CHECK(method == 0 || method == 1 || method == 2, "f0 method must be 0 (DIO), 1 (Harvest) or 2 (CREPE)");
   E(h)->f0_method = method;
   return 0;
 }

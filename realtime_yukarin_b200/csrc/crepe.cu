@@ -6,17 +6,27 @@
 //   frames (1024 samples, zero mean / unit std)  ->  im2col of the stride-4 k512 first layer  ->  six [conv -> ReLU -> BatchNorm ->
 //   MaxPool 2] blocks  ->  Dense 360 + sigmoid  ->  Viterbi pitch path + local weighted average of cents  ->  2-state voicing Viterbi
 //
-// The convolutions run on the FP32 CUDA-core implicit-GEMM kernel (conv_direct.cu): the reference computes CREPE in FP32 (Keras), the
-// decoding is a per-frame ARGMAX over 360 sigmoid outputs, and an FP16 tensor-core evaluation moves those maxima; this mode is outside
-// the benchmarked path (BASELINE config 2 uses WORLD f0), so reference precision is kept.  'same' padding is materialised: every block
+// The reference computes CREPE in FP32 (Keras) and decodes with a per-frame ARGMAX over 360 sigmoid outputs, which an FP16 (or plain
+// TF32) tensor-core evaluation moves.  So the convolutions run either on the FP32 CUDA-core implicit-GEMM kernel (conv_direct.cu:
+// ryk_crepe_predict, sessions in precision 0) or on the error-compensated 3xTF32 tensor-core kernel (crepe_tc.cu: sessions in
+// precision 1), which is at least as accurate.  'same' padding is materialised: every block
 // writes its pooled output into the zero-framed input buffer of the next one, so all convolutions run with padding 0.  The Viterbi
 // decoders use log-probability tables computed by the host mirror (realtime_yukarin_b200/crepe.py) -- the sums are then bit-identical
 // to the CPU restatement and so are the arg-max decisions (hmmlearn semantics: first maximum wins).
+//
+// Two callers share the network (crepe_network):
+//   ryk_crepe_predict   host 16 kHz signal in, host arrays out; uses the model's own workspace, grown on demand.
+//   CrepePlan           the session's analysis stage (f0 method 2): a caller-owned workspace sized for one window length, so the
+//                       forward (resample to 16 kHz -> network -> decoders -> voicing rule) allocates nothing, copies nothing to the
+//                       host and never synchronises, and a CUDA graph can capture it.  Its f0 (0 where unvoiced) is what
+//                       spectral_analysis_run reads in place of DIO/StoneMask.  While a plan exists the model refuses to change.
 #include <math.h>
 
 #include <vector>
 
+#include "../../include/ryk.h"
 #include "conv.h"
+#include "crepe_tc.h"
 #include "engine.h"
 
 namespace ryk {
@@ -25,6 +35,21 @@ constexpr int kCrepeBins = 360;
 static const int kCrepeFilters[6] = {32, 4, 4, 4, 8, 16};
 static const int kCrepeWidths[6] = {512, 64, 64, 64, 64, 64};
 static const int kCrepeStrides[6] = {4, 1, 1, 1, 1, 1};
+
+// Buffers of one forward over F frames of n16 samples at 16 kHz.
+struct CrepeWork {
+  int F = 0, n16 = 0;
+  float* d_audio = nullptr;
+  float* d_im2col = nullptr; float* d_conv[6] = {}; float* d_in[6] = {};   // d_in[l]: zero-framed input of block l (l >= 1)
+  float* d_flat = nullptr; float* d_logit = nullptr; float* d_act = nullptr;
+  float* d_conf = nullptr; int* d_obs = nullptr;
+  double* d_lattice = nullptr; int* d_path = nullptr; double* d_f0 = nullptr; int* d_voicing = nullptr; double* d_vlat = nullptr;
+  bool tc = false;                 // convolutions on the 3xTF32 tensor-core kernel (crepe_tc.cu) instead of conv_direct
+  float* d_tc_ws = nullptr;        // its split-K workspace (largest layer)
+};
+
+// Polyphase filter that brings an input rate to the model's 16 kHz (wave_io.resample_filter(up, down)).
+struct CrepeResampler { int fs = 0, up = 0, down = 0, n_taps = 0; double* d_taps = nullptr; };
 
 struct CrepeModel {
   int mult = 32;
@@ -41,13 +66,17 @@ struct CrepeModel {
   double h_log_start = 0, h_log_emit[2] = {0, 0};
   bool tables = false;
   bool loaded[7] = {};
-  // workspace of the last plan (grown on demand)
-  int cap_frames = 0;
-  float *d_audio = nullptr; int cap_audio = 0;
-  float* d_im2col = nullptr; float* d_conv[6] = {}; float* d_in[6] = {};   // d_in[l]: zero-framed input of block l (l >= 1)
-  float* d_flat = nullptr; float* d_logit = nullptr; float* d_act = nullptr;
-  float* d_conf = nullptr; int* d_obs = nullptr;
-  double* d_lattice = nullptr; int* d_path = nullptr; double* d_f0 = nullptr; int* d_voicing = nullptr; double* d_vlat = nullptr;
+  std::vector<CrepeResampler> resamplers;
+  CrepeWork work;            // workspace of ryk_crepe_predict (grown on demand)
+  int plans = 0;             // live CrepePlans: captured session graphs point at the weights, so the model may not change under them
+};
+
+// A caller-owned forward for a fixed input length n at rate fs: fixed buffers, so it can be captured in a CUDA graph.
+struct CrepePlan {
+  CrepeWork w;
+  int n = 0, hop16 = 0, up = 0, down = 0, n_taps = 0;
+  const double* d_taps = nullptr;
+  double* d_f0 = nullptr;    // [F] f0 after the voicing rule (0 where unvoiced)
 };
 
 static CrepeModel* g_crepe = nullptr;     // one model per process (one engine per process / GPU)
@@ -238,19 +267,42 @@ __global__ void __launch_bounds__(384) k_crepe_decode(const float* __restrict__ 
   }
 }
 
+// the reference's rule (acoustic_feature_wrapper.py:78-79): voiced = (predict_voicing == 1) | (confidence > 0.1); f0[~voiced] = 0.
+// numpy compares the float32 confidence with the Python scalar in float32.
+__global__ void k_crepe_voiced(const double* __restrict__ f0, const float* __restrict__ conf, const int* __restrict__ voicing, int F,
+                               double* __restrict__ out) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < F) out[t] = (voicing[t] == 1 || conf[t] > 0.1f) ? f0[t] : 0.0;
+}
+
 // ---- host side -----------------------------------------------------------------------------------------------------------------
+static void work_free(CrepeWork& w) {
+  for (int l = 0; l < 6; ++l) { cudaFree(w.d_conv[l]); cudaFree(w.d_in[l]); }
+  void* ptrs[] = {w.d_audio, w.d_im2col, w.d_flat, w.d_logit, w.d_act, w.d_conf, w.d_obs, w.d_lattice, w.d_path, w.d_f0, w.d_voicing, w.d_vlat,
+                  w.d_tc_ws};
+  for (void* p : ptrs) cudaFree(p);
+  w = CrepeWork();
+}
+
 static void crepe_free(CrepeModel* m) {
   if (!m) return;
-  for (int l = 0; l < 6; ++l) { cudaFree(m->d_w[l]); cudaFree(m->d_bias[l]); cudaFree(m->d_bn_a[l]); cudaFree(m->d_bn_c[l]); cudaFree(m->d_conv[l]); cudaFree(m->d_in[l]); }
-  void* ptrs[] = {m->d_ones, m->d_dense_w, m->d_dense_b, m->d_log_trans, m->d_cents, m->d_audio, m->d_im2col, m->d_flat, m->d_logit, m->d_act, m->d_conf, m->d_obs,
-                  m->d_lattice, m->d_path, m->d_f0, m->d_voicing, m->d_vlat};
+  for (int l = 0; l < 6; ++l) { cudaFree(m->d_w[l]); cudaFree(m->d_bias[l]); cudaFree(m->d_bn_a[l]); cudaFree(m->d_bn_c[l]); }
+  void* ptrs[] = {m->d_ones, m->d_dense_w, m->d_dense_b, m->d_log_trans, m->d_cents};
   for (void* p : ptrs) cudaFree(p);
+  for (CrepeResampler& r : m->resamplers) cudaFree(r.d_taps);
+  work_free(m->work);
   delete m;
+}
+
+static int crepe_check_unused(const CrepeModel* m) {
+  RYK_CHECK(m == nullptr || m->plans == 0, "the CREPE model is in use by a live session (f0 method 2): destroy those sessions before changing it");
+  return 0;
 }
 
 int crepe_create(Engine* e, int capacity_multiplier) {
   RYK_CHECK(capacity_multiplier == 4 || capacity_multiplier == 8 || capacity_multiplier == 16 || capacity_multiplier == 24 || capacity_multiplier == 32,
             "CREPE capacity multiplier must be 4 (tiny), 8, 16, 24 or 32 (full)");
+  if (crepe_check_unused(g_crepe)) return -1;
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   crepe_free(g_crepe);
   CrepeModel* m = new CrepeModel();
@@ -269,6 +321,7 @@ void crepe_destroy() { crepe_free(g_crepe); g_crepe = nullptr; }
 int crepe_set_conv(Engine* e, int layer, const float* W, const float* bias, const float* gamma, const float* beta, const float* mean, const float* var) {
   CrepeModel* m = g_crepe;
   RYK_CHECK(m != nullptr && layer >= 0 && layer < 6, "create the CREPE model first; layers are 0..5");
+  if (crepe_check_unused(m)) return -1;
   const int cin = m->cin[layer], cout = m->cout[layer], k = kCrepeWidths[layer];
   const size_t nw = (size_t)cout * cin * k;
   float* d_tmp = nullptr;
@@ -296,6 +349,7 @@ int crepe_set_conv(Engine* e, int layer, const float* W, const float* bias, cons
 int crepe_set_dense(Engine* e, const float* W, const float* bias) {
   CrepeModel* m = g_crepe;
   RYK_CHECK(m != nullptr, "create the CREPE model first");
+  if (crepe_check_unused(m)) return -1;
   const int nin = 4 * m->cout[5];
   float* d_tmp = nullptr;
   RYK_CUDA(cudaMalloc(&d_tmp, sizeof(float) * nin * kCrepeBins));
@@ -312,6 +366,7 @@ int crepe_set_dense(Engine* e, const float* W, const float* bias) {
 int crepe_set_tables(Engine* e, const double* log_trans, const double* cents_mapping, double log_start, double log_emit_self, double log_emit_other) {
   CrepeModel* m = g_crepe;
   RYK_CHECK(m != nullptr, "create the CREPE model first");
+  if (crepe_check_unused(m)) return -1;
   if (!m->d_log_trans) RYK_CUDA(cudaMalloc(&m->d_log_trans, sizeof(double) * kCrepeBins * kCrepeBins));
   RYK_CUDA(cudaMemcpy(m->d_log_trans, log_trans, sizeof(double) * kCrepeBins * kCrepeBins, cudaMemcpyHostToDevice));
   if (!m->d_cents) RYK_CUDA(cudaMalloc(&m->d_cents, sizeof(double) * kCrepeBins));
@@ -326,45 +381,105 @@ int crepe_num_frames(int n16, double step_ms) {
   return hop > 0 ? 1 + (int)((n16 + 1024 - 1024) / hop) : 0;
 }
 
-static int crepe_reserve(CrepeModel* m, int F, int n) {
-  if (n > m->cap_audio) { cudaFree(m->d_audio); RYK_CUDA(cudaMalloc(&m->d_audio, sizeof(float) * n)); m->cap_audio = n; }
-  if (F <= m->cap_frames) return 0;
-  cudaFree(m->d_im2col); cudaFree(m->d_flat); cudaFree(m->d_logit); cudaFree(m->d_act); cudaFree(m->d_conf); cudaFree(m->d_obs);
-  cudaFree(m->d_lattice); cudaFree(m->d_path); cudaFree(m->d_f0); cudaFree(m->d_voicing); cudaFree(m->d_vlat);
-  for (int l = 0; l < 6; ++l) { cudaFree(m->d_conv[l]); cudaFree(m->d_in[l]); m->d_conv[l] = m->d_in[l] = nullptr; }
-  RYK_CUDA(cudaMalloc(&m->d_im2col, sizeof(float) * (size_t)F * 256 * 512));
+static int work_alloc(const CrepeModel* m, CrepeWork& w, int F, int n16, bool tc) {
+  RYK_CUDA(cudaMalloc(&w.d_audio, sizeof(float) * n16));
+  RYK_CUDA(cudaMalloc(&w.d_im2col, sizeof(float) * (size_t)F * 256 * 512));
   int W = 256;                                           // output length of block 0 before pooling
   for (int l = 0; l < 6; ++l) {
-    RYK_CUDA(cudaMalloc(&m->d_conv[l], sizeof(float) * (size_t)F * W * m->cout[l]));
+    RYK_CUDA(cudaMalloc(&w.d_conv[l], sizeof(float) * (size_t)F * W * m->cout[l]));
     const int Wo = W / 2;
     if (l < 5) {
       int n_out, left, right; same_padding(Wo, kCrepeWidths[l + 1], kCrepeStrides[l + 1], &n_out, &left, &right);
-      RYK_CUDA(cudaMalloc(&m->d_in[l + 1], sizeof(float) * (size_t)F * (Wo + left + right) * m->cout[l]));
+      RYK_CUDA(cudaMalloc(&w.d_in[l + 1], sizeof(float) * (size_t)F * (Wo + left + right) * m->cout[l]));
       W = n_out;
     }
   }
-  RYK_CUDA(cudaMalloc(&m->d_flat, sizeof(float) * (size_t)F * 4 * m->cout[5]));
-  RYK_CUDA(cudaMalloc(&m->d_logit, sizeof(float) * (size_t)F * kCrepeBins));
-  RYK_CUDA(cudaMalloc(&m->d_act, sizeof(float) * (size_t)F * kCrepeBins));
-  RYK_CUDA(cudaMalloc(&m->d_conf, sizeof(float) * F));
-  RYK_CUDA(cudaMalloc(&m->d_obs, sizeof(int) * F));
-  RYK_CUDA(cudaMalloc(&m->d_lattice, sizeof(double) * (size_t)F * kCrepeBins));
-  RYK_CUDA(cudaMalloc(&m->d_path, sizeof(int) * F));
-  RYK_CUDA(cudaMalloc(&m->d_f0, sizeof(double) * F));
-  RYK_CUDA(cudaMalloc(&m->d_voicing, sizeof(int) * F));
-  RYK_CUDA(cudaMalloc(&m->d_vlat, sizeof(double) * 2 * F));
-  m->cap_frames = F;
+  RYK_CUDA(cudaMalloc(&w.d_flat, sizeof(float) * (size_t)F * 4 * m->cout[5]));
+  RYK_CUDA(cudaMalloc(&w.d_logit, sizeof(float) * (size_t)F * kCrepeBins));
+  RYK_CUDA(cudaMalloc(&w.d_act, sizeof(float) * (size_t)F * kCrepeBins));
+  RYK_CUDA(cudaMalloc(&w.d_conf, sizeof(float) * F));
+  RYK_CUDA(cudaMalloc(&w.d_obs, sizeof(int) * F));
+  RYK_CUDA(cudaMalloc(&w.d_lattice, sizeof(double) * (size_t)F * kCrepeBins));
+  RYK_CUDA(cudaMalloc(&w.d_path, sizeof(int) * F));
+  RYK_CUDA(cudaMalloc(&w.d_f0, sizeof(double) * F));
+  RYK_CUDA(cudaMalloc(&w.d_voicing, sizeof(int) * F));
+  RYK_CUDA(cudaMalloc(&w.d_vlat, sizeof(double) * 2 * F));
+  if (tc) {
+    size_t ws = crepe_tc_ws_floats(F * 256, 512, m->cout[0]);
+    int Wl = 128;
+    for (int l = 1; l < 6; ++l) {
+      const size_t need = crepe_tc_ws_floats(F * Wl, kCrepeWidths[l] * m->cin[l], m->cout[l]);
+      if (need > ws) ws = need;
+      Wl /= 2;
+    }
+    if (ws) RYK_CUDA(cudaMalloc(&w.d_tc_ws, sizeof(float) * ws));
+  }
+  w.F = F; w.n16 = n16; w.tc = tc;
   return 0;
 }
 
-static int crepe_conv(Engine* e, CrepeModel* m, int l, const float* d_in, int F, int Win, int Cin, int KW, int SW, int Wout, float* d_out, cudaStream_t st) {
+// conv layer l over x = [F][Win][Cin] (layer 0: the im2col rows, Win = 256, Cin = 512, KW = 1) -> ReLU(conv + bias) [F][Wout][Cout],
+// stride 1, no padding (the buffers are already zero-framed)
+static int crepe_conv(Engine* e, CrepeModel* m, const CrepeWork& w, int l, const float* x, int F, int Win, int Cin, int KW, int Wout, float* y,
+                      cudaStream_t st) {
+  if (w.tc) {
+    CrepeGemm g;
+    g.x = x; g.M = F * Wout; g.W = Wout; g.fstride = (long long)Win * Cin; g.wstep = Cin; g.K = KW * Cin; g.N = m->cout[l];
+    g.w = m->d_w[l]; g.bias = m->d_bias[l]; g.y = y;
+    return crepe_tc_run(g, w.d_tc_ws, st, &e->launches);
+  }
   ConvLayer L;
   L.transposed = 0; L.B = F; L.Hin = 1; L.Win = Win; L.Hout = 1; L.Wout = Wout; L.C0 = Cin; L.C1 = 0; L.Cout = m->cout[l];
-  L.KH = 1; L.KW = KW; L.SH = 1; L.SW = SW; L.PH = 0; L.PW = 0; L.act = ACT_RELU;
-  L.in0 = d_in; L.in_dtype = DT_F32; L.out = d_out; L.out_dtype = DT_F32;
+  L.KH = 1; L.KW = KW; L.SH = 1; L.SW = 1; L.PH = 0; L.PW = 0; L.act = ACT_RELU;
+  L.in0 = x; L.in_dtype = DT_F32; L.out = y; L.out_dtype = DT_F32;
   L.w_direct = m->d_w[l]; L.scale = m->d_ones; L.shift = m->d_bias[l];
   e->launches += 1;
   return conv_direct_run(L, st);
+}
+
+static bool crepe_complete(const CrepeModel* m) {
+  if (m == nullptr || !m->tables) return false;
+  for (bool b : m->loaded) if (!b) return false;
+  return true;
+}
+
+// frames -> network -> sigmoid -> decoders over the n16 samples in w.d_audio (F frames at hop samples); stream-ordered only
+static int crepe_network(Engine* e, CrepeModel* m, CrepeWork& w, int n16, int hop, int F, cudaStream_t st) {
+  int n_out, left, right;
+  same_padding(1024, 512, 4, &n_out, &left, &right);                 // 256 outputs, 254 + 254
+  k_crepe_frames<<<F, 256, 0, st>>>(w.d_audio, n16, hop, left, w.d_im2col);
+  e->launches += 1;
+  // block 0: 1x1 conv over the im2col rows ([F][256][512] x [512][cout])
+  if (crepe_conv(e, m, w, 0, w.d_im2col, F, 256, 512, 1, 256, w.d_conv[0], st)) return -1;
+  int W = 256;
+  for (int l = 0; l < 6; ++l) {
+    const int Wo = W / 2;
+    if (l < 5) {
+      int nl, pl, pr; same_padding(Wo, kCrepeWidths[l + 1], kCrepeStrides[l + 1], &nl, &pl, &pr);
+      k_crepe_bn_pool<<<296, 256, 0, st>>>(w.d_conv[l], F, W, m->cout[l], m->d_bn_a[l], m->d_bn_c[l], pl, pr, w.d_in[l + 1]);
+      e->launches += 1;
+      if (crepe_conv(e, m, w, l + 1, w.d_in[l + 1], F, Wo + pl + pr, m->cout[l], kCrepeWidths[l + 1], nl, w.d_conv[l + 1], st)) return -1;
+      W = nl;
+    } else {
+      k_crepe_bn_pool<<<296, 256, 0, st>>>(w.d_conv[l], F, W, m->cout[l], m->d_bn_a[l], m->d_bn_c[l], 0, 0, w.d_flat);   // [F][4][C] = time-major flatten
+      e->launches += 1;
+    }
+  }
+  {                                                                   // Dense(360): 1x1 conv over [F][1][64 m]
+    ConvLayer L;
+    L.transposed = 0; L.B = F; L.Hin = 1; L.Win = 1; L.Hout = 1; L.Wout = 1; L.C0 = 4 * m->cout[5]; L.C1 = 0; L.Cout = kCrepeBins;
+    L.KH = 1; L.KW = 1; L.SH = 1; L.SW = 1; L.PH = 0; L.PW = 0; L.act = ACT_NONE;
+    L.in0 = w.d_flat; L.in_dtype = DT_F32; L.out = w.d_logit; L.out_dtype = DT_F32;
+    L.w_direct = m->d_dense_w; L.scale = m->d_ones; L.shift = m->d_dense_b;
+    if (conv_direct_run(L, st)) return -1;
+    e->launches += 1;
+  }
+  k_crepe_sigmoid<<<F, 128, 0, st>>>(w.d_logit, w.d_act, w.d_conf, w.d_obs);
+  k_crepe_decode<<<1, 384, 0, st>>>(w.d_act, w.d_conf, w.d_obs, F, m->d_log_trans, m->d_cents, m->h_log_start, m->h_log_emit[0], m->h_log_emit[1],
+                                   w.d_lattice, w.d_path, w.d_vlat, w.d_f0, w.d_voicing);
+  RYK_CUDA(cudaGetLastError());
+  e->launches += 2;
+  return 0;
 }
 
 // audio16k: host float32, n samples at 16 kHz.  Outputs (host, any may be null): f0 / confidence [F], voicing [F] (HMM state), activation [F][360].
@@ -372,58 +487,171 @@ int crepe_predict(Engine* e, const float* audio16k, int n, double step_ms, doubl
                   int* path_out) {
   CrepeModel* m = g_crepe;
   RYK_CHECK(m != nullptr && m->tables, "CREPE model / decoder tables not loaded");
-  for (int i = 0; i < 7; ++i) RYK_CHECK(m->loaded[i], "CREPE model is missing a layer");
+  RYK_CHECK(crepe_complete(m), "CREPE model is missing a layer");
   RYK_CHECK(m->cout[0] <= 1024, "scale vector too short");
   const int hop = (int)(16000 * step_ms / 1000);
   RYK_CHECK(hop > 0 && n > 0, "bad step size or empty signal");
   const int F = crepe_num_frames(n, step_ms);
   cudaStream_t st = e->stream;
-  if (crepe_reserve(m, F, n)) return -1;
-  RYK_CUDA(cudaMemcpyAsync(m->d_audio, audio16k, sizeof(float) * n, cudaMemcpyHostToDevice, st));
-  int n_out, left, right;
-  same_padding(1024, 512, 4, &n_out, &left, &right);                 // 256 outputs, 254 + 254
-  k_crepe_frames<<<F, 256, 0, st>>>(m->d_audio, n, hop, left, m->d_im2col);
-  // block 0: 1x1 conv over the im2col rows ([F][256][512] x [512][cout])
-  {
-    ConvLayer L;
-    L.transposed = 0; L.B = F; L.Hin = 1; L.Win = 256; L.Hout = 1; L.Wout = 256; L.C0 = 512; L.C1 = 0; L.Cout = m->cout[0];
-    L.KH = 1; L.KW = 1; L.SH = 1; L.SW = 1; L.PH = 0; L.PW = 0; L.act = ACT_RELU;
-    L.in0 = m->d_im2col; L.in_dtype = DT_F32; L.out = m->d_conv[0]; L.out_dtype = DT_F32;
-    L.w_direct = m->d_w[0]; L.scale = m->d_ones; L.shift = m->d_bias[0];
-    if (conv_direct_run(L, st)) return -1;
+  CrepeWork& w = m->work;
+  if (F > w.F || n > w.n16) {
+    const int F_cap = F > w.F ? F : w.F, n_cap = n > w.n16 ? n : w.n16;
+    RYK_CUDA(cudaStreamSynchronize(st));
+    work_free(w);
+    if (work_alloc(m, w, F_cap, n_cap, false)) { work_free(w); return -1; }
   }
-  int W = 256;
-  for (int l = 0; l < 6; ++l) {
-    const int Wo = W / 2;
-    if (l < 5) {
-      int nl, pl, pr; same_padding(Wo, kCrepeWidths[l + 1], kCrepeStrides[l + 1], &nl, &pl, &pr);
-      k_crepe_bn_pool<<<296, 256, 0, st>>>(m->d_conv[l], F, W, m->cout[l], m->d_bn_a[l], m->d_bn_c[l], pl, pr, m->d_in[l + 1]);
-      if (crepe_conv(e, m, l + 1, m->d_in[l + 1], F, Wo + pl + pr, m->cout[l], kCrepeWidths[l + 1], 1, nl, m->d_conv[l + 1], st)) return -1;
-      W = nl;
-    } else {
-      k_crepe_bn_pool<<<296, 256, 0, st>>>(m->d_conv[l], F, W, m->cout[l], m->d_bn_a[l], m->d_bn_c[l], 0, 0, m->d_flat);   // [F][4][C] = time-major flatten
-    }
-  }
-  {                                                                   // Dense(360): 1x1 conv over [F][1][64 m]
-    ConvLayer L;
-    L.transposed = 0; L.B = F; L.Hin = 1; L.Win = 1; L.Hout = 1; L.Wout = 1; L.C0 = 4 * m->cout[5]; L.C1 = 0; L.Cout = kCrepeBins;
-    L.KH = 1; L.KW = 1; L.SH = 1; L.SW = 1; L.PH = 0; L.PW = 0; L.act = ACT_NONE;
-    L.in0 = m->d_flat; L.in_dtype = DT_F32; L.out = m->d_logit; L.out_dtype = DT_F32;
-    L.w_direct = m->d_dense_w; L.scale = m->d_ones; L.shift = m->d_dense_b;
-    if (conv_direct_run(L, st)) return -1;
-  }
-  k_crepe_sigmoid<<<F, 128, 0, st>>>(m->d_logit, m->d_act, m->d_conf, m->d_obs);
-  k_crepe_decode<<<1, 384, 0, st>>>(m->d_act, m->d_conf, m->d_obs, F, m->d_log_trans, m->d_cents, m->h_log_start, m->h_log_emit[0], m->h_log_emit[1],
-                                   m->d_lattice, m->d_path, m->d_vlat, m->d_f0, m->d_voicing);
-  RYK_CUDA(cudaGetLastError());
-  e->launches += 12;
-  if (f0) RYK_CUDA(cudaMemcpyAsync(f0, m->d_f0, sizeof(double) * F, cudaMemcpyDeviceToHost, st));
-  if (confidence) RYK_CUDA(cudaMemcpyAsync(confidence, m->d_conf, sizeof(float) * F, cudaMemcpyDeviceToHost, st));
-  if (voicing) RYK_CUDA(cudaMemcpyAsync(voicing, m->d_voicing, sizeof(int) * F, cudaMemcpyDeviceToHost, st));
-  if (activation) RYK_CUDA(cudaMemcpyAsync(activation, m->d_act, sizeof(float) * (size_t)F * kCrepeBins, cudaMemcpyDeviceToHost, st));
-  if (path_out) RYK_CUDA(cudaMemcpyAsync(path_out, m->d_path, sizeof(int) * F, cudaMemcpyDeviceToHost, st));
+  RYK_CUDA(cudaMemcpyAsync(w.d_audio, audio16k, sizeof(float) * n, cudaMemcpyHostToDevice, st));
+  if (crepe_network(e, m, w, n, hop, F, st)) return -1;
+  if (f0) RYK_CUDA(cudaMemcpyAsync(f0, w.d_f0, sizeof(double) * F, cudaMemcpyDeviceToHost, st));
+  if (confidence) RYK_CUDA(cudaMemcpyAsync(confidence, w.d_conf, sizeof(float) * F, cudaMemcpyDeviceToHost, st));
+  if (voicing) RYK_CUDA(cudaMemcpyAsync(voicing, w.d_voicing, sizeof(int) * F, cudaMemcpyDeviceToHost, st));
+  if (activation) RYK_CUDA(cudaMemcpyAsync(activation, w.d_act, sizeof(float) * (size_t)F * kCrepeBins, cudaMemcpyDeviceToHost, st));
+  if (path_out) RYK_CUDA(cudaMemcpyAsync(path_out, w.d_path, sizeof(int) * F, cudaMemcpyDeviceToHost, st));
   RYK_CUDA(cudaStreamSynchronize(st));
   return 0;
+}
+
+// taps: the (odd-length) resample_poly filter for fs -> 16 kHz, up / down = 16000 / fs reduced
+int crepe_set_resampler(Engine* e, int fs, int up, int down, const double* taps, int n_taps) {
+  CrepeModel* m = g_crepe;
+  RYK_CHECK(m != nullptr, "create the CREPE model first");
+  if (crepe_check_unused(m)) return -1;
+  RYK_CHECK(fs > 0 && up > 0 && down > 0 && (long long)fs * up == 16000LL * down, "up / down must map fs to 16 kHz");
+  RYK_CHECK(taps != nullptr && n_taps > 0 && (n_taps & 1), "the resampler filter must have an odd number of taps");
+  CrepeResampler* r = nullptr;
+  for (CrepeResampler& x : m->resamplers) if (x.fs == fs) r = &x;
+  if (!r) { m->resamplers.emplace_back(); r = &m->resamplers.back(); r->fs = fs; }
+  if (r->d_taps && r->n_taps != n_taps) { RYK_CUDA(cudaFree(r->d_taps)); r->d_taps = nullptr; }
+  if (!r->d_taps) RYK_CUDA(cudaMalloc(&r->d_taps, sizeof(double) * n_taps));
+  RYK_CUDA(cudaMemcpy(r->d_taps, taps, sizeof(double) * n_taps, cudaMemcpyHostToDevice));
+  r->up = up; r->down = down; r->n_taps = n_taps;
+  return 0;
+}
+
+void crepe_plan_free(CrepePlan* p) {
+  if (!p) return;
+  work_free(p->w);
+  cudaFree(p->d_f0);
+  if (g_crepe) g_crepe->plans--;
+  delete p;
+}
+
+// A forward for n samples at fs, analysed with frame_period: the frames must coincide with WORLD's n / hop + 1.
+// Precision mode 1 runs the convolutions on the 3xTF32 tensor-core kernel, mode 0 on conv_direct (the FP32 bisect mode).
+int crepe_plan_create(Engine* e, int n, int fs, double frame_period, CrepePlan** out) {
+  CrepeModel* m = g_crepe;
+  RYK_CHECK(crepe_complete(m), "f0 method 2 (CREPE) needs a complete CREPE model and decoder tables: load one first (RYK_CREPE_MODEL)");
+  const CrepeResampler* r = nullptr;
+  for (const CrepeResampler& x : m->resamplers) if (x.fs == fs) r = &x;
+  RYK_CHECK(r != nullptr, "f0 method 2 (CREPE): no resampler taps to 16 kHz for this sampling rate (ryk_crepe_set_resampler)");
+  const int hop = (int)(fs * frame_period / 1000.0), hop16 = (int)(16000 * frame_period / 1000);
+  const int n16 = ryk_resample_length(n, r->up, r->down);
+  RYK_CHECK(hop > 0 && hop16 > 0 && n > 0, "bad frame period or empty window");
+  const int F = crepe_num_frames(n16, frame_period);
+  RYK_CHECK(F == n / hop + 1, "f0 method 2 (CREPE): the CREPE frame count of the analysis window differs from WORLD's n / hop + 1");
+  CrepePlan* p = new CrepePlan();
+  m->plans++;
+  p->n = n; p->hop16 = hop16; p->up = r->up; p->down = r->down; p->n_taps = r->n_taps; p->d_taps = r->d_taps;
+  if (work_alloc(m, p->w, F, n16, e->precision == 1) || cudaMalloc(&p->d_f0, sizeof(double) * F) != cudaSuccess) {
+    crepe_plan_free(p);
+    RYK_CHECK(false, "f0 method 2 (CREPE): out of device memory for the analysis plan");
+  }
+  *out = p;
+  return 0;
+}
+
+// resample d_x (n samples at fs) to 16 kHz, run the network and decoders and apply the voicing rule into crepe_plan_f0(p).
+// No allocation, host copy or synchronisation: the sequence can be captured in a CUDA graph.
+int crepe_plan_run(Engine* e, CrepePlan* p, const float* d_x, cudaStream_t st) {
+  CrepeModel* m = g_crepe;
+  CrepeWork& w = p->w;
+  if (resample_poly_run(e, d_x, p->n, p->up, p->down, p->d_taps, p->n_taps, w.d_audio, w.n16, st)) return -1;
+  if (crepe_network(e, m, w, w.n16, p->hop16, w.F, st)) return -1;
+  k_crepe_voiced<<<(w.F + 127) / 128, 128, 0, st>>>(w.d_f0, w.d_conf, w.d_voicing, w.F, p->d_f0);
+  RYK_CUDA(cudaGetLastError());
+  e->launches += 1;
+  return 0;
+}
+
+const double* crepe_plan_f0(const CrepePlan* p) { return p->d_f0; }
+
+// ---- test entry points ---------------------------------------------------------------------------------------------------------
+// One CREPE-shaped conv layer in isolation: x [F][Win][Cin], W (Cout, Cin, k), stride 1, no padding -> y = ReLU(conv + bias)
+// [F][Win - k + 1][Cout].  Layer 1 is given as its im2col form (Win = 256, Cin = 512, k = 1).  backend 0: conv_direct, 1: crepe_tc.
+int crepe_test_conv(Engine* e, int backend, int F, int Win, int Cin, int Cout, int k, const float* x, const float* W, const float* bias, float* y) {
+  RYK_CHECK((backend == 0 || backend == 1) && F > 0 && Cin > 0 && Cout > 0 && k > 0 && Win >= k, "bad CREPE test-conv arguments");
+  const int Wout = Win - k + 1;
+  const size_t nx = (size_t)F * Win * Cin, nw = (size_t)Cout * Cin * k, ny = (size_t)F * Wout * Cout;
+  const size_t nws = backend ? crepe_tc_ws_floats(F * Wout, k * Cin, Cout) : 0;
+  cudaStream_t st = e->stream;
+  std::vector<void*> frees;
+  auto A = [&](size_t bytes) -> float* { void* p = nullptr; if (cudaMalloc(&p, bytes ? bytes : 16) != cudaSuccess) return nullptr; frees.push_back(p); return (float*)p; };
+  float *d_x = A(nx * 4), *d_wraw = A(nw * 4), *d_w = A(nw * 4), *d_b = A(Cout * 4), *d_ones = A(Cout * 4), *d_y = A(ny * 4), *d_ws = A(nws * 4);
+  int rc = -1;
+  if (d_x && d_wraw && d_w && d_b && d_ones && d_y && d_ws) {
+    std::vector<float> ones(Cout, 1.f);
+    cudaMemcpyAsync(d_x, x, nx * 4, cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(d_wraw, W, nw * 4, cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(d_b, bias, Cout * 4, cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(d_ones, ones.data(), Cout * 4, cudaMemcpyHostToDevice, st);
+    rc = pack_weights_direct(d_wraw, 0, Cin, Cout, 1, k, d_w, st);
+    if (!rc && backend) {
+      CrepeGemm g;
+      g.x = d_x; g.M = F * Wout; g.W = Wout; g.fstride = (long long)Win * Cin; g.wstep = Cin; g.K = k * Cin; g.N = Cout;
+      g.w = d_w; g.bias = d_b; g.y = d_y;
+      rc = crepe_tc_run(g, d_ws, st, &e->launches);
+    } else if (!rc) {
+      ConvLayer L;
+      L.transposed = 0; L.B = F; L.Hin = 1; L.Win = Win; L.Hout = 1; L.Wout = Wout; L.C0 = Cin; L.C1 = 0; L.Cout = Cout;
+      L.KH = 1; L.KW = k; L.SH = 1; L.SW = 1; L.PH = 0; L.PW = 0; L.act = ACT_RELU;
+      L.in0 = d_x; L.in_dtype = DT_F32; L.out = d_y; L.out_dtype = DT_F32; L.w_direct = d_w; L.scale = d_ones; L.shift = d_b;
+      rc = conv_direct_run(L, st);
+    }
+    if (!rc && (cudaMemcpyAsync(y, d_y, ny * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)) {
+      rc = -1;
+      set_error("CREPE test conv failed on the device");
+    }
+  } else {
+    set_error("cudaMalloc failed in the CREPE test conv");
+  }
+  cudaStreamSynchronize(st);
+  for (void* p : frees) cudaFree(p);
+  return rc;
+}
+
+// The network and decoders on a host 16 kHz signal with an explicit conv backend (0: conv_direct, 1: crepe_tc), on a workspace of its
+// own.  activation [F][360], path / voicing [F] (any may be null).  repeat > 0: that many further network runs are timed with CUDA
+// events and *ms_per_run receives their mean device time.
+int crepe_test_network(Engine* e, int backend, const float* audio16k, int n, double step_ms, float* activation, int* path, int* voicing,
+                       int repeat, float* ms_per_run) {
+  CrepeModel* m = g_crepe;
+  RYK_CHECK(crepe_complete(m), "CREPE model / decoder tables not loaded");
+  RYK_CHECK(backend == 0 || backend == 1, "backend must be 0 (conv_direct) or 1 (3xTF32 tensor cores)");
+  const int hop = (int)(16000 * step_ms / 1000);
+  RYK_CHECK(hop > 0 && n > 0, "bad step size or empty signal");
+  const int F = crepe_num_frames(n, step_ms);
+  cudaStream_t st = e->stream;
+  CrepeWork w;
+  int rc = work_alloc(m, w, F, n, backend == 1);
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  if (!rc) rc = cudaMemcpyAsync(w.d_audio, audio16k, sizeof(float) * n, cudaMemcpyHostToDevice, st) == cudaSuccess ? 0 : -1;
+  if (!rc) rc = crepe_network(e, m, w, n, hop, F, st);
+  if (!rc && activation) rc = cudaMemcpyAsync(activation, w.d_act, sizeof(float) * (size_t)F * kCrepeBins, cudaMemcpyDeviceToHost, st) == cudaSuccess ? 0 : -1;
+  if (!rc && path) rc = cudaMemcpyAsync(path, w.d_path, sizeof(int) * F, cudaMemcpyDeviceToHost, st) == cudaSuccess ? 0 : -1;
+  if (!rc && voicing) rc = cudaMemcpyAsync(voicing, w.d_voicing, sizeof(int) * F, cudaMemcpyDeviceToHost, st) == cudaSuccess ? 0 : -1;
+  if (!rc && repeat > 0 && ms_per_run) {
+    rc = (cudaEventCreate(&ev[0]) == cudaSuccess && cudaEventCreate(&ev[1]) == cudaSuccess && cudaEventRecord(ev[0], st) == cudaSuccess) ? 0 : -1;
+    for (int i = 0; i < repeat && !rc; ++i) rc = crepe_network(e, m, w, n, hop, F, st);
+    float ms = 0.f;
+    if (!rc) rc = (cudaEventRecord(ev[1], st) == cudaSuccess && cudaEventSynchronize(ev[1]) == cudaSuccess &&
+                   cudaEventElapsedTime(&ms, ev[0], ev[1]) == cudaSuccess) ? 0 : -1;
+    if (!rc) *ms_per_run = ms / repeat;
+  }
+  if (cudaStreamSynchronize(st) != cudaSuccess && !rc) rc = -1;
+  for (cudaEvent_t x : ev) if (x) cudaEventDestroy(x);
+  work_free(w);
+  if (rc) set_error("CREPE test network failed");
+  return rc;
 }
 
 }  // namespace ryk

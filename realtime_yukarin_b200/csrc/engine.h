@@ -14,6 +14,7 @@ namespace ryk {
 
 struct DioPlan;
 struct HarvestPlan;
+struct CrepePlan;
 struct Session;
 struct Group;
 struct Reblock;
@@ -22,7 +23,7 @@ struct Engine {
   int device = 0;
   cudaStream_t stream = nullptr;
   int precision = 1;                 // 0: FP32 CUDA-core convs everywhere, 1: FP16 wgmma tensor-core convs where eligible
-  int f0_method = 0;                 // 0: DIO + StoneMask, 1: Harvest + StoneMask (world_harvest.cu)
+  int f0_method = 0;                 // 0: DIO + StoneMask, 1: Harvest + StoneMask (world_harvest.cu), 2: CREPE (sessions only, crepe.cu)
   bool s1_fused = true;              // FP16 mode: stage 1 as ONE cluster kernel (s1_fused.cu) instead of 16 layer launches
   // FFT twiddles
   double2* d_twiddle = nullptr;
@@ -87,6 +88,14 @@ int crepe_set_dense(Engine* e, const float* W, const float* bias);
 int crepe_set_tables(Engine* e, const double* log_trans, const double* cents_mapping, double log_start, double log_emit_self, double log_emit_other);
 int crepe_num_frames(int n16, double step_ms);
 int crepe_predict(Engine* e, const float* audio16k, int n, double step_ms, double* f0, float* confidence, int* voicing, float* activation, int* path_out);
+int crepe_set_resampler(Engine* e, int fs, int up, int down, const double* taps, int n_taps);
+int crepe_plan_create(Engine* e, int n, int fs, double frame_period, CrepePlan** out);
+void crepe_plan_free(CrepePlan* p);
+int crepe_plan_run(Engine* e, CrepePlan* p, const float* d_x, cudaStream_t st);
+const double* crepe_plan_f0(const CrepePlan* p);
+int crepe_test_conv(Engine* e, int backend, int F, int Win, int Cin, int Cout, int k, const float* x, const float* W, const float* bias, float* y);
+int crepe_test_network(Engine* e, int backend, const float* audio16k, int n, double step_ms, float* activation, int* path, int* voicing,
+                       int repeat, float* ms_per_run);
 int spectral_analysis_run(Engine* e, const float* d_x, int n, int fs, double frame_period, const double* d_f0, int n_out,
                           int fft_size, int order, float* d_sp, float* d_ap, float* d_mc, float* d_f0_out, uint8_t* d_voiced,
                           cudaStream_t st);

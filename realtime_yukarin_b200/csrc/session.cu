@@ -12,7 +12,7 @@
 //   converted window (n_feat + 2 e_dec frames of f0/ap/sp)                      -> realtime synthesizer -> NaN scrub
 //
 // Pipelining = what run.py does with three OS processes and queues (run.py:58-93), done with streams and events:
-//   stream E: slide wave, silence gate (needs only the samples), DIO/StoneMask/CheapTrick/D4C          of chunk k+1
+//   stream E: slide wave, silence gate (needs only the samples), DIO/StoneMask (or CREPE)/CheapTrick/D4C of chunk k+1
 //   stream C: slide features, stage-1 U-Net (+f0 map), mc2sp                                          of chunk k
 //   stream C2: stage-2 U-Net (the wgmma layers)                                                     of chunk k-1
 //   stream D: slide converted features, synthesizer add/plan/pulse/overlap-add, NaN scrub             of chunk k-2
@@ -112,7 +112,8 @@ struct Session {
   // whose body i is the stage-1 sequence for the padded length 128 i (0: no effective frame)}; no host sync on the submit path
   cudaGraphExec_t s1_switch[2] = {nullptr, nullptr}; long long s1_switch_launches[2][16]; int s1_buckets = 0; int last_bucket = 0;
   Synth* synth = nullptr;
-  DioPlan* dio[2] = {nullptr, nullptr};     // one analysis plan per chunk parity (owned)
+  DioPlan* dio[2] = {nullptr, nullptr};     // one analysis plan per chunk parity (owned), f0 methods 0 and 1
+  CrepePlan* crepe[2] = {nullptr, nullptr}; // f0 method 2: one CREPE forward per chunk parity (owned) in place of DIO/Harvest
   std::vector<void*> allocs, pinned;
 };
 
@@ -264,6 +265,7 @@ static void session_free(Session* s) {
   for (void* p : s->allocs) cudaFree(p);
   for (void* p : s->pinned) cudaFreeHost(p);
   for (DioPlan* p : s->dio) dio_plan_free(p);
+  for (CrepePlan* p : s->crepe) crepe_plan_free(p);
   synth_destroy(s->synth);
   delete s;                                       // drops the stage graphs
 }
@@ -483,10 +485,18 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
   if (k >= 2) RYK_CUDA(cudaStreamWaitEvent(sA, s->ev[(k - 2) % kRing].cslide, 0));   // enc_*[b] consumed by stage 1 of k-2
   if (stage_time(s, 1, 0, r, sA)) return -1;
   if (run_graph(e, pg.analysis, sA, [&]() -> int {
-        if (dio_stonemask_run(e, s->dio[b], s->wave_win[g], sA)) return -1;
+        const double* d_f0 = nullptr;
+        if (s->crepe[b]) {
+          if (crepe_plan_run(e, s->crepe[b], s->wave_win[g], sA)) return -1;
+          d_f0 = crepe_plan_f0(s->crepe[b]);
+          e->launches += 3;                       // spectral_analysis_run (crepe_plan_run counts its own)
+        } else {
+          if (dio_stonemask_run(e, s->dio[b], s->wave_win[g], sA)) return -1;
+          d_f0 = dio_plan_f0(s->dio[b]);
+          e->launches += 13;
+        }
         const int n_enc = s->Lw / s->hop;
-        e->launches += 13;
-        return spectral_analysis_run(e, s->wave_win[g], s->Lw, c.fs, c.frame_period_ms, dio_plan_f0(s->dio[b]), n_enc, c.fft_length, c.order,
+        return spectral_analysis_run(e, s->wave_win[g], s->Lw, c.fs, c.frame_period_ms, d_f0, n_enc, c.fft_length, c.order,
                                      s->enc_sp[b], s->enc_ap[b], s->enc_mc[b], s->enc_f0[b], s->enc_voiced[b], sA);
       })) return -1;
   if (stage_time(s, 1, 1, r, sA)) return -1;
@@ -677,12 +687,29 @@ struct ryk_engine { Engine impl; };
 
 extern "C" {
 
+static int session_build(Engine* e, Session* s, const ryk_session_config* cfg);
+
 int ryk_session_create(ryk_engine* h, const ryk_session_config* cfg, int* session_id) {
   Engine* e = &h->impl;
   RYK_CUDA(cudaSetDevice(e->device));
   RYK_CHECK(cfg && session_id, "null argument");
   RYK_CHECK(e->stage1 && e->stage2, "load both models before creating a session");
   Session* s = new Session();
+  if (session_build(e, s, cfg)) {
+    // free whatever the build made (buffers, analysis / CREPE plans, graphs, U-Net plans); ryk_last_error keeps the cause
+    const int s1_owner = s->s1_owner, s2_owner[2] = {s->s2_owner[0], s->s2_owner[1]};
+    session_free(s);
+    if (s1_owner) unet_release_owner(e->stage1, s1_owner);
+    for (int owner : s2_owner) if (owner) unet_release_owner(e->stage2, owner);
+    return -1;
+  }
+  e->sessions.push_back(s);
+  *session_id = (int)e->sessions.size() - 1;
+  return 0;
+}
+
+// Everything a session allocates and captures; on failure the caller frees the partly built session.
+static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
   s->cfg = *cfg;
   s->hop = (int)(cfg->fs * cfg->frame_period_ms / 1000.0);
   s->rate = (int)lround(1000.0 / cfg->frame_period_ms);
@@ -767,8 +794,12 @@ int ryk_session_create(ryk_engine* h, const ryk_session_config* cfg, int* sessio
     if (P((void**)&s->h_n[i], sizeof(int))) return -1;
     if (P((void**)&s->h_count[i], sizeof(int) * 2)) return -1;
   }
-  for (int i = 0; i < 2; ++i)
-    if (dio_plan_create(e, s->Lw, cfg->fs, cfg->frame_period_ms, cfg->f0_floor, cfg->f0_ceil, &s->dio[i], e->f0_method)) return -1;
+  // f0 method 2: each step's encode window is analysed on its own, like one crepe.predict call per fetched window (DESIGN.md C3)
+  for (int i = 0; i < 2; ++i) {
+    const int rc = e->f0_method == 2 ? crepe_plan_create(e, s->Lw, cfg->fs, cfg->frame_period_ms, &s->crepe[i])
+                                     : dio_plan_create(e, s->Lw, cfg->fs, cfg->frame_period_ms, cfg->f0_floor, cfg->f0_ceil, &s->dio[i], e->f0_method);
+    if (rc) return -1;
+  }
   if (synth_create(e, cfg->fs, cfg->frame_period_ms, cheaptrick_fft_size(cfg->fs, 71.0), cfg->vocoder_buffer_size, 4096, &s->synth)) return -1;
   // build the U-Net plans this session can need up front (allocation + tensor maps), not on the first chunk
   UNetPlan* p = nullptr;
@@ -779,8 +810,6 @@ int ryk_session_create(ryk_engine* h, const ryk_session_config* cfg, int* sessio
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   RYK_CUDA(cudaDeviceSynchronize());
   for (int b = 0; b < 2; ++b) if (stage1_build_switch(e, s, b)) return -1;
-  e->sessions.push_back(s);
-  *session_id = (int)e->sessions.size() - 1;
   return 0;
 }
 

@@ -58,6 +58,7 @@ EXPORTED_SYMBOLS = [
     'ryk_resample_poly', 'ryk_session_poll', 'ryk_reblock_poll', 'ryk_engine_profile_read2', 'ryk_engine_set_stage1_fused',
     'ryk_engine_set_f0_method', 'ryk_engine_get_f0_method', 'ryk_debug_harvest',
     'ryk_crepe_create', 'ryk_crepe_set_conv', 'ryk_crepe_set_dense', 'ryk_crepe_set_decoder_tables', 'ryk_crepe_num_frames', 'ryk_crepe_predict',
+    'ryk_crepe_set_resampler', 'ryk_crepe_test_conv', 'ryk_crepe_test_network',
 ]
 
 
@@ -373,16 +374,17 @@ class Engine(object):
         self._check(self.lib.ryk_resample_poly(self._h, _fp(x), len(x), int(up), int(down), _dp(taps), len(taps), _fp(y), len(y), ctypes.byref(no)))
         return y[:no.value]
 
-    F0_METHODS = {'dio': 0, 'harvest': 1}
+    F0_METHODS = {'dio': 0, 'harvest': 1, 'crepe': 2}
 
     def set_f0_method(self, method: str):
-        """f0 extractor of world_f0 / world_analyze / sessions created afterwards: 'dio' (pyworld.dio + stonemask, default) or
-        'harvest' (pyworld.harvest + stonemask) -- yukarin's AcousticFeature.extract f0 hook (acoustic_feature_wrapper.py:28-33)."""
+        """f0 extractor of world_f0 / world_analyze / sessions created afterwards: 'dio' (pyworld.dio + stonemask, default),
+        'harvest' (pyworld.harvest + stonemask) -- yukarin's AcousticFeature.extract f0 hook (acoustic_feature_wrapper.py:28-33) --
+        or 'crepe' (sessions only; needs a loaded CREPE model, realtime_yukarin_b200.crepe.load_crepe_model)."""
         self._check(self.lib.ryk_engine_set_f0_method(self._h, self.F0_METHODS[method]))
 
     @property
     def f0_method(self) -> str:
-        return ['dio', 'harvest'][self.lib.ryk_engine_get_f0_method(self._h)]
+        return ['dio', 'harvest', 'crepe'][self.lib.ryk_engine_get_f0_method(self._h)]
 
     def debug_harvest(self, n, fs, frame_period, f0_floor, f0_ceil):
         """Intermediate arrays of the last Harvest analysis with this plan (see ryk_debug_harvest)."""

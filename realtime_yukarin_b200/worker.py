@@ -23,7 +23,7 @@ from typing import Any, Deque, List, Optional, Tuple
 
 import numpy
 
-from .config import Config
+from .config import Config, VocodeMode
 from .engine import Engine, SessionConfig, default_engine
 
 
@@ -101,15 +101,28 @@ class RealtimePipeline(object):
         # Here the stages are CUDA streams, so the figures are device times between CUDA events (ryk_session_stage_times).
         self._loggers = {k: logging.getLogger(k) for k in ('encode', 'convert', 'decode')}
         self._timing = any(lg.isEnabledFor(logging.DEBUG) for lg in self._loggers.values())
+        # extract_f0_mode: crepe (run.py:40-44 hands it to the encode worker's Vocoder) analyses each encode window with CREPE
+        # instead of DIO.  The session takes the engine's f0 method at creation; the engine's own setting is restored afterwards.
+        crepe_mode = VocodeMode(config.extract_f0_mode) is VocodeMode.CREPE
+        if crepe_mode:
+            from . import crepe
+            crepe.engine_with_model(self.engine)
+            crepe.set_session_rate(config.input_rate, self.engine)
+            prev_method = self.engine.f0_method
+            self.engine.set_f0_method('crepe')
         if self._timing:
             prev = os.environ.get('RYK_STAGE_TIMES')
             os.environ['RYK_STAGE_TIMES'] = '1'
-        self._sid = self.engine.session_create(cfg)
-        if self._timing:
-            if prev is None:
-                os.environ.pop('RYK_STAGE_TIMES', None)
-            else:
-                os.environ['RYK_STAGE_TIMES'] = prev
+        try:
+            self._sid = self.engine.session_create(cfg)
+        finally:
+            if self._timing:
+                if prev is None:
+                    os.environ.pop('RYK_STAGE_TIMES', None)
+                else:
+                    os.environ['RYK_STAGE_TIMES'] = prev
+            if crepe_mode:
+                self.engine.set_f0_method(prev_method)
         # capacity of one step's synthesizer output, as the session sizes it: (decode-window samples // block + 4) blocks
         rate = round(1000 / float(config.frame_period))
         hop = round(config.output_rate * float(config.frame_period) / 1000)
