@@ -246,6 +246,17 @@ int ryk_group_push_device(ryk_engine* e, int group_id, const float* const* waves
  * [frames][columns] (after refinement and removal), best / basic [frames], f0_raw [n / hop + 1] (before StoneMask).  Any may be NULL. */
 int ryk_debug_harvest(ryk_engine* e, int n, int fs, double frame_period_ms, double f0_floor, double f0_ceil, int* info, double* y,
                       double* raw, double* cand, double* score, double* best, double* basic, double* f0_raw);
+/* Stage-2 row bands.  A streaming session keeps only the chunk's frames of each converted window, so its stage-2 forward computes
+ * only the decoder rows those frames depend on.
+ * ryk_stage2_row_bands (host only): for a (Tp, W) input of which rows [keep_begin, keep_begin + keep_len) are kept,
+ *   bands[2 i], bands[2 i + 1] = the class-local output rows [y0, y1) that layer i (0..15) of an FP16 plan computes.
+ * ryk_test_stage2_forward: one forward of the loaded stage-2 net on a fresh plan whose buffers are first filled with NaN;
+ *   x, y: [B][Tp][512] float32 network input / output.  mode 0 = every row; 1 = banded for the hull of the n_keep ranges
+ *   [keep_begin[i], keep_begin[i] + keep_len[i]); 2 = as 1 with every layer split along K as in the full plan.  Rows outside the
+ *   band are left NaN. */
+int ryk_stage2_row_bands(int Tp, int W, int keep_begin, int keep_len, int* bands);
+int ryk_test_stage2_forward(ryk_engine* e, int B, int Tp, int n_keep, const int* keep_begin, const int* keep_len, int mode, const float* x,
+                            float* y);
 /* One conv (transposed = 0) or transposed-conv layer of the U-Nets in isolation, host fp32 NHWC tensors in and
  * out, weights in the Chainer layout; use_tc selects the FP16 wgmma kernel (1) or the FP32 CUDA-core kernel (0).
  * `repeat` extra timed runs report the mean device time per run (ms) -- used by the unit parity tests and ncu. */

@@ -716,6 +716,53 @@ int ryk_debug_harvest(ryk_engine* h, int n, int fs, double fp, double f0_floor, 
   return harvest_plan_debug_copy(dio_plan_harvest(plan), info, y, raw, cand, score, best, basic, e->stream);
 }
 
+// ---- stage-2 row bands ----------------------------------------------------------------------------
+// Host only: the row band of every layer of a stage-2 FP16 plan for a (Tp, W) input of which rows [keep_begin, keep_begin + keep_len)
+// are kept.  bands[2 i], bands[2 i + 1] = class-local output rows [y0, y1) that layer i computes (every row when it is not banded).
+int ryk_stage2_row_bands(int Tp, int W, int keep_begin, int keep_len, int* bands) {
+  RYK_CHECK(bands && Tp >= 128 && Tp % 128 == 0 && W >= 128 && W % 128 == 0, "stage-2 input extents must be multiples of 128");
+  RYK_CHECK(keep_len > 0 && keep_begin >= 0 && keep_begin + keep_len <= Tp, "kept rows outside the stage-2 input");
+  UNet* n = unet_create(2, 1, 1, 64);
+  std::vector<ConvLayer> layers(16);
+  for (int i = 0; i < 16; ++i) unet_layer_shape(n, i, 1, Tp, W, layers[i]);
+  unet_destroy(n);
+  unet_derive_bands(layers, keep_begin, keep_len);
+  for (int i = 0; i < 16; ++i) { bands[2 * i] = layers[i].band_y0; bands[2 * i + 1] = layer_band_end(layers[i]); }
+  return 0;
+}
+
+// One stage-2 forward on a fresh plan whose buffers (activations, split-K workspaces, output) are first filled with NaN, so that
+// a row the banded decoder reads without having computed it shows up in the output.  x, y: host [B][Tp][512] float32 (network
+// input and output, the log-spectrum without its last bin).  mode 0: full plan; 1: banded plan for the hull of the n_keep row
+// ranges [keep_begin[i], keep_begin[i] + keep_len[i]); 2: as 1, with each banded layer split along K as in the full plan.
+int ryk_test_stage2_forward(ryk_engine* h, int B, int Tp, int n_keep, const int* keep_begin, const int* keep_len, int mode, const float* x,
+                            float* y) {
+  Engine* e = E(h);
+  RYK_CUDA(cudaSetDevice(e->device));
+  RYK_CHECK(e->stage2 != nullptr, "stage-2 model not loaded");
+  RYK_CHECK(B >= 1 && Tp >= 128 && Tp % 128 == 0 && mode >= 0 && mode <= 2 && (mode == 0 || n_keep >= 1), "bad stage-2 test arguments");
+  int kb = 0, kl = 0;
+  if (mode != 0) keep_hull(n_keep, keep_begin, keep_len, &kb, &kl);
+  const int owner = ++e->plan_owners;
+  UNetPlan* p = nullptr;
+  int rc = unet_get_plan(e, e->stage2, B, Tp, 512, e->precision, &p, owner, kb, kl, mode == 2);
+  if (!rc) {
+    cudaStream_t st = e->stream;
+    const size_t nx = (size_t)B * Tp * 512;
+    cudaError_t err = cudaSuccess;
+    for (size_t i = 0; i < p->buffers.size() && err == cudaSuccess; ++i)      // 0xFFFF: FP16 NaN; 0xFFFFFFFF: FP32 NaN
+      err = cudaMemsetAsync(p->buffers[i], 0xFF, p->buffer_bytes[i], st);
+    if (err == cudaSuccess) err = cudaMemcpyAsync(p->d_in, x, sizeof(float) * nx, cudaMemcpyHostToDevice, st);
+    if (err == cudaSuccess) rc = unet_forward(e, p, st);
+    if (err == cudaSuccess && !rc) err = cudaMemcpyAsync(y, p->d_out, sizeof(float) * nx, cudaMemcpyDeviceToHost, st);
+    if (err == cudaSuccess) err = cudaStreamSynchronize(st);
+    if (err != cudaSuccess) { set_error(std::string("stage-2 test forward failed: ") + cudaGetErrorString(err)); rc = -1; }
+  }
+  cudaStreamSynchronize(e->stream);
+  unet_release_owner(e->stage2, owner);
+  return rc;
+}
+
 // ---- diagnostics: one conv / transposed-conv layer in isolation (unit parity + profiling) -------
 // in0/in1: host fp32 NHWC [B][Hin][Win][C0|C1]; W: Chainer layout; out: host fp32 NHWC [B][Hout][Wout][Cout].
 // use_tc = 1 runs the FP16 wgmma kernel (activations rounded to fp16), 0 the FP32 CUDA-core kernel.

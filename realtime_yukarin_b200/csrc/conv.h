@@ -18,6 +18,10 @@ struct ConvLayer {
   int C0 = 0, C1 = 0, Cout = 0;           // Cin = C0 + C1
   int KH = 1, KW = 1, SH = 1, SW = 1, PH = 0, PW = 0;
   int act = ACT_NONE;
+  // Output row band: the layer computes only class-local output rows [band_y0, band_y1) of every batch item (transposed layers:
+  // output rows SH * band_y0 .. SH * band_y1 - 1).  The band is a range of whole tile rows (band_y1 may also be the last row);
+  // band_y1 == 0 means every row.  See unet_derive_bands.
+  int band_y0 = 0, band_y1 = 0;
   // device pointers
   const void* in0 = nullptr; const void* in1 = nullptr; int in_dtype = DT_F32;
   void* out = nullptr; int out_dtype = DT_F32;
@@ -29,13 +33,24 @@ struct ConvLayer {
   // tensor-core path (filled by tc_layer_prepare)
   const __half* w_tc = nullptr;           // conv: [Cout][KH*KW*Cin]; deconv: [4 classes][Cout][4*Cin]
   const __half* w_frag = nullptr;         // 1-D k4 layers: mma.sync B-fragment order for the fused stage-1 kernel (s1_map.h)
-  float* splitk_ws = nullptr;             // [pixels][Cout] fp32 when ksplit > 1
+  float* splitk_ws = nullptr;             // [ksplit][B][band's output rows][Wout][Cout] fp32 when ksplit > 1
   int ksplit = 1;
+  int ksplit_tiles = 0;                   // > 0: split K as for a layer of this many output tiles instead of the band's own count
   CUtensorMap tmA0, tmA1, tmB, tmO, tmW;     // inputs, weights, fp16 output, fp32 split-K workspace
   int tile_w = 0, tile_h = 0;             // pixel tile = tile_w x tile_h = 128
   int block_n = 0;
   bool tc_ready = false;
 };
+
+// class-local output rows of a layer (transposed convs run per output-parity class) and the end of its row band
+inline int layer_class_rows(const ConvLayer& L) { return L.transposed ? L.Hin : L.Hout; }
+inline int layer_band_end(const ConvLayer& L) { return L.band_y1 > 0 ? L.band_y1 : layer_class_rows(L); }
+// output rows [*r0, *r1) of one batch item that the band covers
+inline void layer_band_out_rows(const ConvLayer& L, int* r0, int* r1) {
+  const int s = L.transposed ? L.SH : 1;
+  *r0 = L.band_y0 * s;
+  *r1 = layer_band_end(L) * s < L.Hout ? layer_band_end(L) * s : L.Hout;
+}
 
 // Weight repacking from the Chainer layouts the model files use:
 //   conv   W: (Cout, Cin, KH, KW)      deconv W: (Cin, Cout, KH, KW)
@@ -43,12 +58,15 @@ int pack_weights_direct(const float* d_w_chainer, int transposed, int Cin, int C
 int pack_weights_tc(const float* d_w_chainer, int transposed, int Cin, int Cout, int KH, int KW, int SH, int SW, __half* d_out, cudaStream_t st);
 
 int conv_direct_run(const ConvLayer& L, cudaStream_t st);
+bool conv_direct_band_supported(const ConvLayer& L);
 
 bool tc_layer_eligible(const ConvLayer& L);
 int tc_init();                                           // resolves cuTensorMapEncodeTiled, sets smem attributes
 int tc_layer_prepare(ConvLayer& L, int num_sms);         // builds tensor maps, picks tiles / split-K (needs final pointers)
 int conv_tc_run(const ConvLayer& L, cudaStream_t st);
 size_t tc_splitk_ws_bytes(const ConvLayer& L, int num_sms);
+int tc_tile_rows(const ConvLayer& L);                    // class-local output rows per tile of the tensor-core kernel
+int tc_tile_count(const ConvLayer& L);                   // output tiles (all classes, all N blocks) of the layer's band
 
 // s1_fused.cu: the whole 1-D U-Net as one cluster kernel
 int s1_pack_weights(const float* d_w_chainer, int transposed, int Cin, int Cout, __half* d_out, cudaStream_t st);

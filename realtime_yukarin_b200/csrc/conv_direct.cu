@@ -216,12 +216,13 @@ __global__ void __launch_bounds__(256) k_conv3x3_cin1(const float* __restrict__ 
 // Cout = 1 from two fp16 sources of 64 channels each (skip concat) -> fp32.  One warp = 8 consecutive pixels of a row:
 // lanes 0-15 own 4 channels each of source 0, lanes 16-31 of source 1; the 3 x 10 input pixels are loaded once
 // (30 independent 8-byte loads in flight per lane) and feed all 8 outputs, which are then reduced across the warp.
+// Computes output rows y0 .. y0 + gridDim.y - 1.
 __global__ void __launch_bounds__(256) k_conv3x3_cout1_h(const __half* __restrict__ in0, const __half* __restrict__ in1,
                                                         const float* __restrict__ w /*[9][128][1]*/, float scale, float shift, int act,
-                                                        int B, int H, int W, float* __restrict__ out) {
+                                                        int B, int H, int W, int y0, float* __restrict__ out) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int x0 = (blockIdx.x * 8 + warp) * 8;          // 8 warps x 8 pixels = 64 pixels of a row per block
-  const int y = blockIdx.y, b = blockIdx.z;
+  const int y = y0 + blockIdx.y, b = blockIdx.z;
   if (x0 >= W) return;
   const __half* src = lane < 16 ? in0 : in1;
   const int c = (lane & 15) * 4;
@@ -317,7 +318,15 @@ __global__ void __launch_bounds__(256) k_conv1d_k3_small(const __half* __restric
 
 __global__ void k_read2(const float* a, const float* b, float* out) { out[0] = a[0]; out[1] = b[0]; }
 
+// the last stage-2 layer in FP16 plans (k_conv3x3_cout1_h), the one CUDA-core kernel that computes a row band
+bool conv_direct_band_supported(const ConvLayer& L) {
+  return !L.transposed && L.KH == 3 && L.KW == 3 && L.SH == 1 && L.SW == 1 && L.PH == 1 && L.PW == 1 && L.Cout == 1 && L.C0 == 64 &&
+         L.C1 == 64 && L.in_dtype == DT_F16 && L.out_dtype == DT_F32 && L.host_scale_valid;
+}
+
 int conv_direct_run(const ConvLayer& L, cudaStream_t st) {
+  const bool cout1_h = conv_direct_band_supported(L);
+  RYK_CHECK(cout1_h || (L.band_y0 == 0 && L.band_y1 == 0), "of the CUDA-core kernels only the Cout = 1 3x3 kernel computes a row band");
   // dedicated kernels for the stage-2 edge layers
   if (!L.transposed && L.KH == 3 && L.KW == 3 && L.SH == 1 && L.SW == 1 && L.PH == 1 && L.PW == 1) {
     if (L.C0 == 1 && L.C1 == 0 && L.in_dtype == DT_F32 && L.Cout % 8 == 0 && L.Cout <= 64) {
@@ -330,10 +339,10 @@ int conv_direct_run(const ConvLayer& L, cudaStream_t st) {
       RYK_CUDA(cudaGetLastError());
       return 0;
     }
-    if (L.Cout == 1 && L.C0 == 64 && L.C1 == 64 && L.in_dtype == DT_F16 && L.out_dtype == DT_F32 && L.host_scale_valid) {
-      dim3 blocks((L.Win + 63) / 64, L.Hin, L.B);
+    if (cout1_h) {
+      dim3 blocks((L.Win + 63) / 64, layer_band_end(L) - L.band_y0, L.B);       // the layer's row band
       k_conv3x3_cout1_h<<<blocks, 256, 0, st>>>((const __half*)L.in0, (const __half*)L.in1, L.w_direct, L.host_scale, L.host_shift, L.act,
-                                                L.B, L.Hin, L.Win, (float*)L.out);
+                                                L.B, L.Hin, L.Win, L.band_y0, (float*)L.out);
       RYK_CUDA(cudaGetLastError());
       return 0;
     }

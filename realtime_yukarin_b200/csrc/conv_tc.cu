@@ -30,7 +30,9 @@ namespace ryk {
 struct TcParams {
   int transposed, B, Hout, Wout, Cout;
   int Hc, Wc;                    // class-local output grid (== Hout, Wout for convs)
-  int tile_w, tile_h, tiles_w, tiles_h;
+  int tile_w, tile_h, tiles_w, tiles_h;  // tiles_h: tile rows of the band, which starts at tile row th0
+  int th0;
+  int ws_y0;                     // output row of the band's first row: row 0 of the split-K workspace
   int chunks0, chunks1;          // 64-channel chunks of source 0 / 1
   int taps_w, ntaps;             // taps per class: conv KH*KW (taps_w = KW); deconv (KH/SH)*(KW/SW)
   int sh, sw, ph, pw;            // conv stride / padding per dimension (1-D nets: sh = 1, ph = 0)
@@ -74,7 +76,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
   // tile coordinates
   int mt = blockIdx.x;
   const int tw = mt % p.tiles_w; mt /= p.tiles_w;
-  const int th = mt % p.tiles_h; mt /= p.tiles_h;
+  const int th = mt % p.tiles_h + p.th0; mt /= p.tiles_h;
   const int b = mt;
   const int n0 = blockIdx.y * BLOCK_N;
   const int cls = blockIdx.z / p.ksplit, split = blockIdx.z % p.ksplit;
@@ -192,7 +194,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
 #pragma unroll
           for (int jb = 0; jb < BLOCK_N / 32; ++jb)
             asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
-                         ::"l"(&tmW), "r"(smem_u32(smem + jb * (kBlockM * 128))), "r"(n0 + jb * 32), "r"(xs), "r"(ys), "r"(b), "r"(split) : "memory");
+                         ::"l"(&tmW), "r"(smem_u32(smem + jb * (kBlockM * 128))), "r"(n0 + jb * 32), "r"(xs), "r"(ys - p.ws_y0), "r"(b), "r"(split) : "memory");
         }
         asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
@@ -202,11 +204,13 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
 }
 
 // split-K reduce + epilogue: out = act((sum over splits of ws[s]) * scale + shift) as fp16, 4 channels per thread.
+// The workspace holds the layer's row band: band4 float4s per batch item, written to out at out_off4 + b * out_stride4 (float4 units).
 // Block = G warps x 32 lanes: lane = one float4 of the output (512 contiguous bytes per warp load), warp g sums the
 // slices g, g + G, g + 2G, ... ; the G partial sums are combined through shared memory in a fixed order, so the result
 // is deterministic (same summation tree every run) while G x more loads are in flight than with one thread per output.
 __global__ void __launch_bounds__(256) k_splitk_reduce(const float* __restrict__ ws, size_t total4, size_t slice_elems, int ksplit, int Cout,
-                                const float* __restrict__ scale, const float* __restrict__ shift, int act, __half* __restrict__ out) {
+                                const float* __restrict__ scale, const float* __restrict__ shift, int act, __half* __restrict__ out,
+                                size_t band4, size_t out_stride4, size_t out_off4) {
   __shared__ float4 part[8][32];
   pdl_trigger();
   pdl_wait();
@@ -226,7 +230,8 @@ __global__ void __launch_bounds__(256) k_splitk_reduce(const float* __restrict__
   __syncthreads();
   if (g != 0 || i >= total4) return;
   for (int k = 1; k < G; ++k) { const float4 b = part[k][lane]; a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w; }
-  const int n = (int)((i * 4) % Cout);
+  const size_t o = (i / band4) * out_stride4 + out_off4 + i % band4;
+  const int n = (int)((o * 4) % Cout);
   const float4 sc = __ldg(reinterpret_cast<const float4*>(scale + n)), sh = __ldg(reinterpret_cast<const float4*>(shift + n));
   float v[4] = {fmaf(a.x, sc.x, sh.x), fmaf(a.y, sc.y, sh.y), fmaf(a.z, sc.z, sh.z), fmaf(a.w, sc.w, sh.w)};
 #pragma unroll
@@ -234,12 +239,13 @@ __global__ void __launch_bounds__(256) k_splitk_reduce(const float* __restrict__
     if (act == ACT_LEAKY) v[j] = v[j] > 0.f ? v[j] : 0.2f * v[j]; else if (act == ACT_RELU) v[j] = fmaxf(v[j], 0.f);
   }
   __half2 h0 = __floats2half2_rn(v[0], v[1]), h1 = __floats2half2_rn(v[2], v[3]);
-  reinterpret_cast<uint2*>(out)[i] = make_uint2(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1));
+  reinterpret_cast<uint2*>(out)[o] = make_uint2(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1));
 }
 
 // few splits, large outputs (c3 / c4 / d3): one thread per float4 of the output, grid-stride, all slices summed in order
 __global__ void __launch_bounds__(256) k_splitk_reduce_few(const float* __restrict__ ws, size_t total4, size_t slice_elems, int ksplit, int Cout,
-                                    const float* __restrict__ scale, const float* __restrict__ shift, int act, __half* __restrict__ out) {
+                                    const float* __restrict__ scale, const float* __restrict__ shift, int act, __half* __restrict__ out,
+                                    size_t band4, size_t out_stride4, size_t out_off4) {
   const size_t stride4 = slice_elems / 4;
   pdl_trigger();
   pdl_wait();
@@ -251,7 +257,8 @@ __global__ void __launch_bounds__(256) k_splitk_reduce_few(const float* __restri
       const float4 b = __ldg(p + (size_t)s * stride4);
       a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
     }
-    const int n = (int)((i * 4) % Cout);
+    const size_t o = (i / band4) * out_stride4 + out_off4 + i % band4;
+    const int n = (int)((o * 4) % Cout);
     const float4 sc = __ldg(reinterpret_cast<const float4*>(scale + n)), sh = __ldg(reinterpret_cast<const float4*>(shift + n));
     float v[4] = {fmaf(a.x, sc.x, sh.x), fmaf(a.y, sc.y, sh.y), fmaf(a.z, sc.z, sh.z), fmaf(a.w, sc.w, sh.w)};
 #pragma unroll
@@ -259,7 +266,7 @@ __global__ void __launch_bounds__(256) k_splitk_reduce_few(const float* __restri
       if (act == ACT_LEAKY) v[j] = v[j] > 0.f ? v[j] : 0.2f * v[j]; else if (act == ACT_RELU) v[j] = fmaxf(v[j], 0.f);
     }
     __half2 h0 = __floats2half2_rn(v[0], v[1]), h1 = __floats2half2_rn(v[2], v[3]);
-    reinterpret_cast<uint2*>(out)[i] = make_uint2(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1));
+    reinterpret_cast<uint2*>(out)[o] = make_uint2(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1));
   }
 }
 
@@ -337,14 +344,31 @@ static int make_weight_map(CUtensorMap* m, const void* ptr, size_t K, size_t row
   return 0;
 }
 
+static void tc_tile_shape(const ConvLayer& L, int* tile_w, int* tile_h) {
+  const int Wc = L.transposed ? L.Win : L.Wout;
+  *tile_w = pow2_floor(Wc < kBlockM ? Wc : kBlockM);
+  *tile_h = kBlockM / *tile_w;
+}
+
+int tc_tile_rows(const ConvLayer& L) { int tw, th; tc_tile_shape(L, &tw, &th); return th; }
+
+int tc_tile_count(const ConvLayer& L) {
+  int tw, th;
+  tc_tile_shape(L, &tw, &th);
+  const int Wc = L.transposed ? L.Win : L.Wout;
+  const int band_tiles_h = (layer_band_end(L) - L.band_y0 + th - 1) / th;
+  const int bn = L.Cout >= 128 ? 128 : 64;
+  const int classes = L.transposed ? L.SH * L.SW : 1;
+  return L.B * ((Wc + tw - 1) / tw) * band_tiles_h * (L.Cout / bn) * classes;
+}
+
+// Tile shape, N block and split-K of a layer.  Split-K fills the SMs when the band has few tiles, so a banded layer may split
+// K further than the same layer over every row (L.ksplit_tiles overrides the tile count this rule sees).
 static void tc_geometry(const ConvLayer& L, int num_sms, int* tile_w, int* tile_h, int* block_n, int* ksplit) {
-  int Wc = L.transposed ? L.Win : L.Wout;
-  int Hc = L.transposed ? L.Hin : L.Hout;
-  int tw = pow2_floor(Wc < kBlockM ? Wc : kBlockM);
-  int th = kBlockM / tw;
+  int tw, th;
+  tc_tile_shape(L, &tw, &th);
   int bn = L.Cout >= 128 ? 128 : 64;
-  int classes = L.transposed ? L.SH * L.SW : 1;
-  int tiles = L.B * ((Wc + tw - 1) / tw) * ((Hc + th - 1) / th) * (L.Cout / bn) * classes;
+  int tiles = L.ksplit_tiles > 0 ? L.ksplit_tiles : tc_tile_count(L);
   int ntaps = L.transposed ? (L.KH / L.SH) * (L.KW / L.SW) : L.KH * L.KW;
   int total_chunks = ntaps * (L.C0 + L.C1) / kBlockK;
   int ks = 1;
@@ -363,7 +387,9 @@ static void tc_geometry(const ConvLayer& L, int num_sms, int* tile_w, int* tile_
 size_t tc_splitk_ws_bytes(const ConvLayer& L, int num_sms) {
   int tw, th, bn, ks;
   tc_geometry(L, num_sms, &tw, &th, &bn, &ks);
-  return ks > 1 ? (size_t)ks * L.B * L.Hout * L.Wout * L.Cout * sizeof(float) : 0;
+  int r0, r1;
+  layer_band_out_rows(L, &r0, &r1);
+  return ks > 1 ? (size_t)ks * L.B * (r1 - r0) * L.Wout * L.Cout * sizeof(float) : 0;
 }
 
 int tc_layer_prepare(ConvLayer& L, int num_sms) {
@@ -382,8 +408,13 @@ int tc_layer_prepare(ConvLayer& L, int num_sms) {
   // output map for the TMA-store epilogue: deconv classes write every other pixel (element strides = conv strides)
   if (make_act_map(&L.tmO, L.out, L.Cout, L.Wout, L.Hout, L.B, L.tile_w, L.tile_h, L.transposed ? L.SW : 1, L.transposed ? L.SH : 1)) return -1;
   RYK_CHECK(L.ksplit == 1 || L.splitk_ws != nullptr, "split-K layer without a workspace");
+  RYK_CHECK(L.band_y0 >= 0 && L.band_y0 % L.tile_h == 0 && L.band_y0 < layer_band_end(L) && layer_band_end(L) <= layer_class_rows(L) &&
+            (layer_band_end(L) % L.tile_h == 0 || layer_band_end(L) == layer_class_rows(L)), "row band is not a range of whole tile rows");
   if (L.ksplit > 1) {
-    if (make_ws_map(&L.tmW, L.splitk_ws, L.Cout, L.Wout, L.Hout, L.B, L.ksplit, L.tile_w, L.tile_h, L.transposed ? L.SW : 1, L.transposed ? L.SH : 1)) return -1;
+    // the workspace holds the band's output rows only
+    int r0, r1;
+    layer_band_out_rows(L, &r0, &r1);
+    if (make_ws_map(&L.tmW, L.splitk_ws, L.Cout, L.Wout, r1 - r0, L.B, L.ksplit, L.tile_w, L.tile_h, L.transposed ? L.SW : 1, L.transposed ? L.SH : 1)) return -1;
   } else L.tmW = L.tmO;
   L.tc_ready = true;
   return 0;
@@ -406,7 +437,12 @@ int conv_tc_run(const ConvLayer& L, cudaStream_t st) {
   p.transposed = L.transposed; p.B = L.B; p.Hout = L.Hout; p.Wout = L.Wout; p.Cout = L.Cout;
   p.Hc = L.transposed ? L.Hin : L.Hout; p.Wc = L.transposed ? L.Win : L.Wout;
   p.tile_w = L.tile_w; p.tile_h = L.tile_h;
-  p.tiles_w = (p.Wc + L.tile_w - 1) / L.tile_w; p.tiles_h = (p.Hc + L.tile_h - 1) / L.tile_h;
+  // the grid covers the band's tile rows of the layer's tile grid: every output pixel keeps its tile and so its K order
+  p.tiles_w = (p.Wc + L.tile_w - 1) / L.tile_w; p.tiles_h = (layer_band_end(L) - L.band_y0 + L.tile_h - 1) / L.tile_h;
+  p.th0 = L.band_y0 / L.tile_h;
+  int r0, r1;
+  layer_band_out_rows(L, &r0, &r1);
+  p.ws_y0 = r0;
   p.chunks0 = L.C0 / kBlockK; p.chunks1 = L.C1 / kBlockK;
   p.taps_w = L.transposed ? L.KW / L.SW : L.KW;
   p.ntaps = L.transposed ? (L.KH / L.SH) * (L.KW / L.SW) : L.KH * L.KW;
@@ -419,18 +455,21 @@ int conv_tc_run(const ConvLayer& L, cudaStream_t st) {
   p.act = L.act; p.scale = L.scale; p.shift = L.shift;
   p.ws = L.ksplit > 1 ? L.splitk_ws : nullptr;
   p.out_pixels = (size_t)L.B * L.Hout * L.Wout;
-  size_t out_elems = (size_t)L.B * L.Hout * L.Wout * L.Cout;
+  const size_t row_elems = (size_t)L.Wout * L.Cout;
+  const size_t band_elems = (size_t)L.B * (r1 - r0) * row_elems;      // one workspace slice
   dim3 grid(L.B * p.tiles_w * p.tiles_h, L.Cout / L.block_n, classes * L.ksplit);
   if (L.block_n == 128) RYK_CUDA(launch_pdl(RYK_TC_N128, grid, dim3(kTcThreads), tc_smem_bytes<128, 3>(), st, L.tmA0, L.tmA1, L.tmB, L.tmO, L.tmW, p));
   else RYK_CUDA(launch_pdl(RYK_TC_N64, grid, dim3(kTcThreads), tc_smem_bytes<64, 4>(), st, L.tmA0, L.tmA1, L.tmB, L.tmO, L.tmW, p));
   RYK_CUDA(cudaGetLastError());
   if (p.ws) {
-    size_t total4 = out_elems / 4;
+    const size_t total4 = band_elems / 4, band4 = (r1 - r0) * row_elems / 4, stride4 = L.Hout * row_elems / 4, off4 = r0 * row_elems / 4;
     if (L.ksplit <= 4) {
       int blocks = (int)((total4 + 255) / 256); if (blocks > 2112) blocks = 2112;     // 16 per SM of 132
-      RYK_CUDA(launch_pdl(k_splitk_reduce_few, dim3(blocks), dim3(256), 0, st, (const float*)p.ws, total4, out_elems, L.ksplit, L.Cout, L.scale, L.shift, L.act, (__half*)L.out));
+      RYK_CUDA(launch_pdl(k_splitk_reduce_few, dim3(blocks), dim3(256), 0, st, (const float*)p.ws, total4, band_elems, L.ksplit, L.Cout, L.scale, L.shift, L.act,
+                          (__half*)L.out, band4, stride4, off4));
     } else {
-      RYK_CUDA(launch_pdl(k_splitk_reduce, dim3((unsigned)((total4 + 31) / 32)), dim3(256), 0, st, (const float*)p.ws, total4, out_elems, L.ksplit, L.Cout, L.scale, L.shift, L.act, (__half*)L.out));
+      RYK_CUDA(launch_pdl(k_splitk_reduce, dim3((unsigned)((total4 + 31) / 32)), dim3(256), 0, st, (const float*)p.ws, total4, band_elems, L.ksplit, L.Cout, L.scale, L.shift, L.act,
+                          (__half*)L.out, band4, stride4, off4));
     }
     RYK_CUDA(cudaGetLastError());
   }

@@ -245,8 +245,8 @@ __global__ void k_sr_prologue(const float* __restrict__ sp, const float* __restr
   x[(size_t)t * (nb - 1) + k] = logf(v);
 }
 
-__global__ void k_sr_epilogue(const float* __restrict__ y, int T, int nb, float* __restrict__ sp_out) {
-  int t = blockIdx.y;
+__global__ void k_sr_epilogue(const float* __restrict__ y, int T, int nb, int t0, float* __restrict__ sp_out) {
+  int t = t0 + blockIdx.y;
   int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= T || k >= nb) return;
   int ks = k < nb - 1 ? k : nb - 2;
@@ -286,9 +286,11 @@ int sr_prologue_run(Engine* e, const float* d_sp, int T, int Tp, int nb, float* 
   return 0;
 }
 
-int sr_epilogue_run(Engine* e, const float* d_y, int T, int nb, float* d_sp_out, cudaStream_t st) {
-  if (T <= 0) return 0;
-  k_sr_epilogue<<<dim3((nb + 127) / 128, T), 128, 0, st>>>(d_y, T, nb, d_sp_out);
+int sr_epilogue_run(Engine* e, const float* d_y, int T, int nb, float* d_sp_out, cudaStream_t st, int t0, int t1) {
+  if (t1 < 0) t1 = T;
+  RYK_CHECK(0 <= t0 && t0 <= t1 && t1 <= T, "stage-2 epilogue rows out of range");
+  if (t1 == t0) return 0;
+  k_sr_epilogue<<<dim3((nb + 127) / 128, t1 - t0), 128, 0, st>>>(d_y, T, nb, t0, d_sp_out);
   RYK_CUDA(cudaGetLastError());
   e->launches++;
   return 0;

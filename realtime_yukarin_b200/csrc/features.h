@@ -12,7 +12,8 @@ int stage1_epilogue_run(Engine* e, const float* d_y, const int* d_index, const u
                         float* d_mc_out, float* d_f0_out, float* d_ap_out, uint8_t* d_voiced_out, cudaStream_t st);
 constexpr int kColminFloats = 64 * 512;      // column-minimum partials of the stage-2 prologue (one scratch per concurrent stream)
 int sr_prologue_run(Engine* e, const float* d_sp, int T, int Tp, int nb, float* d_x, cudaStream_t st, float* d_colmin = nullptr);
-int sr_epilogue_run(Engine* e, const float* d_y, int T, int nb, float* d_sp_out, cudaStream_t st);
+// frames [t0, t1) of the T-frame window (t1 < 0: T); the other rows of d_sp_out are not written
+int sr_epilogue_run(Engine* e, const float* d_y, int T, int nb, float* d_sp_out, cudaStream_t st, int t0 = 0, int t1 = -1);
 
 constexpr float kSilentMc0 = -18.420680743952367f;   // ln(1e-8): silent template mel-cepstrum c0 (DESIGN.md, DECIDE)
 

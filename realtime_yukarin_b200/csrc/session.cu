@@ -441,8 +441,10 @@ static int stage1_body(Engine* e, Session* s, int b, int tp1) {
 
 // stage 2 of a single session alternates its stream (and plan) by chunk parity; a group member always uses the first stream
 static cudaStream_t s2_stream(const Session* s, int b) { return s->sC2s[s->group ? 0 : b]; }
+// The decode slide reads only the chunk's frames [e_conv, e_conv + n_feat) of the converted window, so stage 2 computes only the
+// decoder rows those frames depend on.
 static int s2_plan(Engine* e, const Session* s, int b, UNetPlan** p2) {
-  return unet_get_plan(e, e->stage2, 1, s->Tp, 512, e->precision, p2, s->s2_owner[b]);
+  return unet_get_plan(e, e->stage2, 1, s->Tp, 512, e->precision, p2, s->s2_owner[b], s->e_conv, s->n_feat);
 }
 
 // begin (which = 0) / end (1) of a stage in the RYK_STAGE_TIMES timeline
@@ -568,13 +570,13 @@ static int session_back(Engine* e, Session* s) {
     Group* G = s->group;
     RYK_CUDA(cudaStreamWaitEvent(sC2, G->ev_fwd[G->step % kRing], 0));
     const float* src = (const float*)G->p2->d_out + (size_t)s->slot * s->Tp * 512;
-    if (run_graph(e, pg.s2_epi, sC2, [&]() -> int { return sr_epilogue_run(e, src, s->Tw, s->nb, s->cv_sp_out[b], sC2); })) return -1;
+    if (run_graph(e, pg.s2_epi, sC2, [&]() -> int { return sr_epilogue_run(e, src, s->Tw, s->nb, s->cv_sp_out[b], sC2, pc, pc + s->n_feat); })) return -1;
   } else {
     UNetPlan* p2 = nullptr;
     if (s2_plan(e, s, b, &p2)) return -1;
     if (run_graph(e, pg.s2_epi, sC2, [&]() -> int {
           if (unet_forward(e, p2, sC2, 15, 15)) return -1;
-          return sr_epilogue_run(e, (const float*)p2->d_out, s->Tw, s->nb, s->cv_sp_out[b], sC2);
+          return sr_epilogue_run(e, (const float*)p2->d_out, s->Tw, s->nb, s->cv_sp_out[b], sC2, pc, pc + s->n_feat);
         })) return -1;
   }
   if (stage_time(s, 3, 1, r, sC2)) return -1;
@@ -909,7 +911,15 @@ int ryk_group_create(ryk_engine* h, const int* session_ids, int n_sessions, int*
     s->group = G; s->slot = i;
     G->members.push_back(s);
   }
-  if (unet_get_plan(e, e->stage2, n_sessions, G->members[0]->Tp, 512, e->precision, &G->p2, G->owner)) { group_free(G); return -1; }
+  // the batched forward computes the decoder rows of the hull of the members' kept frames (their e_conv may differ)
+  std::vector<int> kb, kl;
+  for (Session* m : G->members) { kb.push_back(m->e_conv); kl.push_back(m->n_feat); }
+  int keep_begin = 0, keep_len = 0;
+  keep_hull(n_sessions, kb.data(), kl.data(), &keep_begin, &keep_len);
+  if (unet_get_plan(e, e->stage2, n_sessions, G->members[0]->Tp, 512, e->precision, &G->p2, G->owner, keep_begin, keep_len)) {
+    group_free(G);
+    return -1;
+  }
   { int lo = 0, hi = 0; RYK_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi)); RYK_CUDA(cudaStreamCreateWithPriority(&G->sG, cudaStreamNonBlocking, lo)); }
   for (int i = 0; i < kRing; ++i) RYK_CUDA(cudaEventCreateWithFlags(&G->ev_fwd[i], cudaEventDisableTiming));
   RYK_CUDA(cudaDeviceSynchronize());

@@ -5,6 +5,7 @@
 // Topology (both): enc c0 = conv k3 s1 p1 + LeakyReLU(0.2); enc c1..c7 = conv k4 s2 p1 + BN + LeakyReLU;
 // dec c0..c6 = deconv k4 s2 p1 + BN + ReLU with skip concat (by pointer) before c1..c7;
 // dec c7 = conv k3 s1 p1.  BatchNorm (eval, eps 2e-5) and biases arrive folded into scale/shift.
+#include <algorithm>
 #include <vector>
 
 #include "conv.h"
@@ -98,10 +99,67 @@ int unet_set_layer(Engine* e, UNet* n, int idx, const float* W, const float* sca
   return 0;
 }
 
+void unet_layer_shape(const UNet* n, int i, int B, int H, int W, ConvLayer& L) {
+  const UNetLayerW& LW = n->layers[i];
+  auto lvlH = [&](int l) { return n->ndim == 2 ? H >> l : 1; };
+  auto lvlW = [&](int l) { return W >> l; };
+  L.transposed = LW.transposed; L.B = B; L.Cout = LW.cout; L.act = LW.act;
+  L.KH = n->ndim == 2 ? LW.k : 1; L.KW = LW.k;
+  L.SH = n->ndim == 2 ? LW.s : 1; L.SW = LW.s;
+  L.PH = n->ndim == 2 ? LW.p : 0; L.PW = LW.p;
+  if (i == 0) {
+    L.Hin = lvlH(0); L.Win = lvlW(0); L.Hout = lvlH(0); L.Wout = lvlW(0); L.C0 = n->in_ch; L.C1 = 0;
+  } else if (i < 8) {
+    L.Hin = lvlH(i - 1); L.Win = lvlW(i - 1); L.Hout = lvlH(i); L.Wout = lvlW(i); L.C0 = LW.cin; L.C1 = 0;
+  } else if (i < 15) {
+    int d = i - 8;
+    L.Hin = lvlH(7 - d); L.Win = lvlW(7 - d); L.Hout = lvlH(6 - d); L.Wout = lvlW(6 - d);
+    if (d == 0) { L.C0 = LW.cin; L.C1 = 0; }
+    else { L.C0 = dec_out_channels(n->base, d - 1); L.C1 = level_channels(n->base, 7 - d); }
+  } else {
+    L.Hin = lvlH(0); L.Win = lvlW(0); L.Hout = lvlH(0); L.Wout = lvlW(0); L.C0 = n->base; L.C1 = n->base;
+  }
+}
+
+// Walks back from the last layer.  Layer i must produce output rows [lo, hi); its band is the class-local rows those come from
+// (transposed k4 s2 p1: output row 2m + py is class-local row m), rounded out to whole tile rows of the kernel that runs the layer
+// (the tensor-core tile grid; one row for the 3x3 CUDA-core layer).  The rows the next layer down must produce are then the input
+// rows the ROUNDED band reads, so every row that a computed tile reads has itself been computed.  Tiles keep their place in the
+// layer's tile grid, so each computed pixel is summed exactly as in the full layer (same tile, same K order).
+void unet_derive_bands(std::vector<ConvLayer>& layers, int keep_begin, int keep_len) {
+  int lo = keep_begin, hi = keep_begin + keep_len;
+  for (int i = 15; i >= 8; --i) {
+    ConvLayer& L = layers[i];
+    const int rows = layer_class_rows(L);
+    const int th = L.transposed ? tc_tile_rows(L) : 1;
+    const int m0 = L.transposed ? lo / L.SH : lo, m1 = L.transposed ? (hi - 1) / L.SH + 1 : hi;
+    const int y0 = m0 / th * th, y1 = std::min(rows, (m1 + th - 1) / th * th);
+    if (y0 == 0 && y1 == rows) { L.band_y0 = 0; L.band_y1 = 0; }
+    else { L.band_y0 = y0; L.band_y1 = y1; }
+    if (L.transposed) {   // class-local row m of parity py reads input rows m - 1 + py + ty, ty in {0, 1} (k4 s2 p1); m (k1 s1 p0)
+      lo = L.SH == 2 ? y0 - 1 : y0;
+      hi = L.SH == 2 ? y1 + 1 : y1;
+    } else {
+      lo = y0 * L.SH - L.PH;
+      hi = (y1 - 1) * L.SH - L.PH + L.KH;
+    }
+    lo = std::max(lo, 0); hi = std::min(hi, L.Hin);
+  }
+}
+
+void keep_hull(int n, const int* begins, const int* lens, int* begin, int* len) {
+  int lo = begins[0], hi = begins[0] + lens[0];
+  for (int i = 1; i < n; ++i) { lo = std::min(lo, begins[i]); hi = std::max(hi, begins[i] + lens[i]); }
+  *begin = lo; *len = hi - lo;
+}
+
 // Plan for a (batch, H, W) input; H = 1 for 1-D nets. precision: 0 = FP32 everywhere, 1 = FP16 activations + wgmma.
-int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPlan** out, int owner) {
+int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPlan** out, int owner, int keep_begin, int keep_len,
+                  bool full_ksplit) {
   for (auto& L : n->layers) RYK_CHECK(L.loaded, "U-Net layer weights not loaded");
-  auto key = std::make_tuple(B, H, W, precision, owner);
+  if (keep_len > 0) RYK_CHECK(keep_begin >= 0 && keep_begin + keep_len <= H, "kept rows outside the U-Net input");
+  if (keep_len <= 0 || (keep_begin == 0 && keep_len == H)) { keep_begin = 0; keep_len = 0; full_ksplit = false; }
+  auto key = std::make_tuple(B, H, W, precision, owner, keep_begin, keep_len, full_ksplit ? 1 : 0);
   auto it = n->plans.find(key);
   if (it != n->plans.end()) { *out = it->second; return 0; }
   RYK_CHECK(W % 128 == 0 && (n->ndim == 1 || H % 128 == 0), "U-Net input extent must be a multiple of 128");
@@ -117,6 +175,7 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
     RYK_CUDA(cudaMalloc(ptr, bytes));
     RYK_CUDA(cudaMemsetAsync(*ptr, 0, bytes, e->stream));
     p->buffers.push_back(*ptr);
+    p->buffer_bytes.push_back(bytes);
     return 0;
   };
   void* enc[8]; void* dec[7];
@@ -130,33 +189,49 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
   for (int i = 0; i < 16; ++i) {
     const UNetLayerW& LW = n->layers[i];
     ConvLayer& L = p->layers[i];
-    L.transposed = LW.transposed; L.B = B; L.Cout = LW.cout; L.act = LW.act;
-    L.KH = n->ndim == 2 ? LW.k : 1; L.KW = LW.k;
-    L.SH = n->ndim == 2 ? LW.s : 1; L.SW = LW.s;
-    L.PH = n->ndim == 2 ? LW.p : 0; L.PW = LW.p;
+    unet_layer_shape(n, i, B, H, W, L);
     L.w_direct = LW.d_w_direct; L.w_tc = LW.d_w_tc; L.w_frag = LW.d_w_frag; L.scale = LW.d_scale; L.shift = LW.d_shift;
     L.host_scale_valid = true; L.host_scale = LW.h_scale0; L.host_shift = LW.h_shift0;
     L.in_dtype = act_dt; L.out_dtype = act_dt;
     if (i == 0) {
-      L.Hin = lvlH(0); L.Win = lvlW(0); L.Hout = lvlH(0); L.Wout = lvlW(0);
-      L.C0 = n->in_ch; L.C1 = 0; L.in0 = p->d_in; L.in_dtype = DT_F32; L.out = enc[0];
+      L.in0 = p->d_in; L.in_dtype = DT_F32; L.out = enc[0];
     } else if (i < 8) {
-      L.Hin = lvlH(i - 1); L.Win = lvlW(i - 1); L.Hout = lvlH(i); L.Wout = lvlW(i);
-      L.C0 = LW.cin; L.C1 = 0; L.in0 = enc[i - 1]; L.out = enc[i];
+      L.in0 = enc[i - 1]; L.out = enc[i];
     } else if (i < 15) {
       int d = i - 8;
-      L.Hin = lvlH(7 - d); L.Win = lvlW(7 - d); L.Hout = lvlH(6 - d); L.Wout = lvlW(6 - d);
-      if (d == 0) { L.C0 = LW.cin; L.C1 = 0; L.in0 = enc[7]; }
-      else { L.C0 = dec_out_channels(n->base, d - 1); L.C1 = level_channels(n->base, 7 - d); L.in0 = dec[d - 1]; L.in1 = enc[7 - d]; }
+      if (d == 0) L.in0 = enc[7];
+      else { L.in0 = dec[d - 1]; L.in1 = enc[7 - d]; }
       L.out = dec[d];
     } else {
-      L.Hin = lvlH(0); L.Win = lvlW(0); L.Hout = lvlH(0); L.Wout = lvlW(0);
-      L.C0 = n->base; L.C1 = n->base; L.in0 = dec[6]; L.in1 = enc[0]; L.out = p->d_out; L.out_dtype = DT_F32;
+      L.in0 = dec[6]; L.in1 = enc[0]; L.out = p->d_out; L.out_dtype = DT_F32;
     }
     L.tc_ready = false;
+  }
+  // The decoder computes a row band only where every layer of it runs on a kernel that supports one.
+  bool bandable = keep_len > 0 && n->ndim == 2 && precision == 1 && conv_direct_band_supported(p->layers[15]);
+  for (int i = 8; i < 15; ++i) bandable = bandable && p->layers[i].w_tc && tc_layer_eligible(p->layers[i]);
+  if (bandable) {
+    p->keep_begin = keep_begin; p->keep_len = keep_len;
+    unet_derive_bands(p->layers, keep_begin, keep_len);
+    if (full_ksplit)
+      for (int i = 8; i < 15; ++i) {
+        ConvLayer full = p->layers[i];
+        full.band_y0 = full.band_y1 = 0;
+        p->layers[i].ksplit_tiles = tc_tile_count(full);
+      }
+  }
+  // One split-K workspace serves every layer of the plan: the layers run in stream order, and a layer's conv kernel writes the
+  // workspace only after its programmatic-launch wait, i.e. after the previous layer's reduce kernel has finished reading it.
+  size_t ws_bytes = 0;
+  for (int i = 0; i < 16; ++i)
+    if (precision == 1 && p->layers[i].w_tc && tc_layer_eligible(p->layers[i]))
+      ws_bytes = std::max(ws_bytes, tc_splitk_ws_bytes(p->layers[i], num_sms));
+  void* ws = nullptr;
+  if (ws_bytes && alloc(ws_bytes, &ws)) return -1;
+  for (int i = 0; i < 16; ++i) {
+    ConvLayer& L = p->layers[i];
     if (precision == 1 && L.w_tc && tc_layer_eligible(L)) {
-      size_t ws = tc_splitk_ws_bytes(L, num_sms);
-      if (ws) { void* w = nullptr; if (alloc(ws, &w)) return -1; L.splitk_ws = (float*)w; }
+      if (tc_splitk_ws_bytes(L, num_sms)) L.splitk_ws = (float*)ws;
       if (tc_layer_prepare(L, num_sms)) return -1;
     }
   }

@@ -23,8 +23,10 @@ struct UNetLayerW {
 
 struct UNetPlan {
   int B = 1, H = 1, W = 0, precision = 0;
+  int keep_begin = 0, keep_len = 0;   // output rows of every batch item the plan computes (keep_len == 0: all); see unet_derive_bands
   std::vector<ConvLayer> layers;
   std::vector<void*> buffers;
+  std::vector<size_t> buffer_bytes;
   void* d_in = nullptr;     // fp32 NHWC input  [B][H][W][in_ch]
   void* d_out = nullptr;    // fp32 NHWC output [B][H][W][out_ch]
   bool fused = false;       // 1-D FP16 plan that s1_fused.cu can run as one launch
@@ -33,7 +35,8 @@ struct UNetPlan {
 struct UNet {
   int ndim = 2, in_ch = 1, out_ch = 1, base = 64;
   std::vector<UNetLayerW> layers;                                  // 0..7 encoder, 8..15 decoder
-  std::map<std::tuple<int, int, int, int, int>, UNetPlan*> plans;  // (B, H, W, precision, owner)
+  // (B, H, W, precision, owner, keep_begin, keep_len, ksplit as for full layers)
+  std::map<std::tuple<int, int, int, int, int, int, int, int>, UNetPlan*> plans;
 };
 
 UNet* unet_create(int ndim, int in_ch, int out_ch, int base);
@@ -41,8 +44,20 @@ void unet_destroy(UNet* n);
 int unet_set_layer(Engine* e, UNet* n, int idx, const float* W, const float* scale, const float* shift);
 // owner: 0 = the engine's shared plans (per-op host API, serialised on the engine stream); every session / group passes its own
 // id so that concurrently running streams never share activation buffers.
-int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPlan** out, int owner = 0);
+// keep_len > 0 (2-D FP16 plans): the caller reads only output rows [keep_begin, keep_begin + keep_len) of every batch item, and
+// the decoder computes only the row bands those rows depend on (unet_derive_bands); the other rows of d_out are not written.
+// full_ksplit: each banded layer splits K as it would over every row (tests: bitwise comparison with the full plan).
+int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPlan** out, int owner = 0, int keep_begin = 0,
+                  int keep_len = 0, bool full_ksplit = false);
 void unet_release_owner(UNet* n, int owner);
+// Fill the geometry of layer i of net n for a (B, H, W) input (shapes, kernel, stride, padding, channels; no pointers).
+void unet_layer_shape(const UNet* n, int i, int B, int H, int W, ConvLayer& L);
+// Row bands of the 2-D decoder (layers 8..15) for a caller that reads output rows [keep_begin, keep_begin + keep_len): writes
+// band_y0 / band_y1 of those layers, rounded out to each layer's tile rows.  Layers 0..7 and every layer whose band covers all its
+// rows stay full.
+void unet_derive_bands(std::vector<ConvLayer>& layers, int keep_begin, int keep_len);
+// smallest row range [*begin, *begin + *len) that holds the n ranges [begins[i], begins[i] + lens[i])
+void keep_hull(int n, const int* begins, const int* lens, int* begin, int* len);
 int unet_forward(Engine* e, UNetPlan* p, cudaStream_t st, int first_layer = 0, int last_layer = 15);
 // s1_fused.cu
 bool s1_fused_eligible(const UNet* n, const UNetPlan* p);

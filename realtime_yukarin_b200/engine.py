@@ -58,8 +58,18 @@ EXPORTED_SYMBOLS = [
     'ryk_resample_poly', 'ryk_session_poll', 'ryk_reblock_poll', 'ryk_engine_profile_read2', 'ryk_engine_set_stage1_fused',
     'ryk_engine_set_f0_method', 'ryk_engine_get_f0_method', 'ryk_debug_harvest',
     'ryk_crepe_create', 'ryk_crepe_set_conv', 'ryk_crepe_set_dense', 'ryk_crepe_set_decoder_tables', 'ryk_crepe_num_frames', 'ryk_crepe_predict',
-    'ryk_crepe_set_resampler', 'ryk_crepe_test_conv', 'ryk_crepe_test_network',
+    'ryk_crepe_set_resampler', 'ryk_crepe_test_conv', 'ryk_crepe_test_network', 'ryk_stage2_row_bands', 'ryk_test_stage2_forward',
 ]
+
+
+def stage2_row_bands(Tp: int, W: int, keep_begin: int, keep_len: int) -> numpy.ndarray:
+    """[16][2] class-local output rows [y0, y1) that each stage-2 layer computes when rows [keep_begin, keep_begin + keep_len) are
+    kept (host only, no device needed)."""
+    lib = load_library()
+    out = numpy.zeros((16, 2), numpy.int32)
+    if lib.ryk_stage2_row_bands(int(Tp), int(W), int(keep_begin), int(keep_len), out.ctypes.data_as(c_int_p)) < 0:
+        raise RykError(lib.ryk_last_error().decode('utf-8', 'replace'))
+    return out
 
 
 def load_library() -> ctypes.CDLL:
@@ -423,6 +433,19 @@ class Engine(object):
             self._h, int(transposed), int(k), int(stride), int(pad), B, H, Wd, C0, C1, cout, _fp(in0), _fp(in1a), _fp(W),
             _fp(scale), _fp(shift), int(act), int(use_tc), int(repeat), _fp(out), ctypes.byref(ms)))
         return out, ms.value
+
+    def test_stage2_forward(self, x, keep=(), mode=0):
+        """One stage-2 forward on NaN-filled buffers (ryk_test_stage2_forward); x [B][Tp][512] float32, keep = [(begin, len), ...].
+        Returns y [B][Tp][512]; rows the plan does not compute stay NaN."""
+        x = _f32(x)
+        B, Tp, W = x.shape
+        assert W == 512
+        kb = numpy.array([k[0] for k in keep] or [0], numpy.int32)
+        kl = numpy.array([k[1] for k in keep] or [0], numpy.int32)
+        y = numpy.empty_like(x)
+        self._check(self.lib.ryk_test_stage2_forward(self._h, B, Tp, len(keep), kb.ctypes.data_as(c_int_p), kl.ctypes.data_as(c_int_p),
+                                                     int(mode), _fp(x), _fp(y)))
+        return y
 
     # ---- sessions ----
     def session_create(self, cfg: SessionConfig) -> int:
