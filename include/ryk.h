@@ -222,6 +222,22 @@ int ryk_session_poll(ryk_engine* e, int session_id, long long ticket, int* done)
 int ryk_session_push_device(ryk_engine* e, int session_id, const float* wave_dev, int n, double* out_dev, int out_capacity,
                             int* n_out_dev);
 
+/* Device rates.  A session analyses, converts and synthesises at cfg.fs; it may also take its chunks at a sound card's input rate and
+ * return its samples at the card's output rate, resampling on the GPU inside its captured stages (no host synchronisation).
+ * `taps` is the odd-length low-pass filter of ryk_resample_poly (realtime_yukarin_b200/wave_io.py: resample_filter(up, down)), up / down
+ * the coprime ratio of the resampler's output rate to its input rate: fs / rate on the input side, rate / fs on the output side.
+ * rate == fs leaves that side without a resampler.  Valid only on a fresh session (no chunk pushed, not in a group); each side once.
+ * Input:  a chunk is n_in = round(rate * buffer_time) samples, and n_in * up must equal round(fs * buffer_time) * down.  Step k
+ *         analyses samples [k n, (k + 1) n) of zeros(delay_in) followed by resample_poly(all chunks so far), n = round(fs * buffer_time).
+ * Output: after step k the session has returned resample_poly(y)[:M_k], y = the synthesizer's samples of steps 0..k (N_k of them) and
+ *         M_k = the outputs whose filter support lies inside [0, N_k); a step returns M_k - M_{k-1} samples, at most max_out.
+ * ryk_session_io_geometry: n_in = samples per pushed chunk, max_out = the most samples one step returns (out_capacity of
+ * ryk_session_push_device, max_in of an attached re-blocker), delay_in = the input delay in model-rate samples, in_rate / out_rate =
+ * the device rates (fs when unset).  Any output pointer may be NULL.  Groups need members with the same device rates. */
+int ryk_session_set_input_rate(ryk_engine* e, int session_id, int rate, int up, int down, const double* taps, int n_taps);
+int ryk_session_set_output_rate(ryk_engine* e, int session_id, int rate, int up, int down, const double* taps, int n_taps);
+int ryk_session_io_geometry(ryk_engine* e, int session_id, int* n_in, int* max_out, int* delay_in, int* in_rate, int* out_rate);
+
 /* Diagnostics: device timeline (ms) of the last <= 8 steps x 5 stages {gate, analysis, stage 1, stage 2, synthesis}; needs
  * RYK_STAGE_TIMES=1 in the environment at session creation.  start/end hold 40 floats; returns the number of steps. */
 int ryk_session_stage_times(ryk_engine* e, int session_id, float* start, float* end);

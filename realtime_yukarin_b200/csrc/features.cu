@@ -298,32 +298,102 @@ int sr_epilogue_run(Engine* e, const float* d_y, int T, int nb, float* d_sp_out,
 
 // ------------------------------------------------------------------------------------ polyphase resampler
 // SURVEY 8(f) rank 3 (check.py:80 librosa.load(..., sr=input_rate)): scipy.signal.resample_poly's upfirdn step on the device.
-//   y[i] = sum over j of x[j] * h[(i + n_pre_remove) * down - j * up - n_pre_pad],  0 <= tap index < n_taps, x zero outside [0, n)
-// One thread per output sample, FP64 accumulation over the ~n_taps / up taps that hit an input sample (ascending j).
-__global__ void __launch_bounds__(256) k_resample_poly(const float* __restrict__ x, int n, int up, int down, const double* __restrict__ h, int n_taps,
-                                                      int n_pre_pad, int n_pre_remove, float* __restrict__ y, int n_out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_out) return;
-  const long long t = (long long)(i + n_pre_remove) * down - n_pre_pad;       // tap index of x[0]
-  // tap = t - j * up in [0, n_taps)  <=>  (t - n_taps + 1) / up <= j <= t / up
-  long long jlo = t - (n_taps - 1);
-  jlo = jlo <= 0 ? 0 : (jlo + up - 1) / up;
-  long long jhi = t < 0 ? -1 : t / up;
-  if (jhi > n - 1) jhi = n - 1;
-  double acc = 0.0;
-  for (long long j = jlo; j <= jhi; ++j) acc += (double)x[j] * h[t - j * up];
-  y[i] = (float)acc;
+//   y[i] = sum over j of x[j] * h[(i + n_pre_remove) * down - j * up - n_pre_pad] = sum over j of x[j] * h[half_len + i * down - j * up],
+//   0 <= tap index < n_taps, x zero outside [0, in_end)
+// One thread per output sample, FP64 accumulation over the ~n_taps / up taps that hit an input sample (ascending j).  i and j are
+// global indices of the whole signal, so the whole-signal call and the two streaming sides of a session sum the same terms in the
+// same order: streamed output is bitwise the whole-signal output.
+//   whole:      x = the whole signal (x_len samples), outputs 0 .. n_out-1.
+//   stream in:  a fixed chunk of `chunk` samples per step; x = the history window ending at the newest sample (x_len samples, slid by
+//               the caller).  Outputs out_end - delay .. + n_out - 1 of the resampled signal; those with a negative index are the
+//               leading zeros of the delay.
+//   stream out: *n_new new samples per step in x_new; x = the x_len samples before them (the kept history).  Emits the outputs not
+//               yet emitted whose filter support ends inside the samples received so far (at most n_out of them), writes their count
+//               to *n_out_dev and the history for the next step to hist_next.
+// Streaming positions are read from *st and the next step's written to *st_next (double-buffered by the caller), so no host value
+// changes from step to step and the launch can sit in a captured graph.
+template <typename Tin, typename Tout>
+__global__ void __launch_bounds__(256) k_resample_poly(PolyArgs<Tin, Tout> a) {
+  const int half_len = (a.n_taps - 1) / 2;
+  long long in_end, x_first, new_first, out_first;
+  int n_out = a.n_out;
+  if (a.mode == kPolyWhole) {
+    in_end = a.x_len; x_first = 0; new_first = in_end; out_first = 0;
+  } else {
+    const ResampleState s = *a.st;
+    if (a.mode == kPolyStreamIn) {
+      in_end = s.in_end + a.chunk; x_first = in_end - a.x_len; new_first = in_end; out_first = s.out_end - a.delay;
+    } else {
+      const int n_new = *a.n_new > 0 ? *a.n_new : 0;
+      in_end = s.in_end + n_new; x_first = s.in_end - a.x_len; new_first = s.in_end; out_first = s.out_end;
+      // outputs 0 .. m-1 have their whole support in [0, in_end): half_len + i * down - j * up <= n_taps - 1 for j = in_end - 1
+      const long long num = in_end * a.up - 1 - half_len;
+      const long long m = (num >= 0 ? num / a.down : -((-num + a.down - 1) / a.down)) + 1;
+      const long long avail = m - s.out_end;
+      n_out = avail <= 0 ? 0 : (avail < n_out ? (int)avail : n_out);
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+      a.st_next->in_end = in_end;
+      a.st_next->out_end = s.out_end + n_out;
+      if (a.n_out_dev) *a.n_out_dev = n_out;
+    }
+  }
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  auto sample = [&](long long j) -> Tin { return j < new_first ? a.x[j - x_first] : a.x_new[j - new_first]; };
+  if (t < n_out) {
+    const long long i = out_first + t;
+    double acc = 0.0;
+    if (i >= 0) {
+      const long long c = i * a.down + half_len;                       // tap index of input sample 0
+      // tap = c - j * up in [0, n_taps)  <=>  (c - n_taps + 1) / up <= j <= c / up
+      long long jlo = c - (a.n_taps - 1);
+      jlo = jlo <= 0 ? 0 : (jlo + a.up - 1) / a.up;
+      long long jhi = c / a.up;
+      if (jlo < x_first) jlo = x_first;
+      if (jhi > in_end - 1) jhi = in_end - 1;
+      for (long long j = jlo; j <= jhi; ++j) acc += (double)sample(j) * a.h[c - j * a.up];
+    }
+    a.y[t] = (Tout)acc;
+  }
+  if (a.hist_next && t < a.x_len) {
+    const long long j = in_end - a.x_len + t;
+    a.hist_next[t] = j < 0 ? (Tin)0 : sample(j);
+  }
 }
 
-int resample_poly_run(Engine* e, const float* d_x, int n, int up, int down, const double* d_h, int n_taps, float* d_y, int n_out, cudaStream_t st) {
-  const int half_len = (n_taps - 1) / 2;
-  const int n_pre_pad = down - half_len % down;
-  const int n_pre_remove = (half_len + n_pre_pad) / down;
-  if (n_out <= 0) return 0;
-  k_resample_poly<<<(n_out + 255) / 256, 256, 0, st>>>(d_x, n, up, down, d_h, n_taps, n_pre_pad, n_pre_remove, d_y, n_out);
+template <typename Tin, typename Tout>
+static int resample_launch(Engine* e, const PolyArgs<Tin, Tout>& a, cudaStream_t st) {
+  const int threads = a.hist_next && a.x_len > a.n_out ? a.x_len : a.n_out;
+  if (threads <= 0) return 0;
+  k_resample_poly<Tin, Tout><<<(threads + 255) / 256, 256, 0, st>>>(a);
   RYK_CUDA(cudaGetLastError());
   e->launches++;
   return 0;
+}
+
+int resample_poly_run(Engine* e, const float* d_x, int n, int up, int down, const double* d_h, int n_taps, float* d_y, int n_out, cudaStream_t st) {
+  PolyArgs<float, float> a = {};
+  a.mode = kPolyWhole; a.h = d_h; a.n_taps = n_taps; a.up = up; a.down = down;
+  a.x = d_x; a.x_len = n; a.y = d_y; a.n_out = n_out;
+  return resample_launch(e, a, st);
+}
+
+int resample_stream_in_run(Engine* e, const float* d_window, int window, int chunk, int delay, int up, int down, const double* d_h, int n_taps,
+                           const ResampleState* d_st, ResampleState* d_st_next, float* d_y, int n_out, cudaStream_t st) {
+  PolyArgs<float, float> a = {};
+  a.mode = kPolyStreamIn; a.h = d_h; a.n_taps = n_taps; a.up = up; a.down = down;
+  a.x = d_window; a.x_len = window; a.chunk = chunk; a.delay = delay; a.y = d_y; a.n_out = n_out; a.st = d_st; a.st_next = d_st_next;
+  return resample_launch(e, a, st);
+}
+
+int resample_stream_out_run(Engine* e, const double* d_hist, double* d_hist_next, int hist, const double* d_new, const int* d_n_new, int up,
+                            int down, const double* d_h, int n_taps, const ResampleState* d_st, ResampleState* d_st_next, double* d_y,
+                            int max_out, int* d_n_out, cudaStream_t st) {
+  PolyArgs<double, double> a = {};
+  a.mode = kPolyStreamOut; a.h = d_h; a.n_taps = n_taps; a.up = up; a.down = down;
+  a.x = d_hist; a.x_len = hist; a.hist_next = d_hist_next; a.x_new = d_new; a.n_new = d_n_new;
+  a.y = d_y; a.n_out = max_out; a.n_out_dev = d_n_out; a.st = d_st; a.st_next = d_st_next;
+  return resample_launch(e, a, st);
 }
 
 }  // namespace ryk

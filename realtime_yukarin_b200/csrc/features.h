@@ -28,6 +28,28 @@ int convert_buffers_get(Engine* e, int T, int n_wave, int nb, int C, ConvertBuff
 int convert_window_device(Engine* e, const ConvertBuffers& cb, int T, int n_wave, int frame_length, int hop, double threshold_db,
                           int order, int fftlen, cudaStream_t st);
 
+// polyphase resampler (features.cu: k_resample_poly): the whole-signal call of ryk_resample_poly and the two streaming sides of a
+// session's device-rate conversion.  Streaming positions live on the device, double-buffered by step parity.
+struct ResampleState { long long in_end, out_end; };     // input samples received, output samples emitted (before the step)
+enum PolyMode { kPolyWhole = 0, kPolyStreamIn = 1, kPolyStreamOut = 2 };
+template <typename Tin, typename Tout>
+struct PolyArgs {
+  int mode;
+  const double* h; int n_taps, up, down;
+  const Tin* x; int x_len;                 // whole signal | history window ending at the newest sample | kept history
+  const Tin* x_new; const int* n_new;      // stream out: the step's new samples and their count
+  int chunk, delay;                        // stream in: samples per step, leading zeros of the output (model-rate samples)
+  Tout* y; int n_out;                      // outputs (stream out: the most one step may emit)
+  int* n_out_dev;                          // stream out: outputs emitted by the step
+  const ResampleState* st; ResampleState* st_next;
+  Tin* hist_next;                          // stream out: the kept history after the step (x_len samples)
+};
+int resample_stream_in_run(Engine* e, const float* d_window, int window, int chunk, int delay, int up, int down, const double* d_h, int n_taps,
+                           const ResampleState* d_st, ResampleState* d_st_next, float* d_y, int n_out, cudaStream_t st);
+int resample_stream_out_run(Engine* e, const double* d_hist, double* d_hist_next, int hist, const double* d_new, const int* d_n_new, int up,
+                            int down, const double* d_h, int n_taps, const ResampleState* d_st, ResampleState* d_st_next, double* d_y,
+                            int max_out, int* d_n_out, cudaStream_t st);
+
 void session_destroy_all(Engine* e);
 int session_streams_fork(Engine* e, cudaEvent_t ev);
 int session_streams_join(Engine* e);

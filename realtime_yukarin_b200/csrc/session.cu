@@ -23,6 +23,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <array>
+#include <numeric>
 #include <vector>
 
 #include "../../include/ryk.h"
@@ -114,6 +115,21 @@ struct Session {
   Synth* synth = nullptr;
   DioPlan* dio[2] = {nullptr, nullptr};     // one analysis plan per chunk parity (owned), f0 methods 0 and 1
   CrepePlan* crepe[2] = {nullptr, nullptr}; // f0 method 2: one CREPE forward per chunk parity (owned) in place of DIO/Harvest
+  // Device rates (ryk_session_set_input_rate / _output_rate): chunks arrive at in.rate and outputs leave at out.rate; analysis, the
+  // U-Nets and synthesis stay at cfg.fs.  rate 0 = that side runs at fs (no resampler).
+  struct RateSide {
+    int rate = 0, up = 1, down = 1, n_taps = 0;
+    int hist = 0;                                 // input: history window (chunk + left support); output: kept synthesizer samples
+    double* d_h = nullptr;
+    ResampleState* d_st = nullptr;                // [2] by step parity
+  } in, out;
+  int n_in = 0;                    // samples per pushed chunk (n_wave without an input resampler)
+  int delay_in = 0;                // leading zeros of the model-rate input (model samples)
+  int max_out = 0;                 // most output samples one step can return
+  float* in_win[2] = {nullptr, nullptr};      // input history windows (in.hist device-rate samples)
+  float* d_chunk_model = nullptr;             // the step's resampled chunk (n_wave model-rate samples)
+  double* out_hist[2] = {nullptr, nullptr};   // kept synthesizer samples (out.hist)
+  double* d_rout_fixed[2] = {nullptr, nullptr}; int* d_rn_fixed[2] = {nullptr, nullptr};   // device-rate output of a step, by parity
   std::vector<void*> allocs, pinned;
 };
 
@@ -463,14 +479,22 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
   ParityGraphs& pg = s->graphs[b];
 
   // ================= stream E: gate + WORLD analysis =================
-  RYK_CUDA(cudaMemcpyAsync(s->d_chunk_fixed, d_chunk_user, sizeof(float) * s->n_wave, cudaMemcpyDeviceToDevice, s->sE));
+  RYK_CUDA(cudaMemcpyAsync(s->d_chunk_fixed, d_chunk_user, sizeof(float) * s->n_in, cudaMemcpyDeviceToDevice, s->sE));
   if (k >= 2) {
     RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev[(k - 2) % kRing].s1, 0));      // mask/index/count[b]: last read by stage 1 of k-2
     RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev[(k - 2) % kRing].enc, 0));     // wave_win[g]: last read by the analysis of k-2
   }
   if (stage_time(s, 0, 0, r, s->sE)) return -1;
   if (run_graph(e, pg.gate, s->sE, [&]() -> int {
-        if (slide<float>(s->wave_win[f], s->d_chunk_fixed, s->wave_win[g], s->Lw, s->n_wave, 1, s->sE)) return -1;
+        const float* chunk = s->d_chunk_fixed;
+        if (s->in.rate) {            // device rate -> fs in front of the wave slide
+          if (slide<float>(s->in_win[f], s->d_chunk_fixed, s->in_win[g], s->in.hist, s->n_in, 1, s->sE)) return -1;
+          e->launches += 1;
+          if (resample_stream_in_run(e, s->in_win[g], s->in.hist, s->n_in, s->delay_in, s->in.up, s->in.down, s->in.d_h, s->in.n_taps,
+                                     s->in.d_st + f, s->in.d_st + g, s->d_chunk_model, s->n_wave, s->sE)) return -1;
+          chunk = s->d_chunk_model;
+        }
+        if (slide<float>(s->wave_win[f], chunk, s->wave_win[g], s->Lw, s->n_wave, 1, s->sE)) return -1;
         if (slide<float>(s->cw_wave[f], s->wave_win[g] + (size_t)pe * s->hop, s->cw_wave[g], (size_t)s->Tw * s->hop, (size_t)s->n_feat * s->hop, 1, s->sE)) return -1;
         e->launches += 2;
         return gate_mask_run(e, s->cw_wave[g], s->Tw * s->hop, c.fft_length, s->hop, c.threshold_db, s->Tw, s->d_mse, s->d_mask[b], s->d_index[b],
@@ -606,7 +630,11 @@ static int session_back(Engine* e, Session* s) {
         k_scrub<<<8, 256, 0, s->sD>>>(s->d_out_fixed[b], s->synth->dev.state, c.vocoder_buffer_size, max_blocks * c.vocoder_buffer_size, s->d_n_fixed[b]);
         e->launches += 1;
         RYK_CUDA(cudaGetLastError());
-        return 0;
+        if (!s->out.rate) return 0;
+        // fs -> device rate: the outputs whose filter support the synthesizer has produced; the rest waits for the next step
+        return resample_stream_out_run(e, s->out_hist[f], s->out_hist[g], s->out.hist, s->d_out_fixed[b], s->d_n_fixed[b], s->out.up, s->out.down,
+                                       s->out.d_h, s->out.n_taps, s->out.d_st + f, s->out.d_st + g, s->d_rout_fixed[b], s->max_out,
+                                       s->d_rn_fixed[b], s->sD);
       })) return -1;
   if (stage_time(s, 4, 1, r, s->sD)) return -1;
   // ev[r].dec is recorded by stage_out after the copies it appends to stream D
@@ -654,18 +682,21 @@ static int group_enqueue(Engine* e, Group* G, const float* const* d_chunks) {
 // ---- host-API staging shared by sessions and groups (ring slot r = step % kRing) ----
 // host chunk -> pinned slot -> s->d_chunk[r] on stream E
 static int stage_in(Session* s, int r, const float* wave) {
-  memcpy(s->h_in[r], wave, sizeof(float) * s->n_wave);
-  RYK_CUDA(cudaMemcpyAsync(s->d_chunk[r], s->h_in[r], sizeof(float) * s->n_wave, cudaMemcpyHostToDevice, s->sE));
+  memcpy(s->h_in[r], wave, sizeof(float) * s->n_in);
+  RYK_CUDA(cudaMemcpyAsync(s->d_chunk[r], s->h_in[r], sizeof(float) * s->n_in, cudaMemcpyHostToDevice, s->sE));
   return 0;
 }
 
-// after step k was enqueued: copy its blocks and sample count to out / n_out (kind: to the host ring or to device buffers) behind
+// the samples a step of parity b returns and their count: the synthesizer's blocks, or their device-rate resampling
+static double* step_out(Session* s, int b) { return s->out.rate ? s->d_rout_fixed[b] : s->d_out_fixed[b]; }
+static int* step_n_out(Session* s, int b) { return s->out.rate ? s->d_rn_fixed[b] : s->d_n_fixed[b]; }
+
+// after step k was enqueued: copy its samples and sample count to out / n_out (kind: to the host ring or to device buffers) behind
 // the decode stream and record ev[r].dec
 static int stage_out(Session* s, long long k, double* out, int* n_out, cudaMemcpyKind kind) {
   const int b = (int)(k & 1), r = (int)(k % kRing);
-  const size_t cap = (size_t)s->max_blocks * s->cfg.vocoder_buffer_size;
-  RYK_CUDA(cudaMemcpyAsync(n_out, s->d_n_fixed[b], sizeof(int), kind, s->sD));
-  RYK_CUDA(cudaMemcpyAsync(out, s->d_out_fixed[b], sizeof(double) * cap, kind, s->sD));
+  RYK_CUDA(cudaMemcpyAsync(n_out, step_n_out(s, b), sizeof(int), kind, s->sD));
+  RYK_CUDA(cudaMemcpyAsync(out, step_out(s, b), sizeof(double) * s->max_out, kind, s->sD));
   RYK_CUDA(cudaEventRecord(s->ev[r].dec, s->sD));
   return 0;
 }
@@ -730,6 +761,11 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
   RYK_CHECK(s->n_wave == s->n_feat * s->hop && s->e_wave == s->e_enc_frames * s->hop, "buffer_time / encode_extra_time must be whole frames");
   RYK_CHECK(s->Lw / s->hop - 2 * s->e_enc_frames == s->n_feat, "encode window does not trim to one chunk of frames");
   RYK_CHECK(s->nb == 513 && e->stage1->in_ch == s->C, "session configuration does not match the loaded models");
+  // the synthesizer's spectra are cheaptrick_fft_size(fs) / 2 + 1 bins wide and read rows of the fft_length / 2 + 1 bin decode window
+  RYK_CHECK(cheaptrick_fft_size(cfg->fs, 71.0) / 2 + 1 == s->nb,
+            "fs does not match fft_length: the synthesizer at this fs needs a different spectrum width (run the session at the model's "
+            "rate and set a device rate with ryk_session_set_input_rate / ryk_session_set_output_rate)");
+  s->n_in = s->n_wave;
   if (sptk_prepare(e, cfg->order, cfg->alpha, cfg->fft_length)) return -1;
   // The analysis, stage-1 and synthesis stages are chains of small, latency-bound kernels; stage 2 is bulk work that fills
   // every SM.  Higher stream priority for the former lets their CTAs take freed SM slots first, so their latency does not
@@ -782,7 +818,8 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
   if (A((void**)&s->dec_f0_f64, sizeof(double) * s->Td)) return -1;
   if (A((void**)&s->d_chunk_fixed, sizeof(float) * s->n_wave)) return -1;
   s->max_blocks = (s->Td * s->hop) / cfg->vocoder_buffer_size + 4;
-  const size_t out_samples = (size_t)s->max_blocks * cfg->vocoder_buffer_size;
+  s->max_out = s->max_blocks * cfg->vocoder_buffer_size;
+  const size_t out_samples = (size_t)s->max_out;
   for (int i = 0; i < 2; ++i) {
     if (A((void**)&s->d_out_fixed[i], sizeof(double) * out_samples)) return -1;
     if (A((void**)&s->d_n_fixed[i], sizeof(int))) return -1;
@@ -835,7 +872,7 @@ int ryk_session_submit(ryk_engine* h, int id, const float* wave, int n, long lon
   RYK_CUDA(cudaSetDevice(e->device));
   Session* s = get_session(e, id);
   RYK_CHECK(s != nullptr, "no such session");
-  RYK_CHECK(n == s->n_wave, "chunk length must be round(fs * buffer_time)");
+  RYK_CHECK(n == s->n_in, "chunk length must be round(rate * buffer_time) at the session's input rate");
   RYK_CHECK(s->group == nullptr, "session belongs to a group: use ryk_group_submit");
   RYK_CHECK(s->step - s->collected < kRing - 2, "too many chunks in flight: collect before submitting more");
   const long long k = s->step;
@@ -882,13 +919,106 @@ int ryk_session_push_device(ryk_engine* h, int id, const float* wave_dev, int n,
   RYK_CUDA(cudaSetDevice(e->device));
   Session* s = get_session(e, id);
   RYK_CHECK(s != nullptr, "no such session");
-  RYK_CHECK(n == s->n_wave, "chunk length must be round(fs * buffer_time)");
+  RYK_CHECK(n == s->n_in, "chunk length must be round(rate * buffer_time) at the session's input rate");
   RYK_CHECK(s->group == nullptr, "session belongs to a group: use ryk_group_push_device");
-  RYK_CHECK(out_capacity >= s->max_blocks * s->cfg.vocoder_buffer_size, "out_capacity must hold (frames * hop / block + 4) synthesizer blocks");
+  RYK_CHECK(out_capacity >= s->max_out, "out_capacity must hold the most samples a step returns (ryk_session_io_geometry max_out)");
   const long long k = s->step;
   if (session_enqueue(e, s, wave_dev)) return -1;
   if (stage_out(s, k, out_dev, n_out_dev, cudaMemcpyDeviceToDevice)) return -1;
   s->collected = s->step;         // device-resident steps are not collected through the host API
+  return 0;
+}
+
+// ---- device rates: the session takes chunks at in.rate and returns samples at out.rate, converting on its own streams ----
+// A zeroed allocation owned by the session (device, or pinned host); a buffer already at *p is released first.
+static int session_realloc(Session* s, void** p, size_t bytes, bool host) {
+  std::vector<void*>& owned = host ? s->pinned : s->allocs;
+  if (*p) {
+    for (size_t i = 0; i < owned.size(); ++i) if (owned[i] == *p) { owned.erase(owned.begin() + i); break; }
+    if (host) cudaFreeHost(*p); else cudaFree(*p);
+    *p = nullptr;
+  }
+  if (host) { RYK_CUDA(cudaMallocHost(p, bytes)); memset(*p, 0, bytes); }
+  else { RYK_CUDA(cudaMalloc(p, bytes)); RYK_CUDA(cudaMemset(*p, 0, bytes)); }
+  owned.push_back(*p);
+  return 0;
+}
+
+// Geometry (DESIGN.md §4, DECIDE R1), with half = (n_taps - 1) / 2 and up / down = the resampler's output rate / input rate:
+//   input:  delay_in = half / down model samples, the smallest delay for which every sample of a step's model-rate chunk has its whole
+//           filter support in the chunks received; the history window holds the chunk and the ceil((delay_in * down + half) / up)
+//           samples before it.
+//   output: a step emits the outputs whose support ends inside the synthesizer samples so far; the kept history covers the left
+//           support of the first output not yet emitted, and max_out bounds one step's count.
+static int session_set_rate(Engine* e, int id, bool input, int rate, int up, int down, const double* taps, int n_taps) {
+  RYK_CUDA(cudaSetDevice(e->device));
+  Session* s = get_session(e, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  RYK_CHECK(s->step == 0 && s->group == nullptr, "device rates can only be set on a fresh session (no chunk pushed, not in a group)");
+  Session::RateSide& side = input ? s->in : s->out;
+  RYK_CHECK(side.rate == 0, "this side's device rate is already set");
+  RYK_CHECK(rate > 0, "device rate must be positive");
+  const int fs = s->cfg.fs;
+  if (rate == fs) return 0;                         // the session's own rate: no resampler on this side
+  RYK_CHECK(taps && n_taps > 0 && (n_taps & 1) && up > 0 && down > 0 && std::gcd(up, down) == 1,
+            "bad resampler arguments (coprime up / down, an odd number of taps)");
+  const long long r_from = input ? rate : fs, r_to = input ? fs : rate;
+  RYK_CHECK(r_to * down == r_from * up, "up / down must be the resampler's output rate / input rate, reduced");
+  const int half = (n_taps - 1) / 2;
+  if (input) {
+    const int n_in = (int)lrint(s->cfg.buffer_time * rate);
+    RYK_CHECK((long long)n_in * up == (long long)s->n_wave * down,
+              "the chunk at this device rate is not a whole number of samples: round(rate * buffer_time) * up != round(fs * buffer_time) * down");
+    const int delay = half / down;
+    side.hist = n_in + (delay * down + half + up - 1) / up;
+    for (int i = 0; i < 2; ++i) if (session_realloc(s, (void**)&s->in_win[i], sizeof(float) * side.hist, false)) return -1;
+    if (session_realloc(s, (void**)&s->d_chunk_model, sizeof(float) * s->n_wave, false)) return -1;
+    if (session_realloc(s, (void**)&s->d_chunk_fixed, sizeof(float) * n_in, false)) return -1;
+    for (int r = 0; r < kRing; ++r) {
+      if (session_realloc(s, (void**)&s->d_chunk[r], sizeof(float) * n_in, false)) return -1;
+      if (session_realloc(s, (void**)&s->h_in[r], sizeof(float) * n_in, true)) return -1;
+    }
+  } else {
+    const long long blocks = (long long)s->max_blocks * s->cfg.vocoder_buffer_size;
+    const int max_out = (int)((blocks * up + down - 1) / down);
+    side.hist = (2 * half + down + up - 1) / up + 1;
+    for (int i = 0; i < 2; ++i) {
+      if (session_realloc(s, (void**)&s->out_hist[i], sizeof(double) * side.hist, false)) return -1;
+      if (session_realloc(s, (void**)&s->d_rout_fixed[i], sizeof(double) * max_out, false)) return -1;
+      if (session_realloc(s, (void**)&s->d_rn_fixed[i], sizeof(int), false)) return -1;
+    }
+    for (int r = 0; r < kRing; ++r) if (session_realloc(s, (void**)&s->h_out[r], sizeof(double) * max_out, true)) return -1;
+  }
+  if (session_realloc(s, (void**)&side.d_h, sizeof(double) * n_taps, false)) return -1;
+  if (session_realloc(s, (void**)&side.d_st, sizeof(ResampleState) * 2, false)) return -1;
+  RYK_CUDA(cudaMemcpy(side.d_h, taps, sizeof(double) * n_taps, cudaMemcpyHostToDevice));
+  RYK_CUDA(cudaDeviceSynchronize());               // the zero-fills ran on the legacy default stream; the session's streams do not wait for it
+  side.rate = rate; side.up = up; side.down = down; side.n_taps = n_taps;
+  if (input) {
+    s->n_in = (int)lrint(s->cfg.buffer_time * rate);
+    s->delay_in = half / down;
+  } else {
+    s->max_out = (int)(((long long)s->max_blocks * s->cfg.vocoder_buffer_size * up + down - 1) / down);
+  }
+  return 0;
+}
+
+int ryk_session_set_input_rate(ryk_engine* h, int id, int rate, int up, int down, const double* taps, int n_taps) {
+  return session_set_rate(&h->impl, id, true, rate, up, down, taps, n_taps);
+}
+
+int ryk_session_set_output_rate(ryk_engine* h, int id, int rate, int up, int down, const double* taps, int n_taps) {
+  return session_set_rate(&h->impl, id, false, rate, up, down, taps, n_taps);
+}
+
+int ryk_session_io_geometry(ryk_engine* h, int id, int* n_in, int* max_out, int* delay_in, int* in_rate, int* out_rate) {
+  Session* s = get_session(&h->impl, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  if (n_in) *n_in = s->n_in;
+  if (max_out) *max_out = s->max_out;
+  if (delay_in) *delay_in = s->delay_in;
+  if (in_rate) *in_rate = s->in.rate ? s->in.rate : s->cfg.fs;
+  if (out_rate) *out_rate = s->out.rate ? s->out.rate : s->cfg.fs;
   return 0;
 }
 
@@ -907,6 +1037,12 @@ int ryk_group_create(ryk_engine* h, const int* session_ids, int n_sessions, int*
       for (Session* m : G->members) m->group = nullptr;
       delete G;
       RYK_CHECK(false, "group members must be distinct fresh sessions (no chunk pushed yet) with the same window length");
+    }
+    // one chunk length serves every member in ryk_group_submit / ryk_group_push_device
+    if (i > 0 && (s->n_in != G->members[0]->n_in || s->in.rate != G->members[0]->in.rate || s->out.rate != G->members[0]->out.rate)) {
+      for (Session* m : G->members) m->group = nullptr;
+      delete G;
+      RYK_CHECK(false, "group members must have the same device input and output rates");
     }
     s->group = G; s->slot = i;
     G->members.push_back(s);
@@ -957,7 +1093,7 @@ int ryk_group_submit(ryk_engine* h, int group_id, const float* const* waves, int
   std::vector<const float*> d_chunks(G->members.size());
   for (size_t i = 0; i < G->members.size(); ++i) {
     Session* s = G->members[i];
-    RYK_CHECK(n == s->n_wave, "chunk length must be round(fs * buffer_time)");
+    RYK_CHECK(n == s->n_in, "chunk length must be round(rate * buffer_time) at the session's input rate");
     if (stage_in(s, r, waves[i])) return -1;
     d_chunks[i] = s->d_chunk[r];
   }
@@ -988,8 +1124,8 @@ int ryk_group_push_device(ryk_engine* h, int group_id, const float* const* waves
   Group* G = get_group(e, group_id);
   RYK_CHECK(G != nullptr, "no such group");
   for (Session* s : G->members) {
-    RYK_CHECK(n == s->n_wave, "chunk length must be round(fs * buffer_time)");
-    RYK_CHECK(out_capacity >= s->max_blocks * s->cfg.vocoder_buffer_size, "out_capacity must hold (frames * hop / block + 4) synthesizer blocks");
+    RYK_CHECK(n == s->n_in, "chunk length must be round(rate * buffer_time) at the session's input rate");
+    RYK_CHECK(out_capacity >= s->max_out, "out_capacity must hold the most samples a step returns (ryk_session_io_geometry max_out)");
   }
   const long long k = G->step;
   if (group_enqueue(e, G, waves_dev)) return -1;
@@ -1087,8 +1223,8 @@ int ryk_reblock_push_device(ryk_engine* h, int id, int session_id, const double*
     st = s->sD;
     if (!wave_dev) {
       const int b = (int)((s->step - 1) & 1);
-      RYK_CHECK(s->max_blocks * s->cfg.vocoder_buffer_size <= R->max_in, "re-blocker max_in is smaller than the session's block capacity");
-      wave_dev = s->d_out_fixed[b]; n_dev = s->d_n_fixed[b];
+      RYK_CHECK(s->max_out <= R->max_in, "re-blocker max_in is smaller than the most samples a session step returns");
+      wave_dev = step_out(s, b); n_dev = step_n_out(s, b);
     }
   }
   RYK_CHECK(wave_dev != nullptr && n_dev != nullptr, "wave_dev / n_dev are required without an attached session");

@@ -8,6 +8,7 @@ import os as _os
 _os.environ.setdefault('CUDA_DEVICE_MAX_CONNECTIONS', '32')
 
 import ctypes
+import math
 import os
 import threading
 from pathlib import Path
@@ -59,6 +60,7 @@ EXPORTED_SYMBOLS = [
     'ryk_engine_set_f0_method', 'ryk_engine_get_f0_method', 'ryk_debug_harvest',
     'ryk_crepe_create', 'ryk_crepe_set_conv', 'ryk_crepe_set_dense', 'ryk_crepe_set_decoder_tables', 'ryk_crepe_num_frames', 'ryk_crepe_predict',
     'ryk_crepe_set_resampler', 'ryk_crepe_test_conv', 'ryk_crepe_test_network', 'ryk_stage2_row_bands', 'ryk_test_stage2_forward',
+    'ryk_session_set_input_rate', 'ryk_session_set_output_rate', 'ryk_session_io_geometry',
 ]
 
 
@@ -117,6 +119,7 @@ class Engine(object):
         self._h = h
         self._synth_block = {}
         self._reblock_chunk = {}           # re-blocker id -> out_audio_chunk
+        self._session_fs = {}              # session id -> the session's (model) rate
 
     # ---- plumbing ----
     def _check(self, rc: int):
@@ -451,15 +454,42 @@ class Engine(object):
     def session_create(self, cfg: SessionConfig) -> int:
         sid = ctypes.c_int()
         self._check(self.lib.ryk_session_create(self._h, ctypes.byref(cfg), ctypes.byref(sid)))
+        self._session_fs[sid.value] = int(cfg.fs)
         return sid.value
+
+    def _session_set_rate(self, fn, sid: int, rate: int, rate_from: int, rate_to: int):
+        from .wave_io import resample_filter
+        g = math.gcd(int(rate_from), int(rate_to))
+        up, down = int(rate_to) // g, int(rate_from) // g
+        taps = numpy.ascontiguousarray(resample_filter(up, down), dtype=numpy.float64)
+        self._check(fn(self._h, sid, int(rate), up, down, _dp(taps), len(taps)))
+
+    def session_set_input_rate(self, sid: int, rate: int):
+        """Take this fresh session's chunks at `rate` (round(rate * buffer_time) samples each), resampled to the session's rate on the
+        device with wave_io.resample_filter.  rate == the session's rate: nothing to do."""
+        fs = self._session_fs[sid]
+        self._session_set_rate(self.lib.ryk_session_set_input_rate, sid, rate, rate, fs)
+
+    def session_set_output_rate(self, sid: int, rate: int):
+        """Return this fresh session's samples at `rate`, resampled from the session's rate on the device."""
+        fs = self._session_fs[sid]
+        self._session_set_rate(self.lib.ryk_session_set_output_rate, sid, rate, fs, rate)
+
+    def session_io_geometry(self, sid: int) -> Dict[str, int]:
+        """n_in (samples per chunk), max_out (most samples one step returns), delay_in (input delay, model-rate samples), in_rate,
+        out_rate (device rates; the session's rate when unset)."""
+        v = [ctypes.c_int() for _ in range(5)]
+        self._check(self.lib.ryk_session_io_geometry(self._h, sid, *[ctypes.byref(x) for x in v]))
+        return dict(zip(('n_in', 'max_out', 'delay_in', 'in_rate', 'out_rate'), (x.value for x in v)))
 
     def session_destroy(self, sid: int):
         self._check(self.lib.ryk_session_destroy(self._h, sid))
+        self._session_fs.pop(sid, None)
 
     def session_push(self, sid: int, wave, out: Optional[numpy.ndarray] = None) -> numpy.ndarray:
         w = _f32(wave)
         if out is None:
-            out = numpy.empty(len(w) * 2 + 8192, dtype=numpy.float64)
+            out = numpy.empty(max(len(w) * 2 + 8192, self.session_io_geometry(sid)['max_out']), dtype=numpy.float64)
         n_out = ctypes.c_int()
         self._check(self.lib.ryk_session_push(self._h, sid, _fp(w), len(w), _dp(out), len(out), ctypes.byref(n_out)))
         return out[:n_out.value]

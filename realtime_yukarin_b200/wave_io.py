@@ -40,6 +40,26 @@ def resample_geometry(n_in: int, up: int, down: int) -> Tuple[int, int, int, int
     return up, down, n_out, n_pre_pad, n_pre_remove
 
 
+def stream_input_geometry(rate: int, fs: int, buffer_time: float) -> Tuple[int, int, int]:
+    """(n_in, n, delay) of a session at `fs` that takes its chunks at device rate `rate` (DESIGN.md DECIDE R1): n_in device samples per
+    chunk, n model samples per step, and the delay in model samples -- the smallest for which every sample of step k's chunk,
+    concat(zeros(delay), resample_poly(x))[k n:(k + 1) n], has its whole filter support inside the chunks received."""
+    n_in, n = round(rate * buffer_time), round(fs * buffer_time)
+    g = math.gcd(int(fs), int(rate))
+    up, down = int(fs) // g, int(rate) // g
+    if n_in * up != n * down:
+        raise ValueError(f'a {buffer_time} s chunk at {rate} Hz is not a whole number of samples at {fs} Hz')
+    return n_in, n, (10 * max(up, down)) // down
+
+
+def stream_output_count(n_samples: int, rate: int, fs: int) -> int:
+    """M: how many samples of resample_poly(y) (fs -> device rate `rate`) have their whole filter support inside the first
+    `n_samples` samples of y -- what a session has returned once its synthesizer produced n_samples (DESIGN.md DECIDE R1)."""
+    g = math.gcd(int(fs), int(rate))
+    up, down = int(rate) // g, int(fs) // g
+    return max(0, (n_samples * up - 1 - 10 * max(up, down)) // down + 1)
+
+
 def resample(x: numpy.ndarray, rate_in: int, rate_out: int, engine=None) -> numpy.ndarray:
     """float32 signal at rate_in -> float32 signal at rate_out (ceil(len * rate_out / rate_in) samples)."""
     x = numpy.ascontiguousarray(x, dtype=numpy.float32)

@@ -87,14 +87,15 @@ class RealtimePipeline(object):
         self.config = config
         self.engine = engine or default_engine()
         p = acoustic_param
+        # analysis, the U-Nets and synthesis run at the models' rate; the sound card's rates are the session's device rates
+        fs = int(getattr(p, 'sampling_rate', 24000))
         cfg = SessionConfig(
-            fs=int(config.input_rate), frame_period_ms=float(config.frame_period),
+            fs=fs, frame_period_ms=float(config.frame_period),
             f0_floor=float(getattr(p, 'f0_floor', 71.0)), f0_ceil=float(getattr(p, 'f0_ceil', 800.0)),
             fft_length=int(getattr(p, 'fft_length', 1024)), order=int(getattr(p, 'order', 8)), alpha=float(getattr(p, 'alpha', 0.466)),
             buffer_time=float(config.buffer_time), encode_extra_time=float(config.encode_extra_time),
             convert_extra_time=float(config.convert_extra_time), decode_extra_time=float(config.decode_extra_time),
             threshold_db=float(config.input_silent_threshold), vocoder_buffer_size=int(config.vocoder_buffer_size))
-        assert config.input_rate == config.output_rate, 'the accelerated path runs analysis and synthesis at one rate'
         self.depth = max(1, min(int(depth), 5))
         # per-item stage timing at DEBUG, as the reference's workers log it (encode_worker.py:34,44, convert_worker.py:47,59,
         # decode_worker.py:42,66: `logger.debug(f'{item.index}: {time.time() - start}')` on loggers 'encode' / 'convert' / 'decode').
@@ -107,7 +108,7 @@ class RealtimePipeline(object):
         if crepe_mode:
             from . import crepe
             crepe.engine_with_model(self.engine)
-            crepe.set_session_rate(config.input_rate, self.engine)
+            crepe.set_session_rate(fs, self.engine)
             prev_method = self.engine.f0_method
             self.engine.set_f0_method('crepe')
         if self._timing:
@@ -123,11 +124,17 @@ class RealtimePipeline(object):
                     os.environ['RYK_STAGE_TIMES'] = prev
             if crepe_mode:
                 self.engine.set_f0_method(prev_method)
-        # capacity of one step's synthesizer output, as the session sizes it: (decode-window samples // block + 4) blocks
-        rate = round(1000 / float(config.frame_period))
-        hop = round(config.output_rate * float(config.frame_period) / 1000)
-        td = round(config.buffer_time * rate) + 2 * round(config.decode_extra_time * rate)
-        n_out_cap = (td * hop // config.vocoder_buffer_size + 4) * config.vocoder_buffer_size
+        if int(config.input_rate) != fs or int(config.output_rate) != fs:
+            # the session resamples the sound card's chunks to fs and its output back to the card's rate on the device
+            self.engine.session_set_input_rate(self._sid, int(config.input_rate))
+            self.engine.session_set_output_rate(self._sid, int(config.output_rate))
+            n_out_cap = self.engine.session_io_geometry(self._sid)['max_out']
+        else:
+            # capacity of one step's synthesizer output, as the session sizes it: (decode-window samples // block + 4) blocks
+            rate = round(1000 / float(config.frame_period))
+            hop = round(fs * float(config.frame_period) / 1000)
+            td = round(config.buffer_time * rate) + 2 * round(config.decode_extra_time * rate)
+            n_out_cap = (td * hop // config.vocoder_buffer_size + 4) * config.vocoder_buffer_size
         self._scratch = numpy.empty(n_out_cap, dtype=numpy.float64)
         self._rid = self.engine.reblock_create(config.out_audio_chunk, n_out_cap, float(config.output_silent_threshold))
         self._inflight: Deque[Tuple[Item, int, int, float]] = deque()      # (item, session ticket, re-blocker ticket, host time of put)
