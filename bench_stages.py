@@ -1,0 +1,225 @@
+"""Where a streaming session's step goes: per-kernel device time of the gate, WORLD-analysis and stage-1 graphs, and the stage timeline.
+
+One session of the headline workload (0.3 s chunks at 24 kHz, extras 0 / 0.5 / 0, base-64 seeded U-Nets, FP16, device-resident steps)
+is run three ways:
+  * isolated  -- one step with nothing else queued, a device synchronise before and after (--isolated steps, averaged);
+  * pipelined -- --steps back-to-back steps after --warmup, as bench.py runs them; figures are per step (total over the steps / steps);
+  * timeline  -- RYK_STAGE_TIMES=1: begin / end of the five stages of the last 8 pipelined steps (ryk_session_stage_times).
+Kernel times come from torch.profiler with CUDA activities (CUPTI), which sees the kernels inside the session's CUDA graphs.  A kernel
+is attributed to the stage whose stream it ran on; a stream's stage is named by the kernels it carries (the analysis graph's own
+branch streams carry only analysis kernels).  The card's name, power limit and SM clocks are read in the same run.
+
+    python bench_stages.py --out DIR [--steps 40 --warmup 10 --isolated 8 --f0 dio|harvest]
+
+Writes DIR/bench_stages.json, DIR/bench_stages.md and the profiler traces, and prints the markdown.  Needs a CUDA device.  RYK_LIB
+selects another build of the library (engine.py), so two builds can be profiled by the same script."""
+import argparse
+import json
+import os
+import re
+import subprocess
+import tempfile
+from collections import defaultdict
+from pathlib import Path
+
+os.environ['RYK_STAGE_TIMES'] = '1'             # read by ryk_session_create
+os.environ.setdefault('CUDA_DEVICE_MAX_CONNECTIONS', '32')
+
+import numpy as np  # noqa: E402
+
+T, EXTRA, FS = 0.3, (0.0, 0.5, 0.0), 24000
+STAGES = ['gate_slides', 'world_analysis', 'stage1', 'stage2', 'synthesis']
+# a stream's stage = the first of these whose kernel-name pattern occurs on it
+STREAM_ROLES = [
+    ('world_analysis', re.compile(r'k_dio|k_stonemask|k_cheaptrick|k_d4c|k_f0_out|k_hv_|crepe', re.I)),
+    ('stage2', re.compile(r'k_conv_tc|splitk|k_sr_', re.I)),
+    ('stage1', re.compile(r'k_set_bucket|k_s1_|stage1', re.I)),
+    ('synthesis', re.compile(r'k_scrub|synth', re.I)),
+    ('gate_slides', re.compile(r'k_slide<|resample|k_frame_mse|k_gate\b', re.I)),
+]
+REPORTED = ('gate_slides', 'world_analysis', 'stage1')
+
+
+def card():
+    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm,clocks.sm', '--format=csv,noheader'],
+                       capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else 'unknown (nvidia-smi unavailable)'
+
+
+def short_name(name):
+    n = name.split('(')[0] if '(' in name else name
+    n = re.sub(r'^void\s+', '', n).replace('ryk::', '').replace('(anonymous namespace)::', '')
+    return n.strip()
+
+
+def kernels_of(trace_path):
+    """[(stream, name, ts_us, dur_us)] of the CUDA kernels in a chrome trace written by torch.profiler."""
+    ev = json.loads(Path(trace_path).read_text())
+    ev = ev['traceEvents'] if isinstance(ev, dict) else ev
+    out = []
+    for e in ev:
+        if e.get('cat') == 'kernel' and e.get('ph') == 'X':
+            out.append((e.get('args', {}).get('stream', e.get('tid')), short_name(e['name']), float(e['ts']), float(e['dur'])))
+    return out
+
+
+def stream_roles(kernels):
+    names = defaultdict(set)
+    for st, n, _, _ in kernels:
+        names[st].add(n)
+    roles = {}
+    for st, ns in names.items():
+        roles[st] = next((role for role, pat in STREAM_ROLES if any(pat.search(n) for n in ns)), 'other')
+    return roles
+
+
+def per_kernel(kernels, n_steps):
+    """{stage: {kernel: [calls per step, us per call, us per step]}} and {stage: us per step}"""
+    roles = stream_roles(kernels)
+    acc = defaultdict(lambda: defaultdict(lambda: [0, 0.0]))
+    for st, n, _, d in kernels:
+        a = acc[roles[st]][n]
+        a[0] += 1
+        a[1] += d
+    table, totals = {}, {}
+    for role, ks in acc.items():
+        table[role] = {n: [c / n_steps, s / c, s / n_steps] for n, (c, s) in sorted(ks.items(), key=lambda kv: -kv[1][1])}
+        totals[role] = sum(s for _, s in ks.values()) / n_steps
+    return table, totals
+
+
+def spans(kernels):
+    """{stage: first kernel start to last kernel end (us)} of one isolated step"""
+    roles = stream_roles(kernels)
+    lo, hi = {}, {}
+    for st, _, ts, d in kernels:
+        r = roles[st]
+        lo[r] = min(lo.get(r, ts), ts)
+        hi[r] = max(hi.get(r, ts + d), ts + d)
+    return {r: hi[r] - lo[r] for r in lo}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--out', type=Path, required=True)
+    ap.add_argument('--steps', type=int, default=40)
+    ap.add_argument('--warmup', type=int, default=10)
+    ap.add_argument('--isolated', type=int, default=8)
+    ap.add_argument('--f0', default='dio', choices=['dio', 'harvest'])
+    args = ap.parse_args()
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    if not torch.cuda.is_available():
+        raise SystemExit('bench_stages.py needs a CUDA device')
+    from realtime_yukarin_b200 import synthetic
+    from realtime_yukarin_b200.engine import Engine, SessionConfig
+    from realtime_yukarin_b200.models import AcousticConverter, F0Converter, SuperResolution
+    from realtime_yukarin_b200.params import create_from_json, create_sr_from_json
+
+    args.out.mkdir(parents=True, exist_ok=True)
+    tmp = Path(tempfile.mkdtemp(prefix='bench_stages_'))       # synthetic model files: never written into the tree
+    paths = synthetic.write_synthetic_models(tmp, seed=0)
+    eng = Engine()
+    f0c = F0Converter(paths['input_statistics_path'], paths['target_statistics_path'])
+    AcousticConverter(create_from_json(paths['stage1_config_path']), paths['stage1_model_path'], f0_converter=f0c, engine=eng)
+    SuperResolution(create_sr_from_json(paths['stage2_config_path']), paths['stage2_model_path'], engine=eng)
+    eng.set_precision('fp16')
+    eng.set_f0_method(args.f0)
+    cfg = SessionConfig(fs=FS, frame_period_ms=5.0, f0_floor=71.0, f0_ceil=800.0, fft_length=1024, order=8, alpha=0.466, buffer_time=T,
+                        encode_extra_time=EXTRA[0], convert_extra_time=EXTRA[1], decode_extra_time=EXTRA[2], threshold_db=60.0,
+                        vocoder_buffer_size=1024)
+    n = round(T * FS)
+    total = args.warmup + max(args.steps, args.isolated)
+    x = synthetic.synthetic_speech((total + 1) * T, stream=0)
+    d_in = torch.from_numpy(np.stack([x[k * n:(k + 1) * n] for k in range(total)]).astype(np.float32)).cuda()
+    out_cap = (n // 1024 + 5) * 1024 + 8192
+    d_out = torch.empty((8, out_cap), dtype=torch.float64, device='cuda')
+    d_n = torch.zeros(8, dtype=torch.int32, device='cuda')
+    card_before = card()
+
+    def fresh_session():
+        sid = eng.session_create(cfg)
+        for k in range(args.warmup):
+            eng.session_push_device(sid, d_in[k].data_ptr(), n, d_out[k % 8].data_ptr(), out_cap, d_n[k % 8:].data_ptr())
+        eng.synchronize()
+        torch.cuda.synchronize()
+        return sid
+
+    def push(sid, k):
+        eng.session_push_device(sid, d_in[k].data_ptr(), n, d_out[k % 8].data_ptr(), out_cap, d_n[k % 8:].data_ptr())
+
+    acts = [ProfilerActivity.CPU, ProfilerActivity.CUDA]
+    # ---- isolated steps ----
+    sid = fresh_session()
+    iso_kernels, iso_spans = [], defaultdict(list)
+    for i in range(args.isolated):
+        with profile(activities=acts) as prof:
+            push(sid, args.warmup + i)
+            eng.synchronize()
+            torch.cuda.synchronize()
+        tp = args.out / f'trace_isolated_{i}.json'
+        prof.export_chrome_trace(str(tp))
+        ks = kernels_of(tp)
+        iso_kernels += ks
+        for r, v in spans(ks).items():
+            iso_spans[r].append(v)
+    eng.session_destroy(sid)
+    iso_table, iso_totals = per_kernel(iso_kernels, args.isolated)
+
+    # ---- pipelined steps ----
+    sid = fresh_session()
+    with profile(activities=acts) as prof:
+        for k in range(args.warmup, args.warmup + args.steps):
+            push(sid, k)
+        eng.synchronize()
+        torch.cuda.synchronize()
+    tp = args.out / 'trace_pipelined.json'
+    prof.export_chrome_trace(str(tp))
+    pipe_table, pipe_totals = per_kernel(kernels_of(tp), args.steps)
+    eng.session_destroy(sid)
+
+    # ---- stage timeline, profiler off ----
+    sid = fresh_session()
+    eng.timer_start()
+    for k in range(args.warmup, args.warmup + args.steps):
+        push(sid, k)
+    ms = eng.timer_stop()
+    st, en = eng.session_stage_times(sid)
+    eng.session_destroy(sid)
+    # gate of step k against the end of stage 1 of step k-2 (> 0: the gate started after it)
+    gate_vs_s1 = [float(st[i, 0] - en[i - 2, 2]) for i in range(2, len(st))]
+
+    res = dict(card=card_before, card_after=card(), f0=args.f0, steps=args.steps, warmup=args.warmup, isolated=args.isolated,
+               lib=os.environ.get('RYK_LIB', 'realtime_yukarin_b200/csrc/libryk.so'),
+               isolated_us=iso_table, isolated_stage_us=iso_totals,
+               isolated_stage_span_us={r: float(np.mean(v)) for r, v in iso_spans.items()},
+               pipelined_us=pipe_table, pipelined_stage_us=pipe_totals,
+               timeline=dict(stages=STAGES, start_ms=np.round(st, 4).tolist(), end_ms=np.round(en, 4).tolist(),
+                             ms_per_step=ms / args.steps, gate_start_minus_stage1_end_of_k_minus_2_ms=np.round(gate_vs_s1, 4).tolist()))
+    (args.out / 'bench_stages.json').write_text(json.dumps(res, indent=1))
+
+    lines = [f'card: {res["card"]} (after: {res["card_after"]}); f0 {args.f0}; library {res["lib"]}', '']
+    for role in REPORTED:
+        lines += [f'### {role}: {iso_totals.get(role, 0):.1f} us of kernels per isolated step (span '
+                  f'{res["isolated_stage_span_us"].get(role, 0):.1f} us), {pipe_totals.get(role, 0):.1f} us per pipelined step', '',
+                  '| kernel | calls / step | isolated us / call | isolated us / step | pipelined us / step |', '|---|---|---|---|---|']
+        names = list(iso_table.get(role, {})) + [k for k in pipe_table.get(role, {}) if k not in iso_table.get(role, {})]
+        for k in names:
+            c, per, tot = iso_table.get(role, {}).get(k, [0, 0, 0])
+            pt = pipe_table.get(role, {}).get(k, [0, 0, 0])[2]
+            lines.append(f'| `{k}` | {c:g} | {per:.2f} | {tot:.2f} | {pt:.2f} |')
+        lines.append('')
+    other = {r: v for r, v in pipe_totals.items() if r not in REPORTED}
+    lines += ['other stages, pipelined us of kernels per step: ' + ', '.join(f'{r} {v:.1f}' for r, v in sorted(other.items())), '',
+              f'timeline (RYK_STAGE_TIMES=1, profiler off): {res["timeline"]["ms_per_step"]:.4f} ms per step over {args.steps} steps', '',
+              '| step | ' + ' | '.join(STAGES) + ' |', '|---' * (len(STAGES) + 1) + '|']
+    for i in range(len(st)):
+        lines.append(f'| {i} | ' + ' | '.join(f'{st[i, a]:.3f}-{en[i, a]:.3f}' for a in range(len(STAGES))) + ' |')
+    lines += ['', 'gate start of step k minus stage-1 end of step k-2 (ms): ' + ', '.join(f'{v:.3f}' for v in gate_vs_s1)]
+    md = '\n'.join(lines) + '\n'
+    (args.out / 'bench_stages.md').write_text(md)
+    print(md)
+
+
+if __name__ == '__main__':
+    main()

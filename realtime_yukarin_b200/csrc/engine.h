@@ -96,9 +96,10 @@ const double* crepe_plan_f0(const CrepePlan* p);
 int crepe_test_conv(Engine* e, int backend, int F, int Win, int Cin, int Cout, int k, const float* x, const float* W, const float* bias, float* y);
 int crepe_test_network(Engine* e, int backend, const float* audio16k, int n, double step_ms, float* activation, int* path, int* voicing,
                        int repeat, float* ms_per_run);
+// side (only while st is being captured into a graph): D4C becomes a branch of its own, concurrent with CheapTrick
 int spectral_analysis_run(Engine* e, const float* d_x, int n, int fs, double frame_period, const double* d_f0, int n_out,
                           int fft_size, int order, float* d_sp, float* d_ap, float* d_mc, float* d_f0_out, uint8_t* d_voiced,
-                          cudaStream_t st);
+                          cudaStream_t st, cudaStream_t side = nullptr);
 
 // world_synth.cu: offline Synthesis() (pyworld.synthesize) and the output silence gate
 int world_synthesize_run(Engine* e, const double* f0, int n_frames, const float* sp, const float* ap, int fs, double frame_period_ms,

@@ -12,8 +12,9 @@
 //   converted window (n_feat + 2 e_dec frames of f0/ap/sp)                      -> realtime synthesizer -> NaN scrub
 //
 // Pipelining = what run.py does with three OS processes and queues (run.py:58-93), done with streams and events:
-//   stream E: slide wave, silence gate (needs only the samples), DIO/StoneMask (or CREPE)/CheapTrick/D4C of chunk k+1
-//   stream C: slide features, stage-1 U-Net (+f0 map), mc2sp                                          of chunk k
+//   stream E: slide wave (+ input resampler)                                                           of chunk k+1
+//   stream A: DIO/StoneMask (or CREPE), then CheapTrick || D4C (two branches of one graph)             of chunk k+1
+//   stream C: head (slide features, silence gate), then stage-1 U-Net (+f0 map), mc2sp                 of chunk k
 //   stream C2: stage-2 U-Net (the wgmma layers)                                                     of chunk k-1
 //   stream D: slide converted features, synthesizer add/plan/pulse/overlap-add, NaN scrub             of chunk k-2
 // Inter-stage buffers are double-buffered (index = step parity); events order producer/consumer and guard reuse.
@@ -45,10 +46,11 @@ struct StageGraph {
   ~StageGraph() { reset(); }
   void reset() { if (exec) cudaGraphExecDestroy(exec); exec = nullptr; launches = 0; }
 };
-// The stage graphs of the chunks of one parity, in step order (stage 1 is the separate SWITCH graph Session::s1_switch).
+// The stage graphs of the chunks of one parity, in step order (the body of stage 1 is the separate SWITCH graph Session::s1_switch).
 struct ParityGraphs {
-  StageGraph gate;         // stream E: wave slides + silence gate
-  StageGraph analysis;     // stream A: DIO/Harvest + StoneMask, CheapTrick, D4C
+  StageGraph gate;         // stream E: wave slides (the "gate" stage of RYK_STAGE_TIMES; the silence gate itself runs in s1_head)
+  StageGraph analysis;     // stream A: DIO/Harvest + StoneMask, then CheapTrick || D4C
+  StageGraph s1_head;      // stream C: feature-window slides + silence gate (mask / index / count of the step)
   StageGraph s2_pro;       // stage-2 prologue (single session: + layer 0; group member: into the group's batched input)
   StageGraph s2_layers;    // single session: stage-2 layers 1..14
   StageGraph s2_epi;       // stage-2 epilogue (single session: layer 15 +; group member: from the group's batched output)
@@ -57,10 +59,10 @@ struct ParityGraphs {
 };
 // Events of one ring slot r = step % kRing.  Null until created, so a partly built session can be freed.
 struct StepEvents {
-  cudaEvent_t gate = nullptr;      // gate of step r done (stream E)
+  cudaEvent_t gate = nullptr;      // wave slides of step r done (stream E)
   cudaEvent_t count = nullptr;     // effective-frame count of step r copied to the host (launch bookkeeping only)
   cudaEvent_t enc = nullptr;       // analysis of step r done
-  cudaEvent_t cslide = nullptr;    // stage 1 of step r has consumed the analysis outputs
+  cudaEvent_t cslide = nullptr;    // head of stage 1 of step r done: enc_*[b] and cw_wave[g] consumed
   cudaEvent_t s1 = nullptr;        // stage 1 of step r done
   cudaEvent_t pro = nullptr;       // stage-2 prologue of step r done (group members only)
   cudaEvent_t conv = nullptr;      // stage 2 of step r done
@@ -87,6 +89,7 @@ struct Session {
   // bottleneck layers (c4-d2: 30 % of a forward's time, a few CTAs each) of one chunk overlap the GPU-filling layers of its neighbour
   cudaStream_t sC2s[2] = {nullptr, nullptr};
   cudaStream_t sA[2] = {nullptr, nullptr};   // WORLD analysis of even / odd chunks: two chunks' analyses may be in flight
+  cudaStream_t sA_side = nullptr;            // D4C branch of the analysis graphs while they are captured; never used at step time
   std::array<cudaStream_t, 7> streams() const { return {sE, sA[0], sA[1], sC, sC2s[0], sC2s[1], sD}; }
   StepEvents ev[kRing];
   // sliding windows, double-buffered by step parity
@@ -274,6 +277,7 @@ static Session* get_session(Engine* e, int id) { return (id >= 0 && id < (int)e-
 static void session_free(Session* s) {
   if (!s) return;
   for (cudaStream_t st : s->streams()) if (st) { cudaStreamSynchronize(st); cudaStreamDestroy(st); }
+  if (s->sA_side) cudaStreamDestroy(s->sA_side);
   for (StepEvents& ev : s->ev)
     for (cudaEvent_t* p : ev.all()) if (*p) cudaEventDestroy(*p);
   for (int b = 0; b < 2; ++b) if (s->s1_switch[b]) cudaGraphExecDestroy(s->s1_switch[b]);
@@ -421,11 +425,10 @@ static int stage1_build_switch(Engine* e, Session* s, int b) {
   return 0;
 }
 
-// Stage 1 of a chunk of parity b: slide the feature window, (gather ->) 1-D U-Net at padded length tp1 (0: no effective frame,
-// voice_changer.py:32-35 skips the net) -> scatter into the silent template + f0 map, mc2sp.  Enqueued on stream C while it is
-// captured as one body of the parity's SWITCH graph; every body is captured when the session is created so that no chunk ever
-// pays for a capture in the middle of a stream.
-static int stage1_body(Engine* e, Session* s, int b, int tp1) {
+// The head of stage 1 of a chunk of parity b: slide the feature window by the analysis outputs and run the silence gate on the
+// chunk's wave window (mask / index / count[b], which only stage 1 reads).  It is all of stage 1 that the next chunks of this parity
+// wait for: once it ran, their analysis may overwrite enc_*[b] and their wave slide cw_wave[g].
+static int stage1_head(Engine* e, Session* s, int b) {
   const int f = b, g = b ^ 1, pe = s->e_enc_frames;
   const ryk_session_config& c = s->cfg;
   SlideBatch sb; sb.n = 0;
@@ -435,6 +438,17 @@ static int stage1_body(Engine* e, Session* s, int b, int tp1) {
   slide_add<uint8_t>(sb, s->cw_voiced[f], s->enc_voiced[b] + pe, s->cw_voiced[g], s->Tw, s->n_feat, 1);
   if (slide_batch(sb, s->sC)) return -1;
   e->launches += 1;
+  return gate_mask_run(e, s->cw_wave[g], s->Tw * s->hop, c.fft_length, s->hop, c.threshold_db, s->Tw, s->d_mse, s->d_mask[b], s->d_index[b],
+                       s->d_count[b], s->sC);
+}
+
+// The rest of stage 1 of a chunk of parity b: (gather ->) 1-D U-Net at padded length tp1 (0: no effective frame, voice_changer.py:32-35
+// skips the net) -> scatter into the silent template + f0 map, mc2sp.  Enqueued on stream C while it is captured as one body of the
+// parity's SWITCH graph; every body is captured when the session is created so that no chunk ever pays for a capture in the middle of
+// a stream.
+static int stage1_body(Engine* e, Session* s, int b, int tp1) {
+  const int g = b ^ 1;
+  const ryk_session_config& c = s->cfg;
   const float* d_y = nullptr;
   if (tp1 > 0) {
     UNetPlan* p1 = nullptr;
@@ -478,10 +492,10 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
   float* d_colmin = s->d_colmin[s->group ? 0 : b];
   ParityGraphs& pg = s->graphs[b];
 
-  // ================= stream E: gate + WORLD analysis =================
+  // ================= stream E: wave slides =================
   RYK_CUDA(cudaMemcpyAsync(s->d_chunk_fixed, d_chunk_user, sizeof(float) * s->n_in, cudaMemcpyDeviceToDevice, s->sE));
   if (k >= 2) {
-    RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev[(k - 2) % kRing].s1, 0));      // mask/index/count[b]: last read by stage 1 of k-2
+    RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev[(k - 2) % kRing].cslide, 0));  // cw_wave[g]: last read by the silence gate in the head of stage 1 of k-2
     RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev[(k - 2) % kRing].enc, 0));     // wave_win[g]: last read by the analysis of k-2
   }
   if (stage_time(s, 0, 0, r, s->sE)) return -1;
@@ -497,12 +511,9 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
         if (slide<float>(s->wave_win[f], chunk, s->wave_win[g], s->Lw, s->n_wave, 1, s->sE)) return -1;
         if (slide<float>(s->cw_wave[f], s->wave_win[g] + (size_t)pe * s->hop, s->cw_wave[g], (size_t)s->Tw * s->hop, (size_t)s->n_feat * s->hop, 1, s->sE)) return -1;
         e->launches += 2;
-        return gate_mask_run(e, s->cw_wave[g], s->Tw * s->hop, c.fft_length, s->hop, c.threshold_db, s->Tw, s->d_mse, s->d_mask[b], s->d_index[b],
-                             s->d_count[b], s->sE);
+        return 0;
       })) return -1;
   if (stage_time(s, 0, 1, r, s->sE)) return -1;
-  RYK_CUDA(cudaMemcpyAsync(s->h_count[r], s->d_count[b], sizeof(int) * 2, cudaMemcpyDeviceToHost, s->sE));
-  RYK_CUDA(cudaEventRecord(s->ev[r].count, s->sE));
   RYK_CUDA(cudaEventRecord(s->ev[r].gate, s->sE));
 
   // ================= stream A[b]: WORLD analysis (the chunks of one parity share a plan and a stream) =================
@@ -523,18 +534,24 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
         }
         const int n_enc = s->Lw / s->hop;
         return spectral_analysis_run(e, s->wave_win[g], s->Lw, c.fs, c.frame_period_ms, d_f0, n_enc, c.fft_length, c.order,
-                                     s->enc_sp[b], s->enc_ap[b], s->enc_mc[b], s->enc_f0[b], s->enc_voiced[b], sA);
+                                     s->enc_sp[b], s->enc_ap[b], s->enc_mc[b], s->enc_f0[b], s->enc_voiced[b], sA, s->sA_side);
       })) return -1;
   if (stage_time(s, 1, 1, r, sA)) return -1;
   RYK_CUDA(cudaEventRecord(s->ev[r].enc, sA));
 
-  // ================= stream C: stage 1 (+ f0 map, mc2sp) =================
-  RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[r].enc, 0));
+  // ================= stream C: stage 1 (head: feature slides + silence gate; then U-Net, f0 map, mc2sp) =================
+  // mask / index / count[b] are written by the head and read by the SWITCH graph, both on stream C: no guard between steps needed
+  RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[r].enc, 0));                       // (the analysis of step r waited for its wave slides)
+  if (stage_time(s, 2, 0, r, s->sC)) return -1;
+  if (run_graph(e, pg.s1_head, s->sC, [&]() -> int { return stage1_head(e, s, b); })) return -1;
+  // the next chunks of this parity wait only for the head, so stage 1's U-Net is off the gate -> analysis -> stage 1 recurrence
+  RYK_CUDA(cudaEventRecord(s->ev[r].cslide, s->sC));
+  RYK_CUDA(cudaMemcpyAsync(s->h_count[r], s->d_count[b], sizeof(int) * 2, cudaMemcpyDeviceToHost, s->sC));
+  RYK_CUDA(cudaEventRecord(s->ev[r].count, s->sC));
   if (k >= 2) {
     RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[(k - 2) % kRing].dslide, 0));   // cv_{f0,ap,voiced}_out[b] consumed by decode k-2
     RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[(k - 2) % kRing].conv, 0));     // cv_sp_mid[b] consumed by stage 2 of k-2
   }
-  if (stage_time(s, 2, 0, r, s->sC)) return -1;
   // launch-count bookkeeping only (never waits): the newest count that has already arrived tells which body ran last
   for (int back = 1; back <= 3 && k - back >= 0; ++back) {
     const int rr = (int)((k - back) % kRing);
@@ -543,10 +560,7 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
   if (s->last_bucket < 0 || s->last_bucket >= s->s1_buckets) s->last_bucket = s->s1_buckets - 1;
   RYK_CUDA(cudaGraphLaunch(s->s1_switch[b], s->sC));
   e->launches += s->s1_switch_launches[b][s->last_bucket];
-  // NB: enc_*[b] may be overwritten by encode k+2 once this stage's slides ran; the stage-1 graph is short, so the
-  // guard event is simply the end of the stage.
   if (stage_time(s, 2, 1, r, s->sC)) return -1;
-  RYK_CUDA(cudaEventRecord(s->ev[r].cslide, s->sC));
   RYK_CUDA(cudaEventRecord(s->ev[r].s1, s->sC));
 
   // ================= stream C2: stage-2 prologue =================
@@ -774,6 +788,7 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
   RYK_CUDA(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));      // lo = least (numerically largest), hi = greatest
   RYK_CUDA(cudaStreamCreateWithPriority(&s->sE, cudaStreamNonBlocking, prio_hi));
   for (int i = 0; i < 2; ++i) RYK_CUDA(cudaStreamCreateWithPriority(&s->sA[i], cudaStreamNonBlocking, prio_hi));
+  RYK_CUDA(cudaStreamCreateWithPriority(&s->sA_side, cudaStreamNonBlocking, prio_hi));
   RYK_CUDA(cudaStreamCreateWithPriority(&s->sC, cudaStreamNonBlocking, prio_hi));
   for (int i = 0; i < 2; ++i) RYK_CUDA(cudaStreamCreateWithPriority(&s->sC2s[i], cudaStreamNonBlocking, prio_lo));
   RYK_CUDA(cudaStreamCreateWithPriority(&s->sD, cudaStreamNonBlocking, prio_hi));
@@ -1139,8 +1154,8 @@ int ryk_group_push_device(ryk_engine* h, int group_id, const float* const* waves
 }
 
 // Diagnostics (RYK_STAGE_TIMES=1 at session creation): device timeline of the last min(steps, 8) steps.  start/end[i*5 + a] =
-// ms since the oldest listed step began, for stage a in {gate+slides, WORLD analysis, stage 1 (+mc2sp), stage 2
-// (prologue..epilogue), synthesis}; returns the number of steps listed (oldest first).
+// ms since the oldest listed step began, for stage a in {wave slides (+ input resampler), WORLD analysis, stage 1 (feature slides +
+// silence gate, U-Net, mc2sp), stage 2 (prologue..epilogue), synthesis}; returns the number of steps listed (oldest first).
 int ryk_session_stage_times(ryk_engine* h, int id, float* start, float* end) {
   Engine* e = &h->impl;
   Session* s = get_session(e, id);

@@ -195,25 +195,45 @@ __device__ inline double stonemask_fix(const double* power, const double* numer,
   return num / (den + kSafeMin);
 }
 
-// one CTA per frame; smem: 2 * 4096 double2 (main / diff spectra) + 2 * 2049 doubles
+// StoneMask's window half length and FFT size for an f0 estimate f0i (40 < f0i <= fs / 12).  WORLD's size is
+// 2^(2 + floor(log2(2 half + 1))); 2 half + 1 is odd, never a power of two, so the integer bit length gives the same floor as
+// log() / log(2) in any rounding, on the host and on the device alike.
+__host__ __device__ inline int stonemask_half(int fs, double f0i) { return (int)(1.5 * fs / f0i + 1.0); }
+__host__ __device__ inline int stonemask_fft_size(int half) {
+  const unsigned m = 2u * (unsigned)half + 1u;
+  int lg = 0;
+  while (m >> (lg + 1)) ++lg;
+  return 1 << (2 + lg);
+}
+// The largest FFT k_stonemask can form on a plan whose f0 contour is 0 or >= f0_min: the half length falls as f0i grows (correctly
+// rounded division and the truncation are monotonic), and the kernel skips f0i <= 40, so f0_min below 40 bounds nothing.  The shared-
+// memory FFT stops at kTwiddleN points; a frame that would need more (only from 27.3 kHz up, with f0 near 40 Hz) keeps its estimate.
+static int stonemask_max_fft(int fs, double f0_min) {
+  const int n = stonemask_fft_size(stonemask_half(fs, f0_min > 40.0 ? f0_min : 40.0));
+  return n < kTwiddleN ? n : kTwiddleN;
+}
+static size_t stonemask_smem_bytes(int max_fft) { return sizeof(double2) * 2 * max_fft + sizeof(double) * 2 * (max_fft / 2 + 1) + 64; }
+
+// one CTA per frame; smem: 2 * max_fft double2 (main / diff spectra) + 2 * (max_fft / 2 + 1) doubles, max_fft from stonemask_max_fft
 __global__ void __launch_bounds__(256) k_stonemask(const float* __restrict__ x, int x_length, int fs, double frame_period,
                                                   const double* __restrict__ f0_in, double* __restrict__ f0_out,
-                                                  const double2* __restrict__ tw) {
+                                                  const double2* __restrict__ tw, int max_fft) {
   extern __shared__ double2 sm2[];
   int frame = blockIdx.x;
   double f0i = f0_in[frame];
   if (f0i <= 40.0 || f0i > fs / 12.0) { if (threadIdx.x == 0) f0_out[frame] = 0.0; return; }
   double pos = frame * frame_period / 1000.0;
-  int half = (int)(1.5 * fs / f0i + 1.0);
+  int half = stonemask_half(fs, f0i);
   double wlen_time = (2.0 * half + 1.0) / fs;
   int blen = half * 2 + 1;
-  // NB: device pow() is not exact for integer powers (2 ulp): a truncated 2047 would wreck the FFT. Shift instead.
-  int fft_size = 1 << (2 + (int)(log(half * 2.0 + 1.0) / kLog2));
+  int fft_size = stonemask_fft_size(half);
+  // cannot happen for a contour within the plan's f0 range below 27.3 kHz (stonemask_max_fft); never write past the smem
+  if (fft_size > max_fft) { if (threadIdx.x == 0) f0_out[frame] = f0i; return; }
   int lg = ilog2(fft_size);
   double2* A = sm2;                 // main
-  double2* B = sm2 + 4096;          // diff
-  double* power = (double*)(sm2 + 8192);
-  double* numer = power + 2049;
+  double2* B = sm2 + max_fft;       // diff
+  double* power = (double*)(sm2 + 2 * max_fft);
+  double* numer = power + max_fft / 2 + 1;
   int basic_index = matlab_round((pos + (double)(-half) / fs) * fs + 0.001);
   auto mainw = [&](int i) {
     double tmp = ((basic_index + i) - 1.0) / fs - pos;
@@ -449,48 +469,60 @@ __device__ inline void d4c_centroid_smem(double2* A, int fft_size, int lg, const
   __syncthreads();
 }
 
-// bitonic sort (ascending) of v[0..n2) in smem, n2 power of two.  Warp w owns the contiguous segment [seg w, seg (w + 1)): every
-// compare-exchange with distance j < seg stays inside one warp's segment and needs only __syncwarp(); block barriers remain for the
-// log2(n2 / seg) widest distances of each merge (n2 = 2048, 16 warps: 15 block barriers instead of 67; same network, same result).
-__device__ inline void bitonic_sort_smem(double* v, int n2) {
-  const int nw = blockDim.x >> 5, w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  const int seg = n2 / nw;
-  if (seg < 32 || seg * nw != n2) {           // small arrays: the plain one-barrier-per-stage form
-    for (int k = 2; k <= n2; k <<= 1) {
-      for (int j = k >> 1; j > 0; j >>= 1) {
-        __syncthreads();
-        for (int i = threadIdx.x; i < n2; i += blockDim.x) {
-          int ixj = i ^ j;
-          if (ixj > i) {
-            double a = v[i], b = v[ixj];
-            bool up = (i & k) == 0;
-            if ((a > b) == up) { v[i] = b; v[ixj] = a; }
-          }
+// Sums of the `need` smallest of v[0..n) and of all n values (1 <= need <= n; v >= 0 in smem), without sorting.  The bit patterns of
+// non-negative doubles order like their values, so a radix select over them, 8 bits per pass from the top, finds t = the need-th
+// smallest value; it stops early once one candidate is left.  sum_lo = sum(v < t) + (copies of t among the need smallest) * t is the
+// same multiset sum as a cumulative sum over the sorted values, only in another order.  hist: 256 ints, sel: 4 ints (smem).
+__device__ inline void select_sums_smem(const double* v, int n, int need, unsigned* hist, unsigned* sel, double* scratch,
+                                        double* sum_lo, double* sum_all) {
+  unsigned long long prefix = 0, mask = 0;
+  unsigned k = (unsigned)need;          // rank of t among the values that match prefix under mask
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0;
+    __syncthreads();
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      const unsigned long long u = (unsigned long long)__double_as_longlong(v[i]);
+      if ((u & mask) == prefix) atomicAdd(&hist[(u >> shift) & 255], 1u);
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {             // warp 0: the bin that holds rank k (lane l owns bins 8 l .. 8 l + 7)
+      const int l = threadIdx.x;
+      unsigned c[8], own = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { c[j] = hist[l * 8 + j]; own += c[j]; }
+      unsigned incl = own;
+#pragma unroll
+      for (int off = 1; off < 32; off <<= 1) {
+        const unsigned y = __shfl_up_sync(0xffffffffu, incl, off);
+        if (l >= off) incl += y;
+      }
+      unsigned run = incl - own;
+      if (run < k && k <= incl) {
+        for (int j = 0; j < 8; ++j) {
+          if (k <= run + c[j]) { sel[0] = l * 8 + j; sel[1] = k - run; sel[2] = c[j]; break; }
+          run += c[j];
         }
       }
     }
     __syncthreads();
-    return;
+    const unsigned digit = sel[0], cnt = sel[2];
+    k = sel[1];
+    prefix |= (unsigned long long)digit << shift;
+    mask |= 255ull << shift;
+    if (cnt == 1) break;                // block-uniform: read from smem
   }
+  // t = the candidate left (unique), or every candidate (all equal once the mask is full)
   __syncthreads();
-  bool prev_block = false;
-  for (int k = 2; k <= n2; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      const bool block_stage = j >= seg;
-      if (block_stage || prev_block) __syncthreads(); else __syncwarp();
-      prev_block = block_stage;
-      for (int m = 0; m < seg; m += 32) {
-        const int i = seg * w + m + l;
-        const int ixj = i ^ j;
-        if (ixj > i) {
-          double a = v[i], b = v[ixj];
-          bool up = (i & k) == 0;
-          if ((a > b) == up) { v[i] = b; v[ixj] = a; }
-        }
-      }
-    }
-  }
+  for (int i = threadIdx.x; i < n; i += blockDim.x)
+    if (((unsigned long long)__double_as_longlong(v[i]) & mask) == prefix) scratch[0] = v[i];
   __syncthreads();
+  const double t = scratch[0];
+  double lo = 0.0, all = 0.0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) { const double x = v[i]; all += x; if (x < t) lo += x; }
+  // the values below t are need - k of the need smallest; k copies of t complete them
+  const double s_lo = block_sum(lo, scratch);
+  *sum_all = block_sum(all, scratch);
+  *sum_lo = s_lo + (double)k * t;
 }
 
 // one CTA (512 threads) per frame
@@ -566,7 +598,7 @@ __global__ void __launch_bounds__(512) k_d4c(const float* __restrict__ x, int x_
   const int half_wl = window_length / 2;
   const int boundary = matlab_round(fft_d4c * 8.0 / window_length);
   double* coarse = t2;                // nap + 2 values
-  double* srt = (double*)A;           // 2*maxfft doubles available; sort buffer of 2048
+  unsigned* hist = (unsigned*)A;      // selection histogram (256) + result (4): A is free once the power spectrum is in t1
   if (threadIdx.x == 0) { coarse[0] = -60.0; coarse[nap + 1] = -kSafeMin; }
   for (int b = 0; b < nap; ++b) {
     int center = (int)(3000.0 * (b + 1) * fft_d4c / fs);
@@ -581,17 +613,12 @@ __global__ void __launch_bounds__(512) k_d4c(const float* __restrict__ x, int x_
       A[i] = make_double2(v, 0.0);
     }
     fft_smem(A, fft_d4c, lg, -1, tw);
-    // power spectrum -> t1 (hb values), then sort in srt (padded to pow2 with +inf)
+    // power spectrum -> t1 (hb values); WORLD sorts it and takes the cumulative sums at fft / 2 - boundary - 1 and fft / 2 (= all):
+    // the sum of all but the boundary + 1 largest values, and the sum of all of them
     for (int i = threadIdx.x; i < hb; i += blockDim.x) { double2 v = A[i]; t1[i] = v.x * v.x + v.y * v.y; }
     __syncthreads();
-    int n2 = 1; while (n2 < hb) n2 <<= 1;
-    for (int i = threadIdx.x; i < n2; i += blockDim.x) srt[i] = i < hb ? t1[i] : INFINITY;
-    bitonic_sort_smem(srt, n2);
-    // cumulative sums at two indices
-    int idx_a = fft_d4c / 2 - boundary - 1, idx_b = fft_d4c / 2;
-    double pa = 0.0, pb = 0.0;
-    for (int i = threadIdx.x; i <= idx_b; i += blockDim.x) { double v = srt[i]; pb += v; if (i <= idx_a) pa += v; }
-    double sa = block_sum(pa, scratch), sb = block_sum(pb, scratch);
+    double sa, sb;
+    select_sums_smem(t1, hb, fft_d4c / 2 - boundary, hist, hist + 256, scratch, &sa, &sb);
     if (threadIdx.x == 0) {
       double ca = 10 * log10(sa / sb);
       coarse[1 + b] = fmin(0.0, ca + (cf0 - 100) / 50.0);
@@ -635,6 +662,7 @@ struct DioPlan {
   double* d_cand = nullptr; double* d_score = nullptr; double* d_scratch = nullptr; int* d_iscratch = nullptr;
   double* d_f0 = nullptr; double* d_f0r = nullptr;
   HarvestPlan* harvest = nullptr;          // f0 method 1: Harvest writes d_f0 instead of DIO
+  int sm_fft = 0;                          // largest FFT k_stonemask can form on this plan's f0 contours (its smem stride)
 };
 
 
@@ -654,6 +682,9 @@ int dio_plan_create(Engine* e, int n, int fs, double frame_period, double f0_flo
   DioPlan* p = new DioPlan();
   if (f0_method == 1 && harvest_plan_create(e, n, fs, frame_period, f0_floor, f0_ceil, &p->harvest)) { delete p; return -1; }
   p->n = n; p->fs = fs; p->frame_period = frame_period; p->f0_floor = f0_floor; p->f0_ceil = f0_ceil;
+  // DIO's contour is 0 or a band candidate >= f0_floor (k_dio_candidates zeroes the rest; the repair only copies candidates).  Harvest's
+  // lowest output is not bounded by f0_floor in a way this code shows, so its plans keep the bound of k_stonemask itself (40 Hz).
+  p->sm_fft = stonemask_max_fft(fs, f0_method == 1 ? 40.0 : f0_floor);
   p->nbands = 1 + (int)(log(f0_ceil / f0_floor) / kLog2 * 2.0);
   std::vector<double> boundary(p->nbands);
   std::vector<int> half_avg(p->nbands);
@@ -701,10 +732,10 @@ int dio_plan_create(Engine* e, int n, int fs, double frame_period, double f0_flo
 
 // DIO + StoneMask: x (device float32, n samples) -> plan->d_f0r (double, f0_length frames). Stream-ordered, no sync.
 int dio_stonemask_run(Engine* e, DioPlan* p, const float* d_x, cudaStream_t st) {
-  const size_t sm_smem = sizeof(double2) * 8192 + sizeof(double) * 2 * 2049 + 64;
+  const size_t sm_smem = stonemask_smem_bytes(p->sm_fft);
   if (p->harvest) {                                  // Harvest replaces DIO as the contour StoneMask refines
     if (harvest_run(e, p->harvest, d_x, p->d_f0, st)) return -1;
-    k_stonemask<<<p->f0_length, 256, sm_smem, st>>>(d_x, p->n, p->fs, p->frame_period, p->d_f0, p->d_f0r, e->d_twiddle);
+    k_stonemask<<<p->f0_length, 256, sm_smem, st>>>(d_x, p->n, p->fs, p->frame_period, p->d_f0, p->d_f0r, e->d_twiddle, p->sm_fft);
     RYK_CUDA(cudaGetLastError());
     return 0;
   }
@@ -723,8 +754,7 @@ int dio_stonemask_run(Engine* e, DioPlan* p, const float* d_x, cudaStream_t st) 
       p->d_boundary, p->d_cand, p->d_score);
   k_dio_fix<<<1, 256, 0, st>>>(p->d_cand, p->d_score, p->nbands, p->f0_length, p->frame_period, p->f0_floor, p->d_scratch,
                                p->d_iscratch, p->d_f0);
-  size_t smem = sizeof(double2) * 8192 + sizeof(double) * 2 * 2049 + 64;
-  k_stonemask<<<p->f0_length, 256, smem, st>>>(d_x, p->n, p->fs, p->frame_period, p->d_f0, p->d_f0r, e->d_twiddle);
+  k_stonemask<<<p->f0_length, 256, sm_smem, st>>>(d_x, p->n, p->fs, p->frame_period, p->d_f0, p->d_f0r, e->d_twiddle, p->sm_fft);
   RYK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -756,19 +786,36 @@ int analysis_kernels_init() {
 }
 
 // CheapTrick(+sp2mc) and D4C on the refined f0 in d_f0 (double, >= n_out frames). Stream-ordered.
+// Both read only the wave and the f0 and write disjoint outputs.  With a side stream (st being captured) D4C is forked onto it and
+// joined back, so the captured graph holds CheapTrick (+ f0 out) and D4C as two concurrent branches; otherwise they run in turn on st.
 int spectral_analysis_run(Engine* e, const float* d_x, int n, int fs, double frame_period, const double* d_f0, int n_out,
                           int fft_size, int order, float* d_sp, float* d_ap, float* d_mc, float* d_f0_out, uint8_t* d_voiced,
-                          cudaStream_t st) {
+                          cudaStream_t st, cudaStream_t side) {
   RYK_CHECK(fft_size <= kCtMaxFft && fft_size >= 64, "unsupported CheapTrick fft size");
   RYK_CHECK(e->d_G != nullptr && e->G_order == order && e->G_fft == fft_size, "sp2mc matrix not prepared for this (order, fft)");
   if (n_out <= 0) return 0;
-  k_cheaptrick<<<n_out, 256, cheaptrick_smem_bytes(fft_size, fs), st>>>(d_x, n, fs, frame_period, d_f0, fft_size, -0.15, e->d_G, order,
-                                                                      n_out, d_sp, d_mc, nullptr, e->d_twiddle);
   const int fft_d4c = (int)pow(2.0, 1.0 + (int)(log(4.0 * fs / 47.0 + 1) / kLog2));   // host pow: exact
   const int lt_fft = (int)pow(2.0, 1.0 + (int)(log(3.0 * fs / 40.0 + 1) / kLog2));
-  k_d4c<<<n_out, 512, d4c_smem_bytes(fs), st>>>(d_x, n, fs, frame_period, d_f0, fft_size, 0.85, n_out, d_ap, e->d_twiddle, fft_d4c, lt_fft);
+  cudaEvent_t fork = nullptr, join = nullptr;
+  cudaStream_t sd = st;
+  if (side) {
+    RYK_CUDA(cudaEventCreateWithFlags(&fork, cudaEventDisableTiming));
+    RYK_CUDA(cudaEventCreateWithFlags(&join, cudaEventDisableTiming));
+    RYK_CUDA(cudaEventRecord(fork, st));
+    RYK_CUDA(cudaStreamWaitEvent(side, fork, 0));
+    sd = side;
+  }
+  k_d4c<<<n_out, 512, d4c_smem_bytes(fs), sd>>>(d_x, n, fs, frame_period, d_f0, fft_size, 0.85, n_out, d_ap, e->d_twiddle, fft_d4c, lt_fft);
+  k_cheaptrick<<<n_out, 256, cheaptrick_smem_bytes(fft_size, fs), st>>>(d_x, n, fs, frame_period, d_f0, fft_size, -0.15, e->d_G, order,
+                                                                      n_out, d_sp, d_mc, nullptr, e->d_twiddle);
   k_f0_out<<<(n_out + 127) / 128, 128, 0, st>>>(d_f0, n_out, d_f0_out, d_voiced);
   RYK_CUDA(cudaGetLastError());
+  if (side) {
+    RYK_CUDA(cudaEventRecord(join, side));
+    RYK_CUDA(cudaStreamWaitEvent(st, join, 0));
+    RYK_CUDA(cudaEventDestroy(fork));           // the captured graph keeps the dependencies, not the events
+    RYK_CUDA(cudaEventDestroy(join));
+  }
   return 0;
 }
 
