@@ -52,14 +52,18 @@ int ryk_engine_get_precision(ryk_engine* e);
  * kernel (default, s1_fused.cu) or as 16 layer launches (enable = 0).  Returns the cluster size in use, <= 0 when the kernel is
  * unavailable.  Sessions capture their stage-1 graphs at creation, so switch before ryk_session_create. */
 int ryk_engine_set_stage1_fused(ryk_engine* e, int enable);
-long long ryk_engine_launch_count(ryk_engine* e);        /* kernels launched by this engine so far */
+/* Kernels run by the steps of this engine's sessions and groups so far: the kernel nodes of every stage graph a step launches
+ * (cuFFT's included), the kernels of the stage-1 body the device selected, and the synthesizer's noise top-up.  The per-op calls
+ * below and re-blocker pushes are not counted.  Synchronises the device; -1 on a CUDA error. */
+long long ryk_engine_launch_count(ryk_engine* e);
 int ryk_engine_synchronize(ryk_engine* e);
 /* CUDA-event timing of the stage-2 k4-layer block (layers 1..14, the wgmma kernel) on the engine's stream */
 int ryk_engine_timer_start(ryk_engine* e);                    /* cudaEventRecord on the engine's stream */
 int ryk_engine_timer_stop(ryk_engine* e, float* elapsed_ms);  /* record + synchronize + elapsed */
+/* Time the stage-2 forwards of session and group steps (only those; per-op calls are never timed) */
 int ryk_engine_profile(ryk_engine* e, int enable);
-/* Device time (ms) of the stage-2 k4-layer block over all forwards since the last read: the sum of the per-forward durations and
- * the UNION of the per-forward intervals (a session alternates its stage-2 forwards between two streams, so they overlap) */
+/* Device time (ms) of the stage-2 k4-layer block over all session and group forwards since the last read: the sum of the per-forward
+ * durations and the UNION of the per-forward intervals (a session alternates its stage-2 forwards between two streams, so they overlap) */
 int ryk_engine_profile_read2(ryk_engine* e, double* stage2_ms_total, double* stage2_ms_union, int* stage2_runs);
 
 /* ---- WORLD analysis (encode) -------------------------------------------------------------- */

@@ -166,6 +166,8 @@ int ryk_engine_create(int device, ryk_engine** out) {
   if (tc_init()) return -1;
   if (s1_fused_init()) return -1;
   RYK_CUDA(cudaMalloc(&e->d_colmin, sizeof(float) * 64 * 512));   // stage-2 prologue scratch (never allocated inside a graph capture)
+  RYK_CUDA(cudaMalloc(&e->d_launches, sizeof(*e->d_launches)));
+  RYK_CUDA(cudaMemset(e->d_launches, 0, sizeof(*e->d_launches)));
   *out = h;
   return 0;
 }
@@ -180,7 +182,7 @@ int ryk_engine_destroy(ryk_engine* h) {
   for (Synth* s : e->synths) synth_destroy(s);
   session_destroy_all(e);
   crepe_destroy();                                  // after the sessions: their CREPE plans are counted on the model
-  void* ptrs[] = {e->d_colmin, e->d_twiddle, e->d_jump, e->d_G, e->d_H, e->d_s1_in_mean, e->d_s1_in_std, e->d_s1_out_mean, e->d_s1_out_std, e->d_scratch};
+  void* ptrs[] = {e->d_colmin, e->d_launches, e->d_twiddle, e->d_jump, e->d_G, e->d_H, e->d_s1_in_mean, e->d_s1_in_std, e->d_s1_out_mean, e->d_s1_out_std, e->d_scratch};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (e->h_pinned) cudaFreeHost(e->h_pinned);
   cudaStreamDestroy(e->stream);
@@ -197,7 +199,15 @@ int ryk_engine_get_precision(ryk_engine* h) { return E(h)->precision; }
 // Stage 1 as one cluster kernel (default) or as the 16-layer sequence; returns the cluster size in use (<= 0: kernel unavailable).
 // Sessions capture their stage-1 graphs at creation: switch before creating them.
 int ryk_engine_set_stage1_fused(ryk_engine* h, int enable) { E(h)->s1_fused = enable != 0; return s1_fused_cluster_size(); }
-long long ryk_engine_launch_count(ryk_engine* h) { return E(h)->launches; }
+// Synchronises the device: the kernels of the stage-1 SWITCH bodies are counted on the device.
+long long ryk_engine_launch_count(ryk_engine* h) {
+  Engine* e = E(h);
+  unsigned long long device_count = 0;
+  RYK_CUDA(cudaSetDevice(e->device));
+  RYK_CUDA(cudaDeviceSynchronize());
+  RYK_CUDA(cudaMemcpy(&device_count, e->d_launches, sizeof(device_count), cudaMemcpyDeviceToHost));
+  return e->launches + (long long)device_count;
+}
 int ryk_engine_synchronize(ryk_engine* h) { RYK_CUDA(cudaSetDevice(E(h)->device)); RYK_CUDA(cudaDeviceSynchronize()); return 0; }
 
 int ryk_engine_profile(ryk_engine* h, int enable) { E(h)->profile = enable != 0; return 0; }
@@ -265,7 +275,6 @@ int ryk_world_f0(ryk_engine* h, const float* wave, int n, int fs, double fp, dou
   float* d_x = (float*)scratch;
   RYK_CUDA(cudaMemcpyAsync(d_x, wave, sizeof(float) * n, cudaMemcpyHostToDevice, e->stream));
   if (dio_stonemask_run(e, plan, d_x, e->stream)) return -1;
-  e->launches += 9;
   int nf = dio_plan_frames(plan);
   RYK_CUDA(cudaMemcpyAsync(f0, dio_plan_f0(plan), sizeof(double) * nf, cudaMemcpyDeviceToHost, e->stream));
   RYK_CUDA(cudaStreamSynchronize(e->stream));
@@ -302,10 +311,8 @@ int ryk_world_analyze(ryk_engine* h, const float* wave, int n, int fs, double fp
     RYK_CUDA(cudaMemcpyAsync(dio_plan_f0_mut(plan), f0_override, sizeof(double) * dio_plan_frames(plan), cudaMemcpyHostToDevice, e->stream));
   } else {
     if (dio_stonemask_run(e, plan, d_x, e->stream)) return -1;
-    e->launches += 9;
   }
   if (spectral_analysis_run(e, d_x, n, fs, fp, dio_plan_f0(plan), n_out, fft_length, order, d_sp, d_ap, d_mc, d_f0, d_v, e->stream)) return -1;
-  e->launches += 3;
   if (f0) RYK_CUDA(cudaMemcpyAsync(f0, d_f0, sizeof(float) * n_out, cudaMemcpyDeviceToHost, e->stream));
   if (sp) RYK_CUDA(cudaMemcpyAsync(sp, d_sp, sizeof(float) * n_out * nb, cudaMemcpyDeviceToHost, e->stream));
   if (ap) RYK_CUDA(cudaMemcpyAsync(ap, d_ap, sizeof(float) * n_out * nb, cudaMemcpyDeviceToHost, e->stream));
@@ -403,7 +410,6 @@ int ryk_stage1_convert(ryk_engine* h, const float* x, int T, float* y) {
   if (stage1_prologue_run(e, d_x, nullptr, d_count, C, (float*)plan->d_in, Tp, e->stream)) return -1;
   if (unet_forward(e, plan, e->stream)) return -1;
   k_affine_rows<<<(T * Co + 255) / 256, 256, 0, e->stream>>>((const float*)plan->d_out, T, Co, e->d_s1_out_std, e->d_s1_out_mean, d_y);
-  e->launches++;
   RYK_CUDA(cudaMemcpyAsync(y, d_y, sizeof(float) * T * Co, cudaMemcpyDeviceToHost, e->stream));
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   return 0;
@@ -421,7 +427,6 @@ int ryk_f0_convert(ryk_engine* h, const float* f0, const uint8_t* voiced, int T,
   RYK_CUDA(cudaMemcpyAsync(d_v, voiced, T, cudaMemcpyHostToDevice, e->stream));
   k_f0_convert<<<(T + 127) / 128, 128, 0, e->stream>>>(d_f0, d_v, T, e->f0_in_mean, e->f0_in_std, e->f0_tgt_mean, e->f0_tgt_std,
                                                       e->has_f0_stats ? 1 : 0, d_o);
-  e->launches++;
   RYK_CUDA(cudaMemcpyAsync(out, d_o, sizeof(float) * T, cudaMemcpyDeviceToHost, e->stream));
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   return 0;

@@ -426,14 +426,13 @@ static int crepe_conv(Engine* e, CrepeModel* m, const CrepeWork& w, int l, const
     CrepeGemm g;
     g.x = x; g.M = F * Wout; g.W = Wout; g.fstride = (long long)Win * Cin; g.wstep = Cin; g.K = KW * Cin; g.N = m->cout[l];
     g.w = m->d_w[l]; g.bias = m->d_bias[l]; g.y = y;
-    return crepe_tc_run(g, w.d_tc_ws, st, &e->launches);
+    return crepe_tc_run(g, w.d_tc_ws, st);
   }
   ConvLayer L;
   L.transposed = 0; L.B = F; L.Hin = 1; L.Win = Win; L.Hout = 1; L.Wout = Wout; L.C0 = Cin; L.C1 = 0; L.Cout = m->cout[l];
   L.KH = 1; L.KW = KW; L.SH = 1; L.SW = 1; L.PH = 0; L.PW = 0; L.act = ACT_RELU;
   L.in0 = x; L.in_dtype = DT_F32; L.out = y; L.out_dtype = DT_F32;
   L.w_direct = m->d_w[l]; L.scale = m->d_ones; L.shift = m->d_bias[l];
-  e->launches += 1;
   return conv_direct_run(L, st);
 }
 
@@ -448,7 +447,6 @@ static int crepe_network(Engine* e, CrepeModel* m, CrepeWork& w, int n16, int ho
   int n_out, left, right;
   same_padding(1024, 512, 4, &n_out, &left, &right);                 // 256 outputs, 254 + 254
   k_crepe_frames<<<F, 256, 0, st>>>(w.d_audio, n16, hop, left, w.d_im2col);
-  e->launches += 1;
   // block 0: 1x1 conv over the im2col rows ([F][256][512] x [512][cout])
   if (crepe_conv(e, m, w, 0, w.d_im2col, F, 256, 512, 1, 256, w.d_conv[0], st)) return -1;
   int W = 256;
@@ -457,12 +455,10 @@ static int crepe_network(Engine* e, CrepeModel* m, CrepeWork& w, int n16, int ho
     if (l < 5) {
       int nl, pl, pr; same_padding(Wo, kCrepeWidths[l + 1], kCrepeStrides[l + 1], &nl, &pl, &pr);
       k_crepe_bn_pool<<<296, 256, 0, st>>>(w.d_conv[l], F, W, m->cout[l], m->d_bn_a[l], m->d_bn_c[l], pl, pr, w.d_in[l + 1]);
-      e->launches += 1;
       if (crepe_conv(e, m, w, l + 1, w.d_in[l + 1], F, Wo + pl + pr, m->cout[l], kCrepeWidths[l + 1], nl, w.d_conv[l + 1], st)) return -1;
       W = nl;
     } else {
       k_crepe_bn_pool<<<296, 256, 0, st>>>(w.d_conv[l], F, W, m->cout[l], m->d_bn_a[l], m->d_bn_c[l], 0, 0, w.d_flat);   // [F][4][C] = time-major flatten
-      e->launches += 1;
     }
   }
   {                                                                   // Dense(360): 1x1 conv over [F][1][64 m]
@@ -472,13 +468,11 @@ static int crepe_network(Engine* e, CrepeModel* m, CrepeWork& w, int n16, int ho
     L.in0 = w.d_flat; L.in_dtype = DT_F32; L.out = w.d_logit; L.out_dtype = DT_F32;
     L.w_direct = m->d_dense_w; L.scale = m->d_ones; L.shift = m->d_dense_b;
     if (conv_direct_run(L, st)) return -1;
-    e->launches += 1;
   }
   k_crepe_sigmoid<<<F, 128, 0, st>>>(w.d_logit, w.d_act, w.d_conf, w.d_obs);
   k_crepe_decode<<<1, 384, 0, st>>>(w.d_act, w.d_conf, w.d_obs, F, m->d_log_trans, m->d_cents, m->h_log_start, m->h_log_emit[0], m->h_log_emit[1],
                                    w.d_lattice, w.d_path, w.d_vlat, w.d_f0, w.d_voicing);
   RYK_CUDA(cudaGetLastError());
-  e->launches += 2;
   return 0;
 }
 
@@ -569,7 +563,6 @@ int crepe_plan_run(Engine* e, CrepePlan* p, const float* d_x, cudaStream_t st) {
   if (crepe_network(e, m, w, w.n16, p->hop16, w.F, st)) return -1;
   k_crepe_voiced<<<(w.F + 127) / 128, 128, 0, st>>>(w.d_f0, w.d_conf, w.d_voicing, w.F, p->d_f0);
   RYK_CUDA(cudaGetLastError());
-  e->launches += 1;
   return 0;
 }
 
@@ -599,7 +592,7 @@ int crepe_test_conv(Engine* e, int backend, int F, int Win, int Cin, int Cout, i
       CrepeGemm g;
       g.x = d_x; g.M = F * Wout; g.W = Wout; g.fstride = (long long)Win * Cin; g.wstep = Cin; g.K = k * Cin; g.N = Cout;
       g.w = d_w; g.bias = d_b; g.y = d_y;
-      rc = crepe_tc_run(g, d_ws, st, &e->launches);
+      rc = crepe_tc_run(g, d_ws, st);
     } else if (!rc) {
       ConvLayer L;
       L.transposed = 0; L.B = F; L.Hin = 1; L.Win = Win; L.Hout = 1; L.Wout = Wout; L.C0 = Cin; L.C1 = 0; L.Cout = Cout;

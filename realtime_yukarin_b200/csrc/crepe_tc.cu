@@ -203,7 +203,7 @@ size_t crepe_tc_ws_floats(int M, int K, int N) {
   return S > 1 ? (size_t)S * M * N : 0;
 }
 
-int crepe_tc_run(const CrepeGemm& g, float* ws, cudaStream_t st, long long* launches) {
+int crepe_tc_run(const CrepeGemm& g, float* ws, cudaStream_t st) {
   RYK_CHECK(g.M > 0 && g.N % 16 == 0 && g.K % kBK == 0 && g.wstep % 4 == 0 && g.fstride % 4 == 0,
             "CREPE tensor-core conv: Cout must be a multiple of 16, K of 32 and the row offsets of 4 floats");
   int S, per;
@@ -214,12 +214,10 @@ int crepe_tc_run(const CrepeGemm& g, float* ws, cudaStream_t st, long long* laun
   if (bn == 64) k_crepe_tc<64><<<grid, kThreads, 0, st>>>(g, per, ws);
   else if (bn == 32) k_crepe_tc<32><<<grid, kThreads, 0, st>>>(g, per, ws);
   else k_crepe_tc<16><<<grid, kThreads, 0, st>>>(g, per, ws);
-  *launches += 1;
   if (S > 1) {
     const long long MN = (long long)g.M * g.N;
     int blocks = (int)((MN + 255) / 256); if (blocks > 4 * kNumSms) blocks = 4 * kNumSms;
     k_crepe_tc_reduce<<<blocks, 256, 0, st>>>(ws, S, MN, g.N, g.bias, g.y);
-    *launches += 1;
   }
   RYK_CUDA(cudaGetLastError());
   return 0;

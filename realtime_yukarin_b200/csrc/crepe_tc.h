@@ -14,6 +14,6 @@ struct CrepeGemm {
 };
 
 size_t crepe_tc_ws_floats(int M, int K, int N);                       // split-K workspace the layer needs (0: none)
-int crepe_tc_run(const CrepeGemm& g, float* ws, cudaStream_t st, long long* launches);
+int crepe_tc_run(const CrepeGemm& g, float* ws, cudaStream_t st);
 
 }  // namespace ryk

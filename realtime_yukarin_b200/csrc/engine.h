@@ -51,10 +51,12 @@ struct Engine {
   // scratch arena for the per-op host-pointer API (grown on demand)
   void* d_scratch = nullptr; size_t scratch_bytes = 0;
   void* h_pinned = nullptr; size_t pinned_bytes = 0;
-  // counters
+  // kernels run by session and group steps (ryk_engine_launch_count): the kernel nodes of the stage graphs they launch plus the
+  // synthesizer's noise top-up; the device counter gets the kernels of the stage-1 SWITCH bodies the device selected
   long long launches = 0;
+  unsigned long long* d_launches = nullptr;
   int plan_owners = 0;               // U-Net plan owner ids handed out to sessions and groups (0 is the engine's own plans)
-  // optional device-side timing of the stage-2 tensor-core layers (bench roofline): event pairs per forward
+  // optional device-side timing of the stage-2 tensor-core layers of session and group steps (bench roofline): event pairs per forward
   bool profile = false;
   cudaEvent_t timer_ev[2] = {nullptr, nullptr};
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events;

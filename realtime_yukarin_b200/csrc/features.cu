@@ -81,7 +81,6 @@ int mc2sp_run(Engine* e, const float* d_mc, int T, int order, int fft_size, doub
   int nb = fft_size / 2 + 1;
   k_mc2sp<<<dim3((nb + 127) / 128, T), 128, 0, st>>>(d_mc, T, order, nb, e->d_H, add, d_sp32, d_sp64);
   RYK_CUDA(cudaGetLastError());
-  e->launches++;
   return 0;
 }
 
@@ -156,7 +155,6 @@ int gate_mask_run(Engine* e, const float* d_wave, int n, int frame_length, int h
   k_frame_mse<<<n_frames, 256, 0, st>>>(d_wave, n, frame_length, hop, n_frames, d_mse);
   k_gate<<<1, 1024, 0, st>>>(d_mse, n_frames, threshold_db, d_mask, d_index, d_count);
   RYK_CUDA(cudaGetLastError());
-  e->launches += 2;
   return 0;
 }
 
@@ -256,7 +254,6 @@ __global__ void k_sr_epilogue(const float* __restrict__ y, int T, int nb, int t0
 int stage1_prologue_run(Engine* e, const float* d_mc, const int* d_index, const int* d_count, int C, float* d_x, int Tp_capacity, cudaStream_t st) {
   k_stage1_prologue<<<1, 256, 0, st>>>(d_mc, d_index, d_count, C, e->d_s1_in_mean, e->d_s1_in_std, d_x, Tp_capacity);
   RYK_CUDA(cudaGetLastError());
-  e->launches++;
   return 0;
 }
 
@@ -268,7 +265,6 @@ int stage1_epilogue_run(Engine* e, const float* d_y, const int* d_index, const u
                                        d_voiced_in, nb, e->f0_in_mean, e->f0_in_std, e->f0_tgt_mean, e->f0_tgt_std,
                                        e->has_f0_stats ? 1 : 0, silent_mc0, d_mc_out, d_f0_out, d_ap_out, d_voiced_out);
   RYK_CUDA(cudaGetLastError());
-  e->launches++;
   return 0;
 }
 
@@ -282,7 +278,6 @@ int sr_prologue_run(Engine* e, const float* d_sp, int T, int Tp, int nb, float* 
   k_sr_colmin<<<dim3((nb - 1 + 127) / 128, nparts), 128, 0, st>>>(d_sp, T, nb, rows_per_block, d_colmin);
   k_sr_prologue<<<dim3((nb - 1 + 127) / 128, Tp), 128, 0, st>>>(d_sp, d_colmin, nparts, T, Tp, nb, d_x);
   RYK_CUDA(cudaGetLastError());
-  e->launches += 2;
   return 0;
 }
 
@@ -292,7 +287,6 @@ int sr_epilogue_run(Engine* e, const float* d_y, int T, int nb, float* d_sp_out,
   if (t1 == t0) return 0;
   k_sr_epilogue<<<dim3((nb + 127) / 128, t1 - t0), 128, 0, st>>>(d_y, T, nb, t0, d_sp_out);
   RYK_CUDA(cudaGetLastError());
-  e->launches++;
   return 0;
 }
 
@@ -367,7 +361,6 @@ static int resample_launch(Engine* e, const PolyArgs<Tin, Tout>& a, cudaStream_t
   if (threads <= 0) return 0;
   k_resample_poly<Tin, Tout><<<(threads + 255) / 256, 256, 0, st>>>(a);
   RYK_CUDA(cudaGetLastError());
-  e->launches++;
   return 0;
 }
 

@@ -424,7 +424,6 @@ int s1_fused_run(Engine* e, const UNetPlan* p, cudaStream_t st) {
   at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = g_s1_cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
   cfg.attrs = at; cfg.numAttrs = 1;
   RYK_CUDA(cudaLaunchKernelEx(&cfg, k_s1_fused, P));
-  e->launches += 1;
   return 0;
 }
 

@@ -39,18 +39,21 @@ constexpr int kRing = 8;          // event / output-slot ring (pipeline depth is
 
 // One captured stage of a step (see run_graph).  Destroying it drops the executable graph.
 struct StageGraph {
-  cudaGraphExec_t exec = nullptr; long long launches = 0;
+  cudaGraphExec_t exec = nullptr; long long launches = 0;       // launches: kernel nodes of the graph (one launch runs them all)
   StageGraph() = default;
   StageGraph(const StageGraph&) = delete;
   StageGraph& operator=(const StageGraph&) = delete;
   ~StageGraph() { reset(); }
   void reset() { if (exec) cudaGraphExecDestroy(exec); exec = nullptr; launches = 0; }
 };
-// The stage graphs of the chunks of one parity, in step order (the body of stage 1 is the separate SWITCH graph Session::s1_switch).
+// The stage graphs of the chunks of one parity, in step order.
 struct ParityGraphs {
   StageGraph gate;         // stream E: wave slides (the "gate" stage of RYK_STAGE_TIMES; the silence gate itself runs in s1_head)
   StageGraph analysis;     // stream A: DIO/Harvest + StoneMask, then CheapTrick || D4C
   StageGraph s1_head;      // stream C: feature-window slides + silence gate (mask / index / count of the step)
+  // stream C: the rest of stage 1 with the padded-length bucket chosen ON THE DEVICE = {k_set_bucket -> SWITCH conditional node whose
+  // body i is the stage-1 sequence for the padded length 128 i (0: no effective frame)}; built at session creation, no host sync
+  StageGraph s1;
   StageGraph s2_pro;       // stage-2 prologue (single session: + layer 0; group member: into the group's batched input)
   StageGraph s2_layers;    // single session: stage-2 layers 1..14
   StageGraph s2_epi;       // stage-2 epilogue (single session: layer 15 +; group member: from the group's batched output)
@@ -60,7 +63,6 @@ struct ParityGraphs {
 // Events of one ring slot r = step % kRing.  Null until created, so a partly built session can be freed.
 struct StepEvents {
   cudaEvent_t gate = nullptr;      // wave slides of step r done (stream E)
-  cudaEvent_t count = nullptr;     // effective-frame count of step r copied to the host (launch bookkeeping only)
   cudaEvent_t enc = nullptr;       // analysis of step r done
   cudaEvent_t cslide = nullptr;    // head of stage 1 of step r done: enc_*[b] and cw_wave[g] consumed
   cudaEvent_t s1 = nullptr;        // stage 1 of step r done
@@ -68,7 +70,7 @@ struct StepEvents {
   cudaEvent_t conv = nullptr;      // stage 2 of step r done
   cudaEvent_t dslide = nullptr;    // the converted features of step r sit in the decode window
   cudaEvent_t dec = nullptr;       // output of step r staged (after the copies the entry point appends to stream D)
-  std::array<cudaEvent_t*, 9> all() { return {&gate, &count, &enc, &cslide, &s1, &pro, &conv, &dslide, &dec}; }
+  std::array<cudaEvent_t*, 8> all() { return {&gate, &enc, &cslide, &s1, &pro, &conv, &dslide, &dec}; }
 };
 struct Group;
 struct Session {
@@ -107,14 +109,10 @@ struct Session {
   float* d_chunk[kRing]; float* h_in[kRing];
   double* d_out[kRing]; double* h_out[kRing];
   int* d_n_out[kRing]; int* h_n[kRing];
-  int* h_count[kRing];
   float* d_chunk_fixed = nullptr;      // the chunk the (captured) encode graph reads
   double* d_out_fixed[2];              // blocks written by the (captured) decode graph, by parity
   int* d_n_fixed[2];
   ParityGraphs graphs[2];
-  // stage 1 with the padded-length bucket chosen ON THE DEVICE: one graph per chunk parity = {k_set_bucket -> SWITCH conditional node
-  // whose body i is the stage-1 sequence for the padded length 128 i (0: no effective frame)}; no host sync on the submit path
-  cudaGraphExec_t s1_switch[2] = {nullptr, nullptr}; long long s1_switch_launches[2][16]; int s1_buckets = 0; int last_bucket = 0;
   Synth* synth = nullptr;
   DioPlan* dio[2] = {nullptr, nullptr};     // one analysis plan per chunk parity (owned), f0 methods 0 and 1
   CrepePlan* crepe[2] = {nullptr, nullptr}; // f0 method 2: one CREPE forward per chunk parity (owned) in place of DIO/Harvest
@@ -280,7 +278,6 @@ static void session_free(Session* s) {
   if (s->sA_side) cudaStreamDestroy(s->sA_side);
   for (StepEvents& ev : s->ev)
     for (cudaEvent_t* p : ev.all()) if (*p) cudaEventDestroy(*p);
-  for (int b = 0; b < 2; ++b) if (s->s1_switch[b]) cudaGraphExecDestroy(s->s1_switch[b]);
   if (s->stage_times) for (int a = 0; a < 5; ++a) for (int w = 0; w < 2; ++w) for (int i = 0; i < kRing; ++i) cudaEventDestroy(s->tev[a][w][i]);
   for (void* p : s->allocs) cudaFree(p);
   for (void* p : s->pinned) cudaFreeHost(p);
@@ -349,33 +346,71 @@ int session_streams_join(Engine* e) {
 // Every stage of a step is a fixed kernel sequence over fixed buffers (selected by chunk parity, and for stage 1 by the
 // padded effective length), so each variant is stream-captured once and replayed: a step costs ~6 graph launches on
 // the host instead of ~90 kernel launches (the host was the bottleneck at 0.75 ms of launch overhead per 0.78 ms step).
-// run_graph captures body() on stream st into g on first use and replays g; e->launches counts the kernels of every replay.
+
+// Kernel nodes of a graph, or -1 on a CUDA error.  cuFFT's kernels and cluster and programmatic launches are kernel nodes; memset and
+// memcpy nodes are not.  A conditional node is not either: its bodies are counted on their own (stage1_build_switch).
+static int graph_kernels(cudaGraph_t graph) {
+  size_t n = 0;
+  RYK_CUDA(cudaGraphGetNodes(graph, nullptr, &n));
+  std::vector<cudaGraphNode_t> nodes(n);
+  RYK_CUDA(cudaGraphGetNodes(graph, nodes.data(), &n));
+  int kernels = 0;
+  for (cudaGraphNode_t node : nodes) {
+    cudaGraphNodeType type;
+    if (cudaGraphNodeGetType(node, &type) != cudaSuccess) {
+      // the CUDA 12.9 runtime under a 13.0 driver cannot name a conditional node's type (cudaErrorUnknown); kernel nodes always resolve.
+      // Clear the error so that no later cudaGetLastError reports it.
+      (void)cudaGetLastError();
+      continue;
+    }
+    kernels += type == cudaGraphNodeTypeKernel;
+  }
+  return kernels;
+}
+
+// instantiate graph into g, count its kernels, destroy graph
+static int stage_graph_init(StageGraph& g, cudaGraph_t graph) {
+  const int kernels = graph_kernels(graph);
+  if (kernels < 0) return -1;
+  RYK_CUDA(cudaGraphInstantiate(&g.exec, graph, 0));
+  RYK_CUDA(cudaGraphDestroy(graph));
+  g.launches = kernels;
+  return 0;
+}
+
+// every launch of a stage graph adds its kernel nodes to e->launches
+static int stage_graph_launch(Engine* e, const StageGraph& g, cudaStream_t st) {
+  RYK_CUDA(cudaGraphLaunch(g.exec, st));
+  e->launches += g.launches;
+  return 0;
+}
+
+// run_graph captures body() on stream st into g on first use and replays g.
 template <typename F>
 static int run_graph(Engine* e, StageGraph& g, cudaStream_t st, F&& body) {
   if (!g.exec) {
-    long long before = e->launches;
     cudaGraph_t graph = nullptr;
     RYK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
     int rc = body();
     cudaError_t err = cudaStreamEndCapture(st, &graph);
     if (rc) return rc;
     RYK_CUDA(err);
-    RYK_CUDA(cudaGraphInstantiate(&g.exec, graph, 0));
-    RYK_CUDA(cudaGraphDestroy(graph));
-    g.launches = e->launches - before;
-    e->launches = before;
+    if (stage_graph_init(g, graph)) return -1;
   }
-  RYK_CUDA(cudaGraphLaunch(g.exec, st));
-  e->launches += g.launches;
-  return 0;
+  return stage_graph_launch(e, g, st);
 }
 
-// value of the SWITCH node = padded effective length / 128 (count[1] / 128), 0 when no frame is effective (count[0] == 0)
-__global__ void k_set_bucket(cudaGraphConditionalHandle handle, const int* __restrict__ count, int n_buckets) {
+struct BucketKernels { int n[16]; };     // kernel nodes of each body of a stage-1 SWITCH
+
+// value of the SWITCH node = padded effective length / 128 (count[1] / 128), 0 when no frame is effective (count[0] == 0); the kernels
+// of the selected body go to the engine's device launch counter (other sessions' setters may add at the same time)
+__global__ void k_set_bucket(cudaGraphConditionalHandle handle, const int* __restrict__ count, int n_buckets, BucketKernels kernels,
+                             unsigned long long* __restrict__ launches) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
     int v = count[0] > 0 ? count[1] / 128 : 0;
     if (v < 0 || v >= n_buckets) v = n_buckets - 1;        // cannot happen (count[1] <= Tw + 128); keeps the node in range
     cudaGraphSetConditional(handle, (unsigned)v);
+    atomicAdd(launches, (unsigned long long)kernels.n[v]);
   }
 }
 
@@ -385,21 +420,19 @@ static int stage1_body(Engine* e, Session* s, int b, int tp1);
 static int stage1_build_switch(Engine* e, Session* s, int b) {
   const int n_buckets = s->Tp / 128 + 1;
   RYK_CHECK(n_buckets <= 16, "window too long for the stage-1 graph table");
-  s->s1_buckets = n_buckets;
   cudaGraph_t graph = nullptr;
   RYK_CUDA(cudaGraphCreate(&graph, 0));
   cudaGraphConditionalHandle handle;
   RYK_CUDA(cudaGraphConditionalHandleCreate(&handle, graph, 0, cudaGraphCondAssignDefault));
-  // node 1: the setter
+  // node 1: the setter (its body table is filled in once the bodies are captured)
   cudaGraphNode_t set_node = nullptr;
-  {
-    cudaKernelNodeParams kp = {};
-    const int* cnt = s->d_count[b];
-    int nb_ = n_buckets;
-    void* args[3] = {(void*)&handle, (void*)&cnt, (void*)&nb_};
-    kp.func = (void*)k_set_bucket; kp.gridDim = dim3(1); kp.blockDim = dim3(32); kp.sharedMemBytes = 0; kp.kernelParams = args; kp.extra = nullptr;
-    RYK_CUDA(cudaGraphAddKernelNode(&set_node, graph, nullptr, 0, &kp));
-  }
+  const int* cnt = s->d_count[b];
+  int nb_ = n_buckets;
+  BucketKernels kernels = {};
+  void* args[5] = {(void*)&handle, (void*)&cnt, (void*)&nb_, (void*)&kernels, (void*)&e->d_launches};
+  cudaKernelNodeParams kp = {};
+  kp.func = (void*)k_set_bucket; kp.gridDim = dim3(1); kp.blockDim = dim3(32); kp.sharedMemBytes = 0; kp.kernelParams = args; kp.extra = nullptr;
+  RYK_CUDA(cudaGraphAddKernelNode(&set_node, graph, nullptr, 0, &kp));
   // node 2: SWITCH
   cudaGraphNodeParams cp = {};
   cp.type = cudaGraphNodeTypeConditional;
@@ -410,19 +443,17 @@ static int stage1_build_switch(Engine* e, Session* s, int b) {
   RYK_CUDA(cudaGraphAddNode(&sw, graph, &set_node, 1, &cp));
   for (int i = 0; i < n_buckets; ++i) {
     cudaGraph_t body = cp.conditional.phGraph_out[i];
-    const long long before = e->launches;
     RYK_CUDA(cudaStreamBeginCaptureToGraph(s->sC, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
     int rc = stage1_body(e, s, b, i * 128);
     cudaGraph_t out = nullptr;
     cudaError_t err = cudaStreamEndCapture(s->sC, &out);
     if (rc) return rc;
     RYK_CUDA(err);
-    s->s1_switch_launches[b][i] = e->launches - before + 1;     // + the setter
-    e->launches = before;
+    kernels.n[i] = graph_kernels(body);
+    if (kernels.n[i] < 0) return -1;
   }
-  RYK_CUDA(cudaGraphInstantiate(&s->s1_switch[b], graph, 0));
-  RYK_CUDA(cudaGraphDestroy(graph));
-  return 0;
+  RYK_CUDA(cudaGraphKernelNodeSetParams(set_node, &kp));
+  return stage_graph_init(s->graphs[b].s1, graph);
 }
 
 // The head of stage 1 of a chunk of parity b: slide the feature window by the analysis outputs and run the silence gate on the
@@ -437,7 +468,6 @@ static int stage1_head(Engine* e, Session* s, int b) {
   slide_add<float>(sb, s->cw_mc[f], s->enc_mc[b] + (size_t)pe * s->C, s->cw_mc[g], s->Tw, s->n_feat, s->C);
   slide_add<uint8_t>(sb, s->cw_voiced[f], s->enc_voiced[b] + pe, s->cw_voiced[g], s->Tw, s->n_feat, 1);
   if (slide_batch(sb, s->sC)) return -1;
-  e->launches += 1;
   return gate_mask_run(e, s->cw_wave[g], s->Tw * s->hop, c.fft_length, s->hop, c.threshold_db, s->Tw, s->d_mse, s->d_mask[b], s->d_index[b],
                        s->d_count[b], s->sC);
 }
@@ -503,15 +533,12 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
         const float* chunk = s->d_chunk_fixed;
         if (s->in.rate) {            // device rate -> fs in front of the wave slide
           if (slide<float>(s->in_win[f], s->d_chunk_fixed, s->in_win[g], s->in.hist, s->n_in, 1, s->sE)) return -1;
-          e->launches += 1;
           if (resample_stream_in_run(e, s->in_win[g], s->in.hist, s->n_in, s->delay_in, s->in.up, s->in.down, s->in.d_h, s->in.n_taps,
                                      s->in.d_st + f, s->in.d_st + g, s->d_chunk_model, s->n_wave, s->sE)) return -1;
           chunk = s->d_chunk_model;
         }
         if (slide<float>(s->wave_win[f], chunk, s->wave_win[g], s->Lw, s->n_wave, 1, s->sE)) return -1;
-        if (slide<float>(s->cw_wave[f], s->wave_win[g] + (size_t)pe * s->hop, s->cw_wave[g], (size_t)s->Tw * s->hop, (size_t)s->n_feat * s->hop, 1, s->sE)) return -1;
-        e->launches += 2;
-        return 0;
+        return slide<float>(s->cw_wave[f], s->wave_win[g] + (size_t)pe * s->hop, s->cw_wave[g], (size_t)s->Tw * s->hop, (size_t)s->n_feat * s->hop, 1, s->sE);
       })) return -1;
   if (stage_time(s, 0, 1, r, s->sE)) return -1;
   RYK_CUDA(cudaEventRecord(s->ev[r].gate, s->sE));
@@ -526,11 +553,9 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
         if (s->crepe[b]) {
           if (crepe_plan_run(e, s->crepe[b], s->wave_win[g], sA)) return -1;
           d_f0 = crepe_plan_f0(s->crepe[b]);
-          e->launches += 3;                       // spectral_analysis_run (crepe_plan_run counts its own)
         } else {
           if (dio_stonemask_run(e, s->dio[b], s->wave_win[g], sA)) return -1;
           d_f0 = dio_plan_f0(s->dio[b]);
-          e->launches += 13;
         }
         const int n_enc = s->Lw / s->hop;
         return spectral_analysis_run(e, s->wave_win[g], s->Lw, c.fs, c.frame_period_ms, d_f0, n_enc, c.fft_length, c.order,
@@ -546,20 +571,11 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
   if (run_graph(e, pg.s1_head, s->sC, [&]() -> int { return stage1_head(e, s, b); })) return -1;
   // the next chunks of this parity wait only for the head, so stage 1's U-Net is off the gate -> analysis -> stage 1 recurrence
   RYK_CUDA(cudaEventRecord(s->ev[r].cslide, s->sC));
-  RYK_CUDA(cudaMemcpyAsync(s->h_count[r], s->d_count[b], sizeof(int) * 2, cudaMemcpyDeviceToHost, s->sC));
-  RYK_CUDA(cudaEventRecord(s->ev[r].count, s->sC));
   if (k >= 2) {
     RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[(k - 2) % kRing].dslide, 0));   // cv_{f0,ap,voiced}_out[b] consumed by decode k-2
     RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[(k - 2) % kRing].conv, 0));     // cv_sp_mid[b] consumed by stage 2 of k-2
   }
-  // launch-count bookkeeping only (never waits): the newest count that has already arrived tells which body ran last
-  for (int back = 1; back <= 3 && k - back >= 0; ++back) {
-    const int rr = (int)((k - back) % kRing);
-    if (cudaEventQuery(s->ev[rr].count) == cudaSuccess) { s->last_bucket = s->h_count[rr][0] > 0 ? s->h_count[rr][1] / 128 : 0; break; }
-  }
-  if (s->last_bucket < 0 || s->last_bucket >= s->s1_buckets) s->last_bucket = s->s1_buckets - 1;
-  RYK_CUDA(cudaGraphLaunch(s->s1_switch[b], s->sC));
-  e->launches += s->s1_switch_launches[b][s->last_bucket];
+  if (stage_graph_launch(e, pg.s1, s->sC)) return -1;     // counts the setter; k_set_bucket counts the body it selects
   if (stage_time(s, 2, 1, r, s->sC)) return -1;
   RYK_CUDA(cudaEventRecord(s->ev[r].s1, s->sC));
 
@@ -585,15 +601,15 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
 }
 
 // single session: stage-2 layers 1..14 (the wgmma layers) on the session's own stream
-static int session_mid_single(Engine* e, Session* s, bool was_profiling) {
+static int session_mid_single(Engine* e, Session* s) {
   const int b = (int)(s->step & 1);
   cudaStream_t sC2 = s2_stream(s, b);
   UNetPlan* p2 = nullptr;
   if (s2_plan(e, s, b, &p2)) return -1;
   cudaEvent_t pe0 = nullptr, pe1 = nullptr;
-  if (was_profiling) { RYK_CUDA(cudaEventCreate(&pe0)); RYK_CUDA(cudaEventCreate(&pe1)); RYK_CUDA(cudaEventRecord(pe0, sC2)); }
+  if (e->profile) { RYK_CUDA(cudaEventCreate(&pe0)); RYK_CUDA(cudaEventCreate(&pe1)); RYK_CUDA(cudaEventRecord(pe0, sC2)); }
   if (run_graph(e, s->graphs[b].s2_layers, sC2, [&]() -> int { return unet_forward(e, p2, sC2, 1, 14); })) return -1;
-  if (was_profiling) { RYK_CUDA(cudaEventRecord(pe1, sC2)); e->prof_events.emplace_back(pe0, pe1); }
+  if (e->profile) { RYK_CUDA(cudaEventRecord(pe1, sC2)); e->prof_events.emplace_back(pe0, pe1); }
   return 0;
 }
 
@@ -632,7 +648,6 @@ static int session_back(Engine* e, Session* s) {
         slide_add<float>(sb, s->dw_sp[f], s->cv_sp_out[b] + (size_t)pc * s->nb, s->dw_sp[g], s->Td, s->n_feat, s->nb);
         if (slide_batch(sb, s->sD)) return -1;
         k_f32_to_f64<<<(s->Td + 127) / 128, 128, 0, s->sD>>>(s->dw_f0[g], s->dec_f0_f64, s->Td);
-        e->launches += 2;
         RYK_CUDA(cudaGetLastError());
         return 0;
       })) return -1;
@@ -642,7 +657,6 @@ static int session_back(Engine* e, Session* s) {
         if (synth_add_kernel(e, s->synth, s->dec_f0_f64, s->Td, s->dw_sp[g], s->dw_ap[g], s->sD)) return -1;
         if (synth_drain_async(e, s->synth, s->d_out_fixed[b], max_blocks, s->sD)) return -1;
         k_scrub<<<8, 256, 0, s->sD>>>(s->d_out_fixed[b], s->synth->dev.state, c.vocoder_buffer_size, max_blocks * c.vocoder_buffer_size, s->d_n_fixed[b]);
-        e->launches += 1;
         RYK_CUDA(cudaGetLastError());
         if (!s->out.rate) return 0;
         // fs -> device rate: the outputs whose filter support the synthesizer has produced; the rest waits for the next step
@@ -657,17 +671,14 @@ static int session_back(Engine* e, Session* s) {
 }
 
 static int session_enqueue(Engine* e, Session* s, const float* d_chunk_user) {
-  const bool was_profiling = e->profile;
-  e->profile = false;                                      // the session places its own timing events (between graph launches)
   int rc = session_front(e, s, d_chunk_user);
-  if (!rc) rc = session_mid_single(e, s, was_profiling);
+  if (!rc) rc = session_mid_single(e, s);
   if (!rc) rc = session_back(e, s);
-  e->profile = was_profiling;
   return rc;
 }
 
 // One step of every member + the batched stage-2 forward between their front and back halves.
-static int group_enqueue_impl(Engine* e, Group* G, const float* const* d_chunks, bool was_profiling) {
+static int group_enqueue(Engine* e, Group* G, const float* const* d_chunks) {
   const int r = (int)(G->step % kRing);
   for (size_t i = 0; i < G->members.size(); ++i)
     if (session_front(e, G->members[i], d_chunks[i])) return -1;
@@ -676,21 +687,14 @@ static int group_enqueue_impl(Engine* e, Group* G, const float* const* d_chunks,
     if (m->step >= 1) RYK_CUDA(cudaStreamWaitEvent(G->sG, m->ev[(m->step - 1) % kRing].conv, 0));   // batched output read by epilogue k-1
   }
   cudaEvent_t pe0 = nullptr, pe1 = nullptr;
-  if (was_profiling) { RYK_CUDA(cudaEventCreate(&pe0)); RYK_CUDA(cudaEventCreate(&pe1)); RYK_CUDA(cudaEventRecord(pe0, G->sG)); }
+  if (e->profile) { RYK_CUDA(cudaEventCreate(&pe0)); RYK_CUDA(cudaEventCreate(&pe1)); RYK_CUDA(cudaEventRecord(pe0, G->sG)); }
   if (run_graph(e, G->fwd_graph, G->sG, [&]() -> int { return unet_forward(e, G->p2, G->sG, 0, 15); })) return -1;
-  if (was_profiling) { RYK_CUDA(cudaEventRecord(pe1, G->sG)); e->prof_events.emplace_back(pe0, pe1); }
+  if (e->profile) { RYK_CUDA(cudaEventRecord(pe1, G->sG)); e->prof_events.emplace_back(pe0, pe1); }
   RYK_CUDA(cudaEventRecord(G->ev_fwd[r], G->sG));
   for (Session* m : G->members)
     if (session_back(e, m)) return -1;
   G->step++;
   return 0;
-}
-static int group_enqueue(Engine* e, Group* G, const float* const* d_chunks) {
-  const bool was_profiling = e->profile;
-  e->profile = false;
-  int rc = group_enqueue_impl(e, G, d_chunks, was_profiling);
-  e->profile = was_profiling;
-  return rc;
 }
 
 // ---- host-API staging shared by sessions and groups (ring slot r = step % kRing) ----
@@ -846,7 +850,6 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
     if (P((void**)&s->h_in[i], sizeof(float) * s->n_wave)) return -1;
     if (P((void**)&s->h_out[i], sizeof(double) * out_samples)) return -1;
     if (P((void**)&s->h_n[i], sizeof(int))) return -1;
-    if (P((void**)&s->h_count[i], sizeof(int) * 2)) return -1;
   }
   // f0 method 2: each step's encode window is analysed on its own, like one crepe.predict call per fetched window (DESIGN.md C3)
   for (int i = 0; i < 2; ++i) {
@@ -1246,7 +1249,6 @@ int ryk_reblock_push_device(ryk_engine* h, int id, int session_id, const double*
   const long long k = R->pushed;
   const int r = (int)(k % kRing);
   k_reblock<<<1, 1024, 0, st>>>(R->d_state, R->d_frag[0], R->d_frag[1], R->cap, wave_dev, n_dev, R->max_in, R->chunk, R->d_chunk[r], R->d_nvalid[r]);
-  e->launches += 1;
   RYK_CUDA(cudaGetLastError());
   if (output_gate_async(e, R->d_chunk[r], R->d_nvalid[r], R->chunk, R->n_fft, R->hop, R->threshold_db, R->d_scratch, R->d_power[r], R->d_status[r], st)) return -1;
   RYK_CUDA(cudaMemcpyAsync(R->h_status[r], R->d_status[r], sizeof(int), cudaMemcpyDeviceToHost, st));

@@ -245,15 +245,10 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
 // d_in / d_out live in the plan (p->d_in, p->d_out); callers fill / read them stream-ordered.
 int unet_forward(Engine* e, UNetPlan* p, cudaStream_t st, int first_layer, int last_layer) {
   if (p->fused && e->s1_fused && first_layer == 0 && last_layer == 15) return s1_fused_run(e, p, st);
-  const bool prof = e->profile && p->H > 1;        // time the k4 layers (1..14) of the 2-D (stage-2) net
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   for (int i = first_layer; i <= last_layer; ++i) {
     const ConvLayer& L = p->layers[i];
-    if (prof && i == 1) { RYK_CUDA(cudaEventCreate(&ev0)); RYK_CUDA(cudaEventCreate(&ev1)); RYK_CUDA(cudaEventRecord(ev0, st)); }
     int rc = L.tc_ready ? conv_tc_run(L, st) : conv_direct_run(L, st);
     if (rc) return rc;
-    if (prof && i == 14 && ev0) { RYK_CUDA(cudaEventRecord(ev1, st)); e->prof_events.emplace_back(ev0, ev1); }
-    e->launches += (L.tc_ready && L.ksplit > 1) ? 2 : 1;     // split-K: kernel + reduce
   }
   return 0;
 }

@@ -635,7 +635,6 @@ int harvest_run(Engine* e, HarvestPlan* p, const float* d_x, double* d_f0, cudaS
   k_hv_smooth<<<1, 64, 0, st>>>(p->d_best, p->nf1, p->max_sections, p->d_work, p->d_iwork, p->d_basic);
   k_hv_subsample<<<(p->f0_length + 127) / 128, 128, 0, st>>>(p->d_basic, p->nf1, p->frame_period, p->f0_length, d_f0);
   RYK_CUDA(cudaGetLastError());
-  e->launches += 14;
   return 0;
 }
 

