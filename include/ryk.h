@@ -125,6 +125,17 @@ int ryk_model_layer_shape(ryk_engine* e, int stage, int layer, int* transposed, 
 int ryk_stage1_set_stats(ryk_engine* e, int channels, const float* in_mean, const float* in_std,
                          const float* out_mean, const float* out_std);
 int ryk_f0_set_stats(ryk_engine* e, double in_mean, double in_std, double target_mean, double target_std);
+/* Voices: an engine holds several target voices, each its own pair of models with their statistics.  Voice 0 is the engine's built-in
+ * voice, the one the calls above and the per-op conversions address.  ryk_voice_create returns ids >= 1; the ryk_voice_* calls take
+ * the same arguments as the calls above plus the voice.  A voice >= 1 is fixed while a session or group uses it: changing its models
+ * or statistics, or destroying it (which frees its weights), fails until those are destroyed. */
+int ryk_voice_create(ryk_engine* e, int* voice_id);
+int ryk_voice_destroy(ryk_engine* e, int voice_id);
+int ryk_voice_model_create(ryk_engine* e, int voice_id, int stage, int in_channels, int out_channels, int base_channels);
+int ryk_voice_model_set_layer(ryk_engine* e, int voice_id, int stage, int layer, const float* W, const float* scale, const float* shift);
+int ryk_voice_stage1_set_stats(ryk_engine* e, int voice_id, int channels, const float* in_mean, const float* in_std,
+                               const float* out_mean, const float* out_std);
+int ryk_voice_f0_set_stats(ryk_engine* e, int voice_id, double in_mean, double in_std, double target_mean, double target_std);
 /* x, y: [T][channels] float32 (T >= 1; internally padded to the next multiple of 128 with the per-channel minimum) */
 int ryk_stage1_convert(ryk_engine* e, const float* x, int T, float* y);
 /* f0_out[i] = voiced[i] ? exp((ln f0[i] - mu_in) / sd_in * sd_tgt + mu_tgt) : 0 */
@@ -209,6 +220,10 @@ typedef struct {
 } ryk_session_config;
 
 int ryk_session_create(ryk_engine* e, const ryk_session_config* cfg, int* session_id);
+/* A session that converts into voice_id for its whole lifetime (ryk_session_create: voice 0).  A voice >= 1 needs both models with
+ * every layer loaded; without stage-1 statistics it uses identity statistics. */
+int ryk_session_create_voice(ryk_engine* e, const ryk_session_config* cfg, int voice_id, int* session_id);
+int ryk_session_voice(ryk_engine* e, int session_id);        /* the voice a session converts into, or -1 */
 int ryk_session_destroy(ryk_engine* e, int session_id);
 /* One chunk through encode -> convert -> decode with host buffers (H2D + kernels + D2H inside).
  * wave: round(fs * buffer_time) float32 samples; out: up to out_capacity float64 samples; *n_out is a
@@ -251,7 +266,10 @@ int ryk_session_stage_times(ryk_engine* e, int session_id, float* start, float* 
  * SuperResolution.convert (voice_changer.py:41) per stream; a group stacks the members' padded log-spectrograms into
  * one (B, 1, Tp, 512) stage-2 input per step.  Analysis, gate, stage 1 and synthesis stay per stream (per-stream state,
  * data-dependent lengths).  Members are fresh sessions with the same window length; member i of every call is
- * session_ids[i].  Outputs per member are those of an ungrouped session up to the FP16 stage-2 rounding. */
+ * session_ids[i].  Outputs per member are those of an ungrouped session up to the FP16 stage-2 rounding.
+ * Members may convert into different voices when their stage-2 models have the same channels, the engine is in precision 1, every
+ * stage-2 layer runs on a kernel that reads weights per batch item (the base-64 nets) and there are at most 8 distinct voices: the one
+ * batched forward reads each member's weights from its voice.  Other groups of several voices are refused. */
 int ryk_group_create(ryk_engine* e, const int* session_ids, int n_sessions, int* group_id);
 int ryk_group_destroy(ryk_engine* e, int group_id);        /* members survive, ungrouped */
 int ryk_group_size(ryk_engine* e, int group_id);

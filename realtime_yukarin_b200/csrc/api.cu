@@ -78,7 +78,7 @@ int dio_get_plan(Engine* e, int n, int fs, double frame_period, double f0_floor,
   return 0;
 }
 
-static UNet*& stage_net(Engine* e, int stage) { return stage == 1 ? e->stage1 : e->stage2; }
+static UNet*& stage_net(Voice* v, int stage) { return stage == 1 ? v->stage1 : v->stage2; }
 
 static int upload_vec(float** d, const float* h, int n) {
   if (*d) cudaFree(*d);
@@ -87,15 +87,35 @@ static int upload_vec(float** d, const float* h, int n) {
   return 0;
 }
 
-static int ensure_stage1_stats(Engine* e, int C) {
-  if (e->d_s1_in_mean && (int)e->s1_in_mean.size() == C) return 0;
-  std::vector<float> zero(C, 0.f), one(C, 1.f);
-  e->s1_in_mean = zero; e->s1_in_std = one; e->s1_out_mean = zero; e->s1_out_std = one;
-  if (upload_vec(&e->d_s1_in_mean, zero.data(), C)) return -1;
-  if (upload_vec(&e->d_s1_in_std, one.data(), C)) return -1;
-  if (upload_vec(&e->d_s1_out_mean, zero.data(), C)) return -1;
-  if (upload_vec(&e->d_s1_out_std, one.data(), C)) return -1;
+static int voice_set_stage1_stats(Voice* v, int C, const float* in_mean, const float* in_std, const float* out_mean, const float* out_std) {
+  v->s1_in_mean.assign(in_mean, in_mean + C); v->s1_in_std.assign(in_std, in_std + C);
+  v->s1_out_mean.assign(out_mean, out_mean + C); v->s1_out_std.assign(out_std, out_std + C);
+  if (upload_vec(&v->d_s1_in_mean, in_mean, C)) return -1;
+  if (upload_vec(&v->d_s1_in_std, in_std, C)) return -1;
+  if (upload_vec(&v->d_s1_out_mean, out_mean, C)) return -1;
+  if (upload_vec(&v->d_s1_out_std, out_std, C)) return -1;
   return 0;
+}
+
+int voice_default_stage1_stats(Voice* v, int C) {
+  if (v->d_s1_in_mean && (int)v->s1_in_mean.size() == C) return 0;
+  std::vector<float> zero(C, 0.f), one(C, 1.f);
+  return voice_set_stage1_stats(v, C, zero.data(), one.data(), zero.data(), one.data());
+}
+
+bool voice_models_loaded(const Voice* v) {
+  for (const UNet* n : {v->stage1, v->stage2}) {
+    if (!n) return false;
+    for (const UNetLayerW& L : n->layers) if (!L.loaded) return false;
+  }
+  return true;
+}
+
+static void voice_free(Voice* v) {
+  if (!v) return;
+  unet_destroy(v->stage1); unet_destroy(v->stage2);
+  for (float* p : {v->d_s1_in_mean, v->d_s1_in_std, v->d_s1_out_mean, v->d_s1_out_std}) if (p) cudaFree(p);
+  delete v;
 }
 
 __global__ void k_affine_rows(const float* __restrict__ y, int T, int C, const float* __restrict__ scale, const float* __restrict__ shift, float* __restrict__ out) {
@@ -120,13 +140,24 @@ __global__ void k_f0_convert(const float* __restrict__ f0, const uint8_t* __rest
 }
 
 // stage-1 forward on device buffers: x already normalised+padded in plan->d_in; returns plan
+// (the per-op API runs on voice 0)
 static int stage1_plan_for(Engine* e, int Tp, UNetPlan** plan) {
-  RYK_CHECK(e->stage1 != nullptr, "stage-1 model not loaded");
-  return unet_get_plan(e, e->stage1, 1, 1, Tp, e->precision, plan);
+  RYK_CHECK(e->voices[0]->stage1 != nullptr, "stage-1 model not loaded");
+  return unet_get_plan(e, e->voices[0]->stage1, 1, 1, Tp, e->precision, plan);
 }
 static int stage2_plan_for(Engine* e, int Tp, UNetPlan** plan) {
-  RYK_CHECK(e->stage2 != nullptr, "stage-2 model not loaded");
-  return unet_get_plan(e, e->stage2, 1, Tp, 512, e->precision, plan);
+  RYK_CHECK(e->voices[0]->stage2 != nullptr, "stage-2 model not loaded");
+  return unet_get_plan(e, e->voices[0]->stage2, 1, Tp, 512, e->precision, plan);
+}
+
+// The voice a model / statistics call addresses.  Voices >= 1 stay fixed while a session or group uses them: the session's captured
+// graphs point at the weights and hold the f0 statistics by value.  Voice 0 keeps the engine's original rules.
+static int voice_for_update(Engine* e, int id, Voice** out) {
+  Voice* v = engine_voice(e, id);
+  RYK_CHECK(v != nullptr, "no such voice");
+  RYK_CHECK(id == 0 || v->users == 0, "voice is in use by a session or group: destroy them before changing its models or statistics");
+  *out = v;
+  return 0;
 }
 
 }  // namespace ryk
@@ -157,6 +188,7 @@ int ryk_engine_create(int device, ryk_engine** out) {
   ryk_engine* h = new ryk_engine();
   Engine* e = &h->impl;
   e->device = device;
+  e->voices.push_back(new Voice());
   RYK_CUDA(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
   std::vector<double2> tw(kTwiddleN / 2);
   fft_fill_twiddles(tw.data());
@@ -178,11 +210,11 @@ int ryk_engine_destroy(ryk_engine* h) {
   cudaSetDevice(e->device);
   cudaStreamSynchronize(e->stream);
   for (auto& kv : e->dio_plans) dio_plan_free(kv.second);
-  unet_destroy(e->stage1); unet_destroy(e->stage2);
+  for (Voice* v : e->voices) voice_free(v);
   for (Synth* s : e->synths) synth_destroy(s);
   session_destroy_all(e);
   crepe_destroy();                                  // after the sessions: their CREPE plans are counted on the model
-  void* ptrs[] = {e->d_colmin, e->d_launches, e->d_twiddle, e->d_jump, e->d_G, e->d_H, e->d_s1_in_mean, e->d_s1_in_std, e->d_s1_out_mean, e->d_s1_out_std, e->d_scratch};
+  void* ptrs[] = {e->d_colmin, e->d_launches, e->d_twiddle, e->d_jump, e->d_G, e->d_H, e->d_scratch};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (e->h_pinned) cudaFreeHost(e->h_pinned);
   cudaStreamDestroy(e->stream);
@@ -342,26 +374,74 @@ int ryk_silence_mask(ryk_engine* h, const float* wave, int n, int frame_length, 
   return 0;
 }
 
-int ryk_model_create(ryk_engine* h, int stage, int in_ch, int out_ch, int base) {
+int ryk_voice_create(ryk_engine* h, int* voice_id) {
+  Engine* e = E(h);
+  RYK_CHECK(voice_id != nullptr, "null out pointer");
+  e->voices.push_back(new Voice());
+  *voice_id = (int)e->voices.size() - 1;
+  return 0;
+}
+
+int ryk_voice_destroy(ryk_engine* h, int voice_id) {
+  Engine* e = E(h);
+  RYK_CUDA(cudaSetDevice(e->device));
+  Voice* v = engine_voice(e, voice_id);
+  RYK_CHECK(v != nullptr && voice_id >= 1, "no such voice (voice 0 is the engine's own and is never destroyed)");
+  RYK_CHECK(v->users == 0, "voice is in use by a session or group: destroy them first");
+  RYK_CUDA(cudaStreamSynchronize(e->stream));
+  voice_free(v);
+  e->voices[voice_id] = nullptr;
+  return 0;
+}
+
+int ryk_voice_model_create(ryk_engine* h, int voice_id, int stage, int in_ch, int out_ch, int base) {
   Engine* e = E(h);
   RYK_CUDA(cudaSetDevice(e->device));
   RYK_CHECK(stage == 1 || stage == 2, "stage must be 1 or 2");
-  UNet*& net = stage_net(e, stage);
+  Voice* v = nullptr;
+  if (voice_for_update(e, voice_id, &v)) return -1;
+  UNet*& net = stage_net(v, stage);
   if (net) { RYK_CUDA(cudaStreamSynchronize(e->stream)); unet_destroy(net); net = nullptr; }
   net = unet_create(stage == 1 ? 1 : 2, in_ch, out_ch, base);
   return 0;
 }
 
-int ryk_model_set_layer(ryk_engine* h, int stage, int layer, const float* W, const float* scale, const float* shift) {
+int ryk_voice_model_set_layer(ryk_engine* h, int voice_id, int stage, int layer, const float* W, const float* scale, const float* shift) {
   Engine* e = E(h);
   RYK_CUDA(cudaSetDevice(e->device));
-  UNet* net = stage_net(e, stage);
+  Voice* v = nullptr;
+  if (voice_for_update(e, voice_id, &v)) return -1;
+  UNet* net = stage_net(v, stage);
   RYK_CHECK(net != nullptr, "ryk_model_create was not called for this stage");
   return unet_set_layer(e, net, layer, W, scale, shift);
 }
 
+int ryk_voice_stage1_set_stats(ryk_engine* h, int voice_id, int C, const float* in_mean, const float* in_std, const float* out_mean,
+                               const float* out_std) {
+  Engine* e = E(h);
+  RYK_CUDA(cudaSetDevice(e->device));
+  Voice* v = nullptr;
+  if (voice_for_update(e, voice_id, &v)) return -1;
+  RYK_CUDA(cudaStreamSynchronize(e->stream));
+  return voice_set_stage1_stats(v, C, in_mean, in_std, out_mean, out_std);
+}
+
+int ryk_voice_f0_set_stats(ryk_engine* h, int voice_id, double in_mean, double in_std, double target_mean, double target_std) {
+  Voice* v = nullptr;
+  if (voice_for_update(E(h), voice_id, &v)) return -1;
+  v->f0_in_mean = in_mean; v->f0_in_std = in_std; v->f0_tgt_mean = target_mean; v->f0_tgt_std = target_std;
+  v->has_f0_stats = true;
+  return 0;
+}
+
+int ryk_model_create(ryk_engine* h, int stage, int in_ch, int out_ch, int base) { return ryk_voice_model_create(h, 0, stage, in_ch, out_ch, base); }
+
+int ryk_model_set_layer(ryk_engine* h, int stage, int layer, const float* W, const float* scale, const float* shift) {
+  return ryk_voice_model_set_layer(h, 0, stage, layer, W, scale, shift);
+}
+
 int ryk_model_layer_shape(ryk_engine* h, int stage, int layer, int* transposed, int* cin, int* cout, int* k) {
-  UNet* net = stage_net(E(h), stage);
+  UNet* net = stage_net(E(h)->voices[0], stage);
   RYK_CHECK(net != nullptr && layer >= 0 && layer < 16, "no such layer");
   const UNetLayerW& L = net->layers[layer];
   *transposed = L.transposed; *cin = L.cin; *cout = L.cout; *k = L.k;
@@ -369,32 +449,21 @@ int ryk_model_layer_shape(ryk_engine* h, int stage, int layer, int* transposed, 
 }
 
 int ryk_stage1_set_stats(ryk_engine* h, int C, const float* in_mean, const float* in_std, const float* out_mean, const float* out_std) {
-  Engine* e = E(h);
-  RYK_CUDA(cudaSetDevice(e->device));
-  RYK_CUDA(cudaStreamSynchronize(e->stream));
-  e->s1_in_mean.assign(in_mean, in_mean + C); e->s1_in_std.assign(in_std, in_std + C);
-  e->s1_out_mean.assign(out_mean, out_mean + C); e->s1_out_std.assign(out_std, out_std + C);
-  if (upload_vec(&e->d_s1_in_mean, in_mean, C)) return -1;
-  if (upload_vec(&e->d_s1_in_std, in_std, C)) return -1;
-  if (upload_vec(&e->d_s1_out_mean, out_mean, C)) return -1;
-  if (upload_vec(&e->d_s1_out_std, out_std, C)) return -1;
-  return 0;
+  return ryk_voice_stage1_set_stats(h, 0, C, in_mean, in_std, out_mean, out_std);
 }
 
 int ryk_f0_set_stats(ryk_engine* h, double in_mean, double in_std, double target_mean, double target_std) {
-  Engine* e = E(h);
-  e->f0_in_mean = in_mean; e->f0_in_std = in_std; e->f0_tgt_mean = target_mean; e->f0_tgt_std = target_std;
-  e->has_f0_stats = true;
-  return 0;
+  return ryk_voice_f0_set_stats(h, 0, in_mean, in_std, target_mean, target_std);
 }
 
 int ryk_stage1_convert(ryk_engine* h, const float* x, int T, float* y) {
   Engine* e = E(h);
   RYK_CUDA(cudaSetDevice(e->device));
-  RYK_CHECK(e->stage1 != nullptr, "stage-1 model not loaded");
+  Voice* v = e->voices[0];
+  RYK_CHECK(v->stage1 != nullptr, "stage-1 model not loaded");
   RYK_CHECK(T > 0, "empty input");
-  const int C = e->stage1->in_ch, Co = e->stage1->out_ch;
-  if (ensure_stage1_stats(e, C)) return -1;
+  const int C = v->stage1->in_ch, Co = v->stage1->out_ch;
+  if (voice_default_stage1_stats(v, C)) return -1;
   const int Tp = T + (128 - T % 128);
   UNetPlan* plan = nullptr;
   if (stage1_plan_for(e, Tp, &plan)) return -1;
@@ -407,9 +476,9 @@ int ryk_stage1_convert(ryk_engine* h, const float* x, int T, float* y) {
   int cnt[2] = {T, Tp};
   RYK_CUDA(cudaMemcpyAsync(d_x, x, sizeof(float) * T * C, cudaMemcpyHostToDevice, e->stream));
   RYK_CUDA(cudaMemcpyAsync(d_count, cnt, sizeof(cnt), cudaMemcpyHostToDevice, e->stream));
-  if (stage1_prologue_run(e, d_x, nullptr, d_count, C, (float*)plan->d_in, Tp, e->stream)) return -1;
+  if (stage1_prologue_run(v, d_x, nullptr, d_count, C, (float*)plan->d_in, Tp, e->stream)) return -1;
   if (unet_forward(e, plan, e->stream)) return -1;
-  k_affine_rows<<<(T * Co + 255) / 256, 256, 0, e->stream>>>((const float*)plan->d_out, T, Co, e->d_s1_out_std, e->d_s1_out_mean, d_y);
+  k_affine_rows<<<(T * Co + 255) / 256, 256, 0, e->stream>>>((const float*)plan->d_out, T, Co, v->d_s1_out_std, v->d_s1_out_mean, d_y);
   RYK_CUDA(cudaMemcpyAsync(y, d_y, sizeof(float) * T * Co, cudaMemcpyDeviceToHost, e->stream));
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   return 0;
@@ -425,8 +494,9 @@ int ryk_f0_convert(ryk_engine* h, const float* f0, const uint8_t* voiced, int T,
   float* d_f0 = A.take<float>(T); uint8_t* d_v = A.take<uint8_t>(T); float* d_o = A.take<float>(T);
   RYK_CUDA(cudaMemcpyAsync(d_f0, f0, sizeof(float) * T, cudaMemcpyHostToDevice, e->stream));
   RYK_CUDA(cudaMemcpyAsync(d_v, voiced, T, cudaMemcpyHostToDevice, e->stream));
-  k_f0_convert<<<(T + 127) / 128, 128, 0, e->stream>>>(d_f0, d_v, T, e->f0_in_mean, e->f0_in_std, e->f0_tgt_mean, e->f0_tgt_std,
-                                                      e->has_f0_stats ? 1 : 0, d_o);
+  const Voice* v = e->voices[0];
+  k_f0_convert<<<(T + 127) / 128, 128, 0, e->stream>>>(d_f0, d_v, T, v->f0_in_mean, v->f0_in_std, v->f0_tgt_mean, v->f0_tgt_std,
+                                                      v->has_f0_stats ? 1 : 0, d_o);
   RYK_CUDA(cudaMemcpyAsync(out, d_o, sizeof(float) * T, cudaMemcpyDeviceToHost, e->stream));
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   return 0;
@@ -478,12 +548,13 @@ int ryk_convert_window(ryk_engine* h, const float* wave, int n_wave, int fs, int
   Engine* e = E(h);
   RYK_CUDA(cudaSetDevice(e->device));
   RYK_CHECK(T > 0, "empty window");
-  RYK_CHECK(e->stage1 && e->stage2, "models not loaded");
+  Voice* v = e->voices[0];
+  RYK_CHECK(v->stage1 && v->stage2, "models not loaded");
   const int nb = fftlen / 2 + 1, C = order + 1;
   RYK_CHECK(nb == 513, "stage 2 expects 513-bin spectra");
-  RYK_CHECK(e->stage1->in_ch == C && e->stage1->out_ch == C, "stage-1 channel count does not match order + 1");
+  RYK_CHECK(v->stage1->in_ch == C && v->stage1->out_ch == C, "stage-1 channel count does not match order + 1");
   if (sptk_prepare(e, order, alpha, fftlen)) return -1;
-  if (ensure_stage1_stats(e, C)) return -1;
+  if (voice_default_stage1_stats(v, C)) return -1;
   ConvertBuffers cb;
   if (convert_buffers_get(e, T, n_wave, nb, C, &cb)) return -1;
   cudaStream_t st = e->stream;
@@ -744,13 +815,14 @@ int ryk_test_stage2_forward(ryk_engine* h, int B, int Tp, int n_keep, const int*
                             float* y) {
   Engine* e = E(h);
   RYK_CUDA(cudaSetDevice(e->device));
-  RYK_CHECK(e->stage2 != nullptr, "stage-2 model not loaded");
+  UNet* net = e->voices[0]->stage2;
+  RYK_CHECK(net != nullptr, "stage-2 model not loaded");
   RYK_CHECK(B >= 1 && Tp >= 128 && Tp % 128 == 0 && mode >= 0 && mode <= 2 && (mode == 0 || n_keep >= 1), "bad stage-2 test arguments");
   int kb = 0, kl = 0;
   if (mode != 0) keep_hull(n_keep, keep_begin, keep_len, &kb, &kl);
   const int owner = ++e->plan_owners;
   UNetPlan* p = nullptr;
-  int rc = unet_get_plan(e, e->stage2, B, Tp, 512, e->precision, &p, owner, kb, kl, mode == 2);
+  int rc = unet_get_plan(e, net, B, Tp, 512, e->precision, &p, owner, kb, kl, mode == 2);
   if (!rc) {
     cudaStream_t st = e->stream;
     const size_t nx = (size_t)B * Tp * 512;
@@ -764,7 +836,7 @@ int ryk_test_stage2_forward(ryk_engine* h, int B, int Tp, int n_keep, const int*
     if (err != cudaSuccess) { set_error(std::string("stage-2 test forward failed: ") + cudaGetErrorString(err)); rc = -1; }
   }
   cudaStreamSynchronize(e->stream);
-  unet_release_owner(e->stage2, owner);
+  unet_release_owner(net, owner);
   return rc;
 }
 
@@ -799,7 +871,7 @@ int ryk_test_conv_layer(ryk_engine* h, int transposed, int k, int stride, int pa
   RYK_CUDA(cudaMemcpyAsync(d_scale, scale, Cout * 4, cudaMemcpyHostToDevice, st));
   RYK_CUDA(cudaMemcpyAsync(d_shift, shift, Cout * 4, cudaMemcpyHostToDevice, st));
   if (pack_weights_direct(d_w, transposed, Cin, Cout, L.KH, k, d_wd, st)) return -1;
-  L.w_direct = d_wd; L.scale = d_scale; L.shift = d_shift;
+  L.wt.w[0] = d_wd; L.wt.scale[0] = d_scale; L.wt.shift[0] = d_shift;
   int rc = 0;
   cudaEvent_t ev0, ev1;
   RYK_CUDA(cudaEventCreate(&ev0)); RYK_CUDA(cudaEventCreate(&ev1));
@@ -825,7 +897,7 @@ int ryk_test_conv_layer(ryk_engine* h, int transposed, int k, int stride, int pa
     if (pack_weights_tc(d_w, transposed, Cin, Cout, L.KH, k, L.SH, stride, d_wt, st)) return -1;
     k_f32_to_f16<<<1184, 256, 0, st>>>(d_in0, d_h0, n0);
     if (n1) k_f32_to_f16<<<1184, 256, 0, st>>>(d_in1, d_h1, n1);
-    L.in0 = d_h0; L.in1 = n1 ? d_h1 : nullptr; L.in_dtype = DT_F16; L.out = d_ho; L.out_dtype = DT_F16; L.w_tc = d_wt;
+    L.in0 = d_h0; L.in1 = n1 ? d_h1 : nullptr; L.in_dtype = DT_F16; L.out = d_ho; L.out_dtype = DT_F16; L.w_tc[0] = d_wt;
     RYK_CHECK(tc_layer_eligible(L), "layer shape is not eligible for the tensor-core kernel");
     int num_sms = 132;
     cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, e->device);
@@ -842,7 +914,7 @@ int ryk_test_conv_layer(ryk_engine* h, int transposed, int k, int stride, int pa
     if (in_h) { k_f32_to_f16<<<1184, 256, 0, st>>>(d_in0, d_h0, n0); if (n1) k_f32_to_f16<<<1184, 256, 0, st>>>(d_in1, d_h1, n1); }
     L.in0 = in_h ? (const void*)d_h0 : (const void*)d_in0; L.in1 = n1 ? (in_h ? (const void*)d_h1 : (const void*)d_in1) : nullptr;
     L.in_dtype = in_h ? DT_F16 : DT_F32; L.out = out_h ? (void*)d_ho : (void*)d_out; L.out_dtype = out_h ? DT_F16 : DT_F32;
-    if (Cout == 1) { L.host_scale_valid = true; L.host_scale = scale[0]; L.host_shift = shift[0]; }
+    if (Cout == 1) { L.host_scale_valid = true; L.wt.host_scale[0] = scale[0]; L.wt.host_shift[0] = shift[0]; }
     rc = conv_direct_run(L, st);
     if (!rc && repeat > 0) rc = timed_graph([&]() { return conv_direct_run(L, st); });
     if (out_h) k_f16_to_f32<<<1184, 256, 0, st>>>(d_ho, d_out, no);

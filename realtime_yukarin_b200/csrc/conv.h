@@ -10,6 +10,23 @@ namespace ryk {
 enum Act { ACT_NONE = 0, ACT_LEAKY = 1, ACT_RELU = 2 };
 enum DType { DT_F32 = 0, DT_F16 = 1 };
 
+constexpr int kMaxGroupVoices = 8;      // distinct voices of one mixed-voice group
+constexpr int kMaxGroupBatch = 64;      // sessions of one group
+
+// A layer's weights per batch item, as the kernels receive them (by value): batch item b reads entry voice_of[b] of each array.
+// Every plan except a mixed-voice group's has one entry and voice_of all 0.
+struct LayerWeights {
+  const float* w[kMaxGroupVoices];                                  // [KH][KW][Cin][Cout] fp32 (CUDA-core kernels)
+  const float* scale[kMaxGroupVoices];                              // [Cout] folded BN scale (1 when no BN)
+  const float* shift[kMaxGroupVoices];                              // [Cout] folded bias / BN shift
+  float host_scale[kMaxGroupVoices], host_shift[kMaxGroupVoices];   // Cout == 1 layers: the scalar scale / shift
+  uint8_t voice_of[kMaxGroupBatch];
+};
+// Plans with more batch items than a group holds have one voice.
+__host__ __device__ inline int item_voice(const LayerWeights& wt, int b) { return b < kMaxGroupBatch ? wt.voice_of[b] : 0; }
+// The tensor-core kernel's weight tensor maps, one per voice (one __grid_constant__ kernel parameter).
+struct TcWeightMaps { CUtensorMap m[kMaxGroupVoices]; };
+
 // One conv / transposed-conv layer over NHWC activations (1-D nets use H = 1, KH = 1).
 // The input is the channel-concatenation of up to two tensors (U-Net skip "concat by pointer").
 struct ConvLayer {
@@ -25,18 +42,18 @@ struct ConvLayer {
   // device pointers
   const void* in0 = nullptr; const void* in1 = nullptr; int in_dtype = DT_F32;
   void* out = nullptr; int out_dtype = DT_F32;
-  const float* w_direct = nullptr;        // [KH][KW][Cin][Cout] fp32
-  const float* scale = nullptr;           // [Cout] folded BN scale (1 when no BN)
-  const float* shift = nullptr;           // [Cout] folded bias / BN shift
-  bool host_scale_valid = false;          // Cout == 1 layers: scalar scale/shift mirrored on the host
-  float host_scale = 1.f, host_shift = 0.f;
+  // weights of voices 0 .. n_voices - 1 (n_voices > 1 only in a mixed-voice group's stage-2 plan; see unet_plan_set_voices)
+  int n_voices = 1;
+  LayerWeights wt = {};
+  bool host_scale_valid = false;          // Cout == 1 layers: scalar scale/shift mirrored on the host (wt.host_scale / host_shift)
   // tensor-core path (filled by tc_layer_prepare)
-  const __half* w_tc = nullptr;           // conv: [Cout][KH*KW*Cin]; deconv: [4 classes][Cout][4*Cin]
+  const __half* w_tc[kMaxGroupVoices] = {};   // per voice; conv: [Cout][KH*KW*Cin]; deconv: [4 classes][Cout][4*Cin]
   const __half* w_frag = nullptr;         // 1-D k4 layers: mma.sync B-fragment order for the fused stage-1 kernel (s1_map.h)
   float* splitk_ws = nullptr;             // [ksplit][B][band's output rows][Wout][Cout] fp32 when ksplit > 1
   int ksplit = 1;
   int ksplit_tiles = 0;                   // > 0: split K as for a layer of this many output tiles instead of the band's own count
-  CUtensorMap tmA0, tmA1, tmB, tmO, tmW;     // inputs, weights, fp16 output, fp32 split-K workspace
+  CUtensorMap tmA0, tmA1, tmO, tmW;       // inputs, fp16 output, fp32 split-K workspace
+  TcWeightMaps tmB;                       // weights, per voice
   int tile_w = 0, tile_h = 0;             // pixel tile = tile_w x tile_h = 128
   int block_n = 0;
   bool tc_ready = false;
@@ -59,10 +76,13 @@ int pack_weights_tc(const float* d_w_chainer, int transposed, int Cin, int Cout,
 
 int conv_direct_run(const ConvLayer& L, cudaStream_t st);
 bool conv_direct_band_supported(const ConvLayer& L);
+// the CUDA-core kernels that read weights per batch item (LayerWeights::voice_of): the stage-2 edge layers of FP16 plans
+bool conv_direct_per_item_weights(const ConvLayer& L);
 
 bool tc_layer_eligible(const ConvLayer& L);
 int tc_init();                                           // resolves cuTensorMapEncodeTiled, sets smem attributes
 int tc_layer_prepare(ConvLayer& L, int num_sms);         // builds tensor maps, picks tiles / split-K (needs final pointers)
+int tc_layer_weight_maps(ConvLayer& L);                  // (re)builds the weight maps of voices 0 .. n_voices - 1 of a prepared layer
 int conv_tc_run(const ConvLayer& L, cudaStream_t st);
 size_t tc_splitk_ws_bytes(const ConvLayer& L, int num_sms);
 int tc_tile_rows(const ConvLayer& L);                    // class-local output rows per tile of the tensor-core kernel

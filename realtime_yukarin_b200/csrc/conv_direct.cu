@@ -140,8 +140,8 @@ static int conv_direct_generic(const ConvLayer& L, cudaStream_t st) {
   p.classH = L.transposed ? L.SH : 1; p.classW = L.transposed ? L.SW : 1;
   RYK_CHECK(L.Hout % p.classH == 0 && L.Wout % p.classW == 0, "transposed conv output must be a multiple of the stride");
   p.Hc = L.Hout / p.classH; p.Wc = L.Wout / p.classW;
-  p.in0 = L.in0; p.in1 = L.in1; p.out = L.out; p.w = L.w_direct; p.scale = L.scale; p.shift = L.shift;
-  RYK_CHECK(L.w_direct && L.scale && L.shift && L.in0 && L.out, "direct conv layer is missing a device pointer");
+  p.in0 = L.in0; p.in1 = L.in1; p.out = L.out; p.w = L.wt.w[0]; p.scale = L.wt.scale[0]; p.shift = L.wt.shift[0];
+  RYK_CHECK(p.w && p.scale && p.shift && L.in0 && L.out, "direct conv layer is missing a device pointer");
   int npix = L.B * p.Hc * p.Wc;
   dim3 grid((npix + 63) / 64, (L.Cout + 63) / 64, p.classH * p.classW);
   if (L.in_dtype == DT_F32 && L.out_dtype == DT_F32) k_conv_direct<float, float><<<grid, 256, 0, st>>>(p);
@@ -161,9 +161,9 @@ static int conv_direct_generic(const ConvLayer& L, cudaStream_t st) {
 // Cin = 1, fp32 input -> Cout (multiple of 8, <= 64) channels.  Block = 32 pixels (x) x Cout/8 channel groups, walking
 // kRows rows of the image with a 3-row register window: every input value is loaded once per thread column, every
 // store is a full 16-byte piece of a 128-byte pixel (4 pixels per warp instruction), no integer divisions.
+// Weights [9][1][Cout] of batch item b's voice.
 template <typename TOut>
-__global__ void __launch_bounds__(256) k_conv3x3_cin1(const float* __restrict__ in, const float* __restrict__ w /*[9][1][Cout]*/,
-                                                     const float* __restrict__ scale, const float* __restrict__ shift, int act,
+__global__ void __launch_bounds__(256) k_conv3x3_cin1(const float* __restrict__ in, const __grid_constant__ LayerWeights wt, int act,
                                                      int B, int H, int W, int Cout, TOut* __restrict__ out) {
   constexpr int kRows = 8;
   const int groups = Cout >> 3;                   // blockDim.x = 32 * groups  (<= 256)
@@ -171,6 +171,10 @@ __global__ void __launch_bounds__(256) k_conv3x3_cin1(const float* __restrict__ 
   const int x = blockIdx.x * 32 + xl;
   const int y0 = blockIdx.y * kRows;
   const int b = blockIdx.z;
+  const int voice = item_voice(wt, b);
+  const float* __restrict__ w = wt.w[voice];
+  const float* __restrict__ scale = wt.scale[voice];
+  const float* __restrict__ shift = wt.shift[voice];
   float wr[9][8], sc[8], sh[8];
 #pragma unroll
   for (int t = 0; t < 9; ++t)
@@ -216,13 +220,16 @@ __global__ void __launch_bounds__(256) k_conv3x3_cin1(const float* __restrict__ 
 // Cout = 1 from two fp16 sources of 64 channels each (skip concat) -> fp32.  One warp = 8 consecutive pixels of a row:
 // lanes 0-15 own 4 channels each of source 0, lanes 16-31 of source 1; the 3 x 10 input pixels are loaded once
 // (30 independent 8-byte loads in flight per lane) and feed all 8 outputs, which are then reduced across the warp.
-// Computes output rows y0 .. y0 + gridDim.y - 1.
+// Computes output rows y0 .. y0 + gridDim.y - 1, with the weights [9][128][1] and scalar scale / shift of batch item b's voice.
 __global__ void __launch_bounds__(256) k_conv3x3_cout1_h(const __half* __restrict__ in0, const __half* __restrict__ in1,
-                                                        const float* __restrict__ w /*[9][128][1]*/, float scale, float shift, int act,
+                                                        const __grid_constant__ LayerWeights weights, int act,
                                                         int B, int H, int W, int y0, float* __restrict__ out) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int x0 = (blockIdx.x * 8 + warp) * 8;          // 8 warps x 8 pixels = 64 pixels of a row per block
   const int y = y0 + blockIdx.y, b = blockIdx.z;
+  const int voice = item_voice(weights, b);
+  const float* __restrict__ w = weights.w[voice];
+  const float scale = weights.host_scale[voice], shift = weights.host_shift[voice];
   if (x0 >= W) return;
   const __half* src = lane < 16 ? in0 : in1;
   const int c = (lane & 15) * 4;
@@ -324,24 +331,34 @@ bool conv_direct_band_supported(const ConvLayer& L) {
          L.C1 == 64 && L.in_dtype == DT_F16 && L.out_dtype == DT_F32 && L.host_scale_valid;
 }
 
+// the first layer of stage-2 plans (k_conv3x3_cin1)
+static bool conv_direct_cin1(const ConvLayer& L) {
+  return !L.transposed && L.KH == 3 && L.KW == 3 && L.SH == 1 && L.SW == 1 && L.PH == 1 && L.PW == 1 && L.C0 == 1 && L.C1 == 0 &&
+         L.in_dtype == DT_F32 && L.Cout % 8 == 0 && L.Cout <= 64;
+}
+
+bool conv_direct_per_item_weights(const ConvLayer& L) { return conv_direct_cin1(L) || conv_direct_band_supported(L); }
+
 int conv_direct_run(const ConvLayer& L, cudaStream_t st) {
   const bool cout1_h = conv_direct_band_supported(L);
+  const bool cin1 = conv_direct_cin1(L);
+  RYK_CHECK(L.n_voices == 1 || cout1_h || cin1, "of the CUDA-core kernels only the stage-2 edge layers take weights per batch item");
   RYK_CHECK(cout1_h || (L.band_y0 == 0 && L.band_y1 == 0), "of the CUDA-core kernels only the Cout = 1 3x3 kernel computes a row band");
   // dedicated kernels for the stage-2 edge layers
   if (!L.transposed && L.KH == 3 && L.KW == 3 && L.SH == 1 && L.SW == 1 && L.PH == 1 && L.PW == 1) {
-    if (L.C0 == 1 && L.C1 == 0 && L.in_dtype == DT_F32 && L.Cout % 8 == 0 && L.Cout <= 64) {
+    if (cin1) {
       dim3 grid((L.Win + 31) / 32, (L.Hin + 7) / 8, L.B);
       int threads = 32 * (L.Cout / 8);
       if (L.out_dtype == DT_F16)
-        k_conv3x3_cin1<__half><<<grid, threads, 0, st>>>((const float*)L.in0, L.w_direct, L.scale, L.shift, L.act, L.B, L.Hin, L.Win, L.Cout, (__half*)L.out);
+        k_conv3x3_cin1<__half><<<grid, threads, 0, st>>>((const float*)L.in0, L.wt, L.act, L.B, L.Hin, L.Win, L.Cout, (__half*)L.out);
       else
-        k_conv3x3_cin1<float><<<grid, threads, 0, st>>>((const float*)L.in0, L.w_direct, L.scale, L.shift, L.act, L.B, L.Hin, L.Win, L.Cout, (float*)L.out);
+        k_conv3x3_cin1<float><<<grid, threads, 0, st>>>((const float*)L.in0, L.wt, L.act, L.B, L.Hin, L.Win, L.Cout, (float*)L.out);
       RYK_CUDA(cudaGetLastError());
       return 0;
     }
     if (cout1_h) {
       dim3 blocks((L.Win + 63) / 64, layer_band_end(L) - L.band_y0, L.B);       // the layer's row band
-      k_conv3x3_cout1_h<<<blocks, 256, 0, st>>>((const __half*)L.in0, (const __half*)L.in1, L.w_direct, L.host_scale, L.host_shift, L.act,
+      k_conv3x3_cout1_h<<<blocks, 256, 0, st>>>((const __half*)L.in0, (const __half*)L.in1, L.wt, L.act,
                                                 L.B, L.Hin, L.Win, L.band_y0, (float*)L.out);
       RYK_CUDA(cudaGetLastError());
       return 0;
@@ -350,7 +367,7 @@ int conv_direct_run(const ConvLayer& L, cudaStream_t st) {
   if (!L.transposed && L.KH == 1 && L.KW == 3 && L.SW == 1 && L.PW == 1 && L.Hin == 1 && L.C0 == 64 && L.C1 == 64 && L.Cout <= 16 &&
       L.in_dtype == DT_F16 && L.out_dtype == DT_F32) {
     const int npos = L.B * L.Win;
-    k_conv1d_k3_small<<<(npos + 7) / 8, 256, 0, st>>>((const __half*)L.in0, (const __half*)L.in1, L.w_direct, L.scale, L.shift, L.act, L.B, L.Win, L.Cout,
+    k_conv1d_k3_small<<<(npos + 7) / 8, 256, 0, st>>>((const __half*)L.in0, (const __half*)L.in1, L.wt.w[0], L.wt.scale[0], L.wt.shift[0], L.act, L.B, L.Win, L.Cout,
                                                      (float*)L.out);
     RYK_CUDA(cudaGetLastError());
     return 0;

@@ -39,7 +39,7 @@ struct TcParams {
   int classes_w;                 // deconv output-parity classes along W (SW); along H it is SH
   int ksplit, chunks_per_split;
   int act;
-  const float* scale; const float* shift;
+  LayerWeights wt;               // per-voice scale / shift and the voice of each batch item (weights: the per-voice tensor maps)
   float* ws;                     // split-K workspace [ksplit][pixels][Cout] or nullptr
   size_t out_pixels;             // B * Hout * Wout
 };
@@ -53,8 +53,8 @@ __device__ __forceinline__ void wgmma_tile(float (&acc)[BLOCK_N / 2], uint64_t a
 template <int BLOCK_N, int kStages, int kMinBlocks>
 __global__ void __launch_bounds__(kTcThreads, kMinBlocks)
 k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-          const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmW,
-          const TcParams p) {
+          const __grid_constant__ TcWeightMaps tmB, const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmW,
+          const __grid_constant__ TcParams p) {
   static_assert(BLOCK_N == 64 || BLOCK_N == 128, "BLOCK_N");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   constexpr uint32_t kABytes = kBlockM * kBlockK * 2;
@@ -87,10 +87,12 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
   const int kc_begin = split * p.chunks_per_split;
   const int kc_end = min(total_chunks, kc_begin + p.chunks_per_split);
   const int my_chunks = kc_end - kc_begin;
+  const int voice = item_voice(p.wt, b);                     // this tile's batch item reads its voice's weights
+  const CUtensorMap* tmBv = &tmB.m[voice];
 
   if (threadIdx.x == kTcConsumers) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA0) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(tmBv) : "memory");
     if (p.chunks1 > 0) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA1) : "memory");
     if (!p.ws) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
     else asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW) : "memory");
@@ -98,7 +100,8 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (threadIdx.x < kTcConsumers && !p.ws) {
-    for (int i = threadIdx.x; i < BLOCK_N; i += kTcConsumers) { s_scale[i] = __ldg(p.scale + n0 + i); s_shift[i] = __ldg(p.shift + n0 + i); }
+    const float* scale = p.wt.scale[voice]; const float* shift = p.wt.shift[voice];
+    for (int i = threadIdx.x; i < BLOCK_N; i += kTcConsumers) { s_scale[i] = __ldg(scale + n0 + i); s_shift[i] = __ldg(shift + n0 + i); }
   }
   __syncthreads();
   pdl_wait();                      // the previous layer's outputs (our A operand) are complete from here on
@@ -123,7 +126,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
         mbar_expect_tx(&full_bar[s], kABytes + kBBytes);
         if (cc < p.chunks0) tma_load_4d(smem_a + s * kABytes, &tmA0, &full_bar[s], cc * kBlockK, ix, iy, b);
         else tma_load_4d(smem_a + s * kABytes, &tmA1, &full_bar[s], (cc - p.chunks0) * kBlockK, ix, iy, b);
-        tma_load_2d(smem_b + s * kBBytes, &tmB, &full_bar[s], kc * kBlockK, cls * p.Cout + n0);
+        tma_load_2d(smem_b + s * kBBytes, tmBv, &full_bar[s], kc * kBlockK, cls * p.Cout + n0);
       }
     }
   } else if (warp < kTcConsumers / 32) {
@@ -209,7 +212,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
 // slices g, g + G, g + 2G, ... ; the G partial sums are combined through shared memory in a fixed order, so the result
 // is deterministic (same summation tree every run) while G x more loads are in flight than with one thread per output.
 __global__ void __launch_bounds__(256) k_splitk_reduce(const float* __restrict__ ws, size_t total4, size_t slice_elems, int ksplit, int Cout,
-                                const float* __restrict__ scale, const float* __restrict__ shift, int act, __half* __restrict__ out,
+                                const __grid_constant__ LayerWeights wt, int act, __half* __restrict__ out,
                                 size_t band4, size_t out_stride4, size_t out_off4) {
   __shared__ float4 part[8][32];
   pdl_trigger();
@@ -230,8 +233,11 @@ __global__ void __launch_bounds__(256) k_splitk_reduce(const float* __restrict__
   __syncthreads();
   if (g != 0 || i >= total4) return;
   for (int k = 1; k < G; ++k) { const float4 b = part[k][lane]; a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w; }
-  const size_t o = (i / band4) * out_stride4 + out_off4 + i % band4;
+  const size_t item = i / band4;
+  const size_t o = item * out_stride4 + out_off4 + i % band4;
   const int n = (int)((o * 4) % Cout);
+  const int voice = item_voice(wt, (int)item);
+  const float* scale = wt.scale[voice]; const float* shift = wt.shift[voice];
   const float4 sc = __ldg(reinterpret_cast<const float4*>(scale + n)), sh = __ldg(reinterpret_cast<const float4*>(shift + n));
   float v[4] = {fmaf(a.x, sc.x, sh.x), fmaf(a.y, sc.y, sh.y), fmaf(a.z, sc.z, sh.z), fmaf(a.w, sc.w, sh.w)};
 #pragma unroll
@@ -244,7 +250,7 @@ __global__ void __launch_bounds__(256) k_splitk_reduce(const float* __restrict__
 
 // few splits, large outputs (c3 / c4 / d3): one thread per float4 of the output, grid-stride, all slices summed in order
 __global__ void __launch_bounds__(256) k_splitk_reduce_few(const float* __restrict__ ws, size_t total4, size_t slice_elems, int ksplit, int Cout,
-                                    const float* __restrict__ scale, const float* __restrict__ shift, int act, __half* __restrict__ out,
+                                    const __grid_constant__ LayerWeights wt, int act, __half* __restrict__ out,
                                     size_t band4, size_t out_stride4, size_t out_off4) {
   const size_t stride4 = slice_elems / 4;
   pdl_trigger();
@@ -257,8 +263,11 @@ __global__ void __launch_bounds__(256) k_splitk_reduce_few(const float* __restri
       const float4 b = __ldg(p + (size_t)s * stride4);
       a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
     }
-    const size_t o = (i / band4) * out_stride4 + out_off4 + i % band4;
+    const size_t item = i / band4;
+    const size_t o = item * out_stride4 + out_off4 + i % band4;
     const int n = (int)((o * 4) % Cout);
+    const int voice = item_voice(wt, (int)item);
+    const float* scale = wt.scale[voice]; const float* shift = wt.shift[voice];
     const float4 sc = __ldg(reinterpret_cast<const float4*>(scale + n)), sh = __ldg(reinterpret_cast<const float4*>(shift + n));
     float v[4] = {fmaf(a.x, sc.x, sh.x), fmaf(a.y, sc.y, sh.y), fmaf(a.z, sc.z, sh.z), fmaf(a.w, sc.w, sh.w)};
 #pragma unroll
@@ -392,6 +401,19 @@ size_t tc_splitk_ws_bytes(const ConvLayer& L, int num_sms) {
   return ks > 1 ? (size_t)ks * L.B * (r1 - r0) * L.Wout * L.Cout * sizeof(float) : 0;
 }
 
+int tc_layer_weight_maps(ConvLayer& L) {
+  RYK_CHECK(L.n_voices >= 1 && L.n_voices <= kMaxGroupVoices, "a layer holds 1..8 voices");
+  const int classes = L.transposed ? L.SH * L.SW : 1;
+  const int ntaps = L.transposed ? (L.KH / L.SH) * (L.KW / L.SW) : L.KH * L.KW;
+  const size_t K = (size_t)ntaps * (L.C0 + L.C1), rows = (size_t)classes * L.Cout;
+  for (int v = 0; v < L.n_voices; ++v) {
+    RYK_CHECK(L.w_tc[v] != nullptr, "tensor-core layer without packed weights for one of its voices");
+    if (make_weight_map(&L.tmB.m[v], L.w_tc[v], K, rows, L.block_n)) return -1;
+  }
+  for (int v = L.n_voices; v < kMaxGroupVoices; ++v) L.tmB.m[v] = L.tmB.m[0];    // never selected
+  return 0;
+}
+
 int tc_layer_prepare(ConvLayer& L, int num_sms) {
   RYK_CHECK(g_encode != nullptr, "tc_init() was not called");
   RYK_CHECK(tc_layer_eligible(L), "layer is not eligible for the tensor-core path");
@@ -400,11 +422,7 @@ int tc_layer_prepare(ConvLayer& L, int num_sms) {
   if (make_act_map(&L.tmA0, L.in0, L.C0, L.Win, L.Hin, L.B, L.tile_w, L.tile_h, stw, sth)) return -1;
   if (L.C1 > 0) { if (make_act_map(&L.tmA1, L.in1, L.C1, L.Win, L.Hin, L.B, L.tile_w, L.tile_h, stw, sth)) return -1; }
   else L.tmA1 = L.tmA0;
-  int classes = L.transposed ? L.SH * L.SW : 1;
-  int ntaps = L.transposed ? (L.KH / L.SH) * (L.KW / L.SW) : L.KH * L.KW;
-  size_t K = (size_t)ntaps * (L.C0 + L.C1);
-  size_t rows = (size_t)classes * L.Cout;
-  if (make_weight_map(&L.tmB, L.w_tc, K, rows, L.block_n)) return -1;
+  if (tc_layer_weight_maps(L)) return -1;
   // output map for the TMA-store epilogue: deconv classes write every other pixel (element strides = conv strides)
   if (make_act_map(&L.tmO, L.out, L.Cout, L.Wout, L.Hout, L.B, L.tile_w, L.tile_h, L.transposed ? L.SW : 1, L.transposed ? L.SH : 1)) return -1;
   RYK_CHECK(L.ksplit == 1 || L.splitk_ws != nullptr, "split-K layer without a workspace");
@@ -452,7 +470,7 @@ int conv_tc_run(const ConvLayer& L, cudaStream_t st) {
   p.ksplit = L.ksplit;
   int total_chunks = p.ntaps * (p.chunks0 + p.chunks1);
   p.chunks_per_split = (total_chunks + L.ksplit - 1) / L.ksplit;
-  p.act = L.act; p.scale = L.scale; p.shift = L.shift;
+  p.act = L.act; p.wt = L.wt;
   p.ws = L.ksplit > 1 ? L.splitk_ws : nullptr;
   p.out_pixels = (size_t)L.B * L.Hout * L.Wout;
   const size_t row_elems = (size_t)L.Wout * L.Cout;
@@ -465,10 +483,10 @@ int conv_tc_run(const ConvLayer& L, cudaStream_t st) {
     const size_t total4 = band_elems / 4, band4 = (r1 - r0) * row_elems / 4, stride4 = L.Hout * row_elems / 4, off4 = r0 * row_elems / 4;
     if (L.ksplit <= 4) {
       int blocks = (int)((total4 + 255) / 256); if (blocks > 2112) blocks = 2112;     // 16 per SM of 132
-      RYK_CUDA(launch_pdl(k_splitk_reduce_few, dim3(blocks), dim3(256), 0, st, (const float*)p.ws, total4, band_elems, L.ksplit, L.Cout, L.scale, L.shift, L.act,
+      RYK_CUDA(launch_pdl(k_splitk_reduce_few, dim3(blocks), dim3(256), 0, st, (const float*)p.ws, total4, band_elems, L.ksplit, L.Cout, L.wt, L.act,
                           (__half*)L.out, band4, stride4, off4));
     } else {
-      RYK_CUDA(launch_pdl(k_splitk_reduce, dim3((unsigned)((total4 + 31) / 32)), dim3(256), 0, st, (const float*)p.ws, total4, band_elems, L.ksplit, L.Cout, L.scale, L.shift, L.act,
+      RYK_CUDA(launch_pdl(k_splitk_reduce, dim3((unsigned)((total4 + 31) / 32)), dim3(256), 0, st, (const float*)p.ws, total4, band_elems, L.ksplit, L.Cout, L.wt, L.act,
                           (__half*)L.out, band4, stride4, off4));
     }
     RYK_CUDA(cudaGetLastError());

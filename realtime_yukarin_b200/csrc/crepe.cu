@@ -432,7 +432,7 @@ static int crepe_conv(Engine* e, CrepeModel* m, const CrepeWork& w, int l, const
   L.transposed = 0; L.B = F; L.Hin = 1; L.Win = Win; L.Hout = 1; L.Wout = Wout; L.C0 = Cin; L.C1 = 0; L.Cout = m->cout[l];
   L.KH = 1; L.KW = KW; L.SH = 1; L.SW = 1; L.PH = 0; L.PW = 0; L.act = ACT_RELU;
   L.in0 = x; L.in_dtype = DT_F32; L.out = y; L.out_dtype = DT_F32;
-  L.w_direct = m->d_w[l]; L.scale = m->d_ones; L.shift = m->d_bias[l];
+  L.wt.w[0] = m->d_w[l]; L.wt.scale[0] = m->d_ones; L.wt.shift[0] = m->d_bias[l];
   return conv_direct_run(L, st);
 }
 
@@ -466,7 +466,7 @@ static int crepe_network(Engine* e, CrepeModel* m, CrepeWork& w, int n16, int ho
     L.transposed = 0; L.B = F; L.Hin = 1; L.Win = 1; L.Hout = 1; L.Wout = 1; L.C0 = 4 * m->cout[5]; L.C1 = 0; L.Cout = kCrepeBins;
     L.KH = 1; L.KW = 1; L.SH = 1; L.SW = 1; L.PH = 0; L.PW = 0; L.act = ACT_NONE;
     L.in0 = w.d_flat; L.in_dtype = DT_F32; L.out = w.d_logit; L.out_dtype = DT_F32;
-    L.w_direct = m->d_dense_w; L.scale = m->d_ones; L.shift = m->d_dense_b;
+    L.wt.w[0] = m->d_dense_w; L.wt.scale[0] = m->d_ones; L.wt.shift[0] = m->d_dense_b;
     if (conv_direct_run(L, st)) return -1;
   }
   k_crepe_sigmoid<<<F, 128, 0, st>>>(w.d_logit, w.d_act, w.d_conf, w.d_obs);
@@ -597,7 +597,7 @@ int crepe_test_conv(Engine* e, int backend, int F, int Win, int Cin, int Cout, i
       ConvLayer L;
       L.transposed = 0; L.B = F; L.Hin = 1; L.Win = Win; L.Hout = 1; L.Wout = Wout; L.C0 = Cin; L.C1 = 0; L.Cout = Cout;
       L.KH = 1; L.KW = k; L.SH = 1; L.SW = 1; L.PH = 0; L.PW = 0; L.act = ACT_RELU;
-      L.in0 = d_x; L.in_dtype = DT_F32; L.out = d_y; L.out_dtype = DT_F32; L.w_direct = d_w; L.scale = d_ones; L.shift = d_b;
+      L.in0 = d_x; L.in_dtype = DT_F32; L.out = d_y; L.out_dtype = DT_F32; L.wt.w[0] = d_w; L.wt.scale[0] = d_ones; L.wt.shift[0] = d_b;
       rc = conv_direct_run(L, st);
     }
     if (!rc && (cudaMemcpyAsync(y, d_y, ny * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)) {

@@ -19,6 +19,19 @@ struct Session;
 struct Group;
 struct Reblock;
 
+// One target voice: the two U-Nets and the statistics that convert into one speaker.  Voice 0 is the engine's built-in voice (the
+// ryk_model_* / ryk_stage1_set_stats / ryk_f0_set_stats calls and the per-op API); voices >= 1 come from ryk_voice_create.
+struct Voice {
+  UNet* stage1 = nullptr;
+  UNet* stage2 = nullptr;
+  // stage-1 statistics
+  std::vector<float> s1_in_mean, s1_in_std, s1_out_mean, s1_out_std;
+  float *d_s1_in_mean = nullptr, *d_s1_in_std = nullptr, *d_s1_out_mean = nullptr, *d_s1_out_std = nullptr;
+  double f0_in_mean = 0, f0_in_std = 1, f0_tgt_mean = 0, f0_tgt_std = 1;
+  bool has_f0_stats = false;
+  int users = 0;                     // sessions and groups that convert into this voice
+};
+
 struct Engine {
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -34,14 +47,8 @@ struct Engine {
   double* d_H = nullptr; int H_order = -1, H_fft = 0; double H_alpha = 0;     // mc2sp: nb x (order+1)
   // DIO plans keyed by (n, fs, frame_period*1000, floor*1000, ceil*1000)
   std::map<std::tuple<int, int, int, int, int>, DioPlan*> dio_plans;
-  // networks
-  UNet* stage1 = nullptr;
-  UNet* stage2 = nullptr;
-  // stage-1 statistics
-  std::vector<float> s1_in_mean, s1_in_std, s1_out_mean, s1_out_std;
-  float *d_s1_in_mean = nullptr, *d_s1_in_std = nullptr, *d_s1_out_mean = nullptr, *d_s1_out_std = nullptr;
-  double f0_in_mean = 0, f0_in_std = 1, f0_tgt_mean = 0, f0_tgt_std = 1;
-  bool has_f0_stats = false;
+  // voices by id (voice 0 always exists; a destroyed voice leaves nullptr)
+  std::vector<Voice*> voices;
   // synthesizers
   std::vector<Synth*> synths;
   std::vector<Session*> sessions;
@@ -63,6 +70,11 @@ struct Engine {
 };
 
 int engine_scratch(Engine* e, size_t bytes, void** out);
+inline Voice* engine_voice(Engine* e, int id) { return id >= 0 && id < (int)e->voices.size() ? e->voices[id] : nullptr; }
+// identity stage-1 statistics of C channels unless statistics of C channels are loaded
+int voice_default_stage1_stats(Voice* v, int C);
+// both U-Nets created and every layer loaded
+bool voice_models_loaded(const Voice* v);
 int engine_pinned(Engine* e, size_t bytes, void** out);
 
 // world_analysis.cu

@@ -251,19 +251,19 @@ __global__ void k_sr_epilogue(const float* __restrict__ y, int T, int nb, int t0
   sp_out[(size_t)t * nb + k] = expf(y[(size_t)t * (nb - 1) + ks]);
 }
 
-int stage1_prologue_run(Engine* e, const float* d_mc, const int* d_index, const int* d_count, int C, float* d_x, int Tp_capacity, cudaStream_t st) {
-  k_stage1_prologue<<<1, 256, 0, st>>>(d_mc, d_index, d_count, C, e->d_s1_in_mean, e->d_s1_in_std, d_x, Tp_capacity);
+int stage1_prologue_run(const Voice* v, const float* d_mc, const int* d_index, const int* d_count, int C, float* d_x, int Tp_capacity, cudaStream_t st) {
+  k_stage1_prologue<<<1, 256, 0, st>>>(d_mc, d_index, d_count, C, v->d_s1_in_mean, v->d_s1_in_std, d_x, Tp_capacity);
   RYK_CUDA(cudaGetLastError());
   return 0;
 }
 
-int stage1_epilogue_run(Engine* e, const float* d_y, const int* d_index, const uint8_t* d_mask, const int* d_count, int T, int C,
+int stage1_epilogue_run(const Voice* v, const float* d_y, const int* d_index, const uint8_t* d_mask, const int* d_count, int T, int C,
                         const float* d_f0_in, const float* d_ap_in, const uint8_t* d_voiced_in, int nb, float silent_mc0,
                         float* d_mc_out, float* d_f0_out, float* d_ap_out, uint8_t* d_voiced_out, cudaStream_t st) {
   if (T <= 0) return 0;
-  k_stage1_epilogue<<<T, 128, 0, st>>>(d_y, d_index, d_mask, d_count, T, C, e->d_s1_out_mean, e->d_s1_out_std, d_f0_in, d_ap_in,
-                                       d_voiced_in, nb, e->f0_in_mean, e->f0_in_std, e->f0_tgt_mean, e->f0_tgt_std,
-                                       e->has_f0_stats ? 1 : 0, silent_mc0, d_mc_out, d_f0_out, d_ap_out, d_voiced_out);
+  k_stage1_epilogue<<<T, 128, 0, st>>>(d_y, d_index, d_mask, d_count, T, C, v->d_s1_out_mean, v->d_s1_out_std, d_f0_in, d_ap_in,
+                                       d_voiced_in, nb, v->f0_in_mean, v->f0_in_std, v->f0_tgt_mean, v->f0_tgt_std,
+                                       v->has_f0_stats ? 1 : 0, silent_mc0, d_mc_out, d_f0_out, d_ap_out, d_voiced_out);
   RYK_CUDA(cudaGetLastError());
   return 0;
 }

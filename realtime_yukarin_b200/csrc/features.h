@@ -5,9 +5,12 @@
 namespace ryk {
 
 struct Engine;
+struct Voice;
 
-int stage1_prologue_run(Engine* e, const float* d_mc, const int* d_index, const int* d_count, int C, float* d_x, int Tp_capacity, cudaStream_t st);
-int stage1_epilogue_run(Engine* e, const float* d_y, const int* d_index, const uint8_t* d_mask, const int* d_count, int T, int C,
+// normalisation with the stage-1 statistics of voice v
+int stage1_prologue_run(const Voice* v, const float* d_mc, const int* d_index, const int* d_count, int C, float* d_x, int Tp_capacity, cudaStream_t st);
+// de-normalisation and f0 conversion with the statistics of voice v
+int stage1_epilogue_run(const Voice* v, const float* d_y, const int* d_index, const uint8_t* d_mask, const int* d_count, int T, int C,
                         const float* d_f0_in, const float* d_ap_in, const uint8_t* d_voiced_in, int nb, float silent_mc0,
                         float* d_mc_out, float* d_f0_out, float* d_ap_out, uint8_t* d_voiced_out, cudaStream_t st);
 constexpr int kColminFloats = 64 * 512;      // column-minimum partials of the stage-2 prologue (one scratch per concurrent stream)

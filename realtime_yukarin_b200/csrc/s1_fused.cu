@@ -402,20 +402,21 @@ bool s1_fused_eligible(const UNet* n, const UNetPlan* p) {
 
 int s1_fused_run(Engine* e, const UNetPlan* p, cudaStream_t st) {
   RYK_CHECK(g_s1_cluster > 0 && p->fused, "fused stage-1 kernel not available for this plan");
+  for (const ConvLayer& L : p->layers) RYK_CHECK(L.n_voices == 1, "the fused stage-1 kernel runs plans of one voice");
   S1Params P;
   for (int i = 1; i <= 14; ++i) {
     const ConvLayer& L = p->layers[i];
     S1LayerP& Q = P.L[i - 1];
     Q.in0 = (const __half*)L.in0; Q.in1 = (const __half*)L.in1; Q.out = (__half*)L.out;
-    Q.w = (const uint4*)L.w_frag; Q.scale = L.scale; Q.shift = L.shift;
+    Q.w = (const uint4*)L.w_frag; Q.scale = L.wt.scale[0]; Q.shift = L.wt.shift[0];
     Q.transposed = L.transposed; Q.Win = L.Win; Q.C0 = L.C0; Q.C1 = L.C1; Q.Cout = L.Cout; Q.act = L.act;
     Q.lgCin = 0; while ((1 << Q.lgCin) < L.C0 + L.C1) ++Q.lgCin;
     Q.cut = s1_cut(S1Geom{L.transposed, L.Win, L.C0 + L.C1, L.Cout}, g_s1_cluster);
   }
   const ConvLayer& A = p->layers[0];
-  P.x = (const float*)A.in0; P.w0 = A.w_direct; P.sc0 = A.scale; P.sh0 = A.shift; P.enc0 = (__half*)A.out; P.in_ch = A.C0; P.base = A.Cout; P.act0 = A.act;
+  P.x = (const float*)A.in0; P.w0 = A.wt.w[0]; P.sc0 = A.wt.scale[0]; P.sh0 = A.wt.shift[0]; P.enc0 = (__half*)A.out; P.in_ch = A.C0; P.base = A.Cout; P.act0 = A.act;
   const ConvLayer& Z = p->layers[15];
-  P.yin0 = (const __half*)Z.in0; P.yin1 = (const __half*)Z.in1; P.w15 = Z.w_direct; P.sc15 = Z.scale; P.sh15 = Z.shift; P.y = (float*)Z.out;
+  P.yin0 = (const __half*)Z.in0; P.yin1 = (const __half*)Z.in1; P.w15 = Z.wt.w[0]; P.sc15 = Z.wt.scale[0]; P.sh15 = Z.wt.shift[0]; P.y = (float*)Z.out;
   P.yc0 = Z.C0; P.yc1 = Z.C1; P.out_ch = Z.Cout; P.act15 = Z.act;
   P.W = p->W;
   cudaLaunchConfig_t cfg = {};

@@ -23,6 +23,7 @@
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <array>
 #include <numeric>
 #include <vector>
@@ -80,6 +81,7 @@ struct Session {
   int s1_owner = 0, s2_owner[2] = {0, 0};
   float* d_colmin[2] = {nullptr, nullptr};
   Group* group = nullptr; int slot = 0;        // member of a batched stage-2 group (config 5), else nullptr
+  Voice* voice = nullptr; int voice_id = 0;    // the voice the session converts into (fixed for its lifetime)
   ryk_session_config cfg;
   int hop, rate, n_wave, n_feat, e_wave, e_enc_frames, e_conv, e_dec;
   int Lw, Tw, Td, nb, C;
@@ -139,8 +141,9 @@ struct Session {
 // stages carry per-stream state and data-dependent lengths, and they are a small share of the SM time.
 struct Group {
   std::vector<Session*> members;
+  std::vector<Voice*> voices;                  // the members' distinct voices in the order of their first member; p2 lives on voices[0]
   int owner = 0;                               // plan-cache owner id of p2
-  UNetPlan* p2 = nullptr;                      // stage-2 plan at batch = members.size()
+  UNetPlan* p2 = nullptr;                      // stage-2 plan at batch = members.size(), member i on the weights of its voice
   cudaStream_t sG = nullptr;
   cudaEvent_t ev_fwd[kRing] = {};              // batched forward of step r done
   long long step = 0, collected = 0;
@@ -482,12 +485,12 @@ static int stage1_body(Engine* e, Session* s, int b, int tp1) {
   const float* d_y = nullptr;
   if (tp1 > 0) {
     UNetPlan* p1 = nullptr;
-    if (unet_get_plan(e, e->stage1, 1, 1, tp1, e->precision, &p1, s->s1_owner)) return -1;
-    if (stage1_prologue_run(e, s->cw_mc[g], s->d_index[b], s->d_count[b], s->C, (float*)p1->d_in, tp1, s->sC)) return -1;
+    if (unet_get_plan(e, s->voice->stage1, 1, 1, tp1, e->precision, &p1, s->s1_owner)) return -1;
+    if (stage1_prologue_run(s->voice, s->cw_mc[g], s->d_index[b], s->d_count[b], s->C, (float*)p1->d_in, tp1, s->sC)) return -1;
     if (unet_forward(e, p1, s->sC)) return -1;
     d_y = (const float*)p1->d_out;
   }
-  if (stage1_epilogue_run(e, d_y, s->d_index[b], s->d_mask[b], s->d_count[b], s->Tw, s->C, s->cw_f0[g], s->cw_ap[g], s->cw_voiced[g], s->nb,
+  if (stage1_epilogue_run(s->voice, d_y, s->d_index[b], s->d_mask[b], s->d_count[b], s->Tw, s->C, s->cw_f0[g], s->cw_ap[g], s->cw_voiced[g], s->nb,
                           kSilentMc0, s->cv_mc_out[b], s->cv_f0_out[b], s->cv_ap_out[b], s->cv_voiced_out[b], s->sC)) return -1;
   return mc2sp_run(e, s->cv_mc_out[b], s->Tw, c.order, c.fft_length, 1e-16, s->cv_sp_mid[b], nullptr, s->sC);
 }
@@ -504,7 +507,7 @@ static cudaStream_t s2_stream(const Session* s, int b) { return s->sC2s[s->group
 // The decode slide reads only the chunk's frames [e_conv, e_conv + n_feat) of the converted window, so stage 2 computes only the
 // decoder rows those frames depend on.
 static int s2_plan(Engine* e, const Session* s, int b, UNetPlan** p2) {
-  return unet_get_plan(e, e->stage2, 1, s->Tp, 512, e->precision, p2, s->s2_owner[b], s->e_conv, s->n_feat);
+  return unet_get_plan(e, s->voice->stage2, 1, s->Tp, 512, e->precision, p2, s->s2_owner[b], s->e_conv, s->n_feat);
 }
 
 // begin (which = 0) / end (1) of a stage in the RYK_STAGE_TIMES timeline
@@ -740,23 +743,39 @@ extern "C" {
 
 static int session_build(Engine* e, Session* s, const ryk_session_config* cfg);
 
-int ryk_session_create(ryk_engine* h, const ryk_session_config* cfg, int* session_id) {
+int ryk_session_create_voice(ryk_engine* h, const ryk_session_config* cfg, int voice_id, int* session_id) {
   Engine* e = &h->impl;
   RYK_CUDA(cudaSetDevice(e->device));
   RYK_CHECK(cfg && session_id, "null argument");
-  RYK_CHECK(e->stage1 && e->stage2, "load both models before creating a session");
+  Voice* v = engine_voice(e, voice_id);
+  RYK_CHECK(v != nullptr, "no such voice");
+  RYK_CHECK(v->stage1 && v->stage2, "load both models before creating a session");
+  if (voice_id >= 1) {
+    RYK_CHECK(voice_models_loaded(v), "load every layer of both of the voice's models before creating a session on it");
+    if (voice_default_stage1_stats(v, v->stage1->in_ch)) return -1;
+  }
   Session* s = new Session();
+  s->voice = v; s->voice_id = voice_id;
   if (session_build(e, s, cfg)) {
     // free whatever the build made (buffers, analysis / CREPE plans, graphs, U-Net plans); ryk_last_error keeps the cause
     const int s1_owner = s->s1_owner, s2_owner[2] = {s->s2_owner[0], s->s2_owner[1]};
     session_free(s);
-    if (s1_owner) unet_release_owner(e->stage1, s1_owner);
-    for (int owner : s2_owner) if (owner) unet_release_owner(e->stage2, owner);
+    if (s1_owner) unet_release_owner(v->stage1, s1_owner);
+    for (int owner : s2_owner) if (owner) unet_release_owner(v->stage2, owner);
     return -1;
   }
+  v->users++;
   e->sessions.push_back(s);
   *session_id = (int)e->sessions.size() - 1;
   return 0;
+}
+
+int ryk_session_create(ryk_engine* h, const ryk_session_config* cfg, int* session_id) { return ryk_session_create_voice(h, cfg, 0, session_id); }
+
+int ryk_session_voice(ryk_engine* h, int id) {
+  Session* s = get_session(&h->impl, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  return s->voice_id;
 }
 
 // Everything a session allocates and captures; on failure the caller frees the partly built session.
@@ -778,7 +797,7 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
   s->C = cfg->order + 1;
   RYK_CHECK(s->n_wave == s->n_feat * s->hop && s->e_wave == s->e_enc_frames * s->hop, "buffer_time / encode_extra_time must be whole frames");
   RYK_CHECK(s->Lw / s->hop - 2 * s->e_enc_frames == s->n_feat, "encode window does not trim to one chunk of frames");
-  RYK_CHECK(s->nb == 513 && e->stage1->in_ch == s->C, "session configuration does not match the loaded models");
+  RYK_CHECK(s->nb == 513 && s->voice->stage1->in_ch == s->C, "session configuration does not match the loaded models");
   // the synthesizer's spectra are cheaptrick_fft_size(fs) / 2 + 1 bins wide and read rows of the fft_length / 2 + 1 bin decode window
   RYK_CHECK(cheaptrick_fft_size(cfg->fs, 71.0) / 2 + 1 == s->nb,
             "fs does not match fft_length: the synthesizer at this fs needs a different spectrum width (run the session at the model's "
@@ -862,7 +881,7 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
   UNetPlan* p = nullptr;
   s->s1_owner = ++e->plan_owners;
   for (int b = 0; b < 2; ++b) s->s2_owner[b] = ++e->plan_owners;
-  for (int Tp = 128; Tp <= s->Tp; Tp += 128) if (unet_get_plan(e, e->stage1, 1, 1, Tp, e->precision, &p, s->s1_owner)) return -1;
+  for (int Tp = 128; Tp <= s->Tp; Tp += 128) if (unet_get_plan(e, s->voice->stage1, 1, 1, Tp, e->precision, &p, s->s1_owner)) return -1;
   // (the stage-2 plans are created on first use: a session that joins a group never needs its own)
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   RYK_CUDA(cudaDeviceSynchronize());
@@ -877,9 +896,11 @@ int ryk_session_destroy(ryk_engine* h, int id) {
   RYK_CHECK(s->group == nullptr, "session belongs to a group: destroy the group first");
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   const int s1_owner = s->s1_owner, s2_owner[2] = {s->s2_owner[0], s->s2_owner[1]};
+  Voice* v = s->voice;
   session_free(s);                         // synchronises the session's streams
-  unet_release_owner(e->stage1, s1_owner);
-  for (int owner : s2_owner) unet_release_owner(e->stage2, owner);
+  unet_release_owner(v->stage1, s1_owner);
+  for (int owner : s2_owner) unet_release_owner(v->stage2, owner);
+  v->users--;
   e->sessions[id] = nullptr;
   return 0;
 }
@@ -1065,18 +1086,44 @@ int ryk_group_create(ryk_engine* h, const int* session_ids, int n_sessions, int*
     s->group = G; s->slot = i;
     G->members.push_back(s);
   }
+  // Members of different voices share the forward: each batch item reads its voice's weights (unet_plan_set_voices).
+  std::vector<int> voice_of;
+  for (Session* m : G->members) {
+    const auto it = std::find(G->voices.begin(), G->voices.end(), m->voice);
+    voice_of.push_back((int)(it - G->voices.begin()));
+    if (it == G->voices.end()) G->voices.push_back(m->voice);
+  }
+  const UNet* n0 = G->voices[0]->stage2;
+  const char* refusal = nullptr;
+  if (G->voices.size() > 1 && e->precision != 1) refusal = "a group of several voices needs precision 1 (FP16 tensor cores)";
+  else if ((int)G->voices.size() > kMaxGroupVoices) refusal = "a group holds at most 8 distinct voices";
+  for (const Voice* v : G->voices)
+    if (!refusal && (v->stage2->in_ch != n0->in_ch || v->stage2->out_ch != n0->out_ch || v->stage2->base != n0->base))
+      refusal = "the members' stage-2 models must have the same (in, out, base) channels";
+  if (refusal) {
+    group_free(G);
+    set_error(refusal);
+    return -1;
+  }
+  std::vector<const UNet*> nets;
+  for (const Voice* v : G->voices) nets.push_back(v->stage2);
   // the batched forward computes the decoder rows of the hull of the members' kept frames (their e_conv may differ)
   std::vector<int> kb, kl;
   for (Session* m : G->members) { kb.push_back(m->e_conv); kl.push_back(m->n_feat); }
   int keep_begin = 0, keep_len = 0;
   keep_hull(n_sessions, kb.data(), kl.data(), &keep_begin, &keep_len);
-  if (unet_get_plan(e, e->stage2, n_sessions, G->members[0]->Tp, 512, e->precision, &G->p2, G->owner, keep_begin, keep_len)) {
+  if (unet_get_plan(e, G->voices[0]->stage2, n_sessions, G->members[0]->Tp, 512, e->precision, &G->p2, G->owner, keep_begin, keep_len) ||
+      unet_plan_set_voices(G->p2, nets, voice_of)) {
+    const int owner = G->owner;
+    UNet* net = G->voices[0]->stage2;
     group_free(G);
+    unet_release_owner(net, owner);
     return -1;
   }
   { int lo = 0, hi = 0; RYK_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi)); RYK_CUDA(cudaStreamCreateWithPriority(&G->sG, cudaStreamNonBlocking, lo)); }
   for (int i = 0; i < kRing; ++i) RYK_CUDA(cudaEventCreateWithFlags(&G->ev_fwd[i], cudaEventDisableTiming));
   RYK_CUDA(cudaDeviceSynchronize());
+  for (Voice* v : G->voices) v->users++;
   e->groups.push_back(G);
   *group_id = (int)e->groups.size() - 1;
   return 0;
@@ -1088,8 +1135,10 @@ int ryk_group_destroy(ryk_engine* h, int group_id) {
   RYK_CHECK(G != nullptr, "no such group");
   RYK_CUDA(cudaDeviceSynchronize());
   const int owner = G->owner;
+  const std::vector<Voice*> voices = G->voices;
   group_free(G);                     // the member sessions survive (ungrouped) and are destroyed separately
-  unet_release_owner(e->stage2, owner);
+  unet_release_owner(voices[0]->stage2, owner);
+  for (Voice* v : voices) v->users--;
   e->groups[group_id] = nullptr;
   return 0;
 }

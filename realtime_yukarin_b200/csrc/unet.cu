@@ -23,6 +23,7 @@ static int dec_out_channels(int base, int i) {     // decoder c0..c6 output chan
   return base * mult[i];
 }
 
+// The layer shapes are restated in Python (engine._unet_layer_shapes, which checks the model files of voices >= 1); change both together.
 UNet* unet_create(int ndim, int in_ch, int out_ch, int base) {
   UNet* n = new UNet();
   n->ndim = ndim; n->in_ch = in_ch; n->out_ch = out_ch; n->base = base;
@@ -190,8 +191,8 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
     const UNetLayerW& LW = n->layers[i];
     ConvLayer& L = p->layers[i];
     unet_layer_shape(n, i, B, H, W, L);
-    L.w_direct = LW.d_w_direct; L.w_tc = LW.d_w_tc; L.w_frag = LW.d_w_frag; L.scale = LW.d_scale; L.shift = LW.d_shift;
-    L.host_scale_valid = true; L.host_scale = LW.h_scale0; L.host_shift = LW.h_shift0;
+    L.wt.w[0] = LW.d_w_direct; L.w_tc[0] = LW.d_w_tc; L.w_frag = LW.d_w_frag; L.wt.scale[0] = LW.d_scale; L.wt.shift[0] = LW.d_shift;
+    L.host_scale_valid = true; L.wt.host_scale[0] = LW.h_scale0; L.wt.host_shift[0] = LW.h_shift0;
     L.in_dtype = act_dt; L.out_dtype = act_dt;
     if (i == 0) {
       L.in0 = p->d_in; L.in_dtype = DT_F32; L.out = enc[0];
@@ -209,7 +210,7 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
   }
   // The decoder computes a row band only where every layer of it runs on a kernel that supports one.
   bool bandable = keep_len > 0 && n->ndim == 2 && precision == 1 && conv_direct_band_supported(p->layers[15]);
-  for (int i = 8; i < 15; ++i) bandable = bandable && p->layers[i].w_tc && tc_layer_eligible(p->layers[i]);
+  for (int i = 8; i < 15; ++i) bandable = bandable && p->layers[i].w_tc[0] && tc_layer_eligible(p->layers[i]);
   if (bandable) {
     p->keep_begin = keep_begin; p->keep_len = keep_len;
     unet_derive_bands(p->layers, keep_begin, keep_len);
@@ -224,13 +225,13 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
   // workspace only after its programmatic-launch wait, i.e. after the previous layer's reduce kernel has finished reading it.
   size_t ws_bytes = 0;
   for (int i = 0; i < 16; ++i)
-    if (precision == 1 && p->layers[i].w_tc && tc_layer_eligible(p->layers[i]))
+    if (precision == 1 && p->layers[i].w_tc[0] && tc_layer_eligible(p->layers[i]))
       ws_bytes = std::max(ws_bytes, tc_splitk_ws_bytes(p->layers[i], num_sms));
   void* ws = nullptr;
   if (ws_bytes && alloc(ws_bytes, &ws)) return -1;
   for (int i = 0; i < 16; ++i) {
     ConvLayer& L = p->layers[i];
-    if (precision == 1 && L.w_tc && tc_layer_eligible(L)) {
+    if (precision == 1 && L.w_tc[0] && tc_layer_eligible(L)) {
       if (tc_splitk_ws_bytes(L, num_sms)) L.splitk_ws = (float*)ws;
       if (tc_layer_prepare(L, num_sms)) return -1;
     }
@@ -239,6 +240,34 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
   p->fused = s1_fused_eligible(n, p);
   n->plans[key] = p;
   *out = p;
+  return 0;
+}
+
+int unet_plan_set_voices(UNetPlan* p, const std::vector<const UNet*>& nets, const std::vector<int>& voice_of) {
+  const int V = (int)nets.size();
+  RYK_CHECK(V >= 1 && V <= kMaxGroupVoices && (int)voice_of.size() == p->B && p->B <= kMaxGroupBatch, "a plan holds 1..8 voices over 1..64 batch items");
+  for (const UNet* n : nets)
+    RYK_CHECK(n->ndim == nets[0]->ndim && n->in_ch == nets[0]->in_ch && n->out_ch == nets[0]->out_ch && n->base == nets[0]->base,
+              "the voices of one plan must have U-Nets of the same shape");
+  for (int b = 0; b < p->B; ++b) RYK_CHECK(voice_of[b] >= 0 && voice_of[b] < V, "batch item of an unknown voice");
+  // Only the tensor-core kernel and the stage-2 edge-layer kernels read weights per batch item: at other widths than base 64 some
+  // layer runs on the generic CUDA-core kernel, so a plan of several voices is refused here, before any forward is captured.
+  if (V > 1)
+    for (const ConvLayer& L : p->layers)
+      RYK_CHECK(L.tc_ready || conv_direct_per_item_weights(L),
+                "a plan of several voices needs every layer on a kernel that reads weights per batch item (FP16 stage-2 nets of base 64)");
+  for (int i = 0; i < 16; ++i) {
+    ConvLayer& L = p->layers[i];
+    L.n_voices = V;
+    for (int v = 0; v < V; ++v) {
+      const UNetLayerW& LW = nets[v]->layers[i];
+      RYK_CHECK(LW.loaded, "U-Net layer weights not loaded");
+      L.wt.w[v] = LW.d_w_direct; L.w_tc[v] = LW.d_w_tc; L.wt.scale[v] = LW.d_scale; L.wt.shift[v] = LW.d_shift;
+      L.wt.host_scale[v] = LW.h_scale0; L.wt.host_shift[v] = LW.h_shift0;
+    }
+    for (int b = 0; b < p->B; ++b) L.wt.voice_of[b] = (uint8_t)voice_of[b];
+    if (L.tc_ready && tc_layer_weight_maps(L)) return -1;
+  }
   return 0;
 }
 

@@ -50,6 +50,9 @@ int unet_set_layer(Engine* e, UNet* n, int idx, const float* W, const float* sca
 int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPlan** out, int owner = 0, int keep_begin = 0,
                   int keep_len = 0, bool full_ksplit = false);
 void unet_release_owner(UNet* n, int owner);
+// Per-batch-item weights of a mixed-voice group's plan (built on nets[0]): batch item b runs on the weights of nets[voice_of[b]].  The
+// nets must have the same shape; the tile grid, K order and split-K stay those of the plan, so only the weights differ per item.
+int unet_plan_set_voices(UNetPlan* p, const std::vector<const UNet*>& nets, const std::vector<int>& voice_of);
 // Fill the geometry of layer i of net n for a (B, H, W) input (shapes, kernel, stride, padding, channels; no pointers).
 void unet_layer_shape(const UNet* n, int i, int B, int H, int W, ConvLayer& L);
 // Row bands of the 2-D decoder (layers 8..15) for a caller that reads output rows [keep_begin, keep_begin + keep_len): writes

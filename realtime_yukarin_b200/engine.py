@@ -61,6 +61,8 @@ EXPORTED_SYMBOLS = [
     'ryk_crepe_create', 'ryk_crepe_set_conv', 'ryk_crepe_set_dense', 'ryk_crepe_set_decoder_tables', 'ryk_crepe_num_frames', 'ryk_crepe_predict',
     'ryk_crepe_set_resampler', 'ryk_crepe_test_conv', 'ryk_crepe_test_network', 'ryk_stage2_row_bands', 'ryk_test_stage2_forward',
     'ryk_session_set_input_rate', 'ryk_session_set_output_rate', 'ryk_session_io_geometry',
+    'ryk_voice_create', 'ryk_voice_destroy', 'ryk_voice_model_create', 'ryk_voice_model_set_layer', 'ryk_voice_stage1_set_stats',
+    'ryk_voice_f0_set_stats', 'ryk_session_create_voice', 'ryk_session_voice',
 ]
 
 
@@ -72,6 +74,16 @@ def stage2_row_bands(Tp: int, W: int, keep_begin: int, keep_len: int) -> numpy.n
     if lib.ryk_stage2_row_bands(int(Tp), int(W), int(keep_begin), int(keep_len), out.ctypes.data_as(c_int_p)) < 0:
         raise RykError(lib.ryk_last_error().decode('utf-8', 'replace'))
     return out
+
+
+def _unet_layer_shapes(stage: int, in_ch: int, out_ch: int, base: int):
+    """(transposed, cin, cout, k) of the 16 layers of a U-Net (csrc/unet.cu unet_create): the layer shapes of a voice >= 1, which the
+    C ABI does not report."""
+    lvl = [base * m for m in (1, 2, 4, 8, 8, 8, 8, 8)]
+    dec = [base * m for m in (8, 8, 8, 8, 4, 2, 1)]
+    shapes = [(False, in_ch, base, 3)] + [(False, lvl[i - 1], lvl[i], 4) for i in range(1, 8)]
+    shapes += [(True, lvl[7] if d == 0 else dec[d - 1] + lvl[7 - d], dec[d], 4) for d in range(7)]
+    return shapes + [(False, 2 * base, out_ch, 3)]
 
 
 def load_library() -> ctypes.CDLL:
@@ -120,6 +132,7 @@ class Engine(object):
         self._synth_block = {}
         self._reblock_chunk = {}           # re-blocker id -> out_audio_chunk
         self._session_fs = {}              # session id -> the session's (model) rate
+        self._voice_shapes = {}            # voice id >= 1 -> stage -> the 16 (transposed, cin, cout, k) of its U-Net
 
     # ---- plumbing ----
     def _check(self, rc: int):
@@ -216,27 +229,60 @@ class Engine(object):
                                               int(n_frames), _bp(mask)))
         return mask.astype(bool)
 
-    # ---- models ----
-    def model_create(self, stage: int, in_channels: int, out_channels: int, base_channels: int):
-        self._check(self.lib.ryk_model_create(self._h, stage, in_channels, out_channels, base_channels))
+    # ---- voices: voice 0 is the engine's built-in voice (the per-op calls use it); voice_create adds more ----
+    def voice_create(self) -> int:
+        vid = ctypes.c_int()
+        self._check(self.lib.ryk_voice_create(self._h, ctypes.byref(vid)))
+        self._voice_shapes[vid.value] = {}
+        return vid.value
 
-    def model_layer_shape(self, stage: int, layer: int):
+    def voice_destroy(self, voice: int):
+        """Free a voice >= 1 and its weights (fails while a session or group uses it)."""
+        self._check(self.lib.ryk_voice_destroy(self._h, int(voice)))
+        self._voice_shapes.pop(int(voice), None)
+
+    def session_voice(self, sid: int) -> int:
+        return self._check(self.lib.ryk_session_voice(self._h, sid))
+
+    # ---- models (voice 0 goes through the original entry points) ----
+    def model_create(self, stage: int, in_channels: int, out_channels: int, base_channels: int, voice: int = 0):
+        if voice == 0:
+            self._check(self.lib.ryk_model_create(self._h, stage, in_channels, out_channels, base_channels))
+            return
+        self._check(self.lib.ryk_voice_model_create(self._h, int(voice), stage, in_channels, out_channels, base_channels))
+        self._voice_shapes[int(voice)][int(stage)] = _unet_layer_shapes(stage, in_channels, out_channels, base_channels)
+
+    def model_layer_shape(self, stage: int, layer: int, voice: int = 0):
+        if voice != 0:
+            shapes = self._voice_shapes.get(int(voice), {}).get(int(stage))
+            if shapes is None or not 0 <= layer < 16:
+                raise RykError(f'voice {voice}: no stage-{stage} model created, or no such layer')
+            return shapes[layer]
         tr, cin, cout, k = ctypes.c_int(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
         self._check(self.lib.ryk_model_layer_shape(self._h, stage, layer, ctypes.byref(tr), ctypes.byref(cin),
                                                    ctypes.byref(cout), ctypes.byref(k)))
         return bool(tr.value), cin.value, cout.value, k.value
 
-    def model_set_layer(self, stage: int, layer: int, W, scale, shift):
+    def model_set_layer(self, stage: int, layer: int, W, scale, shift, voice: int = 0):
         W, scale, shift = _f32(W), _f32(scale), _f32(shift)
-        self._check(self.lib.ryk_model_set_layer(self._h, stage, layer, _fp(W), _fp(scale), _fp(shift)))
+        if voice == 0:
+            self._check(self.lib.ryk_model_set_layer(self._h, stage, layer, _fp(W), _fp(scale), _fp(shift)))
+        else:
+            self._check(self.lib.ryk_voice_model_set_layer(self._h, int(voice), stage, layer, _fp(W), _fp(scale), _fp(shift)))
 
-    def stage1_set_stats(self, in_mean, in_std, out_mean, out_std):
+    def stage1_set_stats(self, in_mean, in_std, out_mean, out_std, voice: int = 0):
         a, b, c, d = _f32(in_mean), _f32(in_std), _f32(out_mean), _f32(out_std)
-        self._check(self.lib.ryk_stage1_set_stats(self._h, len(a), _fp(a), _fp(b), _fp(c), _fp(d)))
+        if voice == 0:
+            self._check(self.lib.ryk_stage1_set_stats(self._h, len(a), _fp(a), _fp(b), _fp(c), _fp(d)))
+        else:
+            self._check(self.lib.ryk_voice_stage1_set_stats(self._h, int(voice), len(a), _fp(a), _fp(b), _fp(c), _fp(d)))
 
-    def f0_set_stats(self, in_mean, in_std, target_mean, target_std):
-        self._check(self.lib.ryk_f0_set_stats(self._h, ctypes.c_double(in_mean), ctypes.c_double(in_std),
-                                              ctypes.c_double(target_mean), ctypes.c_double(target_std)))
+    def f0_set_stats(self, in_mean, in_std, target_mean, target_std, voice: int = 0):
+        args = [ctypes.c_double(in_mean), ctypes.c_double(in_std), ctypes.c_double(target_mean), ctypes.c_double(target_std)]
+        if voice == 0:
+            self._check(self.lib.ryk_f0_set_stats(self._h, *args))
+        else:
+            self._check(self.lib.ryk_voice_f0_set_stats(self._h, int(voice), *args))
 
     def stage1_convert(self, x) -> numpy.ndarray:
         x = _f32(x)
@@ -452,9 +498,12 @@ class Engine(object):
         return y
 
     # ---- sessions ----
-    def session_create(self, cfg: SessionConfig) -> int:
+    def session_create(self, cfg: SessionConfig, voice: int = 0) -> int:
         sid = ctypes.c_int()
-        self._check(self.lib.ryk_session_create(self._h, ctypes.byref(cfg), ctypes.byref(sid)))
+        if voice == 0:
+            self._check(self.lib.ryk_session_create(self._h, ctypes.byref(cfg), ctypes.byref(sid)))
+        else:
+            self._check(self.lib.ryk_session_create_voice(self._h, ctypes.byref(cfg), int(voice), ctypes.byref(sid)))
         self._session_fs[sid.value] = int(cfg.fs)
         return sid.value
 

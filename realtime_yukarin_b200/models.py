@@ -61,20 +61,34 @@ def fold_layers(params: Dict[str, numpy.ndarray]):
     return layers
 
 
-def upload_unet(engine: Engine, stage: int, params: Dict[str, numpy.ndarray]):
+def upload_unet(engine: Engine, stage: int, params: Dict[str, numpy.ndarray], voice: int = 0):
     layers = fold_layers(params)
     w0 = layers[0][0]
     in_ch, base = w0.shape[1], w0.shape[0]
     out_ch = layers[15][0].shape[0]
-    engine.model_create(stage, in_ch, out_ch, base)
+    kw = {'voice': voice} if voice else {}          # voice 0: the calls existing callers make
+    engine.model_create(stage, in_ch, out_ch, base, **kw)
     for i, (W, scale, shift) in enumerate(layers):
-        tr, cin, cout, k = engine.model_layer_shape(stage, i)
+        tr, cin, cout, k = engine.model_layer_shape(stage, i, **kw)
         expect = (cin, cout) if tr else (cout, cin)
         if tuple(W.shape[:2]) != expect or W.shape[-1] != k:
             raise ValueError(f'stage {stage} layer {i}: weight shape {W.shape} does not match the U-Net topology '
                              f'(transposed={tr}, cin={cin}, cout={cout}, k={k})')
-        engine.model_set_layer(stage, i, W, scale, shift)
+        engine.model_set_layer(stage, i, W, scale, shift, **kw)
     return in_ch, out_ch, base
+
+
+def load_voice(engine: Engine, voice: int, *, stage1_model_path, stage2_model_path, input_statistics_path, target_statistics_path,
+               feature_stats=None) -> None:
+    """Load one target voice into `engine` (voice 0, or an id from engine.voice_create()): both U-Nets, the stage-1 feature
+    statistics and the log-f0 statistics, with the same model-file rules as AcousticConverter / SuperResolution / F0Converter.
+    Sessions created with engine.session_create(cfg, voice=voice) then convert into it."""
+    params = load_npz(stage1_model_path)
+    in_ch, out_ch, _ = upload_unet(engine, 1, params, voice=voice)
+    stats = load_stage1_stats(params, stage1_model_path, in_ch, out_ch, feature_stats)
+    upload_unet(engine, 2, load_npz(stage2_model_path), voice=voice)
+    engine.stage1_set_stats(*stats, voice=voice)
+    engine.f0_set_stats(*F0Converter(input_statistics_path, target_statistics_path).stats(), voice=voice)
 
 
 class F0Converter(object):

@@ -80,10 +80,11 @@ class OutputReblocker(object):
 class RealtimePipeline(object):
     """encode_worker | convert_worker | decode_worker of one audio stream as one device-resident session.
 
-    The models must already be loaded into `engine` (YukarinConverter.make_yukarin_converter does that).  `depth` chunks may
-    be in flight (the reference's queues are unbounded; the session keeps up to 5 steps in flight)."""
+    The models must already be loaded into `engine` (YukarinConverter.make_yukarin_converter does that for voice 0,
+    models.load_voice for any voice); the session converts into `voice`.  `depth` chunks may be in flight (the reference's queues
+    are unbounded; the session keeps up to 5 steps in flight)."""
 
-    def __init__(self, config: Config, acoustic_param=None, engine: Optional[Engine] = None, depth: int = 3):
+    def __init__(self, config: Config, acoustic_param=None, engine: Optional[Engine] = None, depth: int = 3, voice: int = 0):
         self.config = config
         self.engine = engine or default_engine()
         p = acoustic_param
@@ -115,7 +116,7 @@ class RealtimePipeline(object):
             prev = os.environ.get('RYK_STAGE_TIMES')
             os.environ['RYK_STAGE_TIMES'] = '1'
         try:
-            self._sid = self.engine.session_create(cfg)
+            self._sid = self.engine.session_create(cfg, voice=voice) if voice else self.engine.session_create(cfg)
         finally:
             if self._timing:
                 if prev is None:
