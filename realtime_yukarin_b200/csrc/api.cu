@@ -214,7 +214,8 @@ int ryk_engine_destroy(ryk_engine* h) {
   for (Synth* s : e->synths) synth_destroy(s);
   session_destroy_all(e);
   crepe_destroy();                                  // after the sessions: their CREPE plans are counted on the model
-  void* ptrs[] = {e->d_colmin, e->d_launches, e->d_twiddle, e->d_jump, e->d_G, e->d_H, e->d_scratch};
+  for (auto& kv : e->sptk) { cudaFree(kv.second.d_G); cudaFree(kv.second.d_H); }
+  void* ptrs[] = {e->d_colmin, e->d_launches, e->d_twiddle, e->d_jump, e->d_scratch};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (e->h_pinned) cudaFreeHost(e->h_pinned);
   cudaStreamDestroy(e->stream);
@@ -324,7 +325,8 @@ int ryk_world_analyze(ryk_engine* h, const float* wave, int n, int fs, double fp
   int n_out = n / hop;
   if (n_out <= 0) return 0;
   int nb = fft_length / 2 + 1;
-  if (sptk_prepare(e, order, alpha, fft_length)) return -1;
+  SptkMats mats;
+  if (sptk_prepare(e, order, alpha, fft_length, &mats)) return -1;
   DioPlan* plan = nullptr;
   if (dio_get_plan(e, n, fs, fp, f0_floor, f0_ceil, &plan)) return -1;
   void* scratch = nullptr;
@@ -344,7 +346,8 @@ int ryk_world_analyze(ryk_engine* h, const float* wave, int n, int fs, double fp
   } else {
     if (dio_stonemask_run(e, plan, d_x, e->stream)) return -1;
   }
-  if (spectral_analysis_run(e, d_x, n, fs, fp, dio_plan_f0(plan), n_out, fft_length, order, d_sp, d_ap, d_mc, d_f0, d_v, e->stream)) return -1;
+  if (spectral_analysis_run(e, d_x, n, fs, fp, dio_plan_f0(plan), n_out, fft_length, order, mats.d_G, d_sp, d_ap, d_mc, d_f0, d_v, e->stream))
+    return -1;
   if (f0) RYK_CUDA(cudaMemcpyAsync(f0, d_f0, sizeof(float) * n_out, cudaMemcpyDeviceToHost, e->stream));
   if (sp) RYK_CUDA(cudaMemcpyAsync(sp, d_sp, sizeof(float) * n_out * nb, cudaMemcpyDeviceToHost, e->stream));
   if (ap) RYK_CUDA(cudaMemcpyAsync(ap, d_ap, sizeof(float) * n_out * nb, cudaMemcpyDeviceToHost, e->stream));
@@ -506,7 +509,8 @@ int ryk_mc2sp(ryk_engine* h, const float* mc, int T, int order, double alpha, in
   Engine* e = E(h);
   RYK_CUDA(cudaSetDevice(e->device));
   if (T <= 0) return 0;
-  if (sptk_prepare(e, order, alpha, fftlen)) return -1;
+  SptkMats mats;
+  if (sptk_prepare(e, order, alpha, fftlen, &mats)) return -1;
   int nb = fftlen / 2 + 1;
   void* scratch = nullptr;
   if (engine_scratch(e, arena_need({sizeof(float) * T * (order + 1), sizeof(double) * T * nb}), &scratch)) return -1;
@@ -514,7 +518,7 @@ int ryk_mc2sp(ryk_engine* h, const float* mc, int T, int order, double alpha, in
   float* d_mc = A.take<float>((size_t)T * (order + 1));
   double* d_sp = A.take<double>((size_t)T * nb);
   RYK_CUDA(cudaMemcpyAsync(d_mc, mc, sizeof(float) * T * (order + 1), cudaMemcpyHostToDevice, e->stream));
-  if (mc2sp_run(e, d_mc, T, order, fftlen, 0.0, nullptr, d_sp, e->stream)) return -1;
+  if (mc2sp_run(e, mats.d_H, d_mc, T, order, fftlen, 0.0, nullptr, d_sp, e->stream)) return -1;
   RYK_CUDA(cudaMemcpyAsync(sp, d_sp, sizeof(double) * T * nb, cudaMemcpyDeviceToHost, e->stream));
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   return 0;
@@ -553,7 +557,8 @@ int ryk_convert_window(ryk_engine* h, const float* wave, int n_wave, int fs, int
   const int nb = fftlen / 2 + 1, C = order + 1;
   RYK_CHECK(nb == 513, "stage 2 expects 513-bin spectra");
   RYK_CHECK(v->stage1->in_ch == C && v->stage1->out_ch == C, "stage-1 channel count does not match order + 1");
-  if (sptk_prepare(e, order, alpha, fftlen)) return -1;
+  SptkMats mats;
+  if (sptk_prepare(e, order, alpha, fftlen, &mats)) return -1;
   if (voice_default_stage1_stats(v, C)) return -1;
   ConvertBuffers cb;
   if (convert_buffers_get(e, T, n_wave, nb, C, &cb)) return -1;
@@ -563,7 +568,7 @@ int ryk_convert_window(ryk_engine* h, const float* wave, int n_wave, int fs, int
   RYK_CUDA(cudaMemcpyAsync(cb.d_ap, ap, sizeof(float) * T * nb, cudaMemcpyHostToDevice, st));
   RYK_CUDA(cudaMemcpyAsync(cb.d_mc, mc, sizeof(float) * T * C, cudaMemcpyHostToDevice, st));
   RYK_CUDA(cudaMemcpyAsync(cb.d_voiced, voiced, T, cudaMemcpyHostToDevice, st));
-  if (convert_window_device(e, cb, T, n_wave, frame_length, hop, threshold_db, order, fftlen, st)) return -1;
+  if (convert_window_device(e, cb, T, n_wave, frame_length, hop, threshold_db, order, fftlen, mats.d_H, st)) return -1;
   RYK_CUDA(cudaMemcpyAsync(f0_out, cb.d_f0_out, sizeof(float) * T, cudaMemcpyDeviceToHost, st));
   RYK_CUDA(cudaMemcpyAsync(ap_out, cb.d_ap_out, sizeof(float) * T * nb, cudaMemcpyDeviceToHost, st));
   RYK_CUDA(cudaMemcpyAsync(sp_out, cb.d_sp_out, sizeof(float) * T * nb, cudaMemcpyDeviceToHost, st));

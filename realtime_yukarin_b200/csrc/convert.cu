@@ -27,7 +27,7 @@ int convert_buffers_get(Engine* e, int T, int n_wave, int nb, int C, ConvertBuff
 }
 
 int convert_window_device(Engine* e, const ConvertBuffers& cb, int T, int n_wave, int frame_length, int hop, double threshold_db,
-                          int order, int fftlen, cudaStream_t st) {
+                          int order, int fftlen, const double* d_H, cudaStream_t st) {
   const int nb = fftlen / 2 + 1, C = order + 1;
   const Voice* v = e->voices[0];                 // the per-op API converts into the built-in voice
   if (gate_mask_run(e, cb.d_wave, n_wave, frame_length, hop, threshold_db, T, cb.d_mse, cb.d_mask, cb.d_index, cb.d_count, st)) return -1;
@@ -44,7 +44,7 @@ int convert_window_device(Engine* e, const ConvertBuffers& cb, int T, int n_wave
   }
   if (stage1_epilogue_run(v, d_y, cb.d_index, cb.d_mask, cb.d_count, T, C, cb.d_f0, cb.d_ap, cb.d_voiced, nb, kSilentMc0,
                           cb.d_mc_out, cb.d_f0_out, cb.d_ap_out, cb.d_voiced_out, st)) return -1;
-  if (mc2sp_run(e, cb.d_mc_out, T, order, fftlen, 1e-16, cb.d_sp_mid, nullptr, st)) return -1;
+  if (mc2sp_run(e, d_H, cb.d_mc_out, T, order, fftlen, 1e-16, cb.d_sp_mid, nullptr, st)) return -1;
   const int Tp = T + (128 - T % 128);
   UNetPlan* p2 = nullptr;
   if (unet_get_plan(e, v->stage2, 1, Tp, 512, e->precision, &p2)) return -1;

@@ -32,6 +32,12 @@ struct Voice {
   int users = 0;                     // sessions and groups that convert into this voice
 };
 
+// The SPTK conversions of one (order, alpha, fft_size) as linear maps (features.cu: sptk_prepare)
+struct SptkMats {
+  double* d_G = nullptr;             // sp2mc: (order+1) x nb
+  double* d_H = nullptr;             // mc2sp: nb x (order+1)
+};
+
 struct Engine {
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -42,9 +48,9 @@ struct Engine {
   double2* d_twiddle = nullptr;
   // xorshift128 jump-ahead matrices (synthesis noise stream)
   uint32_t* d_jump = nullptr;
-  // SPTK matrices
-  double* d_G = nullptr; int G_order = -1, G_fft = 0; double G_alpha = 0;     // sp2mc: (order+1) x nb
-  double* d_H = nullptr; int H_order = -1, H_fft = 0; double H_alpha = 0;     // mc2sp: nb x (order+1)
+  // SPTK matrices keyed by (order, alpha, fft_size), alpha compared exactly.  Built on first use and freed only with the engine:
+  // captured session graphs hold their addresses, so a per-op call or a session at another key must not replace them.
+  std::map<std::tuple<int, double, int>, SptkMats> sptk;
   // DIO plans keyed by (n, fs, frame_period*1000, floor*1000, ceil*1000)
   std::map<std::tuple<int, int, int, int, int>, DioPlan*> dio_plans;
   // voices by id (voice 0 always exists; a destroyed voice leaves nullptr)
@@ -111,9 +117,10 @@ int crepe_test_conv(Engine* e, int backend, int F, int Win, int Cin, int Cout, i
 int crepe_test_network(Engine* e, int backend, const float* audio16k, int n, double step_ms, float* activation, int* path, int* voicing,
                        int repeat, float* ms_per_run);
 // side (only while st is being captured into a graph): D4C becomes a branch of its own, concurrent with CheapTrick
+// d_G: sp2mc matrix of (order, alpha, fft_size) from sptk_prepare
 int spectral_analysis_run(Engine* e, const float* d_x, int n, int fs, double frame_period, const double* d_f0, int n_out,
-                          int fft_size, int order, float* d_sp, float* d_ap, float* d_mc, float* d_f0_out, uint8_t* d_voiced,
-                          cudaStream_t st, cudaStream_t side = nullptr);
+                          int fft_size, int order, const double* d_G, float* d_sp, float* d_ap, float* d_mc, float* d_f0_out,
+                          uint8_t* d_voiced, cudaStream_t st, cudaStream_t side = nullptr);
 
 // world_synth.cu: offline Synthesis() (pyworld.synthesize) and the output silence gate
 int world_synthesize_run(Engine* e, const double* f0, int n_frames, const float* sp, const float* ap, int fs, double frame_period_ms,
@@ -123,8 +130,11 @@ int output_gate_async(Engine* e, const double* d_wave, const int* d_n_valid, int
 size_t output_gate_scratch_doubles(int n, int n_fft, int hop);
 
 // sptk.cu
-int sptk_prepare(Engine* e, int order, double alpha, int fft_size);                 // builds G and H on the device
-int mc2sp_run(Engine* e, const float* d_mc, int T, int order, int fft_size, double add, float* d_sp_f32, double* d_sp_f64, cudaStream_t st);
+// the engine's G and H of (order, alpha, fft_size), built on the device on first use
+int sptk_prepare(Engine* e, int order, double alpha, int fft_size, SptkMats* out);
+// d_H: mc2sp matrix of (order, alpha, fft_size) from sptk_prepare
+int mc2sp_run(Engine* e, const double* d_H, const float* d_mc, int T, int order, int fft_size, double add, float* d_sp_f32, double* d_sp_f64,
+              cudaStream_t st);
 
 // features.cu: polyphase resampler (wav I/O row)
 int resample_poly_run(Engine* e, const float* d_x, int n, int up, int down, const double* d_h, int n_taps, float* d_y, int n_out, cudaStream_t st);

@@ -26,8 +26,10 @@ static void freqt_host(const double* c1, int m1, double* c2, int m2, double a) {
   for (int j = 0; j <= m2; ++j) c2[j] = g[j];
 }
 
-int sptk_prepare(Engine* e, int order, double alpha, int fft_size) {
-  if (e->d_G && e->G_order == order && e->G_fft == fft_size && e->G_alpha == alpha) return 0;
+int sptk_prepare(Engine* e, int order, double alpha, int fft_size, SptkMats* out) {
+  const auto key = std::make_tuple(order, alpha, fft_size);
+  auto it = e->sptk.find(key);
+  if (it != e->sptk.end()) { *out = it->second; return 0; }
   const int nb = fft_size / 2 + 1, N = fft_size;
   // G: mc = freqt(irfft(logsp) with c[0] /= 2, order, alpha); column k = response to the unit log-spectrum e_k
   std::vector<double> G((size_t)(order + 1) * nb), H((size_t)nb * (order + 1));
@@ -52,13 +54,18 @@ int sptk_prepare(Engine* e, int order, double alpha, int fft_size) {
       H[(size_t)k * (order + 1) + j] = s;
     }
   }
-  if (e->d_G) cudaFree(e->d_G);
-  if (e->d_H) cudaFree(e->d_H);
-  RYK_CUDA(cudaMalloc(&e->d_G, G.size() * sizeof(double)));
-  RYK_CUDA(cudaMalloc(&e->d_H, H.size() * sizeof(double)));
-  RYK_CUDA(cudaMemcpy(e->d_G, G.data(), G.size() * sizeof(double), cudaMemcpyHostToDevice));
-  RYK_CUDA(cudaMemcpy(e->d_H, H.data(), H.size() * sizeof(double), cudaMemcpyHostToDevice));
-  e->G_order = e->H_order = order; e->G_fft = e->H_fft = fft_size; e->G_alpha = e->H_alpha = alpha;
+  SptkMats m;
+  cudaError_t err = cudaMalloc(&m.d_G, G.size() * sizeof(double));
+  if (err == cudaSuccess) err = cudaMalloc(&m.d_H, H.size() * sizeof(double));
+  if (err == cudaSuccess) err = cudaMemcpy(m.d_G, G.data(), G.size() * sizeof(double), cudaMemcpyHostToDevice);
+  if (err == cudaSuccess) err = cudaMemcpy(m.d_H, H.data(), H.size() * sizeof(double), cudaMemcpyHostToDevice);
+  if (err != cudaSuccess) {          // the entry was never handed out: nothing else holds these addresses
+    cudaFree(m.d_G);
+    cudaFree(m.d_H);
+    RYK_CUDA(err);
+  }
+  e->sptk[key] = m;
+  *out = m;
   return 0;
 }
 
@@ -75,11 +82,11 @@ __global__ void k_mc2sp(const float* __restrict__ mc, int T, int order, int nb, 
   if (sp64) sp64[(size_t)t * nb + k] = v;
 }
 
-int mc2sp_run(Engine* e, const float* d_mc, int T, int order, int fft_size, double add, float* d_sp32, double* d_sp64, cudaStream_t st) {
-  RYK_CHECK(e->d_H && e->H_order == order && e->H_fft == fft_size, "mc2sp matrix not prepared");
+int mc2sp_run(Engine* e, const double* d_H, const float* d_mc, int T, int order, int fft_size, double add, float* d_sp32, double* d_sp64,
+              cudaStream_t st) {
   if (T <= 0) return 0;
   int nb = fft_size / 2 + 1;
-  k_mc2sp<<<dim3((nb + 127) / 128, T), 128, 0, st>>>(d_mc, T, order, nb, e->d_H, add, d_sp32, d_sp64);
+  k_mc2sp<<<dim3((nb + 127) / 128, T), 128, 0, st>>>(d_mc, T, order, nb, d_H, add, d_sp32, d_sp64);
   RYK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -27,9 +27,9 @@ struct ConvertBuffers {
   float *d_mc_out, *d_f0_out, *d_ap_out, *d_sp_mid, *d_sp_out; uint8_t* d_voiced_out;
 };
 int convert_buffers_get(Engine* e, int T, int n_wave, int nb, int C, ConvertBuffers* out);
-// stream-ordered except for one 8-byte D2H of the effective-frame count (picks the stage-1 plan)
+// stream-ordered except for one 8-byte D2H of the effective-frame count (picks the stage-1 plan); d_H: mc2sp matrix of the key
 int convert_window_device(Engine* e, const ConvertBuffers& cb, int T, int n_wave, int frame_length, int hop, double threshold_db,
-                          int order, int fftlen, cudaStream_t st);
+                          int order, int fftlen, const double* d_H, cudaStream_t st);
 
 // polyphase resampler (features.cu: k_resample_poly): the whole-signal call of ryk_resample_poly and the two streaming sides of a
 // session's device-rate conversion.  Streaming positions live on the device, double-buffered by step parity.

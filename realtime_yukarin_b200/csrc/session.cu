@@ -83,6 +83,7 @@ struct Session {
   Group* group = nullptr; int slot = 0;        // member of a batched stage-2 group (config 5), else nullptr
   Voice* voice = nullptr; int voice_id = 0;    // the voice the session converts into (fixed for its lifetime)
   ryk_session_config cfg;
+  SptkMats sptk;                   // the engine's sp2mc / mc2sp matrices of cfg's (order, alpha, fft_length), captured in the graphs
   int hop, rate, n_wave, n_feat, e_wave, e_enc_frames, e_conv, e_dec;
   int Lw, Tw, Td, nb, C;
   int Tp;                          // stage-2 padded length: Tw rounded up to the next multiple of 128 (always > Tw)
@@ -492,7 +493,7 @@ static int stage1_body(Engine* e, Session* s, int b, int tp1) {
   }
   if (stage1_epilogue_run(s->voice, d_y, s->d_index[b], s->d_mask[b], s->d_count[b], s->Tw, s->C, s->cw_f0[g], s->cw_ap[g], s->cw_voiced[g], s->nb,
                           kSilentMc0, s->cv_mc_out[b], s->cv_f0_out[b], s->cv_ap_out[b], s->cv_voiced_out[b], s->sC)) return -1;
-  return mc2sp_run(e, s->cv_mc_out[b], s->Tw, c.order, c.fft_length, 1e-16, s->cv_sp_mid[b], nullptr, s->sC);
+  return mc2sp_run(e, s->sptk.d_H, s->cv_mc_out[b], s->Tw, c.order, c.fft_length, 1e-16, s->cv_sp_mid[b], nullptr, s->sC);
 }
 
 // Step k = s->step is enqueued in three parts so that a group can interleave its members:
@@ -561,7 +562,7 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
           d_f0 = dio_plan_f0(s->dio[b]);
         }
         const int n_enc = s->Lw / s->hop;
-        return spectral_analysis_run(e, s->wave_win[g], s->Lw, c.fs, c.frame_period_ms, d_f0, n_enc, c.fft_length, c.order,
+        return spectral_analysis_run(e, s->wave_win[g], s->Lw, c.fs, c.frame_period_ms, d_f0, n_enc, c.fft_length, c.order, s->sptk.d_G,
                                      s->enc_sp[b], s->enc_ap[b], s->enc_mc[b], s->enc_f0[b], s->enc_voiced[b], sA, s->sA_side);
       })) return -1;
   if (stage_time(s, 1, 1, r, sA)) return -1;
@@ -803,7 +804,7 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
             "fs does not match fft_length: the synthesizer at this fs needs a different spectrum width (run the session at the model's "
             "rate and set a device rate with ryk_session_set_input_rate / ryk_session_set_output_rate)");
   s->n_in = s->n_wave;
-  if (sptk_prepare(e, cfg->order, cfg->alpha, cfg->fft_length)) return -1;
+  if (sptk_prepare(e, cfg->order, cfg->alpha, cfg->fft_length, &s->sptk)) return -1;
   // The analysis, stage-1 and synthesis stages are chains of small, latency-bound kernels; stage 2 is bulk work that fills
   // every SM.  Higher stream priority for the former lets their CTAs take freed SM slots first, so their latency does not
   // inflate behind stage-2 waves.

@@ -789,10 +789,9 @@ int analysis_kernels_init() {
 // Both read only the wave and the f0 and write disjoint outputs.  With a side stream (st being captured) D4C is forked onto it and
 // joined back, so the captured graph holds CheapTrick (+ f0 out) and D4C as two concurrent branches; otherwise they run in turn on st.
 int spectral_analysis_run(Engine* e, const float* d_x, int n, int fs, double frame_period, const double* d_f0, int n_out,
-                          int fft_size, int order, float* d_sp, float* d_ap, float* d_mc, float* d_f0_out, uint8_t* d_voiced,
-                          cudaStream_t st, cudaStream_t side) {
+                          int fft_size, int order, const double* d_G, float* d_sp, float* d_ap, float* d_mc, float* d_f0_out,
+                          uint8_t* d_voiced, cudaStream_t st, cudaStream_t side) {
   RYK_CHECK(fft_size <= kCtMaxFft && fft_size >= 64, "unsupported CheapTrick fft size");
-  RYK_CHECK(e->d_G != nullptr && e->G_order == order && e->G_fft == fft_size, "sp2mc matrix not prepared for this (order, fft)");
   if (n_out <= 0) return 0;
   const int fft_d4c = (int)pow(2.0, 1.0 + (int)(log(4.0 * fs / 47.0 + 1) / kLog2));   // host pow: exact
   const int lt_fft = (int)pow(2.0, 1.0 + (int)(log(3.0 * fs / 40.0 + 1) / kLog2));
@@ -806,7 +805,7 @@ int spectral_analysis_run(Engine* e, const float* d_x, int n, int fs, double fra
     sd = side;
   }
   k_d4c<<<n_out, 512, d4c_smem_bytes(fs), sd>>>(d_x, n, fs, frame_period, d_f0, fft_size, 0.85, n_out, d_ap, e->d_twiddle, fft_d4c, lt_fft);
-  k_cheaptrick<<<n_out, 256, cheaptrick_smem_bytes(fft_size, fs), st>>>(d_x, n, fs, frame_period, d_f0, fft_size, -0.15, e->d_G, order,
+  k_cheaptrick<<<n_out, 256, cheaptrick_smem_bytes(fft_size, fs), st>>>(d_x, n, fs, frame_period, d_f0, fft_size, -0.15, d_G, order,
                                                                       n_out, d_sp, d_mc, nullptr, e->d_twiddle);
   k_f0_out<<<(n_out + 127) / 128, 128, 0, st>>>(d_f0, n_out, d_f0_out, d_voiced);
   RYK_CUDA(cudaGetLastError());

@@ -132,6 +132,7 @@ def test_world_analysis_matches_oracle_48k(engine):
         assert ref['voiced'].sum() > 0
         assert np.allclose(np.log(got['sp']), np.log(ref['sp']), atol=2e-4), np.abs(np.log(got['sp']) - np.log(ref['sp'])).max()
         assert np.allclose(got['ap'], ref['ap'], rtol=1e-4, atol=1e-6), np.abs(got['ap'] - ref['ap']).max()
+        assert np.allclose(got['mc'], ref['mc'], atol=2e-4), np.abs(got['mc'] - ref['mc']).max()
 
 
 def _glide(f_lo, f_hi, seconds=1.0, seed=0):
