@@ -265,14 +265,27 @@ int ryk_session_stage_times(ryk_engine* e, int session_id, float* start, float* 
  * BASELINE config 5 / SURVEY 8(e) "per-GPU batch = streams resident on it": the reference would run one
  * SuperResolution.convert (voice_changer.py:41) per stream; a group stacks the members' padded log-spectrograms into
  * one (B, 1, Tp, 512) stage-2 input per step.  Analysis, gate, stage 1 and synthesis stay per stream (per-stream state,
- * data-dependent lengths).  Members are fresh sessions with the same window length; member i of every call is
- * session_ids[i].  Outputs per member are those of an ungrouped session up to the FP16 stage-2 rounding.
+ * data-dependent lengths).  Members are distinct sessions in no group, with the same window length, chunk length and device rates;
+ * they may be fresh or may have run steps, alone or in another group.  Member i of every call is the session in slot i: session_ids[i]
+ * after ryk_group_create, then as ryk_group_add / _remove change it (ryk_group_members lists it).  Outputs per member are those of an
+ * ungrouped session up to the FP16 stage-2 rounding.
  * Members may convert into different voices when their stage-2 models have the same channels, the engine is in precision 1, every
  * stage-2 layer runs on a kernel that reads weights per batch item (the base-64 nets) and there are at most 8 distinct voices: the one
- * batched forward reads each member's weights from its voice.  Other groups of several voices are refused. */
+ * batched forward reads each member's weights from its voice.  Other groups of several voices are refused.
+ * Membership changes between steps.  ryk_group_add makes the session the group's last member: its next step is the group's next step.
+ * ryk_group_remove takes a member out (the members after it move down one slot); it continues as an ungrouped session
+ * (ryk_session_submit / _collect / _push_device).  Either way the session's stream state (windows, synthesizer, step count) carries
+ * over, so its audio continues as if nothing happened.  ryk_group_create and ryk_group_add refuse a session with an uncollected
+ * ryk_session_submit chunk, and _add / _remove refuse while the group has an uncollected ryk_group_submit chunk; device-resident steps
+ * count as collected.  The last member cannot be removed: destroy the group instead.  A refused call changes nothing.  A change waits
+ * for the device (the group's stage-2 plan is rebuilt at the new batch size) and launches no kernel.
+ * ryk_group_members returns the member count and writes up to `capacity` member ids in slot order (session_ids may be NULL). */
 int ryk_group_create(ryk_engine* e, const int* session_ids, int n_sessions, int* group_id);
 int ryk_group_destroy(ryk_engine* e, int group_id);        /* members survive, ungrouped */
 int ryk_group_size(ryk_engine* e, int group_id);
+int ryk_group_add(ryk_engine* e, int group_id, int session_id);
+int ryk_group_remove(ryk_engine* e, int group_id, int session_id);
+int ryk_group_members(ryk_engine* e, int group_id, int* session_ids, int capacity);
 int ryk_group_submit(ryk_engine* e, int group_id, const float* const* waves, int n, long long* ticket);
 int ryk_group_collect(ryk_engine* e, int group_id, long long ticket, double* const* outs, int out_capacity, int* n_outs);
 int ryk_group_push_device(ryk_engine* e, int group_id, const float* const* waves_dev, int n, double* const* outs_dev,

@@ -140,8 +140,9 @@ struct Session {
 // Several sessions on one GPU sharing ONE batched stage-2 forward per step (BASELINE config 5: 8 streams per GPU,
 // stage-2 input (B, 1, Tp, 512)).  Everything else (analysis, gate, stage 1, synthesis) stays per stream: those
 // stages carry per-stream state and data-dependent lengths, and they are a small share of the SM time.
+// Members may join and leave between steps (ryk_group_add / _remove): group_rebuild then builds p2 anew around the new member list.
 struct Group {
-  std::vector<Session*> members;
+  std::vector<Session*> members;               // in slot order: member i reads and writes batch item i of p2
   std::vector<Voice*> voices;                  // the members' distinct voices in the order of their first member; p2 lives on voices[0]
   int owner = 0;                               // plan-cache owner id of p2
   UNetPlan* p2 = nullptr;                      // stage-2 plan at batch = members.size(), member i on the weights of its voice
@@ -713,10 +714,12 @@ static int stage_in(Session* s, int r, const float* wave) {
 static double* step_out(Session* s, int b) { return s->out.rate ? s->d_rout_fixed[b] : s->d_out_fixed[b]; }
 static int* step_n_out(Session* s, int b) { return s->out.rate ? s->d_rn_fixed[b] : s->d_n_fixed[b]; }
 
-// after step k was enqueued: copy its samples and sample count to out / n_out (kind: to the host ring or to device buffers) behind
-// the decode stream and record ev[r].dec
-static int stage_out(Session* s, long long k, double* out, int* n_out, cudaMemcpyKind kind) {
-  const int b = (int)(k & 1), r = (int)(k % kRing);
+// after a step of s was enqueued: copy its samples and sample count to out / n_out (kind: to the host ring or to device buffers) behind
+// the decode stream and record ev[r].dec.  r is the caller's ring slot (the session's step, or the group's step for a member); the
+// output buffers are those of the parity of the session's own step, which differs from the group's for a member that joined at a
+// group step of the other parity.
+static int stage_out(Session* s, int r, double* out, int* n_out, cudaMemcpyKind kind) {
+  const int b = (int)((s->step - 1) & 1);
   RYK_CUDA(cudaMemcpyAsync(n_out, step_n_out(s, b), sizeof(int), kind, s->sD));
   RYK_CUDA(cudaMemcpyAsync(out, step_out(s, b), sizeof(double) * s->max_out, kind, s->sD));
   RYK_CUDA(cudaEventRecord(s->ev[r].dec, s->sD));
@@ -919,7 +922,7 @@ int ryk_session_submit(ryk_engine* h, int id, const float* wave, int n, long lon
   const int r = (int)(k % kRing);
   if (stage_in(s, r, wave)) return -1;
   if (session_enqueue(e, s, s->d_chunk[r])) return -1;
-  if (stage_out(s, k, s->h_out[r], s->h_n[r], cudaMemcpyDeviceToHost)) return -1;
+  if (stage_out(s, r, s->h_out[r], s->h_n[r], cudaMemcpyDeviceToHost)) return -1;
   if (ticket) *ticket = k;
   return 0;
 }
@@ -962,9 +965,9 @@ int ryk_session_push_device(ryk_engine* h, int id, const float* wave_dev, int n,
   RYK_CHECK(n == s->n_in, "chunk length must be round(rate * buffer_time) at the session's input rate");
   RYK_CHECK(s->group == nullptr, "session belongs to a group: use ryk_group_push_device");
   RYK_CHECK(out_capacity >= s->max_out, "out_capacity must hold the most samples a step returns (ryk_session_io_geometry max_out)");
-  const long long k = s->step;
+  const int r = (int)(s->step % kRing);
   if (session_enqueue(e, s, wave_dev)) return -1;
-  if (stage_out(s, k, out_dev, n_out_dev, cudaMemcpyDeviceToDevice)) return -1;
+  if (stage_out(s, r, out_dev, n_out_dev, cudaMemcpyDeviceToDevice)) return -1;
   s->collected = s->step;         // device-resident steps are not collected through the host API
   return 0;
 }
@@ -1065,69 +1068,169 @@ int ryk_session_io_geometry(ryk_engine* h, int id, int* n_in, int* max_out, int*
 // ---- groups: several sessions of one GPU sharing one batched stage-2 forward per step (BASELINE config 5) ----
 static Group* get_group(Engine* e, int id) { return (id >= 0 && id < (int)e->groups.size()) ? e->groups[id] : nullptr; }
 
+// Why a member's stream state survives a membership change.  A change runs only when none of the session's or the group's host-API
+// steps is uncollected, and it synchronises the device before it frees or rebuilds anything, so no step of the old layout is in flight.
+// The guards of the steps after it still hold across the switch of a member's stage 2 between sC2s[0] (grouped) and sC2s[b] (alone):
+//   * every cross-stage guard is an event of the member's own ring, indexed by its own step count (which a change keeps), so the
+//     waits of step k on the events of steps k-1 and k-2 find them wherever those steps ran;
+//   * d_colmin[0] is only ever written on sC2s[0] and d_colmin[1] only on sC2s[1] (a member uses sC2s[0] with d_colmin[0], a single
+//     session sC2s[b] with d_colmin[b]), so each stays ordered by its stream;
+//   * the stage-2 plans a step uses are new after a change (the group's rebuilt plan, or the leaving member's own plans built by the
+//     change), and the group's waits on ev_fwd / pro / conv of steps before the change find completed events.
+// The host staging ring (h_in / h_out / h_n, ev[r].dec) is indexed by the group's step while grouped and by the session's step alone;
+// with nothing in flight at a change, no slot of one indexing is still in use when the other takes over.
+
+// The conditions on a group's member list (create, add and remove all end in one); nullptr when it may form a group.
+static const char* group_refusal(Engine* e, const std::vector<Session*>& members) {
+  if (members.empty() || (int)members.size() > kMaxGroupBatch) return "a group holds 1..64 sessions";
+  const Session* s0 = members[0];
+  for (const Session* s : members)
+    if (s->Tw != s0->Tw) return "group members must be distinct sessions with the same window length";
+  // one chunk length serves every member in ryk_group_submit / ryk_group_push_device
+  for (const Session* s : members)
+    if (s->n_in != s0->n_in || s->in.rate != s0->in.rate || s->out.rate != s0->out.rate)
+      return "group members must have the same device input and output rates";
+  std::vector<const Voice*> voices;
+  for (const Session* s : members)
+    if (std::find(voices.begin(), voices.end(), s->voice) == voices.end()) voices.push_back(s->voice);
+  if (voices.size() > 1 && e->precision != 1) return "a group of several voices needs precision 1 (FP16 tensor cores)";
+  if ((int)voices.size() > kMaxGroupVoices) return "a group holds at most 8 distinct voices";
+  const UNet* n0 = voices[0]->stage2;
+  for (const Voice* v : voices)
+    if (v->stage2->in_ch != n0->in_ch || v->stage2->out_ch != n0->out_ch || v->stage2->base != n0->base)
+      return "the members' stage-2 models must have the same (in, out, base) channels";
+  return nullptr;
+}
+
+// A session's host-API steps are all collected (device-resident steps count as collected).
+static bool session_idle(const Session* s) { return s->collected == s->step; }
+
+// The one way a group's batched stage 2 is built: around `members` (slot i = members[i]), for ryk_group_create, _add and _remove.
+// Builds the voice table, a plan at the new batch size and keep hull under a new owner id and its per-item weights first; only when
+// all of that succeeded does it release the old plan (on the net of the old first voice), move the voices' `users` counts, and reset
+// the graphs that hold slot offsets into the old plan (the group's forward, every member's stage-2 prologue / epilogue).  A session
+// that was not a member before also drops its own stage-2 plans and graphs: a session that ran alone captured s2_layers on them.  On
+// failure the group and every session are left as they were.  Waits for the device: the old graphs may still be running.
+static int group_rebuild(Engine* e, Group* G, const std::vector<Session*>& members) {
+  const char* refusal = group_refusal(e, members);
+  if (refusal) { set_error(refusal); return -1; }
+  RYK_CUDA(cudaDeviceSynchronize());
+  // Members of different voices share the forward: each batch item reads its voice's weights (unet_plan_set_voices).
+  std::vector<Voice*> voices;
+  std::vector<int> voice_of;
+  for (Session* m : members) {
+    const auto it = std::find(voices.begin(), voices.end(), m->voice);
+    voice_of.push_back((int)(it - voices.begin()));
+    if (it == voices.end()) voices.push_back(m->voice);
+  }
+  std::vector<const UNet*> nets;
+  for (const Voice* v : voices) nets.push_back(v->stage2);
+  // the batched forward computes the decoder rows of the hull of the members' kept frames (their e_conv may differ)
+  std::vector<int> kb, kl;
+  for (Session* m : members) { kb.push_back(m->e_conv); kl.push_back(m->n_feat); }
+  int keep_begin = 0, keep_len = 0;
+  keep_hull((int)members.size(), kb.data(), kl.data(), &keep_begin, &keep_len);
+  const int owner = ++e->plan_owners;
+  UNetPlan* p2 = nullptr;
+  if (unet_get_plan(e, voices[0]->stage2, (int)members.size(), members[0]->Tp, 512, e->precision, &p2, owner, keep_begin, keep_len) ||
+      unet_plan_set_voices(p2, nets, voice_of)) {
+    unet_release_owner(voices[0]->stage2, owner);
+    return -1;
+  }
+  if (G->p2) unet_release_owner(G->voices[0]->stage2, G->owner);
+  for (Voice* v : G->voices) v->users--;
+  for (Voice* v : voices) v->users++;
+  G->voices = voices; G->owner = owner; G->p2 = p2;
+  G->fwd_graph.reset();
+  for (size_t i = 0; i < members.size(); ++i) {
+    Session* m = members[i];
+    if (m->group != G) {
+      for (int b = 0; b < 2; ++b) unet_release_owner(m->voice->stage2, m->s2_owner[b]);
+      for (ParityGraphs& pg : m->graphs) pg.s2_layers.reset();
+    }
+    m->group = G; m->slot = (int)i;
+    for (ParityGraphs& pg : m->graphs) { pg.s2_pro.reset(); pg.s2_epi.reset(); }
+  }
+  G->members = members;
+  return 0;
+}
+
 int ryk_group_create(ryk_engine* h, const int* session_ids, int n_sessions, int* group_id) {
   Engine* e = &h->impl;
   RYK_CUDA(cudaSetDevice(e->device));
-  RYK_CHECK(session_ids && group_id && n_sessions >= 1 && n_sessions <= 64, "a group holds 1..64 sessions");
-  Group* G = new Group();
-  G->owner = ++e->plan_owners;
+  RYK_CHECK(session_ids && group_id && n_sessions >= 1 && n_sessions <= kMaxGroupBatch, "a group holds 1..64 sessions");
+  std::vector<Session*> members;
   for (int i = 0; i < n_sessions; ++i) {
     Session* s = get_session(e, session_ids[i]);
-    if (!s || s->group || s->step != 0 || (i > 0 && s->Tw != G->members[0]->Tw)) {
-      for (Session* m : G->members) m->group = nullptr;
-      delete G;
-      RYK_CHECK(false, "group members must be distinct fresh sessions (no chunk pushed yet) with the same window length");
-    }
-    // one chunk length serves every member in ryk_group_submit / ryk_group_push_device
-    if (i > 0 && (s->n_in != G->members[0]->n_in || s->in.rate != G->members[0]->in.rate || s->out.rate != G->members[0]->out.rate)) {
-      for (Session* m : G->members) m->group = nullptr;
-      delete G;
-      RYK_CHECK(false, "group members must have the same device input and output rates");
-    }
-    s->group = G; s->slot = i;
-    G->members.push_back(s);
+    RYK_CHECK(s && !s->group && std::find(members.begin(), members.end(), s) == members.end(),
+              "group members must be distinct sessions with the same window length, none of them in a group");
+    RYK_CHECK(session_idle(s), "collect every submitted chunk of a session before it joins a group");
+    members.push_back(s);
   }
-  // Members of different voices share the forward: each batch item reads its voice's weights (unet_plan_set_voices).
-  std::vector<int> voice_of;
-  for (Session* m : G->members) {
-    const auto it = std::find(G->voices.begin(), G->voices.end(), m->voice);
-    voice_of.push_back((int)(it - G->voices.begin()));
-    if (it == G->voices.end()) G->voices.push_back(m->voice);
-  }
-  const UNet* n0 = G->voices[0]->stage2;
-  const char* refusal = nullptr;
-  if (G->voices.size() > 1 && e->precision != 1) refusal = "a group of several voices needs precision 1 (FP16 tensor cores)";
-  else if ((int)G->voices.size() > kMaxGroupVoices) refusal = "a group holds at most 8 distinct voices";
-  for (const Voice* v : G->voices)
-    if (!refusal && (v->stage2->in_ch != n0->in_ch || v->stage2->out_ch != n0->out_ch || v->stage2->base != n0->base))
-      refusal = "the members' stage-2 models must have the same (in, out, base) channels";
-  if (refusal) {
-    group_free(G);
-    set_error(refusal);
-    return -1;
-  }
-  std::vector<const UNet*> nets;
-  for (const Voice* v : G->voices) nets.push_back(v->stage2);
-  // the batched forward computes the decoder rows of the hull of the members' kept frames (their e_conv may differ)
-  std::vector<int> kb, kl;
-  for (Session* m : G->members) { kb.push_back(m->e_conv); kl.push_back(m->n_feat); }
-  int keep_begin = 0, keep_len = 0;
-  keep_hull(n_sessions, kb.data(), kl.data(), &keep_begin, &keep_len);
-  if (unet_get_plan(e, G->voices[0]->stage2, n_sessions, G->members[0]->Tp, 512, e->precision, &G->p2, G->owner, keep_begin, keep_len) ||
-      unet_plan_set_voices(G->p2, nets, voice_of)) {
-    const int owner = G->owner;
-    UNet* net = G->voices[0]->stage2;
-    group_free(G);
-    unet_release_owner(net, owner);
-    return -1;
-  }
+  Group* G = new Group();
+  if (group_rebuild(e, G, members)) { delete G; return -1; }
   { int lo = 0, hi = 0; RYK_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi)); RYK_CUDA(cudaStreamCreateWithPriority(&G->sG, cudaStreamNonBlocking, lo)); }
   for (int i = 0; i < kRing; ++i) RYK_CUDA(cudaEventCreateWithFlags(&G->ev_fwd[i], cudaEventDisableTiming));
   RYK_CUDA(cudaDeviceSynchronize());
-  for (Voice* v : G->voices) v->users++;
   e->groups.push_back(G);
   *group_id = (int)e->groups.size() - 1;
   return 0;
+}
+
+int ryk_group_add(ryk_engine* h, int group_id, int session_id) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Group* G = get_group(e, group_id);
+  RYK_CHECK(G != nullptr, "no such group");
+  Session* s = get_session(e, session_id);
+  RYK_CHECK(s != nullptr, "no such session");
+  RYK_CHECK(s->group == nullptr, "the session is already in a group");
+  RYK_CHECK(G->collected == G->step, "collect every submitted chunk of the group before changing its members");
+  RYK_CHECK(session_idle(s), "collect every submitted chunk of a session before it joins a group");
+  std::vector<Session*> members = G->members;
+  members.push_back(s);
+  return group_rebuild(e, G, members);
+}
+
+int ryk_group_remove(ryk_engine* h, int group_id, int session_id) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Group* G = get_group(e, group_id);
+  RYK_CHECK(G != nullptr, "no such group");
+  Session* s = get_session(e, session_id);
+  RYK_CHECK(s != nullptr && s->group == G, "the session is not a member of this group");
+  RYK_CHECK(G->members.size() > 1, "the session is the group's last member: destroy the group instead");
+  RYK_CHECK(G->collected == G->step, "collect every submitted chunk of the group before changing its members");
+  std::vector<Session*> members = G->members;
+  members.erase(members.begin() + s->slot);
+  RYK_CUDA(cudaDeviceSynchronize());
+  // the session's own stage-2 plans, as session_build makes its stage-1 plans: its next step (alone) allocates nothing
+  for (int b = 0; b < 2; ++b) {
+    UNetPlan* p = nullptr;
+    if (s2_plan(e, s, b, &p)) {
+      for (int c = 0; c < 2; ++c) unet_release_owner(s->voice->stage2, s->s2_owner[c]);
+      return -1;
+    }
+  }
+  if (group_rebuild(e, G, members)) {
+    for (int b = 0; b < 2; ++b) unet_release_owner(s->voice->stage2, s->s2_owner[b]);
+    return -1;
+  }
+  s->group = nullptr; s->slot = 0;
+  for (ParityGraphs& pg : s->graphs) { pg.s2_pro.reset(); pg.s2_layers.reset(); pg.s2_epi.reset(); }
+  return 0;
+}
+
+int ryk_group_members(ryk_engine* h, int group_id, int* session_ids, int capacity) {
+  Engine* e = &h->impl;
+  Group* G = get_group(e, group_id);
+  RYK_CHECK(G != nullptr, "no such group");
+  const int n = (int)G->members.size();
+  for (int i = 0; i < n && i < capacity && session_ids; ++i) {
+    const auto it = std::find(e->sessions.begin(), e->sessions.end(), G->members[i]);
+    session_ids[i] = (int)(it - e->sessions.begin());
+  }
+  return n;
 }
 
 int ryk_group_destroy(ryk_engine* h, int group_id) {
@@ -1149,7 +1252,7 @@ int ryk_group_size(ryk_engine* h, int group_id) {
   return G ? (int)G->members.size() : -1;
 }
 
-// Queue one chunk per member (host samples; waves[i] belongs to member i in creation order).
+// Queue one chunk per member (host samples; waves[i] belongs to the member in slot i, see ryk_group_members).
 int ryk_group_submit(ryk_engine* h, int group_id, const float* const* waves, int n, long long* ticket) {
   Engine* e = &h->impl;
   RYK_CUDA(cudaSetDevice(e->device));
@@ -1167,7 +1270,7 @@ int ryk_group_submit(ryk_engine* h, int group_id, const float* const* waves, int
   }
   if (group_enqueue(e, G, d_chunks.data())) return -1;
   for (Session* s : G->members)
-    if (stage_out(s, k, s->h_out[r], s->h_n[r], cudaMemcpyDeviceToHost)) return -1;
+    if (stage_out(s, r, s->h_out[r], s->h_n[r], cudaMemcpyDeviceToHost)) return -1;
   if (ticket) *ticket = k;
   return 0;
 }
@@ -1195,11 +1298,11 @@ int ryk_group_push_device(ryk_engine* h, int group_id, const float* const* waves
     RYK_CHECK(n == s->n_in, "chunk length must be round(rate * buffer_time) at the session's input rate");
     RYK_CHECK(out_capacity >= s->max_out, "out_capacity must hold the most samples a step returns (ryk_session_io_geometry max_out)");
   }
-  const long long k = G->step;
+  const int r = (int)(G->step % kRing);
   if (group_enqueue(e, G, waves_dev)) return -1;
   for (size_t i = 0; i < G->members.size(); ++i) {
     Session* s = G->members[i];
-    if (stage_out(s, k, outs_dev[i], n_outs_dev[i], cudaMemcpyDeviceToDevice)) return -1;
+    if (stage_out(s, r, outs_dev[i], n_outs_dev[i], cudaMemcpyDeviceToDevice)) return -1;
     s->collected = s->step;
   }
   G->collected = G->step;

@@ -43,7 +43,7 @@ UNet* unet_create(int ndim, int in_ch, int out_ch, int base) {
 }
 
 static void free_plan(UNetPlan* p) {
-  for (void* q : p->buffers) cudaFree(q);
+  if (p->arena) cudaFree(p->arena);          // every buffer of the plan lives in it
   delete p;
 }
 
@@ -172,20 +172,6 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
   const size_t esz = precision ? 2 : 4;
   auto lvlH = [&](int l) { return n->ndim == 2 ? H >> l : 1; };
   auto lvlW = [&](int l) { return W >> l; };
-  auto alloc = [&](size_t bytes, void** ptr) -> int {
-    RYK_CUDA(cudaMalloc(ptr, bytes));
-    RYK_CUDA(cudaMemsetAsync(*ptr, 0, bytes, e->stream));
-    p->buffers.push_back(*ptr);
-    p->buffer_bytes.push_back(bytes);
-    return 0;
-  };
-  void* enc[8]; void* dec[7];
-  for (int l = 0; l < 8; ++l)
-    if (alloc((size_t)B * lvlH(l) * lvlW(l) * level_channels(n->base, l) * esz, &enc[l])) return -1;
-  for (int d = 0; d < 7; ++d)
-    if (alloc((size_t)B * lvlH(6 - d) * lvlW(6 - d) * dec_out_channels(n->base, d) * esz, &dec[d])) return -1;
-  if (alloc((size_t)B * H * W * n->in_ch * sizeof(float), &p->d_in)) return -1;
-  if (alloc((size_t)B * H * W * n->out_ch * sizeof(float), &p->d_out)) return -1;
   p->layers.resize(16);
   for (int i = 0; i < 16; ++i) {
     const UNetLayerW& LW = n->layers[i];
@@ -194,18 +180,8 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
     L.wt.w[0] = LW.d_w_direct; L.w_tc[0] = LW.d_w_tc; L.w_frag = LW.d_w_frag; L.wt.scale[0] = LW.d_scale; L.wt.shift[0] = LW.d_shift;
     L.host_scale_valid = true; L.wt.host_scale[0] = LW.h_scale0; L.wt.host_shift[0] = LW.h_shift0;
     L.in_dtype = act_dt; L.out_dtype = act_dt;
-    if (i == 0) {
-      L.in0 = p->d_in; L.in_dtype = DT_F32; L.out = enc[0];
-    } else if (i < 8) {
-      L.in0 = enc[i - 1]; L.out = enc[i];
-    } else if (i < 15) {
-      int d = i - 8;
-      if (d == 0) L.in0 = enc[7];
-      else { L.in0 = dec[d - 1]; L.in1 = enc[7 - d]; }
-      L.out = dec[d];
-    } else {
-      L.in0 = dec[6]; L.in1 = enc[0]; L.out = p->d_out; L.out_dtype = DT_F32;
-    }
+    if (i == 0) L.in_dtype = DT_F32;
+    if (i == 15) L.out_dtype = DT_F32;
     L.tc_ready = false;
   }
   // The decoder computes a row band only where every layer of it runs on a kernel that supports one.
@@ -227,8 +203,43 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
   for (int i = 0; i < 16; ++i)
     if (precision == 1 && p->layers[i].w_tc[0] && tc_layer_eligible(p->layers[i]))
       ws_bytes = std::max(ws_bytes, tc_splitk_ws_bytes(p->layers[i], num_sms));
-  void* ws = nullptr;
-  if (ws_bytes && alloc(ws_bytes, &ws)) return -1;
+  // Every buffer of the plan is carved from one zeroed allocation: plans are built and freed whenever a group's members change, and
+  // separate small buffers would share the allocator's pages with other plans' and keep them in use after this plan is freed.
+  std::vector<size_t> bytes;
+  for (int l = 0; l < 8; ++l) bytes.push_back((size_t)B * lvlH(l) * lvlW(l) * level_channels(n->base, l) * esz);        // enc[l]
+  for (int d = 0; d < 7; ++d) bytes.push_back((size_t)B * lvlH(6 - d) * lvlW(6 - d) * dec_out_channels(n->base, d) * esz);  // dec[d]
+  bytes.push_back((size_t)B * H * W * n->in_ch * sizeof(float));                                                          // d_in
+  bytes.push_back((size_t)B * H * W * n->out_ch * sizeof(float));                                                         // d_out
+  if (ws_bytes) bytes.push_back(ws_bytes);                                                                                // split-K
+  constexpr size_t kAlign = 1024;
+  size_t total = 0;
+  for (size_t b : bytes) total += (b + kAlign - 1) / kAlign * kAlign;
+  RYK_CUDA(cudaMalloc(&p->arena, total));
+  RYK_CUDA(cudaMemsetAsync(p->arena, 0, total, e->stream));
+  for (size_t i = 0, off = 0; i < bytes.size(); off += (bytes[i] + kAlign - 1) / kAlign * kAlign, ++i) {
+    p->buffers.push_back((char*)p->arena + off);
+    p->buffer_bytes.push_back(bytes[i]);
+  }
+  void* const* enc = p->buffers.data();
+  void* const* dec = p->buffers.data() + 8;
+  p->d_in = p->buffers[15];
+  p->d_out = p->buffers[16];
+  void* ws = ws_bytes ? p->buffers[17] : nullptr;
+  for (int i = 0; i < 16; ++i) {
+    ConvLayer& L = p->layers[i];
+    if (i == 0) {
+      L.in0 = p->d_in; L.out = enc[0];
+    } else if (i < 8) {
+      L.in0 = enc[i - 1]; L.out = enc[i];
+    } else if (i < 15) {
+      int d = i - 8;
+      if (d == 0) L.in0 = enc[7];
+      else { L.in0 = dec[d - 1]; L.in1 = enc[7 - d]; }
+      L.out = dec[d];
+    } else {
+      L.in0 = dec[6]; L.in1 = enc[0]; L.out = p->d_out;
+    }
+  }
   for (int i = 0; i < 16; ++i) {
     ConvLayer& L = p->layers[i];
     if (precision == 1 && L.w_tc[0] && tc_layer_eligible(L)) {

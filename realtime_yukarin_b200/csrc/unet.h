@@ -25,7 +25,8 @@ struct UNetPlan {
   int B = 1, H = 1, W = 0, precision = 0;
   int keep_begin = 0, keep_len = 0;   // output rows of every batch item the plan computes (keep_len == 0: all); see unet_derive_bands
   std::vector<ConvLayer> layers;
-  std::vector<void*> buffers;
+  void* arena = nullptr;    // one device allocation holding every buffer below
+  std::vector<void*> buffers;          // enc[0..7], dec[0..6], d_in, d_out, then the split-K workspace when a layer splits K
   std::vector<size_t> buffer_bytes;
   void* d_in = nullptr;     // fp32 NHWC input  [B][H][W][in_ch]
   void* d_out = nullptr;    // fp32 NHWC output [B][H][W][out_ch]

@@ -62,7 +62,7 @@ EXPORTED_SYMBOLS = [
     'ryk_crepe_set_resampler', 'ryk_crepe_test_conv', 'ryk_crepe_test_network', 'ryk_stage2_row_bands', 'ryk_test_stage2_forward',
     'ryk_session_set_input_rate', 'ryk_session_set_output_rate', 'ryk_session_io_geometry',
     'ryk_voice_create', 'ryk_voice_destroy', 'ryk_voice_model_create', 'ryk_voice_model_set_layer', 'ryk_voice_stage1_set_stats',
-    'ryk_voice_f0_set_stats', 'ryk_session_create_voice', 'ryk_session_voice',
+    'ryk_voice_f0_set_stats', 'ryk_session_create_voice', 'ryk_session_voice', 'ryk_group_add', 'ryk_group_remove', 'ryk_group_members',
 ]
 
 
@@ -583,6 +583,23 @@ class Engine(object):
 
     def group_size(self, gid: int) -> int:
         return self._check(self.lib.ryk_group_size(self._h, gid))
+
+    def group_add(self, gid: int, sid: int):
+        """Make session `sid` (fresh or running, in no group, nothing uncollected) the group's last member between two steps; its
+        stream continues where it was."""
+        self._check(self.lib.ryk_group_add(self._h, gid, int(sid)))
+
+    def group_remove(self, gid: int, sid: int):
+        """Take member `sid` out of the group between two steps (the members after it move down one slot); it continues as an
+        ungrouped session."""
+        self._check(self.lib.ryk_group_remove(self._h, gid, int(sid)))
+
+    def group_members(self, gid: int) -> List[int]:
+        """Member session ids in slot order: the order of the waves / outputs of group_submit, group_collect and group_push_device."""
+        n = self._check(self.lib.ryk_group_members(self._h, gid, None, 0))
+        ids = (ctypes.c_int * max(n, 1))()
+        n = self._check(self.lib.ryk_group_members(self._h, gid, ids, n))
+        return [int(ids[i]) for i in range(n)]
 
     def group_submit(self, gid: int, waves: Sequence) -> int:
         ws = [_f32(w) for w in waves]
