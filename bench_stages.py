@@ -7,7 +7,9 @@ is run three ways:
   * timeline  -- RYK_STAGE_TIMES=1: begin / end of the five stages of the last 8 pipelined steps (ryk_session_stage_times).
 Kernel times come from torch.profiler with CUDA activities (CUPTI), which sees the kernels inside the session's CUDA graphs.  A kernel
 is attributed to the stage whose stream it ran on; a stream's stage is named by the kernels it carries (the analysis graph's own
-branch streams carry only analysis kernels).  The card's name, power limit and SM clocks are read in the same run.
+branch streams carry only analysis kernels).  The stage-2 kernels are further attributed to the U-Net's 16 layers by their order on
+their stream: the first layer's kernel opens a forward, each k_conv_tc is the next layer (a split-K reduce belongs to the conv before
+it) and the Cout = 1 kernel is the last layer.  The card's name, power limit and SM clocks are read in the same run.
 
     python bench_stages.py --out DIR [--steps 40 --warmup 10 --isolated 8 --f0 dio|harvest]
 
@@ -88,6 +90,29 @@ def per_kernel(kernels, n_steps):
     return table, totals
 
 
+LAYERS = [f'e{i}' for i in range(8)] + [f'd{i}' for i in range(8)]
+
+
+def per_layer(kernels, n_steps):
+    """{layer: [kernels per step, us per step]} of the stage-2 U-Net"""
+    roles = stream_roles(kernels)
+    acc = defaultdict(lambda: [0, 0.0])
+    layer = {}
+    for st, n, _, d in sorted((k for k in kernels if roles[k[0]] == 'stage2'), key=lambda k: (k[0], k[2])):
+        if n.startswith('k_conv3x3_cin1'):
+            layer[st] = 0
+        elif n.startswith('k_conv_tc'):
+            layer[st] = layer.get(st, -1) + 1
+        elif n.startswith('k_conv3x3_cout1'):
+            layer[st] = 15
+        elif 'splitk' not in n:
+            continue
+        a = acc[LAYERS[layer[st]]]
+        a[0] += 1
+        a[1] += d
+    return {k: [acc[k][0] / n_steps, acc[k][1] / n_steps] for k in LAYERS if k in acc}
+
+
 def spans(kernels):
     """{stage: first kernel start to last kernel end (us)} of one isolated step"""
     roles = stream_roles(kernels)
@@ -165,6 +190,7 @@ def main():
             iso_spans[r].append(v)
     eng.session_destroy(sid)
     iso_table, iso_totals = per_kernel(iso_kernels, args.isolated)
+    iso_layers = per_layer(iso_kernels, args.isolated)
 
     # ---- pipelined steps ----
     sid = fresh_session()
@@ -175,7 +201,9 @@ def main():
         torch.cuda.synchronize()
     tp = args.out / 'trace_pipelined.json'
     prof.export_chrome_trace(str(tp))
-    pipe_table, pipe_totals = per_kernel(kernels_of(tp), args.steps)
+    pipe_kernels = kernels_of(tp)
+    pipe_table, pipe_totals = per_kernel(pipe_kernels, args.steps)
+    pipe_layers = per_layer(pipe_kernels, args.steps)
     eng.session_destroy(sid)
 
     # ---- stage timeline, profiler off ----
@@ -194,6 +222,7 @@ def main():
                isolated_us=iso_table, isolated_stage_us=iso_totals,
                isolated_stage_span_us={r: float(np.mean(v)) for r, v in iso_spans.items()},
                pipelined_us=pipe_table, pipelined_stage_us=pipe_totals,
+               stage2_layers=dict(isolated_us=iso_layers, pipelined_us=pipe_layers),
                timeline=dict(stages=STAGES, start_ms=np.round(st, 4).tolist(), end_ms=np.round(en, 4).tolist(),
                              ms_per_step=ms / args.steps, gate_start_minus_stage1_end_of_k_minus_2_ms=np.round(gate_vs_s1, 4).tolist()))
     (args.out / 'bench_stages.json').write_text(json.dumps(res, indent=1))
@@ -209,6 +238,13 @@ def main():
             pt = pipe_table.get(role, {}).get(k, [0, 0, 0])[2]
             lines.append(f'| `{k}` | {c:g} | {per:.2f} | {tot:.2f} | {pt:.2f} |')
         lines.append('')
+    lines += [f'### stage 2 per layer: {sum(v[1] for v in iso_layers.values()):.1f} us of kernels per isolated step, '
+              f'{sum(v[1] for v in pipe_layers.values()):.1f} us per pipelined step', '',
+              '| layer | kernels / step | isolated us / step | pipelined us / step |', '|---|---|---|---|']
+    for k in LAYERS:
+        c, iso = iso_layers.get(k, [0, 0])
+        lines.append(f'| {k} | {c:g} | {iso:.2f} | {pipe_layers.get(k, [0, 0])[1]:.2f} |')
+    lines.append('')
     other = {r: v for r, v in pipe_totals.items() if r not in REPORTED}
     lines += ['other stages, pipelined us of kernels per step: ' + ', '.join(f'{r} {v:.1f}' for r, v in sorted(other.items())), '',
               f'timeline (RYK_STAGE_TIMES=1, profiler off): {res["timeline"]["ms_per_step"]:.4f} ms per step over {args.steps} steps', '',

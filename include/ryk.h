@@ -301,13 +301,18 @@ int ryk_debug_harvest(ryk_engine* e, int n, int fs, double frame_period_ms, doub
  * only the decoder rows those frames depend on.
  * ryk_stage2_row_bands (host only): for a (Tp, W) input of which rows [keep_begin, keep_begin + keep_len) are kept,
  *   bands[2 i], bands[2 i + 1] = the class-local output rows [y0, y1) that layer i (0..15) of an FP16 plan computes.
+ * ryk_stage2_tail_rows (host only): a session pads its Tw-frame window to Tp rows with one repeated row, and the encoder computes
+ *   one copy of the rows that depend only on that padding.  For such a window with the rows above kept, tail[4 i .. 4 i + 3] =
+ *   {skip_y0, skip_y1, run_y0, run_y1} of layer i: it does not compute output rows [skip_y0, skip_y1), and its load boxes wholly
+ *   inside input rows [run_y0, run_y1) read from row run_y0 instead (zeros: none).
  * ryk_test_stage2_forward: one forward of the loaded stage-2 net on a fresh plan whose buffers are first filled with NaN;
  *   x, y: [B][Tp][512] float32 network input / output.  mode 0 = every row; 1 = banded for the hull of the n_keep ranges
- *   [keep_begin[i], keep_begin[i] + keep_len[i]); 2 = as 1 with every layer split along K as in the full plan.  Rows outside the
- *   band are left NaN. */
+ *   [keep_begin[i], keep_begin[i] + keep_len[i]); 2 = as 1 with every layer split along K as in the full plan; 3 = as 2 with the
+ *   encoder skipping the padded tail of an input whose rows [Tw, Tp) are equal.  Rows outside the band are left NaN. */
 int ryk_stage2_row_bands(int Tp, int W, int keep_begin, int keep_len, int* bands);
-int ryk_test_stage2_forward(ryk_engine* e, int B, int Tp, int n_keep, const int* keep_begin, const int* keep_len, int mode, const float* x,
-                            float* y);
+int ryk_stage2_tail_rows(int Tp, int W, int Tw, int keep_begin, int keep_len, int* tail);
+int ryk_test_stage2_forward(ryk_engine* e, int B, int Tp, int n_keep, const int* keep_begin, const int* keep_len, int mode, int Tw,
+                            const float* x, float* y);
 /* One conv (transposed = 0) or transposed-conv layer of the U-Nets in isolation, host fp32 NHWC tensors in and
  * out, weights in the Chainer layout; use_tc selects the FP16 wgmma kernel (1) or the FP32 CUDA-core kernel (0).
  * `repeat` extra timed runs report the mean device time per run (ms) -- used by the unit parity tests and ncu. */

@@ -812,22 +812,43 @@ int ryk_stage2_row_bands(int Tp, int W, int keep_begin, int keep_len, int* bands
   return 0;
 }
 
+// Host only: the padded-tail skip of a stage-2 FP16 plan as ryk_stage2_row_bands, for a window of Tw real rows.  tail[4 i .. 4 i + 3] =
+// rows [skip_y0, skip_y1) that layer i does not compute and rows [run_y0, run_y1) of its input whose load boxes it reads from run_y0.
+int ryk_stage2_tail_rows(int Tp, int W, int Tw, int keep_begin, int keep_len, int* tail) {
+  RYK_CHECK(tail && Tp >= 128 && Tp % 128 == 0 && W >= 128 && W % 128 == 0, "stage-2 input extents must be multiples of 128");
+  RYK_CHECK(keep_len > 0 && keep_begin >= 0 && keep_begin + keep_len <= Tp, "kept rows outside the stage-2 input");
+  RYK_CHECK(Tw > 0 && Tw < Tp, "the window must end inside the padded input");
+  UNet* n = unet_create(2, 1, 1, 64);
+  std::vector<ConvLayer> layers(16);
+  for (int i = 0; i < 16; ++i) unet_layer_shape(n, i, 1, Tp, W, layers[i]);
+  unet_destroy(n);
+  unet_derive_bands(layers, keep_begin, keep_len);
+  unet_derive_tail(layers, Tw);
+  for (int i = 0; i < 16; ++i) {
+    const ConvLayer& L = layers[i];
+    tail[4 * i] = L.skip_y0; tail[4 * i + 1] = L.skip_y1; tail[4 * i + 2] = L.run_y0; tail[4 * i + 3] = L.run_y1;
+  }
+  return 0;
+}
+
 // One stage-2 forward on a fresh plan whose buffers (activations, split-K workspaces, output) are first filled with NaN, so that
 // a row the banded decoder reads without having computed it shows up in the output.  x, y: host [B][Tp][512] float32 (network
 // input and output, the log-spectrum without its last bin).  mode 0: full plan; 1: banded plan for the hull of the n_keep row
-// ranges [keep_begin[i], keep_begin[i] + keep_len[i]); 2: as 1, with each banded layer split along K as in the full plan.
-int ryk_test_stage2_forward(ryk_engine* h, int B, int Tp, int n_keep, const int* keep_begin, const int* keep_len, int mode, const float* x,
-                            float* y) {
+// ranges [keep_begin[i], keep_begin[i] + keep_len[i]); 2: as 1, with each banded layer split along K as in the full plan; 3: as 2, with
+// the encoder skipping the rows that repeat input rows [Tw, Tp) (which the caller fills with one row).
+int ryk_test_stage2_forward(ryk_engine* h, int B, int Tp, int n_keep, const int* keep_begin, const int* keep_len, int mode, int Tw,
+                            const float* x, float* y) {
   Engine* e = E(h);
   RYK_CUDA(cudaSetDevice(e->device));
   UNet* net = e->voices[0]->stage2;
   RYK_CHECK(net != nullptr, "stage-2 model not loaded");
-  RYK_CHECK(B >= 1 && Tp >= 128 && Tp % 128 == 0 && mode >= 0 && mode <= 2 && (mode == 0 || n_keep >= 1), "bad stage-2 test arguments");
+  RYK_CHECK(B >= 1 && Tp >= 128 && Tp % 128 == 0 && mode >= 0 && mode <= 3 && (mode == 0 || n_keep >= 1) && (mode != 3 || (Tw > 0 && Tw < Tp)),
+            "bad stage-2 test arguments");
   int kb = 0, kl = 0;
   if (mode != 0) keep_hull(n_keep, keep_begin, keep_len, &kb, &kl);
   const int owner = ++e->plan_owners;
   UNetPlan* p = nullptr;
-  int rc = unet_get_plan(e, net, B, Tp, 512, e->precision, &p, owner, kb, kl, mode == 2);
+  int rc = unet_get_plan(e, net, B, Tp, 512, e->precision, &p, owner, kb, kl, mode >= 2, mode == 3 ? Tw : 0);
   if (!rc) {
     cudaStream_t st = e->stream;
     const size_t nx = (size_t)B * Tp * 512;

@@ -39,6 +39,11 @@ struct ConvLayer {
   // output rows SH * band_y0 .. SH * band_y1 - 1).  The band is a range of whole tile rows (band_y1 may also be the last row);
   // band_y1 == 0 means every row.  See unet_derive_bands.
   int band_y0 = 0, band_y1 = 0;
+  // Padded tail (encoder layers of a session's stage-2 plan; see unet_derive_tail): output rows [skip_y0, skip_y1) repeat the
+  // representative row of their run and are not computed (whole tile rows; skip_y1 == 0: none).  Rows [run_y0, run_y1) of in0
+  // repeat row run_y0: a load box wholly inside them reads from run_y0 instead (run_y1 == 0: no remapping).
+  int skip_y0 = 0, skip_y1 = 0;
+  int run_y0 = 0, run_y1 = 0;
   // device pointers
   const void* in0 = nullptr; const void* in1 = nullptr; int in_dtype = DT_F32;
   void* out = nullptr; int out_dtype = DT_F32;
@@ -76,6 +81,9 @@ int pack_weights_tc(const float* d_w_chainer, int transposed, int Cin, int Cout,
 
 int conv_direct_run(const ConvLayer& L, cudaStream_t st);
 bool conv_direct_band_supported(const ConvLayer& L);
+// the first layer of stage-2 plans (k_conv3x3_cin1), which skips the padded tail in blocks of kCin1Rows output rows
+bool conv_direct_cin1(const ConvLayer& L);
+constexpr int kCin1Rows = 8;
 // the CUDA-core kernels that read weights per batch item (LayerWeights::voice_of): the stage-2 edge layers of FP16 plans
 bool conv_direct_per_item_weights(const ConvLayer& L);
 

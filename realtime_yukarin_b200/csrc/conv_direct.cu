@@ -161,15 +161,16 @@ static int conv_direct_generic(const ConvLayer& L, cudaStream_t st) {
 // Cin = 1, fp32 input -> Cout (multiple of 8, <= 64) channels.  Block = 32 pixels (x) x Cout/8 channel groups, walking
 // kRows rows of the image with a 3-row register window: every input value is loaded once per thread column, every
 // store is a full 16-byte piece of a 128-byte pixel (4 pixels per warp instruction), no integer divisions.
-// Weights [9][1][Cout] of batch item b's voice.
+// Weights [9][1][Cout] of batch item b's voice.  The row blocks [skip_b0, skip_b0 + skip_nb) (a padded tail; ConvLayer::skip_y0) are
+// not launched.
 template <typename TOut>
 __global__ void __launch_bounds__(256) k_conv3x3_cin1(const float* __restrict__ in, const __grid_constant__ LayerWeights wt, int act,
-                                                     int B, int H, int W, int Cout, TOut* __restrict__ out) {
-  constexpr int kRows = 8;
+                                                     int B, int H, int W, int Cout, int skip_b0, int skip_nb, TOut* __restrict__ out) {
+  constexpr int kRows = kCin1Rows;
   const int groups = Cout >> 3;                   // blockDim.x = 32 * groups  (<= 256)
   const int g = threadIdx.x % groups, xl = threadIdx.x / groups;
   const int x = blockIdx.x * 32 + xl;
-  const int y0 = blockIdx.y * kRows;
+  const int y0 = (blockIdx.y + (blockIdx.y >= skip_b0 ? skip_nb : 0)) * kRows;
   const int b = blockIdx.z;
   const int voice = item_voice(wt, b);
   const float* __restrict__ w = wt.w[voice];
@@ -331,8 +332,7 @@ bool conv_direct_band_supported(const ConvLayer& L) {
          L.C1 == 64 && L.in_dtype == DT_F16 && L.out_dtype == DT_F32 && L.host_scale_valid;
 }
 
-// the first layer of stage-2 plans (k_conv3x3_cin1)
-static bool conv_direct_cin1(const ConvLayer& L) {
+bool conv_direct_cin1(const ConvLayer& L) {
   return !L.transposed && L.KH == 3 && L.KW == 3 && L.SH == 1 && L.SW == 1 && L.PH == 1 && L.PW == 1 && L.C0 == 1 && L.C1 == 0 &&
          L.in_dtype == DT_F32 && L.Cout % 8 == 0 && L.Cout <= 64;
 }
@@ -344,15 +344,19 @@ int conv_direct_run(const ConvLayer& L, cudaStream_t st) {
   const bool cin1 = conv_direct_cin1(L);
   RYK_CHECK(L.n_voices == 1 || cout1_h || cin1, "of the CUDA-core kernels only the stage-2 edge layers take weights per batch item");
   RYK_CHECK(cout1_h || (L.band_y0 == 0 && L.band_y1 == 0), "of the CUDA-core kernels only the Cout = 1 3x3 kernel computes a row band");
+  RYK_CHECK(cin1 || L.skip_y1 == 0, "of the CUDA-core kernels only the Cin = 1 3x3 kernel skips a padded tail");
   // dedicated kernels for the stage-2 edge layers
   if (!L.transposed && L.KH == 3 && L.KW == 3 && L.SH == 1 && L.SW == 1 && L.PH == 1 && L.PW == 1) {
     if (cin1) {
-      dim3 grid((L.Win + 31) / 32, (L.Hin + 7) / 8, L.B);
+      RYK_CHECK(L.skip_y0 % kCin1Rows == 0 && L.skip_y1 % kCin1Rows == 0 && L.skip_y0 <= L.skip_y1 && L.skip_y1 <= L.Hout,
+                "skipped rows are not whole row blocks of the first layer");
+      const int skip_b0 = L.skip_y0 / kCin1Rows, skip_nb = (L.skip_y1 - L.skip_y0) / kCin1Rows;
+      dim3 grid((L.Win + 31) / 32, (L.Hin + kCin1Rows - 1) / kCin1Rows - skip_nb, L.B);
       int threads = 32 * (L.Cout / 8);
       if (L.out_dtype == DT_F16)
-        k_conv3x3_cin1<__half><<<grid, threads, 0, st>>>((const float*)L.in0, L.wt, L.act, L.B, L.Hin, L.Win, L.Cout, (__half*)L.out);
+        k_conv3x3_cin1<__half><<<grid, threads, 0, st>>>((const float*)L.in0, L.wt, L.act, L.B, L.Hin, L.Win, L.Cout, skip_b0, skip_nb, (__half*)L.out);
       else
-        k_conv3x3_cin1<float><<<grid, threads, 0, st>>>((const float*)L.in0, L.wt, L.act, L.B, L.Hin, L.Win, L.Cout, (float*)L.out);
+        k_conv3x3_cin1<float><<<grid, threads, 0, st>>>((const float*)L.in0, L.wt, L.act, L.B, L.Hin, L.Win, L.Cout, skip_b0, skip_nb, (float*)L.out);
       RYK_CUDA(cudaGetLastError());
       return 0;
     }

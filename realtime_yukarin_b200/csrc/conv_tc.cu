@@ -32,6 +32,8 @@ struct TcParams {
   int Hc, Wc;                    // class-local output grid (== Hout, Wout for convs)
   int tile_w, tile_h, tiles_w, tiles_h;  // tiles_h: tile rows of the band, which starts at tile row th0
   int th0;
+  int skip_t0, skip_tn;          // tile rows [skip_t0, skip_t0 + skip_tn) are not launched (padded tail); the workspace omits them
+  int run_y0, run_y1;            // rows [run_y0, run_y1) of source 0 repeat row run_y0: a box wholly inside them reads from run_y0
   int ws_y0;                     // output row of the band's first row: row 0 of the split-K workspace
   int chunks0, chunks1;          // 64-channel chunks of source 0 / 1
   int taps_w, ntaps;             // taps per class: conv KH*KW (taps_w = KW); deconv (KH/SH)*(KW/SW)
@@ -76,7 +78,9 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
   // tile coordinates
   int mt = blockIdx.x;
   const int tw = mt % p.tiles_w; mt /= p.tiles_w;
-  const int th = mt % p.tiles_h + p.th0; mt /= p.tiles_h;
+  int th = mt % p.tiles_h + p.th0; mt /= p.tiles_h;
+  const bool past_skip = th >= p.skip_t0;
+  th += past_skip ? p.skip_tn : 0;
   const int b = mt;
   const int n0 = blockIdx.y * BLOCK_N;
   const int cls = blockIdx.z / p.ksplit, split = blockIdx.z % p.ksplit;
@@ -117,7 +121,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
       const int cc = kc - tap * chunks_per_tap;
       const int ty = tap / p.taps_w, tx = tap - ty * p.taps_w;
       int ix, iy;
-      if (!p.transposed) { ix = ox0 * p.sw + tx - p.pw; iy = oy0 * p.sh + ty - p.ph; }
+      if (!p.transposed) {
+        ix = ox0 * p.sw + tx - p.pw; iy = oy0 * p.sh + ty - p.ph;
+        if (iy >= p.run_y0 && iy + p.sh * (p.tile_h - 1) < p.run_y1) iy = p.run_y0;
+      }
       else {   // k4 s2 p1 along a strided dimension: input = m + d - 1 + parity; k1 s1 p0 along the other: input = m
         ix = p.sw == 2 ? ox0 + tx - 1 + px : ox0;
         iy = p.sh == 2 ? oy0 + ty - 1 + py : oy0;
@@ -197,7 +204,8 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
 #pragma unroll
           for (int jb = 0; jb < BLOCK_N / 32; ++jb)
             asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
-                         ::"l"(&tmW), "r"(smem_u32(smem + jb * (kBlockM * 128))), "r"(n0 + jb * 32), "r"(xs), "r"(ys - p.ws_y0), "r"(b), "r"(split) : "memory");
+                         ::"l"(&tmW), "r"(smem_u32(smem + jb * (kBlockM * 128))), "r"(n0 + jb * 32), "r"(xs),
+                         "r"(ys - p.ws_y0 - (past_skip ? p.skip_tn * p.tile_h : 0)), "r"(b), "r"(split) : "memory");
         }
         asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
@@ -213,7 +221,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
 // is deterministic (same summation tree every run) while G x more loads are in flight than with one thread per output.
 __global__ void __launch_bounds__(256) k_splitk_reduce(const float* __restrict__ ws, size_t total4, size_t slice_elems, int ksplit, int Cout,
                                 const __grid_constant__ LayerWeights wt, int act, __half* __restrict__ out,
-                                size_t band4, size_t out_stride4, size_t out_off4) {
+                                size_t band4, size_t out_stride4, size_t out_off4, size_t gap_at4, size_t gap4) {
   __shared__ float4 part[8][32];
   pdl_trigger();
   pdl_wait();
@@ -234,7 +242,7 @@ __global__ void __launch_bounds__(256) k_splitk_reduce(const float* __restrict__
   if (g != 0 || i >= total4) return;
   for (int k = 1; k < G; ++k) { const float4 b = part[k][lane]; a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w; }
   const size_t item = i / band4;
-  const size_t o = item * out_stride4 + out_off4 + i % band4;
+  const size_t r = i % band4, o = item * out_stride4 + out_off4 + r + (r >= gap_at4 ? gap4 : 0);
   const int n = (int)((o * 4) % Cout);
   const int voice = item_voice(wt, (int)item);
   const float* scale = wt.scale[voice]; const float* shift = wt.shift[voice];
@@ -251,7 +259,7 @@ __global__ void __launch_bounds__(256) k_splitk_reduce(const float* __restrict__
 // few splits, large outputs (c3 / c4 / d3): one thread per float4 of the output, grid-stride, all slices summed in order
 __global__ void __launch_bounds__(256) k_splitk_reduce_few(const float* __restrict__ ws, size_t total4, size_t slice_elems, int ksplit, int Cout,
                                     const __grid_constant__ LayerWeights wt, int act, __half* __restrict__ out,
-                                    size_t band4, size_t out_stride4, size_t out_off4) {
+                                    size_t band4, size_t out_stride4, size_t out_off4, size_t gap_at4, size_t gap4) {
   const size_t stride4 = slice_elems / 4;
   pdl_trigger();
   pdl_wait();
@@ -264,7 +272,7 @@ __global__ void __launch_bounds__(256) k_splitk_reduce_few(const float* __restri
       a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
     }
     const size_t item = i / band4;
-    const size_t o = item * out_stride4 + out_off4 + i % band4;
+    const size_t r = i % band4, o = item * out_stride4 + out_off4 + r + (r >= gap_at4 ? gap4 : 0);
     const int n = (int)((o * 4) % Cout);
     const int voice = item_voice(wt, (int)item);
     const float* scale = wt.scale[voice]; const float* shift = wt.shift[voice];
@@ -393,12 +401,22 @@ static void tc_geometry(const ConvLayer& L, int num_sms, int* tile_w, int* tile_
   *tile_w = tw; *tile_h = th; *block_n = bn; *ksplit = ks;
 }
 
+// Rows of one batch item in the split-K workspace: the band's output rows [r0, r1) less the skipped tail rows, which leave a gap of
+// `gap` rows after workspace row `gap_at` (workspace row w holds output row r0 + w, or r0 + w + gap from gap_at on).
+static int tc_ws_rows(const ConvLayer& L, int* r0, int* gap_at, int* gap) {
+  int r1;
+  layer_band_out_rows(L, r0, &r1);
+  *gap = L.skip_y1 - L.skip_y0;
+  *gap_at = *gap ? L.skip_y0 - *r0 : 0;
+  return r1 - *r0 - *gap;
+}
+
 size_t tc_splitk_ws_bytes(const ConvLayer& L, int num_sms) {
   int tw, th, bn, ks;
   tc_geometry(L, num_sms, &tw, &th, &bn, &ks);
-  int r0, r1;
-  layer_band_out_rows(L, &r0, &r1);
-  return ks > 1 ? (size_t)ks * L.B * (r1 - r0) * L.Wout * L.Cout * sizeof(float) : 0;
+  int r0, gap_at, gap;
+  const int rows = tc_ws_rows(L, &r0, &gap_at, &gap);
+  return ks > 1 ? (size_t)ks * L.B * rows * L.Wout * L.Cout * sizeof(float) : 0;
 }
 
 int tc_layer_weight_maps(ConvLayer& L) {
@@ -428,11 +446,14 @@ int tc_layer_prepare(ConvLayer& L, int num_sms) {
   RYK_CHECK(L.ksplit == 1 || L.splitk_ws != nullptr, "split-K layer without a workspace");
   RYK_CHECK(L.band_y0 >= 0 && L.band_y0 % L.tile_h == 0 && L.band_y0 < layer_band_end(L) && layer_band_end(L) <= layer_class_rows(L) &&
             (layer_band_end(L) % L.tile_h == 0 || layer_band_end(L) == layer_class_rows(L)), "row band is not a range of whole tile rows");
+  RYK_CHECK(L.skip_y1 == 0 || (!L.transposed && L.skip_y0 % L.tile_h == 0 && L.skip_y1 % L.tile_h == 0 && L.band_y0 <= L.skip_y0 &&
+                               L.skip_y0 < L.skip_y1 && L.skip_y1 <= layer_band_end(L)),
+            "skipped rows are not a range of whole tile rows inside the band of a convolution");
   if (L.ksplit > 1) {
-    // the workspace holds the band's output rows only
-    int r0, r1;
-    layer_band_out_rows(L, &r0, &r1);
-    if (make_ws_map(&L.tmW, L.splitk_ws, L.Cout, L.Wout, r1 - r0, L.B, L.ksplit, L.tile_w, L.tile_h, L.transposed ? L.SW : 1, L.transposed ? L.SH : 1)) return -1;
+    // the workspace holds the band's computed output rows only
+    int r0, gap_at, gap;
+    const int rows = tc_ws_rows(L, &r0, &gap_at, &gap);
+    if (make_ws_map(&L.tmW, L.splitk_ws, L.Cout, L.Wout, rows, L.B, L.ksplit, L.tile_w, L.tile_h, L.transposed ? L.SW : 1, L.transposed ? L.SH : 1)) return -1;
   } else L.tmW = L.tmO;
   L.tc_ready = true;
   return 0;
@@ -455,11 +476,14 @@ int conv_tc_run(const ConvLayer& L, cudaStream_t st) {
   p.transposed = L.transposed; p.B = L.B; p.Hout = L.Hout; p.Wout = L.Wout; p.Cout = L.Cout;
   p.Hc = L.transposed ? L.Hin : L.Hout; p.Wc = L.transposed ? L.Win : L.Wout;
   p.tile_w = L.tile_w; p.tile_h = L.tile_h;
-  // the grid covers the band's tile rows of the layer's tile grid: every output pixel keeps its tile and so its K order
-  p.tiles_w = (p.Wc + L.tile_w - 1) / L.tile_w; p.tiles_h = (layer_band_end(L) - L.band_y0 + L.tile_h - 1) / L.tile_h;
+  // the grid covers the band's tile rows of the layer's tile grid less the skipped ones: every output pixel keeps its tile and so
+  // its K order
+  p.skip_t0 = L.skip_y0 / L.tile_h; p.skip_tn = (L.skip_y1 - L.skip_y0) / L.tile_h;
+  p.tiles_w = (p.Wc + L.tile_w - 1) / L.tile_w; p.tiles_h = (layer_band_end(L) - L.band_y0 + L.tile_h - 1) / L.tile_h - p.skip_tn;
   p.th0 = L.band_y0 / L.tile_h;
-  int r0, r1;
-  layer_band_out_rows(L, &r0, &r1);
+  p.run_y0 = L.run_y0; p.run_y1 = L.run_y1;
+  int r0, gap_at, gap;
+  const int ws_rows = tc_ws_rows(L, &r0, &gap_at, &gap);
   p.ws_y0 = r0;
   p.chunks0 = L.C0 / kBlockK; p.chunks1 = L.C1 / kBlockK;
   p.taps_w = L.transposed ? L.KW / L.SW : L.KW;
@@ -474,20 +498,21 @@ int conv_tc_run(const ConvLayer& L, cudaStream_t st) {
   p.ws = L.ksplit > 1 ? L.splitk_ws : nullptr;
   p.out_pixels = (size_t)L.B * L.Hout * L.Wout;
   const size_t row_elems = (size_t)L.Wout * L.Cout;
-  const size_t band_elems = (size_t)L.B * (r1 - r0) * row_elems;      // one workspace slice
+  const size_t band_elems = (size_t)L.B * ws_rows * row_elems;        // one workspace slice
   dim3 grid(L.B * p.tiles_w * p.tiles_h, L.Cout / L.block_n, classes * L.ksplit);
   if (L.block_n == 128) RYK_CUDA(launch_pdl(RYK_TC_N128, grid, dim3(kTcThreads), tc_smem_bytes<128, 3>(), st, L.tmA0, L.tmA1, L.tmB, L.tmO, L.tmW, p));
   else RYK_CUDA(launch_pdl(RYK_TC_N64, grid, dim3(kTcThreads), tc_smem_bytes<64, 4>(), st, L.tmA0, L.tmA1, L.tmB, L.tmO, L.tmW, p));
   RYK_CUDA(cudaGetLastError());
   if (p.ws) {
-    const size_t total4 = band_elems / 4, band4 = (r1 - r0) * row_elems / 4, stride4 = L.Hout * row_elems / 4, off4 = r0 * row_elems / 4;
+    const size_t total4 = band_elems / 4, band4 = ws_rows * row_elems / 4, stride4 = L.Hout * row_elems / 4, off4 = r0 * row_elems / 4;
+    const size_t gap_at4 = gap_at * row_elems / 4, gap4 = gap * row_elems / 4;
     if (L.ksplit <= 4) {
       int blocks = (int)((total4 + 255) / 256); if (blocks > 2112) blocks = 2112;     // 16 per SM of 132
       RYK_CUDA(launch_pdl(k_splitk_reduce_few, dim3(blocks), dim3(256), 0, st, (const float*)p.ws, total4, band_elems, L.ksplit, L.Cout, L.wt, L.act,
-                          (__half*)L.out, band4, stride4, off4));
+                          (__half*)L.out, band4, stride4, off4, gap_at4, gap4));
     } else {
       RYK_CUDA(launch_pdl(k_splitk_reduce, dim3((unsigned)((total4 + 31) / 32)), dim3(256), 0, st, (const float*)p.ws, total4, band_elems, L.ksplit, L.Cout, L.wt, L.act,
-                          (__half*)L.out, band4, stride4, off4));
+                          (__half*)L.out, band4, stride4, off4, gap_at4, gap4));
     }
     RYK_CUDA(cudaGetLastError());
   }

@@ -507,9 +507,10 @@ static int stage1_body(Engine* e, Session* s, int b, int tp1) {
 // stage 2 of a single session alternates its stream (and plan) by chunk parity; a group member always uses the first stream
 static cudaStream_t s2_stream(const Session* s, int b) { return s->sC2s[s->group ? 0 : b]; }
 // The decode slide reads only the chunk's frames [e_conv, e_conv + n_feat) of the converted window, so stage 2 computes only the
-// decoder rows those frames depend on.
+// decoder rows those frames depend on; the prologue pads rows [Tw, Tp) with one row, so the encoder computes one copy of the rows
+// that depend only on it.
 static int s2_plan(Engine* e, const Session* s, int b, UNetPlan** p2) {
-  return unet_get_plan(e, s->voice->stage2, 1, s->Tp, 512, e->precision, p2, s->s2_owner[b], s->e_conv, s->n_feat);
+  return unet_get_plan(e, s->voice->stage2, 1, s->Tp, 512, e->precision, p2, s->s2_owner[b], s->e_conv, s->n_feat, false, s->Tw);
 }
 
 // begin (which = 0) / end (1) of a stage in the RYK_STAGE_TIMES timeline
@@ -1125,14 +1126,16 @@ static int group_rebuild(Engine* e, Group* G, const std::vector<Session*>& membe
   }
   std::vector<const UNet*> nets;
   for (const Voice* v : voices) nets.push_back(v->stage2);
-  // the batched forward computes the decoder rows of the hull of the members' kept frames (their e_conv may differ)
+  // the batched forward computes the decoder rows of the hull of the members' kept frames (their e_conv may differ); the members
+  // share Tw, so their padded tails start at the same row
   std::vector<int> kb, kl;
   for (Session* m : members) { kb.push_back(m->e_conv); kl.push_back(m->n_feat); }
   int keep_begin = 0, keep_len = 0;
   keep_hull((int)members.size(), kb.data(), kl.data(), &keep_begin, &keep_len);
   const int owner = ++e->plan_owners;
   UNetPlan* p2 = nullptr;
-  if (unet_get_plan(e, voices[0]->stage2, (int)members.size(), members[0]->Tp, 512, e->precision, &p2, owner, keep_begin, keep_len) ||
+  if (unet_get_plan(e, voices[0]->stage2, (int)members.size(), members[0]->Tp, 512, e->precision, &p2, owner, keep_begin, keep_len, false,
+                    members[0]->Tw) ||
       unet_plan_set_voices(p2, nets, voice_of)) {
     unet_release_owner(voices[0]->stage2, owner);
     return -1;

@@ -148,6 +148,60 @@ void unet_derive_bands(std::vector<ConvLayer>& layers, int keep_begin, int keep_
   }
 }
 
+static int floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
+static int round_up(int a, int m) { return -floor_div(-a, m) * m; }
+static int round_down(int a, int m) { return floor_div(a, m) * m; }
+
+// rows [*r0, *r1) of the output of encoder layer i (0..6) that the decoder reads: layer 15 - i takes it as its second source, over the
+// rows its band reads (3x3 s1 p1 conv and k4 s2 p1 transposed conv alike: class-local row m reads rows m - 1 .. m + 1)
+static void decoder_reads(const std::vector<ConvLayer>& layers, int i, int* r0, int* r1) {
+  const ConvLayer& D = layers[15 - i];
+  *r0 = std::max(D.band_y0 - 1, 0);
+  *r1 = std::min(layer_band_end(D) + 1, D.Hin);
+}
+
+// Rows [Tw, H) of the input all hold one vector (the padded tail of a session's window).  Walking forward, each encoder layer's
+// output rows that read only such rows form a run [lo, hi] of equal rows: a conv of stride s, padding p and k taps maps the run
+// [lo, hi] of its input to the output rows o with o s - p >= lo and o s - p + k - 1 <= hi.
+// Walking back from layer 6, layer i skips whole tile rows [a, b) of its run (rows of kCin1Rows for layer 0).  Layer i + 1 reads
+// a load box of rows iy, iy + 2, .., iy + 2 (tile_h - 1); a box wholly inside the run reads the first rows of the run instead (the
+// representative rows, which stay computed), so [a, b) starts after them.  Every other box of a tile that layer i + 1 computes
+// crosses the end of the run and must miss [a, b), and so must the rows the decoder reads.  Rows of equal inputs get equal sums
+// (same kernel, tile row position and K order), so the remapped boxes load exactly the values the skipped rows would have held.
+void unet_derive_tail(std::vector<ConvLayer>& layers, int tail_begin) {
+  int lo[8], hi[8];
+  int l = tail_begin, h = layers[0].Hin - 1;
+  for (int i = 0; i < 8; ++i) {
+    const ConvLayer& L = layers[i];
+    l = -floor_div(-(l + L.PH), L.SH);
+    h = floor_div(h + L.PH - L.KH + 1, L.SH);
+    lo[i] = l; hi[i] = h;
+  }
+  for (int i = 6; i >= 0; --i) {
+    ConvLayer& L = layers[i];
+    ConvLayer& N = layers[i + 1];
+    if (lo[i] > hi[i]) continue;
+    const int th = i == 0 ? kCin1Rows : tc_tile_rows(L);
+    const int nth = tc_tile_rows(N), span = N.SH * (nth - 1) + 1;
+    int a = round_up(lo[i] + span, th), b = round_down(hi[i] + 1, th);
+    for (int t = 0; t * nth < N.Hout; ++t) {
+      if (t * nth >= N.skip_y0 && t * nth < N.skip_y1) continue;        // not computed
+      for (int ty = 0; ty < N.KH; ++ty) {
+        const int s = t * nth * N.SH + ty - N.PH, e = s + span - 1;
+        if ((s >= lo[i] && e <= hi[i]) || e < a || s >= b) continue;
+        if (s >= a) b = round_down(s, th); else a = round_up(e + 1, th);
+      }
+    }
+    int r0, r1;
+    decoder_reads(layers, i, &r0, &r1);
+    if (r0 < b && r1 > a) {
+      if (round_down(r0, th) - a >= b - round_up(r1, th)) b = round_down(r0, th);
+      else a = round_up(r1, th);
+    }
+    if (a < b) { L.skip_y0 = a; L.skip_y1 = b; N.run_y0 = lo[i]; N.run_y1 = hi[i] + 1; }
+  }
+}
+
 void keep_hull(int n, const int* begins, const int* lens, int* begin, int* len) {
   int lo = begins[0], hi = begins[0] + lens[0];
   for (int i = 1; i < n; ++i) { lo = std::min(lo, begins[i]); hi = std::max(hi, begins[i] + lens[i]); }
@@ -156,11 +210,12 @@ void keep_hull(int n, const int* begins, const int* lens, int* begin, int* len) 
 
 // Plan for a (batch, H, W) input; H = 1 for 1-D nets. precision: 0 = FP32 everywhere, 1 = FP16 activations + wgmma.
 int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPlan** out, int owner, int keep_begin, int keep_len,
-                  bool full_ksplit) {
+                  bool full_ksplit, int tail_begin) {
   for (auto& L : n->layers) RYK_CHECK(L.loaded, "U-Net layer weights not loaded");
   if (keep_len > 0) RYK_CHECK(keep_begin >= 0 && keep_begin + keep_len <= H, "kept rows outside the U-Net input");
   if (keep_len <= 0 || (keep_begin == 0 && keep_len == H)) { keep_begin = 0; keep_len = 0; full_ksplit = false; }
-  auto key = std::make_tuple(B, H, W, precision, owner, keep_begin, keep_len, full_ksplit ? 1 : 0);
+  if (keep_len == 0 || tail_begin <= 0 || tail_begin >= H) tail_begin = 0;     // the full decoder reads every encoder row
+  auto key = std::make_tuple(B, H, W, precision, owner, keep_begin, keep_len, full_ksplit ? 1 : 0, tail_begin);
   auto it = n->plans.find(key);
   if (it != n->plans.end()) { *out = it->second; return 0; }
   RYK_CHECK(W % 128 == 0 && (n->ndim == 1 || H % 128 == 0), "U-Net input extent must be a multiple of 128");
@@ -196,6 +251,20 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
         full.band_y0 = full.band_y1 = 0;
         p->layers[i].ksplit_tiles = tc_tile_count(full);
       }
+    // The encoder skips the rows that repeat the padded tail where its first layer is the Cin = 1 kernel and the others run on
+    // tensor cores (every stage-2 net of base 64).
+    bool tail = tail_begin > 0 && conv_direct_cin1(p->layers[0]);
+    for (int i = 1; i < 8; ++i) tail = tail && p->layers[i].w_tc[0] && tc_layer_eligible(p->layers[i]);
+    if (tail) {
+      p->tail_begin = tail_begin;
+      unet_derive_tail(p->layers, tail_begin);
+      for (int i = 0; i < 7; ++i) {
+        int r0, r1;
+        decoder_reads(p->layers, i, &r0, &r1);
+        const ConvLayer& L = p->layers[i];
+        RYK_CHECK(L.skip_y1 <= r0 || L.skip_y0 >= r1, "the decoder reads an encoder row that the padded-tail skip does not compute");
+      }
+    }
   }
   // One split-K workspace serves every layer of the plan: the layers run in stream order, and a layer's conv kernel writes the
   // workspace only after its programmatic-launch wait, i.e. after the previous layer's reduce kernel has finished reading it.

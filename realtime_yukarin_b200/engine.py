@@ -60,6 +60,7 @@ EXPORTED_SYMBOLS = [
     'ryk_engine_set_f0_method', 'ryk_engine_get_f0_method', 'ryk_debug_harvest',
     'ryk_crepe_create', 'ryk_crepe_set_conv', 'ryk_crepe_set_dense', 'ryk_crepe_set_decoder_tables', 'ryk_crepe_num_frames', 'ryk_crepe_predict',
     'ryk_crepe_set_resampler', 'ryk_crepe_test_conv', 'ryk_crepe_test_network', 'ryk_stage2_row_bands', 'ryk_test_stage2_forward',
+    'ryk_stage2_tail_rows',
     'ryk_session_set_input_rate', 'ryk_session_set_output_rate', 'ryk_session_io_geometry',
     'ryk_voice_create', 'ryk_voice_destroy', 'ryk_voice_model_create', 'ryk_voice_model_set_layer', 'ryk_voice_stage1_set_stats',
     'ryk_voice_f0_set_stats', 'ryk_session_create_voice', 'ryk_session_voice', 'ryk_group_add', 'ryk_group_remove', 'ryk_group_members',
@@ -72,6 +73,16 @@ def stage2_row_bands(Tp: int, W: int, keep_begin: int, keep_len: int) -> numpy.n
     lib = load_library()
     out = numpy.zeros((16, 2), numpy.int32)
     if lib.ryk_stage2_row_bands(int(Tp), int(W), int(keep_begin), int(keep_len), out.ctypes.data_as(c_int_p)) < 0:
+        raise RykError(lib.ryk_last_error().decode('utf-8', 'replace'))
+    return out
+
+
+def stage2_tail_rows(Tp: int, W: int, Tw: int, keep_begin: int, keep_len: int) -> numpy.ndarray:
+    """[16][4] (skip_y0, skip_y1, run_y0, run_y1) per stage-2 layer for a window of Tw frames padded to Tp rows with one repeated row:
+    the output rows the layer does not compute and the input rows whose load boxes it reads from run_y0 (host only)."""
+    lib = load_library()
+    out = numpy.zeros((16, 4), numpy.int32)
+    if lib.ryk_stage2_tail_rows(int(Tp), int(W), int(Tw), int(keep_begin), int(keep_len), out.ctypes.data_as(c_int_p)) < 0:
         raise RykError(lib.ryk_last_error().decode('utf-8', 'replace'))
     return out
 
@@ -484,9 +495,9 @@ class Engine(object):
             _fp(scale), _fp(shift), int(act), int(use_tc), int(repeat), _fp(out), ctypes.byref(ms)))
         return out, ms.value
 
-    def test_stage2_forward(self, x, keep=(), mode=0):
-        """One stage-2 forward on NaN-filled buffers (ryk_test_stage2_forward); x [B][Tp][512] float32, keep = [(begin, len), ...].
-        Returns y [B][Tp][512]; rows the plan does not compute stay NaN."""
+    def test_stage2_forward(self, x, keep=(), mode=0, tw=0):
+        """One stage-2 forward on NaN-filled buffers (ryk_test_stage2_forward); x [B][Tp][512] float32, keep = [(begin, len), ...];
+        mode 3 skips the padded tail from row tw on.  Returns y [B][Tp][512]; rows the plan does not compute stay NaN."""
         x = _f32(x)
         B, Tp, W = x.shape
         assert W == 512
@@ -494,7 +505,7 @@ class Engine(object):
         kl = numpy.array([k[1] for k in keep] or [0], numpy.int32)
         y = numpy.empty_like(x)
         self._check(self.lib.ryk_test_stage2_forward(self._h, B, Tp, len(keep), kb.ctypes.data_as(c_int_p), kl.ctypes.data_as(c_int_p),
-                                                     int(mode), _fp(x), _fp(y)))
+                                                     int(mode), int(tw), _fp(x), _fp(y)))
         return y
 
     # ---- sessions ----
