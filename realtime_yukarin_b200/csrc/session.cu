@@ -17,7 +17,9 @@
 //   stream C: head (slide features, silence gate), then stage-1 U-Net (+f0 map), mc2sp                 of chunk k
 //   stream C2: stage-2 U-Net (the wgmma layers)                                                     of chunk k-1
 //   stream D: slide converted features, synthesizer add/plan/pulse/overlap-add, NaN scrub             of chunk k-2
-// Inter-stage buffers are double-buffered (index = step parity); events order producer/consumer and guard reuse.
+// Inter-stage buffers are double-buffered (index = step parity), except the stage-1 -> stage-2 -> decode hand-off set, which has three
+// slots (index = step % 3) so that stage 1 of a chunk does not wait for stage 2 of the chunk two steps before; events order
+// producer/consumer and guard reuse.
 // The effective-frame count that selects the stage-1 plan (T_eff + 128 - T_eff % 128) is read on the device by a
 // conditional graph node, so the host never waits inside a step.
 #include <math.h>
@@ -37,6 +39,8 @@
 namespace ryk {
 
 constexpr int kRing = 8;          // event / output-slot ring (pipeline depth is bounded by the buffer guards below)
+constexpr int kHandoff = 3;       // slots of the stage-1 -> stage-2 -> decode hand-off buffers (cv_*), h = step % kHandoff
+constexpr int kHandoffGraphs = 6; // graphs that read or write both a parity buffer and a hand-off slot: one per step % 6 = (b, h)
 
 // One captured stage of a step (see run_graph).  Destroying it drops the executable graph.
 struct StageGraph {
@@ -52,14 +56,17 @@ struct ParityGraphs {
   StageGraph gate;         // stream E: wave slides (the "gate" stage of RYK_STAGE_TIMES; the silence gate itself runs in s1_head)
   StageGraph analysis;     // stream A: DIO/Harvest + StoneMask, then CheapTrick || D4C
   StageGraph s1_head;      // stream C: feature-window slides + silence gate (mask / index / count of the step)
+  StageGraph s2_layers;    // single session: stage-2 layers 1..14
+  StageGraph synth;        // stream D: synthesizer + NaN scrub
+};
+// The stage graphs that touch the hand-off slot h as well as parity buffers, for the chunks of one step % 6 (b = j & 1, h = j % 3).
+struct HandoffGraphs {
   // stream C: the rest of stage 1 with the padded-length bucket chosen ON THE DEVICE = {k_set_bucket -> SWITCH conditional node whose
   // body i is the stage-1 sequence for the padded length 128 i (0: no effective frame)}; built at session creation, no host sync
   StageGraph s1;
   StageGraph s2_pro;       // stage-2 prologue (single session: + layer 0; group member: into the group's batched input)
-  StageGraph s2_layers;    // single session: stage-2 layers 1..14
   StageGraph s2_epi;       // stage-2 epilogue (single session: layer 15 +; group member: from the group's batched output)
   StageGraph dec_slide;    // stream D: decode-window slides
-  StageGraph synth;        // stream D: synthesizer + NaN scrub
 };
 // Events of one ring slot r = step % kRing.  Null until created, so a partly built session can be freed.
 struct StepEvents {
@@ -104,8 +111,9 @@ struct Session {
   // inter-stage buffers, double-buffered by step parity
   float *enc_f0[2], *enc_sp[2], *enc_ap[2], *enc_mc[2]; uint8_t* enc_voiced[2];
   double* d_mse; uint8_t* d_mask[2]; int* d_index[2]; int* d_count[2];
-  float *cv_mc_out[2], *cv_f0_out[2], *cv_ap_out[2], *cv_sp_out[2]; uint8_t* cv_voiced_out[2];
-  float* cv_sp_mid[2];
+  // the hand-off set: written by stage 1 (and cv_sp_out by the stage-2 epilogue), read by stage 2 and the decode slide; slot = step % 3
+  float *cv_mc_out[kHandoff], *cv_f0_out[kHandoff], *cv_ap_out[kHandoff], *cv_sp_out[kHandoff]; uint8_t* cv_voiced_out[kHandoff];
+  float* cv_sp_mid[kHandoff];
   double* dec_f0_f64;
   int max_blocks;
   // host-API staging rings (pinned host + device), slot = step % kRing
@@ -116,6 +124,7 @@ struct Session {
   double* d_out_fixed[2];              // blocks written by the (captured) decode graph, by parity
   int* d_n_fixed[2];
   ParityGraphs graphs[2];
+  HandoffGraphs hgraphs[kHandoffGraphs];
   Synth* synth = nullptr;
   DioPlan* dio[2] = {nullptr, nullptr};     // one analysis plan per chunk parity (owned), f0 methods 0 and 1
   CrepePlan* crepe[2] = {nullptr, nullptr}; // f0 method 2: one CREPE forward per chunk parity (owned) in place of DIO/Harvest
@@ -298,9 +307,9 @@ static void group_free(Group* G) {
   for (int i = 0; i < kRing; ++i) if (G->ev_fwd[i]) cudaEventDestroy(G->ev_fwd[i]);
   for (Session* m : G->members) {
     m->group = nullptr;
-    for (ParityGraphs& pg : m->graphs) {          // the captured stage-2 prologue / epilogue graphs point into the group's plan
-      pg.s2_pro.reset();
-      pg.s2_epi.reset();
+    for (HandoffGraphs& hg : m->hgraphs) {        // the captured stage-2 prologue / epilogue graphs point into the group's plan
+      hg.s2_pro.reset();
+      hg.s2_epi.reset();
     }
   }
   delete G;
@@ -390,18 +399,38 @@ static int stage_graph_launch(Engine* e, const StageGraph& g, cudaStream_t st) {
   return 0;
 }
 
+// capture body() on stream st into g
+template <typename F>
+static int capture_graph(StageGraph& g, cudaStream_t st, F&& body) {
+  cudaGraph_t graph = nullptr;
+  RYK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+  int rc = body();
+  cudaError_t err = cudaStreamEndCapture(st, &graph);
+  if (rc) return rc;
+  RYK_CUDA(err);
+  return stage_graph_init(g, graph);
+}
+
 // run_graph captures body() on stream st into g on first use and replays g.
 template <typename F>
 static int run_graph(Engine* e, StageGraph& g, cudaStream_t st, F&& body) {
-  if (!g.exec) {
-    cudaGraph_t graph = nullptr;
-    RYK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    int rc = body();
-    cudaError_t err = cudaStreamEndCapture(st, &graph);
-    if (rc) return rc;
-    RYK_CUDA(err);
-    if (stage_graph_init(g, graph)) return -1;
-  }
+  if (!g.exec && capture_graph(g, st, body)) return -1;
+  return stage_graph_launch(e, g, st);
+}
+
+// The same for a graph of step k that has a copy per hand-off slot (member `which` of s->hgraphs[k % 6]; body(h) enqueues the copy of
+// slot h).  The first step of a parity captures the copies of all three slots and uploads the two it does not launch, so the steps
+// after the first two pay for no capture or upload, as with the graphs kept per parity.
+template <typename F>
+static int run_handoff_graph(Engine* e, Session* s, long long k, StageGraph HandoffGraphs::*which, cudaStream_t st, F&& body) {
+  StageGraph& g = s->hgraphs[k % kHandoffGraphs].*which;
+  if (!g.exec)
+    for (int j = (int)(k & 1); j < kHandoffGraphs; j += 2) {
+      StageGraph& gj = s->hgraphs[j].*which;
+      if (gj.exec) continue;
+      if (capture_graph(gj, st, [&]() -> int { return body(j % kHandoff); })) return -1;
+      if (&gj != &g) RYK_CUDA(cudaGraphUpload(gj.exec, st));
+    }
   return stage_graph_launch(e, g, st);
 }
 
@@ -419,10 +448,12 @@ __global__ void k_set_bucket(cudaGraphConditionalHandle handle, const int* __res
   }
 }
 
-static int stage1_body(Engine* e, Session* s, int b, int tp1);
+static int stage1_body(Engine* e, Session* s, int b, int h, int tp1);
 
-// Build the per-parity stage-1 graph with a device-side switch over the padded-length buckets (CUDA conditional nodes, 12.8+).
-static int stage1_build_switch(Engine* e, Session* s, int b) {
+// Build the stage-1 graph of the chunks of step % 6 = j with a device-side switch over the padded-length buckets (CUDA conditional
+// nodes, 12.8+).
+static int stage1_build_switch(Engine* e, Session* s, int j) {
+  const int b = j & 1, h = j % kHandoff;
   const int n_buckets = s->Tp / 128 + 1;
   RYK_CHECK(n_buckets <= 16, "window too long for the stage-1 graph table");
   cudaGraph_t graph = nullptr;
@@ -449,7 +480,7 @@ static int stage1_build_switch(Engine* e, Session* s, int b) {
   for (int i = 0; i < n_buckets; ++i) {
     cudaGraph_t body = cp.conditional.phGraph_out[i];
     RYK_CUDA(cudaStreamBeginCaptureToGraph(s->sC, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-    int rc = stage1_body(e, s, b, i * 128);
+    int rc = stage1_body(e, s, b, h, i * 128);
     cudaGraph_t out = nullptr;
     cudaError_t err = cudaStreamEndCapture(s->sC, &out);
     if (rc) return rc;
@@ -458,7 +489,9 @@ static int stage1_build_switch(Engine* e, Session* s, int b) {
     if (kernels.n[i] < 0) return -1;
   }
   RYK_CUDA(cudaGraphKernelNodeSetParams(set_node, &kp));
-  return stage_graph_init(s->graphs[b].s1, graph);
+  if (stage_graph_init(s->hgraphs[j].s1, graph)) return -1;
+  RYK_CUDA(cudaGraphUpload(s->hgraphs[j].s1.exec, s->sC));     // the first step of each copy does not pay for the upload
+  return 0;
 }
 
 // The head of stage 1 of a chunk of parity b: slide the feature window by the analysis outputs and run the silence gate on the
@@ -477,11 +510,11 @@ static int stage1_head(Engine* e, Session* s, int b) {
                        s->d_count[b], s->sC);
 }
 
-// The rest of stage 1 of a chunk of parity b: (gather ->) 1-D U-Net at padded length tp1 (0: no effective frame, voice_changer.py:32-35
-// skips the net) -> scatter into the silent template + f0 map, mc2sp.  Enqueued on stream C while it is captured as one body of the
-// parity's SWITCH graph; every body is captured when the session is created so that no chunk ever pays for a capture in the middle of
-// a stream.
-static int stage1_body(Engine* e, Session* s, int b, int tp1) {
+// The rest of stage 1 of a chunk of parity b and hand-off slot h: (gather ->) 1-D U-Net at padded length tp1 (0: no effective frame,
+// voice_changer.py:32-35 skips the net) -> scatter into the silent template + f0 map, mc2sp.  Enqueued on stream C while it is captured
+// as one body of the chunk's SWITCH graph; every body is captured when the session is created so that no chunk ever pays for a capture
+// in the middle of a stream.
+static int stage1_body(Engine* e, Session* s, int b, int h, int tp1) {
   const int g = b ^ 1;
   const ryk_session_config& c = s->cfg;
   const float* d_y = nullptr;
@@ -493,8 +526,8 @@ static int stage1_body(Engine* e, Session* s, int b, int tp1) {
     d_y = (const float*)p1->d_out;
   }
   if (stage1_epilogue_run(s->voice, d_y, s->d_index[b], s->d_mask[b], s->d_count[b], s->Tw, s->C, s->cw_f0[g], s->cw_ap[g], s->cw_voiced[g], s->nb,
-                          kSilentMc0, s->cv_mc_out[b], s->cv_f0_out[b], s->cv_ap_out[b], s->cv_voiced_out[b], s->sC)) return -1;
-  return mc2sp_run(e, s->sptk.d_H, s->cv_mc_out[b], s->Tw, c.order, c.fft_length, 1e-16, s->cv_sp_mid[b], nullptr, s->sC);
+                          kSilentMc0, s->cv_mc_out[h], s->cv_f0_out[h], s->cv_ap_out[h], s->cv_voiced_out[h], s->sC)) return -1;
+  return mc2sp_run(e, s->sptk.d_H, s->cv_mc_out[h], s->Tw, c.order, c.fft_length, 1e-16, s->cv_sp_mid[h], nullptr, s->sC);
 }
 
 // Step k = s->step is enqueued in three parts so that a group can interleave its members:
@@ -502,7 +535,7 @@ static int stage1_body(Engine* e, Session* s, int b, int tp1) {
 //   mid:   the stage-2 U-Net forward (single session: on its own stream C2; group: one batched forward on the group stream)
 //   back:  stage-2 epilogue and stream D (synthesizer); results land in s->d_out_fixed[b] / s->d_n_fixed[b]; s->step advances.
 // In each part b = k & 1 selects the inter-stage buffer set; the sliding windows are read from [f] = [b] and written to [g] = [b ^ 1];
-// r = k % kRing is the event slot.
+// h = k % 3 is the hand-off slot, hgraphs[k % 6] the graphs that touch it, and r = k % kRing the event slot.
 
 // stage 2 of a single session alternates its stream (and plan) by chunk parity; a group member always uses the first stream
 static cudaStream_t s2_stream(const Session* s, int b) { return s->sC2s[s->group ? 0 : b]; }
@@ -577,29 +610,32 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
   if (run_graph(e, pg.s1_head, s->sC, [&]() -> int { return stage1_head(e, s, b); })) return -1;
   // the next chunks of this parity wait only for the head, so stage 1's U-Net is off the gate -> analysis -> stage 1 recurrence
   RYK_CUDA(cudaEventRecord(s->ev[r].cslide, s->sC));
-  if (k >= 2) {
-    RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[(k - 2) % kRing].dslide, 0));   // cv_{f0,ap,voiced}_out[b] consumed by decode k-2
-    RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[(k - 2) % kRing].conv, 0));     // cv_sp_mid[b] consumed by stage 2 of k-2
+  // three hand-off slots: stage 1 rewrites what step k-3 handed on, so it runs beside stage 2 of k-2 (and k-1)
+  if (k >= kHandoff) {
+    RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[(k - 3) % kRing].dslide, 0));   // cv_{f0,ap}_out[h] consumed by decode k-3
+    RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[(k - 3) % kRing].conv, 0));     // cv_sp_mid[h] consumed by stage 2 of k-3
   }
-  if (stage_graph_launch(e, pg.s1, s->sC)) return -1;     // counts the setter; k_set_bucket counts the body it selects
+  if (stage_graph_launch(e, s->hgraphs[k % kHandoffGraphs].s1, s->sC)) return -1;   // counts the setter; k_set_bucket counts the body
   if (stage_time(s, 2, 1, r, s->sC)) return -1;
   RYK_CUDA(cudaEventRecord(s->ev[r].s1, s->sC));
 
   // ================= stream C2: stage-2 prologue =================
   RYK_CUDA(cudaStreamWaitEvent(sC2, s->ev[r].s1, 0));
-  if (k >= 2) RYK_CUDA(cudaStreamWaitEvent(sC2, s->ev[(k - 2) % kRing].dslide, 0));  // cv_sp_out[b] consumed by decode k-2
+  if (k >= kHandoff) RYK_CUDA(cudaStreamWaitEvent(sC2, s->ev[(k - 3) % kRing].dslide, 0));  // cv_sp_out[h] consumed by decode k-3
   if (stage_time(s, 3, 0, r, sC2)) return -1;
   if (s->group) {
     Group* G = s->group;
     if (G->step >= 1) RYK_CUDA(cudaStreamWaitEvent(sC2, G->ev_fwd[(G->step - 1) % kRing], 0));   // batched input read by forward k-1
     float* dst = (float*)G->p2->d_in + (size_t)s->slot * s->Tp * 512;
-    if (run_graph(e, pg.s2_pro, sC2, [&]() -> int { return sr_prologue_run(e, s->cv_sp_mid[b], s->Tw, s->Tp, s->nb, dst, sC2, d_colmin); })) return -1;
+    if (run_handoff_graph(e, s, k, &HandoffGraphs::s2_pro, sC2, [&](int h) -> int {
+          return sr_prologue_run(e, s->cv_sp_mid[h], s->Tw, s->Tp, s->nb, dst, sC2, d_colmin);
+        })) return -1;
     RYK_CUDA(cudaEventRecord(s->ev[r].pro, sC2));
   } else {
     UNetPlan* p2 = nullptr;
     if (s2_plan(e, s, b, &p2)) return -1;
-    if (run_graph(e, pg.s2_pro, sC2, [&]() -> int {
-          if (sr_prologue_run(e, s->cv_sp_mid[b], s->Tw, s->Tp, s->nb, (float*)p2->d_in, sC2, d_colmin)) return -1;
+    if (run_handoff_graph(e, s, k, &HandoffGraphs::s2_pro, sC2, [&](int h) -> int {
+          if (sr_prologue_run(e, s->cv_sp_mid[h], s->Tw, s->Tp, s->nb, (float*)p2->d_in, sC2, d_colmin)) return -1;
           return unet_forward(e, p2, sC2, 0, 0);
         })) return -1;
   }
@@ -630,13 +666,15 @@ static int session_back(Engine* e, Session* s) {
     Group* G = s->group;
     RYK_CUDA(cudaStreamWaitEvent(sC2, G->ev_fwd[G->step % kRing], 0));
     const float* src = (const float*)G->p2->d_out + (size_t)s->slot * s->Tp * 512;
-    if (run_graph(e, pg.s2_epi, sC2, [&]() -> int { return sr_epilogue_run(e, src, s->Tw, s->nb, s->cv_sp_out[b], sC2, pc, pc + s->n_feat); })) return -1;
+    if (run_handoff_graph(e, s, k, &HandoffGraphs::s2_epi, sC2, [&](int h) -> int {
+          return sr_epilogue_run(e, src, s->Tw, s->nb, s->cv_sp_out[h], sC2, pc, pc + s->n_feat);
+        })) return -1;
   } else {
     UNetPlan* p2 = nullptr;
     if (s2_plan(e, s, b, &p2)) return -1;
-    if (run_graph(e, pg.s2_epi, sC2, [&]() -> int {
+    if (run_handoff_graph(e, s, k, &HandoffGraphs::s2_epi, sC2, [&](int h) -> int {
           if (unet_forward(e, p2, sC2, 15, 15)) return -1;
-          return sr_epilogue_run(e, (const float*)p2->d_out, s->Tw, s->nb, s->cv_sp_out[b], sC2, pc, pc + s->n_feat);
+          return sr_epilogue_run(e, (const float*)p2->d_out, s->Tw, s->nb, s->cv_sp_out[h], sC2, pc, pc + s->n_feat);
         })) return -1;
   }
   if (stage_time(s, 3, 1, r, sC2)) return -1;
@@ -647,17 +685,17 @@ static int session_back(Engine* e, Session* s) {
   if (stage_time(s, 4, 0, r, s->sD)) return -1;
   if (synth_host_advance(e, s->synth, s->Td, s->sD)) return -1;
   const int max_blocks = s->max_blocks;
-  if (run_graph(e, pg.dec_slide, s->sD, [&]() -> int {
+  if (run_handoff_graph(e, s, k, &HandoffGraphs::dec_slide, s->sD, [&](int h) -> int {
         SlideBatch sb; sb.n = 0;
-        slide_add<float>(sb, s->dw_f0[f], s->cv_f0_out[b] + pc, s->dw_f0[g], s->Td, s->n_feat, 1);
-        slide_add<float>(sb, s->dw_ap[f], s->cv_ap_out[b] + (size_t)pc * s->nb, s->dw_ap[g], s->Td, s->n_feat, s->nb);
-        slide_add<float>(sb, s->dw_sp[f], s->cv_sp_out[b] + (size_t)pc * s->nb, s->dw_sp[g], s->Td, s->n_feat, s->nb);
+        slide_add<float>(sb, s->dw_f0[f], s->cv_f0_out[h] + pc, s->dw_f0[g], s->Td, s->n_feat, 1);
+        slide_add<float>(sb, s->dw_ap[f], s->cv_ap_out[h] + (size_t)pc * s->nb, s->dw_ap[g], s->Td, s->n_feat, s->nb);
+        slide_add<float>(sb, s->dw_sp[f], s->cv_sp_out[h] + (size_t)pc * s->nb, s->dw_sp[g], s->Td, s->n_feat, s->nb);
         if (slide_batch(sb, s->sD)) return -1;
         k_f32_to_f64<<<(s->Td + 127) / 128, 128, 0, s->sD>>>(s->dw_f0[g], s->dec_f0_f64, s->Td);
         RYK_CUDA(cudaGetLastError());
         return 0;
       })) return -1;
-  // the converted features of this parity are free again as soon as they sit in the decode window
+  // the converted features of this hand-off slot are free again as soon as they sit in the decode window
   RYK_CUDA(cudaEventRecord(s->ev[r].dslide, s->sD));
   if (run_graph(e, pg.synth, s->sD, [&]() -> int {
         if (synth_add_kernel(e, s->synth, s->dec_f0_f64, s->Td, s->dw_sp[g], s->dw_ap[g], s->sD)) return -1;
@@ -849,6 +887,8 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
     if (A((void**)&s->d_mask[i], (size_t)s->Tw)) return -1;
     if (A((void**)&s->d_index[i], sizeof(int) * s->Tw)) return -1;
     if (A((void**)&s->d_count[i], sizeof(int) * 2)) return -1;
+  }
+  for (int i = 0; i < kHandoff; ++i) {
     if (A((void**)&s->cv_mc_out[i], sizeof(float) * (size_t)s->Tw * s->C)) return -1;
     if (A((void**)&s->cv_f0_out[i], sizeof(float) * s->Tw)) return -1;
     if (A((void**)&s->cv_ap_out[i], sizeof(float) * (size_t)s->Tw * s->nb)) return -1;
@@ -890,7 +930,7 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
   // (the stage-2 plans are created on first use: a session that joins a group never needs its own)
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   RYK_CUDA(cudaDeviceSynchronize());
-  for (int b = 0; b < 2; ++b) if (stage1_build_switch(e, s, b)) return -1;
+  for (int j = 0; j < kHandoffGraphs; ++j) if (stage1_build_switch(e, s, j)) return -1;
   return 0;
 }
 
@@ -1073,7 +1113,7 @@ static Group* get_group(Engine* e, int id) { return (id >= 0 && id < (int)e->gro
 // steps is uncollected, and it synchronises the device before it frees or rebuilds anything, so no step of the old layout is in flight.
 // The guards of the steps after it still hold across the switch of a member's stage 2 between sC2s[0] (grouped) and sC2s[b] (alone):
 //   * every cross-stage guard is an event of the member's own ring, indexed by its own step count (which a change keeps), so the
-//     waits of step k on the events of steps k-1 and k-2 find them wherever those steps ran;
+//     waits of step k on the events of steps k-1, k-2 and k-3 find them wherever those steps ran;
 //   * d_colmin[0] is only ever written on sC2s[0] and d_colmin[1] only on sC2s[1] (a member uses sC2s[0] with d_colmin[0], a single
 //     session sC2s[b] with d_colmin[b]), so each stays ordered by its stream;
 //   * the stage-2 plans a step uses are new after a change (the group's rebuilt plan, or the leaving member's own plans built by the
@@ -1152,7 +1192,7 @@ static int group_rebuild(Engine* e, Group* G, const std::vector<Session*>& membe
       for (ParityGraphs& pg : m->graphs) pg.s2_layers.reset();
     }
     m->group = G; m->slot = (int)i;
-    for (ParityGraphs& pg : m->graphs) { pg.s2_pro.reset(); pg.s2_epi.reset(); }
+    for (HandoffGraphs& hg : m->hgraphs) { hg.s2_pro.reset(); hg.s2_epi.reset(); }
   }
   G->members = members;
   return 0;
@@ -1220,7 +1260,8 @@ int ryk_group_remove(ryk_engine* h, int group_id, int session_id) {
     return -1;
   }
   s->group = nullptr; s->slot = 0;
-  for (ParityGraphs& pg : s->graphs) { pg.s2_pro.reset(); pg.s2_layers.reset(); pg.s2_epi.reset(); }
+  for (ParityGraphs& pg : s->graphs) pg.s2_layers.reset();
+  for (HandoffGraphs& hg : s->hgraphs) { hg.s2_pro.reset(); hg.s2_epi.reset(); }
   return 0;
 }
 
