@@ -257,6 +257,40 @@ int ryk_session_set_input_rate(ryk_engine* e, int session_id, int rate, int up, 
 int ryk_session_set_output_rate(ryk_engine* e, int session_id, int rate, int up, int down, const double* taps, int n_taps);
 int ryk_session_io_geometry(ryk_engine* e, int session_id, int* n_in, int* max_out, int* delay_in, int* in_rate, int* out_rate);
 
+/* The f0 map of a session and the log-f0 statistics of its speaker.  A session converts f0 by
+ * exp((ln f0 - in_mean) / in_std * target_std + target_mean) (yukarin's F0Converter).  The map starts as the f0 statistics of the
+ * session's voice and belongs to the session from then on: setting it never touches the voice or another session, so several callers
+ * converting into one voice can each have the input statistics of their own speaker, and target_mean + s * ln(2) / 12 shifts the pitch
+ * by s semitones (the spectral envelope is not moved).
+ * ryk_session_get_f0_map: the values the NEXT submitted step will use (in follow mode: the fallback input side).
+ * ryk_session_set_f0_map: takes effect at the next submitted step and for every later one; steps already submitted keep the map they
+ *   were submitted with.  Allowed with chunks in flight and for a group member; it does not wait for the device and launches nothing.
+ *   On a session whose voice has no f0 statistics (identity map) it turns the map on for this session only.
+ * ryk_session_f0_measure: fresh session only (no chunk pushed).  Each step then adds the voiced frames of its chunk -- every 5 ms
+ *   frame of the input exactly once, whatever the silence gate decides about it -- to a running count, mean and variance of ln f0
+ *   kept on the device in FP64 (one more kernel per step).  The result depends on the input stream alone: it is bit-identical from
+ *   run to run and does not depend on what else the engine runs.
+ * ryk_session_f0_follow: needs measuring and a map.  With follow = 1, from the next submitted step on, every step whose running count
+ *   (its own chunk included) has reached min_voiced_frames (>= 1) converts with in_mean = the measured mean and in_std =
+ *   max(measured std, sd_floor); before that it uses the input side last set from the host.  sd_floor (finite, > 0; 0.05, about 0.9
+ *   semitones, is a reasonable value) keeps a monotone speaker from dividing by zero.  The estimate is cumulative (no forgetting).
+ *   ryk_session_set_f0_map while following replaces the target side and the fallback input side.  follow = 0 (the other two arguments
+ *   are ignored) returns to the host's input side.
+ * ryk_session_f0_measure_reset: the statistics restart from zero at the next submitted step (in follow mode the input side falls
+ *   back to the host's until min_voiced_frames are counted again).
+ * ryk_session_f0_measured: waits for stage 1 of the session's submitted steps, then returns the voiced frames counted and the mean
+ *   and (population) standard deviation of ln f0 over them (std 0 when fewer than 2 frames).  The variance std * std and the mean are
+ *   what an input_statistics file holds.  Any output pointer may be NULL.
+ * Refused, changing nothing: a non-finite value, a standard deviation <= 0, follow without measuring or without a map, measuring
+ * switched on a session that has run a step, an unknown session. */
+typedef struct { double in_mean, in_std, target_mean, target_std; } ryk_f0_map;
+int ryk_session_get_f0_map(ryk_engine* e, int session_id, ryk_f0_map* map);
+int ryk_session_set_f0_map(ryk_engine* e, int session_id, const ryk_f0_map* map);
+int ryk_session_f0_measure(ryk_engine* e, int session_id, int enable);
+int ryk_session_f0_follow(ryk_engine* e, int session_id, int follow, int min_voiced_frames, double sd_floor);
+int ryk_session_f0_measure_reset(ryk_engine* e, int session_id);
+int ryk_session_f0_measured(ryk_engine* e, int session_id, long long* n_voiced, double* mean, double* std);
+
 /* Diagnostics: device timeline (ms) of the last <= 8 steps x 5 stages {gate, analysis, stage 1, stage 2, synthesis}; needs
  * RYK_STAGE_TIMES=1 in the environment at session creation.  start/end hold 40 floats; returns the number of steps. */
 int ryk_session_stage_times(ryk_engine* e, int session_id, float* start, float* end);

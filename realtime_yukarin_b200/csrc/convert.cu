@@ -43,7 +43,7 @@ int convert_window_device(Engine* e, const ConvertBuffers& cb, int T, int n_wave
     d_y = (const float*)p1->d_out;
   }
   if (stage1_epilogue_run(v, d_y, cb.d_index, cb.d_mask, cb.d_count, T, C, cb.d_f0, cb.d_ap, cb.d_voiced, nb, kSilentMc0,
-                          cb.d_mc_out, cb.d_f0_out, cb.d_ap_out, cb.d_voiced_out, st)) return -1;
+                          cb.d_mc_out, cb.d_f0_out, cb.d_ap_out, cb.d_voiced_out, nullptr, st)) return -1;
   if (mc2sp_run(e, d_H, cb.d_mc_out, T, order, fftlen, 1e-16, cb.d_sp_mid, nullptr, st)) return -1;
   const int Tp = T + (128 - T % 128);
   UNetPlan* p2 = nullptr;

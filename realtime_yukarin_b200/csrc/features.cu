@@ -196,7 +196,7 @@ __global__ void k_stage1_epilogue(const float* __restrict__ y /*[Tp][C] network 
                                   const uint8_t* __restrict__ mask, const int* __restrict__ count, int T, int C,
                                   const float* __restrict__ mean, const float* __restrict__ std_,
                                   const float* __restrict__ f0_in, const float* __restrict__ ap_in, const uint8_t* __restrict__ voiced_in,
-                                  int nb, double mu_i, double sd_i, double mu_t, double sd_t, int has_f0_stats, float silent_mc0,
+                                  int nb, F0Map voice_map, const F0Map* __restrict__ session_map, float silent_mc0,
                                   float* __restrict__ mc_out, float* __restrict__ f0_out, float* __restrict__ ap_out,
                                   uint8_t* __restrict__ voiced_out) {
   int t = blockIdx.x;
@@ -217,6 +217,13 @@ __global__ void k_stage1_epilogue(const float* __restrict__ y /*[Tp][C] network 
     float f = 0.f;
     if (v) {
       float fi = f0_in[t];
+      // a session's map lives in device memory (it changes between steps without a new capture); the per-op calls pass the voice's
+      double mu_i = voice_map.mu_in, sd_i = voice_map.sd_in, mu_t = voice_map.mu_tgt, sd_t = voice_map.sd_tgt;
+      int has_f0_stats = voice_map.has_stats;
+      if (session_map) {
+        mu_i = session_map->mu_in; sd_i = session_map->sd_in; mu_t = session_map->mu_tgt; sd_t = session_map->sd_tgt;
+        has_f0_stats = session_map->has_stats;
+      }
       if (has_f0_stats) {
         // F0Converter: exp((ln f0 - mu_i) / sd_i * sd_t + mu_t); DECIDE: evaluated in float64, rounded to float32
         f = (float)exp((log((double)fi) - mu_i) / sd_i * sd_t + mu_t);
@@ -264,13 +271,80 @@ int stage1_prologue_run(const Voice* v, const float* d_mc, const int* d_index, c
   return 0;
 }
 
+F0Map voice_f0_map(const Voice* v) {
+  F0Map m = {};
+  m.mu_in = v->f0_in_mean; m.sd_in = v->f0_in_std; m.mu_tgt = v->f0_tgt_mean; m.sd_tgt = v->f0_tgt_std;
+  m.has_stats = v->has_f0_stats ? 1 : 0;
+  return m;
+}
+
 int stage1_epilogue_run(const Voice* v, const float* d_y, const int* d_index, const uint8_t* d_mask, const int* d_count, int T, int C,
                         const float* d_f0_in, const float* d_ap_in, const uint8_t* d_voiced_in, int nb, float silent_mc0,
-                        float* d_mc_out, float* d_f0_out, float* d_ap_out, uint8_t* d_voiced_out, cudaStream_t st) {
+                        float* d_mc_out, float* d_f0_out, float* d_ap_out, uint8_t* d_voiced_out, const F0Map* d_map, cudaStream_t st) {
   if (T <= 0) return 0;
   k_stage1_epilogue<<<T, 128, 0, st>>>(d_y, d_index, d_mask, d_count, T, C, v->d_s1_out_mean, v->d_s1_out_std, d_f0_in, d_ap_in,
-                                       d_voiced_in, nb, v->f0_in_mean, v->f0_in_std, v->f0_tgt_mean, v->f0_tgt_std,
-                                       v->has_f0_stats ? 1 : 0, silent_mc0, d_mc_out, d_f0_out, d_ap_out, d_voiced_out);
+                                       d_voiced_in, nb, voice_f0_map(v), d_map, silent_mc0, d_mc_out, d_f0_out, d_ap_out, d_voiced_out);
+  RYK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------ speaker statistics of ln f0
+// (count, mean, M2) of two disjoint sets -> of their union (Chan et al.): no sum of squares, so no cancellation at large counts
+__device__ __forceinline__ void f0_stats_merge(long long& n, double& mean, double& m2, long long nb, double mean_b, double m2_b) {
+  if (nb == 0) return;
+  if (n == 0) { n = nb; mean = mean_b; m2 = m2_b; return; }
+  const long long nn = n + nb;
+  const double d = mean_b - mean;
+  mean += d * ((double)nb / (double)nn);
+  m2 += m2_b + d * d * ((double)n * (double)nb / (double)nn);
+  n = nn;
+}
+
+// One CTA: the voiced frames of the chunk's n frames are folded into (count, mean, M2) of ln f0 in a fixed order -- thread i takes
+// frames i, i + 256, ... one by one, then a pairwise tree over the 256 partial triples -- and thread 0 merges the chunk into the
+// running triple.  No atomics: the result depends on the frames alone.  Follow mode: once min_voiced frames are counted the measured
+// mean and max(sqrt(M2 / count), sd_floor) become the input side of the session's f0 map, which the stage-1 epilogue of this step reads
+// next on the same stream.
+constexpr int kF0MeasureThreads = 256;
+__global__ void __launch_bounds__(kF0MeasureThreads) k_f0_measure(const float* __restrict__ f0, const uint8_t* __restrict__ voiced, int n,
+                                                                 F0Stats* __restrict__ stats, F0Map* __restrict__ map) {
+  __shared__ long long s_n[kF0MeasureThreads];
+  __shared__ double s_mean[kF0MeasureThreads], s_m2[kF0MeasureThreads];
+  const int tid = threadIdx.x;
+  long long cn = 0; double mean = 0.0, m2 = 0.0;
+#pragma unroll 1                   // a chunk is rarely longer than one pass; unrolled, the FP64 log and division bodies spill
+  for (int i = tid; i < n; i += kF0MeasureThreads) {
+    const float f = f0[i];
+    if (voiced[i] != 0 && f > 0.f) {
+      const double x = log((double)f);
+      const double d = x - mean;
+      ++cn;
+      mean += d / (double)cn;
+      m2 += d * (x - mean);
+    }
+  }
+  s_n[tid] = cn; s_mean[tid] = mean; s_m2[tid] = m2;
+  __syncthreads();
+  for (int s = kF0MeasureThreads / 2; s > 0; s >>= 1) {
+    if (tid < s) {
+      f0_stats_merge(cn, mean, m2, s_n[tid + s], s_mean[tid + s], s_m2[tid + s]);
+      s_n[tid] = cn; s_mean[tid] = mean; s_m2[tid] = m2;
+    }
+    __syncthreads();
+  }
+  if (tid == 0) {
+    long long rn = stats->n; double rmean = stats->mean, rm2 = stats->m2;
+    f0_stats_merge(rn, rmean, rm2, cn, mean, m2);
+    stats->n = rn; stats->mean = rmean; stats->m2 = rm2;
+    if (map->follow && rn >= (long long)map->min_voiced) {
+      map->mu_in = rmean;
+      map->sd_in = fmax(sqrt(rm2 / (double)rn), map->sd_floor);
+    }
+  }
+}
+
+int f0_measure_run(const float* d_f0, const uint8_t* d_voiced, int n, F0Stats* d_stats, F0Map* d_map, cudaStream_t st) {
+  k_f0_measure<<<1, kF0MeasureThreads, 0, st>>>(d_f0, d_voiced, n, d_stats, d_map);
   RYK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -7,12 +7,27 @@ namespace ryk {
 struct Engine;
 struct Voice;
 
+// The f0 map of one session, exp((ln f0 - mu_in) / sd_in * sd_tgt + mu_tgt), as one block of device memory that the stage-1 epilogue
+// reads at run time (DESIGN.md §4a).  The host stages a new block between steps; in follow mode k_f0_measure rewrites mu_in / sd_in.
+struct F0Map {
+  double mu_in, sd_in, mu_tgt, sd_tgt;
+  double sd_floor;                  // follow mode: lower bound of the measured sd_in
+  int has_stats;                    // 0: identity map (a voice without f0 statistics and no map set on the session)
+  int follow, min_voiced;           // follow mode: input side = the measured statistics once min_voiced voiced frames are counted
+  int pad_;
+};
+// running statistics of ln f0 over the voiced frames of a session's input: count, mean, sum of squared deviations
+struct F0Stats { long long n; double mean, m2; };
+
 // normalisation with the stage-1 statistics of voice v
 int stage1_prologue_run(const Voice* v, const float* d_mc, const int* d_index, const int* d_count, int C, float* d_x, int Tp_capacity, cudaStream_t st);
-// de-normalisation and f0 conversion with the statistics of voice v
+// de-normalisation with the statistics of voice v, and f0 conversion with the map in *d_map (nullptr: the f0 statistics of voice v)
 int stage1_epilogue_run(const Voice* v, const float* d_y, const int* d_index, const uint8_t* d_mask, const int* d_count, int T, int C,
                         const float* d_f0_in, const float* d_ap_in, const uint8_t* d_voiced_in, int nb, float silent_mc0,
-                        float* d_mc_out, float* d_f0_out, float* d_ap_out, uint8_t* d_voiced_out, cudaStream_t st);
+                        float* d_mc_out, float* d_f0_out, float* d_ap_out, uint8_t* d_voiced_out, const F0Map* d_map, cudaStream_t st);
+F0Map voice_f0_map(const Voice* v);
+// merge the n frames of one chunk into *d_stats; in follow mode (d_map->follow) also write the measured input side into *d_map
+int f0_measure_run(const float* d_f0, const uint8_t* d_voiced, int n, F0Stats* d_stats, F0Map* d_map, cudaStream_t st);
 constexpr int kColminFloats = 64 * 512;      // column-minimum partials of the stage-2 prologue (one scratch per concurrent stream)
 int sr_prologue_run(Engine* e, const float* d_sp, int T, int Tp, int nb, float* d_x, cudaStream_t st, float* d_colmin = nullptr);
 // frames [t0, t1) of the T-frame window (t1 < 0: T); the other rows of d_sp_out are not written

@@ -143,6 +143,14 @@ struct Session {
   float* d_chunk_model = nullptr;             // the step's resampled chunk (n_wave model-rate samples)
   double* out_hist[2] = {nullptr, nullptr};   // kept synthesizer samples (out.hist)
   double* d_rout_fixed[2] = {nullptr, nullptr}; int* d_rn_fixed[2] = {nullptr, nullptr};   // device-rate output of a step, by parity
+  // The session's f0 map (ryk_session_set_f0_map / _f0_follow) and the statistics of its speaker (ryk_session_f0_measure).  The captured
+  // stage-1 graphs read *d_f0_map; f0_map_sync brings it up to date on stream C in front of a step's stage 1.
+  F0Map f0_map = {};               // what the next submitted step uses (follow mode: its input side is the fallback)
+  bool f0_dirty = false;           // f0_map changed since the last submitted step
+  bool f0_measure = false;         // the head of stage 1 ends with k_f0_measure
+  bool f0_reset = false;           // the statistics restart at the next submitted step
+  F0Map* d_f0_map = nullptr; F0Stats* d_f0_stats = nullptr;
+  F0Map* h_f0_map = nullptr;       // pinned staging, slot = step % kRing
   std::vector<void*> allocs, pinned;
 };
 
@@ -506,8 +514,30 @@ static int stage1_head(Engine* e, Session* s, int b) {
   slide_add<float>(sb, s->cw_mc[f], s->enc_mc[b] + (size_t)pe * s->C, s->cw_mc[g], s->Tw, s->n_feat, s->C);
   slide_add<uint8_t>(sb, s->cw_voiced[f], s->enc_voiced[b] + pe, s->cw_voiced[g], s->Tw, s->n_feat, 1);
   if (slide_batch(sb, s->sC)) return -1;
-  return gate_mask_run(e, s->cw_wave[g], s->Tw * s->hop, c.fft_length, s->hop, c.threshold_db, s->Tw, s->d_mse, s->d_mask[b], s->d_index[b],
-                       s->d_count[b], s->sC);
+  if (gate_mask_run(e, s->cw_wave[g], s->Tw * s->hop, c.fft_length, s->hop, c.threshold_db, s->Tw, s->d_mse, s->d_mask[b], s->d_index[b],
+                    s->d_count[b], s->sC)) return -1;
+  // the chunk's own frames: over a stream they tile the input, every 5 ms frame exactly once
+  if (s->f0_measure && f0_measure_run(s->enc_f0[b] + pe, s->enc_voiced[b] + pe, s->n_feat, s->d_f0_stats, s->d_f0_map, s->sC)) return -1;
+  return 0;
+}
+
+// In front of stage 1 of step k on stream C: restart the speaker statistics and copy the f0 map into the block the stage-1 graphs read,
+// when either was asked for since the previous step.  Stage 1 of every step runs on stream C in step order, so the steps already
+// submitted keep the map they were submitted with and step k is the first to see the new one; the host does not wait and no kernel runs.
+// The copy reads pinned slot k % kRing when the stream reaches it; that slot was last used by step k - kRing, whose copy ended before
+// the head of its stage 1 did (the wait returns at once unless the host is a whole ring ahead of the device).
+static int f0_map_sync(Session* s, long long k) {
+  if (s->f0_reset) {
+    RYK_CUDA(cudaMemsetAsync(s->d_f0_stats, 0, sizeof(F0Stats), s->sC));
+    s->f0_reset = false;
+  }
+  if (!s->f0_dirty) return 0;
+  const int r = (int)(k % kRing);
+  if (k >= kRing) RYK_CUDA(cudaEventSynchronize(s->ev[r].cslide));
+  s->h_f0_map[r] = s->f0_map;
+  RYK_CUDA(cudaMemcpyAsync(s->d_f0_map, s->h_f0_map + r, sizeof(F0Map), cudaMemcpyHostToDevice, s->sC));
+  s->f0_dirty = false;
+  return 0;
 }
 
 // The rest of stage 1 of a chunk of parity b and hand-off slot h: (gather ->) 1-D U-Net at padded length tp1 (0: no effective frame,
@@ -526,7 +556,7 @@ static int stage1_body(Engine* e, Session* s, int b, int h, int tp1) {
     d_y = (const float*)p1->d_out;
   }
   if (stage1_epilogue_run(s->voice, d_y, s->d_index[b], s->d_mask[b], s->d_count[b], s->Tw, s->C, s->cw_f0[g], s->cw_ap[g], s->cw_voiced[g], s->nb,
-                          kSilentMc0, s->cv_mc_out[h], s->cv_f0_out[h], s->cv_ap_out[h], s->cv_voiced_out[h], s->sC)) return -1;
+                          kSilentMc0, s->cv_mc_out[h], s->cv_f0_out[h], s->cv_ap_out[h], s->cv_voiced_out[h], s->d_f0_map, s->sC)) return -1;
   return mc2sp_run(e, s->sptk.d_H, s->cv_mc_out[h], s->Tw, c.order, c.fft_length, 1e-16, s->cv_sp_mid[h], nullptr, s->sC);
 }
 
@@ -605,6 +635,9 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
 
   // ================= stream C: stage 1 (head: feature slides + silence gate; then U-Net, f0 map, mc2sp) =================
   // mask / index / count[b] are written by the head and read by the SWITCH graph, both on stream C: no guard between steps needed
+  // (nor for the f0 map: the host's copy, the measuring kernel in the head and the epilogue in the SWITCH graph are all on stream C;
+  // the copy goes before the head so that it cannot overwrite what this step's measurement writes in follow mode)
+  if (f0_map_sync(s, k)) return -1;
   RYK_CUDA(cudaStreamWaitEvent(s->sC, s->ev[r].enc, 0));                       // (the analysis of step r waited for its wave slides)
   if (stage_time(s, 2, 0, r, s->sC)) return -1;
   if (run_graph(e, pg.s1_head, s->sC, [&]() -> int { return stage1_head(e, s, b); })) return -1;
@@ -900,6 +933,12 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
   for (int i = 0; i < 2; ++i) if (A((void**)&s->d_colmin[i], sizeof(float) * kColminFloats)) return -1;
   if (A((void**)&s->dec_f0_f64, sizeof(double) * s->Td)) return -1;
   if (A((void**)&s->d_chunk_fixed, sizeof(float) * s->n_wave)) return -1;
+  // the session starts on its voice's f0 map
+  if (A((void**)&s->d_f0_map, sizeof(F0Map))) return -1;
+  if (A((void**)&s->d_f0_stats, sizeof(F0Stats))) return -1;
+  if (P((void**)&s->h_f0_map, sizeof(F0Map) * kRing)) return -1;
+  s->f0_map = s->h_f0_map[0] = voice_f0_map(s->voice);
+  RYK_CUDA(cudaMemcpyAsync(s->d_f0_map, s->h_f0_map, sizeof(F0Map), cudaMemcpyHostToDevice, e->stream));
   s->max_blocks = (s->Td * s->hop) / cfg->vocoder_buffer_size + 4;
   s->max_out = s->max_blocks * cfg->vocoder_buffer_size;
   const size_t out_samples = (size_t)s->max_out;
@@ -1103,6 +1142,79 @@ int ryk_session_io_geometry(ryk_engine* h, int id, int* n_in, int* max_out, int*
   if (delay_in) *delay_in = s->delay_in;
   if (in_rate) *in_rate = s->in.rate ? s->in.rate : s->cfg.fs;
   if (out_rate) *out_rate = s->out.rate ? s->out.rate : s->cfg.fs;
+  return 0;
+}
+
+// ---- the session's f0 map and the statistics of its speaker (DESIGN.md §4a) ----
+// These calls change host state only; f0_map_sync carries it to the device at the next submitted step, alone or in a group.
+int ryk_session_get_f0_map(ryk_engine* h, int id, ryk_f0_map* map) {
+  Session* s = get_session(&h->impl, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  RYK_CHECK(map != nullptr, "null argument");
+  map->in_mean = s->f0_map.mu_in; map->in_std = s->f0_map.sd_in; map->target_mean = s->f0_map.mu_tgt; map->target_std = s->f0_map.sd_tgt;
+  return 0;
+}
+
+int ryk_session_set_f0_map(ryk_engine* h, int id, const ryk_f0_map* map) {
+  Session* s = get_session(&h->impl, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  RYK_CHECK(map != nullptr, "null argument");
+  RYK_CHECK(isfinite(map->in_mean) && isfinite(map->in_std) && isfinite(map->target_mean) && isfinite(map->target_std),
+            "the f0 map must be finite");
+  RYK_CHECK(map->in_std > 0 && map->target_std > 0, "the standard deviations of the f0 map must be positive");
+  s->f0_map.mu_in = map->in_mean; s->f0_map.sd_in = map->in_std; s->f0_map.mu_tgt = map->target_mean; s->f0_map.sd_tgt = map->target_std;
+  s->f0_map.has_stats = 1;
+  s->f0_dirty = true;
+  return 0;
+}
+
+int ryk_session_f0_measure(ryk_engine* h, int id, int enable) {
+  Session* s = get_session(&h->impl, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  RYK_CHECK(s->step == 0, "f0 measurement can only be switched on a fresh session (no chunk pushed): the head of stage 1 is captured at the first steps");
+  RYK_CHECK(enable || !s->f0_map.follow, "the session follows its measurement: turn follow mode off first");
+  s->f0_measure = enable != 0;
+  return 0;
+}
+
+int ryk_session_f0_follow(ryk_engine* h, int id, int follow, int min_voiced_frames, double sd_floor) {
+  Session* s = get_session(&h->impl, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  if (follow) {
+    RYK_CHECK(s->f0_measure, "follow mode needs f0 measurement (ryk_session_f0_measure)");
+    RYK_CHECK(s->f0_map.has_stats, "follow mode needs an f0 map: the voice has no f0 statistics and none were set on the session");
+    RYK_CHECK(min_voiced_frames >= 1, "min_voiced_frames must be at least 1");
+    RYK_CHECK(isfinite(sd_floor) && sd_floor > 0, "sd_floor must be finite and positive");
+    s->f0_map.min_voiced = min_voiced_frames; s->f0_map.sd_floor = sd_floor;
+  }
+  s->f0_map.follow = follow != 0;
+  s->f0_dirty = true;
+  return 0;
+}
+
+int ryk_session_f0_measure_reset(ryk_engine* h, int id) {
+  Session* s = get_session(&h->impl, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  RYK_CHECK(s->f0_measure, "f0 measurement is not enabled for this session");
+  s->f0_reset = true;
+  s->f0_dirty = true;            // follow mode: back to the host's input side until min_voiced_frames are counted again
+  return 0;
+}
+
+int ryk_session_f0_measured(ryk_engine* h, int id, long long* n_voiced, double* mean, double* std_) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Session* s = get_session(e, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  RYK_CHECK(s->f0_measure, "f0 measurement is not enabled for this session");
+  F0Stats st = {};
+  if (!s->f0_reset) {             // (a reset not yet submitted already reads as empty)
+    RYK_CUDA(cudaMemcpyAsync(&st, s->d_f0_stats, sizeof(st), cudaMemcpyDeviceToHost, s->sC));
+    RYK_CUDA(cudaStreamSynchronize(s->sC));      // behind the head of stage 1 of every submitted step
+  }
+  if (n_voiced) *n_voiced = st.n;
+  if (mean) *mean = st.mean;
+  if (std_) *std_ = st.n >= 2 ? sqrt(st.m2 / (double)st.n) : 0.0;
   return 0;
 }
 

@@ -64,7 +64,29 @@ EXPORTED_SYMBOLS = [
     'ryk_session_set_input_rate', 'ryk_session_set_output_rate', 'ryk_session_io_geometry',
     'ryk_voice_create', 'ryk_voice_destroy', 'ryk_voice_model_create', 'ryk_voice_model_set_layer', 'ryk_voice_stage1_set_stats',
     'ryk_voice_f0_set_stats', 'ryk_session_create_voice', 'ryk_session_voice', 'ryk_group_add', 'ryk_group_remove', 'ryk_group_members',
+    'ryk_session_get_f0_map', 'ryk_session_set_f0_map', 'ryk_session_f0_measure', 'ryk_session_f0_follow', 'ryk_session_f0_measure_reset',
+    'ryk_session_f0_measured',
 ]
+
+SEMITONE = math.log(2.0) / 12.0          # one semitone in ln f0
+F0_SD_FLOOR = 0.05                       # follow mode: least in_std (ln f0), about 0.9 semitones
+
+
+class F0Map(ctypes.Structure):
+    """ryk_f0_map: exp((ln f0 - in_mean) / in_std * target_std + target_mean)"""
+    _fields_ = [('in_mean', ctypes.c_double), ('in_std', ctypes.c_double), ('target_mean', ctypes.c_double), ('target_std', ctypes.c_double)]
+    KEYS = ('in_mean', 'in_std', 'target_mean', 'target_std')
+
+
+def updated_f0_map(current: Dict[str, float], in_mean=None, in_std=None, target_mean=None, target_std=None,
+                   semitones: float = 0.0) -> Dict[str, float]:
+    """`current` with the given values replaced (None keeps one) and the target mean raised by `semitones`."""
+    new = dict(current)
+    for key, value in zip(F0Map.KEYS, (in_mean, in_std, target_mean, target_std)):
+        if value is not None:
+            new[key] = float(value)
+    new['target_mean'] += float(semitones) * SEMITONE
+    return new
 
 
 def stage2_row_bands(Tp: int, W: int, keep_begin: int, keep_len: int) -> numpy.ndarray:
@@ -542,6 +564,42 @@ class Engine(object):
         v = [ctypes.c_int() for _ in range(5)]
         self._check(self.lib.ryk_session_io_geometry(self._h, sid, *[ctypes.byref(x) for x in v]))
         return dict(zip(('n_in', 'max_out', 'delay_in', 'in_rate', 'out_rate'), (x.value for x in v)))
+
+    # ---- the session's f0 map and the log-f0 statistics of its speaker ----
+    def session_get_f0_map(self, sid: int) -> Dict[str, float]:
+        """in_mean, in_std, target_mean, target_std that the next submitted step of the session uses (in follow mode the input side is
+        the fallback)."""
+        m = F0Map()
+        self._check(self.lib.ryk_session_get_f0_map(self._h, sid, ctypes.byref(m)))
+        return {k: getattr(m, k) for k in F0Map.KEYS}
+
+    def session_set_f0_map(self, sid: int, in_mean=None, in_std=None, target_mean=None, target_std=None, semitones: float = 0.0):
+        """Change this session's f0 map from its next submitted step on (chunks in flight keep theirs; other sessions of the voice are
+        not affected).  None keeps the current value.  `semitones` adds semitones * ln(2) / 12 to the target mean (the one given, else
+        the current one): that is the whole pitch control -- f0 moves, the spectral envelope (the formants) does not."""
+        new = updated_f0_map(self.session_get_f0_map(sid), in_mean, in_std, target_mean, target_std, semitones)
+        m = F0Map(*[new[k] for k in F0Map.KEYS])
+        self._check(self.lib.ryk_session_set_f0_map(self._h, sid, ctypes.byref(m)))
+
+    def session_f0_measure(self, sid: int, enable: bool = True):
+        """Fresh session only: keep running statistics of ln f0 over the voiced frames of the session's input on the device."""
+        self._check(self.lib.ryk_session_f0_measure(self._h, sid, int(bool(enable))))
+
+    def session_f0_follow(self, sid: int, follow: bool = True, min_voiced_frames: int = 200, sd_floor: float = F0_SD_FLOOR):
+        """Needs session_f0_measure.  From the next submitted step on, a step whose count of voiced frames has reached
+        `min_voiced_frames` (200 frames = 1 s of voiced speech) converts with the measured mean and max(measured std, sd_floor) as the
+        input side of its f0 map; follow=False returns to the values set from the host."""
+        self._check(self.lib.ryk_session_f0_follow(self._h, sid, int(bool(follow)), int(min_voiced_frames), ctypes.c_double(sd_floor)))
+
+    def session_f0_measure_reset(self, sid: int):
+        """The statistics restart from zero at the next submitted step."""
+        self._check(self.lib.ryk_session_f0_measure_reset(self._h, sid))
+
+    def session_f0_measured(self, sid: int):
+        """(voiced frames counted, mean, standard deviation) of ln f0 over the submitted steps (waits for their stage 1)."""
+        n, mean, std = ctypes.c_longlong(), ctypes.c_double(), ctypes.c_double()
+        self._check(self.lib.ryk_session_f0_measured(self._h, sid, ctypes.byref(n), ctypes.byref(mean), ctypes.byref(std)))
+        return n.value, mean.value, std.value
 
     def session_destroy(self, sid: int):
         self._check(self.lib.ryk_session_destroy(self._h, sid))

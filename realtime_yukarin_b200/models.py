@@ -110,6 +110,16 @@ class F0Converter(object):
         return engine.f0_convert(f0.ravel(), f0.ravel() != 0).reshape(f0.shape)
 
 
+def write_f0_statistics(path, mean: float, var: float) -> None:
+    """Write a log-f0 statistics file as upstream's training scripts do and F0Converter reads: a pickled dict {'mean', 'var'} in a
+    `.npy` (numpy.save of a dict), e.g. from engine.session_f0_measured -> (n, mean, std): var = std ** 2."""
+    mean, var = float(mean), float(var)
+    if not (numpy.isfinite(mean) and numpy.isfinite(var) and var > 0):
+        raise ValueError(f'log-f0 statistics need a finite mean and a positive variance, got mean {mean}, var {var}')
+    with open(str(path), 'wb') as f:             # (a file object: numpy.save would append '.npy' to another suffix)
+        numpy.save(f, numpy.array({'mean': mean, 'var': var}, dtype=object), allow_pickle=True)
+
+
 STATS_KEYS = ('stats/in_mean', 'stats/in_std', 'stats/out_mean', 'stats/out_std')
 
 

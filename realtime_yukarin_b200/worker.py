@@ -82,9 +82,14 @@ class RealtimePipeline(object):
 
     The models must already be loaded into `engine` (YukarinConverter.make_yukarin_converter does that for voice 0,
     models.load_voice for any voice); the session converts into `voice`.  `depth` chunks may be in flight (the reference's queues
-    are unbounded; the session keeps up to 5 steps in flight)."""
+    are unbounded; the session keeps up to 5 steps in flight).
 
-    def __init__(self, config: Config, acoustic_param=None, engine: Optional[Engine] = None, depth: int = 3, voice: int = 0):
+    `measure_f0=True` keeps running statistics of the speaker's log-f0 on the device (`measured_f0`); `follow_f0=N` (implies
+    measuring) also makes them the input side of the session's f0 map once N voiced frames are counted.  `set_f0_map` changes the
+    map between chunks."""
+
+    def __init__(self, config: Config, acoustic_param=None, engine: Optional[Engine] = None, depth: int = 3, voice: int = 0,
+                 measure_f0: bool = False, follow_f0: Optional[int] = None):
         self.config = config
         self.engine = engine or default_engine()
         p = acoustic_param
@@ -136,6 +141,10 @@ class RealtimePipeline(object):
             hop = round(fs * float(config.frame_period) / 1000)
             td = round(config.buffer_time * rate) + 2 * round(config.decode_extra_time * rate)
             n_out_cap = (td * hop // config.vocoder_buffer_size + 4) * config.vocoder_buffer_size
+        if measure_f0 or follow_f0 is not None:
+            self.engine.session_f0_measure(self._sid)
+        if follow_f0 is not None:
+            self.engine.session_f0_follow(self._sid, True, min_voiced_frames=int(follow_f0))
         self._scratch = numpy.empty(n_out_cap, dtype=numpy.float64)
         self._rid = self.engine.reblock_create(config.out_audio_chunk, n_out_cap, float(config.output_silent_threshold))
         self._inflight: Deque[Tuple[Item, int, int, float]] = deque()      # (item, session ticket, re-blocker ticket, host time of put)
@@ -144,6 +153,15 @@ class RealtimePipeline(object):
         self._index_input = 0
         self._index_output = 0
         self._popped: List[Item] = []
+
+    # ---- the session's f0 map -----------------------------------------------------------------------------------
+    def set_f0_map(self, **kwargs) -> None:
+        """Engine.session_set_f0_map for this stream (in_mean, in_std, target_mean, target_std, semitones): from the next chunk on."""
+        self.engine.session_set_f0_map(self._sid, **kwargs)
+
+    def measured_f0(self) -> Tuple[int, float, float]:
+        """(voiced frames, mean, standard deviation) of the speaker's ln f0 over the chunks put so far (needs measure_f0)."""
+        return self.engine.session_f0_measured(self._sid)
 
     # ---- queue_input_wave.put -------------------------------------------------------------------------------
     def put(self, item: Item) -> None:
