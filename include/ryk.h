@@ -144,6 +144,9 @@ int ryk_f0_convert(ryk_engine* e, const float* f0, const uint8_t* voiced, int T,
 int ryk_mc2sp(ryk_engine* e, const float* mc, int T, int order, double alpha, int fftlen, double* sp);
 /* sp, out: [T][513] float32 */
 int ryk_stage2_convert(ryk_engine* e, const float* sp, int T, float* out);
+/* ryk_stage2_convert with the envelope warped by a formant ratio in [0.5, 2] (see ryk_session_set_formant); ratio 1 is bitwise
+ * ryk_stage2_convert.  Refused: a non-finite ratio or one outside [0.5, 2]. */
+int ryk_stage2_convert_formant(ryk_engine* e, const float* sp, int T, double ratio, float* out);
 
 /* The whole VoiceChanger.convert_from_acoustic_feature on device: one upload, one download.
  * in : wave [n_wave], f0 [T], ap [T][nb], mc [T][order+1], voiced [T]
@@ -261,7 +264,7 @@ int ryk_session_io_geometry(ryk_engine* e, int session_id, int* n_in, int* max_o
  * exp((ln f0 - in_mean) / in_std * target_std + target_mean) (yukarin's F0Converter).  The map starts as the f0 statistics of the
  * session's voice and belongs to the session from then on: setting it never touches the voice or another session, so several callers
  * converting into one voice can each have the input statistics of their own speaker, and target_mean + s * ln(2) / 12 shifts the pitch
- * by s semitones (the spectral envelope is not moved).
+ * by s semitones (the spectral envelope is not moved: see ryk_session_set_formant).
  * ryk_session_get_f0_map: the values the NEXT submitted step will use (in follow mode: the fallback input side).
  * ryk_session_set_f0_map: takes effect at the next submitted step and for every later one; steps already submitted keep the map they
  *   were submitted with.  Allowed with chunks in flight and for a group member; it does not wait for the device and launches nothing.
@@ -290,6 +293,21 @@ int ryk_session_f0_measure(ryk_engine* e, int session_id, int enable);
 int ryk_session_f0_follow(ryk_engine* e, int session_id, int follow, int min_voiced_frames, double sd_floor);
 int ryk_session_f0_measure_reset(ryk_engine* e, int session_id);
 int ryk_session_f0_measured(ryk_engine* e, int session_id, long long* n_voiced, double* mean, double* std);
+
+/* Formant ratio r of a session's converted spectral envelope, in [0.5, 2]; a session starts at 1 (no warp).
+ * r > 1 moves the envelope up in frequency, sp'(f) = sp(f / r); r = 2^(s/12) moves it by s semitones.  Paired with a pitch shift
+ * (ryk_session_set_f0_map) it changes the apparent size of the speaker rather than only the pitch.
+ * Where (DECIDE F1): on stage 2's output, the envelope the synthesizer reads.  Neither network's input changes.  With the edge-padded
+ *   log row L[j] = y[min(j, 511)] of the network output y, j = 0 .. 512, bin k becomes exp(L at x = k / r), linearly interpolated in
+ *   FP64 and rounded to FP32 (numpy.interp(k / r, arange(513), L)); bins with x >= 512 hold L[512] (r < 1).  r == 1 is the unwarped
+ *   expression, bitwise.
+ * Not warped (DECIDE F2): aperiodicity (it describes the source); the energy of the envelope is not renormalised; a change is not
+ *   smoothed.
+ * ryk_session_set_formant: from the next submitted step on; steps already submitted keep theirs.  Allowed with chunks in flight and on
+ *   a group member; no device wait, no kernel.  Refused, changing nothing: non-finite, outside [0.5, 2], unknown session.
+ * ryk_session_get_formant: the value the NEXT submitted step uses. */
+int ryk_session_set_formant(ryk_engine* e, int session_id, double ratio);
+int ryk_session_get_formant(ryk_engine* e, int session_id, double* ratio);
 
 /* Diagnostics: device timeline (ms) of the last <= 8 steps x 5 stages {gate, analysis, stage 1, stage 2, synthesis}; needs
  * RYK_STAGE_TIMES=1 in the environment at session creation.  start/end hold 40 floats; returns the number of steps. */

@@ -524,10 +524,11 @@ int ryk_mc2sp(ryk_engine* h, const float* mc, int T, int order, double alpha, in
   return 0;
 }
 
-int ryk_stage2_convert(ryk_engine* h, const float* sp, int T, float* out) {
+static int stage2_convert(ryk_engine* h, const float* sp, int T, double formant, float* out) {
   Engine* e = E(h);
   RYK_CUDA(cudaSetDevice(e->device));
   RYK_CHECK(T > 0, "empty input");
+  RYK_CHECK(isfinite(formant) && formant >= 0.5 && formant <= 2.0, "the formant ratio must be finite and within [0.5, 2]");
   const int nb = 513;
   const int Tp = T + (128 - T % 128);
   UNetPlan* plan = nullptr;
@@ -540,10 +541,16 @@ int ryk_stage2_convert(ryk_engine* h, const float* sp, int T, float* out) {
   RYK_CUDA(cudaMemcpyAsync(d_sp, sp, sizeof(float) * T * nb, cudaMemcpyHostToDevice, e->stream));
   if (sr_prologue_run(e, d_sp, T, Tp, nb, (float*)plan->d_in, e->stream)) return -1;
   if (unet_forward(e, plan, e->stream)) return -1;
-  if (sr_epilogue_run(e, (const float*)plan->d_out, T, nb, d_out, e->stream)) return -1;
+  if (sr_epilogue_run(e, (const float*)plan->d_out, T, nb, d_out, e->stream, 0, T, formant)) return -1;
   RYK_CUDA(cudaMemcpyAsync(out, d_out, sizeof(float) * T * nb, cudaMemcpyDeviceToHost, e->stream));
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   return 0;
+}
+
+int ryk_stage2_convert(ryk_engine* h, const float* sp, int T, float* out) { return stage2_convert(h, sp, T, 1.0, out); }
+
+int ryk_stage2_convert_formant(ryk_engine* h, const float* sp, int T, double ratio, float* out) {
+  return stage2_convert(h, sp, T, ratio, out);
 }
 
 int ryk_convert_window(ryk_engine* h, const float* wave, int n_wave, int fs, int frame_length, int hop, double threshold_db,

@@ -198,8 +198,11 @@ __global__ void k_stage1_epilogue(const float* __restrict__ y /*[Tp][C] network 
                                   const float* __restrict__ f0_in, const float* __restrict__ ap_in, const uint8_t* __restrict__ voiced_in,
                                   int nb, F0Map voice_map, const F0Map* __restrict__ session_map, float silent_mc0,
                                   float* __restrict__ mc_out, float* __restrict__ f0_out, float* __restrict__ ap_out,
-                                  uint8_t* __restrict__ voiced_out) {
+                                  uint8_t* __restrict__ voiced_out, double* __restrict__ formant_out) {
   int t = blockIdx.x;
+  // the step's formant ratio goes with its hand-off slot: the stage-2 epilogue of this step reads it there, on another stream, after
+  // the host may already have staged the block of a later step (DESIGN.md §4a)
+  if (formant_out && t == 0 && threadIdx.x == 0) *formant_out = session_map->formant;
   if (t >= T) return;
   const bool eff = mask[t] != 0;
   // rank of t among effective frames = position in index[] (binary search; index is ascending)
@@ -257,12 +260,30 @@ __global__ void k_sr_prologue(const float* __restrict__ sp, const float* __restr
   x[(size_t)t * (nb - 1) + k] = logf(v);
 }
 
-__global__ void k_sr_epilogue(const float* __restrict__ y, int T, int nb, int t0, float* __restrict__ sp_out) {
+// sp_out[t][k] = exp(L[k]) with the edge-padded log row L[j] = y[t][min(j, nb - 2)].  Formant ratio r != 1 (DECIDE F1): sp'(f) = sp(f / r),
+// i.e. bin k reads L at x = k / r, linearly interpolated in FP64 and rounded to FP32 before expf (numpy.interp(k / r, arange(nb), L)),
+// and held at L[nb - 1] from x >= nb - 1 on.  r == 1 keeps the plain expression, so an unwarped envelope is bitwise what it was.
+__global__ void k_sr_epilogue(const float* __restrict__ y, int T, int nb, int t0, double formant, const double* __restrict__ d_formant,
+                              float* __restrict__ sp_out) {
   int t = t0 + blockIdx.y;
   int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= T || k >= nb) return;
-  int ks = k < nb - 1 ? k : nb - 2;
-  sp_out[(size_t)t * nb + k] = expf(y[(size_t)t * (nb - 1) + ks]);
+  const float* row = y + (size_t)t * (nb - 1);
+  const double r = d_formant ? *d_formant : formant;
+  float v;
+  if (r == 1.0) {
+    v = row[k < nb - 1 ? k : nb - 2];
+  } else {
+    const double x = (double)k / r;
+    if (x >= (double)(nb - 1)) {
+      v = row[nb - 2];
+    } else {
+      const int i = (int)x;                        // x >= 0: floor
+      const double w = x - (double)i;
+      v = (float)((1.0 - w) * (double)row[min(i, nb - 2)] + w * (double)row[min(i + 1, nb - 2)]);
+    }
+  }
+  sp_out[(size_t)t * nb + k] = expf(v);
 }
 
 int stage1_prologue_run(const Voice* v, const float* d_mc, const int* d_index, const int* d_count, int C, float* d_x, int Tp_capacity, cudaStream_t st) {
@@ -280,10 +301,13 @@ F0Map voice_f0_map(const Voice* v) {
 
 int stage1_epilogue_run(const Voice* v, const float* d_y, const int* d_index, const uint8_t* d_mask, const int* d_count, int T, int C,
                         const float* d_f0_in, const float* d_ap_in, const uint8_t* d_voiced_in, int nb, float silent_mc0,
-                        float* d_mc_out, float* d_f0_out, float* d_ap_out, uint8_t* d_voiced_out, const F0Map* d_map, cudaStream_t st) {
+                        float* d_mc_out, float* d_f0_out, float* d_ap_out, uint8_t* d_voiced_out, const F0Map* d_map, cudaStream_t st,
+                        double* d_formant_out) {
   if (T <= 0) return 0;
+  RYK_CHECK(d_map || !d_formant_out, "the formant ratio comes from a session's map");
   k_stage1_epilogue<<<T, 128, 0, st>>>(d_y, d_index, d_mask, d_count, T, C, v->d_s1_out_mean, v->d_s1_out_std, d_f0_in, d_ap_in,
-                                       d_voiced_in, nb, voice_f0_map(v), d_map, silent_mc0, d_mc_out, d_f0_out, d_ap_out, d_voiced_out);
+                                       d_voiced_in, nb, voice_f0_map(v), d_map, silent_mc0, d_mc_out, d_f0_out, d_ap_out, d_voiced_out,
+                                       d_formant_out);
   RYK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -362,11 +386,12 @@ int sr_prologue_run(Engine* e, const float* d_sp, int T, int Tp, int nb, float* 
   return 0;
 }
 
-int sr_epilogue_run(Engine* e, const float* d_y, int T, int nb, float* d_sp_out, cudaStream_t st, int t0, int t1) {
+int sr_epilogue_run(Engine* e, const float* d_y, int T, int nb, float* d_sp_out, cudaStream_t st, int t0, int t1, double formant,
+                    const double* d_formant) {
   if (t1 < 0) t1 = T;
   RYK_CHECK(0 <= t0 && t0 <= t1 && t1 <= T, "stage-2 epilogue rows out of range");
   if (t1 == t0) return 0;
-  k_sr_epilogue<<<dim3((nb + 127) / 128, t1 - t0), 128, 0, st>>>(d_y, T, nb, t0, d_sp_out);
+  k_sr_epilogue<<<dim3((nb + 127) / 128, t1 - t0), 128, 0, st>>>(d_y, T, nb, t0, formant, d_formant, d_sp_out);
   RYK_CUDA(cudaGetLastError());
   return 0;
 }

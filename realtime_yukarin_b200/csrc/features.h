@@ -7,31 +7,37 @@ namespace ryk {
 struct Engine;
 struct Voice;
 
-// The f0 map of one session, exp((ln f0 - mu_in) / sd_in * sd_tgt + mu_tgt), as one block of device memory that the stage-1 epilogue
-// reads at run time (DESIGN.md §4a).  The host stages a new block between steps; in follow mode k_f0_measure rewrites mu_in / sd_in.
+// The f0 map of one session, exp((ln f0 - mu_in) / sd_in * sd_tgt + mu_tgt), and its formant ratio, as one block of device memory
+// that the stage-1 epilogue reads at run time (DESIGN.md §4a).  The host stages a new block between steps; in follow mode k_f0_measure
+// rewrites mu_in / sd_in (never formant).
 struct F0Map {
   double mu_in, sd_in, mu_tgt, sd_tgt;
   double sd_floor;                  // follow mode: lower bound of the measured sd_in
   int has_stats;                    // 0: identity map (a voice without f0 statistics and no map set on the session)
   int follow, min_voiced;           // follow mode: input side = the measured statistics once min_voiced voiced frames are counted
   int pad_;
+  double formant;                   // formant ratio of the stage-2 envelope (session_build sets 1; voice_f0_map leaves 0, never read)
 };
 // running statistics of ln f0 over the voiced frames of a session's input: count, mean, sum of squared deviations
 struct F0Stats { long long n; double mean, m2; };
 
 // normalisation with the stage-1 statistics of voice v
 int stage1_prologue_run(const Voice* v, const float* d_mc, const int* d_index, const int* d_count, int C, float* d_x, int Tp_capacity, cudaStream_t st);
-// de-normalisation with the statistics of voice v, and f0 conversion with the map in *d_map (nullptr: the f0 statistics of voice v)
+// de-normalisation with the statistics of voice v, and f0 conversion with the map in *d_map (nullptr: the f0 statistics of voice v);
+// with a map, d_formant_out (non-null) receives d_map->formant, the ratio the stage-2 epilogue of the same step applies
 int stage1_epilogue_run(const Voice* v, const float* d_y, const int* d_index, const uint8_t* d_mask, const int* d_count, int T, int C,
                         const float* d_f0_in, const float* d_ap_in, const uint8_t* d_voiced_in, int nb, float silent_mc0,
-                        float* d_mc_out, float* d_f0_out, float* d_ap_out, uint8_t* d_voiced_out, const F0Map* d_map, cudaStream_t st);
+                        float* d_mc_out, float* d_f0_out, float* d_ap_out, uint8_t* d_voiced_out, const F0Map* d_map, cudaStream_t st,
+                        double* d_formant_out = nullptr);
 F0Map voice_f0_map(const Voice* v);
 // merge the n frames of one chunk into *d_stats; in follow mode (d_map->follow) also write the measured input side into *d_map
 int f0_measure_run(const float* d_f0, const uint8_t* d_voiced, int n, F0Stats* d_stats, F0Map* d_map, cudaStream_t st);
 constexpr int kColminFloats = 64 * 512;      // column-minimum partials of the stage-2 prologue (one scratch per concurrent stream)
 int sr_prologue_run(Engine* e, const float* d_sp, int T, int Tp, int nb, float* d_x, cudaStream_t st, float* d_colmin = nullptr);
-// frames [t0, t1) of the T-frame window (t1 < 0: T); the other rows of d_sp_out are not written
-int sr_epilogue_run(Engine* e, const float* d_y, int T, int nb, float* d_sp_out, cudaStream_t st, int t0 = 0, int t1 = -1);
+// frames [t0, t1) of the T-frame window (t1 < 0: T); the other rows of d_sp_out are not written.  The envelope is warped by the
+// formant ratio *d_formant (non-null: read at run time) or else `formant` (DESIGN.md DECIDE F1); ratio 1 is the plain epilogue, bitwise.
+int sr_epilogue_run(Engine* e, const float* d_y, int T, int nb, float* d_sp_out, cudaStream_t st, int t0 = 0, int t1 = -1,
+                    double formant = 1.0, const double* d_formant = nullptr);
 
 constexpr float kSilentMc0 = -18.420680743952367f;   // ln(1e-8): silent template mel-cepstrum c0 (DESIGN.md, DECIDE)
 

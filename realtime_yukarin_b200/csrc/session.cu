@@ -114,6 +114,7 @@ struct Session {
   // the hand-off set: written by stage 1 (and cv_sp_out by the stage-2 epilogue), read by stage 2 and the decode slide; slot = step % 3
   float *cv_mc_out[kHandoff], *cv_f0_out[kHandoff], *cv_ap_out[kHandoff], *cv_sp_out[kHandoff]; uint8_t* cv_voiced_out[kHandoff];
   float* cv_sp_mid[kHandoff];
+  double* cv_formant[kHandoff];        // the step's formant ratio: written by the stage-1 epilogue, read by the stage-2 epilogue
   double* dec_f0_f64;
   int max_blocks;
   // host-API staging rings (pinned host + device), slot = step % kRing
@@ -143,8 +144,9 @@ struct Session {
   float* d_chunk_model = nullptr;             // the step's resampled chunk (n_wave model-rate samples)
   double* out_hist[2] = {nullptr, nullptr};   // kept synthesizer samples (out.hist)
   double* d_rout_fixed[2] = {nullptr, nullptr}; int* d_rn_fixed[2] = {nullptr, nullptr};   // device-rate output of a step, by parity
-  // The session's f0 map (ryk_session_set_f0_map / _f0_follow) and the statistics of its speaker (ryk_session_f0_measure).  The captured
-  // stage-1 graphs read *d_f0_map; f0_map_sync brings it up to date on stream C in front of a step's stage 1.
+  // The session's f0 map (ryk_session_set_f0_map / _f0_follow), its formant ratio (ryk_session_set_formant) and the statistics of its
+  // speaker (ryk_session_f0_measure).  The captured stage-1 graphs read *d_f0_map; f0_map_sync brings it up to date on stream C in front
+  // of a step's stage 1.  The formant ratio reaches stage 2 through cv_formant[h], never from *d_f0_map (DESIGN.md §4a).
   F0Map f0_map = {};               // what the next submitted step uses (follow mode: its input side is the fallback)
   bool f0_dirty = false;           // f0_map changed since the last submitted step
   bool f0_measure = false;         // the head of stage 1 ends with k_f0_measure
@@ -556,7 +558,8 @@ static int stage1_body(Engine* e, Session* s, int b, int h, int tp1) {
     d_y = (const float*)p1->d_out;
   }
   if (stage1_epilogue_run(s->voice, d_y, s->d_index[b], s->d_mask[b], s->d_count[b], s->Tw, s->C, s->cw_f0[g], s->cw_ap[g], s->cw_voiced[g], s->nb,
-                          kSilentMc0, s->cv_mc_out[h], s->cv_f0_out[h], s->cv_ap_out[h], s->cv_voiced_out[h], s->d_f0_map, s->sC)) return -1;
+                          kSilentMc0, s->cv_mc_out[h], s->cv_f0_out[h], s->cv_ap_out[h], s->cv_voiced_out[h], s->d_f0_map, s->sC,
+                          s->cv_formant[h])) return -1;
   return mc2sp_run(e, s->sptk.d_H, s->cv_mc_out[h], s->Tw, c.order, c.fft_length, 1e-16, s->cv_sp_mid[h], nullptr, s->sC);
 }
 
@@ -700,14 +703,15 @@ static int session_back(Engine* e, Session* s) {
     RYK_CUDA(cudaStreamWaitEvent(sC2, G->ev_fwd[G->step % kRing], 0));
     const float* src = (const float*)G->p2->d_out + (size_t)s->slot * s->Tp * 512;
     if (run_handoff_graph(e, s, k, &HandoffGraphs::s2_epi, sC2, [&](int h) -> int {
-          return sr_epilogue_run(e, src, s->Tw, s->nb, s->cv_sp_out[h], sC2, pc, pc + s->n_feat);
+          return sr_epilogue_run(e, src, s->Tw, s->nb, s->cv_sp_out[h], sC2, pc, pc + s->n_feat, 1.0, s->cv_formant[h]);
         })) return -1;
   } else {
     UNetPlan* p2 = nullptr;
     if (s2_plan(e, s, b, &p2)) return -1;
     if (run_handoff_graph(e, s, k, &HandoffGraphs::s2_epi, sC2, [&](int h) -> int {
           if (unet_forward(e, p2, sC2, 15, 15)) return -1;
-          return sr_epilogue_run(e, (const float*)p2->d_out, s->Tw, s->nb, s->cv_sp_out[h], sC2, pc, pc + s->n_feat);
+          return sr_epilogue_run(e, (const float*)p2->d_out, s->Tw, s->nb, s->cv_sp_out[h], sC2, pc, pc + s->n_feat, 1.0,
+                                 s->cv_formant[h]);
         })) return -1;
   }
   if (stage_time(s, 3, 1, r, sC2)) return -1;
@@ -928,16 +932,19 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
     if (A((void**)&s->cv_sp_out[i], sizeof(float) * (size_t)s->Tw * s->nb)) return -1;
     if (A((void**)&s->cv_voiced_out[i], (size_t)s->Tw)) return -1;
     if (A((void**)&s->cv_sp_mid[i], sizeof(float) * (size_t)s->Tw * s->nb)) return -1;
+    if (A((void**)&s->cv_formant[i], sizeof(double))) return -1;
   }
   if (A((void**)&s->d_mse, sizeof(double) * s->Tw)) return -1;
   for (int i = 0; i < 2; ++i) if (A((void**)&s->d_colmin[i], sizeof(float) * kColminFloats)) return -1;
   if (A((void**)&s->dec_f0_f64, sizeof(double) * s->Td)) return -1;
   if (A((void**)&s->d_chunk_fixed, sizeof(float) * s->n_wave)) return -1;
-  // the session starts on its voice's f0 map
+  // the session starts on its voice's f0 map and an unwarped envelope
   if (A((void**)&s->d_f0_map, sizeof(F0Map))) return -1;
   if (A((void**)&s->d_f0_stats, sizeof(F0Stats))) return -1;
   if (P((void**)&s->h_f0_map, sizeof(F0Map) * kRing)) return -1;
-  s->f0_map = s->h_f0_map[0] = voice_f0_map(s->voice);
+  s->f0_map = voice_f0_map(s->voice);
+  s->f0_map.formant = 1.0;
+  s->h_f0_map[0] = s->f0_map;
   RYK_CUDA(cudaMemcpyAsync(s->d_f0_map, s->h_f0_map, sizeof(F0Map), cudaMemcpyHostToDevice, e->stream));
   s->max_blocks = (s->Td * s->hop) / cfg->vocoder_buffer_size + 4;
   s->max_out = s->max_blocks * cfg->vocoder_buffer_size;
@@ -1215,6 +1222,25 @@ int ryk_session_f0_measured(ryk_engine* h, int id, long long* n_voiced, double* 
   if (n_voiced) *n_voiced = st.n;
   if (mean) *mean = st.mean;
   if (std_) *std_ = st.n >= 2 ? sqrt(st.m2 / (double)st.n) : 0.0;
+  return 0;
+}
+
+// The formant ratio travels in the f0 map block to stage 1 of the next submitted step, whose epilogue copies it into the step's hand-off
+// slot for the stage-2 epilogue.
+int ryk_session_set_formant(ryk_engine* h, int id, double ratio) {
+  Session* s = get_session(&h->impl, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  RYK_CHECK(isfinite(ratio) && ratio >= 0.5 && ratio <= 2.0, "the formant ratio must be finite and within [0.5, 2]");
+  s->f0_map.formant = ratio;
+  s->f0_dirty = true;
+  return 0;
+}
+
+int ryk_session_get_formant(ryk_engine* h, int id, double* ratio) {
+  Session* s = get_session(&h->impl, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  RYK_CHECK(ratio != nullptr, "null argument");
+  *ratio = s->f0_map.formant;
   return 0;
 }
 

@@ -65,11 +65,12 @@ EXPORTED_SYMBOLS = [
     'ryk_voice_create', 'ryk_voice_destroy', 'ryk_voice_model_create', 'ryk_voice_model_set_layer', 'ryk_voice_stage1_set_stats',
     'ryk_voice_f0_set_stats', 'ryk_session_create_voice', 'ryk_session_voice', 'ryk_group_add', 'ryk_group_remove', 'ryk_group_members',
     'ryk_session_get_f0_map', 'ryk_session_set_f0_map', 'ryk_session_f0_measure', 'ryk_session_f0_follow', 'ryk_session_f0_measure_reset',
-    'ryk_session_f0_measured',
+    'ryk_session_f0_measured', 'ryk_session_set_formant', 'ryk_session_get_formant', 'ryk_stage2_convert_formant',
 ]
 
 SEMITONE = math.log(2.0) / 12.0          # one semitone in ln f0
 F0_SD_FLOOR = 0.05                       # follow mode: least in_std (ln f0), about 0.9 semitones
+FORMANT_RANGE = (0.5, 2.0)               # formant ratios a session or ryk_stage2_convert_formant accepts: +-12 semitones
 
 
 class F0Map(ctypes.Structure):
@@ -87,6 +88,14 @@ def updated_f0_map(current: Dict[str, float], in_mean=None, in_std=None, target_
             new[key] = float(value)
     new['target_mean'] += float(semitones) * SEMITONE
     return new
+
+
+def formant_ratio(ratio=None, semitones=None) -> float:
+    """The formant ratio given as a ratio or in semitones (2 ** (semitones / 12)); exactly one of the two.  The range is checked by
+    the library."""
+    if (ratio is None) == (semitones is None):
+        raise ValueError('give exactly one of ratio and semitones')
+    return float(ratio) if ratio is not None else 2.0 ** (float(semitones) / 12.0)
 
 
 def stage2_row_bands(Tp: int, W: int, keep_begin: int, keep_len: int) -> numpy.ndarray:
@@ -337,10 +346,14 @@ class Engine(object):
             self._check(self.lib.ryk_mc2sp(self._h, _fp(mc), mc.shape[0], mc.shape[1] - 1, ctypes.c_double(alpha), int(fftlen), _dp(sp)))
         return sp
 
-    def stage2_convert(self, sp) -> numpy.ndarray:
+    def stage2_convert(self, sp, formant_ratio: float = 1.0) -> numpy.ndarray:
+        """Stage 2 on (T, 513) float32; `formant_ratio` != 1 warps the converted envelope (Engine.session_set_formant)."""
         sp = _f32(sp)
         out = numpy.empty_like(sp)
-        self._check(self.lib.ryk_stage2_convert(self._h, _fp(sp), sp.shape[0], _fp(out)))
+        if formant_ratio == 1.0:
+            self._check(self.lib.ryk_stage2_convert(self._h, _fp(sp), sp.shape[0], _fp(out)))
+        else:
+            self._check(self.lib.ryk_stage2_convert_formant(self._h, _fp(sp), sp.shape[0], ctypes.c_double(formant_ratio), _fp(out)))
         return out
 
     def convert_window(self, wave, fs, frame_length, hop, threshold_db, f0, ap, mc, voiced, order, alpha, fftlen):
@@ -576,7 +589,7 @@ class Engine(object):
     def session_set_f0_map(self, sid: int, in_mean=None, in_std=None, target_mean=None, target_std=None, semitones: float = 0.0):
         """Change this session's f0 map from its next submitted step on (chunks in flight keep theirs; other sessions of the voice are
         not affected).  None keeps the current value.  `semitones` adds semitones * ln(2) / 12 to the target mean (the one given, else
-        the current one): that is the whole pitch control -- f0 moves, the spectral envelope (the formants) does not."""
+        the current one): f0 moves, the spectral envelope does not; session_set_formant moves the formants."""
         new = updated_f0_map(self.session_get_f0_map(sid), in_mean, in_std, target_mean, target_std, semitones)
         m = F0Map(*[new[k] for k in F0Map.KEYS])
         self._check(self.lib.ryk_session_set_f0_map(self._h, sid, ctypes.byref(m)))
@@ -600,6 +613,19 @@ class Engine(object):
         n, mean, std = ctypes.c_longlong(), ctypes.c_double(), ctypes.c_double()
         self._check(self.lib.ryk_session_f0_measured(self._h, sid, ctypes.byref(n), ctypes.byref(mean), ctypes.byref(std)))
         return n.value, mean.value, std.value
+
+    # ---- the session's formant ratio ----
+    def session_set_formant(self, sid: int, ratio: Optional[float] = None, semitones: Optional[float] = None):
+        """Warp this session's converted spectral envelope from its next submitted step on (chunks in flight keep theirs):
+        sp'(f) = sp(f / ratio), ratio in [0.5, 2], or ratio = 2 ** (semitones / 12) with semitones in [-12, 12].  Exactly one of the two.
+        Paired with session_set_f0_map(semitones=) it moves the formants along with the pitch; aperiodicity is not warped."""
+        self._check(self.lib.ryk_session_set_formant(self._h, sid, ctypes.c_double(formant_ratio(ratio, semitones))))
+
+    def session_get_formant(self, sid: int) -> float:
+        """The formant ratio the next submitted step of the session uses."""
+        r = ctypes.c_double()
+        self._check(self.lib.ryk_session_get_formant(self._h, sid, ctypes.byref(r)))
+        return r.value
 
     def session_destroy(self, sid: int):
         self._check(self.lib.ryk_session_destroy(self._h, sid))

@@ -221,5 +221,6 @@ class SuperResolution(object):
         self.engine = engine or default_engine()
         upload_unet(self.engine, 2, load_npz(model_path))
 
-    def convert(self, input: numpy.ndarray) -> numpy.ndarray:
-        return self.engine.stage2_convert(numpy.asarray(input, dtype=numpy.float32))
+    def convert(self, input: numpy.ndarray, formant_ratio: float = 1.0) -> numpy.ndarray:
+        x = numpy.asarray(input, dtype=numpy.float32)
+        return self.engine.stage2_convert(x) if formant_ratio == 1.0 else self.engine.stage2_convert(x, formant_ratio=formant_ratio)

@@ -62,10 +62,10 @@ def save_measured_statistics(pipeline: RealtimePipeline, path: Path) -> bool:
 
 def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path] = None, max_chunks: Optional[int] = None,
         engine=None, depth: int = 3, measure_input_statistics: Optional[Path] = None, follow_input_f0: Optional[int] = None,
-        pitch: float = 0.0) -> int:
+        pitch: float = 0.0, formant: float = 0.0) -> int:
     """`measure_input_statistics`: measure the speaker's log-f0 statistics during the run and write them to this file at the end;
     `follow_input_f0`: convert with the measured statistics once this many voiced frames are counted; `pitch`: semitones added to
-    the target voice's mean f0."""
+    the target voice's mean f0; `formant`: semitones by which the converted spectral envelope moves."""
     logger = logging.getLogger('root')
     logger.info('model loading...')
     config = Config.from_yaml(config_path)
@@ -74,7 +74,7 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
         stage1_model_path=config.stage1_model_path, stage1_config_path=config.stage1_config_path,
         stage2_model_path=config.stage2_model_path, stage2_config_path=config.stage2_config_path)
     pipeline = RealtimePipeline(config, acoustic_param=converter.acoustic_converter.config.dataset.acoustic_param, engine=engine, depth=depth,
-                                measure_f0=measure_input_statistics is not None, follow_f0=follow_input_f0)
+                                measure_f0=measure_input_statistics is not None, follow_f0=follow_input_f0, formant=formant)
     try:
         if pitch:
             pipeline.set_f0_map(semitones=pitch)
@@ -130,14 +130,18 @@ def make_parser() -> argparse.ArgumentParser:
                         help='convert f0 with the statistics measured on the input so far instead of input_statistics_path, once '
                              'MIN_FRAMES voiced 5 ms frames are counted (default 200)')
     parser.add_argument('--pitch', type=float, default=0.0, metavar='SEMITONES',
-                        help='shift the converted f0 by this many semitones (the spectral envelope is not moved)')
+                        help='shift the converted f0 by this many semitones (the spectral envelope is not moved: see --formant)')
+    parser.add_argument('--formant', type=float, default=0.0, metavar='SEMITONES',
+                        help='move the converted spectral envelope (the formants) by this many semitones, -12 to 12; with --pitch '
+                             'by the same amount the voice sounds like a different speaker rather than the same one at another pitch')
     return parser
 
 
 def main(argv: Optional[Iterable[str]] = None) -> None:
     args = make_parser().parse_args(argv)
     run(config_path=args.config_path, wav_in=args.wav_in, wav_out=args.wav_out, max_chunks=args.max_chunks,
-        measure_input_statistics=args.measure_input_statistics, follow_input_f0=args.follow_input_f0, pitch=args.pitch)
+        measure_input_statistics=args.measure_input_statistics, follow_input_f0=args.follow_input_f0, pitch=args.pitch,
+        formant=args.formant)
 
 
 if __name__ == '__main__':

@@ -86,10 +86,11 @@ class RealtimePipeline(object):
 
     `measure_f0=True` keeps running statistics of the speaker's log-f0 on the device (`measured_f0`); `follow_f0=N` (implies
     measuring) also makes them the input side of the session's f0 map once N voiced frames are counted.  `set_f0_map` changes the
-    map between chunks."""
+    map between chunks.  `formant` (semitones, [-12, 12]) warps the converted spectral envelope from the first chunk on; `set_formant`
+    changes it between chunks."""
 
     def __init__(self, config: Config, acoustic_param=None, engine: Optional[Engine] = None, depth: int = 3, voice: int = 0,
-                 measure_f0: bool = False, follow_f0: Optional[int] = None):
+                 measure_f0: bool = False, follow_f0: Optional[int] = None, formant: float = 0.0):
         self.config = config
         self.engine = engine or default_engine()
         p = acoustic_param
@@ -145,6 +146,8 @@ class RealtimePipeline(object):
             self.engine.session_f0_measure(self._sid)
         if follow_f0 is not None:
             self.engine.session_f0_follow(self._sid, True, min_voiced_frames=int(follow_f0))
+        if formant:
+            self.engine.session_set_formant(self._sid, semitones=float(formant))
         self._scratch = numpy.empty(n_out_cap, dtype=numpy.float64)
         self._rid = self.engine.reblock_create(config.out_audio_chunk, n_out_cap, float(config.output_silent_threshold))
         self._inflight: Deque[Tuple[Item, int, int, float]] = deque()      # (item, session ticket, re-blocker ticket, host time of put)
@@ -158,6 +161,10 @@ class RealtimePipeline(object):
     def set_f0_map(self, **kwargs) -> None:
         """Engine.session_set_f0_map for this stream (in_mean, in_std, target_mean, target_std, semitones): from the next chunk on."""
         self.engine.session_set_f0_map(self._sid, **kwargs)
+
+    def set_formant(self, **kwargs) -> None:
+        """Engine.session_set_formant for this stream (ratio or semitones): from the next chunk on."""
+        self.engine.session_set_formant(self._sid, **kwargs)
 
     def measured_f0(self) -> Tuple[int, float, float]:
         """(voiced frames, mean, standard deviation) of the speaker's ln f0 over the chunks put so far (needs measure_f0)."""
