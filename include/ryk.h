@@ -110,7 +110,11 @@ int ryk_crepe_predict(ryk_engine* e, const float* audio16k, int n, double step_m
                       float* activation, int* path);
 
 /* ---- silence gate --------------------------------------------------------------------------- */
-/* mask[n_frames] (0/1); threshold_db < 0 disables the gate (all frames effective). */
+/* mask[n_frames] (0/1): a frame is effective when it lies within threshold_db of the loudest frame of the window
+ * (dB - max dB > -threshold_db).  The same rule holds wherever a threshold_db is passed (ryk_convert_window, ryk_session_config):
+ *   threshold_db > 0   the gate of the reference (60 by default);
+ *   threshold_db == 0  every frame is gated, the loudest included: stage 1 is skipped and the window is the silent template;
+ *   threshold_db < 0   no gate, whatever the value: every frame is effective. */
 int ryk_silence_mask(ryk_engine* e, const float* wave_host, int n, int frame_length, int hop,
                      double threshold_db, int n_frames, uint8_t* mask);
 
@@ -218,7 +222,7 @@ typedef struct {
   double alpha;                 /* 0.466 */
   double buffer_time;           /* seconds of audio per pushed chunk (0.3) */
   double encode_extra_time, convert_extra_time, decode_extra_time;   /* 0, 0.5, 0 */
-  double threshold_db;          /* silence gate, < 0 disables */
+  double threshold_db;          /* silence gate (see ryk_silence_mask): 0 gates every frame, < 0 disables the gate */
   int vocoder_buffer_size;      /* 1024 */
 } ryk_session_config;
 

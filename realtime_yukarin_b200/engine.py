@@ -264,6 +264,8 @@ class Engine(object):
 
     # ---- silence gate ----
     def silence_mask(self, wave, frame_length, hop, threshold_db, n_frames) -> numpy.ndarray:
+        """Effective frames: within `threshold_db` of the window's loudest frame.  None or any negative value: no gate (all True);
+        0: every frame gated (all False).  convert_window and SessionConfig.threshold_db follow the same rule."""
         w = _f32(wave)
         mask = numpy.zeros(n_frames, dtype=numpy.uint8)
         thr = -1.0 if threshold_db is None else float(threshold_db)
