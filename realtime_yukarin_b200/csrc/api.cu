@@ -197,7 +197,7 @@ int ryk_engine_create(int device, ryk_engine** out) {
   if (analysis_kernels_init()) return -1;
   if (tc_init()) return -1;
   if (s1_fused_init()) return -1;
-  RYK_CUDA(cudaMalloc(&e->d_colmin, sizeof(float) * 64 * 512));   // stage-2 prologue scratch (never allocated inside a graph capture)
+  RYK_CUDA(cudaMalloc(&e->d_colmin, sizeof(float) * kColminFloats));   // per-op stage-2 prologue scratch (never allocated inside a graph capture)
   RYK_CUDA(cudaMalloc(&e->d_launches, sizeof(*e->d_launches)));
   RYK_CUDA(cudaMemset(e->d_launches, 0, sizeof(*e->d_launches)));
   *out = h;
@@ -209,11 +209,12 @@ int ryk_engine_destroy(ryk_engine* h) {
   Engine* e = E(h);
   cudaSetDevice(e->device);
   cudaStreamSynchronize(e->stream);
+  reblock_destroy_all(e);                           // before the sessions: a re-blocker's pushes may ride a session's decode stream
+  session_destroy_all(e);                           // before the voices: a session releases its plans on the voice's U-Nets
+  crepe_destroy();                                  // after the sessions: their CREPE plans are counted on the model
   for (auto& kv : e->dio_plans) dio_plan_free(kv.second);
   for (Voice* v : e->voices) voice_free(v);
   for (Synth* s : e->synths) synth_destroy(s);
-  session_destroy_all(e);
-  crepe_destroy();                                  // after the sessions: their CREPE plans are counted on the model
   for (auto& kv : e->sptk) { cudaFree(kv.second.d_G); cudaFree(kv.second.d_H); }
   void* ptrs[] = {e->d_colmin, e->d_launches, e->d_twiddle, e->d_jump, e->d_scratch};
   for (void* p : ptrs) if (p) cudaFree(p);

@@ -1,5 +1,7 @@
 // engine.h -- internal state of one libryk engine (one per process / GPU).
 #pragma once
+#include <string.h>
+#include <algorithm>
 #include <map>
 #include <memory>
 #include <string>
@@ -36,6 +38,33 @@ struct Voice {
 struct SptkMats {
   double* d_G = nullptr;             // sp2mc: (order+1) x nb
   double* d_H = nullptr;             // mc2sp: nb x (order+1)
+};
+
+// The device and pinned host buffers of one session or re-blocker, freed with their owner.  Every buffer starts zeroed: device memory
+// by a cudaMemsetAsync on `stream` (the engine stream: work queued there later, such as a session's template fill, runs after the
+// zeros, and the owner synchronises it before other streams use the buffers), pinned memory by memset.  Allocating into a pointer
+// that holds one of the owner's buffers replaces that buffer.
+struct BufferSet {
+  cudaStream_t stream = nullptr;
+  BufferSet() = default;
+  BufferSet(const BufferSet&) = delete;
+  ~BufferSet() { for (void* p : dev_) cudaFree(p); for (void* p : host_) cudaFreeHost(p); }
+  template <typename T> int device(T** p, size_t n) { return get((void**)p, sizeof(T) * n, false); }
+  template <typename T> int pinned(T** p, size_t n) { return get((void**)p, sizeof(T) * n, true); }
+
+ private:
+  std::vector<void*> dev_, host_;
+  int get(void** p, size_t bytes, bool host) {
+    std::vector<void*>& owned = host ? host_ : dev_;
+    const auto it = std::find(owned.begin(), owned.end(), *p);
+    if (*p && it != owned.end()) { if (host) cudaFreeHost(*p); else cudaFree(*p); owned.erase(it); }
+    *p = nullptr;
+    if (!bytes) bytes = 16;
+    if (host) RYK_CUDA(cudaMallocHost(p, bytes)); else RYK_CUDA(cudaMalloc(p, bytes));
+    owned.push_back(*p);
+    if (host) memset(*p, 0, bytes); else RYK_CUDA(cudaMemsetAsync(*p, 0, bytes, stream));
+    return 0;
+  }
 };
 
 struct Engine {

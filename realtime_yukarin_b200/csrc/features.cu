@@ -376,10 +376,7 @@ int f0_measure_run(const float* d_f0, const uint8_t* d_voiced, int n, F0Stats* d
 int sr_prologue_run(Engine* e, const float* d_sp, int T, int Tp, int nb, float* d_x, cudaStream_t st, float* d_colmin) {
   const int rows_per_block = 32, nparts = (T + rows_per_block - 1) / rows_per_block;
   RYK_CHECK((size_t)nparts * (nb - 1) * sizeof(float) <= sizeof(float) * kColminFloats, "window too long for the column-minimum scratch");
-  if (!d_colmin) {                  // per-op API: the engine's scratch (calls are serialised on the engine stream)
-    if (!e->d_colmin) RYK_CUDA(cudaMalloc(&e->d_colmin, sizeof(float) * kColminFloats));
-    d_colmin = e->d_colmin;
-  }
+  if (!d_colmin) d_colmin = e->d_colmin;     // per-op API: the engine's scratch (calls are serialised on the engine stream)
   k_sr_colmin<<<dim3((nb - 1 + 127) / 128, nparts), 128, 0, st>>>(d_sp, T, nb, rows_per_block, d_colmin);
   k_sr_prologue<<<dim3((nb - 1 + 127) / 128, Tp), 128, 0, st>>>(d_sp, d_colmin, nparts, T, Tp, nb, d_x);
   RYK_CUDA(cudaGetLastError());

@@ -75,6 +75,10 @@ int resample_stream_out_run(Engine* e, const double* d_hist, double* d_hist_next
                             int max_out, int* d_n_out, cudaStream_t st);
 
 void session_destroy_all(Engine* e);
+// what the re-blocker (reblock.cu) reads of session `id`: the samples and sample count of its last step in device memory, the most
+// samples a step returns, and the decode stream that orders work on them
+int session_last_output(Engine* e, int id, const double** out, const int** n_out, int* max_out, cudaStream_t* sD);
+void reblock_destroy_all(Engine* e);
 int session_streams_fork(Engine* e, cudaEvent_t ev);
 int session_streams_join(Engine* e);
 
