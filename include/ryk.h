@@ -227,10 +227,24 @@ typedef struct {
 } ryk_session_config;
 
 int ryk_session_create(ryk_engine* e, const ryk_session_config* cfg, int* session_id);
-/* A session that converts into voice_id for its whole lifetime (ryk_session_create: voice 0).  A voice >= 1 needs both models with
- * every layer loaded; without stage-1 statistics it uses identity statistics. */
+/* A session that converts into voice_id until ryk_session_set_voice switches it (ryk_session_create: voice 0).  A voice >= 1 needs
+ * both models with every layer loaded; without stage-1 statistics it uses identity statistics. */
 int ryk_session_create_voice(ryk_engine* e, const ryk_session_config* cfg, int voice_id, int* session_id);
 int ryk_session_voice(ryk_engine* e, int session_id);        /* the voice a session converts into, or -1 */
+/* Converts the session into voice_id from its next submitted step on.  Windows, synthesizer, resamplers, step count, speaker
+ * statistics, follow mode, formant ratio, attached re-blockers and group membership carry over.  A hard cut at the step boundary (no
+ * crossfade): every later step converts its whole window with the new voice, so only the synthesizer's history differs from a session
+ * created on that voice.
+ * f0 map: both sides become the new voice's f0 statistics (identity without them), as a session created on it starts; a caller's own
+ *   input side or pitch offset is set again with ryk_session_set_f0_map after the switch (it lands on the same next step).
+ * Needs every host-API chunk of the session collected, and of its group for a member (device-resident steps count as collected).  The
+ * call waits for the device, builds the new voice's stage-1 graphs and stage-2 plans (a member: the group's new batched plan, its slot
+ * unchanged) and launches no kernel; the steps after it allocate nothing, and only the first two capture graphs, as on a new session.
+ * The old voice is unlocked, the new one locked.  Switching to the current voice does nothing and does not wait.
+ * Refused, changing nothing: an unknown session or voice, a voice without both models fully loaded or whose stage-1 channels differ from
+ * order + 1, an uncollected chunk, a group rule the member's new voice would break, follow mode on with a voice without f0 statistics,
+ * an engine precision or stage-1 mode changed since the session was created. */
+int ryk_session_set_voice(ryk_engine* e, int session_id, int voice_id);
 int ryk_session_destroy(ryk_engine* e, int session_id);
 /* One chunk through encode -> convert -> decode with host buffers (H2D + kernels + D2H inside).
  * wave: round(fs * buffer_time) float32 samples; out: up to out_capacity float64 samples; *n_out is a

@@ -124,7 +124,8 @@ struct Group;
 struct Session {
   int s1_owner = 0;                // plan-cache owner id of the stage-1 plans (activation buffers are private to the session)
   Group* group = nullptr; int slot = 0;        // member of a batched stage-2 group (config 5), else nullptr
-  Voice* voice = nullptr; int voice_id = 0;    // the voice the session converts into (fixed for its lifetime)
+  Voice* voice = nullptr; int voice_id = 0;    // the voice the session converts into (ryk_session_set_voice changes it between steps)
+  int precision = 1; bool s1_fused = true;     // the engine's precision and stage-1 mode at creation: every plan and graph keeps them
   ryk_session_config cfg;
   SptkMats sptk;                   // the engine's sp2mc / mc2sp matrices of cfg's (order, alpha, fft_length), captured in the graphs
   int hop, rate, n_wave, n_feat, e_wave, e_enc_frames, e_conv, e_dec;
@@ -421,11 +422,11 @@ __global__ void k_set_bucket(cudaGraphConditionalHandle handle, const int* __res
   }
 }
 
-static int stage1_body(Engine* e, Session* s, int b, int h, int tp1);
+static int stage1_body(Engine* e, Session* s, Voice* v, int owner, int b, int h, int tp1);
 
-// Build the stage-1 graph of the chunks of step % 6 = j with a device-side switch over the padded-length buckets (CUDA conditional
-// nodes, 12.8+).
-static int stage1_build_switch(Engine* e, Session* s, int j) {
+// Build into g the stage-1 graph of the chunks of step % 6 = j with a device-side switch over the padded-length buckets (CUDA
+// conditional nodes, 12.8+), on the stage-1 plans of voice v under plan owner `owner`.
+static int stage1_build_switch(Engine* e, Session* s, Voice* v, int owner, int j, StageGraph& g) {
   const int b = j & 1, h = j % kHandoff;
   const int n_buckets = s->Tp / 128 + 1;
   RYK_CHECK(n_buckets <= 16, "window too long for the stage-1 graph table");
@@ -453,7 +454,7 @@ static int stage1_build_switch(Engine* e, Session* s, int j) {
   for (int i = 0; i < n_buckets; ++i) {
     cudaGraph_t body = cp.conditional.phGraph_out[i];
     RYK_CUDA(cudaStreamBeginCaptureToGraph(s->sC, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-    int rc = stage1_body(e, s, b, h, i * 128);
+    int rc = stage1_body(e, s, v, owner, b, h, i * 128);
     cudaGraph_t out = nullptr;
     cudaError_t err = cudaStreamEndCapture(s->sC, &out);
     if (rc) return rc;
@@ -462,8 +463,8 @@ static int stage1_build_switch(Engine* e, Session* s, int j) {
     if (kernels.n[i] < 0) return -1;
   }
   RYK_CUDA(cudaGraphKernelNodeSetParams(set_node, &kp));
-  if (stage_graph_init(s->hgraphs[j].s1, graph)) return -1;
-  RYK_CUDA(cudaGraphUpload(s->hgraphs[j].s1.exec, s->sC));     // the first step of each copy does not pay for the upload
+  if (stage_graph_init(g, graph)) return -1;
+  RYK_CUDA(cudaGraphUpload(g.exec, s->sC));     // the first step of each copy does not pay for the upload
   return 0;
 }
 
@@ -510,19 +511,19 @@ static int f0_map_sync(Session* s, long long k) {
 // voice_changer.py:32-35 skips the net) -> scatter into the silent template + f0 map, mc2sp.  Enqueued on stream C while it is captured
 // as one body of the chunk's SWITCH graph; every body is captured when the session is created so that no chunk ever pays for a capture
 // in the middle of a stream.
-static int stage1_body(Engine* e, Session* s, int b, int h, int tp1) {
+static int stage1_body(Engine* e, Session* s, Voice* v, int owner, int b, int h, int tp1) {
   const ParitySet &p = s->par[b], &q = s->par[b ^ 1];
   const HandoffSlot& o = s->ho[h];
   const ryk_session_config& c = s->cfg;
   const float* d_y = nullptr;
   if (tp1 > 0) {
     UNetPlan* p1 = nullptr;
-    if (unet_get_plan(e, s->voice->stage1, 1, 1, tp1, e->precision, &p1, s->s1_owner)) return -1;
-    if (stage1_prologue_run(s->voice, q.cw_mc, p.d_index, p.d_count, s->C, (float*)p1->d_in, tp1, s->sC)) return -1;
+    if (unet_get_plan(e, v->stage1, 1, 1, tp1, e->precision, &p1, owner)) return -1;
+    if (stage1_prologue_run(v, q.cw_mc, p.d_index, p.d_count, s->C, (float*)p1->d_in, tp1, s->sC)) return -1;
     if (unet_forward(e, p1, s->sC)) return -1;
     d_y = (const float*)p1->d_out;
   }
-  if (stage1_epilogue_run(s->voice, d_y, p.d_index, p.d_mask, p.d_count, s->Tw, s->C, q.cw_f0, q.cw_ap, q.cw_voiced, s->nb, kSilentMc0,
+  if (stage1_epilogue_run(v, d_y, p.d_index, p.d_mask, p.d_count, s->Tw, s->C, q.cw_f0, q.cw_ap, q.cw_voiced, s->nb, kSilentMc0,
                           o.mc_out, o.f0_out, o.ap_out, o.voiced_out, s->d_f0_map, s->sC, o.formant)) return -1;
   return mc2sp_run(e, s->sptk.d_H, o.mc_out, s->Tw, c.order, c.fft_length, 1e-16, o.sp_mid, nullptr, s->sC);
 }
@@ -539,9 +540,10 @@ static Stage2Lane& s2_lane(Session* s, int b) { return s->lane[s->group ? 0 : b]
 // The decode slide reads only the chunk's frames [e_conv, e_conv + n_feat) of the converted window, so stage 2 computes only the
 // decoder rows those frames depend on; the prologue pads rows [Tw, Tp) with one row, so the encoder computes one copy of the rows
 // that depend only on it.
-static int s2_plan(Engine* e, const Session* s, const Stage2Lane& L, UNetPlan** p2) {
-  return unet_get_plan(e, s->voice->stage2, 1, s->Tp, 512, e->precision, p2, L.owner, s->e_conv, s->n_feat, false, s->Tw);
+static int s2_plan(Engine* e, const Session* s, Voice* v, int owner, UNetPlan** p2) {
+  return unet_get_plan(e, v->stage2, 1, s->Tp, 512, e->precision, p2, owner, s->e_conv, s->n_feat, false, s->Tw);
 }
+static int s2_plan(Engine* e, const Session* s, const Stage2Lane& L, UNetPlan** p2) { return s2_plan(e, s, s->voice, L.owner, p2); }
 
 // begin (which = 0) / end (1) of a stage in the RYK_STAGE_TIMES timeline
 static int stage_time(Session* s, int stage, int which, int r, cudaStream_t st) {
@@ -924,7 +926,8 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
   // (the stage-2 plans are created on first use: a session that joins a group never needs its own)
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   RYK_CUDA(cudaDeviceSynchronize());
-  for (int j = 0; j < kHandoffGraphs; ++j) if (stage1_build_switch(e, s, j)) return -1;
+  s->precision = e->precision; s->s1_fused = e->s1_fused;
+  for (int j = 0; j < kHandoffGraphs; ++j) if (stage1_build_switch(e, s, s->voice, s->s1_owner, j, s->hgraphs[j].s1)) return -1;
   return 0;
 }
 
@@ -1316,6 +1319,78 @@ int ryk_group_remove(ryk_engine* h, int group_id, int session_id) {
   s->group = nullptr; s->slot = 0;
   for (Stage2Lane& L : s->lane) L.s2_layers.reset();
   for (HandoffGraphs& hg : s->hgraphs) { hg.s2_pro.reset(); hg.s2_epi.reset(); }
+  return 0;
+}
+
+// ---- voice switch (DESIGN.md §4a): the session converts into another voice from its next submitted step on ----
+// What depends on the voice is rebuilt: the stage-1 plans and the six stage-1 SWITCH graphs that hold the voice's statistics, and the
+// stage-2 plans (the lanes' own, or the group's batched plan through group_rebuild).  Everything that holds stream state carries over.
+// Built first under fresh owner ids, then swapped in: a failure releases what was built and leaves the session on its old voice.  The
+// call waits for the device, so no step of the old plans is in flight when they are released and no event guard is needed.
+int ryk_session_set_voice(ryk_engine* h, int id, int voice_id) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Session* s = get_session(e, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  Voice* v = engine_voice(e, voice_id);
+  RYK_CHECK(v != nullptr, "no such voice");
+  if (v == s->voice) return 0;
+  RYK_CHECK(voice_models_loaded(v), "load every layer of both of the voice's models before switching a session to it");
+  RYK_CHECK(v->stage1->in_ch == s->C, "the voice's stage-1 model does not take the session's mel-cepstrum order");
+  RYK_CHECK(session_idle(s) && (!s->group || s->group->collected == s->group->step),
+            "collect every submitted chunk of the session and of its group before switching its voice");
+  RYK_CHECK(e->precision == s->precision && e->s1_fused == s->s1_fused,
+            "the engine's precision or stage-1 mode changed since the session was created: a session keeps the numerics it was created with");
+  RYK_CHECK(!s->f0_map.follow || v->has_f0_stats, "follow mode needs an f0 map: the voice has no f0 statistics (turn follow mode off first)");
+  Group* G = s->group;
+  Voice* const old = s->voice;
+  if (G) {
+    s->voice = v;                                  // the member list as the switch would leave it
+    const char* refusal = group_refusal(e, G->members);
+    s->voice = old;
+    if (refusal) { set_error(refusal); return -1; }
+  }
+  if (voice_id >= 1 && voice_default_stage1_stats(v, s->C)) return -1;
+  RYK_CUDA(cudaDeviceSynchronize());
+  const int s1_owner = ++e->plan_owners;
+  int lane_owner[2];
+  for (int& o : lane_owner) o = ++e->plan_owners;
+  StageGraph s1[kHandoffGraphs];
+  auto build = [&]() -> int {
+    UNetPlan* p = nullptr;
+    for (int Tp = 128; Tp <= s->Tp; Tp += 128) if (unet_get_plan(e, v->stage1, 1, 1, Tp, e->precision, &p, s1_owner)) return -1;
+    if (!G) for (int o : lane_owner) if (s2_plan(e, s, v, o, &p)) return -1;     // a member runs the group's plan
+    for (int j = 0; j < kHandoffGraphs; ++j) if (stage1_build_switch(e, s, v, s1_owner, j, s1[j])) return -1;
+    if (G) {
+      s->voice = v;
+      const int rc = group_rebuild(e, G, G->members);     // commits the group's new plan only on success
+      s->voice = old;
+      if (rc) return rc;
+    }
+    return 0;
+  };
+  if (int rc = build()) {
+    for (StageGraph& g : s1) g.reset();
+    unet_release_owner(v->stage1, s1_owner);
+    for (int o : lane_owner) unet_release_owner(v->stage2, o);
+    return rc;
+  }
+  // swap: nothing below fails
+  unet_release_owner(old->stage1, s->s1_owner);
+  lanes_release(s);                                // the old lane plans and s2_layers (a group member has none)
+  old->users--; v->users++;
+  s->voice = v; s->voice_id = voice_id; s->s1_owner = s1_owner;
+  for (int i = 0; i < 2; ++i) s->lane[i].owner = lane_owner[i];
+  for (int j = 0; j < kHandoffGraphs; ++j) {
+    HandoffGraphs& hg = s->hgraphs[j];
+    std::swap(hg.s1.exec, s1[j].exec); std::swap(hg.s1.launches, s1[j].launches);     // s1[j] drops the old graph
+    hg.s2_pro.reset(); hg.s2_epi.reset();
+  }
+  // the new voice's f0 map, as a session created on it starts; the speaker statistics, follow mode and formant ratio stay
+  const F0Map vm = voice_f0_map(v);
+  s->f0_map.mu_in = vm.mu_in; s->f0_map.sd_in = vm.sd_in; s->f0_map.mu_tgt = vm.mu_tgt; s->f0_map.sd_tgt = vm.sd_tgt;
+  s->f0_map.has_stats = vm.has_stats;
+  s->f0_dirty = true;
   return 0;
 }
 

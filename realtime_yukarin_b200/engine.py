@@ -66,6 +66,7 @@ EXPORTED_SYMBOLS = [
     'ryk_voice_f0_set_stats', 'ryk_session_create_voice', 'ryk_session_voice', 'ryk_group_add', 'ryk_group_remove', 'ryk_group_members',
     'ryk_session_get_f0_map', 'ryk_session_set_f0_map', 'ryk_session_f0_measure', 'ryk_session_f0_follow', 'ryk_session_f0_measure_reset',
     'ryk_session_f0_measured', 'ryk_session_set_formant', 'ryk_session_get_formant', 'ryk_stage2_convert_formant',
+    'ryk_session_set_voice',
 ]
 
 SEMITONE = math.log(2.0) / 12.0          # one semitone in ln f0
@@ -287,6 +288,12 @@ class Engine(object):
 
     def session_voice(self, sid: int) -> int:
         return self._check(self.lib.ryk_session_voice(self._h, sid))
+
+    def session_set_voice(self, sid: int, voice: int):
+        """Convert this session into `voice` from its next submitted step on, keeping its stream state (windows, synthesizer,
+        resamplers, speaker statistics, follow mode, formant ratio, group).  Every submitted chunk of the session (and of its group)
+        must be collected.  The f0 map becomes the new voice's: set a pitch offset again afterwards.  The same voice is a no-op."""
+        self._check(self.lib.ryk_session_set_voice(self._h, int(sid), int(voice)))
 
     # ---- models (voice 0 goes through the original entry points) ----
     def model_create(self, stage: int, in_channels: int, out_channels: int, base_channels: int, voice: int = 0):

@@ -166,6 +166,15 @@ class RealtimePipeline(object):
         """Engine.session_set_formant for this stream (ratio or semitones): from the next chunk on."""
         self.engine.session_set_formant(self._sid, **kwargs)
 
+    def set_voice(self, voice: int) -> None:
+        """Convert into `voice` from the next chunk on, keeping the stream's state (no gap, no refill from silence).  The chunks in
+        flight are finished first, in the new voice's place in the queue: their outputs stay queued for get / get_nowait in order.
+        The f0 map becomes the new voice's, so a pitch offset set with set_f0_map must be set again afterwards; the formant ratio and
+        the speaker statistics carry over."""
+        while self._inflight:
+            self._finish_one()
+        self.engine.session_set_voice(self._sid, voice)
+
     def measured_f0(self) -> Tuple[int, float, float]:
         """(voiced frames, mean, standard deviation) of the speaker's ln f0 over the chunks put so far (needs measure_f0)."""
         return self.engine.session_f0_measured(self._sid)
