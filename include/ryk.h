@@ -327,6 +327,39 @@ int ryk_session_f0_measured(ryk_engine* e, int session_id, long long* n_voiced, 
 int ryk_session_set_formant(ryk_engine* e, int session_id, double ratio);
 int ryk_session_get_formant(ryk_engine* e, int session_id, double* ratio);
 
+/* Input noise suppression (DESIGN.md §4f, DECIDE N1-N3): a decision-directed Wiener filter (Ephraim-Malah) on the model-rate input,
+ * ahead of the WORLD analysis, so analysis, silence gate, CREPE and f0 measuring all see the filtered signal.  Frames of N = 512
+ * samples at a hop of H = 128 (21.3 ms / 5.3 ms at 24 kHz), periodic sqrt-Hann analysis and synthesis windows, FP64 spectra of 257
+ * bins.  Per bin k with noise power profile phi[k], P_m = |X_m[k]|^2 and g = 10^(-reduction_db / 20):
+ *   xi_m = 0.98 G_{m-1}^2 P_{m-1} / phi + 0.02 max(P_m / phi - 1, 0),   G_m = max(xi_m / (1 + xi_m), g),   G_{-1} = 1, P_{-1} = 0;
+ *   G = 1 where phi[k] == 0.  reduction_db in [0, 40] is the most a bin is attenuated; at 0 the filter only round-trips the FFT.
+ * ryk_session_denoise: fresh session only (no chunk pushed); either order with ryk_session_set_input_rate.  The session then analyses
+ *   concat(zeros(511), z), z = the filtered model-rate input (511 = N - 1, the least delay that completes every emitted sample), and
+ *   ryk_session_io_geometry's delay_in includes the 511.  It starts at reduction_db = 20 with no profile, which passes the signal
+ *   through.  Three more kernels per step, on the gate stream; a session without the filter runs exactly the kernels it ran before.
+ * ryk_session_set_denoise: from the next submitted step on; steps already submitted keep theirs.  Allowed with chunks in flight and on
+ *   a group member; no device wait, no kernel.
+ * ryk_session_denoise_learn: the first n_frames frames processed from the next submitted step on (a step processes the frames whose
+ *   last sample it brings: 56 or 57 at a 0.3 s chunk) add their P to per-bin FP64 sums in frame order; when the last one is added,
+ *   phi = sum / n_frames applies from the following step.  The result depends on the input stream alone: it is bit-identical from run
+ *   to run and does not depend on other work on the engine.  A new call restarts the learning.  About 1 s of the user staying quiet
+ *   (188 frames at 24 kHz) is a reasonable choice.
+ * ryk_session_set_noise_profile: phi[257] from the next submitted step on; it cancels a learning in progress.  This is how a saved
+ *   profile is loaded.
+ * ryk_session_noise_profile: waits for the gate stream of the submitted steps, then writes the profile the next submitted step uses
+ *   and the frames still to learn (0: no learning in progress).  Either pointer may be NULL.
+ * ryk_denoise: the same filter over a whole signal on the same kernels: a fresh state, x zero outside [0, n), z = n samples with no
+ *   delay.  A session's z with constant settings and profile is bitwise ryk_denoise of its input.  phi may be NULL (no profile).
+ * Refused, changing nothing: an unknown session, enabling on a session that ran a step, set / learn / profile calls on a session
+ * without the filter, a non-finite reduction_db or one outside [0, 40], n_frames < 1, a profile entry that is negative or not
+ * finite. */
+int ryk_session_denoise(ryk_engine* e, int session_id);
+int ryk_session_set_denoise(ryk_engine* e, int session_id, double reduction_db);
+int ryk_session_denoise_learn(ryk_engine* e, int session_id, long long n_frames);
+int ryk_session_set_noise_profile(ryk_engine* e, int session_id, const double* phi);
+int ryk_session_noise_profile(ryk_engine* e, int session_id, double* phi, long long* frames_left);
+int ryk_denoise(ryk_engine* e, const float* x, int n, double reduction_db, const double* phi, float* z);
+
 /* Diagnostics: device timeline (ms) of the last <= 8 steps x 5 stages {gate, analysis, stage 1, stage 2, synthesis}; needs
  * RYK_STAGE_TIMES=1 in the environment at session creation.  start/end hold 40 floats; returns the number of steps. */
 int ryk_session_stage_times(ryk_engine* e, int session_id, float* start, float* end);

@@ -31,6 +31,7 @@
 #include <vector>
 
 #include "../../include/ryk.h"
+#include "denoise.h"
 #include "engine.h"
 #include "features.h"
 #include "synth.h"
@@ -77,6 +78,7 @@ struct ParitySet {
   float* in_win = nullptr;                       // device rates: input history window (in.hist device-rate samples)
   double* out_hist = nullptr;                    // device rates: kept synthesizer samples (out.hist)
   ResampleState *in_st = nullptr, *out_st = nullptr;   // device rates: the streaming resamplers' positions
+  DenoiseState* dn = nullptr;                    // input noise suppression: the filter's stream state
   // inter-stage buffers
   float *enc_f0 = nullptr, *enc_sp = nullptr, *enc_ap = nullptr, *enc_mc = nullptr; uint8_t* enc_voiced = nullptr;
   uint8_t* d_mask = nullptr; int* d_index = nullptr; int* d_count = nullptr;     // silence gate
@@ -104,6 +106,7 @@ struct StepEvents {
   std::array<cudaEvent_t*, 7> all() { return {&gate, &enc, &cslide, &s1, &pro, &conv, &dslide}; }
   cudaEvent_t tev[5][2] = {};      // RYK_STAGE_TIMES=1: [stage E1,E2,S1,S2,D][begin/end]
   F0Map* h_f0_map = nullptr;       // pinned staging of the f0 map copy in front of stage 1
+  DenoiseParams* h_dn = nullptr;   // pinned staging of the noise-suppression parameter copy in front of the wave slides
 };
 // The host-API staging of the caller's ticket t in slot t % kRing: the session's own step alone, the group's step while grouped.  A
 // membership change needs every host-API step collected, so no slot of one numbering is in use when the other takes over.
@@ -166,6 +169,13 @@ struct Session {
   bool f0_measure = false;         // the head of stage 1 ends with k_f0_measure
   bool f0_reset = false;           // the statistics restart at the next submitted step
   F0Map* d_f0_map = nullptr; F0Stats* d_f0_stats = nullptr;
+  // Input noise suppression (ryk_session_denoise, DESIGN.md §4f): the filter runs in the wave-slide graph on the model-rate chunk.  Its
+  // parameter block is host-owned (dn_sync copies dn_params in front of the graph when it changed); the learning state is device-owned.
+  bool denoise = false;
+  DenoiseWork dn;
+  DenoiseParams dn_params = {};    // what the next submitted step uses
+  bool dn_dirty = false;           // dn_params changed since the last submitted step
+  float* d_chunk_dn = nullptr;     // the step's filtered chunk (n_wave model-rate samples)
   BufferSet mem;                   // every device and pinned buffer above
 };
 
@@ -507,6 +517,21 @@ static int f0_map_sync(Session* s, long long k) {
   return 0;
 }
 
+// In front of the wave slides of step k on stream E: copy the noise-suppression parameters into the block the filter reads when they
+// changed since the previous step.  The wave slides of every step run on stream E in step order, so the steps already submitted keep
+// their parameters and the host neither waits nor launches a kernel.  The device writes only its own learning block, never this one
+// (DESIGN.md §4f).  The copy reads pinned slot k % kRing; that slot was last read by a copy of step k - kRing or earlier, which ended
+// before the wave slides of step k - kRing did.
+static int dn_sync(Session* s, long long k) {
+  if (!s->dn_dirty) return 0;
+  StepEvents& ev = s->ev[k % kRing];
+  if (k >= kRing) RYK_CUDA(cudaEventSynchronize(ev.gate));
+  *ev.h_dn = s->dn_params;
+  RYK_CUDA(cudaMemcpyAsync(s->dn.params, ev.h_dn, sizeof(DenoiseParams), cudaMemcpyHostToDevice, s->sE));
+  s->dn_dirty = false;
+  return 0;
+}
+
 // The rest of stage 1 of a chunk of parity b and hand-off slot h: (gather ->) 1-D U-Net at padded length tp1 (0: no effective frame,
 // voice_changer.py:32-35 skips the net) -> scatter into the silent template + f0 map, mc2sp.  Enqueued on stream C while it is captured
 // as one body of the chunk's SWITCH graph; every body is captured when the session is created so that no chunk ever pays for a capture
@@ -568,6 +593,7 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
     RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev[(k - 2) % kRing].cslide, 0));  // q.cw_wave: last read by the silence gate in the head of stage 1 of k-2
     RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev[(k - 2) % kRing].enc, 0));     // q.wave_win: last read by the analysis of k-2
   }
+  if (dn_sync(s, k)) return -1;
   if (stage_time(s, 0, 0, r, s->sE)) return -1;
   if (run_graph(e, p.graphs.gate, s->sE, [&]() -> int {
         const float* chunk = s->d_chunk_fixed;
@@ -576,6 +602,10 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
           if (resample_stream_in_run(e, q.in_win, s->in.hist, s->n_in, s->delay_in, s->in.up, s->in.down, s->in.d_h, s->in.n_taps,
                                      p.in_st, q.in_st, s->d_chunk_model, s->n_wave, s->sE)) return -1;
           chunk = s->d_chunk_model;
+        }
+        if (s->denoise) {            // noise suppression of the model-rate chunk in front of the wave slide
+          if (denoise_run(e, s->dn, p.dn, q.dn, chunk, s->n_wave, s->d_chunk_dn, s->sE)) return -1;
+          chunk = s->d_chunk_dn;
         }
         if (slide<float>(p.wave_win, chunk, q.wave_win, s->Lw, s->n_wave, 1, s->sE)) return -1;
         return slide<float>(p.cw_wave, q.wave_win + (size_t)pe * s->hop, q.cw_wave, (size_t)s->Tw * s->hop, (size_t)s->n_feat * s->hop, 1, s->sE);
@@ -1074,7 +1104,7 @@ int ryk_session_io_geometry(ryk_engine* h, int id, int* n_in, int* max_out, int*
   RYK_CHECK(s != nullptr, "no such session");
   if (n_in) *n_in = s->n_in;
   if (max_out) *max_out = s->max_out;
-  if (delay_in) *delay_in = s->delay_in;
+  if (delay_in) *delay_in = s->delay_in + (s->denoise ? kDnDelay : 0);
   if (in_rate) *in_rate = s->in.rate ? s->in.rate : s->cfg.fs;
   if (out_rate) *out_rate = s->out.rate ? s->out.rate : s->cfg.fs;
   return 0;
@@ -1169,6 +1199,94 @@ int ryk_session_get_formant(ryk_engine* h, int id, double* ratio) {
   RYK_CHECK(s != nullptr, "no such session");
   RYK_CHECK(ratio != nullptr, "null argument");
   *ratio = s->f0_map.formant;
+  return 0;
+}
+
+// ---- input noise suppression (DESIGN.md §4f) ----
+// The setters change host state only; dn_sync carries it to the device in front of the wave slides of the next submitted step.
+static Session* denoise_session(Engine* e, int id) {
+  Session* s = get_session(e, id);
+  if (!s) set_error("no such session");
+  else if (!s->denoise) set_error("noise suppression is not enabled for this session (ryk_session_denoise)");
+  return s && s->denoise ? s : nullptr;
+}
+
+int ryk_session_denoise(ryk_engine* h, int id) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Session* s = get_session(e, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  RYK_CHECK(s->step == 0, "noise suppression can only be enabled on a fresh session (no chunk pushed): the wave slides are captured at the first steps");
+  if (s->denoise) return 0;
+  BufferSet& m = s->mem;
+  DenoiseWork& w = s->dn;
+  w.max_frames = denoise_max_frames(s->n_wave);
+  if (m.device(&w.params, 1) || m.device(&w.learn, 1) || m.device(&w.spec, (size_t)kDnBins * w.max_frames) ||
+      m.device(&w.frames, (size_t)kDnN * w.max_frames) || m.device(&w.done, 1) || m.device(&s->d_chunk_dn, s->n_wave))
+    return -1;
+  for (ParitySet& p : s->par) if (m.device(&p.dn, 1)) return -1;
+  for (StepEvents& ev : s->ev) if (m.pinned(&ev.h_dn, 1)) return -1;
+  // step 0 reads par[0]: G_{-1} = 1; the parameter block starts at 20 dB without a profile
+  void* hp = nullptr;
+  if (engine_pinned(e, sizeof(DenoiseState), &hp)) return -1;
+  denoise_state_init((DenoiseState*)hp);
+  RYK_CUDA(cudaMemcpyAsync(s->par[0].dn, hp, sizeof(DenoiseState), cudaMemcpyHostToDevice, e->stream));
+  s->dn_params = {};
+  s->dn_params.gain_floor = pow(10.0, -20.0 / 20.0);
+  *s->ev[0].h_dn = s->dn_params;
+  RYK_CUDA(cudaMemcpyAsync(w.params, s->ev[0].h_dn, sizeof(DenoiseParams), cudaMemcpyHostToDevice, e->stream));
+  RYK_CUDA(cudaStreamSynchronize(e->stream));      // the zero-fills and the copies: the session's streams do not wait for the engine stream
+  s->denoise = true;
+  return 0;
+}
+
+int ryk_session_set_denoise(ryk_engine* h, int id, double reduction_db) {
+  Session* s = denoise_session(&h->impl, id);
+  if (!s) return -2;
+  if (int rc = denoise_check(reduction_db, nullptr)) return rc;
+  s->dn_params.gain_floor = pow(10.0, -reduction_db / 20.0);
+  s->dn_dirty = true;
+  return 0;
+}
+
+int ryk_session_denoise_learn(ryk_engine* h, int id, long long n_frames) {
+  Session* s = denoise_session(&h->impl, id);
+  if (!s) return -2;
+  RYK_CHECK(n_frames >= 1, "n_frames must be at least 1");
+  s->dn_params.learn_serial++;
+  s->dn_params.learn_frames = n_frames;
+  s->dn_dirty = true;
+  return 0;
+}
+
+int ryk_session_set_noise_profile(ryk_engine* h, int id, const double* phi) {
+  Session* s = denoise_session(&h->impl, id);
+  if (!s) return -2;
+  RYK_CHECK(phi != nullptr, "null argument");
+  if (int rc = denoise_check(0.0, phi)) return rc;
+  memcpy(s->dn_params.phi, phi, sizeof(double) * kDnBins);
+  s->dn_params.profile_serial++;
+  s->dn_params.learn_serial++;                     // cancels a learning in progress
+  s->dn_params.learn_frames = 0;
+  s->dn_dirty = true;
+  return 0;
+}
+
+int ryk_session_noise_profile(ryk_engine* h, int id, double* phi, long long* frames_left) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Session* s = denoise_session(e, id);
+  if (!s) return -2;
+  void* hp = nullptr;
+  if (engine_pinned(e, sizeof(DenoiseLearn), &hp)) return -1;
+  DenoiseLearn* L = (DenoiseLearn*)hp;
+  RYK_CUDA(cudaMemcpyAsync(L, s->dn.learn, sizeof(DenoiseLearn), cudaMemcpyDeviceToHost, s->sE));
+  RYK_CUDA(cudaStreamSynchronize(s->sE));          // behind the wave slides of every submitted step
+  // requests not yet applied (not submitted yet: every submitted step's gain scan has run) are what the next step applies
+  const DenoiseParams& P = s->dn_params;
+  const bool new_profile = P.profile_serial != L->profile_serial, new_learn = P.learn_serial != L->learn_serial;
+  if (phi) memcpy(phi, new_profile ? P.phi : L->phi, sizeof(double) * kDnBins);
+  if (frames_left) *frames_left = new_learn ? P.learn_frames : L->remaining;
   return 0;
 }
 

@@ -66,12 +66,15 @@ EXPORTED_SYMBOLS = [
     'ryk_voice_f0_set_stats', 'ryk_session_create_voice', 'ryk_session_voice', 'ryk_group_add', 'ryk_group_remove', 'ryk_group_members',
     'ryk_session_get_f0_map', 'ryk_session_set_f0_map', 'ryk_session_f0_measure', 'ryk_session_f0_follow', 'ryk_session_f0_measure_reset',
     'ryk_session_f0_measured', 'ryk_session_set_formant', 'ryk_session_get_formant', 'ryk_stage2_convert_formant',
-    'ryk_session_set_voice',
+    'ryk_session_set_voice', 'ryk_session_denoise', 'ryk_session_set_denoise', 'ryk_session_denoise_learn', 'ryk_session_set_noise_profile',
+    'ryk_session_noise_profile', 'ryk_denoise',
 ]
 
 SEMITONE = math.log(2.0) / 12.0          # one semitone in ln f0
 F0_SD_FLOOR = 0.05                       # follow mode: least in_std (ln f0), about 0.9 semitones
 FORMANT_RANGE = (0.5, 2.0)               # formant ratios a session or ryk_stage2_convert_formant accepts: +-12 semitones
+NOISE_BINS = 257                         # bins of a noise profile: rfft of the filter's 512-sample frames
+NOISE_HOP = 128                          # model samples per noise-suppression frame
 
 
 class F0Map(ctypes.Structure):
@@ -635,6 +638,53 @@ class Engine(object):
         r = ctypes.c_double()
         self._check(self.lib.ryk_session_get_formant(self._h, sid, ctypes.byref(r)))
         return r.value
+
+    # ---- input noise suppression ----
+    def session_denoise(self, sid: int):
+        """Fresh session only: filter the input ahead of the analysis (reduction 20 dB, no profile yet, so the signal passes through).
+        The session's input delay grows by 511 model samples (session_io_geometry's delay_in)."""
+        self._check(self.lib.ryk_session_denoise(self._h, int(sid)))
+
+    def session_set_denoise(self, sid: int, reduction_db: float):
+        """The most a bin is attenuated, 0 to 40 dB, from the next submitted step on (chunks in flight keep theirs)."""
+        self._check(self.lib.ryk_session_set_denoise(self._h, int(sid), ctypes.c_double(reduction_db)))
+
+    def session_denoise_learn(self, sid: int, frames: Optional[int] = None, seconds: Optional[float] = None):
+        """Learn the noise profile from the next `frames` frames (or `seconds` of input at the session's rate, 128 samples per
+        frame) from the next submitted step on; it applies from the step after the last of them.  Exactly one of the two."""
+        if (frames is None) == (seconds is None):
+            raise ValueError('give exactly one of frames and seconds')
+        if frames is None:
+            frames = max(1, round(float(seconds) * self._session_fs[sid] / NOISE_HOP))
+        self._check(self.lib.ryk_session_denoise_learn(self._h, int(sid), ctypes.c_longlong(int(frames))))
+
+    def session_set_noise_profile(self, sid: int, profile):
+        """Load a noise profile (257 per-bin powers, as session_noise_profile returns) from the next submitted step on; it cancels
+        a learning in progress."""
+        phi = numpy.ascontiguousarray(profile, dtype=numpy.float64).ravel()
+        if len(phi) != NOISE_BINS:
+            raise ValueError(f'a noise profile has {NOISE_BINS} values')
+        self._check(self.lib.ryk_session_set_noise_profile(self._h, int(sid), _dp(phi)))
+
+    def session_noise_profile(self, sid: int):
+        """(profile the next submitted step uses, frames still to learn); waits for the submitted steps' input stage."""
+        phi = numpy.zeros(NOISE_BINS, numpy.float64)
+        left = ctypes.c_longlong()
+        self._check(self.lib.ryk_session_noise_profile(self._h, int(sid), _dp(phi), ctypes.byref(left)))
+        return phi, left.value
+
+    def denoise(self, x, reduction_db: float, profile=None) -> numpy.ndarray:
+        """The session's noise suppression over a whole signal: a fresh filter, no delay, len(x) float32 samples out."""
+        x = _f32(x)
+        z = numpy.empty_like(x)
+        phi = None
+        if profile is not None:
+            phi = numpy.ascontiguousarray(profile, dtype=numpy.float64).ravel()
+            if len(phi) != NOISE_BINS:
+                raise ValueError(f'a noise profile has {NOISE_BINS} values')
+        self._check(self.lib.ryk_denoise(self._h, _fp(x), len(x), ctypes.c_double(reduction_db), _dp(phi) if phi is not None else None,
+                                         _fp(z)))
+        return z
 
     def session_destroy(self, sid: int):
         self._check(self.lib.ryk_session_destroy(self._h, sid))

@@ -60,12 +60,26 @@ def save_measured_statistics(pipeline: RealtimePipeline, path: Path) -> bool:
     return True
 
 
+def save_noise_profile_file(pipeline: RealtimePipeline, path: Path) -> None:
+    """Write the noise profile the stream's filter uses now to `path` (.npy, 257 float64 powers) for a later --noise_profile."""
+    phi, left = pipeline.noise_profile()
+    if left:
+        print(f'the noise profile was still being learned ({left} frames to go): {path} holds the profile in use before it')
+    numpy.save(path, phi)
+    print(f'wrote {path}')
+
+
 def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path] = None, max_chunks: Optional[int] = None,
         engine=None, depth: int = 3, measure_input_statistics: Optional[Path] = None, follow_input_f0: Optional[int] = None,
-        pitch: float = 0.0, formant: float = 0.0) -> int:
+        pitch: float = 0.0, formant: float = 0.0, denoise: Optional[float] = None, noise_profile: Optional[Path] = None,
+        learn_noise: Optional[float] = None, save_noise_profile: Optional[Path] = None) -> int:
     """`measure_input_statistics`: measure the speaker's log-f0 statistics during the run and write them to this file at the end;
     `follow_input_f0`: convert with the measured statistics once this many voiced frames are counted; `pitch`: semitones added to
-    the target voice's mean f0; `formant`: semitones by which the converted spectral envelope moves."""
+    the target voice's mean f0; `formant`: semitones by which the converted spectral envelope moves; `denoise`: filter the input's
+    noise ahead of the analysis with at most this many dB of attenuation, with the profile in `noise_profile` (.npy) or one learned from
+    the first `learn_noise` seconds of input, and write the profile in use to `save_noise_profile` at the end."""
+    if denoise is None and (noise_profile is not None or learn_noise is not None or save_noise_profile is not None):
+        raise ValueError('--noise_profile, --learn_noise and --save_noise_profile need --denoise')
     logger = logging.getLogger('root')
     logger.info('model loading...')
     config = Config.from_yaml(config_path)
@@ -74,7 +88,9 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
         stage1_model_path=config.stage1_model_path, stage1_config_path=config.stage1_config_path,
         stage2_model_path=config.stage2_model_path, stage2_config_path=config.stage2_config_path)
     pipeline = RealtimePipeline(config, acoustic_param=converter.acoustic_converter.config.dataset.acoustic_param, engine=engine, depth=depth,
-                                measure_f0=measure_input_statistics is not None, follow_f0=follow_input_f0, formant=formant)
+                                measure_f0=measure_input_statistics is not None, follow_f0=follow_input_f0, formant=formant,
+                                denoise=denoise, noise_profile=None if noise_profile is None else numpy.load(noise_profile),
+                                learn_noise=learn_noise)
     try:
         if pitch:
             pipeline.set_f0_map(semitones=pitch)
@@ -113,6 +129,9 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
             if measure_input_statistics is not None:
                 pipeline.flush()
                 save_measured_statistics(pipeline, measure_input_statistics)
+            if save_noise_profile is not None:
+                pipeline.flush()
+                save_noise_profile_file(pipeline, save_noise_profile)
         finally:
             pipeline.close()
 
@@ -134,6 +153,14 @@ def make_parser() -> argparse.ArgumentParser:
     parser.add_argument('--formant', type=float, default=0.0, metavar='SEMITONES',
                         help='move the converted spectral envelope (the formants) by this many semitones, -12 to 12; with --pitch '
                              'by the same amount the voice sounds like a different speaker rather than the same one at another pitch')
+    parser.add_argument('--denoise', type=float, default=None, metavar='DB',
+                        help='suppress the noise of the input ahead of the analysis, attenuating by at most DB (0-40; 20 is a good '
+                             'start); the noise profile comes from --noise_profile or --learn_noise (without one the input passes unchanged)')
+    parser.add_argument('--noise_profile', type=Path, default=None, metavar='IN.npy', help='with --denoise: the noise profile to use')
+    parser.add_argument('--learn_noise', type=float, default=None, metavar='SECONDS',
+                        help='with --denoise: learn the noise profile from the first SECONDS of input (stay quiet meanwhile; 1 s is enough)')
+    parser.add_argument('--save_noise_profile', type=Path, default=None, metavar='OUT.npy',
+                        help='with --denoise: write the noise profile in use to this file when the run ends, for --noise_profile')
     return parser
 
 
@@ -141,7 +168,8 @@ def main(argv: Optional[Iterable[str]] = None) -> None:
     args = make_parser().parse_args(argv)
     run(config_path=args.config_path, wav_in=args.wav_in, wav_out=args.wav_out, max_chunks=args.max_chunks,
         measure_input_statistics=args.measure_input_statistics, follow_input_f0=args.follow_input_f0, pitch=args.pitch,
-        formant=args.formant)
+        formant=args.formant, denoise=args.denoise, noise_profile=args.noise_profile, learn_noise=args.learn_noise,
+        save_noise_profile=args.save_noise_profile)
 
 
 if __name__ == '__main__':

@@ -87,10 +87,13 @@ class RealtimePipeline(object):
     `measure_f0=True` keeps running statistics of the speaker's log-f0 on the device (`measured_f0`); `follow_f0=N` (implies
     measuring) also makes them the input side of the session's f0 map once N voiced frames are counted.  `set_f0_map` changes the
     map between chunks.  `formant` (semitones, [-12, 12]) warps the converted spectral envelope from the first chunk on; `set_formant`
-    changes it between chunks."""
+    changes it between chunks.  `denoise=DB` filters the input's noise ahead of the analysis (at most DB of attenuation, 0-40), with
+    `noise_profile` (257 values, as `noise_profile()` returns them) or a profile learned from the first `learn_noise` seconds of input;
+    `set_denoise` changes the reduction between chunks."""
 
     def __init__(self, config: Config, acoustic_param=None, engine: Optional[Engine] = None, depth: int = 3, voice: int = 0,
-                 measure_f0: bool = False, follow_f0: Optional[int] = None, formant: float = 0.0):
+                 measure_f0: bool = False, follow_f0: Optional[int] = None, formant: float = 0.0, denoise: Optional[float] = None,
+                 noise_profile=None, learn_noise: Optional[float] = None):
         self.config = config
         self.engine = engine or default_engine()
         p = acoustic_param
@@ -142,6 +145,15 @@ class RealtimePipeline(object):
             hop = round(fs * float(config.frame_period) / 1000)
             td = round(config.buffer_time * rate) + 2 * round(config.decode_extra_time * rate)
             n_out_cap = (td * hop // config.vocoder_buffer_size + 4) * config.vocoder_buffer_size
+        if denoise is not None:
+            self.engine.session_denoise(self._sid)
+            self.engine.session_set_denoise(self._sid, float(denoise))
+            if noise_profile is not None:
+                self.engine.session_set_noise_profile(self._sid, noise_profile)
+            if learn_noise is not None:
+                self.engine.session_denoise_learn(self._sid, seconds=float(learn_noise))
+        elif noise_profile is not None or learn_noise is not None:
+            raise ValueError('noise_profile and learn_noise need denoise')
         if measure_f0 or follow_f0 is not None:
             self.engine.session_f0_measure(self._sid)
         if follow_f0 is not None:
@@ -174,6 +186,14 @@ class RealtimePipeline(object):
         while self._inflight:
             self._finish_one()
         self.engine.session_set_voice(self._sid, voice)
+
+    def set_denoise(self, reduction_db: float) -> None:
+        """Engine.session_set_denoise for this stream: the most the noise filter attenuates, from the next chunk on."""
+        self.engine.session_set_denoise(self._sid, reduction_db)
+
+    def noise_profile(self) -> Tuple[numpy.ndarray, int]:
+        """(noise profile the next chunk uses, frames still to learn) of the stream's noise filter (needs denoise)."""
+        return self.engine.session_noise_profile(self._sid)
 
     def measured_f0(self) -> Tuple[int, float, float]:
         """(voiced frames, mean, standard deviation) of the speaker's ln f0 over the chunks put so far (needs measure_f0)."""
