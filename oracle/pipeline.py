@@ -139,6 +139,14 @@ class StreamOracle:
             out[lo - first:hi - first] = arr[lo:hi]
         return out
 
+    def _extract(self, win: np.ndarray) -> Dict[str, np.ndarray]:
+        """the encode stage on one encode window; a subclass may put another implementation of the same stage here"""
+        return extract_features(win, self.cfg)
+
+    def _convert(self, wave: np.ndarray, feat: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:
+        """the convert stage on one convert window (wave: its Tw * hop samples); a subclass may put another implementation here"""
+        return convert_window(wave, feat, self.cfg, self.stage1, self.stage2, self.f0_stats, self.backend)
+
     def push(self, chunk: np.ndarray):
         cfg, k = self.cfg, self.k
         hop = cfg.hop
@@ -147,7 +155,7 @@ class StreamOracle:
         # ---- encode ----
         self.wave_hist = np.concatenate([self.wave_hist, np.asarray(chunk, np.float32)])
         win = self._window(self.wave_hist, k * self.n_wave - 2 * self.e_wave - self.wave_base, self.n_wave + 2 * self.e_wave, 0.0)
-        f = extract_features(win, cfg)
+        f = self._extract(win)
         pad = round(self.extra[0] * self.rate)
         aligned = win
         if pad > 0:
@@ -164,7 +172,7 @@ class StreamOracle:
         wfeat = dict(f0=self._window(self.enc_hist['f0'], first, Tw, 0.0), ap=self._window(self.enc_hist['ap'], first, Tw, 0.0),
                      mc=self._window(self.enc_hist['mc'], first, Tw, silent_mc), voiced=self._window(self.enc_hist['voiced'], first, Tw, False))
         wwave = self._window(self.enc_hist['wave'], first * hop, Tw * hop, 0.0)
-        conv = convert_window(wwave, wfeat, cfg, self.stage1, self.stage2, self.f0_stats, self.backend)
+        conv = self._convert(wwave, wfeat)
         if self.e_conv > 0:
             conv = {kk: v[self.e_conv:-self.e_conv] for kk, v in conv.items() if kk in ('f0', 'ap', 'sp')}
         for kk in ('f0', 'ap', 'sp'):

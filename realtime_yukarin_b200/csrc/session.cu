@@ -438,8 +438,7 @@ static int stage1_body(Engine* e, Session* s, Voice* v, int owner, int b, int h,
 // conditional nodes, 12.8+), on the stage-1 plans of voice v under plan owner `owner`.
 static int stage1_build_switch(Engine* e, Session* s, Voice* v, int owner, int j, StageGraph& g) {
   const int b = j & 1, h = j % kHandoff;
-  const int n_buckets = s->Tp / 128 + 1;
-  RYK_CHECK(n_buckets <= 16, "window too long for the stage-1 graph table");
+  const int n_buckets = s->Tp / 128 + 1;                 // <= 16: session_build refuses longer windows
   cudaGraph_t graph = nullptr;
   RYK_CUDA(cudaGraphCreate(&graph, 0));
   cudaGraphConditionalHandle handle;
@@ -888,6 +887,8 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
   RYK_CHECK(s->n_wave == s->n_feat * s->hop && s->e_wave == s->e_enc_frames * s->hop, "buffer_time / encode_extra_time must be whole frames");
   RYK_CHECK(s->Lw / s->hop - 2 * s->e_enc_frames == s->n_feat, "encode window does not trim to one chunk of frames");
   RYK_CHECK(s->nb == 513 && s->voice->stage1->in_ch == s->C, "session configuration does not match the loaded models");
+  // the stage-1 SWITCH has a body per padded-length bucket 0 .. Tp / 128 (BucketKernels holds 16): Tw <= 1919
+  RYK_CHECK(s->Tp / 128 + 1 <= 16, "window too long for the stage-1 graph table");
   // the synthesizer's spectra are cheaptrick_fft_size(fs) / 2 + 1 bins wide and read rows of the fft_length / 2 + 1 bin decode window
   RYK_CHECK(cheaptrick_fft_size(cfg->fs, 71.0) / 2 + 1 == s->nb,
             "fs does not match fft_length: the synthesizer at this fs needs a different spectrum width (run the session at the model's "

@@ -42,6 +42,12 @@ class OracleEngine:
         f = opipe.extract_features(np.asarray(x, np.float32), self.cfg)
         return dict(f0=f['f0'].ravel(), sp=f['sp'], ap=f['ap'], mc=f['mc'], voiced=f['voiced'].ravel())
 
+    def convert_window(self, wave, fs, frame_length, hop, threshold_db, f0, ap, mc, voiced, order, alpha, fftlen):
+        feat = dict(f0=np.asarray(f0, np.float32).reshape(-1, 1), ap=ap, mc=mc, voiced=np.asarray(voiced, bool).reshape(-1, 1))
+        out = opipe.convert_window(np.asarray(wave, np.float32), feat, self.cfg, self.p1, self.p2, self.stats, self.backend,
+                                   threshold_db=threshold_db)
+        return dict(f0=out['f0'].ravel(), ap=out['ap'], sp=out['sp'], voiced=out['voiced'].ravel(), mc=out['mc'])
+
     def silence_mask(self, wave, frame_length, hop, threshold_db, n_frames):
         return opipe.effective_mask(np.asarray(wave, np.float32), n_frames, self.cfg, threshold_db)
 

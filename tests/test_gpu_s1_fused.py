@@ -1,5 +1,6 @@
 """Fused stage-1 kernel (csrc/s1_fused.cu: the whole 1-D U-Net as one cluster launch) against the 16-layer wgmma sequence it replaces
-and against the oracle (oracle/nets.py), base-64 model, every padded-length bucket the BASELINE configurations reach."""
+and against the oracle (oracle/nets.py), base-64 model, every padded-length bucket the BASELINE configurations reach and the longer
+windows of tests/session_geometry.py up to the largest a session accepts (Tw 1919, bucket 1920)."""
 import numpy as np
 import pytest
 
@@ -21,7 +22,7 @@ def test_fused_stage1_matches_layered_and_oracle(engine, full_models):
     try:
         import os
         quick = os.environ.get('RYK_TEST_QUICK') == '1'                     # compute-sanitizer runs: two buckets are enough
-        for T in ((60, 260) if quick else (3, 60, 128, 200, 260, 383, 400, 600, 640, 1000)):     # buckets 128 .. 1024
+        for T in ((60, 260) if quick else (3, 60, 128, 200, 260, 383, 400, 600, 640, 1000, 1100, 1500, 1919)):     # buckets 128 .. 1920
             mc = (synthetic.MC_MEAN_IN + synthetic.MC_STD_IN * rng.standard_normal((T, 9))).astype(np.float32)
             ref = onets.stage1_convert(mc, p1, backend='torch')
             engine.set_stage1_fused(True)

@@ -27,11 +27,11 @@ import pytest
 
 from oracle import nets as onets
 from oracle import pipeline as opipe
-from oracle import world as oworld
 from realtime_yukarin_b200 import synthetic
 
 from . import gated_speech as gs
-from .test_gpu_headline_parity import _rmse, _waveform_spectral_distance
+from .stream_compare import SP_TOL, DeviceRowsOracle, compare_stream, compare_stream_pulse_aware, logspec, run_stream
+from .test_gpu_headline_parity import _rmse
 from .test_gpu_parity import _load
 
 pytestmark = pytest.mark.gpu
@@ -41,7 +41,6 @@ TW = 260
 FS, T, EXTRA = 24000, 0.3, (0.0, 0.5, 0.0)
 SILENT_MC0_BITS = np.float32(opipe.SILENT_MC0).view(np.uint32)
 MC_TOL = {'fp32': 5e-4, 'fp16': 2e-2}                       # test_gpu_parity.test_stage1_matches_oracle
-SP_TOL = {('small', 'fp32'): (2e-3, None), ('small', 'fp16'): (3e-2, 0.25), ('full', 'fp16'): (1e-2, 6e-2)}     # (per-frame log-L2, max)
 WINDOW_IDS = [f'{p}-{t}{"-zeros" if z else ""}' for p, t, z in gs.WINDOW_CASES]
 
 _cache = {}
@@ -89,13 +88,6 @@ def _bits(a):
     return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
-def _logspec(a, b, rows):
-    if not rows.any():
-        return 0.0, 0.0
-    d = np.log(np.asarray(a, np.float64)[rows]) - np.log(np.asarray(b, np.float64)[rows])
-    return float(np.sqrt((d ** 2).mean(axis=1)).max()), float(np.abs(d).max())
-
-
 def _check_window(label, out, ref, enc, stats, models, precision):
     """`out` (f0 (T,), ap, sp, voiced (T,), mc) against the oracle's window `ref`, the mask-derived parts exactly."""
     eff = ref['effective']
@@ -112,8 +104,8 @@ def _check_window(label, out, ref, enc, stats, models, precision):
     assert np.array_equal(f0[eff] != 0, want_f0 != 0) and np.allclose(f0[eff], want_f0, rtol=1e-6, atol=0), label
     row_err = np.abs(out['mc'][eff].astype(np.float64) - ref['mc'][eff]).max(axis=1) if len(index) else np.zeros(0)
     mc_err = float(row_err.max()) if len(index) else 0.0
-    l2_e, mx_e = _logspec(out['sp'], ref['sp'], eff)
-    l2_g, mx_g = _logspec(out['sp'], ref['sp'], ~eff)
+    l2_e, mx_e = logspec(out['sp'], ref['sp'], eff)
+    l2_g, mx_g = logspec(out['sp'], ref['sp'], ~eff)
     tp = len(index) + 128 - len(index) % 128 if len(index) else 0
     print(f'{label} {precision}: T_eff {len(index)} padded {tp} bucket {tp // 128}; mc rows max err {mc_err:.2e}; '
           f'sp log-L2 / max: effective {l2_e:.2e} / {mx_e:.2e}, gated {l2_g:.2e} / {mx_g:.2e}')
@@ -241,17 +233,18 @@ def _chunks(x, steps, buffer_time=T):
     return [np.ascontiguousarray(x[k * n:(k + 1) * n], np.float32) for k in range(steps)]
 
 
-def _oracle_stream(paths, name, chunks, thr, stats, buffer_time=T, converted=False):
-    """The oracle stream's output per step, or (converted=True) the f0 / sp / ap rows its synthesizer was given per step."""
+def _oracle_stream(paths, name, chunks, thr, stats, buffer_time=T):
+    """The oracle stream's run (oracle.pipeline.StreamOracle through stream_compare.run_stream) over the chunks"""
     def make():
         p1, p2 = _nets(paths)
-        orc = opipe.StreamOracle(opipe.PathConfig(threshold_db=thr), p1, p2, stats, buffer_time=buffer_time, extra=EXTRA, backend='torch')
-        refs, convs = [], []
-        for c in chunks:
-            refs.append(orc.push(c))
-            convs.append(orc.last['converted'])
-        return refs, convs
-    return _cached(('stream', str(paths['stage1_model_path']), name, len(chunks), thr, buffer_time), make)[1 if converted else 0]
+        return run_stream(opipe.StreamOracle(opipe.PathConfig(threshold_db=thr), p1, p2, stats, buffer_time=buffer_time, extra=EXTRA,
+                                             backend='torch'), chunks)
+    return _cached(('stream', str(paths['stage1_model_path']), name, len(chunks), thr, buffer_time), make)
+
+
+def _device_stream(engine, chunks, thr, buffer_time=T):
+    """The oracle's stream bookkeeping and synthesizer over the engine's per-op rows, at the engine's current precision"""
+    return run_stream(DeviceRowsOracle(engine, opipe.PathConfig(threshold_db=thr), buffer_time, EXTRA), chunks)
 
 
 def _run_session(engine, cfg, chunks, in_flight=3, measure=False):
@@ -282,115 +275,10 @@ def _bucket_table(label, x, steps, thr, buffer_time=T):
     return rows
 
 
-def _compare_stream(label, outs, refs, rmse_tol, chunk_tol, lsd_tol=None, silent_ok=False):
-    assert [len(o) for o in outs] == [len(r) for r in refs], label
-    per = [_rmse(o, r) if len(r) else 0.0 for o, r in zip(outs, refs)]
-    y, r = np.concatenate(outs), np.concatenate(refs)
-    assert len(r) > 0 and np.isfinite(y).all()
-    rmse, rms, lsd = _rmse(y, r), float(np.sqrt(np.mean(r ** 2))), _waveform_spectral_distance(y, r)
-    print(f'{label}: {len(y)} samples, sample RMSE {rmse:.3e} (signal RMS {rms:.3e}), worst chunk {max(per):.3e} (step {int(np.argmax(per))}), '
-          f'log-STFT distance {lsd:.3e}')
-    if max(per) > chunk_tol:
-        print('  per-chunk (step, rmse):', [(k, f'{e:.1e}') for k, e in enumerate(per) if e > chunk_tol / 10])
-    assert silent_ok or rms > 1e-2
-    assert rmse <= rmse_tol, (label, rmse)
-    assert max(per) <= chunk_tol, (label, max(per))
-    assert lsd_tol is None or lsd <= lsd_tol, (label, lsd)
-
-
-def _device_rows(engine, x, chunks, thr):
-    """The f0 / sp / ap rows a session hands its synthesizer, rebuilt step by step from the per-op calls: world_analyze of every chunk
-    (the session's analysis kernels), the 260-frame window over that history, ryk_convert_window, the 60 kept rows."""
-    nb = CFG.fft_length // 2 + 1
-    hist = dict(f0=np.zeros(0, np.float32), ap=np.zeros((0, nb), np.float32), mc=np.zeros((0, CFG.order + 1), np.float32), voiced=np.zeros(0, bool))
-    silent_mc = np.zeros((1, CFG.order + 1), np.float32)
-    silent_mc[0, 0] = opipe.SILENT_MC0
-    fills = dict(f0=0.0, ap=0.0, mc=silent_mc, voiced=False)
-    rows = []
-    for k, (c, wave) in enumerate(zip(chunks, gs.step_windows(x, len(chunks)))):
-        a = engine.world_analyze(c, CFG.fs, CFG.frame_period, CFG.f0_floor, CFG.f0_ceil, CFG.fft_length, CFG.order, CFG.alpha)
-        hist = {kk: np.concatenate([hist[kk], a[kk]]) for kk in hist}
-        w = {kk: opipe.StreamOracle._window(hist[kk], k * 60 - 200, TW, fills[kk]) for kk in hist}
-        out = _convert(engine, wave, w, thr)
-        rows.append({kk: np.asarray(out[kk])[100:160] for kk in ('f0', 'sp', 'ap')})
-    return rows
-
-
-def _oracle_synth(rows):
-    """The oracle's realtime synthesizer over per-step rows -> (samples per step, NaN scrubbed; pulse sample indices; pulse voicing)"""
-    syn = oworld.RealtimeSynthesizer(CFG.fs, CFG.frame_period, oworld.cheaptrick_fft_size(CFG.fs), 1024)
-    ys = []
-    for r in rows:
-        y = np.array(syn.decode(np.asarray(r['f0'], np.float64).ravel(), r['sp'], r['ap']))
-        y[np.isnan(y)] = 0
-        ys.append(y)
-    idx, _, vuv = syn.pulses()
-    return ys, idx, vuv
-
-
-def _compare_stream_pulse_aware(label, engine, x, chunks, outs, refs, convs, models, precision, lsd_tol=None):
-    """A session against the oracle stream where one sample of pulse placement may differ.
-
-    The synthesizer places a pulse at the first sample after its phase crosses a multiple of 2 pi: a discrete function of the last bits of the
-    f0 history (DESIGN.md section 5, lesson 2).  The device's converted f0 is the oracle's to FP32 rounding, one ulp apart on about one
-    voiced frame in a hundred, which is enough to move a pulse that lands on a sample boundary by one sample; the two outputs then differ
-    by up to the pulse's amplitude over that pulse's response (fft_size samples) and nowhere else.  So the comparison is made in the parts
-    that can each be held tight:
-      * the rows the synthesizer is given (rebuilt through the per-op calls) equal the oracle's to the window tolerances, voicing exactly;
-      * the oracle's own synthesizer, fed those rows, places the same pulses as on the oracle's rows with the same voicing, except that at
-        most one of them sits one sample later or earlier (printed);
-      * FP32: the session's samples are that synthesizer's samples to 1e-9 everywhere, the moved pulse included -- the session's graphs,
-        bucket switch and hand-off slots add nothing of their own;
-      * outside the response of a moved pulse the session equals the oracle stream: 1e-6 per sample in FP32, the headline tolerances in FP16."""
-    fft = oworld.cheaptrick_fft_size(CFG.fs)
-    rows = _device_rows(engine, x, chunks, 60.0)
-    worst = dict(f0=0.0, sp=0.0, ap=0.0)
-    ulps = 0
-    for k, (d, o) in enumerate(zip(rows, convs)):
-        of0 = o['f0'].ravel()
-        assert np.array_equal(d['f0'] != 0, of0 != 0), (label, k)
-        assert np.allclose(d['f0'], of0, rtol=1e-6, atol=0), (label, k)
-        ulps += int((d['f0'].view(np.uint32) != of0.view(np.uint32)).sum())
-        worst['sp'] = max(worst['sp'], _logspec(d['sp'], o['sp'], np.ones(60, bool))[0])
-        worst['ap'] = max(worst['ap'], float(np.abs(d['ap'] - o['ap']).max()))
-    l2_tol = SP_TOL[(models, precision)][0]
-    assert worst['sp'] < l2_tol and worst['ap'] <= 1e-6, (label, worst)
-    y_o, idx_o, vuv_o = _oracle_synth(convs)
-    y_d, idx_d, vuv_d = _oracle_synth(rows)
-    assert all(np.array_equal(a, b) for a, b in zip(y_o, refs)), label          # the oracle stream is its synthesizer on its rows
-    assert len(idx_o) == len(idx_d) and np.array_equal(vuv_o, vuv_d), label
-    moved = np.flatnonzero(idx_o != idx_d)
-    print(f'{label}: synthesizer rows vs oracle: f0 differs by one ulp on {ulps} frames, sp per-frame log-L2 {worst["sp"]:.2e}, ap {worst["ap"]:.1e}; '
-          f'{len(idx_o)} pulses, moved: {[(int(j), int(idx_o[j]), int(idx_d[j])) for j in moved]} (pulse, oracle sample, sample on the device rows)')
-    assert len(moved) <= 1 and (np.abs(idx_o[moved] - idx_d[moved]) == 1).all(), (label, moved)
-    assert [len(o) for o in outs] == [len(r) for r in refs], label
-    y, r, yd = np.concatenate(outs), np.concatenate(refs), np.concatenate(y_d)
-    assert np.isfinite(y).all() and float(np.sqrt(np.mean(r ** 2))) > 1e-2
-    if precision == 'fp32':
-        print(f'{label}: session vs the oracle synthesizer on the device rows: max {np.abs(y - yd).max():.2e}')
-        assert np.abs(y - yd).max() <= 1e-9, label
-    inside = np.zeros(len(r), bool)
-    for j in moved:
-        inside[max(0, int(min(idx_o[j], idx_d[j])) - fft):int(max(idx_o[j], idx_d[j])) + fft] = True
-    if len(moved):
-        print(f'{label}: inside the moved pulse\'s response: {int(inside.sum())} samples, max difference {np.abs(y - r)[inside].max():.2e}; '
-              f'over the whole stream: sample RMSE {_rmse(y, r):.3e}, worst chunk {max(_rmse(o, q) for o, q in zip(outs, refs) if len(q)):.3e}')
-        assert float(np.abs(r[inside]).max()) > 0 and np.abs(y - r)[inside].max() <= 2 * float(np.abs(r).max()), label
-    assert _rmse(y, r) <= 1e-3, (label, _rmse(y, r))                             # the moved pulse included
-    y_out = np.where(inside, r, y)                                               # everything else
-    if precision == 'fp32':
-        print(f'{label}: outside it: max {np.abs(y_out - r).max():.2e}')
-        assert np.abs(y_out - r).max() <= 1e-6, label
-    bounds = np.cumsum([0] + [len(o) for o in outs])
-    _compare_stream(label + ' (outside a moved pulse)', [y_out[a:b] for a, b in zip(bounds[:-1], bounds[1:])], refs, 1e-3,
-                    1e-3 if precision == 'fp32' else 2e-3, lsd_tol=lsd_tol)
-    return len(moved)
-
-
 @pytest.mark.parametrize('zeros', [False, True], ids=['floor', 'zeros'])
 def test_session_walks_the_buckets_fp32(engine, small_models, small, zeros):
     """30 steps on both streams.  With the quiet floor one pulse of the 3416 (at stream sample 165672, in step 23, loud speech) lands on a sample
-    boundary and is placed one sample later on the device's rows than on the oracle's: _compare_stream_pulse_aware."""
+    boundary and is placed one sample later on the device's rows than on the oracle's: stream_compare.compare_stream_pulse_aware."""
     stats, steps = small[2], 30
     name = 'zeros' if zeros else 'floor'
     x = gs.stream_with_pauses(zeros=zeros)
@@ -400,8 +288,8 @@ def test_session_walks_the_buckets_fp32(engine, small_models, small, zeros):
     chunks = _chunks(x, steps)
     engine.set_precision('fp32')
     outs, _ = _run_session(engine, _session_cfg(60.0), chunks)
-    refs, convs = (_oracle_stream(small_models, f'pauses-{zeros}', chunks, 60.0, stats, converted=c) for c in (False, True))
-    _compare_stream_pulse_aware(f'session fp32 base-16, pauses ({name})', engine, x, chunks, outs, refs, convs, 'small', 'fp32')
+    compare_stream_pulse_aware(f'session fp32 base-16, pauses ({name})', outs, _oracle_stream(small_models, f'pauses-{zeros}', chunks, 60.0, stats),
+                               _device_stream(engine, chunks, 60.0), 'small', 'fp32')
 
 
 @pytest.mark.parametrize('fused', [True, False], ids=['fused', 'layered'])
@@ -415,9 +303,9 @@ def test_session_walks_the_buckets_fp16_full_models(engine, full_models, full, f
     assert (engine.set_stage1_fused(fused) >= 1) or not fused
     try:
         outs, _ = _run_session(engine, _session_cfg(60.0), chunks)
-        refs, convs = (_oracle_stream(full_models, 'pauses-False', chunks, 60.0, stats, converted=c) for c in (False, True))
-        _compare_stream_pulse_aware(f'session fp16 base-64 stage 1 {"fused" if fused else "layered"}, pauses (floor)', engine, x, chunks, outs,
-                                    refs, convs, 'full', 'fp16', lsd_tol=0.1)
+        compare_stream_pulse_aware(f'session fp16 base-64 stage 1 {"fused" if fused else "layered"}, pauses (floor)', outs,
+                                   _oracle_stream(full_models, 'pauses-False', chunks, 60.0, stats), _device_stream(engine, chunks, 60.0),
+                                   'full', 'fp16', lsd_tol=0.1)
     finally:
         engine.set_stage1_fused(True)
 
@@ -429,10 +317,10 @@ def test_session_threshold_zero_and_none(engine, small_models, small, thr, steps
     stream included."""
     stats = small[2]
     chunks = _chunks(gs.stream_with_pauses(), steps)
-    refs = _oracle_stream(small_models, 'pauses-False', chunks, thr, stats)
+    refs = _oracle_stream(small_models, 'pauses-False', chunks, thr, stats).outs
     engine.set_precision('fp32')
     outs, _ = _run_session(engine, _session_cfg(thr), chunks)
-    _compare_stream(f'session fp32 base-16, threshold {thr}', outs, refs, 1e-3, 1e-3, silent_ok=thr == 0.0)
+    compare_stream(f'session fp32 base-16, threshold {thr}', outs, refs, 1e-3, 1e-3, silent_ok=thr == 0.0)
 
 
 def test_session_window_of_256_frames(engine, small_models, small):
@@ -445,7 +333,8 @@ def test_session_window_of_256_frames(engine, small_models, small):
     chunks = _chunks(x, steps, bt)
     engine.set_precision('fp32')
     outs, _ = _run_session(engine, _session_cfg(60.0, bt), chunks)
-    _compare_stream('session fp32 base-16, Tw 256', outs, _oracle_stream(small_models, 'speech-93', chunks, 60.0, stats, bt), 1e-3, 1e-3)
+    compare_stream_pulse_aware('session fp32 base-16, Tw 256', outs, _oracle_stream(small_models, 'speech-93', chunks, 60.0, stats, bt),
+                               _device_stream(engine, chunks, 60.0, bt), 'small', 'fp32')
 
 
 # ---- c. group -----------------------------------------------------------------------------------------------------------------
@@ -484,13 +373,13 @@ def test_group_members_pause_at_different_steps(engine, small_models, small):
     differ = sum(len({t[k][1] for t in tables}) > 1 for k in range(steps))
     assert differ >= steps // 2 and {b for t in tables for _, b, _ in t} == {1, 2, 3}, differ       # the members' buckets differ in most steps
     members = [_chunks(x, steps) for x in xs]
-    refs = [_oracle_stream(small_models, f'member-{i}', m, 60.0, stats) for i, m in enumerate(members)]
+    refs = [_oracle_stream(small_models, f'member-{i}', m, 60.0, stats).outs for i, m in enumerate(members)]
     for precision in ('fp32', 'fp16'):
         engine.set_precision(precision)
         grouped = _run_group(engine, _session_cfg(60.0), members)
         again = _run_group(engine, _session_cfg(60.0), members)
         for i in range(len(members)):
-            _compare_stream(f'group {precision} member {i}', grouped[i], refs[i], *((1e-6, 1e-6) if precision == 'fp32' else (1e-3, 2e-3)))
+            compare_stream(f'group {precision} member {i}', grouped[i], refs[i], *((1e-6, 1e-6) if precision == 'fp32' else (1e-3, 2e-3)))
             assert all(np.array_equal(a, b) for a, b in zip(grouped[i], again[i])), i       # the same group twice: bitwise
             alone, _ = _run_session(engine, _session_cfg(60.0), members[i])
             err = _rmse(np.concatenate(grouped[i]), np.concatenate(alone))

@@ -11,11 +11,14 @@ import pytest
 
 from realtime_yukarin_b200 import engine as eng
 
+from .session_geometry import stage2_cases
+
 W = 512
 
 # (Tp, keep_begin, keep_len): the session shapes at 0.1 / 0.3 / 1.0 s chunks with 0.5 s extras, 1.0 s chunks with 1.0 s extras,
-# and bands that touch the first and the last row
-CASES = [(256, 100, 20), (384, 100, 60), (512, 100, 200), (640, 200, 200), (384, 0, 60), (384, 324, 60), (128, 0, 30), (128, 90, 38)]
+# bands that touch the first and the last row, and the session geometries of tests/session_geometry.py (Tp 128 to 1920)
+CASES = ([(256, 100, 20), (384, 100, 60), (512, 100, 200), (640, 200, 200), (384, 0, 60), (384, 324, 60), (128, 0, 30), (128, 90, 38)]
+         + [c[:3] for c in stage2_cases()])
 
 
 def _tile_rows(Win):

@@ -6,12 +6,15 @@ import numpy as np
 import pytest
 
 from realtime_yukarin_b200 import engine as eng
+from tests.session_geometry import stage2_cases
 from tests.test_gpu_stage2_band import W, _load_stage2
 
 # (Tp, Tw, kept ranges): the session shapes at 0.3 s (headline), 0.1 s and 1.0 s chunks, a window whose third encoder layer
-# (split K) skips rows too, a kept band at the end of the window, and a group of two members with different kept rows
-CASES = [(384, 260, [(100, 60)]), (256, 220, [(100, 20)]), (512, 400, [(100, 200)]), (640, 400, [(200, 200)]),
-         (384, 300, [(240, 60)]), (384, 260, [(100, 60), (80, 100)])]
+# (split K) skips rows too, a kept band at the end of the window, a group of two members with different kept rows, and the session
+# geometries of tests/session_geometry.py (Tp 128 to 1920)
+CASES = ([(384, 260, [(100, 60)]), (256, 220, [(100, 20)]), (512, 400, [(100, 200)]), (640, 400, [(200, 200)]),
+          (384, 300, [(240, 60)]), (384, 260, [(100, 60), (80, 100)])]
+         + [(Tp, Tw, [(kb, kl)]) for Tp, kb, kl, Tw in stage2_cases()])
 
 
 def _padded_input(B, Tp, Tw, seed):
@@ -28,7 +31,8 @@ def test_tail_skip_forward_on_nan_buffers(engine, full_models, Tp, Tw, keeps):
     _load_stage2(engine, full_models)
     kb = min(k[0] for k in keeps)
     ke = max(k[0] + k[1] for k in keeps)
-    assert eng.stage2_tail_rows(Tp, W, Tw, kb, ke - kb)[:, 1].any()          # the case skips rows
+    # the case skips rows, unless one row of padding leaves no two rows equal (the forward must then be the full one)
+    assert eng.stage2_tail_rows(Tp, W, Tw, kb, ke - kb)[:, 1].any() == (Tp - Tw > 1)
     x = _padded_input(len(keeps), Tp, Tw, Tp * 1000 + Tw)
     full = engine.test_stage2_forward(x, mode=0)
     assert np.isfinite(full).all()

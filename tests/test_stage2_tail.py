@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 from realtime_yukarin_b200 import engine as eng
+from tests.session_geometry import stage2_cases
 from tests.test_gpu_stage2_band import CASES, W, _python_bands, _tile_rows
 
 CIN1_ROWS = 8          # output rows per CTA of the first layer's kernel (k_conv3x3_cin1)
@@ -75,13 +76,14 @@ def _python_tail(Tp, Tw, keep_begin, keep_len):
     return out
 
 
-def _tws(Tp):
-    return sorted({max(Tp - 128, 1), Tp - 64, Tp - 1})
+def _tws(Tp, kb, kl):
+    """windows padded to Tp: a whole block, half a block and one row of padding, and the session geometries' own"""
+    return sorted({max(Tp - 128, 1), Tp - 64, Tp - 1} | {c[3] for c in stage2_cases() if c[:3] == (Tp, kb, kl)})
 
 
 @pytest.mark.parametrize('Tp,kb,kl', CASES)
 def test_tail_table_matches_independent_walk(Tp, kb, kl):
-    for Tw in _tws(Tp):
+    for Tw in _tws(Tp, kb, kl):
         got = eng.stage2_tail_rows(Tp, W, Tw, kb, kl)
         want = _python_tail(Tp, Tw, kb, kl)
         assert np.array_equal(got, want), (Tw, got.tolist(), want.tolist())
