@@ -418,10 +418,12 @@ int ryk_test_stage2_forward(ryk_engine* e, int B, int Tp, int n_keep, const int*
                             const float* x, float* y);
 /* One conv (transposed = 0) or transposed-conv layer of the U-Nets in isolation, host fp32 NHWC tensors in and
  * out, weights in the Chainer layout; use_tc selects the FP16 wgmma kernel (1) or the FP32 CUDA-core kernel (0).
- * `repeat` extra timed runs report the mean device time per run (ms) -- used by the unit parity tests and ncu. */
+ * `repeat` extra timed runs report the mean device time per run (ms) -- used by the unit parity tests and ncu.
+ * ksplit_tiles > 0 makes the wgmma kernel split K as for a layer of that many output tiles (0: the layer's own count);
+ * *ksplit (may be NULL) receives the split factor the wgmma kernel ran with. */
 int ryk_test_conv_layer(ryk_engine* e, int transposed, int k, int stride, int pad, int B, int Hin, int Win, int C0, int C1, int Cout,
                         const float* in0, const float* in1, const float* W, const float* scale, const float* shift, int act,
-                        int use_tc, int repeat, float* out, float* ms_per_run);
+                        int use_tc, int repeat, int ksplit_tiles, float* out, float* ms_per_run, int* ksplit);
 /* CREPE convolutions with an explicit back-end: 0 = the FP32 CUDA-core kernel (ryk_crepe_predict, sessions in precision 0),
  * 1 = the 3xTF32 tensor-core kernel (sessions in precision 1).
  * ryk_crepe_test_conv: one layer in isolation, x [F][Win][Cin], W (Cout, Cin, k), stride 1, no padding ->

@@ -839,7 +839,7 @@ int ryk_stage2_tail_rows(int Tp, int W, int Tw, int keep_begin, int keep_len, in
   return 0;
 }
 
-// One stage-2 forward on a fresh plan whose buffers (activations, split-K workspaces, output) are first filled with NaN, so that
+// One stage-2 forward on a fresh plan whose buffers (activations, output) are first filled with NaN, so that
 // a row the banded decoder reads without having computed it shows up in the output.  x, y: host [B][Tp][512] float32 (network
 // input and output, the log-spectrum without its last bin).  mode 0: full plan; 1: banded plan for the hull of the n_keep row
 // ranges [keep_begin[i], keep_begin[i] + keep_len[i]); 2: as 1, with each banded layer split along K as in the full plan; 3: as 2, with
@@ -876,15 +876,16 @@ int ryk_test_stage2_forward(ryk_engine* h, int B, int Tp, int n_keep, const int*
 
 // ---- diagnostics: one conv / transposed-conv layer in isolation (unit parity + profiling) -------
 // in0/in1: host fp32 NHWC [B][Hin][Win][C0|C1]; W: Chainer layout; out: host fp32 NHWC [B][Hout][Wout][Cout].
-// use_tc = 1 runs the FP16 wgmma kernel (activations rounded to fp16), 0 the FP32 CUDA-core kernel.
+// use_tc = 1 runs the FP16 wgmma kernel (activations rounded to fp16), 0 the FP32 CUDA-core kernel.  ksplit_tiles > 0: the wgmma
+// kernel splits K as for a layer of that many output tiles; *ksplit (may be NULL) receives the split factor it ran with.
 int ryk_test_conv_layer(ryk_engine* h, int transposed, int k, int stride, int pad, int B, int Hin, int Win, int C0, int C1, int Cout,
                         const float* in0, const float* in1, const float* W, const float* scale, const float* shift, int act,
-                        int use_tc, int repeat, float* out, float* ms_per_run) {
+                        int use_tc, int repeat, int ksplit_tiles, float* out, float* ms_per_run, int* ksplit) {
   Engine* e = E(h);
   RYK_CUDA(cudaSetDevice(e->device));
   cudaStream_t st = e->stream;
   ConvLayer L;
-  L.transposed = transposed; L.B = B; L.Hin = Hin; L.Win = Win; L.C0 = C0; L.C1 = C1; L.Cout = Cout;
+  L.transposed = transposed; L.B = B; L.Hin = Hin; L.Win = Win; L.C0 = C0; L.C1 = C1; L.Cout = Cout; L.ksplit_tiles = ksplit_tiles;
   L.KH = L.KW = k; L.SH = L.SW = stride; L.PH = L.PW = pad; L.act = act;
   if (Hin == 1) { L.KH = 1; L.SH = 1; L.PH = 0; }      // 1-D layer (stage-1 nets): kernel (1 x k), stride (1, s), padding (0, p)
   if (transposed) { L.Hout = (Hin - 1) * L.SH + L.KH - 2 * L.PH; L.Wout = (Win - 1) * stride + k - 2 * pad; }
@@ -935,8 +936,6 @@ int ryk_test_conv_layer(ryk_engine* h, int transposed, int k, int stride, int pa
     RYK_CHECK(tc_layer_eligible(L), "layer shape is not eligible for the tensor-core kernel");
     int num_sms = 132;
     cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, e->device);
-    size_t ws = tc_splitk_ws_bytes(L, num_sms);
-    if (ws) L.splitk_ws = (float*)A(ws);
     if (tc_layer_prepare(L, num_sms)) return -1;
     rc = conv_tc_run(L, st);
     if (!rc && repeat > 0) rc = timed_graph([&]() { return conv_tc_run(L, st); });
@@ -965,6 +964,7 @@ int ryk_test_conv_layer(ryk_engine* h, int transposed, int k, int stride, int pa
   float ms = 0.f;
   if (!rc && repeat > 0) { cudaEventElapsedTime(&ms, ev0, ev1); ms /= repeat; }
   if (ms_per_run) *ms_per_run = ms;
+  if (ksplit) *ksplit = L.ksplit;
   cudaEventDestroy(ev0); cudaEventDestroy(ev1);
   for (void* p : frees) cudaFree(p);
   return rc;

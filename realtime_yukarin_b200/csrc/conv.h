@@ -54,10 +54,9 @@ struct ConvLayer {
   // tensor-core path (filled by tc_layer_prepare)
   const __half* w_tc[kMaxGroupVoices] = {};   // per voice; conv: [Cout][KH*KW*Cin]; deconv: [4 classes][Cout][4*Cin]
   const __half* w_frag = nullptr;         // 1-D k4 layers: mma.sync B-fragment order for the fused stage-1 kernel (s1_map.h)
-  float* splitk_ws = nullptr;             // [ksplit][B][band's output rows][Wout][Cout] fp32 when ksplit > 1
-  int ksplit = 1;
+  int ksplit = 1;                         // > 1: the K splits of one output tile run as one thread-block cluster
   int ksplit_tiles = 0;                   // > 0: split K as for a layer of this many output tiles instead of the band's own count
-  CUtensorMap tmA0, tmA1, tmO, tmW;       // inputs, fp16 output, fp32 split-K workspace
+  CUtensorMap tmA0, tmA1, tmO;            // inputs, fp16 output
   TcWeightMaps tmB;                       // weights, per voice
   int tile_w = 0, tile_h = 0;             // pixel tile = tile_w x tile_h = 128
   int block_n = 0;
@@ -92,7 +91,6 @@ int tc_init();                                           // resolves cuTensorMap
 int tc_layer_prepare(ConvLayer& L, int num_sms);         // builds tensor maps, picks tiles / split-K (needs final pointers)
 int tc_layer_weight_maps(ConvLayer& L);                  // (re)builds the weight maps of voices 0 .. n_voices - 1 of a prepared layer
 int conv_tc_run(const ConvLayer& L, cudaStream_t st);
-size_t tc_splitk_ws_bytes(const ConvLayer& L, int num_sms);
 int tc_tile_rows(const ConvLayer& L);                    // class-local output rows per tile of the tensor-core kernel
 int tc_tile_count(const ConvLayer& L);                   // output tiles (all classes, all N blocks) of the layer's band
 

@@ -18,7 +18,9 @@
 //                                       next stage's MMAs are issued; then folded BN scale/shift + LeakyReLU/ReLU,
 //                                       FP16 staging in the idle stage buffers, TMA store)
 // * Small-M bottleneck layers are weight-bandwidth bound: split-K over blockIdx.z spreads the weight
-//   stream over all SMs; partial sums meet in an FP32 workspace and a reduce kernel applies the epilogue.
+//   stream over all SMs.  The ksplit CTAs of one tile run as one thread-block cluster: each stages its FP32 partial tile in its
+//   own shared memory, and each reduces a share of the tile's pixels over all ranks' partials through distributed shared memory
+//   (splitk_sum fixes the order) before applying the epilogue.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 
@@ -32,18 +34,16 @@ struct TcParams {
   int Hc, Wc;                    // class-local output grid (== Hout, Wout for convs)
   int tile_w, tile_h, tiles_w, tiles_h;  // tiles_h: tile rows of the band, which starts at tile row th0
   int th0;
-  int skip_t0, skip_tn;          // tile rows [skip_t0, skip_t0 + skip_tn) are not launched (padded tail); the workspace omits them
+  int skip_t0, skip_tn;          // tile rows [skip_t0, skip_t0 + skip_tn) are not launched (padded tail)
   int run_y0, run_y1;            // rows [run_y0, run_y1) of source 0 repeat row run_y0: a box wholly inside them reads from run_y0
-  int ws_y0;                     // output row of the band's first row: row 0 of the split-K workspace
   int chunks0, chunks1;          // 64-channel chunks of source 0 / 1
   int taps_w, ntaps;             // taps per class: conv KH*KW (taps_w = KW); deconv (KH/SH)*(KW/SW)
   int sh, sw, ph, pw;            // conv stride / padding per dimension (1-D nets: sh = 1, ph = 0)
   int classes_w;                 // deconv output-parity classes along W (SW); along H it is SH
-  int ksplit, chunks_per_split;
+  int ksplit, chunks_per_split;  // ksplit > 1: the grid runs in clusters of (1, 1, ksplit), one tile's K splits each
   int act;
   LayerWeights wt;               // per-voice scale / shift and the voice of each batch item (weights: the per-voice tensor maps)
-  float* ws;                     // split-K workspace [ksplit][pixels][Cout] or nullptr
-  size_t out_pixels;             // B * Hout * Wout
+  __half* out;                   // NHWC [B][Hout][Wout][Cout]: split-K layers store their reduced tiles here directly
 };
 
 template <int BLOCK_N>
@@ -52,11 +52,42 @@ __device__ __forceinline__ void wgmma_tile(float (&acc)[BLOCK_N / 2], uint64_t a
   else wgmma_m64n64(acc, adesc, bdesc);
 }
 
+// Largest split-K factor: one cluster holds one tile's splits, and 16 CTAs is the largest (non-portable) cluster of sm_90.
+constexpr int kMaxSplits = 16;
+
+__device__ __forceinline__ void add4(float4& a, const float4& b) { a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w; }
+
+// The split-K summation order.  This is a contract: it fixes the FP32 rounding of every split layer's outputs, so the network's
+// results are bitwise the same however the splits are scheduled.  v[s] is split s's partial sum, s < ks <= kMaxSplits.
+//   ks <= 4: a = v[0]; a += v[1]; ...; a += v[ks - 1]
+//   ks >  4: part[g] = 0.f; part[g] += v[g]; part[g] += v[g + 8] (terms with index >= ks left out), g = 0..7;
+//            a = part[0]; a += part[1]; ...; a += part[7]
+__device__ __forceinline__ float4 splitk_sum(const float4 (&v)[kMaxSplits], int ks) {
+  float4 a = v[0];
+  if (ks <= 4) {
+#pragma unroll
+    for (int s = 1; s < 4; ++s) if (s < ks) add4(a, v[s]);
+    return a;
+  }
+#pragma unroll
+  for (int g = 0; g < 8; ++g) {
+    float4 part = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (g < ks) add4(part, v[g]);
+    if (g + 8 < ks) add4(part, v[g + 8]);
+    if (g == 0) a = part; else add4(a, part);
+  }
+  return a;
+}
+
+// Byte offset of 16-byte chunk c (4 channels) of tile row (pixel) `row` in a split CTA's FP32 partial tile [128][BLOCK_N]; the
+// chunk index is XOR-swizzled by row so that both the accumulator stores and the reducers' row reads spread over all banks.
+template <int BLOCK_N>
+__device__ __forceinline__ uint32_t partial_offset(int row, int c) { return (uint32_t)(row * BLOCK_N * 4 + ((c ^ (row & 7)) << 4)); }
+
 template <int BLOCK_N, int kStages, int kMinBlocks>
 __global__ void __launch_bounds__(kTcThreads, kMinBlocks)
 k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-          const __grid_constant__ TcWeightMaps tmB, const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmW,
-          const __grid_constant__ TcParams p) {
+          const __grid_constant__ TcWeightMaps tmB, const __grid_constant__ CUtensorMap tmO, const __grid_constant__ TcParams p) {
   static_assert(BLOCK_N == 64 || BLOCK_N == 128, "BLOCK_N");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   constexpr uint32_t kABytes = kBlockM * kBlockK * 2;
@@ -79,8 +110,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
   int mt = blockIdx.x;
   const int tw = mt % p.tiles_w; mt /= p.tiles_w;
   int th = mt % p.tiles_h + p.th0; mt /= p.tiles_h;
-  const bool past_skip = th >= p.skip_t0;
-  th += past_skip ? p.skip_tn : 0;
+  th += th >= p.skip_t0 ? p.skip_tn : 0;
   const int b = mt;
   const int n0 = blockIdx.y * BLOCK_N;
   const int cls = blockIdx.z / p.ksplit, split = blockIdx.z % p.ksplit;
@@ -98,12 +128,11 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA0) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(tmBv) : "memory");
     if (p.chunks1 > 0) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA1) : "memory");
-    if (!p.ws) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
-    else asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW) : "memory");
+    if (p.ksplit == 1) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
     for (int i = 0; i < kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kTcConsumers / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (threadIdx.x < kTcConsumers && !p.ws) {
+  if (threadIdx.x < kTcConsumers) {
     const float* scale = p.wt.scale[voice]; const float* shift = p.wt.shift[voice];
     for (int i = threadIdx.x; i < BLOCK_N; i += kTcConsumers) { s_scale[i] = __ldg(scale + n0 + i); s_shift[i] = __ldg(shift + n0 + i); }
   }
@@ -136,6 +165,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
         tma_load_2d(smem_b + s * kBBytes, tmBv, &full_bar[s], kc * kBlockK, cls * p.Cout + n0);
       }
     }
+    if (p.ksplit > 1) { cluster_sync_all(); cluster_sync_all(); }     // the split epilogue's two cluster barriers count every thread
   } else if (warp < kTcConsumers / 32) {
     // ===== MMA: warpgroup g owns accumulator rows (tile pixels) 64 g .. 64 g + 63 =====
     const int g = threadIdx.x >> 7, wl = warp & 3, lane = threadIdx.x & 31;
@@ -166,27 +196,60 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
     asm volatile("bar.sync 1, %0;" ::"n"(kTcConsumers) : "memory");
     const int rbase = g * 64 + wl * 16 + (lane >> 2);           // tile rows of registers i with ((i >> 1) & 1) == 0; +8 for the others
     const int cq = 2 * (lane & 3);
-    // (out-of-range pixels of ragged tiles need no masking: both TMA stores below clip at the tensor-map bounds)
+    if (p.ksplit > 1) {
+      // split-K: this split's raw FP32 partial tile -> its own stage buffers; the cluster's ranks then each reduce a share of the
+      // tile's valid pixels over every rank's partial
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; i += 2) {
+        const int row = rbase + 8 * ((i >> 1) & 1);
+        const int col = 8 * (i >> 2) + cq;
+        *reinterpret_cast<float2*>(smem + partial_offset<BLOCK_N>(row, col >> 2) + (col & 3) * 4) = make_float2(acc[i], acc[i + 1]);
+      }
+      cluster_sync_all();                                          // every rank's partial is in its shared memory
+      // valid pixels of the tile: ragged tiles end at the class-local grid's last row / column
+      const int vw = min(p.tile_w, p.Wc - ox0), vh = min(p.tile_h, p.Hc - oy0);
+      constexpr int kChunks = BLOCK_N / 4;
+      const int total = vw * vh * kChunks;
+      const int j1 = (int)((long long)total * (split + 1) / p.ksplit);
+      const uint32_t partial = smem_u32(smem);
+      for (int j = (int)((long long)total * split / p.ksplit) + threadIdx.x; j < j1; j += kTcConsumers) {
+        const int q = j / kChunks, c = j - q * kChunks;
+        const int y = q / vw, x = q - y * vw;
+        const uint32_t off = partial + partial_offset<BLOCK_N>(y * p.tile_w + x, c);
+        float4 v[kMaxSplits];
+#pragma unroll
+        for (int s = 0; s < kMaxSplits; ++s)
+          if (s < p.ksplit) v[s] = ld_cluster_f4(cluster_map(off, s));
+        const float4 a = splitk_sum(v, p.ksplit);
+        const int n = 4 * c;
+        float o[4] = {fmaf(a.x, s_scale[n], s_shift[n]), fmaf(a.y, s_scale[n + 1], s_shift[n + 1]),
+                      fmaf(a.z, s_scale[n + 2], s_shift[n + 2]), fmaf(a.w, s_scale[n + 3], s_shift[n + 3])};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          if (p.act == ACT_LEAKY) o[k] = o[k] > 0.f ? o[k] : 0.2f * o[k]; else if (p.act == ACT_RELU) o[k] = fmaxf(o[k], 0.f);
+        }
+        const int ys = p.transposed ? (oy0 + y) * p.sh + py : oy0 + y;
+        const int xs = p.transposed ? (ox0 + x) * p.sw + px : ox0 + x;
+        __half2 h0 = __floats2half2_rn(o[0], o[1]), h1 = __floats2half2_rn(o[2], o[3]);
+        *reinterpret_cast<uint2*>(p.out + (((size_t)b * p.Hout + ys) * p.Wout + xs) * p.Cout + n0 + n) =
+            make_uint2(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1));
+      }
+      cluster_sync_all();                                          // the peers have read this CTA's partial: its shared memory may go
+      return;
+    }
+    // (out-of-range pixels of ragged tiles need no masking: the TMA store below clips at the tensor-map bounds)
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; i += 2) {
       const int row = rbase + 8 * ((i >> 1) & 1);
       const int col = 8 * (i >> 2) + cq;
-      const float a0 = acc[i], a1 = acc[i + 1];
-      if (p.ws) {
-        // split-K partial tile (raw FP32 sums) -> 128B-swizzled [128 pixels][32 channels] blocks, stored below by TMA into this
-        // split's slice of the workspace; k_splitk_reduce sums the slices
-        uint8_t* blk = smem + (col >> 5) * (kBlockM * 128) + row * 128;
-        *reinterpret_cast<float2*>(blk + ((((col & 31) >> 2) ^ (row & 7)) << 4) + (col & 3) * 4) = make_float2(a0, a1);
-      } else {
-        // scale/shift/activation -> FP16 -> 128B-swizzled [128 pixels][64 channels] blocks; one TMA store per block writes full
-        // 128-byte rows
-        float v0 = fmaf(a0, s_scale[col], s_shift[col]);
-        float v1 = fmaf(a1, s_scale[col + 1], s_shift[col + 1]);
-        if (p.act == ACT_LEAKY) { v0 = v0 > 0.f ? v0 : 0.2f * v0; v1 = v1 > 0.f ? v1 : 0.2f * v1; }
-        else if (p.act == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-        uint8_t* blk = smem + (col >> 6) * (kBlockM * 128) + row * 128;
-        *reinterpret_cast<__half2*>(blk + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2) = __floats2half2_rn(v0, v1);
-      }
+      // scale/shift/activation -> FP16 -> 128B-swizzled [128 pixels][64 channels] blocks; one TMA store per block writes full
+      // 128-byte rows
+      float v0 = fmaf(acc[i], s_scale[col], s_shift[col]);
+      float v1 = fmaf(acc[i + 1], s_scale[col + 1], s_shift[col + 1]);
+      if (p.act == ACT_LEAKY) { v0 = v0 > 0.f ? v0 : 0.2f * v0; v1 = v1 > 0.f ? v1 : 0.2f * v1; }
+      else if (p.act == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+      uint8_t* blk = smem + (col >> 6) * (kBlockM * 128) + row * 128;
+      *reinterpret_cast<__half2*>(blk + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2) = __floats2half2_rn(v0, v1);
     }
     if (my_chunks > 0) {
       // generic-proxy smem writes -> visible to the async proxy; one thread hands the tile to the TMA unit
@@ -195,18 +258,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
       if (threadIdx.x == 0) {
         const int xs = p.transposed ? ox0 * p.sw + px : ox0;
         const int ys = p.transposed ? oy0 * p.sh + py : oy0;
-        if (!p.ws) {
 #pragma unroll
-          for (int jb = 0; jb < BLOCK_N / 64; ++jb)
-            asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                         ::"l"(&tmO), "r"(smem_u32(smem + jb * (kBlockM * 128))), "r"(n0 + jb * 64), "r"(xs), "r"(ys), "r"(b) : "memory");
-        } else {
-#pragma unroll
-          for (int jb = 0; jb < BLOCK_N / 32; ++jb)
-            asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
-                         ::"l"(&tmW), "r"(smem_u32(smem + jb * (kBlockM * 128))), "r"(n0 + jb * 32), "r"(xs),
-                         "r"(ys - p.ws_y0 - (past_skip ? p.skip_tn * p.tile_h : 0)), "r"(b), "r"(split) : "memory");
-        }
+        for (int jb = 0; jb < BLOCK_N / 64; ++jb)
+          asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                       ::"l"(&tmO), "r"(smem_u32(smem + jb * (kBlockM * 128))), "r"(n0 + jb * 64), "r"(xs), "r"(ys), "r"(b) : "memory");
         asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
       }
@@ -214,81 +269,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
   }
 }
 
-// split-K reduce + epilogue: out = act((sum over splits of ws[s]) * scale + shift) as fp16, 4 channels per thread.
-// The workspace holds the layer's row band: band4 float4s per batch item, written to out at out_off4 + b * out_stride4 (float4 units).
-// Block = G warps x 32 lanes: lane = one float4 of the output (512 contiguous bytes per warp load), warp g sums the
-// slices g, g + G, g + 2G, ... ; the G partial sums are combined through shared memory in a fixed order, so the result
-// is deterministic (same summation tree every run) while G x more loads are in flight than with one thread per output.
-__global__ void __launch_bounds__(256) k_splitk_reduce(const float* __restrict__ ws, size_t total4, size_t slice_elems, int ksplit, int Cout,
-                                const __grid_constant__ LayerWeights wt, int act, __half* __restrict__ out,
-                                size_t band4, size_t out_stride4, size_t out_off4, size_t gap_at4, size_t gap4) {
-  __shared__ float4 part[8][32];
-  pdl_trigger();
-  pdl_wait();
-  const int lane = threadIdx.x & 31, g = threadIdx.x >> 5, G = blockDim.x >> 5;
-  const size_t i = (size_t)blockIdx.x * 32 + lane;
-  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (i < total4) {
-    const float4* p = reinterpret_cast<const float4*>(ws) + i;
-    const size_t stride4 = slice_elems / 4;
-#pragma unroll 4
-    for (int s = g; s < ksplit; s += G) {
-      const float4 b = __ldg(p + (size_t)s * stride4);
-      a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
-    }
-  }
-  part[g][lane] = a;
-  __syncthreads();
-  if (g != 0 || i >= total4) return;
-  for (int k = 1; k < G; ++k) { const float4 b = part[k][lane]; a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w; }
-  const size_t item = i / band4;
-  const size_t r = i % band4, o = item * out_stride4 + out_off4 + r + (r >= gap_at4 ? gap4 : 0);
-  const int n = (int)((o * 4) % Cout);
-  const int voice = item_voice(wt, (int)item);
-  const float* scale = wt.scale[voice]; const float* shift = wt.shift[voice];
-  const float4 sc = __ldg(reinterpret_cast<const float4*>(scale + n)), sh = __ldg(reinterpret_cast<const float4*>(shift + n));
-  float v[4] = {fmaf(a.x, sc.x, sh.x), fmaf(a.y, sc.y, sh.y), fmaf(a.z, sc.z, sh.z), fmaf(a.w, sc.w, sh.w)};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    if (act == ACT_LEAKY) v[j] = v[j] > 0.f ? v[j] : 0.2f * v[j]; else if (act == ACT_RELU) v[j] = fmaxf(v[j], 0.f);
-  }
-  __half2 h0 = __floats2half2_rn(v[0], v[1]), h1 = __floats2half2_rn(v[2], v[3]);
-  reinterpret_cast<uint2*>(out)[o] = make_uint2(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1));
-}
-
-// few splits, large outputs (c3 / c4 / d3): one thread per float4 of the output, grid-stride, all slices summed in order
-__global__ void __launch_bounds__(256) k_splitk_reduce_few(const float* __restrict__ ws, size_t total4, size_t slice_elems, int ksplit, int Cout,
-                                    const __grid_constant__ LayerWeights wt, int act, __half* __restrict__ out,
-                                    size_t band4, size_t out_stride4, size_t out_off4, size_t gap_at4, size_t gap4) {
-  const size_t stride4 = slice_elems / 4;
-  pdl_trigger();
-  pdl_wait();
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total4; i += (size_t)gridDim.x * blockDim.x) {
-    const float4* p = reinterpret_cast<const float4*>(ws) + i;
-    float4 a = __ldg(p);
-#pragma unroll 4
-    for (int s = 1; s < ksplit; ++s) {
-      const float4 b = __ldg(p + (size_t)s * stride4);
-      a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
-    }
-    const size_t item = i / band4;
-    const size_t r = i % band4, o = item * out_stride4 + out_off4 + r + (r >= gap_at4 ? gap4 : 0);
-    const int n = (int)((o * 4) % Cout);
-    const int voice = item_voice(wt, (int)item);
-    const float* scale = wt.scale[voice]; const float* shift = wt.shift[voice];
-    const float4 sc = __ldg(reinterpret_cast<const float4*>(scale + n)), sh = __ldg(reinterpret_cast<const float4*>(shift + n));
-    float v[4] = {fmaf(a.x, sc.x, sh.x), fmaf(a.y, sc.y, sh.y), fmaf(a.z, sc.z, sh.z), fmaf(a.w, sc.w, sh.w)};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      if (act == ACT_LEAKY) v[j] = v[j] > 0.f ? v[j] : 0.2f * v[j]; else if (act == ACT_RELU) v[j] = fmaxf(v[j], 0.f);
-    }
-    __half2 h0 = __floats2half2_rn(v[0], v[1]), h1 = __floats2half2_rn(v[2], v[3]);
-    reinterpret_cast<uint2*>(out)[o] = make_uint2(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1));
-  }
-}
-
 // ------------------------------------------------------------------------------------ host side
 static PFN_cuTensorMapEncodeTiled_v12000 g_encode = nullptr;
+// g_clusters[ks]: clusters of (1, 1, ks) k_conv_tc CTAs the device holds at once (the smaller of the two kernel configurations)
+static int g_clusters[kMaxSplits + 1] = {};
 
 template <int BN, int ST> static constexpr size_t tc_smem_bytes() {
   return (size_t)ST * (kBlockM * kBlockK * 2 + BN * kBlockK * 2) + 2 * ST * 8 + 16 + 1024 + 2 * BN * 4 + 32;
@@ -308,8 +292,26 @@ int tc_init() {
   }
   RYK_CUDA(cudaFuncSetAttribute(RYK_TC_N128, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<128, 3>()));
   RYK_CUDA(cudaFuncSetAttribute(RYK_TC_N64, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<64, 4>()));
+  RYK_CUDA(cudaFuncSetAttribute(RYK_TC_N128, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+  RYK_CUDA(cudaFuncSetAttribute(RYK_TC_N64, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+  if (g_clusters[1] == 0) {
+    auto active = [](auto kernel, size_t smem, int ks) {
+      cudaLaunchConfig_t cfg = {};
+      cfg.gridDim = dim3(1, 1, ks); cfg.blockDim = dim3(kTcThreads); cfg.dynamicSmemBytes = smem;
+      cudaLaunchAttribute at[1];
+      at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = ks;
+      cfg.attrs = at; cfg.numAttrs = 1;
+      int n = 0;
+      if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
+      return n;
+    };
+    for (int ks = 1; ks <= kMaxSplits; ++ks)
+      g_clusters[ks] = std::min(active(RYK_TC_N128, tc_smem_bytes<128, 3>(), ks), active(RYK_TC_N64, tc_smem_bytes<64, 4>(), ks));
+    RYK_CHECK(g_clusters[1] > 0, "the tensor-core convolution kernel does not fit an SM");
+  }
   return 0;
 }
+
 
 bool tc_layer_eligible(const ConvLayer& L) {
   const bool k2d = L.KH == 4 && L.KW == 4 && L.SH == 2 && L.SW == 2 && L.PH == 1 && L.PW == 1;
@@ -332,20 +334,6 @@ static int make_act_map(CUtensorMap* m, const void* ptr, int C, int W, int H, in
                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(activation) failed: " + std::to_string((int)r)); return -1; }
-  return 0;
-}
-
-// split-K workspace [ksplit][B][Hout][Wout][Cout] fp32 as a 5-D map: box = (32 channels, tile_w, tile_h, 1, 1) with the same
-// W / H element strides as the output map (deconv parity classes write every other pixel)
-static int make_ws_map(CUtensorMap* m, const void* ptr, int C, int W, int H, int B, int ksplit, int box_w, int box_h, int stride_w, int stride_h) {
-  cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B, (cuuint64_t)ksplit};
-  cuuint64_t strides[4] = {(cuuint64_t)C * 4, (cuuint64_t)W * C * 4, (cuuint64_t)H * W * C * 4, (cuuint64_t)B * H * W * C * 4};
-  cuuint32_t box[5] = {32, (cuuint32_t)(box_w * stride_w), (cuuint32_t)(box_h * stride_h), 1, 1};
-  cuuint32_t estr[5] = {1, (cuuint32_t)stride_w, (cuuint32_t)stride_h, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<void*>(ptr), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(split-K workspace) failed: " + std::to_string((int)r)); return -1; }
   return 0;
 }
 
@@ -380,7 +368,10 @@ int tc_tile_count(const ConvLayer& L) {
 }
 
 // Tile shape, N block and split-K of a layer.  Split-K fills the SMs when the band has few tiles, so a banded layer may split
-// K further than the same layer over every row (L.ksplit_tiles overrides the tile count this rule sees).
+// K further than the same layer over every row (L.ksplit_tiles overrides the tile count this rule sees).  One tile's splits run as one
+// thread-block cluster, and ks is lowered until the device holds all of the layer's clusters at once: a cluster is placed inside
+// one GPC, so the CTA slots left over in each GPC do not add up (an H100 SXM holds 14 clusters of 16 and 30 of 8, fewer than its
+// 264 slots suggest; a layer whose clusters do not all fit would run a second wave of them).
 static void tc_geometry(const ConvLayer& L, int num_sms, int* tile_w, int* tile_h, int* block_n, int* ksplit) {
   int tw, th;
   tc_tile_shape(L, &tw, &th);
@@ -394,29 +385,13 @@ static void tc_geometry(const ConvLayer& L, int num_sms, int* tile_w, int* tile_
     constexpr int kMinChunks = 8;                       // at least this many K chunks per split
     ks = slots / tiles;
     if (ks > total_chunks / kMinChunks) ks = total_chunks / kMinChunks;
+    if (ks > kMaxSplits) ks = kMaxSplits;
     if (ks < 1) ks = 1;
+    while (ks > 1 && tiles > g_clusters[ks]) --ks;
     int cps = (total_chunks + ks - 1) / ks;
     ks = (total_chunks + cps - 1) / cps;                // every split owns at least one chunk
   }
   *tile_w = tw; *tile_h = th; *block_n = bn; *ksplit = ks;
-}
-
-// Rows of one batch item in the split-K workspace: the band's output rows [r0, r1) less the skipped tail rows, which leave a gap of
-// `gap` rows after workspace row `gap_at` (workspace row w holds output row r0 + w, or r0 + w + gap from gap_at on).
-static int tc_ws_rows(const ConvLayer& L, int* r0, int* gap_at, int* gap) {
-  int r1;
-  layer_band_out_rows(L, r0, &r1);
-  *gap = L.skip_y1 - L.skip_y0;
-  *gap_at = *gap ? L.skip_y0 - *r0 : 0;
-  return r1 - *r0 - *gap;
-}
-
-size_t tc_splitk_ws_bytes(const ConvLayer& L, int num_sms) {
-  int tw, th, bn, ks;
-  tc_geometry(L, num_sms, &tw, &th, &bn, &ks);
-  int r0, gap_at, gap;
-  const int rows = tc_ws_rows(L, &r0, &gap_at, &gap);
-  return ks > 1 ? (size_t)ks * L.B * rows * L.Wout * L.Cout * sizeof(float) : 0;
 }
 
 int tc_layer_weight_maps(ConvLayer& L) {
@@ -443,30 +418,25 @@ int tc_layer_prepare(ConvLayer& L, int num_sms) {
   if (tc_layer_weight_maps(L)) return -1;
   // output map for the TMA-store epilogue: deconv classes write every other pixel (element strides = conv strides)
   if (make_act_map(&L.tmO, L.out, L.Cout, L.Wout, L.Hout, L.B, L.tile_w, L.tile_h, L.transposed ? L.SW : 1, L.transposed ? L.SH : 1)) return -1;
-  RYK_CHECK(L.ksplit == 1 || L.splitk_ws != nullptr, "split-K layer without a workspace");
   RYK_CHECK(L.band_y0 >= 0 && L.band_y0 % L.tile_h == 0 && L.band_y0 < layer_band_end(L) && layer_band_end(L) <= layer_class_rows(L) &&
             (layer_band_end(L) % L.tile_h == 0 || layer_band_end(L) == layer_class_rows(L)), "row band is not a range of whole tile rows");
   RYK_CHECK(L.skip_y1 == 0 || (!L.transposed && L.skip_y0 % L.tile_h == 0 && L.skip_y1 % L.tile_h == 0 && L.band_y0 <= L.skip_y0 &&
                                L.skip_y0 < L.skip_y1 && L.skip_y1 <= layer_band_end(L)),
             "skipped rows are not a range of whole tile rows inside the band of a convolution");
-  if (L.ksplit > 1) {
-    // the workspace holds the band's computed output rows only
-    int r0, gap_at, gap;
-    const int rows = tc_ws_rows(L, &r0, &gap_at, &gap);
-    if (make_ws_map(&L.tmW, L.splitk_ws, L.Cout, L.Wout, rows, L.B, L.ksplit, L.tile_w, L.tile_h, L.transposed ? L.SW : 1, L.transposed ? L.SH : 1)) return -1;
-  } else L.tmW = L.tmO;
   L.tc_ready = true;
   return 0;
 }
 
-// Launch with the programmatic-stream-serialization attribute (see pdl_trigger / pdl_wait).
+// Launch with the programmatic-stream-serialization attribute (see pdl_trigger / pdl_wait) and, for cluster_z > 1, in clusters of
+// (1, 1, cluster_z) CTAs.
 template <typename... KArgs, typename... Args>
-static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, int cluster_z, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
+  cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
+  attr[1].id = cudaLaunchAttributeClusterDimension; attr[1].val.clusterDim.x = 1; attr[1].val.clusterDim.y = 1; attr[1].val.clusterDim.z = cluster_z;
+  cfg.attrs = attr; cfg.numAttrs = cluster_z > 1 ? 2 : 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
@@ -482,9 +452,6 @@ int conv_tc_run(const ConvLayer& L, cudaStream_t st) {
   p.tiles_w = (p.Wc + L.tile_w - 1) / L.tile_w; p.tiles_h = (layer_band_end(L) - L.band_y0 + L.tile_h - 1) / L.tile_h - p.skip_tn;
   p.th0 = L.band_y0 / L.tile_h;
   p.run_y0 = L.run_y0; p.run_y1 = L.run_y1;
-  int r0, gap_at, gap;
-  const int ws_rows = tc_ws_rows(L, &r0, &gap_at, &gap);
-  p.ws_y0 = r0;
   p.chunks0 = L.C0 / kBlockK; p.chunks1 = L.C1 / kBlockK;
   p.taps_w = L.transposed ? L.KW / L.SW : L.KW;
   p.ntaps = L.transposed ? (L.KH / L.SH) * (L.KW / L.SW) : L.KH * L.KW;
@@ -495,27 +462,12 @@ int conv_tc_run(const ConvLayer& L, cudaStream_t st) {
   int total_chunks = p.ntaps * (p.chunks0 + p.chunks1);
   p.chunks_per_split = (total_chunks + L.ksplit - 1) / L.ksplit;
   p.act = L.act; p.wt = L.wt;
-  p.ws = L.ksplit > 1 ? L.splitk_ws : nullptr;
-  p.out_pixels = (size_t)L.B * L.Hout * L.Wout;
-  const size_t row_elems = (size_t)L.Wout * L.Cout;
-  const size_t band_elems = (size_t)L.B * ws_rows * row_elems;        // one workspace slice
+  p.out = (__half*)L.out;
+  // blockIdx.z = class * ksplit + split: one cluster of ksplit consecutive z is one tile's splits, and a CTA's rank in it is its split
   dim3 grid(L.B * p.tiles_w * p.tiles_h, L.Cout / L.block_n, classes * L.ksplit);
-  if (L.block_n == 128) RYK_CUDA(launch_pdl(RYK_TC_N128, grid, dim3(kTcThreads), tc_smem_bytes<128, 3>(), st, L.tmA0, L.tmA1, L.tmB, L.tmO, L.tmW, p));
-  else RYK_CUDA(launch_pdl(RYK_TC_N64, grid, dim3(kTcThreads), tc_smem_bytes<64, 4>(), st, L.tmA0, L.tmA1, L.tmB, L.tmO, L.tmW, p));
+  if (L.block_n == 128) RYK_CUDA(launch_pdl(RYK_TC_N128, grid, dim3(kTcThreads), tc_smem_bytes<128, 3>(), st, L.ksplit, L.tmA0, L.tmA1, L.tmB, L.tmO, p));
+  else RYK_CUDA(launch_pdl(RYK_TC_N64, grid, dim3(kTcThreads), tc_smem_bytes<64, 4>(), st, L.ksplit, L.tmA0, L.tmA1, L.tmB, L.tmO, p));
   RYK_CUDA(cudaGetLastError());
-  if (p.ws) {
-    const size_t total4 = band_elems / 4, band4 = ws_rows * row_elems / 4, stride4 = L.Hout * row_elems / 4, off4 = r0 * row_elems / 4;
-    const size_t gap_at4 = gap_at * row_elems / 4, gap4 = gap * row_elems / 4;
-    if (L.ksplit <= 4) {
-      int blocks = (int)((total4 + 255) / 256); if (blocks > 2112) blocks = 2112;     // 16 per SM of 132
-      RYK_CUDA(launch_pdl(k_splitk_reduce_few, dim3(blocks), dim3(256), 0, st, (const float*)p.ws, total4, band_elems, L.ksplit, L.Cout, L.wt, L.act,
-                          (__half*)L.out, band4, stride4, off4, gap_at4, gap4));
-    } else {
-      RYK_CUDA(launch_pdl(k_splitk_reduce, dim3((unsigned)((total4 + 31) / 32)), dim3(256), 0, st, (const float*)p.ws, total4, band_elems, L.ksplit, L.Cout, L.wt, L.act,
-                          (__half*)L.out, band4, stride4, off4, gap_at4, gap4));
-    }
-    RYK_CUDA(cudaGetLastError());
-  }
   return 0;
 }
 

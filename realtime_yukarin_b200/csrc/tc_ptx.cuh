@@ -91,6 +91,22 @@ __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, ui
 }
 // rank of this CTA in its thread-block cluster
 __device__ __forceinline__ uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+// Every thread of every CTA of the cluster arrives (release) and waits (acquire): shared-memory writes before the barrier are
+// visible to the whole cluster's reads after it.  All lanes of a warp execute it together.
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// shared::cluster address of the variable at shared::cta address `a` in the CTA of cluster rank `rank`
+__device__ __forceinline__ uint32_t cluster_map(uint32_t a, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(rank));
+  return r;
+}
+__device__ __forceinline__ float4 ld_cluster_f4(uint32_t a) {
+  float4 v;
+  asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
+  return v;
+}
 
 // K-major, 128B-swizzled operand (the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_128B): 8-row atoms of 1024 B (stride byte
 // offset), leading byte offset unused, layout type 1 = 128B swizzle.  Advancing K by 16 fp16 inside the atom adds 32 B (+2).

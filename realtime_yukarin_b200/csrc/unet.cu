@@ -266,12 +266,6 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
       }
     }
   }
-  // One split-K workspace serves every layer of the plan: the layers run in stream order, and a layer's conv kernel writes the
-  // workspace only after its programmatic-launch wait, i.e. after the previous layer's reduce kernel has finished reading it.
-  size_t ws_bytes = 0;
-  for (int i = 0; i < 16; ++i)
-    if (precision == 1 && p->layers[i].w_tc[0] && tc_layer_eligible(p->layers[i]))
-      ws_bytes = std::max(ws_bytes, tc_splitk_ws_bytes(p->layers[i], num_sms));
   // Every buffer of the plan is carved from one zeroed allocation: plans are built and freed whenever a group's members change, and
   // separate small buffers would share the allocator's pages with other plans' and keep them in use after this plan is freed.
   std::vector<size_t> bytes;
@@ -279,7 +273,6 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
   for (int d = 0; d < 7; ++d) bytes.push_back((size_t)B * lvlH(6 - d) * lvlW(6 - d) * dec_out_channels(n->base, d) * esz);  // dec[d]
   bytes.push_back((size_t)B * H * W * n->in_ch * sizeof(float));                                                          // d_in
   bytes.push_back((size_t)B * H * W * n->out_ch * sizeof(float));                                                         // d_out
-  if (ws_bytes) bytes.push_back(ws_bytes);                                                                                // split-K
   constexpr size_t kAlign = 1024;
   size_t total = 0;
   for (size_t b : bytes) total += (b + kAlign - 1) / kAlign * kAlign;
@@ -293,7 +286,6 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
   void* const* dec = p->buffers.data() + 8;
   p->d_in = p->buffers[15];
   p->d_out = p->buffers[16];
-  void* ws = ws_bytes ? p->buffers[17] : nullptr;
   for (int i = 0; i < 16; ++i) {
     ConvLayer& L = p->layers[i];
     if (i == 0) {
@@ -311,10 +303,7 @@ int unet_get_plan(Engine* e, UNet* n, int B, int H, int W, int precision, UNetPl
   }
   for (int i = 0; i < 16; ++i) {
     ConvLayer& L = p->layers[i];
-    if (precision == 1 && L.w_tc[0] && tc_layer_eligible(L)) {
-      if (tc_splitk_ws_bytes(L, num_sms)) L.splitk_ws = (float*)ws;
-      if (tc_layer_prepare(L, num_sms)) return -1;
-    }
+    if (precision == 1 && L.w_tc[0] && tc_layer_eligible(L) && tc_layer_prepare(L, num_sms)) return -1;
   }
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   p->fused = s1_fused_eligible(n, p);

@@ -27,7 +27,7 @@ struct UNetPlan {
   int tail_begin = 0;                 // > 0: input rows >= tail_begin repeat one row, and the encoder skips them (unet_derive_tail)
   std::vector<ConvLayer> layers;
   void* arena = nullptr;    // one device allocation holding every buffer below
-  std::vector<void*> buffers;          // enc[0..7], dec[0..6], d_in, d_out, then the split-K workspace when a layer splits K
+  std::vector<void*> buffers;          // enc[0..7], dec[0..6], d_in, d_out
   std::vector<size_t> buffer_bytes;
   void* d_in = nullptr;     // fp32 NHWC input  [B][H][W][in_ch]
   void* d_out = nullptr;    // fp32 NHWC output [B][H][W][out_ch]

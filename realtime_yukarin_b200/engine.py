@@ -522,8 +522,10 @@ class Engine(object):
         out['nc'] = int(info[6])
         return out
 
-    def test_conv_layer(self, in0, in1, W, scale, shift, transposed, k, stride, pad, act, use_tc, repeat=0):
-        """One conv layer in isolation; in0/in1 NHWC float32, W in the Chainer layout. Returns (out NHWC, ms per run)."""
+    def test_conv_layer(self, in0, in1, W, scale, shift, transposed, k, stride, pad, act, use_tc, repeat=0, ksplit_tiles=0,
+                        with_ksplit=False):
+        """One conv layer in isolation; in0/in1 NHWC float32, W in the Chainer layout. Returns (out NHWC, ms per run), and the
+        wgmma kernel's split-K factor as a third item with with_ksplit.  ksplit_tiles > 0 splits K as for that many output tiles."""
         in0 = _f32(in0)
         B, H, Wd, C0 = in0.shape
         C1 = 0 if in1 is None else in1.shape[3]
@@ -536,11 +538,11 @@ class Engine(object):
             Ho = (H - 1) * stride + k - 2 * pad if transposed else (H + 2 * pad - k) // stride + 1
         Wo = (Wd - 1) * stride + k - 2 * pad if transposed else (Wd + 2 * pad - k) // stride + 1
         out = numpy.empty((B, Ho, Wo, cout), numpy.float32)
-        ms = ctypes.c_float()
+        ms, ks = ctypes.c_float(), ctypes.c_int()
         self._check(self.lib.ryk_test_conv_layer(
             self._h, int(transposed), int(k), int(stride), int(pad), B, H, Wd, C0, C1, cout, _fp(in0), _fp(in1a), _fp(W),
-            _fp(scale), _fp(shift), int(act), int(use_tc), int(repeat), _fp(out), ctypes.byref(ms)))
-        return out, ms.value
+            _fp(scale), _fp(shift), int(act), int(use_tc), int(repeat), int(ksplit_tiles), _fp(out), ctypes.byref(ms), ctypes.byref(ks)))
+        return (out, ms.value, ks.value) if with_ksplit else (out, ms.value)
 
     def test_stage2_forward(self, x, keep=(), mode=0, tw=0):
         """One stage-2 forward on NaN-filled buffers (ryk_test_stage2_forward); x [B][Tp][512] float32, keep = [(begin, len), ...];
