@@ -360,6 +360,45 @@ int ryk_session_set_noise_profile(ryk_engine* e, int session_id, const double* p
 int ryk_session_noise_profile(ryk_engine* e, int session_id, double* phi, long long* frames_left);
 int ryk_denoise(ryk_engine* e, const float* x, int n, double reduction_db, const double* phi, float* z);
 
+/* Echo cancellation (DESIGN.md §4g, DECIDE E1-E4): removes from the model-rate input the echo of the far end (what the host played
+ * while the chunk was recorded), ahead of the noise suppression and the WORLD analysis.  The microphone and the far end are framed as
+ * the noise suppression frames its input (N = 512, H = 128, sqrt-Hann, FP64, 257 bins).  Per bin, a complex FIR over the far end's
+ * frames, Y_m = sum_{p < taps} W_p X_{m - delay_frames - p}, is adapted by NLMS (mu = 0.5, delta = 1e-6) in two copies: a background
+ * filter B that adapts every frame and a foreground filter F that produces E = D - Y^f.  B is copied into F after 3 consecutive frames
+ * with S_b < 0.5 S_f and S_b < S_d (powers smoothed with lambda = 0.9); F is copied into B, skipping B's update, when S_b > 4 S_f;
+ * F is cleared when S_f > S_d (it would make the output louder than the microphone, as a far end correlated with the near end can).
+ * The output is Z = G E^f with the residual suppression G = max(g_e, 1 - Yhat / (Ehat + 1e-12)), g_e = 10^(-db / 20) (Yhat, Ehat:
+ * smoothed |Y^f|^2, |E^f|^2).  With noise suppression on, its gain scan then runs on Z.
+ * ryk_session_echo_cancel: fresh session only (no chunk pushed); either order with ryk_session_denoise and
+ *   ryk_session_set_input_rate.  taps in [1, 64] frames, delay_frames in [0, 256]: echoes up to (delay_frames + taps) * 128 model
+ *   samples are covered.  The session then analyses concat(zeros(511), z) like the noise suppression; with both on they share one
+ *   frame stage, so the delay grows by 511 once (ryk_session_io_geometry's delay_in).  Residual suppression starts at 0 dB.  Four
+ *   more kernels per step on the gate stream (two forward transforms, the canceller's scan, the inverse transforms; one more kernel
+ *   than the noise suppression alone when both are on), plus the far end's resampler at a device input rate.  A session without it
+ *   runs exactly the kernels it ran before.
+ * ryk_session_echo_reference: the far end of the next submitted step: far[n], n = the session's chunk length at its input rate
+ *   (n_in).  A step submitted without one uses zeros; a second call before the step replaces the first.  It applies to
+ *   ryk_session_submit / _push / _push_device, and for a group member to the next ryk_group_submit / _push_device.  At a device
+ *   input rate the far end goes through its own streaming copy of the input resampler (same taps, same delay), aligned sample for
+ *   sample with the microphone.
+ * ryk_session_set_echo_suppression: db in [0, 40] from the next submitted step on; allowed with chunks in flight and on a group
+ *   member; no device wait, no kernel.  0 dB is a gain of exactly 1: the output is the linear canceller's bit for bit.
+ * ryk_session_echo_stats: waits for the gate stream of the submitted steps, then writes the frames of the last step and its echo
+ *   return loss enhancement 10 log10(sum |D|^2 / sum |Z|^2) over its bins and frames (0 when the microphone was silent).  The per-bin
+ *   sums are added on the host in bin order, so the value is deterministic.  Either pointer may be NULL.
+ * ryk_echo_cancel: the same canceller over a whole signal on the same kernels: a fresh state, mic and far zero outside [0, n), z = n
+ *   samples with no delay; phi == NULL skips the noise suppression (reduction_db is then checked but unused).  A session's z with
+ *   constant settings is bitwise ryk_echo_cancel of its model-rate microphone and far end.
+ * Refused, changing nothing: an unknown session, enabling on a session that ran a step or twice, taps or delay_frames out of range,
+ * a reference of the wrong length, reference / suppression / stats calls on a session without the canceller, a non-finite db or one
+ * outside [0, 40]. */
+int ryk_session_echo_cancel(ryk_engine* e, int session_id, int taps, int delay_frames);
+int ryk_session_echo_reference(ryk_engine* e, int session_id, const float* far, int n);
+int ryk_session_set_echo_suppression(ryk_engine* e, int session_id, double db);
+int ryk_session_echo_stats(ryk_engine* e, int session_id, long long* frames, double* erle_db);
+int ryk_echo_cancel(ryk_engine* e, const float* mic, const float* far, int n, int taps, int delay_frames, double suppression_db,
+                    double reduction_db, const double* phi, float* z);
+
 /* Diagnostics: device timeline (ms) of the last <= 8 steps x 5 stages {gate, analysis, stage 1, stage 2, synthesis}; needs
  * RYK_STAGE_TIMES=1 in the environment at session creation.  start/end hold 40 floats; returns the number of steps. */
 int ryk_session_stage_times(ryk_engine* e, int session_id, float* start, float* end);

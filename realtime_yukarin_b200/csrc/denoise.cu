@@ -138,15 +138,30 @@ void denoise_state_init(DenoiseState* host) {
   for (double& g : host->gain) g = 1.0;
 }
 
-int denoise_run(Engine* e, const DenoiseWork& w, const DenoiseState* st, DenoiseState* st_next, const float* d_x, int n, float* d_z,
-                cudaStream_t stream) {
-  k_dn_forward<<<w.max_frames, kDnThreads, 0, stream>>>(st, st_next, d_x, n, w.spec, e->d_twiddle);
+int denoise_forward(Engine* e, int max_frames, const DenoiseState* st, DenoiseState* st_next, const float* d_x, int n, double2* spec,
+                    cudaStream_t stream) {
+  k_dn_forward<<<max_frames, kDnThreads, 0, stream>>>(st, st_next, d_x, n, spec, e->d_twiddle);
   RYK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int denoise_scan(const DenoiseWork& w, const DenoiseState* st, DenoiseState* st_next, int n, cudaStream_t stream) {
   k_dn_scan<<<1, 288, 0, stream>>>(w.params, w.learn, st, st_next, n, w.spec);
   RYK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int denoise_inverse(Engine* e, const DenoiseWork& w, const DenoiseState* st, DenoiseState* st_next, int n, float* d_z, cudaStream_t stream) {
   k_dn_inverse<<<w.max_frames, kDnThreads, 0, stream>>>(st, st_next, n, w.spec, w.frames, w.done, d_z, e->d_twiddle);
   RYK_CUDA(cudaGetLastError());
   return 0;
+}
+
+int denoise_run(Engine* e, const DenoiseWork& w, const DenoiseState* st, DenoiseState* st_next, const float* d_x, int n, float* d_z,
+                cudaStream_t stream) {
+  if (denoise_forward(e, w.max_frames, st, st_next, d_x, n, w.spec, stream)) return -1;
+  if (denoise_scan(w, st, st_next, n, stream)) return -1;
+  return denoise_inverse(e, w, st, st_next, n, d_z, stream);
 }
 
 // the refusals every entry point that takes a reduction or a profile shares

@@ -53,8 +53,15 @@ void denoise_state_init(DenoiseState* host);
 int denoise_check(double reduction_db, const double* phi);
 // One step: n new samples in d_x -> n filtered samples in d_z, delayed by kDnDelay.  Three kernels (forward transforms, gain scan,
 // inverse transforms + overlap-add); every size is fixed, the frame range is read from st on the device, so the launches can sit in a
-// captured graph.
+// captured graph.  denoise_run is the three launches below in order; the echo canceller runs its own scan between the first and last.
 int denoise_run(Engine* e, const DenoiseWork& w, const DenoiseState* st, DenoiseState* st_next, const float* d_x, int n, float* d_z,
                 cudaStream_t stream);
+// k_dn_forward: X_m of the step's frames into spec ([max_frames][kDnBins]); writes st_next's history and in_end
+int denoise_forward(Engine* e, int max_frames, const DenoiseState* st, DenoiseState* st_next, const float* d_x, int n, double2* spec,
+                    cudaStream_t stream);
+// k_dn_scan: the gain recursion on w.spec
+int denoise_scan(const DenoiseWork& w, const DenoiseState* st, DenoiseState* st_next, int n, cudaStream_t stream);
+// k_dn_inverse: inverse transforms of w.spec and the ordered overlap-add into d_z
+int denoise_inverse(Engine* e, const DenoiseWork& w, const DenoiseState* st, DenoiseState* st_next, int n, float* d_z, cudaStream_t stream);
 
 }  // namespace ryk

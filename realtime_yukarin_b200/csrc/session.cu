@@ -31,7 +31,7 @@
 #include <vector>
 
 #include "../../include/ryk.h"
-#include "denoise.h"
+#include "echo.h"
 #include "engine.h"
 #include "features.h"
 #include "synth.h"
@@ -78,7 +78,10 @@ struct ParitySet {
   float* in_win = nullptr;                       // device rates: input history window (in.hist device-rate samples)
   double* out_hist = nullptr;                    // device rates: kept synthesizer samples (out.hist)
   ResampleState *in_st = nullptr, *out_st = nullptr;   // device rates: the streaming resamplers' positions
-  DenoiseState* dn = nullptr;                    // input noise suppression: the filter's stream state
+  DenoiseState* dn = nullptr;                    // the frame stage of noise suppression / echo cancellation: the microphone's stream state
+  DenoiseState* far = nullptr;                   // echo cancellation: the far end's framing state (in_end and history)
+  float* far_win = nullptr;                      // echo cancellation at a device input rate: the far end's input history window
+  ResampleState* far_st = nullptr;               // ... and its resampler position
   // inter-stage buffers
   float *enc_f0 = nullptr, *enc_sp = nullptr, *enc_ap = nullptr, *enc_mc = nullptr; uint8_t* enc_voiced = nullptr;
   uint8_t* d_mask = nullptr; int* d_index = nullptr; int* d_count = nullptr;     // silence gate
@@ -107,6 +110,8 @@ struct StepEvents {
   cudaEvent_t tev[5][2] = {};      // RYK_STAGE_TIMES=1: [stage E1,E2,S1,S2,D][begin/end]
   F0Map* h_f0_map = nullptr;       // pinned staging of the f0 map copy in front of stage 1
   DenoiseParams* h_dn = nullptr;   // pinned staging of the noise-suppression parameter copy in front of the wave slides
+  EchoParams* h_aec = nullptr;     // pinned staging of the echo-cancellation parameter copy in front of the wave slides
+  float* h_far = nullptr;          // pinned staging of the step's far-end samples (n_in)
 };
 // The host-API staging of the caller's ticket t in slot t % kRing: the session's own step alone, the group's step while grouped.  A
 // membership change needs every host-API step collected, so no slot of one numbering is in use when the other takes over.
@@ -176,6 +181,17 @@ struct Session {
   DenoiseParams dn_params = {};    // what the next submitted step uses
   bool dn_dirty = false;           // dn_params changed since the last submitted step
   float* d_chunk_dn = nullptr;     // the step's filtered chunk (n_wave model-rate samples)
+  // Echo cancellation (ryk_session_echo_cancel, DESIGN.md §4g): the canceller runs in the frame stage it shares with the noise
+  // suppression, on the far end the host hands in for each step.  Its parameter block is host-owned (aec_sync copies it in front of
+  // the graph when it changed); the filter block is device-owned and updated in place.
+  bool echo = false;
+  EchoWork aec;
+  EchoParams aec_params = {};      // what the next submitted step uses
+  bool aec_dirty = false;          // aec_params changed since the last submitted step
+  std::vector<float> far_next;     // the far end of the next submitted step (ryk_session_echo_reference; zeros when none was given)
+  bool far_set = false;
+  float* d_far_fixed = nullptr;    // the step's far end as given (n_in samples), read by the captured wave-slide graph
+  float* d_far_model = nullptr;    // device input rate: its resampling (n_wave model-rate samples)
   BufferSet mem;                   // every device and pinned buffer above
 };
 
@@ -531,6 +547,24 @@ static int dn_sync(Session* s, long long k) {
   return 0;
 }
 
+// In front of the wave slides of step k on stream E, for a session with echo cancellation: the step's far end (the samples given since
+// the previous step, else zeros) and the parameters when they changed.  Pinned slot k % kRing was last read by the copies of step
+// k - kRing, which ended before its wave slides did, as in dn_sync.
+static int aec_sync(Session* s, long long k) {
+  StepEvents& ev = s->ev[k % kRing];
+  if (k >= kRing) RYK_CUDA(cudaEventSynchronize(ev.gate));
+  if (s->far_set) memcpy(ev.h_far, s->far_next.data(), sizeof(float) * s->n_in);
+  else memset(ev.h_far, 0, sizeof(float) * s->n_in);
+  s->far_set = false;
+  RYK_CUDA(cudaMemcpyAsync(s->d_far_fixed, ev.h_far, sizeof(float) * s->n_in, cudaMemcpyHostToDevice, s->sE));
+  if (s->aec_dirty) {
+    *ev.h_aec = s->aec_params;
+    RYK_CUDA(cudaMemcpyAsync(s->aec.params, ev.h_aec, sizeof(EchoParams), cudaMemcpyHostToDevice, s->sE));
+    s->aec_dirty = false;
+  }
+  return 0;
+}
+
 // The rest of stage 1 of a chunk of parity b and hand-off slot h: (gather ->) 1-D U-Net at padded length tp1 (0: no effective frame,
 // voice_changer.py:32-35 skips the net) -> scatter into the silent template + f0 map, mc2sp.  Enqueued on stream C while it is captured
 // as one body of the chunk's SWITCH graph; every body is captured when the session is created so that no chunk ever pays for a capture
@@ -593,6 +627,7 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
     RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev[(k - 2) % kRing].enc, 0));     // q.wave_win: last read by the analysis of k-2
   }
   if (dn_sync(s, k)) return -1;
+  if (s->echo && aec_sync(s, k)) return -1;
   if (stage_time(s, 0, 0, r, s->sE)) return -1;
   if (run_graph(e, p.graphs.gate, s->sE, [&]() -> int {
         const float* chunk = s->d_chunk_fixed;
@@ -602,8 +637,22 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
                                      p.in_st, q.in_st, s->d_chunk_model, s->n_wave, s->sE)) return -1;
           chunk = s->d_chunk_model;
         }
-        if (s->denoise) {            // noise suppression of the model-rate chunk in front of the wave slide
-          if (denoise_run(e, s->dn, p.dn, q.dn, chunk, s->n_wave, s->d_chunk_dn, s->sE)) return -1;
+        const float* far = s->d_far_fixed;
+        if (s->echo && s->in.rate) {  // the far end through its own copy of the input resampler, aligned with the microphone
+          if (slide<float>(p.far_win, s->d_far_fixed, q.far_win, s->in.hist, s->n_in, 1, s->sE)) return -1;
+          if (resample_stream_in_run(e, q.far_win, s->in.hist, s->n_in, s->delay_in, s->in.up, s->in.down, s->in.d_h, s->in.n_taps,
+                                     p.far_st, q.far_st, s->d_far_model, s->n_wave, s->sE)) return -1;
+          far = s->d_far_model;
+        }
+        if (s->denoise || s->echo) {  // the frame stage in front of the wave slide: echo cancellation, then noise suppression
+          const DenoiseWork& w = s->dn;
+          if (denoise_forward(e, w.max_frames, p.dn, q.dn, chunk, s->n_wave, w.spec, s->sE)) return -1;
+          if (s->echo) {
+            if (denoise_forward(e, w.max_frames, p.far, q.far, far, s->n_wave, s->aec.far_spec, s->sE)) return -1;
+            if (echo_scan(s->aec, p.dn, s->n_wave, w.spec, s->sE)) return -1;
+          }
+          if (s->denoise && denoise_scan(w, p.dn, q.dn, s->n_wave, s->sE)) return -1;
+          if (denoise_inverse(e, w, p.dn, q.dn, s->n_wave, s->d_chunk_dn, s->sE)) return -1;
           chunk = s->d_chunk_dn;
         }
         if (slide<float>(p.wave_win, chunk, q.wave_win, s->Lw, s->n_wave, 1, s->sE)) return -1;
@@ -1045,6 +1094,8 @@ int ryk_session_push_device(ryk_engine* h, int id, const float* wave_dev, int n,
 //           samples before it.
 //   output: a step emits the outputs whose support ends inside the synthesizer samples so far; the kept history covers the left
 //           support of the first output not yet emitted, and max_out bounds one step's count.
+static int echo_alloc_far(Session* s);
+
 static int session_set_rate(Engine* e, int id, bool input, int rate, int up, int down, const double* taps, int n_taps) {
   RYK_CUDA(cudaSetDevice(e->device));
   Session* s = get_session(e, id);
@@ -1086,6 +1137,10 @@ static int session_set_rate(Engine* e, int id, bool input, int rate, int up, int
   if (input) {
     s->n_in = (int)lrint(s->cfg.buffer_time * rate);
     s->delay_in = half / down;
+    if (s->echo) {                                  // the far end's buffers at the new chunk length, and its resampler
+      if (echo_alloc_far(s)) return -1;
+      RYK_CUDA(cudaStreamSynchronize(e->stream));
+    }
   } else {
     s->max_out = (int)(((long long)s->max_blocks * s->cfg.vocoder_buffer_size * up + down - 1) / down);
   }
@@ -1105,7 +1160,7 @@ int ryk_session_io_geometry(ryk_engine* h, int id, int* n_in, int* max_out, int*
   RYK_CHECK(s != nullptr, "no such session");
   if (n_in) *n_in = s->n_in;
   if (max_out) *max_out = s->max_out;
-  if (delay_in) *delay_in = s->delay_in + (s->denoise ? kDnDelay : 0);
+  if (delay_in) *delay_in = s->delay_in + (s->denoise || s->echo ? kDnDelay : 0);
   if (in_rate) *in_rate = s->in.rate ? s->in.rate : s->cfg.fs;
   if (out_rate) *out_rate = s->out.rate ? s->out.rate : s->cfg.fs;
   return 0;
@@ -1212,6 +1267,25 @@ static Session* denoise_session(Engine* e, int id) {
   return s && s->denoise ? s : nullptr;
 }
 
+// The frame stage noise suppression and echo cancellation share (N1, E1): the microphone's transforms, overlap-add and stream state,
+// allocated by whichever of the two is enabled first.  Step 0 reads par[0]: G_{-1} = 1.
+static int frame_stage_alloc(Engine* e, Session* s) {
+  if (s->dn.spec) return 0;
+  BufferSet& m = s->mem;
+  DenoiseWork& w = s->dn;
+  w.max_frames = denoise_max_frames(s->n_wave);
+  if (m.device(&w.spec, (size_t)kDnBins * w.max_frames) || m.device(&w.frames, (size_t)kDnN * w.max_frames) || m.device(&w.done, 1) ||
+      m.device(&s->d_chunk_dn, s->n_wave))
+    return -1;
+  for (ParitySet& p : s->par) if (m.device(&p.dn, 1)) return -1;
+  void* hp = nullptr;
+  if (engine_pinned(e, sizeof(DenoiseState), &hp)) return -1;
+  denoise_state_init((DenoiseState*)hp);
+  RYK_CUDA(cudaMemcpyAsync(s->par[0].dn, hp, sizeof(DenoiseState), cudaMemcpyHostToDevice, e->stream));
+  RYK_CUDA(cudaStreamSynchronize(e->stream));      // the staging is the engine's, and the session's streams do not wait for its stream
+  return 0;
+}
+
 int ryk_session_denoise(ryk_engine* h, int id) {
   Engine* e = &h->impl;
   RYK_CUDA(cudaSetDevice(e->device));
@@ -1219,19 +1293,12 @@ int ryk_session_denoise(ryk_engine* h, int id) {
   RYK_CHECK(s != nullptr, "no such session");
   RYK_CHECK(s->step == 0, "noise suppression can only be enabled on a fresh session (no chunk pushed): the wave slides are captured at the first steps");
   if (s->denoise) return 0;
+  if (frame_stage_alloc(e, s)) return -1;
   BufferSet& m = s->mem;
   DenoiseWork& w = s->dn;
-  w.max_frames = denoise_max_frames(s->n_wave);
-  if (m.device(&w.params, 1) || m.device(&w.learn, 1) || m.device(&w.spec, (size_t)kDnBins * w.max_frames) ||
-      m.device(&w.frames, (size_t)kDnN * w.max_frames) || m.device(&w.done, 1) || m.device(&s->d_chunk_dn, s->n_wave))
-    return -1;
-  for (ParitySet& p : s->par) if (m.device(&p.dn, 1)) return -1;
+  if (m.device(&w.params, 1) || m.device(&w.learn, 1)) return -1;
   for (StepEvents& ev : s->ev) if (m.pinned(&ev.h_dn, 1)) return -1;
-  // step 0 reads par[0]: G_{-1} = 1; the parameter block starts at 20 dB without a profile
-  void* hp = nullptr;
-  if (engine_pinned(e, sizeof(DenoiseState), &hp)) return -1;
-  denoise_state_init((DenoiseState*)hp);
-  RYK_CUDA(cudaMemcpyAsync(s->par[0].dn, hp, sizeof(DenoiseState), cudaMemcpyHostToDevice, e->stream));
+  // the parameter block starts at 20 dB without a profile
   s->dn_params = {};
   s->dn_params.gain_floor = pow(10.0, -20.0 / 20.0);
   *s->ev[0].h_dn = s->dn_params;
@@ -1288,6 +1355,92 @@ int ryk_session_noise_profile(ryk_engine* h, int id, double* phi, long long* fra
   const bool new_profile = P.profile_serial != L->profile_serial, new_learn = P.learn_serial != L->learn_serial;
   if (phi) memcpy(phi, new_profile ? P.phi : L->phi, sizeof(double) * kDnBins);
   if (frames_left) *frames_left = new_learn ? P.learn_frames : L->remaining;
+  return 0;
+}
+
+// ---- echo cancellation (DESIGN.md §4g) ----
+// The far end's buffers at the session's input chunk length n_in; with a device input rate, also its own resampler state pair.
+static int echo_alloc_far(Session* s) {
+  BufferSet& m = s->mem;
+  if (m.device(&s->d_far_fixed, s->n_in)) return -1;
+  for (StepEvents& ev : s->ev) if (m.pinned(&ev.h_far, s->n_in)) return -1;
+  if (s->in.rate) {
+    for (ParitySet& p : s->par) if (m.device(&p.far_win, s->in.hist) || m.device(&p.far_st, 1)) return -1;
+    if (m.device(&s->d_far_model, s->n_wave)) return -1;
+  }
+  s->far_next.assign(s->n_in, 0.f);
+  s->far_set = false;
+  return 0;
+}
+
+static Session* echo_session(Engine* e, int id) {
+  Session* s = get_session(e, id);
+  if (!s) set_error("no such session");
+  else if (!s->echo) set_error("echo cancellation is not enabled for this session (ryk_session_echo_cancel)");
+  return s && s->echo ? s : nullptr;
+}
+
+int ryk_session_echo_cancel(ryk_engine* h, int id, int taps, int delay_frames) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Session* s = get_session(e, id);
+  RYK_CHECK(s != nullptr, "no such session");
+  RYK_CHECK(s->step == 0, "echo cancellation can only be enabled on a fresh session (no chunk pushed): the wave slides are captured at the first steps");
+  RYK_CHECK(!s->echo, "echo cancellation is already enabled for this session");
+  if (int rc = echo_check(taps, delay_frames, 0.0)) return rc;
+  if (frame_stage_alloc(e, s)) return -1;
+  BufferSet& m = s->mem;
+  EchoWork& a = s->aec;
+  a.taps = taps; a.delay = delay_frames;
+  if (m.device(&a.params, 1) || m.device(&a.filter, 1) || m.device(&a.ring, (size_t)kDnBins * (taps + delay_frames)) ||
+      m.device(&a.far_spec, (size_t)kDnBins * s->dn.max_frames))
+    return -1;
+  for (ParitySet& p : s->par) if (m.device(&p.far, 1)) return -1;     // zero: in_end 0, an empty history
+  for (StepEvents& ev : s->ev) if (m.pinned(&ev.h_aec, 1)) return -1;
+  if (echo_alloc_far(s)) return -1;
+  // the filters start at zero; the residual suppression at 0 dB (gain 1)
+  s->aec_params = {};
+  s->aec_params.gain_floor = 1.0;
+  *s->ev[0].h_aec = s->aec_params;
+  RYK_CUDA(cudaMemcpyAsync(a.params, s->ev[0].h_aec, sizeof(EchoParams), cudaMemcpyHostToDevice, e->stream));
+  RYK_CUDA(cudaStreamSynchronize(e->stream));      // the zero-fills and the copy: the session's streams do not wait for the engine stream
+  s->echo = true;
+  return 0;
+}
+
+int ryk_session_echo_reference(ryk_engine* h, int id, const float* far, int n) {
+  Session* s = echo_session(&h->impl, id);
+  if (!s) return -2;
+  RYK_CHECK(far != nullptr, "null argument");
+  RYK_CHECK(n == s->n_in, "the far end of a step must be one chunk at the session's input rate (ryk_session_io_geometry n_in)");
+  memcpy(s->far_next.data(), far, sizeof(float) * n);
+  s->far_set = true;
+  return 0;
+}
+
+int ryk_session_set_echo_suppression(ryk_engine* h, int id, double db) {
+  Session* s = echo_session(&h->impl, id);
+  if (!s) return -2;
+  if (int rc = echo_check(1, 0, db)) return rc;
+  s->aec_params.gain_floor = pow(10.0, -db / 20.0);
+  s->aec_dirty = true;
+  return 0;
+}
+
+int ryk_session_echo_stats(ryk_engine* h, int id, long long* frames, double* erle_db) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Session* s = echo_session(e, id);
+  if (!s) return -2;
+  void* hp = nullptr;
+  if (engine_pinned(e, sizeof(EchoStats), &hp)) return -1;
+  RYK_CUDA(cudaMemcpyAsync(hp, &s->aec.filter->stats, sizeof(EchoStats), cudaMemcpyDeviceToHost, s->sE));
+  RYK_CUDA(cudaStreamSynchronize(s->sE));          // behind the wave slides of every submitted step
+  const EchoStats* f = (const EchoStats*)hp;
+  double sd = 0.0, sz = 0.0;
+  for (int k = 0; k < kDnBins; ++k) { sd += f->sum_d[k]; sz += f->sum_z[k]; }
+  if (frames) *frames = f->frames;
+  if (erle_db) *erle_db = sd > 0.0 ? 10.0 * log10(sd / sz) : 0.0;
   return 0;
 }
 

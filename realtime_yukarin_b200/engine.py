@@ -67,7 +67,8 @@ EXPORTED_SYMBOLS = [
     'ryk_session_get_f0_map', 'ryk_session_set_f0_map', 'ryk_session_f0_measure', 'ryk_session_f0_follow', 'ryk_session_f0_measure_reset',
     'ryk_session_f0_measured', 'ryk_session_set_formant', 'ryk_session_get_formant', 'ryk_stage2_convert_formant',
     'ryk_session_set_voice', 'ryk_session_denoise', 'ryk_session_set_denoise', 'ryk_session_denoise_learn', 'ryk_session_set_noise_profile',
-    'ryk_session_noise_profile', 'ryk_denoise',
+    'ryk_session_noise_profile', 'ryk_denoise', 'ryk_session_echo_cancel', 'ryk_session_echo_reference', 'ryk_session_set_echo_suppression',
+    'ryk_session_echo_stats', 'ryk_echo_cancel',
 ]
 
 SEMITONE = math.log(2.0) / 12.0          # one semitone in ln f0
@@ -75,6 +76,8 @@ F0_SD_FLOOR = 0.05                       # follow mode: least in_std (ln f0), ab
 FORMANT_RANGE = (0.5, 2.0)               # formant ratios a session or ryk_stage2_convert_formant accepts: +-12 semitones
 NOISE_BINS = 257                         # bins of a noise profile: rfft of the filter's 512-sample frames
 NOISE_HOP = 128                          # model samples per noise-suppression frame
+ECHO_TAPS = (1, 64)                      # echo canceller: filter lengths in frames a session or echo_cancel accepts
+ECHO_DELAY_FRAMES = (0, 256)             # ... and bulk delays of the far end in frames
 
 
 class F0Map(ctypes.Structure):
@@ -686,6 +689,51 @@ class Engine(object):
                 raise ValueError(f'a noise profile has {NOISE_BINS} values')
         self._check(self.lib.ryk_denoise(self._h, _fp(x), len(x), ctypes.c_double(reduction_db), _dp(phi) if phi is not None else None,
                                          _fp(z)))
+        return z
+
+    # ---- echo cancellation ----
+    def session_echo_cancel(self, sid: int, taps: int = 32, delay_ms: float = 0.0):
+        """Fresh session only: cancel the echo of the far end (what the host played, given per chunk with session_echo_reference)
+        ahead of the noise suppression and the analysis.  `taps` frames of 128 model samples (1-64) after a bulk delay of `delay_ms`,
+        rounded to whole frames of the session's rate (0-256 frames), cover the echo path.  The input delay grows by 511 model samples
+        unless noise suppression already added them (session_io_geometry's delay_in)."""
+        frames = round(float(delay_ms) * self._session_fs.get(sid, 0) / 1000.0 / NOISE_HOP)     # an unknown session: the library refuses
+        self._check(self.lib.ryk_session_echo_cancel(self._h, int(sid), int(taps), int(frames)))
+
+    def session_echo_reference(self, sid: int, far):
+        """The far end of the next submitted chunk: n_in float32 samples at the session's input rate, the audio played while that
+        chunk was recorded.  A chunk submitted without one uses zeros."""
+        far = _f32(far)
+        self._check(self.lib.ryk_session_echo_reference(self._h, int(sid), _fp(far), len(far)))
+
+    def session_set_echo_suppression(self, sid: int, db: float):
+        """Residual-echo suppression, 0 to 40 dB, from the next submitted step on (chunks in flight keep theirs); 0 leaves the linear
+        canceller's output untouched."""
+        self._check(self.lib.ryk_session_set_echo_suppression(self._h, int(sid), ctypes.c_double(db)))
+
+    def session_echo_stats(self, sid: int):
+        """(frames of the last submitted step, its echo return loss enhancement in dB: 10 log10(sum |D|^2 / sum |Z|^2) of the microphone
+        and the canceller's output); waits for the submitted steps' input stage."""
+        frames, erle = ctypes.c_longlong(), ctypes.c_double()
+        self._check(self.lib.ryk_session_echo_stats(self._h, int(sid), ctypes.byref(frames), ctypes.byref(erle)))
+        return frames.value, erle.value
+
+    def echo_cancel(self, mic, far, taps: int = 32, delay_frames: int = 0, suppression_db: float = 0.0, reduction_db: float = 20.0,
+                    profile=None) -> numpy.ndarray:
+        """The session's echo canceller over a whole signal: a fresh filter, no delay, len(mic) float32 samples out.  With a noise
+        profile the noise suppression (reduction_db) runs on its output, as in a session with both."""
+        mic, far = _f32(mic), _f32(far)
+        if len(far) != len(mic):
+            raise ValueError('mic and far must have the same length')
+        z = numpy.empty_like(mic)
+        phi = None
+        if profile is not None:
+            phi = numpy.ascontiguousarray(profile, dtype=numpy.float64).ravel()
+            if len(phi) != NOISE_BINS:
+                raise ValueError(f'a noise profile has {NOISE_BINS} values')
+        self._check(self.lib.ryk_echo_cancel(self._h, _fp(mic), _fp(far), len(mic), int(taps), int(delay_frames),
+                                             ctypes.c_double(suppression_db), ctypes.c_double(reduction_db),
+                                             _dp(phi) if phi is not None else None, _fp(z)))
         return z
 
     def session_destroy(self, sid: int):

@@ -72,12 +72,17 @@ def save_noise_profile_file(pipeline: RealtimePipeline, path: Path) -> None:
 def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path] = None, max_chunks: Optional[int] = None,
         engine=None, depth: int = 3, measure_input_statistics: Optional[Path] = None, follow_input_f0: Optional[int] = None,
         pitch: float = 0.0, formant: float = 0.0, denoise: Optional[float] = None, noise_profile: Optional[Path] = None,
-        learn_noise: Optional[float] = None, save_noise_profile: Optional[Path] = None) -> int:
+        learn_noise: Optional[float] = None, save_noise_profile: Optional[Path] = None, echo_cancel: Optional[int] = None,
+        echo_delay: float = 0.0, echo_suppression: float = 0.0) -> int:
     """`measure_input_statistics`: measure the speaker's log-f0 statistics during the run and write them to this file at the end;
     `follow_input_f0`: convert with the measured statistics once this many voiced frames are counted; `pitch`: semitones added to
     the target voice's mean f0; `formant`: semitones by which the converted spectral envelope moves; `denoise`: filter the input's
     noise ahead of the analysis with at most this many dB of attenuation, with the profile in `noise_profile` (.npy) or one learned from
-    the first `learn_noise` seconds of input, and write the profile in use to `save_noise_profile` at the end."""
+    the first `learn_noise` seconds of input, and write the profile in use to `save_noise_profile` at the end; `echo_cancel`: cancel the
+    echo of the played output in the input with a filter of this many 128-sample frames after a bulk delay of `echo_delay` ms, followed
+    by `echo_suppression` dB of residual-echo suppression."""
+    if echo_cancel is None and (echo_delay or echo_suppression):
+        raise ValueError('--echo_delay and --echo_suppression need --echo_cancel')
     if denoise is None and (noise_profile is not None or learn_noise is not None or save_noise_profile is not None):
         raise ValueError('--noise_profile, --learn_noise and --save_noise_profile need --denoise')
     logger = logging.getLogger('root')
@@ -90,7 +95,9 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
     pipeline = RealtimePipeline(config, acoustic_param=converter.acoustic_converter.config.dataset.acoustic_param, engine=engine, depth=depth,
                                 measure_f0=measure_input_statistics is not None, follow_f0=follow_input_f0, formant=formant,
                                 denoise=denoise, noise_profile=None if noise_profile is None else numpy.load(noise_profile),
-                                learn_noise=learn_noise)
+                                learn_noise=learn_noise, echo_cancel=echo_cancel is not None,
+                                echo_taps=32 if echo_cancel is None else echo_cancel, echo_delay_ms=echo_delay,
+                                echo_suppression=echo_suppression)
     try:
         if pitch:
             pipeline.set_f0_map(semitones=pitch)
@@ -161,6 +168,13 @@ def make_parser() -> argparse.ArgumentParser:
                         help='with --denoise: learn the noise profile from the first SECONDS of input (stay quiet meanwhile; 1 s is enough)')
     parser.add_argument('--save_noise_profile', type=Path, default=None, metavar='OUT.npy',
                         help='with --denoise: write the noise profile in use to this file when the run ends, for --noise_profile')
+    parser.add_argument('--echo_cancel', type=int, nargs='?', const=32, default=None, metavar='TAPS',
+                        help='cancel the echo of the played output that the microphone picks up (speakers instead of headphones), with '
+                             'a filter of TAPS frames of 128 samples at the model rate (1-64, default 32: 170 ms at 24 kHz)')
+    parser.add_argument('--echo_delay', type=float, default=0.0, metavar='MS',
+                        help='with --echo_cancel: the bulk delay of the echo path ahead of the filter, in ms (up to 256 frames)')
+    parser.add_argument('--echo_suppression', type=float, default=0.0, metavar='DB',
+                        help='with --echo_cancel: suppress the residual echo by at most DB (0-40; 0 keeps the linear canceller)')
     return parser
 
 
@@ -169,7 +183,8 @@ def main(argv: Optional[Iterable[str]] = None) -> None:
     run(config_path=args.config_path, wav_in=args.wav_in, wav_out=args.wav_out, max_chunks=args.max_chunks,
         measure_input_statistics=args.measure_input_statistics, follow_input_f0=args.follow_input_f0, pitch=args.pitch,
         formant=args.formant, denoise=args.denoise, noise_profile=args.noise_profile, learn_noise=args.learn_noise,
-        save_noise_profile=args.save_noise_profile)
+        save_noise_profile=args.save_noise_profile, echo_cancel=args.echo_cancel, echo_delay=args.echo_delay,
+        echo_suppression=args.echo_suppression)
 
 
 if __name__ == '__main__':

@@ -89,11 +89,20 @@ class RealtimePipeline(object):
     map between chunks.  `formant` (semitones, [-12, 12]) warps the converted spectral envelope from the first chunk on; `set_formant`
     changes it between chunks.  `denoise=DB` filters the input's noise ahead of the analysis (at most DB of attenuation, 0-40), with
     `noise_profile` (257 values, as `noise_profile()` returns them) or a profile learned from the first `learn_noise` seconds of input;
-    `set_denoise` changes the reduction between chunks."""
+    `set_denoise` changes the reduction between chunks.  `echo_cancel=True` removes the echo of the played output from the input ahead of
+    the analysis (and of the noise filter), for a voice played through speakers: `echo_taps` frames of 128 model samples (1-64) after a
+    bulk delay of `echo_delay_ms` cover the echo path, and `echo_suppression` dB (0-40) of residual-echo suppression follows;
+    `set_echo_suppression` changes it between chunks and `echo_stats` reads how much echo the last chunk lost.  The far end is what
+    `process` returned: mic chunk i is paired with the next n_in samples of the played stream, which starts with one input chunk of
+    zeros (chunk i with the output of chunk i - 1 when the chunk sizes are equal; silence where the output ran short).  It needs
+    input_rate == output_rate."""
 
     def __init__(self, config: Config, acoustic_param=None, engine: Optional[Engine] = None, depth: int = 3, voice: int = 0,
                  measure_f0: bool = False, follow_f0: Optional[int] = None, formant: float = 0.0, denoise: Optional[float] = None,
-                 noise_profile=None, learn_noise: Optional[float] = None):
+                 noise_profile=None, learn_noise: Optional[float] = None, echo_cancel: bool = False, echo_taps: int = 32,
+                 echo_delay_ms: float = 0.0, echo_suppression: float = 0.0):
+        if echo_cancel and int(config.input_rate) != int(config.output_rate):
+            raise ValueError('echo_cancel needs input_rate == output_rate: the played stream is the far end of the input')
         self.config = config
         self.engine = engine or default_engine()
         p = acoustic_param
@@ -154,6 +163,11 @@ class RealtimePipeline(object):
                 self.engine.session_denoise_learn(self._sid, seconds=float(learn_noise))
         elif noise_profile is not None or learn_noise is not None:
             raise ValueError('noise_profile and learn_noise need denoise')
+        self._echo = bool(echo_cancel)
+        if self._echo:
+            self.engine.session_echo_cancel(self._sid, taps=int(echo_taps), delay_ms=float(echo_delay_ms))
+            self.engine.session_set_echo_suppression(self._sid, float(echo_suppression))
+            self._played = numpy.zeros(config.in_audio_chunk, numpy.float32)   # the played stream not yet paired with an input chunk
         if measure_f0 or follow_f0 is not None:
             self.engine.session_f0_measure(self._sid)
         if follow_f0 is not None:
@@ -194,6 +208,14 @@ class RealtimePipeline(object):
     def noise_profile(self) -> Tuple[numpy.ndarray, int]:
         """(noise profile the next chunk uses, frames still to learn) of the stream's noise filter (needs denoise)."""
         return self.engine.session_noise_profile(self._sid)
+
+    def set_echo_suppression(self, db: float) -> None:
+        """Engine.session_set_echo_suppression for this stream: residual-echo suppression in dB, from the next chunk on."""
+        self.engine.session_set_echo_suppression(self._sid, db)
+
+    def echo_stats(self) -> Tuple[int, float]:
+        """(frames, echo return loss enhancement in dB) of the last chunk put (needs echo_cancel)."""
+        return self.engine.session_echo_stats(self._sid)
 
     def measured_f0(self) -> Tuple[int, float, float]:
         """(voiced frames, mean, standard deviation) of the speaker's ln f0 over the chunks put so far (needs measure_f0)."""
@@ -262,6 +284,11 @@ class RealtimePipeline(object):
         """in: in_audio_chunk float32 samples from the input device; out: out_audio_chunk float32 samples for the output
         device (zeros while nothing is ready, as the reference plays silence)."""
         c = self.config
+        if self._echo:
+            n = len(in_wave)
+            far = self._played[:n]
+            self._played = self._played[n:]
+            self.engine.session_echo_reference(self._sid, numpy.concatenate([far, numpy.zeros(n - len(far), numpy.float32)]))
         self.put(Item(item=numpy.asarray(in_wave, dtype=numpy.float32) * c.input_scale, index=self._index_input))
         self._index_input += 1
         if block:
@@ -269,8 +296,10 @@ class RealtimePipeline(object):
         out_wave = self._next_output()
         if out_wave is None:
             out_wave = numpy.zeros(c.out_audio_chunk)
-        out_wave = out_wave * c.output_scale
-        return out_wave[:c.out_audio_chunk].astype(numpy.float32)
+        out_wave = (out_wave * c.output_scale)[:c.out_audio_chunk].astype(numpy.float32)
+        if self._echo:
+            self._played = numpy.concatenate([self._played, out_wave])
+        return out_wave
 
     def _next_output(self) -> Optional[numpy.ndarray]:
         """run.py:176-195: pop every finished item, take the ones whose index is next in order; silent items (None) are
