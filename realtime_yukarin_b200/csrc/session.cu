@@ -68,6 +68,19 @@ struct HandoffGraphs {
   StageGraph s2_epi;       // stage-2 epilogue (single session: layer 15 +; group member: from the group's batched output)
   StageGraph dec_slide;    // stream D: decode-window slides
 };
+// The session's inputs: the microphone, and with echo cancellation the far end.  Each has an InputSignal in Session and an InputState in
+// each ParitySet; one input path (input_alloc, input_to_model) serves both.
+enum { kMic = 0, kFar = 1, kInputs = 2 };
+struct InputSignal {               // the step's samples, read by the captured gate graph
+  float* d_fixed = nullptr;        // as given (n_in samples)
+  float* d_model = nullptr;        // device input rate: their resampling (n_wave model-rate samples)
+};
+// The stream state of one input that step k reads from par[b] and writes for the next step into par[b ^ 1].
+struct InputState {
+  float* win = nullptr;            // device input rate: history window (in.hist device-rate samples)
+  ResampleState* rs = nullptr;     // device input rate: the streaming resampler's position
+  DenoiseState* dn = nullptr;      // the frame stage of noise suppression / echo cancellation (the microphone's also holds the filter's)
+};
 // What the parity b = k & 1 of the session's own step k selects.  Step k reads the sliding windows of par[b] and writes those of
 // par[b ^ 1]; the rest of par[b] is step k's own.  Buffers are null until allocated, so a partly built session can be freed.
 struct ParitySet {
@@ -75,13 +88,9 @@ struct ParitySet {
   float* wave_win = nullptr;
   float *cw_f0 = nullptr, *cw_ap = nullptr, *cw_mc = nullptr, *cw_wave = nullptr; uint8_t* cw_voiced = nullptr;
   float *dw_f0 = nullptr, *dw_ap = nullptr, *dw_sp = nullptr;
-  float* in_win = nullptr;                       // device rates: input history window (in.hist device-rate samples)
+  InputState input[kInputs];                     // the microphone's and the far end's input windows and stream state
   double* out_hist = nullptr;                    // device rates: kept synthesizer samples (out.hist)
-  ResampleState *in_st = nullptr, *out_st = nullptr;   // device rates: the streaming resamplers' positions
-  DenoiseState* dn = nullptr;                    // the frame stage of noise suppression / echo cancellation: the microphone's stream state
-  DenoiseState* far = nullptr;                   // echo cancellation: the far end's framing state (in_end and history)
-  float* far_win = nullptr;                      // echo cancellation at a device input rate: the far end's input history window
-  ResampleState* far_st = nullptr;               // ... and its resampler position
+  ResampleState* out_st = nullptr;               // device rates: the output resampler's position
   // inter-stage buffers
   float *enc_f0 = nullptr, *enc_sp = nullptr, *enc_ap = nullptr, *enc_mc = nullptr; uint8_t* enc_voiced = nullptr;
   uint8_t* d_mask = nullptr; int* d_index = nullptr; int* d_count = nullptr;     // silence gate
@@ -108,10 +117,12 @@ struct StepEvents {
   cudaEvent_t dslide = nullptr;    // the converted features of step k sit in the decode window
   std::array<cudaEvent_t*, 7> all() { return {&gate, &enc, &cslide, &s1, &pro, &conv, &dslide}; }
   cudaEvent_t tev[5][2] = {};      // RYK_STAGE_TIMES=1: [stage E1,E2,S1,S2,D][begin/end]
-  F0Map* h_f0_map = nullptr;       // pinned staging of the f0 map copy in front of stage 1
-  DenoiseParams* h_dn = nullptr;   // pinned staging of the noise-suppression parameter copy in front of the wave slides
-  EchoParams* h_aec = nullptr;     // pinned staging of the echo-cancellation parameter copy in front of the wave slides
-  float* h_far = nullptr;          // pinned staging of the step's far-end samples (n_in)
+};
+// A block the host sets between steps and the captured graphs read: the setters change `next`, host_block_sync copies it (DESIGN.md §4a).
+template <typename T> struct HostBlock {
+  T next = {};                     // what the next submitted step uses
+  bool dirty = false;              // next changed since the last submitted step
+  T* ring = nullptr;               // pinned staging: slot k % kRing for step k (the session's BufferSet)
 };
 // The host-API staging of the caller's ticket t in slot t % kRing: the session's own step alone, the group's step while grouped.  A
 // membership change needs every host-API step collected, so no slot of one numbering is in use when the other takes over.
@@ -152,7 +163,7 @@ struct Session {
   double* d_mse = nullptr;             // silence-gate scratch (stream C)
   double* dec_f0_f64 = nullptr;
   int max_blocks;
-  float* d_chunk_fixed = nullptr;      // the chunk the (captured) wave-slide graph reads
+  InputSignal input[kInputs];          // the microphone (always) and the far end (echo cancellation)
   HandoffGraphs hgraphs[kHandoffGraphs];
   Synth* synth = nullptr;
   // Device rates (ryk_session_set_input_rate / _output_rate): chunks arrive at in.rate and outputs leave at out.rate; analysis, the
@@ -165,33 +176,29 @@ struct Session {
   int n_in = 0;                    // samples per pushed chunk (n_wave without an input resampler)
   int delay_in = 0;                // leading zeros of the model-rate input (model samples)
   int max_out = 0;                 // most output samples one step can return
-  float* d_chunk_model = nullptr;  // the step's resampled chunk (n_wave model-rate samples)
   // The session's f0 map (ryk_session_set_f0_map / _f0_follow), its formant ratio (ryk_session_set_formant) and the statistics of its
-  // speaker (ryk_session_f0_measure).  The captured stage-1 graphs read *d_f0_map; f0_map_sync brings it up to date on stream C in front
-  // of a step's stage 1.  The formant ratio reaches stage 2 through ho[h].formant, never from *d_f0_map (DESIGN.md §4a).
-  F0Map f0_map = {};               // what the next submitted step uses (follow mode: its input side is the fallback)
-  bool f0_dirty = false;           // f0_map changed since the last submitted step
+  // speaker (ryk_session_f0_measure).  The captured stage-1 graphs read *d_f0_map, a host block synced on stream C in front of a step's
+  // stage 1 (follow mode: its input side is the fallback).  The formant ratio reaches stage 2 through ho[h].formant, never from
+  // *d_f0_map (DESIGN.md §4a).
+  HostBlock<F0Map> f0_map;
   bool f0_measure = false;         // the head of stage 1 ends with k_f0_measure
   bool f0_reset = false;           // the statistics restart at the next submitted step
   F0Map* d_f0_map = nullptr; F0Stats* d_f0_stats = nullptr;
   // Input noise suppression (ryk_session_denoise, DESIGN.md §4f): the filter runs in the wave-slide graph on the model-rate chunk.  Its
-  // parameter block is host-owned (dn_sync copies dn_params in front of the graph when it changed); the learning state is device-owned.
+  // parameter block dn.params is a host block synced on stream E in front of the graph; the learning state is device-owned.
   bool denoise = false;
   DenoiseWork dn;
-  DenoiseParams dn_params = {};    // what the next submitted step uses
-  bool dn_dirty = false;           // dn_params changed since the last submitted step
+  HostBlock<DenoiseParams> dn_params;
   float* d_chunk_dn = nullptr;     // the step's filtered chunk (n_wave model-rate samples)
   // Echo cancellation (ryk_session_echo_cancel, DESIGN.md §4g): the canceller runs in the frame stage it shares with the noise
-  // suppression, on the far end the host hands in for each step.  Its parameter block is host-owned (aec_sync copies it in front of
-  // the graph when it changed); the filter block is device-owned and updated in place.
+  // suppression, on the far end (input[kFar]) the host hands in for each step.  Its parameter block aec.params is a host block synced
+  // on stream E in front of the graph; the filter block is device-owned and updated in place.
   bool echo = false;
   EchoWork aec;
-  EchoParams aec_params = {};      // what the next submitted step uses
-  bool aec_dirty = false;          // aec_params changed since the last submitted step
+  HostBlock<EchoParams> aec_params;
   std::vector<float> far_next;     // the far end of the next submitted step (ryk_session_echo_reference; zeros when none was given)
   bool far_set = false;
-  float* d_far_fixed = nullptr;    // the step's far end as given (n_in samples), read by the captured wave-slide graph
-  float* d_far_model = nullptr;    // device input rate: its resampling (n_wave model-rate samples)
+  float* h_far = nullptr;          // pinned staging of the far end: slot k % kRing (n_in samples) for step k
   BufferSet mem;                   // every device and pinned buffer above
 };
 
@@ -280,6 +287,34 @@ static void slide_add(SlideBatch& b, const T* old_, const T* new_, T* dst, size_
 }
 
 static Session* get_session(Engine* e, int id) { return (id >= 0 && id < (int)e->sessions.size()) ? e->sessions[id] : nullptr; }
+
+// The session when it has not run a chunk yet (what its graphs capture at the first steps can still change), else nullptr with the
+// error set: "no such session", or `refusal`.
+static Session* fresh_session(Engine* e, int id, const char* refusal) {
+  Session* s = get_session(e, id);
+  if (!s) set_error("no such session");
+  else if (s->step != 0) set_error(refusal);
+  return s && s->step == 0 ? s : nullptr;
+}
+
+// (Re)allocates input i at chunk length n_in, with a history window and resampler state pair when `resampled` (device input rate, window
+// of in.hist samples).  The far end also gets its host staging, the next step's samples and kRing pinned slots; the microphone is
+// staged through HostSlot::h_in.
+static int input_alloc(Session* s, int i, int n_in, bool resampled) {
+  BufferSet& m = s->mem;
+  InputSignal& x = s->input[i];
+  if (m.device(&x.d_fixed, n_in)) return -1;
+  if (resampled) {
+    for (ParitySet& p : s->par) if (m.device(&p.input[i].win, s->in.hist) || m.device(&p.input[i].rs, 1)) return -1;
+    if (m.device(&x.d_model, s->n_wave)) return -1;
+  }
+  if (i == kFar) {
+    if (m.pinned(&s->h_far, (size_t)kRing * n_in)) return -1;
+    s->far_next.assign(n_in, 0.f);
+    s->far_set = false;
+  }
+  return 0;
+}
 
 // Drop the stage-2 plans of a session's own lanes and the graphs captured on them (a no-op for plans a group already released).
 static void lanes_release(Session* s) {
@@ -513,55 +548,43 @@ static int stage1_head(Engine* e, Session* s, int b) {
   return 0;
 }
 
-// In front of stage 1 of step k on stream C: restart the speaker statistics and copy the f0 map into the block the stage-1 graphs read,
-// when either was asked for since the previous step.  Stage 1 of every step runs on stream C in step order, so the steps already
-// submitted keep the map they were submitted with and step k is the first to see the new one; the host does not wait and no kernel runs.
-// The copy reads pinned slot k % kRing when the stream reaches it; that slot was last used by step k - kRing, whose copy ended before
-// the head of its stage 1 did (the wait returns at once unless the host is a whole ring ahead of the device).
-static int f0_map_sync(Session* s, long long k) {
-  if (s->f0_reset) {
-    RYK_CUDA(cudaMemsetAsync(s->d_f0_stats, 0, sizeof(F0Stats), s->sC));
-    s->f0_reset = false;
-  }
-  if (!s->f0_dirty) return 0;
-  StepEvents& ev = s->ev[k % kRing];
-  if (k >= kRing) RYK_CUDA(cudaEventSynchronize(ev.cslide));
-  *ev.h_f0_map = s->f0_map;
-  RYK_CUDA(cudaMemcpyAsync(s->d_f0_map, ev.h_f0_map, sizeof(F0Map), cudaMemcpyHostToDevice, s->sC));
-  s->f0_dirty = false;
+// In front of the graphs of step k that read *dev, on the stream st that runs them in step order: when the block changed, stage it in
+// pinned slot k % kRing and copy it into *dev, so step k is the first to see it.  The slot was last read by a copy of step k - kRing or
+// earlier, which ended before the guard event of step k - kRing: the host waits for that event (at once unless a whole ring ahead).
+template <typename T>
+static int host_block_sync(HostBlock<T>& b, T* dev, long long k, cudaEvent_t guard, cudaStream_t st) {
+  if (!b.dirty) return 0;
+  if (k >= kRing) RYK_CUDA(cudaEventSynchronize(guard));
+  T* slot = b.ring + k % kRing;
+  *slot = b.next;
+  RYK_CUDA(cudaMemcpyAsync(dev, slot, sizeof(T), cudaMemcpyHostToDevice, st));
+  b.dirty = false;
   return 0;
 }
 
-// In front of the wave slides of step k on stream E: copy the noise-suppression parameters into the block the filter reads when they
-// changed since the previous step.  The wave slides of every step run on stream E in step order, so the steps already submitted keep
-// their parameters and the host neither waits nor launches a kernel.  The device writes only its own learning block, never this one
-// (DESIGN.md §4f).  The copy reads pinned slot k % kRing; that slot was last read by a copy of step k - kRing or earlier, which ended
-// before the wave slides of step k - kRing did.
-static int dn_sync(Session* s, long long k) {
-  if (!s->dn_dirty) return 0;
-  StepEvents& ev = s->ev[k % kRing];
-  if (k >= kRing) RYK_CUDA(cudaEventSynchronize(ev.gate));
-  *ev.h_dn = s->dn_params;
-  RYK_CUDA(cudaMemcpyAsync(s->dn.params, ev.h_dn, sizeof(DenoiseParams), cudaMemcpyHostToDevice, s->sE));
-  s->dn_dirty = false;
-  return 0;
-}
-
-// In front of the wave slides of step k on stream E, for a session with echo cancellation: the step's far end (the samples given since
-// the previous step, else zeros) and the parameters when they changed.  Pinned slot k % kRing was last read by the copies of step
-// k - kRing, which ended before its wave slides did, as in dn_sync.
-static int aec_sync(Session* s, long long k) {
-  StepEvents& ev = s->ev[k % kRing];
-  if (k >= kRing) RYK_CUDA(cudaEventSynchronize(ev.gate));
-  if (s->far_set) memcpy(ev.h_far, s->far_next.data(), sizeof(float) * s->n_in);
-  else memset(ev.h_far, 0, sizeof(float) * s->n_in);
+// In front of the gate graph of step k on stream E, with echo cancellation: the step's far end (the samples given since the previous
+// step, else zeros), copied on every step through pinned slot k % kRing under the guard host_block_sync uses on stream E.
+static int far_sync(Session* s, long long k) {
+  if (k >= kRing) RYK_CUDA(cudaEventSynchronize(s->ev[k % kRing].gate));
+  float* slot = s->h_far + (size_t)(k % kRing) * s->n_in;
+  if (s->far_set) memcpy(slot, s->far_next.data(), sizeof(float) * s->n_in);
+  else memset(slot, 0, sizeof(float) * s->n_in);
   s->far_set = false;
-  RYK_CUDA(cudaMemcpyAsync(s->d_far_fixed, ev.h_far, sizeof(float) * s->n_in, cudaMemcpyHostToDevice, s->sE));
-  if (s->aec_dirty) {
-    *ev.h_aec = s->aec_params;
-    RYK_CUDA(cudaMemcpyAsync(s->aec.params, ev.h_aec, sizeof(EchoParams), cudaMemcpyHostToDevice, s->sE));
-    s->aec_dirty = false;
-  }
+  RYK_CUDA(cudaMemcpyAsync(s->input[kFar].d_fixed, slot, sizeof(float) * s->n_in, cudaMemcpyHostToDevice, s->sE));
+  return 0;
+}
+
+// Input i at the model rate, enqueued on stream E in the gate graph of a step of parity b: at a device input rate its history window
+// slides and its own copy of the streaming resampler runs, so the microphone and the far end stay aligned sample for sample.
+static int input_to_model(Engine* e, Session* s, int b, int i, const float** model) {
+  const InputSignal& x = s->input[i];
+  const InputState &p = s->par[b].input[i], &q = s->par[b ^ 1].input[i];
+  *model = x.d_fixed;
+  if (!s->in.rate) return 0;
+  if (slide<float>(p.win, x.d_fixed, q.win, s->in.hist, s->n_in, 1, s->sE)) return -1;
+  if (resample_stream_in_run(e, q.win, s->in.hist, s->n_in, s->delay_in, s->in.up, s->in.down, s->in.d_h, s->in.n_taps, p.rs, q.rs,
+                             x.d_model, s->n_wave, s->sE)) return -1;
+  *model = x.d_model;
   return 0;
 }
 
@@ -609,7 +632,7 @@ static int stage_time(Session* s, int stage, int which, int r, cudaStream_t st) 
   return 0;
 }
 
-// d_chunk_user: the caller's chunk in device memory, or nullptr when stage_in already copied it into d_chunk_fixed
+// d_chunk_user: the caller's chunk in device memory, or nullptr when stage_in already copied it into input[kMic].d_fixed
 static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
   const long long k = s->step;
   const int b = (int)(k & 1), r = (int)(k % kRing);
@@ -621,38 +644,29 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
   cudaStream_t sC2 = lane.stream;
 
   // ================= stream E: wave slides =================
-  if (d_chunk_user) RYK_CUDA(cudaMemcpyAsync(s->d_chunk_fixed, d_chunk_user, sizeof(float) * s->n_in, cudaMemcpyDeviceToDevice, s->sE));
+  if (d_chunk_user) RYK_CUDA(cudaMemcpyAsync(s->input[kMic].d_fixed, d_chunk_user, sizeof(float) * s->n_in, cudaMemcpyDeviceToDevice, s->sE));
   if (k >= 2) {
     RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev[(k - 2) % kRing].cslide, 0));  // q.cw_wave: last read by the silence gate in the head of stage 1 of k-2
     RYK_CUDA(cudaStreamWaitEvent(s->sE, s->ev[(k - 2) % kRing].enc, 0));     // q.wave_win: last read by the analysis of k-2
   }
-  if (dn_sync(s, k)) return -1;
-  if (s->echo && aec_sync(s, k)) return -1;
+  if (host_block_sync(s->dn_params, s->dn.params, k, ev.gate, s->sE)) return -1;
+  if (host_block_sync(s->aec_params, s->aec.params, k, ev.gate, s->sE)) return -1;
+  if (s->echo && far_sync(s, k)) return -1;
   if (stage_time(s, 0, 0, r, s->sE)) return -1;
   if (run_graph(e, p.graphs.gate, s->sE, [&]() -> int {
-        const float* chunk = s->d_chunk_fixed;
-        if (s->in.rate) {            // device rate -> fs in front of the wave slide
-          if (slide<float>(p.in_win, s->d_chunk_fixed, q.in_win, s->in.hist, s->n_in, 1, s->sE)) return -1;
-          if (resample_stream_in_run(e, q.in_win, s->in.hist, s->n_in, s->delay_in, s->in.up, s->in.down, s->in.d_h, s->in.n_taps,
-                                     p.in_st, q.in_st, s->d_chunk_model, s->n_wave, s->sE)) return -1;
-          chunk = s->d_chunk_model;
-        }
-        const float* far = s->d_far_fixed;
-        if (s->echo && s->in.rate) {  // the far end through its own copy of the input resampler, aligned with the microphone
-          if (slide<float>(p.far_win, s->d_far_fixed, q.far_win, s->in.hist, s->n_in, 1, s->sE)) return -1;
-          if (resample_stream_in_run(e, q.far_win, s->in.hist, s->n_in, s->delay_in, s->in.up, s->in.down, s->in.d_h, s->in.n_taps,
-                                     p.far_st, q.far_st, s->d_far_model, s->n_wave, s->sE)) return -1;
-          far = s->d_far_model;
-        }
+        const float *chunk = nullptr, *far = nullptr;
+        if (input_to_model(e, s, b, kMic, &chunk)) return -1;
+        if (s->echo && input_to_model(e, s, b, kFar, &far)) return -1;
         if (s->denoise || s->echo) {  // the frame stage in front of the wave slide: echo cancellation, then noise suppression
           const DenoiseWork& w = s->dn;
-          if (denoise_forward(e, w.max_frames, p.dn, q.dn, chunk, s->n_wave, w.spec, s->sE)) return -1;
+          const InputState &pm = p.input[kMic], &qm = q.input[kMic], &pf = p.input[kFar], &qf = q.input[kFar];
+          if (denoise_forward(e, w.max_frames, pm.dn, qm.dn, chunk, s->n_wave, w.spec, s->sE)) return -1;
           if (s->echo) {
-            if (denoise_forward(e, w.max_frames, p.far, q.far, far, s->n_wave, s->aec.far_spec, s->sE)) return -1;
-            if (echo_scan(s->aec, p.dn, s->n_wave, w.spec, s->sE)) return -1;
+            if (denoise_forward(e, w.max_frames, pf.dn, qf.dn, far, s->n_wave, s->aec.far_spec, s->sE)) return -1;
+            if (echo_scan(s->aec, pm.dn, s->n_wave, w.spec, s->sE)) return -1;
           }
-          if (s->denoise && denoise_scan(w, p.dn, q.dn, s->n_wave, s->sE)) return -1;
-          if (denoise_inverse(e, w, p.dn, q.dn, s->n_wave, s->d_chunk_dn, s->sE)) return -1;
+          if (s->denoise && denoise_scan(w, pm.dn, qm.dn, s->n_wave, s->sE)) return -1;
+          if (denoise_inverse(e, w, pm.dn, qm.dn, s->n_wave, s->d_chunk_dn, s->sE)) return -1;
           chunk = s->d_chunk_dn;
         }
         if (slide<float>(p.wave_win, chunk, q.wave_win, s->Lw, s->n_wave, 1, s->sE)) return -1;
@@ -686,7 +700,9 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
   // the mask / index / count of par[b] are written by the head and read by the SWITCH graph, both on stream C: no guard between steps
   // needed (nor for the f0 map: the host's copy, the measuring kernel in the head and the epilogue in the SWITCH graph are all on
   // stream C; the copy goes before the head so that it cannot overwrite what this step's measurement writes in follow mode)
-  if (f0_map_sync(s, k)) return -1;
+  if (s->f0_reset) RYK_CUDA(cudaMemsetAsync(s->d_f0_stats, 0, sizeof(F0Stats), s->sC));
+  s->f0_reset = false;
+  if (host_block_sync(s->f0_map, s->d_f0_map, k, ev.cslide, s->sC)) return -1;
   RYK_CUDA(cudaStreamWaitEvent(s->sC, ev.enc, 0));                             // (the analysis of step k waited for its wave slides)
   if (stage_time(s, 2, 0, r, s->sC)) return -1;
   if (run_graph(e, p.graphs.s1_head, s->sC, [&]() -> int { return stage1_head(e, s, b); })) return -1;
@@ -829,10 +845,10 @@ static int group_enqueue(Engine* e, Group* G, const float* const* d_chunks) {
 // The host slot of the caller's ticket: the session's own step alone, the group's step for a member.
 static HostSlot& host_slot(Session* s, long long ticket) { return s->io[ticket % kRing]; }
 
-// host chunk -> pinned slot -> d_chunk_fixed on stream E, in front of the step's wave slides
+// host chunk -> pinned slot -> input[kMic].d_fixed on stream E, in front of the step's wave slides
 static int stage_in(Session* s, HostSlot& io, const float* wave) {
   memcpy(io.h_in, wave, sizeof(float) * s->n_in);
-  RYK_CUDA(cudaMemcpyAsync(s->d_chunk_fixed, io.h_in, sizeof(float) * s->n_in, cudaMemcpyHostToDevice, s->sE));
+  RYK_CUDA(cudaMemcpyAsync(s->input[kMic].d_fixed, io.h_in, sizeof(float) * s->n_in, cudaMemcpyHostToDevice, s->sE));
   return 0;
 }
 
@@ -963,7 +979,6 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
   for (StepEvents& ev : s->ev) {
     for (cudaEvent_t* p : ev.all()) RYK_CUDA(cudaEventCreateWithFlags(p, cudaEventDisableTiming));
     if (s->stage_times) for (auto& pair : ev.tev) for (cudaEvent_t& t : pair) RYK_CUDA(cudaEventCreate(&t));
-    if (m.pinned(&ev.h_f0_map, 1)) return -1;
   }
   for (HostSlot& io : s->io) RYK_CUDA(cudaEventCreateWithFlags(&io.dec, cudaEventDisableTiming));
   s->max_blocks = (s->Td * s->hop) / cfg->vocoder_buffer_size + 4;
@@ -983,13 +998,12 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
     if (m.device(&o.mc_out, Tw * C) || m.device(&o.f0_out, Tw) || m.device(&o.ap_out, Tw * nb) || m.device(&o.sp_out, Tw * nb) ||
         m.device(&o.voiced_out, Tw) || m.device(&o.sp_mid, Tw * nb) || m.device(&o.formant, 1)) return -1;
   for (Stage2Lane& L : s->lane) if (m.device(&L.d_colmin, kColminFloats)) return -1;
-  if (m.device(&s->d_mse, Tw) || m.device(&s->dec_f0_f64, Td) || m.device(&s->d_chunk_fixed, s->n_wave)) return -1;
+  if (m.device(&s->d_mse, Tw) || m.device(&s->dec_f0_f64, Td) || input_alloc(s, kMic, s->n_in, false)) return -1;
   // the session starts on its voice's f0 map and an unwarped envelope
-  if (m.device(&s->d_f0_map, 1) || m.device(&s->d_f0_stats, 1)) return -1;
-  s->f0_map = voice_f0_map(s->voice);
-  s->f0_map.formant = 1.0;
-  *s->ev[0].h_f0_map = s->f0_map;
-  RYK_CUDA(cudaMemcpyAsync(s->d_f0_map, s->ev[0].h_f0_map, sizeof(F0Map), cudaMemcpyHostToDevice, e->stream));
+  if (m.device(&s->d_f0_map, 1) || m.device(&s->d_f0_stats, 1) || m.pinned(&s->f0_map.ring, kRing)) return -1;
+  s->f0_map.next = voice_f0_map(s->voice);
+  s->f0_map.next.formant = 1.0;
+  s->f0_map.dirty = true;
   for (HostSlot& io : s->io) if (m.pinned(&io.h_in, s->n_wave) || m.pinned(&io.h_out, s->max_out) || m.pinned(&io.h_n, 1)) return -1;
   // f0 method 2: each step's encode window is analysed on its own, like one crepe.predict call per fetched window (DESIGN.md C3)
   for (ParitySet& p : s->par) {
@@ -1094,13 +1108,12 @@ int ryk_session_push_device(ryk_engine* h, int id, const float* wave_dev, int n,
 //           samples before it.
 //   output: a step emits the outputs whose support ends inside the synthesizer samples so far; the kept history covers the left
 //           support of the first output not yet emitted, and max_out bounds one step's count.
-static int echo_alloc_far(Session* s);
-
 static int session_set_rate(Engine* e, int id, bool input, int rate, int up, int down, const double* taps, int n_taps) {
   RYK_CUDA(cudaSetDevice(e->device));
-  Session* s = get_session(e, id);
-  RYK_CHECK(s != nullptr, "no such session");
-  RYK_CHECK(s->step == 0 && s->group == nullptr, "device rates can only be set on a fresh session (no chunk pushed, not in a group)");
+  const char* refusal = "device rates can only be set on a fresh session (no chunk pushed, not in a group)";
+  Session* s = fresh_session(e, id, refusal);
+  if (!s) return -2;
+  RYK_CHECK(s->group == nullptr, refusal);
   Session::RateSide& side = input ? s->in : s->out;
   RYK_CHECK(side.rate == 0, "this side's device rate is already set");
   RYK_CHECK(rate > 0, "device rate must be positive");
@@ -1118,8 +1131,7 @@ static int session_set_rate(Engine* e, int id, bool input, int rate, int up, int
               "the chunk at this device rate is not a whole number of samples: round(rate * buffer_time) * up != round(fs * buffer_time) * down");
     const int delay = half / down;
     side.hist = n_in + (delay * down + half + up - 1) / up;
-    for (ParitySet& p : s->par) if (m.device(&p.in_win, side.hist) || m.device(&p.in_st, 1)) return -1;
-    if (m.device(&s->d_chunk_model, s->n_wave) || m.device(&s->d_chunk_fixed, n_in)) return -1;
+    for (int i = 0; i < kInputs; ++i) if (s->input[i].d_fixed && input_alloc(s, i, n_in, true)) return -1;
     for (HostSlot& io : s->io) if (m.pinned(&io.h_in, n_in)) return -1;
   } else {
     const long long blocks = (long long)s->max_blocks * s->cfg.vocoder_buffer_size;
@@ -1137,10 +1149,6 @@ static int session_set_rate(Engine* e, int id, bool input, int rate, int up, int
   if (input) {
     s->n_in = (int)lrint(s->cfg.buffer_time * rate);
     s->delay_in = half / down;
-    if (s->echo) {                                  // the far end's buffers at the new chunk length, and its resampler
-      if (echo_alloc_far(s)) return -1;
-      RYK_CUDA(cudaStreamSynchronize(e->stream));
-    }
   } else {
     s->max_out = (int)(((long long)s->max_blocks * s->cfg.vocoder_buffer_size * up + down - 1) / down);
   }
@@ -1167,12 +1175,13 @@ int ryk_session_io_geometry(ryk_engine* h, int id, int* n_in, int* max_out, int*
 }
 
 // ---- the session's f0 map and the statistics of its speaker (DESIGN.md §4a) ----
-// These calls change host state only; f0_map_sync carries it to the device at the next submitted step, alone or in a group.
+// These calls change host state only; host_block_sync carries it to the device at the next submitted step, alone or in a group.
 int ryk_session_get_f0_map(ryk_engine* h, int id, ryk_f0_map* map) {
   Session* s = get_session(&h->impl, id);
   RYK_CHECK(s != nullptr, "no such session");
   RYK_CHECK(map != nullptr, "null argument");
-  map->in_mean = s->f0_map.mu_in; map->in_std = s->f0_map.sd_in; map->target_mean = s->f0_map.mu_tgt; map->target_std = s->f0_map.sd_tgt;
+  const F0Map& f = s->f0_map.next;
+  map->in_mean = f.mu_in; map->in_std = f.sd_in; map->target_mean = f.mu_tgt; map->target_std = f.sd_tgt;
   return 0;
 }
 
@@ -1183,17 +1192,17 @@ int ryk_session_set_f0_map(ryk_engine* h, int id, const ryk_f0_map* map) {
   RYK_CHECK(isfinite(map->in_mean) && isfinite(map->in_std) && isfinite(map->target_mean) && isfinite(map->target_std),
             "the f0 map must be finite");
   RYK_CHECK(map->in_std > 0 && map->target_std > 0, "the standard deviations of the f0 map must be positive");
-  s->f0_map.mu_in = map->in_mean; s->f0_map.sd_in = map->in_std; s->f0_map.mu_tgt = map->target_mean; s->f0_map.sd_tgt = map->target_std;
-  s->f0_map.has_stats = 1;
-  s->f0_dirty = true;
+  F0Map& f = s->f0_map.next;
+  f.mu_in = map->in_mean; f.sd_in = map->in_std; f.mu_tgt = map->target_mean; f.sd_tgt = map->target_std;
+  f.has_stats = 1;
+  s->f0_map.dirty = true;
   return 0;
 }
 
 int ryk_session_f0_measure(ryk_engine* h, int id, int enable) {
-  Session* s = get_session(&h->impl, id);
-  RYK_CHECK(s != nullptr, "no such session");
-  RYK_CHECK(s->step == 0, "f0 measurement can only be switched on a fresh session (no chunk pushed): the head of stage 1 is captured at the first steps");
-  RYK_CHECK(enable || !s->f0_map.follow, "the session follows its measurement: turn follow mode off first");
+  Session* s = fresh_session(&h->impl, id, "f0 measurement can only be switched on a fresh session (no chunk pushed): the head of stage 1 is captured at the first steps");
+  if (!s) return -2;
+  RYK_CHECK(enable || !s->f0_map.next.follow, "the session follows its measurement: turn follow mode off first");
   s->f0_measure = enable != 0;
   return 0;
 }
@@ -1203,13 +1212,13 @@ int ryk_session_f0_follow(ryk_engine* h, int id, int follow, int min_voiced_fram
   RYK_CHECK(s != nullptr, "no such session");
   if (follow) {
     RYK_CHECK(s->f0_measure, "follow mode needs f0 measurement (ryk_session_f0_measure)");
-    RYK_CHECK(s->f0_map.has_stats, "follow mode needs an f0 map: the voice has no f0 statistics and none were set on the session");
+    RYK_CHECK(s->f0_map.next.has_stats, "follow mode needs an f0 map: the voice has no f0 statistics and none were set on the session");
     RYK_CHECK(min_voiced_frames >= 1, "min_voiced_frames must be at least 1");
     RYK_CHECK(isfinite(sd_floor) && sd_floor > 0, "sd_floor must be finite and positive");
-    s->f0_map.min_voiced = min_voiced_frames; s->f0_map.sd_floor = sd_floor;
+    s->f0_map.next.min_voiced = min_voiced_frames; s->f0_map.next.sd_floor = sd_floor;
   }
-  s->f0_map.follow = follow != 0;
-  s->f0_dirty = true;
+  s->f0_map.next.follow = follow != 0;
+  s->f0_map.dirty = true;
   return 0;
 }
 
@@ -1218,7 +1227,7 @@ int ryk_session_f0_measure_reset(ryk_engine* h, int id) {
   RYK_CHECK(s != nullptr, "no such session");
   RYK_CHECK(s->f0_measure, "f0 measurement is not enabled for this session");
   s->f0_reset = true;
-  s->f0_dirty = true;            // follow mode: back to the host's input side until min_voiced_frames are counted again
+  s->f0_map.dirty = true;            // follow mode: back to the host's input side until min_voiced_frames are counted again
   return 0;
 }
 
@@ -1245,8 +1254,8 @@ int ryk_session_set_formant(ryk_engine* h, int id, double ratio) {
   Session* s = get_session(&h->impl, id);
   RYK_CHECK(s != nullptr, "no such session");
   RYK_CHECK(isfinite(ratio) && ratio >= 0.5 && ratio <= 2.0, "the formant ratio must be finite and within [0.5, 2]");
-  s->f0_map.formant = ratio;
-  s->f0_dirty = true;
+  s->f0_map.next.formant = ratio;
+  s->f0_map.dirty = true;
   return 0;
 }
 
@@ -1254,12 +1263,12 @@ int ryk_session_get_formant(ryk_engine* h, int id, double* ratio) {
   Session* s = get_session(&h->impl, id);
   RYK_CHECK(s != nullptr, "no such session");
   RYK_CHECK(ratio != nullptr, "null argument");
-  *ratio = s->f0_map.formant;
+  *ratio = s->f0_map.next.formant;
   return 0;
 }
 
 // ---- input noise suppression (DESIGN.md §4f) ----
-// The setters change host state only; dn_sync carries it to the device in front of the wave slides of the next submitted step.
+// The setters change host state only; host_block_sync carries it to the device in front of the wave slides of the next submitted step.
 static Session* denoise_session(Engine* e, int id) {
   Session* s = get_session(e, id);
   if (!s) set_error("no such session");
@@ -1277,11 +1286,11 @@ static int frame_stage_alloc(Engine* e, Session* s) {
   if (m.device(&w.spec, (size_t)kDnBins * w.max_frames) || m.device(&w.frames, (size_t)kDnN * w.max_frames) || m.device(&w.done, 1) ||
       m.device(&s->d_chunk_dn, s->n_wave))
     return -1;
-  for (ParitySet& p : s->par) if (m.device(&p.dn, 1)) return -1;
+  for (ParitySet& p : s->par) if (m.device(&p.input[kMic].dn, 1)) return -1;
   void* hp = nullptr;
   if (engine_pinned(e, sizeof(DenoiseState), &hp)) return -1;
   denoise_state_init((DenoiseState*)hp);
-  RYK_CUDA(cudaMemcpyAsync(s->par[0].dn, hp, sizeof(DenoiseState), cudaMemcpyHostToDevice, e->stream));
+  RYK_CUDA(cudaMemcpyAsync(s->par[0].input[kMic].dn, hp, sizeof(DenoiseState), cudaMemcpyHostToDevice, e->stream));
   RYK_CUDA(cudaStreamSynchronize(e->stream));      // the staging is the engine's, and the session's streams do not wait for its stream
   return 0;
 }
@@ -1289,21 +1298,18 @@ static int frame_stage_alloc(Engine* e, Session* s) {
 int ryk_session_denoise(ryk_engine* h, int id) {
   Engine* e = &h->impl;
   RYK_CUDA(cudaSetDevice(e->device));
-  Session* s = get_session(e, id);
-  RYK_CHECK(s != nullptr, "no such session");
-  RYK_CHECK(s->step == 0, "noise suppression can only be enabled on a fresh session (no chunk pushed): the wave slides are captured at the first steps");
+  Session* s = fresh_session(e, id, "noise suppression can only be enabled on a fresh session (no chunk pushed): the wave slides are captured at the first steps");
+  if (!s) return -2;
   if (s->denoise) return 0;
   if (frame_stage_alloc(e, s)) return -1;
   BufferSet& m = s->mem;
   DenoiseWork& w = s->dn;
-  if (m.device(&w.params, 1) || m.device(&w.learn, 1)) return -1;
-  for (StepEvents& ev : s->ev) if (m.pinned(&ev.h_dn, 1)) return -1;
+  if (m.device(&w.params, 1) || m.device(&w.learn, 1) || m.pinned(&s->dn_params.ring, kRing)) return -1;
   // the parameter block starts at 20 dB without a profile
-  s->dn_params = {};
-  s->dn_params.gain_floor = pow(10.0, -20.0 / 20.0);
-  *s->ev[0].h_dn = s->dn_params;
-  RYK_CUDA(cudaMemcpyAsync(w.params, s->ev[0].h_dn, sizeof(DenoiseParams), cudaMemcpyHostToDevice, e->stream));
-  RYK_CUDA(cudaStreamSynchronize(e->stream));      // the zero-fills and the copies: the session's streams do not wait for the engine stream
+  s->dn_params.next = {};
+  s->dn_params.next.gain_floor = pow(10.0, -20.0 / 20.0);
+  s->dn_params.dirty = true;
+  RYK_CUDA(cudaStreamSynchronize(e->stream));      // the zero-fills: the session's streams do not wait for the engine stream
   s->denoise = true;
   return 0;
 }
@@ -1312,8 +1318,8 @@ int ryk_session_set_denoise(ryk_engine* h, int id, double reduction_db) {
   Session* s = denoise_session(&h->impl, id);
   if (!s) return -2;
   if (int rc = denoise_check(reduction_db, nullptr)) return rc;
-  s->dn_params.gain_floor = pow(10.0, -reduction_db / 20.0);
-  s->dn_dirty = true;
+  s->dn_params.next.gain_floor = pow(10.0, -reduction_db / 20.0);
+  s->dn_params.dirty = true;
   return 0;
 }
 
@@ -1321,9 +1327,10 @@ int ryk_session_denoise_learn(ryk_engine* h, int id, long long n_frames) {
   Session* s = denoise_session(&h->impl, id);
   if (!s) return -2;
   RYK_CHECK(n_frames >= 1, "n_frames must be at least 1");
-  s->dn_params.learn_serial++;
-  s->dn_params.learn_frames = n_frames;
-  s->dn_dirty = true;
+  DenoiseParams& P = s->dn_params.next;
+  P.learn_serial++;
+  P.learn_frames = n_frames;
+  s->dn_params.dirty = true;
   return 0;
 }
 
@@ -1332,11 +1339,12 @@ int ryk_session_set_noise_profile(ryk_engine* h, int id, const double* phi) {
   if (!s) return -2;
   RYK_CHECK(phi != nullptr, "null argument");
   if (int rc = denoise_check(0.0, phi)) return rc;
-  memcpy(s->dn_params.phi, phi, sizeof(double) * kDnBins);
-  s->dn_params.profile_serial++;
-  s->dn_params.learn_serial++;                     // cancels a learning in progress
-  s->dn_params.learn_frames = 0;
-  s->dn_dirty = true;
+  DenoiseParams& P = s->dn_params.next;
+  memcpy(P.phi, phi, sizeof(double) * kDnBins);
+  P.profile_serial++;
+  P.learn_serial++;                                // cancels a learning in progress
+  P.learn_frames = 0;
+  s->dn_params.dirty = true;
   return 0;
 }
 
@@ -1351,7 +1359,7 @@ int ryk_session_noise_profile(ryk_engine* h, int id, double* phi, long long* fra
   RYK_CUDA(cudaMemcpyAsync(L, s->dn.learn, sizeof(DenoiseLearn), cudaMemcpyDeviceToHost, s->sE));
   RYK_CUDA(cudaStreamSynchronize(s->sE));          // behind the wave slides of every submitted step
   // requests not yet applied (not submitted yet: every submitted step's gain scan has run) are what the next step applies
-  const DenoiseParams& P = s->dn_params;
+  const DenoiseParams& P = s->dn_params.next;
   const bool new_profile = P.profile_serial != L->profile_serial, new_learn = P.learn_serial != L->learn_serial;
   if (phi) memcpy(phi, new_profile ? P.phi : L->phi, sizeof(double) * kDnBins);
   if (frames_left) *frames_left = new_learn ? P.learn_frames : L->remaining;
@@ -1359,20 +1367,8 @@ int ryk_session_noise_profile(ryk_engine* h, int id, double* phi, long long* fra
 }
 
 // ---- echo cancellation (DESIGN.md §4g) ----
-// The far end's buffers at the session's input chunk length n_in; with a device input rate, also its own resampler state pair.
-static int echo_alloc_far(Session* s) {
-  BufferSet& m = s->mem;
-  if (m.device(&s->d_far_fixed, s->n_in)) return -1;
-  for (StepEvents& ev : s->ev) if (m.pinned(&ev.h_far, s->n_in)) return -1;
-  if (s->in.rate) {
-    for (ParitySet& p : s->par) if (m.device(&p.far_win, s->in.hist) || m.device(&p.far_st, 1)) return -1;
-    if (m.device(&s->d_far_model, s->n_wave)) return -1;
-  }
-  s->far_next.assign(s->n_in, 0.f);
-  s->far_set = false;
-  return 0;
-}
-
+// The setters change host state only; host_block_sync and far_sync carry it to the device in front of the wave slides of the next
+// submitted step.
 static Session* echo_session(Engine* e, int id) {
   Session* s = get_session(e, id);
   if (!s) set_error("no such session");
@@ -1383,9 +1379,8 @@ static Session* echo_session(Engine* e, int id) {
 int ryk_session_echo_cancel(ryk_engine* h, int id, int taps, int delay_frames) {
   Engine* e = &h->impl;
   RYK_CUDA(cudaSetDevice(e->device));
-  Session* s = get_session(e, id);
-  RYK_CHECK(s != nullptr, "no such session");
-  RYK_CHECK(s->step == 0, "echo cancellation can only be enabled on a fresh session (no chunk pushed): the wave slides are captured at the first steps");
+  Session* s = fresh_session(e, id, "echo cancellation can only be enabled on a fresh session (no chunk pushed): the wave slides are captured at the first steps");
+  if (!s) return -2;
   RYK_CHECK(!s->echo, "echo cancellation is already enabled for this session");
   if (int rc = echo_check(taps, delay_frames, 0.0)) return rc;
   if (frame_stage_alloc(e, s)) return -1;
@@ -1393,17 +1388,15 @@ int ryk_session_echo_cancel(ryk_engine* h, int id, int taps, int delay_frames) {
   EchoWork& a = s->aec;
   a.taps = taps; a.delay = delay_frames;
   if (m.device(&a.params, 1) || m.device(&a.filter, 1) || m.device(&a.ring, (size_t)kDnBins * (taps + delay_frames)) ||
-      m.device(&a.far_spec, (size_t)kDnBins * s->dn.max_frames))
+      m.device(&a.far_spec, (size_t)kDnBins * s->dn.max_frames) || m.pinned(&s->aec_params.ring, kRing))
     return -1;
-  for (ParitySet& p : s->par) if (m.device(&p.far, 1)) return -1;     // zero: in_end 0, an empty history
-  for (StepEvents& ev : s->ev) if (m.pinned(&ev.h_aec, 1)) return -1;
-  if (echo_alloc_far(s)) return -1;
+  for (ParitySet& p : s->par) if (m.device(&p.input[kFar].dn, 1)) return -1;     // zero: in_end 0, an empty history
+  if (input_alloc(s, kFar, s->n_in, s->in.rate != 0)) return -1;
   // the filters start at zero; the residual suppression at 0 dB (gain 1)
-  s->aec_params = {};
-  s->aec_params.gain_floor = 1.0;
-  *s->ev[0].h_aec = s->aec_params;
-  RYK_CUDA(cudaMemcpyAsync(a.params, s->ev[0].h_aec, sizeof(EchoParams), cudaMemcpyHostToDevice, e->stream));
-  RYK_CUDA(cudaStreamSynchronize(e->stream));      // the zero-fills and the copy: the session's streams do not wait for the engine stream
+  s->aec_params.next = {};
+  s->aec_params.next.gain_floor = 1.0;
+  s->aec_params.dirty = true;
+  RYK_CUDA(cudaStreamSynchronize(e->stream));      // the zero-fills: the session's streams do not wait for the engine stream
   s->echo = true;
   return 0;
 }
@@ -1422,8 +1415,8 @@ int ryk_session_set_echo_suppression(ryk_engine* h, int id, double db) {
   Session* s = echo_session(&h->impl, id);
   if (!s) return -2;
   if (int rc = echo_check(1, 0, db)) return rc;
-  s->aec_params.gain_floor = pow(10.0, -db / 20.0);
-  s->aec_dirty = true;
+  s->aec_params.next.gain_floor = pow(10.0, -db / 20.0);
+  s->aec_params.dirty = true;
   return 0;
 }
 
@@ -1613,7 +1606,7 @@ int ryk_session_set_voice(ryk_engine* h, int id, int voice_id) {
             "collect every submitted chunk of the session and of its group before switching its voice");
   RYK_CHECK(e->precision == s->precision && e->s1_fused == s->s1_fused,
             "the engine's precision or stage-1 mode changed since the session was created: a session keeps the numerics it was created with");
-  RYK_CHECK(!s->f0_map.follow || v->has_f0_stats, "follow mode needs an f0 map: the voice has no f0 statistics (turn follow mode off first)");
+  RYK_CHECK(!s->f0_map.next.follow || v->has_f0_stats, "follow mode needs an f0 map: the voice has no f0 statistics (turn follow mode off first)");
   Group* G = s->group;
   Voice* const old = s->voice;
   if (G) {
@@ -1660,9 +1653,10 @@ int ryk_session_set_voice(ryk_engine* h, int id, int voice_id) {
   }
   // the new voice's f0 map, as a session created on it starts; the speaker statistics, follow mode and formant ratio stay
   const F0Map vm = voice_f0_map(v);
-  s->f0_map.mu_in = vm.mu_in; s->f0_map.sd_in = vm.sd_in; s->f0_map.mu_tgt = vm.mu_tgt; s->f0_map.sd_tgt = vm.sd_tgt;
-  s->f0_map.has_stats = vm.has_stats;
-  s->f0_dirty = true;
+  F0Map& f = s->f0_map.next;
+  f.mu_in = vm.mu_in; f.sd_in = vm.sd_in; f.mu_tgt = vm.mu_tgt; f.sd_tgt = vm.sd_tgt;
+  f.has_stats = vm.has_stats;
+  s->f0_map.dirty = true;
   return 0;
 }
 
