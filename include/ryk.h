@@ -399,6 +399,40 @@ int ryk_session_echo_stats(ryk_engine* e, int session_id, long long* frames, dou
 int ryk_echo_cancel(ryk_engine* e, const float* mic, const float* far, int n, int taps, int delay_frames, double suppression_db,
                     double reduction_db, const double* phi, float* z);
 
+/* Output limiter (DESIGN.md §4i, DECIDE L1-L4): a look-ahead peak limiter on the samples a session returns, at its output rate, after
+ * the NaN scrub and the output resampler.  With y the stream the session returns without it, in FP64:
+ *   g0[u] = 1 if G |y[u]| <= c else c / (G |y[u]|) (1 for u < 0), c = 10^(ceiling_db / 20), G = gain (the host's output scale: the
+ *   ceiling applies to G y, the played level, while the session keeps returning unscaled samples);
+ *   m[s] = min of g0[u] over u in [s - hold, s + lookahead - 1];  g[t] = (sum over s = t - lookahead + 1 .. t of m[s]) / lookahead,
+ *   summed in ascending s from 0.0;  z[t] = g[t] y[t].
+ * So |G z| <= c (1 + 1e-12); where G |y| <= c over the whole window z is y bit for bit; a lone peak lowers the gain with a linear ramp
+ * over lookahead samples, a hold of hold samples and a linear ramp back.  No sample-to-sample recursion: the streamed output is bitwise
+ * the whole-signal output.
+ * ryk_session_limiter: fresh session only (no chunk pushed), once; either order with ryk_session_set_output_rate (which re-derives the
+ *   limiter at the new rate).  lookahead_ms in [0.5, 10] gives lookahead = max(1, round(lookahead_ms * rate / 1000)) output-rate
+ *   samples, hold_ms in [0, 500] gives hold = round(hold_ms * rate / 1000), both fixed from then on (rounded half to even).  The
+ *   session then returns concat(zeros(lookahead), z): every step returns as many samples as before (max_out unchanged), the output
+ *   delay grows by lookahead and the last lookahead samples of a finite input stay in the limiter.  The limiter starts at
+ *   ceiling_db = -1 and gain = 1.  Three more kernels per step on the decode stream; a session without it runs exactly the kernels it
+ *   ran before.  With constant settings the session's output is bitwise concat(zeros(lookahead), ryk_limit(y)) over its length.
+ * ryk_session_set_limiter: ceiling_db in [-24, 0], gain finite and > 0, from the next submitted step on (g0[u] uses the settings of the
+ *   step that returns y[u] from upstream); allowed with chunks in flight and on a group member; no device wait, no kernel.
+ * ryk_session_get_limiter: the settings of the next step; lookahead and hold in output-rate samples (lookahead is the added output
+ *   delay).  Any pointer may be NULL.
+ * ryk_session_limiter_stats: waits for the decode stream of the submitted steps, then writes for the samples the last step returned
+ *   (the leading zeros excluded) the largest reduction -20 log10(min g) (0 when none) and the number of samples with g < 1.  Either
+ *   pointer may be NULL.
+ * ryk_limit: the same limiter over a whole signal on the same kernels: a fresh state, y zero outside [0, n), z = n samples with no
+ *   delay.
+ * Refused, changing nothing: an unknown session, enabling on a session that ran a step or twice, settings out of range or not finite,
+ * set / get / stats calls on a session without the limiter. */
+int ryk_session_limiter(ryk_engine* e, int session_id, double lookahead_ms, double hold_ms);
+int ryk_session_set_limiter(ryk_engine* e, int session_id, double ceiling_db, double gain);
+int ryk_session_get_limiter(ryk_engine* e, int session_id, double* ceiling_db, double* gain, int* lookahead, int* hold);
+int ryk_session_limiter_stats(ryk_engine* e, int session_id, double* reduction_db, long long* limited);
+int ryk_limit(ryk_engine* e, const double* y, int n, int rate, double lookahead_ms, double hold_ms, double ceiling_db, double gain,
+              double* z);
+
 /* Diagnostics: device timeline (ms) of the last <= 8 steps x 5 stages {gate, analysis, stage 1, stage 2, synthesis}; needs
  * RYK_STAGE_TIMES=1 in the environment at session creation.  start/end hold 40 floats; returns the number of steps. */
 int ryk_session_stage_times(ryk_engine* e, int session_id, float* start, float* end);

@@ -34,6 +34,7 @@
 #include "echo.h"
 #include "engine.h"
 #include "features.h"
+#include "limiter.h"
 #include "synth.h"
 #include "unet.h"
 
@@ -91,11 +92,13 @@ struct ParitySet {
   InputState input[kInputs];                     // the microphone's and the far end's input windows and stream state
   double* out_hist = nullptr;                    // device rates: kept synthesizer samples (out.hist)
   ResampleState* out_st = nullptr;               // device rates: the output resampler's position
+  LimHist lim;                                   // output limiter: the history of y and g0 and the stream position
   // inter-stage buffers
   float *enc_f0 = nullptr, *enc_sp = nullptr, *enc_ap = nullptr, *enc_mc = nullptr; uint8_t* enc_voiced = nullptr;
   uint8_t* d_mask = nullptr; int* d_index = nullptr; int* d_count = nullptr;     // silence gate
   double* d_out_fixed = nullptr; int* d_n_fixed = nullptr;      // blocks written by the (captured) decode graph
   double* d_rout_fixed = nullptr; int* d_rn_fixed = nullptr;    // their device-rate resampling
+  double* d_lim_out = nullptr;                   // output limiter: the samples the step returns (as many as the two above)
   cudaStream_t sA = nullptr;                     // WORLD analysis: two chunks' analyses may be in flight
   DioPlan* dio = nullptr;                        // f0 methods 0 and 1 (owned)
   CrepePlan* crepe = nullptr;                    // f0 method 2: one CREPE forward in place of DIO/Harvest (owned)
@@ -199,6 +202,13 @@ struct Session {
   std::vector<float> far_next;     // the far end of the next submitted step (ryk_session_echo_reference; zeros when none was given)
   bool far_set = false;
   float* h_far = nullptr;          // pinned staging of the far end: slot k % kRing (n_in samples) for step k
+  // Output limiter (ryk_session_limiter, DESIGN.md §4i): runs last in the synthesis graph, at the output rate.  Its settings block
+  // lim.params is a host block synced on stream D in front of the decode slides; the history is double-buffered by parity.
+  bool limiter = false;
+  double lim_lookahead_ms = 0.0, lim_hold_ms = 0.0;   // L and R follow the output rate (ryk_session_set_output_rate reallocates)
+  double lim_ceiling_db = 0.0;     // what the next submitted step uses, with lim_params.next.gain
+  LimWork lim;
+  HostBlock<LimParams> lim_params;
   BufferSet mem;                   // every device and pinned buffer above
 };
 
@@ -752,6 +762,12 @@ static int session_mid_single(Engine* e, Session* s) {
   return 0;
 }
 
+// the samples a step of parity b returns and their count: the synthesizer's blocks, or their device-rate resampling (synth_out), or
+// with the output limiter its output for them
+static double* synth_out(Session* s, int b) { return s->out.rate ? s->par[b].d_rout_fixed : s->par[b].d_out_fixed; }
+static double* step_out(Session* s, int b) { return s->limiter ? s->par[b].d_lim_out : synth_out(s, b); }
+static int* step_n_out(Session* s, int b) { return s->out.rate ? s->par[b].d_rn_fixed : s->par[b].d_n_fixed; }
+
 static int session_back(Engine* e, Session* s) {
   const long long k = s->step;
   const int b = (int)(k & 1), r = (int)(k % kRing);
@@ -784,6 +800,8 @@ static int session_back(Engine* e, Session* s) {
   if (stage_time(s, 4, 0, r, s->sD)) return -1;
   if (synth_host_advance(e, s->synth, s->Td, s->sD)) return -1;
   const int max_blocks = s->max_blocks;
+  // the limiter's settings: its pinned slot was last read by a copy of step k - kRing, ahead of that step's decode slides
+  if (host_block_sync(s->lim_params, s->lim.params, k, ev.dslide, s->sD)) return -1;
   if (run_handoff_graph(e, s, k, &HandoffGraphs::dec_slide, s->sD, [&](int h) -> int {
         const HandoffSlot& o = s->ho[h];
         SlideBatch sb; sb.n = 0;
@@ -802,10 +820,14 @@ static int session_back(Engine* e, Session* s) {
         if (synth_drain_async(e, s->synth, p.d_out_fixed, max_blocks, s->sD)) return -1;
         k_scrub<<<8, 256, 0, s->sD>>>(p.d_out_fixed, s->synth->dev.state, c.vocoder_buffer_size, max_blocks * c.vocoder_buffer_size, p.d_n_fixed);
         RYK_CUDA(cudaGetLastError());
-        if (!s->out.rate) return 0;
         // fs -> device rate: the outputs whose filter support the synthesizer has produced; the rest waits for the next step
-        return resample_stream_out_run(e, p.out_hist, q.out_hist, s->out.hist, p.d_out_fixed, p.d_n_fixed, s->out.up, s->out.down,
-                                       s->out.d_h, s->out.n_taps, p.out_st, q.out_st, p.d_rout_fixed, s->max_out, p.d_rn_fixed, s->sD);
+        if (s->out.rate &&
+            resample_stream_out_run(e, p.out_hist, q.out_hist, s->out.hist, p.d_out_fixed, p.d_n_fixed, s->out.up, s->out.down,
+                                    s->out.d_h, s->out.n_taps, p.out_st, q.out_st, p.d_rout_fixed, s->max_out, p.d_rn_fixed, s->sD))
+          return -1;
+        if (!s->limiter) return 0;
+        // the limiter last, at the output rate: it changes no upstream state
+        return limiter_run(s->lim, p.lim, q.lim, synth_out(s, b), step_n_out(s, b), p.d_lim_out, s->sD);
       })) return -1;
   if (stage_time(s, 4, 1, r, s->sD)) return -1;
   // the step's HostSlot::dec is recorded by stage_out after the copies it appends to stream D
@@ -851,10 +873,6 @@ static int stage_in(Session* s, HostSlot& io, const float* wave) {
   RYK_CUDA(cudaMemcpyAsync(s->input[kMic].d_fixed, io.h_in, sizeof(float) * s->n_in, cudaMemcpyHostToDevice, s->sE));
   return 0;
 }
-
-// the samples a step of parity b returns and their count: the synthesizer's blocks, or their device-rate resampling
-static double* step_out(Session* s, int b) { return s->out.rate ? s->par[b].d_rout_fixed : s->par[b].d_out_fixed; }
-static int* step_n_out(Session* s, int b) { return s->out.rate ? s->par[b].d_rn_fixed : s->par[b].d_n_fixed; }
 
 // after a step of s was enqueued: copy its samples and sample count to out / n_out (kind: to the host slot or to device buffers) behind
 // the decode stream and record io.dec.  The output buffers are those of the parity of the session's own step, which differs from the
@@ -1101,6 +1119,26 @@ int ryk_session_push_device(ryk_engine* h, int id, const float* wave_dev, int n,
   return 0;
 }
 
+// (Re)allocates the output limiter at the session's output rate and max_out (DECIDE L1): its shape, scratch, meter and settings block,
+// and each parity's history, position and output.  The settings block starts as zeros, so the next submitted step copies the settings.
+static int limiter_alloc(Session* s) {
+  BufferSet& m = s->mem;
+  LimWork& w = s->lim;
+  limiter_shape(s->out.rate ? s->out.rate : s->cfg.fs, s->lim_lookahead_ms, s->lim_hold_ms, &w.L, &w.R);
+  w.max_n = s->max_out;
+  size_t n_g0, n_t32, n_t1k, n_m;
+  limiter_scratch_sizes(w, &n_g0, &n_t32, &n_t1k, &n_m);
+  if (m.device(&w.params, 1) || m.device(&w.meter, 1) || m.device(&w.g0, n_g0) || m.device(&w.t32, n_t32) || m.device(&w.t1k, n_t1k) ||
+      m.device(&w.m, n_m))
+    return -1;
+  for (ParitySet& p : s->par)
+    if (m.device(&p.lim.g0, (size_t)w.R + 2 * w.L - 1) || m.device(&p.lim.y, w.L) || m.device(&p.lim.st, 1) ||
+        m.device(&p.d_lim_out, s->max_out))
+      return -1;
+  s->lim_params.dirty = true;
+  return 0;
+}
+
 // ---- device rates: the session takes chunks at in.rate and returns samples at out.rate, converting on its own streams ----
 // Geometry (DESIGN.md §4, DECIDE R1), with half = (n_taps - 1) / 2 and up / down = the resampler's output rate / input rate:
 //   input:  delay_in = half / down model samples, the smallest delay for which every sample of a step's model-rate chunk has its whole
@@ -1151,6 +1189,10 @@ static int session_set_rate(Engine* e, int id, bool input, int rate, int up, int
     s->delay_in = half / down;
   } else {
     s->max_out = (int)(((long long)s->max_blocks * s->cfg.vocoder_buffer_size * up + down - 1) / down);
+    if (s->limiter) {                               // the limiter's L, R and buffers at the new rate and max_out
+      if (limiter_alloc(s)) return -1;
+      RYK_CUDA(cudaStreamSynchronize(e->stream));
+    }
   }
   return 0;
 }
@@ -1434,6 +1476,70 @@ int ryk_session_echo_stats(ryk_engine* h, int id, long long* frames, double* erl
   for (int k = 0; k < kDnBins; ++k) { sd += f->sum_d[k]; sz += f->sum_z[k]; }
   if (frames) *frames = f->frames;
   if (erle_db) *erle_db = sd > 0.0 ? 10.0 * log10(sd / sz) : 0.0;
+  return 0;
+}
+
+// ---- output limiter (DESIGN.md §4i) ----
+// The setter changes host state only; host_block_sync carries it to the device in front of the decode slides of the next submitted step.
+static Session* limiter_session(Engine* e, int id) {
+  Session* s = get_session(e, id);
+  if (!s) set_error("no such session");
+  else if (!s->limiter) set_error("the output limiter is not enabled for this session (ryk_session_limiter)");
+  return s && s->limiter ? s : nullptr;
+}
+
+int ryk_session_limiter(ryk_engine* h, int id, double lookahead_ms, double hold_ms) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Session* s = fresh_session(e, id, "the output limiter can only be enabled on a fresh session (no chunk pushed): the synthesis graphs are captured at the first steps");
+  if (!s) return -2;
+  RYK_CHECK(!s->limiter, "the output limiter is already enabled for this session");
+  if (int rc = limiter_check_shape(lookahead_ms, hold_ms)) return rc;
+  s->lim_lookahead_ms = lookahead_ms;
+  s->lim_hold_ms = hold_ms;
+  if (s->mem.pinned(&s->lim_params.ring, kRing) || limiter_alloc(s)) return -1;
+  // the ceiling starts at -1 dB of the samples as returned (gain 1)
+  s->lim_ceiling_db = -1.0;
+  s->lim_params.next = limiter_params(-1.0, 1.0);
+  RYK_CUDA(cudaStreamSynchronize(e->stream));      // the zero-fills: the session's streams do not wait for the engine stream
+  s->limiter = true;
+  return 0;
+}
+
+int ryk_session_set_limiter(ryk_engine* h, int id, double ceiling_db, double gain) {
+  Session* s = limiter_session(&h->impl, id);
+  if (!s) return -2;
+  if (int rc = limiter_check_settings(ceiling_db, gain)) return rc;
+  s->lim_ceiling_db = ceiling_db;
+  s->lim_params.next = limiter_params(ceiling_db, gain);
+  s->lim_params.dirty = true;
+  return 0;
+}
+
+int ryk_session_get_limiter(ryk_engine* h, int id, double* ceiling_db, double* gain, int* lookahead, int* hold) {
+  Session* s = limiter_session(&h->impl, id);
+  if (!s) return -2;
+  if (ceiling_db) *ceiling_db = s->lim_ceiling_db;
+  if (gain) *gain = s->lim_params.next.gain;
+  if (lookahead) *lookahead = s->lim.L;
+  if (hold) *hold = s->lim.R;
+  return 0;
+}
+
+int ryk_session_limiter_stats(ryk_engine* h, int id, double* reduction_db, long long* limited) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Session* s = limiter_session(e, id);
+  if (!s) return -2;
+  void* hp = nullptr;
+  if (engine_pinned(e, sizeof(LimMeter), &hp)) return -1;
+  RYK_CUDA(cudaMemcpyAsync(hp, s->lim.meter, sizeof(LimMeter), cudaMemcpyDeviceToHost, s->sD));
+  RYK_CUDA(cudaStreamSynchronize(s->sD));          // behind the synthesis of every submitted step
+  const LimMeter* mt = (const LimMeter*)hp;
+  double g = 1.0;
+  memcpy(&g, &mt->min_bits, sizeof(double));
+  if (reduction_db) *reduction_db = mt->limited ? -20.0 * log10(g) : 0.0;
+  if (limited) *limited = (long long)mt->limited;
   return 0;
 }
 

@@ -12,7 +12,7 @@ import math
 import os
 import threading
 from pathlib import Path
-from typing import Dict, List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy
 
@@ -68,7 +68,8 @@ EXPORTED_SYMBOLS = [
     'ryk_session_f0_measured', 'ryk_session_set_formant', 'ryk_session_get_formant', 'ryk_stage2_convert_formant',
     'ryk_session_set_voice', 'ryk_session_denoise', 'ryk_session_set_denoise', 'ryk_session_denoise_learn', 'ryk_session_set_noise_profile',
     'ryk_session_noise_profile', 'ryk_denoise', 'ryk_session_echo_cancel', 'ryk_session_echo_reference', 'ryk_session_set_echo_suppression',
-    'ryk_session_echo_stats', 'ryk_echo_cancel',
+    'ryk_session_echo_stats', 'ryk_echo_cancel', 'ryk_session_limiter', 'ryk_session_set_limiter', 'ryk_session_get_limiter',
+    'ryk_session_limiter_stats', 'ryk_limit',
 ]
 
 SEMITONE = math.log(2.0) / 12.0          # one semitone in ln f0
@@ -78,6 +79,9 @@ NOISE_BINS = 257                         # bins of a noise profile: rfft of the 
 NOISE_HOP = 128                          # model samples per noise-suppression frame
 ECHO_TAPS = (1, 64)                      # echo canceller: filter lengths in frames a session or echo_cancel accepts
 ECHO_DELAY_FRAMES = (0, 256)             # ... and bulk delays of the far end in frames
+LIMITER_CEILING_DB = (-24.0, 0.0)        # output limiter: ceilings it accepts
+LIMITER_LOOKAHEAD_MS = (0.5, 10.0)       # ... look-ahead (the added output delay)
+LIMITER_HOLD_MS = (0.0, 500.0)           # ... and hold of a gain reduction
 
 
 class F0Map(ctypes.Structure):
@@ -734,6 +738,40 @@ class Engine(object):
         self._check(self.lib.ryk_echo_cancel(self._h, _fp(mic), _fp(far), len(mic), int(taps), int(delay_frames),
                                              ctypes.c_double(suppression_db), ctypes.c_double(reduction_db),
                                              _dp(phi) if phi is not None else None, _fp(z)))
+        return z
+
+    # ---- output limiter ----
+    def session_limiter(self, sid: int, lookahead_ms: float = 5.0, hold_ms: float = 50.0):
+        """Fresh session only: limit the samples the session returns so that `gain` times them stays under the ceiling, with a
+        look-ahead of `lookahead_ms` (0.5-10, rounded to whole samples at the output rate; the output delay grows by as much) and a hold
+        of `hold_ms` (0-500).  Starts at ceiling_db = -1, gain = 1; session_set_limiter changes them."""
+        self._check(self.lib.ryk_session_limiter(self._h, int(sid), ctypes.c_double(lookahead_ms), ctypes.c_double(hold_ms)))
+
+    def session_set_limiter(self, sid: int, ceiling_db: float, gain: float = 1.0):
+        """The ceiling (-24 to 0 dB of full scale) and the gain the host applies to the returned samples before it plays them, from the
+        next submitted step on (chunks in flight keep theirs)."""
+        self._check(self.lib.ryk_session_set_limiter(self._h, int(sid), ctypes.c_double(ceiling_db), ctypes.c_double(gain)))
+
+    def session_get_limiter(self, sid: int) -> Dict[str, float]:
+        """ceiling_db and gain of the next submitted step, lookahead and hold in output-rate samples (lookahead: the added delay)."""
+        c, g, la, ho = ctypes.c_double(), ctypes.c_double(), ctypes.c_int(), ctypes.c_int()
+        self._check(self.lib.ryk_session_get_limiter(self._h, int(sid), ctypes.byref(c), ctypes.byref(g), ctypes.byref(la), ctypes.byref(ho)))
+        return {'ceiling_db': c.value, 'gain': g.value, 'lookahead': la.value, 'hold': ho.value}
+
+    def session_limiter_stats(self, sid: int) -> Tuple[float, int]:
+        """(largest gain reduction in dB, samples with a gain below 1) over the samples the last submitted step returned; waits for the
+        submitted steps' synthesis."""
+        red, n = ctypes.c_double(), ctypes.c_longlong()
+        self._check(self.lib.ryk_session_limiter_stats(self._h, int(sid), ctypes.byref(red), ctypes.byref(n)))
+        return red.value, n.value
+
+    def limit(self, y, rate: int, lookahead_ms: float = 5.0, hold_ms: float = 50.0, ceiling_db: float = -1.0,
+              gain: float = 1.0) -> numpy.ndarray:
+        """The session's output limiter over a whole signal at `rate`: a fresh state, no delay, len(y) float64 samples out."""
+        y = numpy.ascontiguousarray(y, dtype=numpy.float64).ravel()
+        z = numpy.empty_like(y)
+        self._check(self.lib.ryk_limit(self._h, _dp(y), len(y), int(rate), ctypes.c_double(lookahead_ms), ctypes.c_double(hold_ms),
+                                       ctypes.c_double(ceiling_db), ctypes.c_double(gain), _dp(z)))
         return z
 
     def session_destroy(self, sid: int):

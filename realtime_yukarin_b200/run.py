@@ -73,14 +73,19 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
         engine=None, depth: int = 3, measure_input_statistics: Optional[Path] = None, follow_input_f0: Optional[int] = None,
         pitch: float = 0.0, formant: float = 0.0, denoise: Optional[float] = None, noise_profile: Optional[Path] = None,
         learn_noise: Optional[float] = None, save_noise_profile: Optional[Path] = None, echo_cancel: Optional[int] = None,
-        echo_delay: float = 0.0, echo_suppression: float = 0.0) -> int:
+        echo_delay: float = 0.0, echo_suppression: float = 0.0, limit: Optional[float] = None,
+        limit_lookahead: Optional[float] = None, limit_hold: Optional[float] = None) -> int:
     """`measure_input_statistics`: measure the speaker's log-f0 statistics during the run and write them to this file at the end;
     `follow_input_f0`: convert with the measured statistics once this many voiced frames are counted; `pitch`: semitones added to
     the target voice's mean f0; `formant`: semitones by which the converted spectral envelope moves; `denoise`: filter the input's
     noise ahead of the analysis with at most this many dB of attenuation, with the profile in `noise_profile` (.npy) or one learned from
     the first `learn_noise` seconds of input, and write the profile in use to `save_noise_profile` at the end; `echo_cancel`: cancel the
     echo of the played output in the input with a filter of this many 128-sample frames after a bulk delay of `echo_delay` ms, followed
-    by `echo_suppression` dB of residual-echo suppression."""
+    by `echo_suppression` dB of residual-echo suppression; `limit`: keep the played output under this ceiling (dB of full scale) with a
+    look-ahead peak limiter of `limit_lookahead` ms (the output delay grows by as much; 5 when None) holding each reduction for
+    `limit_hold` ms (50 when None)."""
+    if limit is None and (limit_lookahead is not None or limit_hold is not None):
+        raise ValueError('--limit_lookahead and --limit_hold need --limit')
     if echo_cancel is None and (echo_delay or echo_suppression):
         raise ValueError('--echo_delay and --echo_suppression need --echo_cancel')
     if denoise is None and (noise_profile is not None or learn_noise is not None or save_noise_profile is not None):
@@ -97,7 +102,9 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
                                 denoise=denoise, noise_profile=None if noise_profile is None else numpy.load(noise_profile),
                                 learn_noise=learn_noise, echo_cancel=echo_cancel is not None,
                                 echo_taps=32 if echo_cancel is None else echo_cancel, echo_delay_ms=echo_delay,
-                                echo_suppression=echo_suppression)
+                                echo_suppression=echo_suppression, limiter=limit,
+                                limiter_lookahead_ms=5.0 if limit_lookahead is None else limit_lookahead,
+                                limiter_hold_ms=50.0 if limit_hold is None else limit_hold)
     try:
         if pitch:
             pipeline.set_f0_map(semitones=pitch)
@@ -175,6 +182,13 @@ def make_parser() -> argparse.ArgumentParser:
                         help='with --echo_cancel: the bulk delay of the echo path ahead of the filter, in ms (up to 256 frames)')
     parser.add_argument('--echo_suppression', type=float, default=0.0, metavar='DB',
                         help='with --echo_cancel: suppress the residual echo by at most DB (0-40; 0 keeps the linear canceller)')
+    parser.add_argument('--limit', type=float, nargs='?', const=-1.0, default=None, metavar='CEILING_DB',
+                        help='keep the played output (after output_scale) under CEILING_DB of full scale with a look-ahead peak '
+                             'limiter on the GPU (-24 to 0, default -1), so that loud syllables do not clip at the sound card')
+    parser.add_argument('--limit_lookahead', type=float, default=None, metavar='MS',
+                        help='with --limit: look-ahead of the limiter in ms (0.5-10, default 5); the output delay grows by as much')
+    parser.add_argument('--limit_hold', type=float, default=None, metavar='MS',
+                        help='with --limit: how long a gain reduction is held before it ramps back, in ms (0-500, default 50)')
     return parser
 
 
@@ -184,7 +198,7 @@ def main(argv: Optional[Iterable[str]] = None) -> None:
         measure_input_statistics=args.measure_input_statistics, follow_input_f0=args.follow_input_f0, pitch=args.pitch,
         formant=args.formant, denoise=args.denoise, noise_profile=args.noise_profile, learn_noise=args.learn_noise,
         save_noise_profile=args.save_noise_profile, echo_cancel=args.echo_cancel, echo_delay=args.echo_delay,
-        echo_suppression=args.echo_suppression)
+        echo_suppression=args.echo_suppression, limit=args.limit, limit_lookahead=args.limit_lookahead, limit_hold=args.limit_hold)
 
 
 if __name__ == '__main__':

@@ -16,6 +16,7 @@ Start offsets: the reference starts every worker at `start_time = extra_time` (e
 pre-fills its windows with silence for exactly those offsets.
 """
 import logging
+import math
 import os
 import time
 from collections import deque
@@ -24,7 +25,7 @@ from typing import Any, Deque, List, Optional, Tuple
 import numpy
 
 from .config import Config, VocodeMode
-from .engine import Engine, SessionConfig, default_engine
+from .engine import LIMITER_CEILING_DB, LIMITER_HOLD_MS, LIMITER_LOOKAHEAD_MS, Engine, SessionConfig, default_engine
 
 
 class Item(object):
@@ -77,6 +78,21 @@ class OutputReblocker(object):
             self._rid = None
 
 
+def _check_limiter(ceiling_db: float, output_scale: float, lookahead_ms: float, hold_ms: float) -> None:
+    """the limiter's settings as Engine.session_limiter / session_set_limiter accept them, checked before a session exists"""
+    lo, hi = LIMITER_CEILING_DB
+    if not lo <= ceiling_db <= hi:
+        raise ValueError(f'the limiter ceiling must be within [{lo}, {hi}] dB')
+    if not (math.isfinite(output_scale) and output_scale > 0):
+        raise ValueError('the limiter needs a finite, positive output_scale')
+    lo, hi = LIMITER_LOOKAHEAD_MS
+    if not lo <= lookahead_ms <= hi:
+        raise ValueError(f'the limiter look-ahead must be within [{lo}, {hi}] ms')
+    lo, hi = LIMITER_HOLD_MS
+    if not lo <= hold_ms <= hi:
+        raise ValueError(f'the limiter hold must be within [{lo}, {hi}] ms')
+
+
 class RealtimePipeline(object):
     """encode_worker | convert_worker | decode_worker of one audio stream as one device-resident session.
 
@@ -95,12 +111,18 @@ class RealtimePipeline(object):
     `set_echo_suppression` changes it between chunks and `echo_stats` reads how much echo the last chunk lost.  The far end is what
     `process` returned: mic chunk i is paired with the next n_in samples of the played stream, which starts with one input chunk of
     zeros (chunk i with the output of chunk i - 1 when the chunk sizes are equal; silence where the output ran short).  It needs
-    input_rate == output_rate."""
+    input_rate == output_rate.  `limiter=CEILING_DB` (-24 to 0) keeps the played samples (the session's times output_scale) under
+    that ceiling with a look-ahead peak limiter on the device: `limiter_lookahead_ms` (0.5-10) of look-ahead, which the output delay
+    grows by, and `limiter_hold_ms` (0-500) of hold; `set_limiter` changes the ceiling between chunks and `limiter_stats` reads how
+    much the last chunk was limited.  With echo_cancel the far end is then the limited played stream."""
 
     def __init__(self, config: Config, acoustic_param=None, engine: Optional[Engine] = None, depth: int = 3, voice: int = 0,
                  measure_f0: bool = False, follow_f0: Optional[int] = None, formant: float = 0.0, denoise: Optional[float] = None,
                  noise_profile=None, learn_noise: Optional[float] = None, echo_cancel: bool = False, echo_taps: int = 32,
-                 echo_delay_ms: float = 0.0, echo_suppression: float = 0.0):
+                 echo_delay_ms: float = 0.0, echo_suppression: float = 0.0, limiter: Optional[float] = None,
+                 limiter_lookahead_ms: float = 5.0, limiter_hold_ms: float = 50.0):
+        if limiter is not None:
+            _check_limiter(float(limiter), float(config.output_scale), float(limiter_lookahead_ms), float(limiter_hold_ms))
         if echo_cancel and int(config.input_rate) != int(config.output_rate):
             raise ValueError('echo_cancel needs input_rate == output_rate: the played stream is the far end of the input')
         self.config = config
@@ -168,6 +190,10 @@ class RealtimePipeline(object):
             self.engine.session_echo_cancel(self._sid, taps=int(echo_taps), delay_ms=float(echo_delay_ms))
             self.engine.session_set_echo_suppression(self._sid, float(echo_suppression))
             self._played = numpy.zeros(config.in_audio_chunk, numpy.float32)   # the played stream not yet paired with an input chunk
+        self._limiter = limiter is not None
+        if self._limiter:             # the ceiling applies to the played level: the session's samples times output_scale
+            self.engine.session_limiter(self._sid, lookahead_ms=float(limiter_lookahead_ms), hold_ms=float(limiter_hold_ms))
+            self.engine.session_set_limiter(self._sid, float(limiter), gain=float(config.output_scale))
         if measure_f0 or follow_f0 is not None:
             self.engine.session_f0_measure(self._sid)
         if follow_f0 is not None:
@@ -216,6 +242,15 @@ class RealtimePipeline(object):
     def echo_stats(self) -> Tuple[int, float]:
         """(frames, echo return loss enhancement in dB) of the last chunk put (needs echo_cancel)."""
         return self.engine.session_echo_stats(self._sid)
+
+    def set_limiter(self, ceiling_db: float) -> None:
+        """Engine.session_set_limiter for this stream: the ceiling of the played samples in dB of full scale, from the next chunk on
+        (needs limiter)."""
+        self.engine.session_set_limiter(self._sid, ceiling_db, gain=float(self.config.output_scale))
+
+    def limiter_stats(self) -> Tuple[float, int]:
+        """(largest gain reduction in dB, samples limited) of the last chunk put (needs limiter)."""
+        return self.engine.session_limiter_stats(self._sid)
 
     def measured_f0(self) -> Tuple[int, float, float]:
         """(voiced frames, mean, standard deviation) of the speaker's ln f0 over the chunks put so far (needs measure_f0)."""
