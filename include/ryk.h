@@ -433,6 +433,38 @@ int ryk_session_limiter_stats(ryk_engine* e, int session_id, double* reduction_d
 int ryk_limit(ryk_engine* e, const double* y, int n, int rate, double lookahead_ms, double hold_ms, double ceiling_db, double gain,
               double* z);
 
+/* Automatic gain control (DESIGN.md §4j, DECIDE A1-A4): brings the speaker to a target level ahead of the WORLD analysis.  It runs on
+ * the model-rate signal x the analysis would read (after the input resampler, the echo canceller and the noise suppression; the leading
+ * zeros of delay_in included), in FP64 with + - * / sqrt min max only:
+ *   P_m = mean of x^2 over block m = [256 m, 256 m + 256) (global positions; squares added in ascending order from 0.0);
+ *   a block is active when P_m > Gt = 10^(gate_db / 10); the level E is P_m at the first active block, then E += a (P_m - E) at each
+ *   active block, a = -expm1(-256 / (0.4 fs)); an inactive block leaves E and the gain;
+ *   on an active block g_m = min(max(g*, g_{m-1} s_dn), g_{m-1} s_up), g* = min(max(sqrt(T / E), 1 / gmax), gmax),
+ *   T = 10^(target_db / 10), gmax = 10^(max_gain_db / 20), s_up = 10^(6 * 256 / (20 fs)), s_dn = 10^(-24 * 256 / (20 fs))
+ *   (at most +6 / -24 dB per second); g_m = 1 for m < 0;
+ *   z[t] = (float)((g_{m-2} + (g_{m-1} - g_{m-2}) (j + 1) / 256) x[t]) for t = 256 m + j.
+ * The gain uses only blocks completed before the sample: it is causal, continuous and adds no delay.  With max_gain_db = 0 from a
+ * fresh state, or an input that never passes the gate, z is x bit for bit.
+ * ryk_session_agc: fresh session only (no chunk pushed), once; either order with ryk_session_denoise, _echo_cancel and
+ *   _set_input_rate (the AGC runs at the model rate, so no rate changes it).  One more kernel per step on the gate stream; delay_in,
+ *   ryk_session_io_geometry and every capacity are unchanged.  A session without it runs exactly the kernels it ran before.  With
+ *   constant settings the session analyses ryk_agc(x) bitwise, however the stream is cut into steps.
+ * ryk_session_set_agc: from the next submitted step on (block m uses the settings of the step that brings its last sample); allowed with
+ *   chunks in flight and on a group member; no device wait, no kernel.
+ * ryk_session_get_agc: the settings of the next submitted step, and in linear[7] (may be NULL) the values the device uses: T, Gt, gmax,
+ *   1 / gmax, a, s_up, s_dn, computed on the host with its libm.  Any pointer may be NULL.
+ * ryk_session_agc_stats: waits for the gate stream of the submitted steps, then writes 10 log10 E (-inf while no block has been
+ *   active), 20 log10 of the last completed block's gain, and the number of blocks completed in the last step that were active.  The
+ *   logarithms are taken on the host.  Any pointer may be NULL.
+ * ryk_agc: the same gain control over a whole signal at model rate fs on the same kernel: a fresh state, z = n samples, no delay.
+ * Refused, changing nothing: an unknown session, enabling on a session that ran a step or twice, settings not finite or outside
+ * target_db [-40, -6], max_gain_db [0, 30], gate_db [-80, -20], set / get / stats calls on a session without the AGC. */
+int ryk_session_agc(ryk_engine* e, int session_id, double target_db, double max_gain_db, double gate_db);
+int ryk_session_set_agc(ryk_engine* e, int session_id, double target_db, double max_gain_db, double gate_db);
+int ryk_session_get_agc(ryk_engine* e, int session_id, double* target_db, double* max_gain_db, double* gate_db, double* linear);
+int ryk_session_agc_stats(ryk_engine* e, int session_id, double* level_db, double* gain_db, int* active);
+int ryk_agc(ryk_engine* e, const float* x, int n, int fs, double target_db, double max_gain_db, double gate_db, float* z);
+
 /* Diagnostics: device timeline (ms) of the last <= 8 steps x 5 stages {gate, analysis, stage 1, stage 2, synthesis}; needs
  * RYK_STAGE_TIMES=1 in the environment at session creation.  start/end hold 40 floats; returns the number of steps. */
 int ryk_session_stage_times(ryk_engine* e, int session_id, float* start, float* end);

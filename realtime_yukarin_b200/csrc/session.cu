@@ -31,6 +31,7 @@
 #include <vector>
 
 #include "../../include/ryk.h"
+#include "agc.h"
 #include "echo.h"
 #include "engine.h"
 #include "features.h"
@@ -93,6 +94,7 @@ struct ParitySet {
   double* out_hist = nullptr;                    // device rates: kept synthesizer samples (out.hist)
   ResampleState* out_st = nullptr;               // device rates: the output resampler's position
   LimHist lim;                                   // output limiter: the history of y and g0 and the stream position
+  AgcState* agc = nullptr;                       // automatic gain control: the stream position, level, gains and block history
   // inter-stage buffers
   float *enc_f0 = nullptr, *enc_sp = nullptr, *enc_ap = nullptr, *enc_mc = nullptr; uint8_t* enc_voiced = nullptr;
   uint8_t* d_mask = nullptr; int* d_index = nullptr; int* d_count = nullptr;     // silence gate
@@ -209,6 +211,13 @@ struct Session {
   double lim_ceiling_db = 0.0;     // what the next submitted step uses, with lim_params.next.gain
   LimWork lim;
   HostBlock<LimParams> lim_params;
+  // Automatic gain control (ryk_session_agc, DESIGN.md §4j): runs in the wave-slide graph after the frame stage, at the model rate.  Its
+  // settings block agc.params is a host block synced on stream E in front of the graph; the state is double-buffered by parity.
+  bool agc = false;
+  double agc_db[3] = {};           // target, max gain and gate in dB of the next submitted step
+  AgcWork agcw;
+  HostBlock<AgcParams> agc_params;
+  float* d_chunk_agc = nullptr;    // the step's gain-controlled chunk (n_wave model-rate samples)
   BufferSet mem;                   // every device and pinned buffer above
 };
 
@@ -661,6 +670,7 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
   }
   if (host_block_sync(s->dn_params, s->dn.params, k, ev.gate, s->sE)) return -1;
   if (host_block_sync(s->aec_params, s->aec.params, k, ev.gate, s->sE)) return -1;
+  if (host_block_sync(s->agc_params, s->agcw.params, k, ev.gate, s->sE)) return -1;
   if (s->echo && far_sync(s, k)) return -1;
   if (stage_time(s, 0, 0, r, s->sE)) return -1;
   if (run_graph(e, p.graphs.gate, s->sE, [&]() -> int {
@@ -678,6 +688,10 @@ static int session_front(Engine* e, Session* s, const float* d_chunk_user) {
           if (s->denoise && denoise_scan(w, pm.dn, qm.dn, s->n_wave, s->sE)) return -1;
           if (denoise_inverse(e, w, pm.dn, qm.dn, s->n_wave, s->d_chunk_dn, s->sE)) return -1;
           chunk = s->d_chunk_dn;
+        }
+        if (s->agc) {                 // the gain control after the frame stage: a varying gain there would look like a moving echo path
+          if (agc_run(s->agcw, p.agc, q.agc, chunk, s->n_wave, s->d_chunk_agc, s->sE)) return -1;
+          chunk = s->d_chunk_agc;
         }
         if (slide<float>(p.wave_win, chunk, q.wave_win, s->Lw, s->n_wave, 1, s->sE)) return -1;
         return slide<float>(p.cw_wave, q.wave_win + (size_t)pe * s->hop, q.cw_wave, (size_t)s->Tw * s->hop, (size_t)s->n_feat * s->hop, 1, s->sE);
@@ -1540,6 +1554,87 @@ int ryk_session_limiter_stats(ryk_engine* h, int id, double* reduction_db, long 
   memcpy(&g, &mt->min_bits, sizeof(double));
   if (reduction_db) *reduction_db = mt->limited ? -20.0 * log10(g) : 0.0;
   if (limited) *limited = (long long)mt->limited;
+  return 0;
+}
+
+// ---- automatic gain control (DESIGN.md §4j) ----
+// The setter changes host state only; host_block_sync carries it to the device in front of the wave slides of the next submitted step.
+static Session* agc_session(Engine* e, int id) {
+  Session* s = get_session(e, id);
+  if (!s) set_error("no such session");
+  else if (!s->agc) set_error("the automatic gain control is not enabled for this session (ryk_session_agc)");
+  return s && s->agc ? s : nullptr;
+}
+
+static void agc_set_next(Session* s, double target_db, double max_gain_db, double gate_db) {
+  s->agc_db[0] = target_db; s->agc_db[1] = max_gain_db; s->agc_db[2] = gate_db;
+  s->agc_params.next = agc_params(s->cfg.fs, target_db, max_gain_db, gate_db);
+  s->agc_params.dirty = true;
+}
+
+// The AGC runs on the model-rate chunk, whose length n_wave no device rate changes: nothing here depends on ryk_session_set_input_rate.
+int ryk_session_agc(ryk_engine* h, int id, double target_db, double max_gain_db, double gate_db) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Session* s = fresh_session(e, id, "the automatic gain control can only be enabled on a fresh session (no chunk pushed): the wave slides are captured at the first steps");
+  if (!s) return -2;
+  RYK_CHECK(!s->agc, "the automatic gain control is already enabled for this session");
+  if (int rc = agc_check(target_db, max_gain_db, gate_db)) return rc;
+  BufferSet& m = s->mem;
+  AgcWork& w = s->agcw;
+  if (m.device(&w.params, 1) || m.device(&w.meter, 1) || m.device(&s->d_chunk_agc, s->n_wave) || m.pinned(&s->agc_params.ring, kRing))
+    return -1;
+  for (ParitySet& p : s->par) if (m.device(&p.agc, 1)) return -1;
+  // step 0 reads par[0]: position 0, gains 1, no level yet
+  void* hp = nullptr;
+  if (engine_pinned(e, sizeof(AgcState) + sizeof(AgcMeter), &hp)) return -1;
+  AgcState* st = (AgcState*)hp;
+  AgcMeter* mt = (AgcMeter*)(st + 1);
+  agc_state_init(st);
+  agc_meter_init(mt);
+  RYK_CUDA(cudaMemcpyAsync(s->par[0].agc, st, sizeof(AgcState), cudaMemcpyHostToDevice, e->stream));
+  RYK_CUDA(cudaMemcpyAsync(w.meter, mt, sizeof(AgcMeter), cudaMemcpyHostToDevice, e->stream));
+  RYK_CUDA(cudaStreamSynchronize(e->stream));      // the staging is the engine's, and the session's streams do not wait for its stream
+  agc_set_next(s, target_db, max_gain_db, gate_db);
+  s->agc = true;
+  return 0;
+}
+
+int ryk_session_set_agc(ryk_engine* h, int id, double target_db, double max_gain_db, double gate_db) {
+  Session* s = agc_session(&h->impl, id);
+  if (!s) return -2;
+  if (int rc = agc_check(target_db, max_gain_db, gate_db)) return rc;
+  agc_set_next(s, target_db, max_gain_db, gate_db);
+  return 0;
+}
+
+int ryk_session_get_agc(ryk_engine* h, int id, double* target_db, double* max_gain_db, double* gate_db, double* linear) {
+  Session* s = agc_session(&h->impl, id);
+  if (!s) return -2;
+  if (target_db) *target_db = s->agc_db[0];
+  if (max_gain_db) *max_gain_db = s->agc_db[1];
+  if (gate_db) *gate_db = s->agc_db[2];
+  if (linear) {
+    const AgcParams& P = s->agc_params.next;
+    const double v[7] = {P.target, P.gate, P.gmax, P.ginv, P.a, P.s_up, P.s_dn};
+    memcpy(linear, v, sizeof(v));
+  }
+  return 0;
+}
+
+int ryk_session_agc_stats(ryk_engine* h, int id, double* level_db, double* gain_db, int* active) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Session* s = agc_session(e, id);
+  if (!s) return -2;
+  void* hp = nullptr;
+  if (engine_pinned(e, sizeof(AgcMeter), &hp)) return -1;
+  RYK_CUDA(cudaMemcpyAsync(hp, s->agcw.meter, sizeof(AgcMeter), cudaMemcpyDeviceToHost, s->sE));
+  RYK_CUDA(cudaStreamSynchronize(s->sE));          // behind the wave slides of every submitted step
+  const AgcMeter* mt = (const AgcMeter*)hp;
+  if (level_db) *level_db = mt->started ? 10.0 * log10(mt->level) : -HUGE_VAL;
+  if (gain_db) *gain_db = 20.0 * log10(mt->gain);
+  if (active) *active = mt->active;
   return 0;
 }
 

@@ -12,7 +12,7 @@ import math
 import os
 import threading
 from pathlib import Path
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import numpy
 
@@ -69,7 +69,8 @@ EXPORTED_SYMBOLS = [
     'ryk_session_set_voice', 'ryk_session_denoise', 'ryk_session_set_denoise', 'ryk_session_denoise_learn', 'ryk_session_set_noise_profile',
     'ryk_session_noise_profile', 'ryk_denoise', 'ryk_session_echo_cancel', 'ryk_session_echo_reference', 'ryk_session_set_echo_suppression',
     'ryk_session_echo_stats', 'ryk_echo_cancel', 'ryk_session_limiter', 'ryk_session_set_limiter', 'ryk_session_get_limiter',
-    'ryk_session_limiter_stats', 'ryk_limit',
+    'ryk_session_limiter_stats', 'ryk_limit', 'ryk_session_agc', 'ryk_session_set_agc', 'ryk_session_get_agc', 'ryk_session_agc_stats',
+    'ryk_agc',
 ]
 
 SEMITONE = math.log(2.0) / 12.0          # one semitone in ln f0
@@ -82,6 +83,10 @@ ECHO_DELAY_FRAMES = (0, 256)             # ... and bulk delays of the far end in
 LIMITER_CEILING_DB = (-24.0, 0.0)        # output limiter: ceilings it accepts
 LIMITER_LOOKAHEAD_MS = (0.5, 10.0)       # ... look-ahead (the added output delay)
 LIMITER_HOLD_MS = (0.0, 500.0)           # ... and hold of a gain reduction
+AGC_TARGET_DB = (-40.0, -6.0)            # automatic gain control: target levels (mean square, dB of full scale) it accepts
+AGC_MAX_GAIN_DB = (0.0, 30.0)            # ... largest gain either way
+AGC_GATE_DB = (-80.0, -20.0)             # ... and gates: blocks at or under the gate leave level and gain as they are
+AGC_LINEAR = ('target', 'gate', 'gmax', 'ginv', 'a', 's_up', 's_dn')     # ryk_session_get_agc's linear values, in order
 
 
 class F0Map(ctypes.Structure):
@@ -772,6 +777,46 @@ class Engine(object):
         z = numpy.empty_like(y)
         self._check(self.lib.ryk_limit(self._h, _dp(y), len(y), int(rate), ctypes.c_double(lookahead_ms), ctypes.c_double(hold_ms),
                                        ctypes.c_double(ceiling_db), ctypes.c_double(gain), _dp(z)))
+        return z
+
+    # ---- automatic gain control ----
+    def session_agc(self, sid: int, target_db: float = -26.0, max_gain_db: float = 20.0, gate_db: float = -50.0):
+        """Fresh session only: bring the model-rate input to `target_db` (mean square, dB of full scale; -40 to -6) ahead of the
+        analysis, with at most `max_gain_db` (0-30) of gain or attenuation, over the 256-sample blocks whose mean square exceeds
+        `gate_db` (-80 to -20).  No delay; one more kernel per step."""
+        self._check(self.lib.ryk_session_agc(self._h, int(sid), ctypes.c_double(target_db), ctypes.c_double(max_gain_db),
+                                             ctypes.c_double(gate_db)))
+
+    def session_set_agc(self, sid: int, target_db: Optional[float] = None, max_gain_db: Optional[float] = None,
+                        gate_db: Optional[float] = None):
+        """New settings from the next submitted step on (chunks in flight keep theirs); a None keeps that setting."""
+        cur = self.session_get_agc(sid)
+        target_db = cur['target_db'] if target_db is None else target_db
+        max_gain_db = cur['max_gain_db'] if max_gain_db is None else max_gain_db
+        gate_db = cur['gate_db'] if gate_db is None else gate_db
+        self._check(self.lib.ryk_session_set_agc(self._h, int(sid), ctypes.c_double(target_db), ctypes.c_double(max_gain_db),
+                                                 ctypes.c_double(gate_db)))
+
+    def session_get_agc(self, sid: int) -> Dict[str, Any]:
+        """target_db, max_gain_db and gate_db of the next submitted step, and under 'linear' the values the device uses (AGC_LINEAR)."""
+        t, m, g = ctypes.c_double(), ctypes.c_double(), ctypes.c_double()
+        lin = numpy.zeros(len(AGC_LINEAR), numpy.float64)
+        self._check(self.lib.ryk_session_get_agc(self._h, int(sid), ctypes.byref(t), ctypes.byref(m), ctypes.byref(g), _dp(lin)))
+        return {'target_db': t.value, 'max_gain_db': m.value, 'gate_db': g.value, 'linear': dict(zip(AGC_LINEAR, lin.tolist()))}
+
+    def session_agc_stats(self, sid: int) -> Tuple[float, float, int]:
+        """(level in dB: 10 log10 E, -inf while no block has been active; gain of the last completed block in dB; active blocks among
+        those the last submitted step completed); waits for the submitted steps' input stage."""
+        level, gain, active = ctypes.c_double(), ctypes.c_double(), ctypes.c_int()
+        self._check(self.lib.ryk_session_agc_stats(self._h, int(sid), ctypes.byref(level), ctypes.byref(gain), ctypes.byref(active)))
+        return level.value, gain.value, active.value
+
+    def agc(self, x, fs: int, target_db: float = -26.0, max_gain_db: float = 20.0, gate_db: float = -50.0) -> numpy.ndarray:
+        """The session's gain control over a whole signal at model rate `fs`: a fresh state, no delay, len(x) float32 samples out."""
+        x = _f32(x)
+        z = numpy.empty_like(x)
+        self._check(self.lib.ryk_agc(self._h, _fp(x), len(x), int(fs), ctypes.c_double(target_db), ctypes.c_double(max_gain_db),
+                                     ctypes.c_double(gate_db), _fp(z)))
         return z
 
     def session_destroy(self, sid: int):

@@ -74,7 +74,8 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
         pitch: float = 0.0, formant: float = 0.0, denoise: Optional[float] = None, noise_profile: Optional[Path] = None,
         learn_noise: Optional[float] = None, save_noise_profile: Optional[Path] = None, echo_cancel: Optional[int] = None,
         echo_delay: float = 0.0, echo_suppression: float = 0.0, limit: Optional[float] = None,
-        limit_lookahead: Optional[float] = None, limit_hold: Optional[float] = None) -> int:
+        limit_lookahead: Optional[float] = None, limit_hold: Optional[float] = None, agc: Optional[float] = None,
+        agc_max_gain: Optional[float] = None, agc_gate: Optional[float] = None) -> int:
     """`measure_input_statistics`: measure the speaker's log-f0 statistics during the run and write them to this file at the end;
     `follow_input_f0`: convert with the measured statistics once this many voiced frames are counted; `pitch`: semitones added to
     the target voice's mean f0; `formant`: semitones by which the converted spectral envelope moves; `denoise`: filter the input's
@@ -83,7 +84,10 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
     echo of the played output in the input with a filter of this many 128-sample frames after a bulk delay of `echo_delay` ms, followed
     by `echo_suppression` dB of residual-echo suppression; `limit`: keep the played output under this ceiling (dB of full scale) with a
     look-ahead peak limiter of `limit_lookahead` ms (the output delay grows by as much; 5 when None) holding each reduction for
-    `limit_hold` ms (50 when None)."""
+    `limit_hold` ms (50 when None); `agc`: bring the speaker's level to this target (dB of full scale) ahead of the analysis with at most
+    `agc_max_gain` dB of gain (20 when None), counting only input louder than `agc_gate` dB (-50 when None)."""
+    if agc is None and (agc_max_gain is not None or agc_gate is not None):
+        raise ValueError('--agc_max_gain and --agc_gate need --agc')
     if limit is None and (limit_lookahead is not None or limit_hold is not None):
         raise ValueError('--limit_lookahead and --limit_hold need --limit')
     if echo_cancel is None and (echo_delay or echo_suppression):
@@ -104,7 +108,9 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
                                 echo_taps=32 if echo_cancel is None else echo_cancel, echo_delay_ms=echo_delay,
                                 echo_suppression=echo_suppression, limiter=limit,
                                 limiter_lookahead_ms=5.0 if limit_lookahead is None else limit_lookahead,
-                                limiter_hold_ms=50.0 if limit_hold is None else limit_hold)
+                                limiter_hold_ms=50.0 if limit_hold is None else limit_hold, agc=agc,
+                                agc_max_gain_db=20.0 if agc_max_gain is None else agc_max_gain,
+                                agc_gate_db=-50.0 if agc_gate is None else agc_gate)
     try:
         if pitch:
             pipeline.set_f0_map(semitones=pitch)
@@ -189,6 +195,14 @@ def make_parser() -> argparse.ArgumentParser:
                         help='with --limit: look-ahead of the limiter in ms (0.5-10, default 5); the output delay grows by as much')
     parser.add_argument('--limit_hold', type=float, default=None, metavar='MS',
                         help='with --limit: how long a gain reduction is held before it ramps back, in ms (0-500, default 50)')
+    parser.add_argument('--agc', type=float, nargs='?', const=-26.0, default=None, metavar='TARGET_DB',
+                        help='bring the speaker to TARGET_DB (mean square, dB of full scale; -40 to -6, default -26) ahead of the '
+                             'analysis with an automatic gain control on the GPU, after input_scale, echo cancellation and noise suppression')
+    parser.add_argument('--agc_max_gain', type=float, default=None, metavar='DB',
+                        help='with --agc: the most the gain control amplifies or attenuates, in dB (0-30, default 20)')
+    parser.add_argument('--agc_gate', type=float, default=None, metavar='DB',
+                        help='with --agc: blocks of input at or under this level (dB of full scale, -80 to -20, default -50) leave '
+                             'the level and the gain as they are')
     return parser
 
 
@@ -198,7 +212,8 @@ def main(argv: Optional[Iterable[str]] = None) -> None:
         measure_input_statistics=args.measure_input_statistics, follow_input_f0=args.follow_input_f0, pitch=args.pitch,
         formant=args.formant, denoise=args.denoise, noise_profile=args.noise_profile, learn_noise=args.learn_noise,
         save_noise_profile=args.save_noise_profile, echo_cancel=args.echo_cancel, echo_delay=args.echo_delay,
-        echo_suppression=args.echo_suppression, limit=args.limit, limit_lookahead=args.limit_lookahead, limit_hold=args.limit_hold)
+        echo_suppression=args.echo_suppression, limit=args.limit, limit_lookahead=args.limit_lookahead, limit_hold=args.limit_hold,
+        agc=args.agc, agc_max_gain=args.agc_max_gain, agc_gate=args.agc_gate)
 
 
 if __name__ == '__main__':

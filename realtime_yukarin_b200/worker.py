@@ -25,7 +25,8 @@ from typing import Any, Deque, List, Optional, Tuple
 import numpy
 
 from .config import Config, VocodeMode
-from .engine import LIMITER_CEILING_DB, LIMITER_HOLD_MS, LIMITER_LOOKAHEAD_MS, Engine, SessionConfig, default_engine
+from .engine import (AGC_GATE_DB, AGC_MAX_GAIN_DB, AGC_TARGET_DB, LIMITER_CEILING_DB, LIMITER_HOLD_MS, LIMITER_LOOKAHEAD_MS, Engine,
+                     SessionConfig, default_engine)
 
 
 class Item(object):
@@ -93,6 +94,14 @@ def _check_limiter(ceiling_db: float, output_scale: float, lookahead_ms: float, 
         raise ValueError(f'the limiter hold must be within [{lo}, {hi}] ms')
 
 
+def _check_agc(target_db: float, max_gain_db: float, gate_db: float) -> None:
+    """the AGC's settings as Engine.session_agc accepts them, checked before a session exists"""
+    for name, v, (lo, hi) in (('target', target_db, AGC_TARGET_DB), ('maximum gain', max_gain_db, AGC_MAX_GAIN_DB),
+                              ('gate', gate_db, AGC_GATE_DB)):
+        if not lo <= v <= hi:
+            raise ValueError(f'the AGC {name} must be within [{lo}, {hi}] dB')
+
+
 class RealtimePipeline(object):
     """encode_worker | convert_worker | decode_worker of one audio stream as one device-resident session.
 
@@ -114,13 +123,21 @@ class RealtimePipeline(object):
     input_rate == output_rate.  `limiter=CEILING_DB` (-24 to 0) keeps the played samples (the session's times output_scale) under
     that ceiling with a look-ahead peak limiter on the device: `limiter_lookahead_ms` (0.5-10) of look-ahead, which the output delay
     grows by, and `limiter_hold_ms` (0-500) of hold; `set_limiter` changes the ceiling between chunks and `limiter_stats` reads how
-    much the last chunk was limited.  With echo_cancel the far end is then the limited played stream."""
+    much the last chunk was limited.  With echo_cancel the far end is then the limited played stream.  `agc=TARGET_DB` (-40 to -6)
+    brings the speaker's level (mean square, dB of full scale) to that target ahead of the analysis with an automatic gain control on the
+    device, after the echo canceller and the noise filter: at most `agc_max_gain_db` (0-30) of gain either way, counting only the
+    256-sample blocks louder than `agc_gate_db` (-80 to -20).  It follows `input_scale`: the host still multiplies each chunk by it
+    first, so the gate applies to the scaled signal.  `set_agc` changes the settings between chunks and `agc_stats` reads the level
+    and gain."""
 
     def __init__(self, config: Config, acoustic_param=None, engine: Optional[Engine] = None, depth: int = 3, voice: int = 0,
                  measure_f0: bool = False, follow_f0: Optional[int] = None, formant: float = 0.0, denoise: Optional[float] = None,
                  noise_profile=None, learn_noise: Optional[float] = None, echo_cancel: bool = False, echo_taps: int = 32,
                  echo_delay_ms: float = 0.0, echo_suppression: float = 0.0, limiter: Optional[float] = None,
-                 limiter_lookahead_ms: float = 5.0, limiter_hold_ms: float = 50.0):
+                 limiter_lookahead_ms: float = 5.0, limiter_hold_ms: float = 50.0, agc: Optional[float] = None,
+                 agc_max_gain_db: float = 20.0, agc_gate_db: float = -50.0):
+        if agc is not None:
+            _check_agc(float(agc), float(agc_max_gain_db), float(agc_gate_db))
         if limiter is not None:
             _check_limiter(float(limiter), float(config.output_scale), float(limiter_lookahead_ms), float(limiter_hold_ms))
         if echo_cancel and int(config.input_rate) != int(config.output_rate):
@@ -194,6 +211,8 @@ class RealtimePipeline(object):
         if self._limiter:             # the ceiling applies to the played level: the session's samples times output_scale
             self.engine.session_limiter(self._sid, lookahead_ms=float(limiter_lookahead_ms), hold_ms=float(limiter_hold_ms))
             self.engine.session_set_limiter(self._sid, float(limiter), gain=float(config.output_scale))
+        if agc is not None:
+            self.engine.session_agc(self._sid, float(agc), float(agc_max_gain_db), float(agc_gate_db))
         if measure_f0 or follow_f0 is not None:
             self.engine.session_f0_measure(self._sid)
         if follow_f0 is not None:
@@ -251,6 +270,14 @@ class RealtimePipeline(object):
     def limiter_stats(self) -> Tuple[float, int]:
         """(largest gain reduction in dB, samples limited) of the last chunk put (needs limiter)."""
         return self.engine.session_limiter_stats(self._sid)
+
+    def set_agc(self, target_db: Optional[float] = None, max_gain_db: Optional[float] = None, gate_db: Optional[float] = None) -> None:
+        """Engine.session_set_agc for this stream: from the next chunk on; a None keeps that setting (needs agc)."""
+        self.engine.session_set_agc(self._sid, target_db, max_gain_db, gate_db)
+
+    def agc_stats(self) -> Tuple[float, float, int]:
+        """(level in dB, -inf before any active block; gain in dB; active blocks of the last chunk) of the chunks put (needs agc)."""
+        return self.engine.session_agc_stats(self._sid)
 
     def measured_f0(self) -> Tuple[int, float, float]:
         """(voiced frames, mean, standard deviation) of the speaker's ln f0 over the chunks put so far (needs measure_f0)."""
