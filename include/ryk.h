@@ -30,6 +30,7 @@
  */
 #ifndef RYK_H_
 #define RYK_H_
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -464,6 +465,65 @@ int ryk_session_set_agc(ryk_engine* e, int session_id, double target_db, double 
 int ryk_session_get_agc(ryk_engine* e, int session_id, double* target_db, double* max_gain_db, double* gate_db, double* linear);
 int ryk_session_agc_stats(ryk_engine* e, int session_id, double* level_db, double* gain_db, int* active);
 int ryk_agc(ryk_engine* e, const float* x, int n, int fs, double target_db, double max_gain_db, double gate_db, float* z);
+
+/* Moving a session (DESIGN.md §4k): a snapshot of a quiescent session's stream state, restored bit for bit as a new session on the same
+ * engine, another engine of the same device or an engine of another device.  After k steps of session A, a snapshot restored as B, the
+ * next chunks fed to A and B give the same outputs bit for bit: windows, resampler positions, the learned noise profile, the echo
+ * canceller's filters and far-end ring, the AGC's level and gains, the limiter's histories, the f0 statistics and f0 map, the
+ * synthesizer's rings and every setting made since the last step carry over.
+ * ryk_session_snapshot_size / ryk_session_snapshot: the session must be quiescent: every ryk_session_submit chunk collected, and for a
+ *   group member every ryk_group_submit chunk of its group.  The call waits for the session's streams, then copies its state into
+ *   `buf` (bytes = the size the first call returned) through one pinned staging buffer.  It changes nothing in the session, which
+ *   keeps running as if no snapshot had been taken.  A group member can be snapshotted: its stream state does not depend on the group.
+ * ryk_session_restore: creates a session on engine e converting into voice_id, with the configuration the blob records (session
+ *   config, device rates and their taps, f0 method, noise suppression, echo cancellation with its taps and delay, limiter with its
+ *   look-ahead and hold, AGC, f0 measuring), through the same code ryk_session_create and the enabling calls run, copies the state
+ *   into the new session's buffers and sets its step count to the source's.  *id receives the new session.  To restore a group,
+ *   restore its members and group them again (ryk_group_create / ryk_group_add).
+ *   voice_id names the source's voice as loaded on engine e: the stream continues, so the f0 map (both sides, a pitch offset or a
+ *   measured input side included) and the formant ratio are carried as they are and nothing of the voice's statistics is applied.  To
+ *   convert the moved stream into another voice, restore it and then call ryk_session_set_voice, which installs that voice's map.
+ *   Refused before anything is allocated: a malformed, truncated or corrupt blob, an unknown format version, an engine whose precision
+ *   or stage-1 mode differ from the recorded ones, a voice whose stage-1 or stage-2 (in, out, base) channels differ from the recorded
+ *   ones, CREPE (f0 method 2) without a complete CREPE model and resampler taps for the session's rate.  A failure later frees
+ *   whatever the call made.
+ * ryk_reblock_snapshot_size / ryk_reblock_snapshot / ryk_reblock_restore: the same for a re-blocker (its fragment, length and
+ *   ping-pong selector, and its push count); the snapshot waits for the re-blocker's last push.
+ * ryk_snapshot_describe (host only, no engine or device): verifies a blob's header, size, checksum and section walk and reports its
+ *   kind (1 session, 2 re-blocker, 3 pipeline), format version, the recorded configuration of a session or re-blocker (either
+ *   pointer may be NULL) and up to `capacity` section tags (four characters, first in the lowest byte) and payload sizes.  Returns the
+ *   number of sections.
+ * ryk_snapshot_seal (host only): writes the total size and the checksum into the header of a blob of `bytes` bytes whose magic,
+ *   version, kind and sections are in place (how a caller writes a blob of its own in the container, e.g. a pipeline blob). */
+typedef struct {
+  ryk_session_config cfg;
+  int voice_id;                              /* the source session's voice */
+  int precision, stage1_fused, f0_method;    /* the source engine's */
+  int stage1_channels[3], stage2_channels[3];   /* (in, out, base) of the voice's U-Nets */
+  int in_rate, in_up, in_down, in_taps;      /* device input rate (0: none) and its resampler */
+  int out_rate, out_up, out_down, out_taps;  /* device output rate (0: none) and its resampler */
+  int denoise, echo, echo_taps, echo_delay_frames, limiter, agc, f0_measure;
+  double limiter_lookahead_ms, limiter_hold_ms;
+  long long step;                            /* chunks the session has processed */
+} ryk_snapshot_session;
+typedef struct {
+  int out_audio_chunk, max_in, n_fft, hop;
+  double threshold_db;
+  long long pushed;
+} ryk_snapshot_reblock;
+int ryk_session_snapshot_size(ryk_engine* e, int session_id, size_t* bytes);
+int ryk_session_snapshot(ryk_engine* e, int session_id, void* buf, size_t bytes);
+int ryk_session_restore(ryk_engine* e, int voice_id, const void* buf, size_t bytes, int* session_id);
+int ryk_reblock_snapshot_size(ryk_engine* e, int reblock_id, size_t* bytes);
+int ryk_reblock_snapshot(ryk_engine* e, int reblock_id, void* buf, size_t bytes);
+int ryk_reblock_restore(ryk_engine* e, const void* buf, size_t bytes, int* reblock_id);
+int ryk_snapshot_describe(const void* buf, size_t bytes, int* kind, int* version, ryk_snapshot_session* session,
+                          ryk_snapshot_reblock* reblock, unsigned* tags, unsigned long long* sizes, int capacity);
+int ryk_snapshot_seal(void* buf, size_t bytes);
+/* Wall time of the engine's last successful snapshot or restore call, in ms: device_ms from enqueueing its staged copies to their end,
+ * host_ms the rest of the call (the waits for the session's streams, building the session, packing, parsing and the checksum).
+ * Either pointer may be NULL. */
+int ryk_snapshot_last_times(ryk_engine* e, double* host_ms, double* device_ms);
 
 /* Diagnostics: device timeline (ms) of the last <= 8 steps x 5 stages {gate, analysis, stage 1, stage 2, synthesis}; needs
  * RYK_STAGE_TIMES=1 in the environment at session creation.  start/end hold 40 floats; returns the number of steps. */

@@ -532,12 +532,17 @@ void crepe_plan_free(CrepePlan* p) {
 
 // A forward for n samples at fs, analysed with frame_period: the frames must coincide with WORLD's n / hop + 1.
 // Precision mode 1 runs the convolutions on the 3xTF32 tensor-core kernel, mode 0 on conv_direct (the FP32 bisect mode).
+const char* crepe_plan_refusal(int fs) {
+  if (!crepe_complete(g_crepe)) return "f0 method 2 (CREPE) needs a complete CREPE model and decoder tables: load one first (RYK_CREPE_MODEL)";
+  for (const CrepeResampler& x : g_crepe->resamplers) if (x.fs == fs) return nullptr;
+  return "f0 method 2 (CREPE): no resampler taps to 16 kHz for this sampling rate (ryk_crepe_set_resampler)";
+}
+
 int crepe_plan_create(Engine* e, int n, int fs, double frame_period, CrepePlan** out) {
+  if (const char* refusal = crepe_plan_refusal(fs)) { set_error(refusal); return -2; }
   CrepeModel* m = g_crepe;
-  RYK_CHECK(crepe_complete(m), "f0 method 2 (CREPE) needs a complete CREPE model and decoder tables: load one first (RYK_CREPE_MODEL)");
   const CrepeResampler* r = nullptr;
   for (const CrepeResampler& x : m->resamplers) if (x.fs == fs) r = &x;
-  RYK_CHECK(r != nullptr, "f0 method 2 (CREPE): no resampler taps to 16 kHz for this sampling rate (ryk_crepe_set_resampler)");
   const int hop = (int)(fs * frame_period / 1000.0), hop16 = (int)(16000 * frame_period / 1000);
   const int n16 = ryk_resample_length(n, r->up, r->down);
   RYK_CHECK(hop > 0 && hop16 > 0 && n > 0, "bad frame period or empty window");

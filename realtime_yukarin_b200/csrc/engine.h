@@ -102,6 +102,8 @@ struct Engine {
   bool profile = false;
   cudaEvent_t timer_ev[2] = {nullptr, nullptr};
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events;
+  // the last session or re-blocker snapshot / restore (ryk_snapshot_last_times): wall time waiting for its staged copies, and the rest
+  double snap_device_ms = 0.0, snap_host_ms = 0.0;
 };
 
 int engine_scratch(Engine* e, size_t bytes, void** out);
@@ -138,6 +140,8 @@ int crepe_set_tables(Engine* e, const double* log_trans, const double* cents_map
 int crepe_num_frames(int n16, double step_ms);
 int crepe_predict(Engine* e, const float* audio16k, int n, double step_ms, double* f0, float* confidence, int* voicing, float* activation, int* path_out);
 int crepe_set_resampler(Engine* e, int fs, int up, int down, const double* taps, int n_taps);
+// why a CREPE plan at rate fs cannot be made (no complete model, no resampler taps for fs), or nullptr
+const char* crepe_plan_refusal(int fs);
 int crepe_plan_create(Engine* e, int n, int fs, double frame_period, CrepePlan** out);
 void crepe_plan_free(CrepePlan* p);
 int crepe_plan_run(Engine* e, CrepePlan* p, const float* d_x, cudaStream_t st);

@@ -6,12 +6,14 @@
 #include "../../include/ryk.h"
 #include "engine.h"
 #include "features.h"
+#include "snapshot.h"
 
 namespace ryk {
 
 constexpr int kRing = 8;          // result slots: a push's results stay readable for 8 pushes
 
 struct ReblockState { int len, sel, overflow; };
+static_assert(sizeof(ReblockState) == 12, "snapshot layout: bump kSnapVersion (snapshot.h)");
 struct Reblock {
   int chunk = 0, max_in = 0, cap = 0, n_fft = 2048, hop = 512;
   double threshold_db = 80.0;
@@ -193,6 +195,92 @@ int ryk_reblock_push(ryk_engine* h, int id, const double* wave, int n, double* c
   long long ticket = 0;
   if (ryk_reblock_push_device(h, id, -1, R->d_stage_in, R->d_stage_n, &ticket)) return -1;
   return ryk_reblock_collect(h, id, ticket, chunk_out, status, power_db);
+}
+
+// ---- snapshot and restore (DESIGN.md §4k): RCNF (ryk_snapshot_reblock), RSTA ({len, sel, overflow}), RFR0 / RFR1 (the fragments).
+// The result slots are not carried: a restored re-blocker's pushes continue the ticket numbering from the recorded push count.
+static void reblock_conf(const Reblock* R, ryk_snapshot_reblock* c) {
+  memset(c, 0, sizeof(*c));
+  c->out_audio_chunk = R->chunk; c->max_in = R->max_in; c->n_fft = R->n_fft; c->hop = R->hop; c->threshold_db = R->threshold_db;
+  c->pushed = R->pushed;
+}
+static size_t reblock_blob_size(const Reblock* R) {
+  return snap_size({sizeof(ryk_snapshot_reblock), sizeof(ReblockState), sizeof(double) * R->cap, sizeof(double) * R->cap});
+}
+
+int ryk_reblock_snapshot_size(ryk_engine* h, int id, size_t* bytes) {
+  Reblock* R = get_reblock(&h->impl, id);
+  RYK_CHECK(R != nullptr && bytes != nullptr, "no such re-blocker");
+  *bytes = reblock_blob_size(R);
+  return 0;
+}
+
+int ryk_reblock_snapshot(ryk_engine* h, int id, void* buf, size_t bytes) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Reblock* R = get_reblock(e, id);
+  RYK_CHECK(R != nullptr && buf != nullptr, "no such re-blocker");
+  RYK_CHECK(bytes == reblock_blob_size(R), "the buffer must be exactly ryk_reblock_snapshot_size bytes");
+  if (R->pushed > 0) RYK_CUDA(cudaEventSynchronize(R->ev[(R->pushed - 1) % kRing]));     // pushes run in order on one stream each
+  const size_t frag = sizeof(double) * R->cap;
+  void* hp = nullptr;
+  if (engine_pinned(e, sizeof(ReblockState) + 2 * frag, &hp)) return -1;
+  uint8_t* st = (uint8_t*)hp;
+  RYK_CUDA(cudaMemcpyAsync(st, R->d_state, sizeof(ReblockState), cudaMemcpyDeviceToHost, e->stream));
+  RYK_CUDA(cudaMemcpyAsync(st + sizeof(ReblockState), R->d_frag[0], frag, cudaMemcpyDeviceToHost, e->stream));
+  RYK_CUDA(cudaMemcpyAsync(st + sizeof(ReblockState) + frag, R->d_frag[1], frag, cudaMemcpyDeviceToHost, e->stream));
+  RYK_CUDA(cudaStreamSynchronize(e->stream));
+  ryk_snapshot_reblock c;
+  reblock_conf(R, &c);
+  uint8_t* cur = snap_begin(buf, kSnapReblock);
+  memcpy(snap_section(&cur, snap_tag("RCNF"), sizeof(c)), &c, sizeof(c));
+  memcpy(snap_section(&cur, snap_tag("RSTA"), sizeof(ReblockState)), st, sizeof(ReblockState));
+  memcpy(snap_section(&cur, snap_tag("RFR0"), frag), st + sizeof(ReblockState), frag);
+  memcpy(snap_section(&cur, snap_tag("RFR1"), frag), st + sizeof(ReblockState) + frag, frag);
+  snap_finish(buf, bytes);
+  return 0;
+}
+
+int ryk_reblock_restore(ryk_engine* h, const void* buf, size_t bytes, int* reblock_id) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  RYK_CHECK(reblock_id != nullptr, "null argument");
+  uint32_t kind = 0, version = 0;
+  std::vector<SnapSection> sec;
+  if (const char* refusal = snap_parse(buf, bytes, &kind, &version, &sec)) { set_error(refusal); return -2; }
+  RYK_CHECK(kind == kSnapReblock, "not a re-blocker snapshot");
+  RYK_CHECK(sec.size() == 4 && sec[0].tag == snap_tag("RCNF") && sec[0].bytes == sizeof(ryk_snapshot_reblock) && sec[1].tag == snap_tag("RSTA") &&
+                sec[1].bytes == sizeof(ReblockState) && sec[2].tag == snap_tag("RFR0") && sec[3].tag == snap_tag("RFR1"),
+            "malformed re-blocker snapshot");
+  ryk_snapshot_reblock c;
+  memcpy(&c, sec[0].data, sizeof(c));
+  const size_t frag = sizeof(double) * (2 * (size_t)c.out_audio_chunk + 2 * (size_t)c.max_in);
+  RYK_CHECK(c.pushed >= 0 && sec[2].bytes == frag && sec[3].bytes == frag, "malformed re-blocker snapshot");
+  int id = -1;
+  if (int rc = ryk_reblock_create(h, c.out_audio_chunk, c.max_in, c.n_fft, c.hop, c.threshold_db, &id)) return rc;
+  Reblock* R = e->reblocks[id];
+  void* hp = nullptr;
+  int rc = engine_pinned(e, sizeof(ReblockState) + 2 * frag, &hp);
+  if (!rc) {
+    uint8_t* st = (uint8_t*)hp;
+    memcpy(st, sec[1].data, sizeof(ReblockState));
+    memcpy(st + sizeof(ReblockState), sec[2].data, frag);
+    memcpy(st + sizeof(ReblockState) + frag, sec[3].data, frag);
+    const cudaError_t err[4] = {cudaMemcpyAsync(R->d_state, st, sizeof(ReblockState), cudaMemcpyHostToDevice, e->stream),
+                                cudaMemcpyAsync(R->d_frag[0], st + sizeof(ReblockState), frag, cudaMemcpyHostToDevice, e->stream),
+                                cudaMemcpyAsync(R->d_frag[1], st + sizeof(ReblockState) + frag, frag, cudaMemcpyHostToDevice, e->stream),
+                                cudaStreamSynchronize(e->stream)};
+    for (cudaError_t x : err) if (x != cudaSuccess && !rc) { set_error(std::string("re-blocker restore copy failed: ") + cudaGetErrorString(x)); rc = -1; }
+  }
+  if (rc) {
+    const std::string cause = ryk_last_error();
+    ryk_reblock_destroy(h, id);
+    set_error(cause);
+    return rc;
+  }
+  R->pushed = c.pushed;
+  *reblock_id = id;
+  return 0;
 }
 
 }  // extern "C"

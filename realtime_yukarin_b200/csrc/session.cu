@@ -27,6 +27,7 @@
 #include <string.h>
 #include <algorithm>
 #include <array>
+#include <chrono>
 #include <numeric>
 #include <vector>
 
@@ -36,6 +37,7 @@
 #include "engine.h"
 #include "features.h"
 #include "limiter.h"
+#include "snapshot.h"
 #include "synth.h"
 #include "unet.h"
 
@@ -934,10 +936,10 @@ struct ryk_engine { Engine impl; };
 
 extern "C" {
 
-static int session_build(Engine* e, Session* s, const ryk_session_config* cfg);
+static int session_build(Engine* e, Session* s, const ryk_session_config* cfg, int f0_method);
 
-int ryk_session_create_voice(ryk_engine* h, const ryk_session_config* cfg, int voice_id, int* session_id) {
-  Engine* e = &h->impl;
+// The one way a session is made (ryk_session_create_voice, ryk_session_restore): f0_method is the engine's, or the one a snapshot records.
+static int session_create(Engine* e, const ryk_session_config* cfg, int voice_id, int f0_method, int* session_id) {
   RYK_CUDA(cudaSetDevice(e->device));
   RYK_CHECK(cfg && session_id, "null argument");
   Voice* v = engine_voice(e, voice_id);
@@ -949,11 +951,15 @@ int ryk_session_create_voice(ryk_engine* h, const ryk_session_config* cfg, int v
   }
   Session* s = new Session();
   s->voice = v; s->voice_id = voice_id;
-  if (session_build(e, s, cfg)) { session_free(s); return -1; }     // frees whatever the build made; ryk_last_error keeps the cause
+  if (session_build(e, s, cfg, f0_method)) { session_free(s); return -1; }     // frees whatever the build made; ryk_last_error keeps the cause
   v->users++;
   e->sessions.push_back(s);
   *session_id = (int)e->sessions.size() - 1;
   return 0;
+}
+
+int ryk_session_create_voice(ryk_engine* h, const ryk_session_config* cfg, int voice_id, int* session_id) {
+  return session_create(&h->impl, cfg, voice_id, h->impl.f0_method, session_id);
 }
 
 int ryk_session_create(ryk_engine* h, const ryk_session_config* cfg, int* session_id) { return ryk_session_create_voice(h, cfg, 0, session_id); }
@@ -965,7 +971,7 @@ int ryk_session_voice(ryk_engine* h, int id) {
 }
 
 // Everything a session allocates and captures; on failure the caller frees the partly built session.
-static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
+static int session_build(Engine* e, Session* s, const ryk_session_config* cfg, int f0_method) {
   s->cfg = *cfg;
   s->hop = (int)(cfg->fs * cfg->frame_period_ms / 1000.0);
   s->rate = (int)lround(1000.0 / cfg->frame_period_ms);
@@ -1039,8 +1045,8 @@ static int session_build(Engine* e, Session* s, const ryk_session_config* cfg) {
   for (HostSlot& io : s->io) if (m.pinned(&io.h_in, s->n_wave) || m.pinned(&io.h_out, s->max_out) || m.pinned(&io.h_n, 1)) return -1;
   // f0 method 2: each step's encode window is analysed on its own, like one crepe.predict call per fetched window (DESIGN.md C3)
   for (ParitySet& p : s->par) {
-    const int rc = e->f0_method == 2 ? crepe_plan_create(e, s->Lw, cfg->fs, cfg->frame_period_ms, &p.crepe)
-                                     : dio_plan_create(e, s->Lw, cfg->fs, cfg->frame_period_ms, cfg->f0_floor, cfg->f0_ceil, &p.dio, e->f0_method);
+    const int rc = f0_method == 2 ? crepe_plan_create(e, s->Lw, cfg->fs, cfg->frame_period_ms, &p.crepe)
+                                  : dio_plan_create(e, s->Lw, cfg->fs, cfg->frame_period_ms, cfg->f0_floor, cfg->f0_ceil, &p.dio, f0_method);
     if (rc) return -1;
   }
   if (synth_create(e, cfg->fs, cfg->frame_period_ms, cheaptrick_fft_size(cfg->fs, 71.0), cfg->vocoder_buffer_size, 4096, &s->synth)) return -1;
@@ -1966,6 +1972,338 @@ int ryk_session_stage_times(ryk_engine* h, int id, float* start, float* end) {
     }
   }
   return n;
+}
+
+// ---- moving a session: snapshot and restore (DESIGN.md §4k) ----
+// A session blob holds, in order: CONF (ryk_snapshot_session), TAPI / TAPO (the device rates' taps, when set), HOST (SnapHost), FARN
+// (the far end of the next step, with echo cancellation), then one section per device region of session_regions, in its order.
+
+// The host side of the stream state: every host block's next value and dirty flag, the f0 reset and far-end flags, the limiter's and
+// AGC's dB settings and the synthesizer's host counters.
+struct SnapHost {
+  long long step;
+  F0Map f0_next; DenoiseParams dn_next; EchoParams aec_next; LimParams lim_next; AgcParams agc_next;
+  double lim_ceiling_db, agc_db[3];
+  long long host_cum_frames, host_noise_generated;
+  int f0_dirty, dn_dirty, aec_dirty, lim_dirty, agc_dirty, f0_reset, far_set, host_noise_slot;
+};
+static_assert(sizeof(SnapHost) == 2320, "snapshot layout: bump kSnapVersion (snapshot.h)");
+
+// One device region of the stream state and the tag of its section.
+struct SnapRegion { uint32_t tag; void* dev; size_t bytes; };
+
+// The device regions that carry stream state, in blob order.  Both parities of every double-buffered region go in: step k reads
+// par[k & 1], and carrying par[k & 1 ^ 1] as well keeps the blob independent of which fields a step rewrites in full.  Everything else a
+// session owns is scratch or derived and goes in no section: the analysis outputs, silence-gate mask, hand-off slots, step outputs,
+// stage-2 lane scratch and per-step spectra (written by a step before it reads them), plans, graphs and events (rebuilt by the
+// restoring session), the resampler taps and constant tables (configuration).
+static std::vector<SnapRegion> session_regions(const Session* s) {
+  std::vector<SnapRegion> r;
+  auto add = [&](const char (&t)[5], const void* p, size_t bytes) { r.push_back({snap_tag(t), (void*)p, bytes}); };
+  const size_t Lw = s->Lw, Tw = s->Tw, Td = s->Td, nb = s->nb, C = s->C, hop = s->hop;
+  for (const ParitySet& p : s->par) {
+    add("WAVE", p.wave_win, sizeof(float) * Lw);
+    add("CWF0", p.cw_f0, sizeof(float) * Tw);
+    add("CWAP", p.cw_ap, sizeof(float) * Tw * nb);
+    add("CWMC", p.cw_mc, sizeof(float) * Tw * C);
+    add("CWVO", p.cw_voiced, Tw);
+    add("CWWV", p.cw_wave, sizeof(float) * Tw * hop);
+    add("DWF0", p.dw_f0, sizeof(float) * Td);
+    add("DWAP", p.dw_ap, sizeof(float) * Td * nb);
+    add("DWSP", p.dw_sp, sizeof(float) * Td * nb);
+    for (int i = 0; i < kInputs; ++i) {
+      const InputState& x = p.input[i];
+      if (x.win) {
+        add(i == kMic ? "MWIN" : "FWIN", x.win, sizeof(float) * s->in.hist);
+        add(i == kMic ? "MRES" : "FRES", x.rs, sizeof(ResampleState));
+      }
+      if (x.dn) add(i == kMic ? "MFRM" : "FFRM", x.dn, sizeof(DenoiseState));
+    }
+    if (p.out_hist) {
+      add("OHIS", p.out_hist, sizeof(double) * s->out.hist);
+      add("ORES", p.out_st, sizeof(ResampleState));
+    }
+    if (s->limiter) {
+      add("LG0H", p.lim.g0, sizeof(double) * (s->lim.R + 2 * s->lim.L - 1));
+      add("LYH ", p.lim.y, sizeof(double) * s->lim.L);
+      add("LPOS", p.lim.st, sizeof(LimState));
+    }
+    if (s->agc) add("AGCS", p.agc, sizeof(AgcState));
+  }
+  add("F0MP", s->d_f0_map, sizeof(F0Map));
+  add("F0ST", s->d_f0_stats, sizeof(F0Stats));
+  if (s->denoise) {
+    add("DNPA", s->dn.params, sizeof(DenoiseParams));
+    add("DNLE", s->dn.learn, sizeof(DenoiseLearn));
+  }
+  if (s->echo) {
+    add("AECP", s->aec.params, sizeof(EchoParams));
+    add("AECF", s->aec.filter, sizeof(EchoFilter));
+    add("AECR", s->aec.ring, sizeof(double2) * kDnBins * (s->aec.taps + s->aec.delay));
+  }
+  if (s->limiter) {
+    add("LIMP", s->lim.params, sizeof(LimParams));
+    add("LIMM", s->lim.meter, sizeof(LimMeter));
+  }
+  if (s->agc) {
+    add("AGCP", s->agcw.params, sizeof(AgcParams));
+    add("AGCM", s->agcw.meter, sizeof(AgcMeter));
+  }
+  const SynthDev& D = s->synth->dev;
+  const size_t sb = D.fft_size / 2 + 1;
+  add("SYST", D.state, sizeof(SynthState));
+  add("SYF0", D.f0, sizeof(double) * D.cap_frames);
+  add("SYSP", D.sp, sizeof(float) * D.cap_frames * sb);
+  add("SYAP", D.ap, sizeof(float) * D.cap_frames * sb);
+  add("SYPI", D.p_index, sizeof(long long) * D.cap_pulses);
+  add("SYPT", D.p_time, sizeof(double) * D.cap_pulses);
+  add("SYPV", D.p_vuv, sizeof(int) * D.cap_pulses);
+  add("SYNZ", D.noise, sizeof(uint32_t) * D.cap_noise);
+  add("SYC0", D.carry[0], sizeof(double) * D.carry_len);
+  add("SYC1", D.carry[1], sizeof(double) * D.carry_len);
+  return r;
+}
+
+static void unet_channels(const UNet* n, int* c) { c[0] = n->in_ch; c[1] = n->out_ch; c[2] = n->base; }
+
+// What a session's blob records besides its device regions.
+struct SessionBlob {
+  ryk_snapshot_session conf;
+  std::vector<double> taps_in, taps_out;
+  SnapHost host;
+  std::vector<SnapRegion> regions;
+  int far_n = 0;                   // far-end samples of the next step (echo cancellation)
+  std::vector<size_t> payloads() const {
+    std::vector<size_t> p = {sizeof(conf)};
+    if (conf.in_rate) p.push_back(sizeof(double) * taps_in.size());
+    if (conf.out_rate) p.push_back(sizeof(double) * taps_out.size());
+    p.push_back(sizeof(host));
+    if (conf.echo) p.push_back(sizeof(float) * far_n);
+    for (const SnapRegion& x : regions) p.push_back(x.bytes);
+    return p;
+  }
+};
+
+// The session when a snapshot may be taken, else nullptr with the refusal set.
+static Session* quiescent_session(Engine* e, int id) {
+  Session* s = get_session(e, id);
+  if (!s) { set_error("no such session"); return nullptr; }
+  if (!session_idle(s)) { set_error("the session has steps in flight: collect every submitted chunk before a snapshot"); return nullptr; }
+  if (s->group && s->group->collected != s->group->step) {
+    set_error("the session's group has steps in flight: collect every submitted group chunk before a snapshot");
+    return nullptr;
+  }
+  return s;
+}
+
+// The configuration and host state of s (the taps are read from the device: the caller has synchronised the session's streams).
+static int session_blob(Session* s, int f0_method, int precision, int s1_fused, SessionBlob* b) {
+  ryk_snapshot_session& c = b->conf;
+  memset(&c, 0, sizeof(c));
+  c.cfg = s->cfg;
+  c.voice_id = s->voice_id;
+  c.precision = precision; c.stage1_fused = s1_fused; c.f0_method = f0_method;
+  unet_channels(s->voice->stage1, c.stage1_channels);
+  unet_channels(s->voice->stage2, c.stage2_channels);
+  c.in_rate = s->in.rate; c.in_up = s->in.up; c.in_down = s->in.down; c.in_taps = s->in.n_taps;
+  c.out_rate = s->out.rate; c.out_up = s->out.up; c.out_down = s->out.down; c.out_taps = s->out.n_taps;
+  c.denoise = s->denoise; c.echo = s->echo; c.echo_taps = s->aec.taps; c.echo_delay_frames = s->aec.delay;
+  c.limiter = s->limiter; c.agc = s->agc; c.f0_measure = s->f0_measure;
+  c.limiter_lookahead_ms = s->lim_lookahead_ms; c.limiter_hold_ms = s->lim_hold_ms;
+  c.step = s->step;
+  b->taps_in.assign(c.in_taps, 0.0);
+  b->taps_out.assign(c.out_taps, 0.0);
+  if (c.in_rate) RYK_CUDA(cudaMemcpy(b->taps_in.data(), s->in.d_h, sizeof(double) * c.in_taps, cudaMemcpyDeviceToHost));
+  if (c.out_rate) RYK_CUDA(cudaMemcpy(b->taps_out.data(), s->out.d_h, sizeof(double) * c.out_taps, cudaMemcpyDeviceToHost));
+  SnapHost& h = b->host;
+  memset(&h, 0, sizeof(h));
+  h.step = s->step;
+  h.f0_next = s->f0_map.next; h.f0_dirty = s->f0_map.dirty; h.f0_reset = s->f0_reset;
+  h.dn_next = s->dn_params.next; h.dn_dirty = s->dn_params.dirty;
+  h.aec_next = s->aec_params.next; h.aec_dirty = s->aec_params.dirty; h.far_set = s->far_set;
+  h.lim_next = s->lim_params.next; h.lim_dirty = s->lim_params.dirty; h.lim_ceiling_db = s->lim_ceiling_db;
+  h.agc_next = s->agc_params.next; h.agc_dirty = s->agc_params.dirty;
+  for (int i = 0; i < 3; ++i) h.agc_db[i] = s->agc_db[i];
+  h.host_cum_frames = s->synth->host_cum_frames; h.host_noise_generated = s->synth->host_noise_generated;
+  h.host_noise_slot = s->synth->host_noise_slot;
+  b->far_n = s->echo ? s->n_in : 0;
+  b->regions = session_regions(s);
+  return 0;
+}
+
+static int session_f0_method(const Session* s) { return s->par[0].crepe ? 2 : dio_plan_harvest(s->par[0].dio) ? 1 : 0; }
+
+using Clock = std::chrono::steady_clock;
+static double ms_since(Clock::time_point t) { return std::chrono::duration<double, std::milli>(Clock::now() - t).count(); }
+
+int ryk_session_snapshot_size(ryk_engine* h, int id, size_t* bytes) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  RYK_CHECK(bytes != nullptr, "null argument");
+  Session* s = quiescent_session(e, id);
+  if (!s) return -2;
+  for (cudaStream_t st : s->streams()) RYK_CUDA(cudaStreamSynchronize(st));
+  SessionBlob b;
+  if (session_blob(s, session_f0_method(s), s->precision, s->s1_fused, &b)) return -1;
+  *bytes = snap_size(b.payloads());
+  return 0;
+}
+
+int ryk_session_snapshot(ryk_engine* h, int id, void* buf, size_t bytes) {
+  Engine* e = &h->impl;
+  const Clock::time_point t0 = Clock::now();
+  RYK_CUDA(cudaSetDevice(e->device));
+  RYK_CHECK(buf != nullptr, "null argument");
+  Session* s = quiescent_session(e, id);
+  if (!s) return -2;
+  for (cudaStream_t st : s->streams()) RYK_CUDA(cudaStreamSynchronize(st));
+  SessionBlob b;
+  if (session_blob(s, session_f0_method(s), s->precision, s->s1_fused, &b)) return -1;
+  const size_t total = snap_size(b.payloads());
+  RYK_CHECK(bytes == total, "the buffer must be exactly ryk_session_snapshot_size bytes");
+  size_t dev_bytes = 0;
+  for (const SnapRegion& x : b.regions) dev_bytes += x.bytes;
+  void* hp = nullptr;
+  if (engine_pinned(e, dev_bytes, &hp)) return -1;
+  const Clock::time_point t1 = Clock::now();
+  size_t off = 0;
+  for (const SnapRegion& x : b.regions) {
+    RYK_CUDA(cudaMemcpyAsync((uint8_t*)hp + off, x.dev, x.bytes, cudaMemcpyDeviceToHost, s->sE));
+    off += x.bytes;
+  }
+  RYK_CUDA(cudaStreamSynchronize(s->sE));
+  const double device_ms = ms_since(t1);
+  uint8_t* cur = snap_begin(buf, kSnapSession);
+  memcpy(snap_section(&cur, snap_tag("CONF"), sizeof(b.conf)), &b.conf, sizeof(b.conf));
+  if (b.conf.in_rate) memcpy(snap_section(&cur, snap_tag("TAPI"), sizeof(double) * b.taps_in.size()), b.taps_in.data(), sizeof(double) * b.taps_in.size());
+  if (b.conf.out_rate) memcpy(snap_section(&cur, snap_tag("TAPO"), sizeof(double) * b.taps_out.size()), b.taps_out.data(), sizeof(double) * b.taps_out.size());
+  memcpy(snap_section(&cur, snap_tag("HOST"), sizeof(b.host)), &b.host, sizeof(b.host));
+  if (b.conf.echo) memcpy(snap_section(&cur, snap_tag("FARN"), sizeof(float) * b.far_n), s->far_next.data(), sizeof(float) * b.far_n);
+  off = 0;
+  for (const SnapRegion& x : b.regions) {
+    memcpy(snap_section(&cur, x.tag, x.bytes), (const uint8_t*)hp + off, x.bytes);
+    off += x.bytes;
+  }
+  snap_finish(buf, total);
+  e->snap_device_ms = device_ms;
+  e->snap_host_ms = ms_since(t0) - device_ms;
+  return 0;
+}
+
+// The checks of a session blob that need no allocation: its configuration and sections, against engine e and voice voice_id.
+static int restore_check(Engine* e, int voice_id, const void* buf, size_t bytes, ryk_snapshot_session* c, std::vector<SnapSection>* sec) {
+  uint32_t kind = 0, version = 0;
+  if (const char* refusal = snap_parse(buf, bytes, &kind, &version, sec)) { set_error(refusal); return -2; }
+  RYK_CHECK(kind == kSnapSession, "not a session snapshot");
+  RYK_CHECK(!sec->empty() && (*sec)[0].tag == snap_tag("CONF") && (*sec)[0].bytes == sizeof(*c), "malformed session snapshot: no configuration");
+  memcpy(c, (*sec)[0].data, sizeof(*c));
+  RYK_CHECK(c->precision == e->precision && c->stage1_fused == (int)e->s1_fused,
+            "the engine's precision or stage-1 mode differ from those the snapshot records: a session keeps the numerics it was created with");
+  Voice* v = engine_voice(e, voice_id);
+  RYK_CHECK(v != nullptr, "no such voice");
+  RYK_CHECK(v->stage1 && v->stage2, "load both models before restoring a session");
+  int c1[3], c2[3];
+  unet_channels(v->stage1, c1);
+  unet_channels(v->stage2, c2);
+  RYK_CHECK(memcmp(c1, c->stage1_channels, sizeof(c1)) == 0 && memcmp(c2, c->stage2_channels, sizeof(c2)) == 0,
+            "the voice's stage-1 or stage-2 (in, out, base) channels differ from those the snapshot records");
+  RYK_CHECK(c->f0_method >= 0 && c->f0_method <= 2, "malformed session snapshot: unknown f0 method");
+  if (c->f0_method == 2) {
+    const char* refusal = crepe_plan_refusal(c->cfg.fs);
+    if (refusal) { set_error(refusal); return -2; }
+  }
+  // CONF, then TAPI / TAPO as the configuration says, HOST and FARN
+  size_t i = 1;
+  auto expect = [&](const char (&t)[5], size_t n) { return i < sec->size() && (*sec)[i].tag == snap_tag(t) && (*sec)[i++].bytes == n; };
+  RYK_CHECK(!c->in_rate || expect("TAPI", sizeof(double) * c->in_taps), "malformed session snapshot: input resampler taps");
+  RYK_CHECK(!c->out_rate || expect("TAPO", sizeof(double) * c->out_taps), "malformed session snapshot: output resampler taps");
+  RYK_CHECK(expect("HOST", sizeof(SnapHost)), "malformed session snapshot: host state");
+  if (c->echo) RYK_CHECK(i < sec->size() && (*sec)[i++].tag == snap_tag("FARN"), "malformed session snapshot: far end");
+  return 0;
+}
+
+// Enables on session id what the blob records, through the public calls; the settings given here are replaced by the recorded ones.
+static int restore_enable(ryk_engine* h, int id, const ryk_snapshot_session& c, const std::vector<SnapSection>& sec) {
+  size_t i = 1;
+  if (c.in_rate && ryk_session_set_input_rate(h, id, c.in_rate, c.in_up, c.in_down, (const double*)sec[i++].data, c.in_taps)) return -1;
+  if (c.out_rate && ryk_session_set_output_rate(h, id, c.out_rate, c.out_up, c.out_down, (const double*)sec[i++].data, c.out_taps)) return -1;
+  if (c.denoise && ryk_session_denoise(h, id)) return -1;
+  if (c.echo && ryk_session_echo_cancel(h, id, c.echo_taps, c.echo_delay_frames)) return -1;
+  if (c.limiter && ryk_session_limiter(h, id, c.limiter_lookahead_ms, c.limiter_hold_ms)) return -1;
+  if (c.agc && ryk_session_agc(h, id, -26.0, 20.0, -50.0)) return -1;
+  if (c.f0_measure && ryk_session_f0_measure(h, id, 1)) return -1;
+  return 0;
+}
+
+// Copies the blob's state into the new session s: its device regions through the engine's pinned staging, then its host state.
+static int restore_state(Engine* e, Session* s, const ryk_snapshot_session& c, const std::vector<SnapSection>& sec, double* device_ms) {
+  size_t i = 1 + (c.in_rate ? 1 : 0) + (c.out_rate ? 1 : 0);
+  SnapHost hs;
+  memcpy(&hs, sec[i++].data, sizeof(hs));
+  const SnapSection* far = c.echo ? &sec[i++] : nullptr;
+  RYK_CHECK(!far || far->bytes == sizeof(float) * s->n_in, "malformed session snapshot: far end");
+  const std::vector<SnapRegion> regions = session_regions(s);
+  RYK_CHECK(sec.size() - i == regions.size(), "the snapshot's state sections do not match the session its configuration makes");
+  size_t dev_bytes = 0;
+  for (size_t r = 0; r < regions.size(); ++r) {
+    RYK_CHECK(sec[i + r].tag == regions[r].tag && sec[i + r].bytes == regions[r].bytes,
+              "the snapshot's state sections do not match the session its configuration makes");
+    dev_bytes += regions[r].bytes;
+  }
+  void* hp = nullptr;
+  if (engine_pinned(e, dev_bytes, &hp)) return -1;
+  size_t off = 0;
+  for (size_t r = 0; r < regions.size(); ++r) { memcpy((uint8_t*)hp + off, sec[i + r].data, regions[r].bytes); off += regions[r].bytes; }
+  // on the engine stream, behind the zero-fills of the new buffers; the session's streams do not wait for it, so wait here
+  const Clock::time_point t1 = Clock::now();
+  off = 0;
+  for (const SnapRegion& x : regions) {
+    RYK_CUDA(cudaMemcpyAsync(x.dev, (const uint8_t*)hp + off, x.bytes, cudaMemcpyHostToDevice, e->stream));
+    off += x.bytes;
+  }
+  RYK_CUDA(cudaStreamSynchronize(e->stream));
+  *device_ms = ms_since(t1);
+  s->step = s->collected = hs.step;
+  s->f0_map.next = hs.f0_next; s->f0_map.dirty = hs.f0_dirty; s->f0_reset = hs.f0_reset;
+  s->dn_params.next = hs.dn_next; s->dn_params.dirty = hs.dn_dirty;
+  s->aec_params.next = hs.aec_next; s->aec_params.dirty = hs.aec_dirty;
+  if (far) memcpy(s->far_next.data(), far->data, far->bytes);
+  s->far_set = hs.far_set;
+  s->lim_params.next = hs.lim_next; s->lim_params.dirty = hs.lim_dirty; s->lim_ceiling_db = hs.lim_ceiling_db;
+  s->agc_params.next = hs.agc_next; s->agc_params.dirty = hs.agc_dirty;
+  for (int k = 0; k < 3; ++k) s->agc_db[k] = hs.agc_db[k];
+  s->synth->host_cum_frames = hs.host_cum_frames; s->synth->host_noise_generated = hs.host_noise_generated;
+  s->synth->host_noise_slot = hs.host_noise_slot;
+  return 0;
+}
+
+int ryk_session_restore(ryk_engine* h, int voice_id, const void* buf, size_t bytes, int* session_id) {
+  Engine* e = &h->impl;
+  const Clock::time_point t0 = Clock::now();
+  RYK_CUDA(cudaSetDevice(e->device));
+  RYK_CHECK(session_id != nullptr, "null argument");
+  ryk_snapshot_session c;
+  std::vector<SnapSection> sec;
+  if (int rc = restore_check(e, voice_id, buf, bytes, &c, &sec)) return rc;
+  int id = -1;
+  if (int rc = session_create(e, &c.cfg, voice_id, c.f0_method, &id)) return rc;
+  double device_ms = 0.0;
+  if (int rc = restore_enable(h, id, c, sec) ? -1 : restore_state(e, e->sessions[id], c, sec, &device_ms)) {
+    const std::string cause = ryk_last_error();
+    ryk_session_destroy(h, id);
+    set_error(cause);
+    return rc;
+  }
+  *session_id = id;
+  e->snap_device_ms = device_ms;
+  e->snap_host_ms = ms_since(t0) - device_ms;
+  return 0;
+}
+
+int ryk_snapshot_last_times(ryk_engine* h, double* host_ms, double* device_ms) {
+  if (host_ms) *host_ms = h->impl.snap_host_ms;
+  if (device_ms) *device_ms = h->impl.snap_device_ms;
+  return 0;
 }
 
 }  // extern "C"

@@ -41,6 +41,70 @@ class SessionConfig(ctypes.Structure):
     ]
 
 
+class SnapshotSession(ctypes.Structure):
+    """ryk_snapshot_session: the configuration a session snapshot records"""
+    _fields_ = [
+        ('cfg', SessionConfig), ('voice_id', ctypes.c_int), ('precision', ctypes.c_int), ('stage1_fused', ctypes.c_int),
+        ('f0_method', ctypes.c_int), ('stage1_channels', ctypes.c_int * 3), ('stage2_channels', ctypes.c_int * 3),
+        ('in_rate', ctypes.c_int), ('in_up', ctypes.c_int), ('in_down', ctypes.c_int), ('in_taps', ctypes.c_int),
+        ('out_rate', ctypes.c_int), ('out_up', ctypes.c_int), ('out_down', ctypes.c_int), ('out_taps', ctypes.c_int),
+        ('denoise', ctypes.c_int), ('echo', ctypes.c_int), ('echo_taps', ctypes.c_int), ('echo_delay_frames', ctypes.c_int),
+        ('limiter', ctypes.c_int), ('agc', ctypes.c_int), ('f0_measure', ctypes.c_int),
+        ('limiter_lookahead_ms', ctypes.c_double), ('limiter_hold_ms', ctypes.c_double), ('step', ctypes.c_longlong),
+    ]
+
+
+class SnapshotReblock(ctypes.Structure):
+    """ryk_snapshot_reblock: the configuration a re-blocker snapshot records"""
+    _fields_ = [('out_audio_chunk', ctypes.c_int), ('max_in', ctypes.c_int), ('n_fft', ctypes.c_int), ('hop', ctypes.c_int),
+                ('threshold_db', ctypes.c_double), ('pushed', ctypes.c_longlong)]
+
+
+SNAPSHOT_KINDS = {1: 'session', 2: 'reblock', 3: 'pipeline'}
+
+
+def _struct_dict(x) -> Dict[str, Any]:
+    out = {}
+    for name, _ in x._fields_:
+        v = getattr(x, name)
+        out[name] = _struct_dict(v) if isinstance(v, ctypes.Structure) else list(v) if isinstance(v, ctypes.Array) else v
+    return out
+
+
+def describe_snapshot(blob: bytes) -> Dict[str, Any]:
+    """ryk_snapshot_describe: verify a snapshot blob (header, size, FNV-1a-64 checksum, section walk) without an engine or a device.
+    Returns kind ('session' / 'reblock' / 'pipeline'), version, config (the recorded configuration of a session or re-blocker, as a
+    dict; None for a pipeline) and sections [(tag, payload bytes)] in blob order; raises RykError for a blob it refuses."""
+    lib = load_library()
+    blob = bytes(blob)
+    kind, version = ctypes.c_int(), ctypes.c_int()
+    ss, sr = SnapshotSession(), SnapshotReblock()
+    n = lib.ryk_snapshot_describe(blob, ctypes.c_size_t(len(blob)), ctypes.byref(kind), ctypes.byref(version), ctypes.byref(ss),
+                                  ctypes.byref(sr), None, None, 0)
+    if n < 0:
+        raise RykError(lib.ryk_last_error().decode('utf-8', 'replace'))
+    tags = (ctypes.c_uint * n)()
+    sizes = (ctypes.c_ulonglong * n)()
+    lib.ryk_snapshot_describe(blob, ctypes.c_size_t(len(blob)), None, None, None, None, tags, sizes, n)
+    names = [int(t).to_bytes(4, 'little').decode('ascii', 'replace') for t in tags]
+    k = SNAPSHOT_KINDS.get(kind.value, kind.value)
+    config = _struct_dict(ss) if k == 'session' else _struct_dict(sr) if k == 'reblock' else None
+    return {'kind': k, 'version': version.value, 'config': config, 'sections': list(zip(names, (int(x) for x in sizes)))}
+
+
+def _first_int(blob: bytes) -> int:
+    """the first int of the first section of a snapshot blob (after the 32-byte header and the 16-byte section header)"""
+    return int.from_bytes(blob[48:52], 'little', signed=True)
+
+
+def seal_snapshot(blob: bytearray) -> None:
+    """ryk_snapshot_seal: write the total size and the checksum into the header of a blob whose sections are in place."""
+    lib = load_library()
+    buf = (ctypes.c_char * len(blob)).from_buffer(blob)
+    if lib.ryk_snapshot_seal(buf, ctypes.c_size_t(len(blob))) < 0:
+        raise RykError(lib.ryk_last_error().decode('utf-8', 'replace'))
+
+
 _lib = None
 _lib_lock = threading.Lock()
 
@@ -70,7 +134,9 @@ EXPORTED_SYMBOLS = [
     'ryk_session_noise_profile', 'ryk_denoise', 'ryk_session_echo_cancel', 'ryk_session_echo_reference', 'ryk_session_set_echo_suppression',
     'ryk_session_echo_stats', 'ryk_echo_cancel', 'ryk_session_limiter', 'ryk_session_set_limiter', 'ryk_session_get_limiter',
     'ryk_session_limiter_stats', 'ryk_limit', 'ryk_session_agc', 'ryk_session_set_agc', 'ryk_session_get_agc', 'ryk_session_agc_stats',
-    'ryk_agc',
+    'ryk_agc', 'ryk_session_snapshot_size', 'ryk_session_snapshot', 'ryk_session_restore', 'ryk_reblock_snapshot_size',
+    'ryk_reblock_snapshot', 'ryk_reblock_restore', 'ryk_snapshot_describe', 'ryk_snapshot_seal',
+    'ryk_snapshot_last_times',
 ]
 
 SEMITONE = math.log(2.0) / 12.0          # one semitone in ln f0
@@ -818,6 +884,45 @@ class Engine(object):
         self._check(self.lib.ryk_agc(self._h, _fp(x), len(x), int(fs), ctypes.c_double(target_db), ctypes.c_double(max_gain_db),
                                      ctypes.c_double(gate_db), _fp(z)))
         return z
+
+    # ---- moving a session (DESIGN.md §4k) ----
+    def session_snapshot(self, sid: int) -> bytes:
+        """The stream state of a quiescent session (every submitted chunk collected) as a self-describing blob; the session itself is
+        not changed."""
+        n = ctypes.c_size_t()
+        self._check(self.lib.ryk_session_snapshot_size(self._h, sid, ctypes.byref(n)))
+        buf = ctypes.create_string_buffer(n.value)
+        self._check(self.lib.ryk_session_snapshot(self._h, sid, buf, n))
+        return buf.raw
+
+    def session_restore(self, blob: bytes, voice: int = 0) -> int:
+        """A new session on this engine, converting into `voice`, that continues the stream of the session the blob was taken from."""
+        blob = bytes(blob)
+        sid = ctypes.c_int()
+        self._check(self.lib.ryk_session_restore(self._h, int(voice), blob, ctypes.c_size_t(len(blob)), ctypes.byref(sid)))
+        self._session_fs[sid.value] = _first_int(blob)     # cfg.fs: the first field of the CONF section, which the call verified
+        return sid.value
+
+    def reblock_snapshot(self, rid: int) -> bytes:
+        """The fragment and push count of a re-blocker, after its last push."""
+        n = ctypes.c_size_t()
+        self._check(self.lib.ryk_reblock_snapshot_size(self._h, rid, ctypes.byref(n)))
+        buf = ctypes.create_string_buffer(n.value)
+        self._check(self.lib.ryk_reblock_snapshot(self._h, rid, buf, n))
+        return buf.raw
+
+    def reblock_restore(self, blob: bytes) -> int:
+        blob = bytes(blob)
+        rid = ctypes.c_int()
+        self._check(self.lib.ryk_reblock_restore(self._h, blob, ctypes.c_size_t(len(blob)), ctypes.byref(rid)))
+        self._reblock_chunk[rid.value] = _first_int(blob)  # out_audio_chunk: the first field of the RCNF section
+        return rid.value
+
+    def snapshot_last_times(self) -> Tuple[float, float]:
+        """(host ms, device ms) of this engine's last snapshot or restore call (ryk_snapshot_last_times)."""
+        host, dev = ctypes.c_double(), ctypes.c_double()
+        self._check(self.lib.ryk_snapshot_last_times(self._h, ctypes.byref(host), ctypes.byref(dev)))
+        return host.value, dev.value
 
     def session_destroy(self, sid: int):
         self._check(self.lib.ryk_session_destroy(self._h, sid))

@@ -20,7 +20,7 @@ from . import wave_io
 from .config import Config
 from .converter import YukarinConverter
 from .models import write_f0_statistics
-from .worker import RealtimePipeline
+from .worker import RealtimePipeline, unpack_pipeline
 
 
 def audio_loop(pipeline: RealtimePipeline, read_chunk: Callable[[], Optional[numpy.ndarray]],
@@ -69,13 +69,27 @@ def save_noise_profile_file(pipeline: RealtimePipeline, path: Path) -> None:
     print(f'wrote {path}')
 
 
+def save_state_file(pipeline: RealtimePipeline, path: Path) -> None:
+    """Write the stream state of `pipeline` to `path` for a later --load_state (after taking the outputs still in flight)."""
+    pipeline.drain()
+    Path(path).write_bytes(pipeline.snapshot())
+    print(f'wrote {path}')
+
+
+# options that set up the stream's stages, with the values that leave them off: a state file brings its own stages
+_STAGE_OPTIONS = {'follow_input_f0': None, 'pitch': 0.0, 'formant': 0.0, 'denoise': None, 'noise_profile': None, 'learn_noise': None,
+                  'echo_cancel': None, 'echo_delay': 0.0, 'echo_suppression': 0.0, 'limit': None, 'limit_lookahead': None,
+                  'limit_hold': None, 'agc': None, 'agc_max_gain': None, 'agc_gate': None}
+
+
 def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path] = None, max_chunks: Optional[int] = None,
         engine=None, depth: int = 3, measure_input_statistics: Optional[Path] = None, follow_input_f0: Optional[int] = None,
         pitch: float = 0.0, formant: float = 0.0, denoise: Optional[float] = None, noise_profile: Optional[Path] = None,
         learn_noise: Optional[float] = None, save_noise_profile: Optional[Path] = None, echo_cancel: Optional[int] = None,
         echo_delay: float = 0.0, echo_suppression: float = 0.0, limit: Optional[float] = None,
         limit_lookahead: Optional[float] = None, limit_hold: Optional[float] = None, agc: Optional[float] = None,
-        agc_max_gain: Optional[float] = None, agc_gate: Optional[float] = None) -> int:
+        agc_max_gain: Optional[float] = None, agc_gate: Optional[float] = None, save_state: Optional[Path] = None,
+        load_state: Optional[Path] = None) -> int:
     """`measure_input_statistics`: measure the speaker's log-f0 statistics during the run and write them to this file at the end;
     `follow_input_f0`: convert with the measured statistics once this many voiced frames are counted; `pitch`: semitones added to
     the target voice's mean f0; `formant`: semitones by which the converted spectral envelope moves; `denoise`: filter the input's
@@ -85,14 +99,30 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
     by `echo_suppression` dB of residual-echo suppression; `limit`: keep the played output under this ceiling (dB of full scale) with a
     look-ahead peak limiter of `limit_lookahead` ms (the output delay grows by as much; 5 when None) holding each reduction for
     `limit_hold` ms (50 when None); `agc`: bring the speaker's level to this target (dB of full scale) ahead of the analysis with at most
-    `agc_max_gain` dB of gain (20 when None), counting only input louder than `agc_gate` dB (-50 when None)."""
+    `agc_max_gain` dB of gain (20 when None), counting only input louder than `agc_gate` dB (-50 when None); `save_state`: write the
+    stream state (worker.RealtimePipeline.snapshot) to this file when the audio loop ends; `load_state`: continue the stream such a file
+    holds (learned noise profile, echo path, AGC level, f0 statistics and every setting), refused when it was written with another
+    configuration and with the options that set up stages, which the file brings; --save_noise_profile and --measure_input_statistics
+    then need the stage in the file."""
+    state = None
+    if load_state is not None:
+        values = locals()
+        given = [name for name, off in _STAGE_OPTIONS.items() if values[name] != off]
+        if given:
+            raise ValueError('--load_state brings the stages of the saved stream: drop ' + ', '.join('--' + n for n in given))
+        state = Path(load_state).read_bytes()
+        recorded = unpack_pipeline(state)['session_config']
+        if save_noise_profile is not None and not recorded['denoise']:
+            raise ValueError('--save_noise_profile needs noise suppression, which the stream in --load_state does not run')
+        if measure_input_statistics is not None and not recorded['f0_measure']:
+            raise ValueError('--measure_input_statistics needs f0 measuring, which the stream in --load_state does not run')
     if agc is None and (agc_max_gain is not None or agc_gate is not None):
         raise ValueError('--agc_max_gain and --agc_gate need --agc')
     if limit is None and (limit_lookahead is not None or limit_hold is not None):
         raise ValueError('--limit_lookahead and --limit_hold need --limit')
     if echo_cancel is None and (echo_delay or echo_suppression):
         raise ValueError('--echo_delay and --echo_suppression need --echo_cancel')
-    if denoise is None and (noise_profile is not None or learn_noise is not None or save_noise_profile is not None):
+    if denoise is None and (noise_profile is not None or learn_noise is not None or (save_noise_profile is not None and state is None)):
         raise ValueError('--noise_profile, --learn_noise and --save_noise_profile need --denoise')
     logger = logging.getLogger('root')
     logger.info('model loading...')
@@ -101,7 +131,10 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
         input_statistics_path=config.input_statistics_path, target_statistics_path=config.target_statistics_path,
         stage1_model_path=config.stage1_model_path, stage1_config_path=config.stage1_config_path,
         stage2_model_path=config.stage2_model_path, stage2_config_path=config.stage2_config_path)
-    pipeline = RealtimePipeline(config, acoustic_param=converter.acoustic_converter.config.dataset.acoustic_param, engine=engine, depth=depth,
+    if load_state is not None:
+        pipeline = RealtimePipeline.restore(state, config, engine=engine, depth=depth)
+    else:
+        pipeline = RealtimePipeline(config, acoustic_param=converter.acoustic_converter.config.dataset.acoustic_param, engine=engine, depth=depth,
                                 measure_f0=measure_input_statistics is not None, follow_f0=follow_input_f0, formant=formant,
                                 denoise=denoise, noise_profile=None if noise_profile is None else numpy.load(noise_profile),
                                 learn_noise=learn_noise, echo_cancel=echo_cancel is not None,
@@ -152,6 +185,8 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
             if save_noise_profile is not None:
                 pipeline.flush()
                 save_noise_profile_file(pipeline, save_noise_profile)
+            if save_state is not None:                # here too when Ctrl-C ends a live loop (SystemExit)
+                save_state_file(pipeline, save_state)
         finally:
             pipeline.close()
 
@@ -203,6 +238,12 @@ def make_parser() -> argparse.ArgumentParser:
     parser.add_argument('--agc_gate', type=float, default=None, metavar='DB',
                         help='with --agc: blocks of input at or under this level (dB of full scale, -80 to -20, default -50) leave '
                              'the level and the gain as they are')
+    parser.add_argument('--save_state', type=Path, default=None, metavar='OUT.state',
+                        help='when the audio loop ends, write the stream state (learned noise profile, echo path, AGC level, f0 '
+                             'statistics, settings) to this file for --load_state')
+    parser.add_argument('--load_state', type=Path, default=None, metavar='IN.state',
+                        help='continue the stream a --save_state file holds; the file must come from the same configuration and '
+                             'brings its own stages, so the stage options are refused with it')
     return parser
 
 
@@ -213,7 +254,7 @@ def main(argv: Optional[Iterable[str]] = None) -> None:
         formant=args.formant, denoise=args.denoise, noise_profile=args.noise_profile, learn_noise=args.learn_noise,
         save_noise_profile=args.save_noise_profile, echo_cancel=args.echo_cancel, echo_delay=args.echo_delay,
         echo_suppression=args.echo_suppression, limit=args.limit, limit_lookahead=args.limit_lookahead, limit_hold=args.limit_hold,
-        agc=args.agc, agc_max_gain=args.agc_max_gain, agc_gate=args.agc_gate)
+        agc=args.agc, agc_max_gain=args.agc_max_gain, agc_gate=args.agc_gate, save_state=args.save_state, load_state=args.load_state)
 
 
 if __name__ == '__main__':

@@ -15,6 +15,7 @@ index (run.py:152-199).  Here the three stages are CUDA streams of one device-re
 Start offsets: the reference starts every worker at `start_time = extra_time` (encode_worker.py:31); the session
 pre-fills its windows with silence for exactly those offsets.
 """
+import json
 import logging
 import math
 import os
@@ -397,9 +398,115 @@ class RealtimePipeline(object):
             outs.append((w * c.output_scale)[:c.out_audio_chunk].astype(numpy.float32))
         return outs
 
+    # ---- moving the stream (DESIGN.md §4k) ----------------------------------------------------------------------
+    def snapshot(self) -> bytes:
+        """The whole stream state as one blob: the session's, the re-blocker's and the pipeline's host state (the next item index,
+        the echo far-end queue, input_scale and output_scale).  Only a drained pipeline can be snapshotted: nothing in flight and
+        every finished item taken (`drain`)."""
+        if self._inflight or self._done or self._popped or self._index_output != self._index_input:
+            raise RuntimeError('the pipeline has chunks in flight or outputs not taken: drain() it before a snapshot')
+        return pack_pipeline(self.engine.session_snapshot(self._sid), self.engine.reblock_snapshot(self._rid),
+                             {'index': self._index_input, 'input_scale': float(self.config.input_scale),
+                              'output_scale': float(self.config.output_scale), 'echo': self._echo, 'limiter': self._limiter},
+                             self._played if self._echo else None)
+
+    @classmethod
+    def restore(cls, blob: bytes, config: Config, engine: Optional[Engine] = None, voice: int = 0, depth: int = 3) -> 'RealtimePipeline':
+        """The pipeline a snapshot was taken of, continued on `engine` (another engine or GPU too) and converting into `voice`: the same
+        items give the same outputs bit for bit.  The models of `voice` must be loaded into `engine`.  Refused (ValueError) when the
+        blob's recorded configuration does not match `config`."""
+        parts = unpack_pipeline(blob)
+        check_pipeline_config(parts, config)
+        self = cls.__new__(cls)
+        self.config = config
+        self.engine = engine or default_engine()
+        if parts['session_config']['f0_method'] == 2:
+            # CREPE: the same model and resampler taps a pipeline created in CREPE mode loads (RYK_CREPE_MODEL when none is loaded)
+            from . import crepe
+            crepe.engine_with_model(self.engine)
+            crepe.set_session_rate(int(parts['session_config']['cfg']['fs']), self.engine)
+        self.depth = max(1, min(int(depth), 5))
+        self._loggers = {k: logging.getLogger(k) for k in ('encode', 'convert', 'decode')}
+        self._timing = False
+        self._sid = self.engine.session_restore(parts['session'], voice=voice)
+        try:
+            self._rid = self.engine.reblock_restore(parts['reblock'])
+        except Exception:
+            self.engine.session_destroy(self._sid)
+            raise
+        host = parts['host']
+        self._echo, self._limiter = bool(host['echo']), bool(host['limiter'])
+        if self._echo:
+            self._played = parts['played']
+        self._scratch = numpy.empty(self.engine.session_io_geometry(self._sid)['max_out'], dtype=numpy.float64)
+        self._inflight = deque()
+        self._done = deque()
+        self._index_input = self._index_output = int(host['index'])
+        self._popped = []
+        return self
+
     def close(self) -> None:
         if self._sid is not None:
             self.flush()
             self.engine.reblock_destroy(self._rid)
             self.engine.session_destroy(self._sid)
             self._sid = None
+
+
+# ---- the pipeline blob: the snapshot container (snapshot.py) of kind 'pipeline' ------------------------------------------------------
+# SESS: the session's blob, RBLK: the re-blocker's blob, PIPE: the pipeline's host state as JSON, FARQ: the echo far-end queue (float32).
+def pack_pipeline(session: bytes, reblock: bytes, host: dict, played: Optional[numpy.ndarray]) -> bytes:
+    from .snapshot import pack
+    sections = [('SESS', session), ('RBLK', reblock), ('PIPE', json.dumps(host, sort_keys=True).encode('utf-8'))]
+    if played is not None:
+        sections.append(('FARQ', numpy.ascontiguousarray(played, dtype=numpy.float32).tobytes()))
+    return pack('pipeline', sections)
+
+
+def unpack_pipeline(blob: bytes) -> dict:
+    """{'session', 'reblock': blobs, 'host': dict, 'played': float32 array or None, 'session_config', 'reblock_config': the configurations
+    the two blobs record}; raises ValueError for a blob that is not a pipeline snapshot."""
+    from .engine import RykError, describe_snapshot
+    from .snapshot import unpack
+    try:
+        kind, sec = unpack(blob)
+        if kind != 'pipeline' or not {'SESS', 'RBLK', 'PIPE'} <= set(sec):
+            raise ValueError('not a pipeline snapshot')
+        host = json.loads(sec['PIPE'].decode('utf-8'))
+        ds, dr = describe_snapshot(sec['SESS']), describe_snapshot(sec['RBLK'])
+    except RykError as exc:
+        raise ValueError(f'not a usable pipeline snapshot: {exc}') from exc
+    if ds['kind'] != 'session' or dr['kind'] != 'reblock':
+        raise ValueError('not a pipeline snapshot')
+    played = numpy.frombuffer(sec['FARQ'], dtype=numpy.float32).copy() if 'FARQ' in sec else None
+    if bool(host.get('echo')) != (played is not None):
+        raise ValueError('malformed pipeline snapshot: the echo far-end queue')
+    return {'session': sec['SESS'], 'reblock': sec['RBLK'], 'host': host, 'played': played, 'session_config': ds['config'],
+            'reblock_config': dr['config']}
+
+
+def check_pipeline_config(parts: dict, config: Config) -> None:
+    """Refuse (ValueError, listing every difference) a pipeline snapshot whose recorded configuration is not what `config` makes."""
+    sc, rc, host = parts['session_config'], parts['reblock_config'], parts['host']
+    cfg = sc['cfg']
+    fs = int(cfg['fs'])
+    crepe = VocodeMode(config.extract_f0_mode) is VocodeMode.CREPE
+    want = [
+        ('frame_period', cfg['frame_period_ms'], float(config.frame_period)),
+        ('buffer_time', cfg['buffer_time'], float(config.buffer_time)),
+        ('encode_extra_time', cfg['encode_extra_time'], float(config.encode_extra_time)),
+        ('convert_extra_time', cfg['convert_extra_time'], float(config.convert_extra_time)),
+        ('decode_extra_time', cfg['decode_extra_time'], float(config.decode_extra_time)),
+        ('input_silent_threshold', cfg['threshold_db'], float(config.input_silent_threshold)),
+        ('vocoder_buffer_size', cfg['vocoder_buffer_size'], int(config.vocoder_buffer_size)),
+        ('input_rate', sc['in_rate'] or fs, int(config.input_rate)),
+        ('output_rate', sc['out_rate'] or fs, int(config.output_rate)),
+        ('extract_f0_mode crepe', sc['f0_method'] == 2, crepe),
+        ('out_audio_chunk', rc['out_audio_chunk'], int(config.out_audio_chunk)),
+        ('output_silent_threshold', rc['threshold_db'], float(config.output_silent_threshold)),
+        ('input_scale', host.get('input_scale'), float(config.input_scale)),
+        ('output_scale', host.get('output_scale'), float(config.output_scale)),
+    ]
+    bad = [f'{name}: recorded {got}, config {exp}' for name, got, exp in want if got != exp]
+    if bad:
+        raise ValueError('the snapshot was taken with another configuration: ' + '; '.join(bad))
