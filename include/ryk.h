@@ -490,7 +490,7 @@ int ryk_agc(ryk_engine* e, const float* x, int n, int fs, double target_db, doub
  * ryk_reblock_snapshot_size / ryk_reblock_snapshot / ryk_reblock_restore: the same for a re-blocker (its fragment, length and
  *   ping-pong selector, and its push count); the snapshot waits for the re-blocker's last push.
  * ryk_snapshot_describe (host only, no engine or device): verifies a blob's header, size, checksum and section walk and reports its
- *   kind (1 session, 2 re-blocker, 3 pipeline), format version, the recorded configuration of a session or re-blocker (either
+ *   kind (1 session, 2 re-blocker, 3 pipeline, 4 drift stage), format version, the recorded configuration of a session or re-blocker (either
  *   pointer may be NULL) and up to `capacity` section tags (four characters, first in the lowest byte) and payload sizes.  Returns the
  *   number of sections.
  * ryk_snapshot_seal (host only): writes the total size and the checksum into the header of a blob of `bytes` bytes whose magic,
@@ -524,6 +524,49 @@ int ryk_snapshot_seal(void* buf, size_t bytes);
  * host_ms the rest of the call (the waits for the session's streams, building the session, packing, parsing and the checksum).
  * Either pointer may be NULL. */
 int ryk_snapshot_last_times(ryk_engine* e, double* host_ms, double* device_ms);
+
+/* Clock drift compensation (DESIGN.md §4l, DECIDE D1-D4): an asynchronous resampler on the played stream, for an output sound card
+ * whose clock differs from the input card's.  A standalone object of the engine, like a re-blocker; no session runs it.  With
+ * z = concat(zeros(W), x) the input stream and inc = llrint(2^32 / (1 + ppm 1e-6)) of the setting in force, output m reads z at
+ * q_m = inc_0 + ... + inc_(m-1) (int64, 2^-32 samples).  For q = i 2^32 + f: phi = f >> 23, w = (f & (2^23 - 1)) 2^-23,
+ *   c_t = T[(2W - 1 - t) P + phi] + w (T[(2W - 1 - t) P + phi + 1] - T[(2W - 1 - t) P + phi]),   t = 0 .. 2W - 1,
+ *   y_m = sum over t of c_t z[i - W + 1 + t] in ascending t from 0.0, in FP64 with round-to-nearest operations only,
+ * with the table T of P = 512 phases and half-width W = 16 (2WP + 1 entries, entry k at k / P - W; wave_io.drift_filter designs it).
+ * Output m is emitted by the push that brings z[i + W]: after N input samples every m with q_m < N 2^32 has been emitted.  So the
+ * delay is W samples, at ppm 0 the output is concat(zeros(W), x) bit for bit (the table's integer entries are 0 and its centre 1),
+ * and however the input is cut into pushes the outputs are those of the whole signal.  The output runs (1 + ppm 1e-6) times as many
+ * samples as the input.
+ * ryk_drift_create: max_in in [1, 2^24] samples per push, max_ppm in (0, 2000], the table (phases 512, half_width 16, finite); the
+ *   setting starts at ppm 0.  It works at whatever rate its caller's samples have and creates no device rate.
+ * ryk_drift_set: ppm finite with |ppm| <= max_ppm, from the next push on; the position continues from where it is.  No device work.
+ * ryk_drift_get: the setting of the next push and its inc.  Either pointer may be NULL.
+ * ryk_drift_push: host buffers, synchronous (as ryk_reblock_push): n in [0, max_in] samples in, *n_out samples out; y_capacity must
+ *   be at least n + ceil(n max_ppm 1e-6) + 2, the most one push can emit.  One kernel launch; the count is decided on the device.
+ * ryk_drift_stats: input samples consumed and outputs produced since creation.  Either pointer may be NULL.
+ * ryk_drift_resample: the same kernel over a whole signal from a fresh state, followed by W zeros: len = n + W samples in, y_capacity
+ *   at least len + ceil(len |ppm| 1e-6) + 2, |ppm| <= 2000.
+ * ryk_drift_snapshot_size / _snapshot / _restore: the object's state as a blob of the snapshot container, kind 4, sections DCNF
+ *   (ryk_snapshot_drift followed by the table), DSTA (position, counts, inc and ppm of the next push) and DHIS (the 2W kept samples).
+ *   The restored object continues the stream bit for bit, on this engine or another.  The restore refuses before it allocates: what
+ *   ryk_snapshot_describe refuses, another kind, sections of other sizes, a configuration or setting ryk_drift_create / _set refuse,
+ *   an inc that is not that of the recorded ppm, a position outside [0, 2^33).
+ * Refused, changing nothing: an unknown id, the arguments named above out of range. */
+typedef struct {
+  int max_in, phases, half_width, reserved;
+  double max_ppm;
+  long long pushed;
+} ryk_snapshot_drift;
+int ryk_drift_create(ryk_engine* e, int max_in, double max_ppm, const double* table, int phases, int half_width, int* drift_id);
+int ryk_drift_destroy(ryk_engine* e, int drift_id);
+int ryk_drift_set(ryk_engine* e, int drift_id, double ppm);
+int ryk_drift_get(ryk_engine* e, int drift_id, double* ppm, long long* inc);
+int ryk_drift_push(ryk_engine* e, int drift_id, const double* x, int n, double* y, int y_capacity, int* n_out);
+int ryk_drift_stats(ryk_engine* e, int drift_id, long long* consumed, long long* produced);
+int ryk_drift_resample(ryk_engine* e, const double* x, int n, double ppm, const double* table, int phases, int half_width, double* y,
+                       int y_capacity, int* n_out);
+int ryk_drift_snapshot_size(ryk_engine* e, int drift_id, size_t* bytes);
+int ryk_drift_snapshot(ryk_engine* e, int drift_id, void* buf, size_t bytes);
+int ryk_drift_restore(ryk_engine* e, const void* buf, size_t bytes, int* drift_id);
 
 /* Diagnostics: device timeline (ms) of the last <= 8 steps x 5 stages {gate, analysis, stage 1, stage 2, synthesis}; needs
  * RYK_STAGE_TIMES=1 in the environment at session creation.  start/end hold 40 floats; returns the number of steps. */

@@ -11,6 +11,7 @@
 
 #include "../../include/ryk.h"
 #include "conv.h"
+#include "drift.h"
 #include "engine.h"
 #include "fft.cuh"
 #include "features.h"
@@ -209,6 +210,7 @@ int ryk_engine_destroy(ryk_engine* h) {
   Engine* e = E(h);
   cudaSetDevice(e->device);
   cudaStreamSynchronize(e->stream);
+  drift_destroy_all(e);
   reblock_destroy_all(e);                           // before the sessions: a re-blocker's pushes may ride a session's decode stream
   session_destroy_all(e);                           // before the voices: a session releases its plans on the voice's U-Nets
   crepe_destroy();                                  // after the sessions: their CREPE plans are counted on the model

@@ -20,6 +20,7 @@ struct CrepePlan;
 struct Session;
 struct Group;
 struct Reblock;
+struct Drift;
 
 // One target voice: the two U-Nets and the statistics that convert into one speaker.  Voice 0 is the engine's built-in voice (the
 // ryk_model_* / ryk_stage1_set_stats / ryk_f0_set_stats calls and the per-op API); voices >= 1 come from ryk_voice_create.
@@ -89,6 +90,7 @@ struct Engine {
   std::vector<Session*> sessions;
   std::vector<Group*> groups;
   std::vector<Reblock*> reblocks;     // output re-blockers + silence gates (decode_worker.py:38-59)
+  std::vector<Drift*> drifts;         // clock drift stages of played streams (drift.cu)
   float* d_colmin = nullptr;         // stage-2 prologue column-minimum partials
   // scratch arena for the per-op host-pointer API (grown on demand)
   void* d_scratch = nullptr; size_t scratch_bytes = 0;

@@ -21,7 +21,7 @@ namespace ryk {
 
 constexpr uint64_t kSnapMagic = 0x0050414e534b5952ull;     // "RYKSNAP\0"
 constexpr uint32_t kSnapVersion = 1;
-// The payloads are these structs as they lie in memory (and SnapHost in session.cu, ReblockState in reblock.cu).  A change to any of them
+// The payloads are these structs as they lie in memory (and SnapHost in session.cu, ReblockState in reblock.cu, DriftSnap in drift.cu).  A change to any of them
 // changes what a blob means: bump kSnapVersion with it, so that an older blob is refused before anything is allocated, and the sizes here.
 static_assert(sizeof(ryk_snapshot_session) == 224 && sizeof(ryk_snapshot_reblock) == 32, "snapshot layout: bump kSnapVersion");
 static_assert(sizeof(F0Map) == 64 && sizeof(F0Stats) == 24 && sizeof(ResampleState) == 16, "snapshot layout: bump kSnapVersion");
@@ -30,7 +30,7 @@ static_assert(sizeof(EchoParams) == 8 && sizeof(EchoFilter) == 541776, "snapshot
 static_assert(sizeof(LimParams) == 16 && sizeof(LimState) == 8 && sizeof(LimMeter) == 16, "snapshot layout: bump kSnapVersion");
 static_assert(sizeof(AgcParams) == 56 && sizeof(AgcState) == 1064 && sizeof(AgcMeter) == 24, "snapshot layout: bump kSnapVersion");
 static_assert(sizeof(SynthState) == 136, "snapshot layout: bump kSnapVersion");
-enum : uint32_t { kSnapSession = 1, kSnapReblock = 2, kSnapPipeline = 3 };   // kinds (a pipeline blob is written by worker.py)
+enum : uint32_t { kSnapSession = 1, kSnapReblock = 2, kSnapPipeline = 3, kSnapDrift = 4 };   // kinds (a pipeline blob is written by worker.py)
 
 struct SnapHeader { uint64_t magic; uint32_t version, kind; uint64_t total, checksum; };
 struct SnapSectionHeader { uint32_t tag, zero; uint64_t bytes; };

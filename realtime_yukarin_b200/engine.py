@@ -60,7 +60,13 @@ class SnapshotReblock(ctypes.Structure):
                 ('threshold_db', ctypes.c_double), ('pushed', ctypes.c_longlong)]
 
 
-SNAPSHOT_KINDS = {1: 'session', 2: 'reblock', 3: 'pipeline'}
+class SnapshotDrift(ctypes.Structure):
+    """ryk_snapshot_drift: the configuration a drift snapshot records (its DCNF section starts with it, the filter table follows)"""
+    _fields_ = [('max_in', ctypes.c_int), ('phases', ctypes.c_int), ('half_width', ctypes.c_int), ('reserved', ctypes.c_int),
+                ('max_ppm', ctypes.c_double), ('pushed', ctypes.c_longlong)]
+
+
+SNAPSHOT_KINDS = {1: 'session', 2: 'reblock', 3: 'pipeline', 4: 'drift'}
 
 
 def _struct_dict(x) -> Dict[str, Any]:
@@ -73,8 +79,9 @@ def _struct_dict(x) -> Dict[str, Any]:
 
 def describe_snapshot(blob: bytes) -> Dict[str, Any]:
     """ryk_snapshot_describe: verify a snapshot blob (header, size, FNV-1a-64 checksum, section walk) without an engine or a device.
-    Returns kind ('session' / 'reblock' / 'pipeline'), version, config (the recorded configuration of a session or re-blocker, as a
-    dict; None for a pipeline) and sections [(tag, payload bytes)] in blob order; raises RykError for a blob it refuses."""
+    Returns kind ('session' / 'reblock' / 'pipeline' / 'drift'), version, config (the recorded configuration of a session, re-blocker or
+    drift stage, as a dict; None for a pipeline) and sections [(tag, payload bytes)] in blob order; raises RykError for a blob it
+    refuses."""
     lib = load_library()
     blob = bytes(blob)
     kind, version = ctypes.c_int(), ctypes.c_int()
@@ -89,6 +96,8 @@ def describe_snapshot(blob: bytes) -> Dict[str, Any]:
     names = [int(t).to_bytes(4, 'little').decode('ascii', 'replace') for t in tags]
     k = SNAPSHOT_KINDS.get(kind.value, kind.value)
     config = _struct_dict(ss) if k == 'session' else _struct_dict(sr) if k == 'reblock' else None
+    if k == 'drift' and names[0] == 'DCNF' and sizes[0] >= ctypes.sizeof(SnapshotDrift):
+        config = _struct_dict(SnapshotDrift.from_buffer_copy(blob, 48))     # after the header and the DCNF section header
     return {'kind': k, 'version': version.value, 'config': config, 'sections': list(zip(names, (int(x) for x in sizes)))}
 
 
@@ -136,7 +145,8 @@ EXPORTED_SYMBOLS = [
     'ryk_session_limiter_stats', 'ryk_limit', 'ryk_session_agc', 'ryk_session_set_agc', 'ryk_session_get_agc', 'ryk_session_agc_stats',
     'ryk_agc', 'ryk_session_snapshot_size', 'ryk_session_snapshot', 'ryk_session_restore', 'ryk_reblock_snapshot_size',
     'ryk_reblock_snapshot', 'ryk_reblock_restore', 'ryk_snapshot_describe', 'ryk_snapshot_seal',
-    'ryk_snapshot_last_times',
+    'ryk_snapshot_last_times', 'ryk_drift_create', 'ryk_drift_destroy', 'ryk_drift_set', 'ryk_drift_get', 'ryk_drift_push',
+    'ryk_drift_stats', 'ryk_drift_resample', 'ryk_drift_snapshot_size', 'ryk_drift_snapshot', 'ryk_drift_restore',
 ]
 
 SEMITONE = math.log(2.0) / 12.0          # one semitone in ln f0
@@ -153,6 +163,7 @@ AGC_TARGET_DB = (-40.0, -6.0)            # automatic gain control: target levels
 AGC_MAX_GAIN_DB = (0.0, 30.0)            # ... largest gain either way
 AGC_GATE_DB = (-80.0, -20.0)             # ... and gates: blocks at or under the gate leave level and gain as they are
 AGC_LINEAR = ('target', 'gate', 'gmax', 'ginv', 'a', 's_up', 's_dn')     # ryk_session_get_agc's linear values, in order
+DRIFT_MAX_PPM = 2000.0                   # clock drift stage: the largest max_ppm a drift object accepts
 
 
 class F0Map(ctypes.Structure):
@@ -255,6 +266,7 @@ class Engine(object):
         self._h = h
         self._synth_block = {}
         self._reblock_chunk = {}           # re-blocker id -> out_audio_chunk
+        self._drift_shape = {}             # drift id -> (max_in, max_ppm)
         self._session_fs = {}              # session id -> the session's (model) rate
         self._voice_shapes = {}            # voice id >= 1 -> stage -> the 16 (transposed, cin, cout, k) of its U-Net
 
@@ -917,6 +929,80 @@ class Engine(object):
         self._check(self.lib.ryk_reblock_restore(self._h, blob, ctypes.c_size_t(len(blob)), ctypes.byref(rid)))
         self._reblock_chunk[rid.value] = _first_int(blob)  # out_audio_chunk: the first field of the RCNF section
         return rid.value
+
+    # ---- clock drift compensation (DESIGN.md §4l) ----
+    def drift_create(self, max_in: int, max_ppm: float = 500.0, table=None) -> int:
+        """A drift stage for pushes of up to `max_in` samples and settings up to +-`max_ppm` (at most 2000), with the prototype filter
+        `table` (wave_io.drift_filter() when None).  Starts at ppm 0."""
+        from .wave_io import DRIFT_HALF_WIDTH, DRIFT_PHASES, drift_filter
+        table = drift_filter() if table is None else numpy.ascontiguousarray(table, dtype=numpy.float64).ravel()
+        if len(table) != 2 * DRIFT_HALF_WIDTH * DRIFT_PHASES + 1:
+            raise RykError(f'the drift filter table must hold {2 * DRIFT_HALF_WIDTH * DRIFT_PHASES + 1} entries, not {len(table)}')
+        did = ctypes.c_int()
+        self._check(self.lib.ryk_drift_create(self._h, int(max_in), ctypes.c_double(max_ppm), _dp(table), DRIFT_PHASES, DRIFT_HALF_WIDTH,
+                                              ctypes.byref(did)))
+        self._drift_shape[did.value] = (int(max_in), float(max_ppm))
+        return did.value
+
+    def drift_destroy(self, did: int):
+        self._check(self.lib.ryk_drift_destroy(self._h, int(did)))
+        self._drift_shape.pop(did, None)
+
+    def drift_set(self, did: int, ppm: float):
+        """The output runs (1 + ppm 1e-6) times as many samples as the input from the next push on."""
+        self._check(self.lib.ryk_drift_set(self._h, int(did), ctypes.c_double(ppm)))
+
+    def drift_get(self, did: int) -> Tuple[float, int]:
+        """(ppm, inc) of the next push: inc = llrint(2^32 / (1 + ppm 1e-6)), the position's advance per output in 2^-32 samples."""
+        ppm, inc = ctypes.c_double(), ctypes.c_longlong()
+        self._check(self.lib.ryk_drift_get(self._h, int(did), ctypes.byref(ppm), ctypes.byref(inc)))
+        return ppm.value, inc.value
+
+    def drift_push(self, did: int, x) -> numpy.ndarray:
+        """Samples in, the float64 outputs they complete out (as many as the input times 1 + ppm 1e-6, give or take one)."""
+        x = numpy.ascontiguousarray(x, dtype=numpy.float64).ravel()
+        max_in, max_ppm = self._drift_shape[did]
+        y = numpy.empty(len(x) + math.ceil(len(x) * max_ppm * 1e-6) + 2, dtype=numpy.float64)
+        n = ctypes.c_int()
+        self._check(self.lib.ryk_drift_push(self._h, int(did), _dp(x), len(x), _dp(y), len(y), ctypes.byref(n)))
+        return y[:n.value]
+
+    def drift_stats(self, did: int) -> Tuple[int, int]:
+        """(input samples consumed, outputs produced) since the stage was created"""
+        c, p = ctypes.c_longlong(), ctypes.c_longlong()
+        self._check(self.lib.ryk_drift_stats(self._h, int(did), ctypes.byref(c), ctypes.byref(p)))
+        return c.value, p.value
+
+    def drift_resample(self, x, ppm: float, table=None) -> numpy.ndarray:
+        """The drift stage over a whole signal from a fresh state, followed by its W zeros: float64 out."""
+        from .wave_io import DRIFT_HALF_WIDTH, DRIFT_PHASES, drift_filter
+        x = numpy.ascontiguousarray(x, dtype=numpy.float64).ravel()
+        table = drift_filter() if table is None else numpy.ascontiguousarray(table, dtype=numpy.float64).ravel()
+        if len(table) != 2 * DRIFT_HALF_WIDTH * DRIFT_PHASES + 1:
+            raise RykError(f'the drift filter table must hold {2 * DRIFT_HALF_WIDTH * DRIFT_PHASES + 1} entries, not {len(table)}')
+        m = len(x) + DRIFT_HALF_WIDTH
+        y = numpy.empty(m + math.ceil(m * abs(float(ppm)) * 1e-6) + 2, dtype=numpy.float64)
+        n = ctypes.c_int()
+        self._check(self.lib.ryk_drift_resample(self._h, _dp(x), len(x), ctypes.c_double(ppm), _dp(table), DRIFT_PHASES, DRIFT_HALF_WIDTH,
+                                                _dp(y), len(y), ctypes.byref(n)))
+        return y[:n.value]
+
+    def drift_snapshot(self, did: int) -> bytes:
+        """The position, totals, setting, kept samples and filter of a drift stage as a blob of kind 'drift'."""
+        n = ctypes.c_size_t()
+        self._check(self.lib.ryk_drift_snapshot_size(self._h, int(did), ctypes.byref(n)))
+        buf = ctypes.create_string_buffer(n.value)
+        self._check(self.lib.ryk_drift_snapshot(self._h, int(did), buf, n))
+        return buf.raw
+
+    def drift_restore(self, blob: bytes) -> int:
+        """A new drift stage on this engine that continues the stream of the one the blob was taken from."""
+        blob = bytes(blob)
+        did = ctypes.c_int()
+        self._check(self.lib.ryk_drift_restore(self._h, blob, ctypes.c_size_t(len(blob)), ctypes.byref(did)))
+        c = describe_snapshot(blob)['config']
+        self._drift_shape[did.value] = (int(c['max_in']), float(c['max_ppm']))
+        return did.value
 
     def snapshot_last_times(self) -> Tuple[float, float]:
         """(host ms, device ms) of this engine's last snapshot or restore call (ryk_snapshot_last_times)."""

@@ -24,15 +24,19 @@ from .worker import RealtimePipeline, unpack_pipeline
 
 
 def audio_loop(pipeline: RealtimePipeline, read_chunk: Callable[[], Optional[numpy.ndarray]],
-               write_chunk: Callable[[numpy.ndarray], None], max_chunks: Optional[int] = None) -> int:
+               write_chunk: Callable[[numpy.ndarray], None], max_chunks: Optional[int] = None,
+               backlog: Optional[Callable[[], float]] = None) -> int:
     """run.py:152-199: read one input chunk, queue it, play whatever output is ready (zeros otherwise).  Returns the number of
-    chunks processed; stops when `read_chunk` returns None (end of a wav file) or after `max_chunks`."""
+    chunks processed; stops when `read_chunk` returns None (end of a wav file) or after `max_chunks`.  `backlog`: read the output
+    card's queue after each write and hand it to the pipeline's drift controller (RealtimePipeline.update_drift)."""
     n = 0
     while max_chunks is None or n < max_chunks:
         in_wave = read_chunk()
         if in_wave is None:
             break
         write_chunk(pipeline.process(in_wave))
+        if backlog is not None:
+            pipeline.update_drift(backlog())
         n += 1
     return n
 
@@ -79,7 +83,7 @@ def save_state_file(pipeline: RealtimePipeline, path: Path) -> None:
 # options that set up the stream's stages, with the values that leave them off: a state file brings its own stages
 _STAGE_OPTIONS = {'follow_input_f0': None, 'pitch': 0.0, 'formant': 0.0, 'denoise': None, 'noise_profile': None, 'learn_noise': None,
                   'echo_cancel': None, 'echo_delay': 0.0, 'echo_suppression': 0.0, 'limit': None, 'limit_lookahead': None,
-                  'limit_hold': None, 'agc': None, 'agc_max_gain': None, 'agc_gate': None}
+                  'limit_hold': None, 'agc': None, 'agc_max_gain': None, 'agc_gate': None, 'drift_ppm': None, 'drift': None}
 
 
 def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path] = None, max_chunks: Optional[int] = None,
@@ -89,7 +93,7 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
         echo_delay: float = 0.0, echo_suppression: float = 0.0, limit: Optional[float] = None,
         limit_lookahead: Optional[float] = None, limit_hold: Optional[float] = None, agc: Optional[float] = None,
         agc_max_gain: Optional[float] = None, agc_gate: Optional[float] = None, save_state: Optional[Path] = None,
-        load_state: Optional[Path] = None) -> int:
+        load_state: Optional[Path] = None, drift_ppm: Optional[float] = None, drift: Optional[float] = None) -> int:
     """`measure_input_statistics`: measure the speaker's log-f0 statistics during the run and write them to this file at the end;
     `follow_input_f0`: convert with the measured statistics once this many voiced frames are counted; `pitch`: semitones added to
     the target voice's mean f0; `formant`: semitones by which the converted spectral envelope moves; `denoise`: filter the input's
@@ -103,7 +107,9 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
     stream state (worker.RealtimePipeline.snapshot) to this file when the audio loop ends; `load_state`: continue the stream such a file
     holds (learned noise profile, echo path, AGC level, f0 statistics and every setting), refused when it was written with another
     configuration and with the options that set up stages, which the file brings; --save_noise_profile and --measure_input_statistics
-    then need the stage in the file."""
+    then need the stage in the file; `drift_ppm`: play the output (1 + drift_ppm 1e-6) times as long through the drift stage, a fixed trim
+    for an output sound card whose clock runs that much fast; `drift`: let a controller find the trim, up to +-drift ppm, from the output
+    card's backlog (live audio only: with wav files there is no second clock)."""
     state = None
     if load_state is not None:
         values = locals()
@@ -116,6 +122,10 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
             raise ValueError('--save_noise_profile needs noise suppression, which the stream in --load_state does not run')
         if measure_input_statistics is not None and not recorded['f0_measure']:
             raise ValueError('--measure_input_statistics needs f0 measuring, which the stream in --load_state does not run')
+    if drift is not None and drift_ppm is not None:
+        raise ValueError('--drift and --drift_ppm exclude each other: the controller sets the trim, or --drift_ppm fixes it')
+    if drift is not None and wav_in is not None:
+        raise ValueError('--drift needs live audio: with --wav_in there is no second clock to follow (--drift_ppm sets a fixed trim)')
     if agc is None and (agc_max_gain is not None or agc_gate is not None):
         raise ValueError('--agc_max_gain and --agc_gate need --agc')
     if limit is None and (limit_lookahead is not None or limit_hold is not None):
@@ -143,7 +153,9 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
                                 limiter_lookahead_ms=5.0 if limit_lookahead is None else limit_lookahead,
                                 limiter_hold_ms=50.0 if limit_hold is None else limit_hold, agc=agc,
                                 agc_max_gain_db=20.0 if agc_max_gain is None else agc_max_gain,
-                                agc_gate_db=-50.0 if agc_gate is None else agc_gate)
+                                agc_gate_db=-50.0 if agc_gate is None else agc_gate,
+                                drift='auto' if drift is not None else drift_ppm,
+                                drift_max_ppm=drift if drift is not None else max(500.0, abs(drift_ppm or 0.0)))
     try:
         if pitch:
             pipeline.set_f0_map(semitones=pitch)
@@ -175,8 +187,10 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
                                 output=True, output_device_index=_find_device(audio, config.output_device_name, 'output'))
         signal.signal(signal.SIGINT, lambda s, f: sys.exit(0))
         logger.debug('audio loop')
+        # the controller regulates the backlog to a set-point it learns, so the free space of the output buffer, negated, serves as its fill
+        backlog = (lambda: -float(stream_out.get_write_available())) if pipeline.drift_auto else None
         return audio_loop(pipeline, lambda: numpy.frombuffer(stream_in.read(config.in_audio_chunk), dtype=numpy.float32),
-                          lambda w: stream_out.write(w.astype(numpy.float32).tobytes()), max_chunks)
+                          lambda w: stream_out.write(w.astype(numpy.float32).tobytes()), max_chunks, backlog=backlog)
     finally:
         try:
             if measure_input_statistics is not None:
@@ -238,6 +252,13 @@ def make_parser() -> argparse.ArgumentParser:
     parser.add_argument('--agc_gate', type=float, default=None, metavar='DB',
                         help='with --agc: blocks of input at or under this level (dB of full scale, -80 to -20, default -50) leave '
                              'the level and the gain as they are')
+    parser.add_argument('--drift_ppm', type=float, default=None, metavar='PPM',
+                        help='play the output (1 + PPM 1e-6) times as long (a fixed trim, -2000 to 2000), for an output sound card whose '
+                             'clock runs PPM ppm fast against the input card\'s; works with --wav_in too')
+    parser.add_argument('--drift', type=float, nargs='?', const=500.0, default=None, metavar='MAX_PPM',
+                        help='follow the clock difference of the input and output sound cards: a controller trims the played stream '
+                             'by up to MAX_PPM (default 500, at most 2000) from the output card\'s backlog, so a long session neither '
+                             'underruns nor falls behind (live audio only)')
     parser.add_argument('--save_state', type=Path, default=None, metavar='OUT.state',
                         help='when the audio loop ends, write the stream state (learned noise profile, echo path, AGC level, f0 '
                              'statistics, settings) to this file for --load_state')
@@ -254,7 +275,8 @@ def main(argv: Optional[Iterable[str]] = None) -> None:
         formant=args.formant, denoise=args.denoise, noise_profile=args.noise_profile, learn_noise=args.learn_noise,
         save_noise_profile=args.save_noise_profile, echo_cancel=args.echo_cancel, echo_delay=args.echo_delay,
         echo_suppression=args.echo_suppression, limit=args.limit, limit_lookahead=args.limit_lookahead, limit_hold=args.limit_hold,
-        agc=args.agc, agc_max_gain=args.agc_max_gain, agc_gate=args.agc_gate, save_state=args.save_state, load_state=args.load_state)
+        agc=args.agc, agc_max_gain=args.agc_max_gain, agc_gate=args.agc_gate, save_state=args.save_state, load_state=args.load_state,
+        drift_ppm=args.drift_ppm, drift=args.drift)
 
 
 if __name__ == '__main__':

@@ -28,6 +28,24 @@ def resample_filter(up: int, down: int) -> numpy.ndarray:
     return h * up
 
 
+DRIFT_PHASES = 512          # clock drift stage (DESIGN.md §4l): phases of the prototype filter per input sample
+DRIFT_HALF_WIDTH = 16       # ... and its half-width in input samples (zero crossings): 32 taps per output
+DRIFT_BETA = 10.0           # ... and the Kaiser window's beta
+
+
+def drift_filter(phases: int = DRIFT_PHASES, half_width: int = DRIFT_HALF_WIDTH, beta: float = DRIFT_BETA) -> numpy.ndarray:
+    """The prototype filter of the clock drift stage (DESIGN.md DECIDE D3): a Kaiser-windowed sinc with its cutoff at Nyquist, sampled
+    at `phases` points per input sample over [-half_width, half_width]: 2 * half_width * phases + 1 float64 values, entry k at
+    t = k / phases - half_width.  The entries at integer t are exactly 0, except the centre, which is exactly 1, so a whole-sample
+    position reads the input sample itself."""
+    n = 2 * half_width * phases + 1
+    t = numpy.arange(n, dtype=numpy.float64) / phases - half_width
+    h = numpy.sinc(t) * numpy.i0(beta * numpy.sqrt(numpy.maximum(0.0, 1.0 - (t / half_width) ** 2))) / numpy.i0(beta)
+    h[::phases] = 0.0
+    h[half_width * phases] = 1.0
+    return h
+
+
 def resample_geometry(n_in: int, up: int, down: int) -> Tuple[int, int, int, int, int]:
     """(up, down) reduced by their gcd, n_out, n_pre_pad, n_pre_remove of scipy.signal.resample_poly."""
     g = math.gcd(up, down)

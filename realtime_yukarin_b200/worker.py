@@ -26,8 +26,10 @@ from typing import Any, Deque, List, Optional, Tuple
 import numpy
 
 from .config import Config, VocodeMode
-from .engine import (AGC_GATE_DB, AGC_MAX_GAIN_DB, AGC_TARGET_DB, LIMITER_CEILING_DB, LIMITER_HOLD_MS, LIMITER_LOOKAHEAD_MS, Engine,
-                     SessionConfig, default_engine)
+from .drift import DriftController
+from .engine import (AGC_GATE_DB, AGC_MAX_GAIN_DB, AGC_TARGET_DB, DRIFT_MAX_PPM, LIMITER_CEILING_DB, LIMITER_HOLD_MS, LIMITER_LOOKAHEAD_MS,
+                     Engine, SessionConfig, default_engine)
+from .wave_io import DRIFT_HALF_WIDTH
 
 
 class Item(object):
@@ -103,6 +105,17 @@ def _check_agc(target_db: float, max_gain_db: float, gate_db: float) -> None:
             raise ValueError(f'the AGC {name} must be within [{lo}, {hi}] dB')
 
 
+def _check_drift(drift, max_ppm: float) -> None:
+    """the drift stage's settings as Engine.drift_create / drift_set accept them, checked before a session exists"""
+    if not (math.isfinite(max_ppm) and 0 < max_ppm <= DRIFT_MAX_PPM):
+        raise ValueError(f'drift_max_ppm must be within (0, {DRIFT_MAX_PPM:g}]')
+    if isinstance(drift, str):
+        if drift != 'auto':
+            raise ValueError("drift must be None, 'auto' or a trim in ppm")
+    elif not (math.isfinite(float(drift)) and abs(float(drift)) <= max_ppm):
+        raise ValueError('the drift trim must be finite and within +-drift_max_ppm')
+
+
 class RealtimePipeline(object):
     """encode_worker | convert_worker | decode_worker of one audio stream as one device-resident session.
 
@@ -129,14 +142,24 @@ class RealtimePipeline(object):
     device, after the echo canceller and the noise filter: at most `agc_max_gain_db` (0-30) of gain either way, counting only the
     256-sample blocks louder than `agc_gate_db` (-80 to -20).  It follows `input_scale`: the host still multiplies each chunk by it
     first, so the gate applies to the scaled signal.  `set_agc` changes the settings between chunks and `agc_stats` reads the level
-    and gain."""
+    and gain.  `drift` compensates the clock difference of two sound cards (DESIGN.md §4l): a drift stage on the device resamples the
+    played stream so that it runs (1 + ppm 1e-6) times as long, with `drift=PPM` a fixed trim and `drift='auto'` a trim that
+    `update_drift` derives from the output card's backlog; |ppm| <= `drift_max_ppm` (at most 2000).  `process` then returns the stage's
+    output for the chunk it would have played: float32, one or two samples more or less than out_audio_chunk, 16 samples later.  The
+    echo canceller's far end stays the chunk before the stage: the microphone hears the played sound in the input card's clock, which
+    the nominal-rate stream is in.  `set_drift` fixes the trim, `drift_stats` reads it with the stage's totals."""
+
+    _drift: Optional[int] = None                        # the drift stage's id on the engine (None: no drift stage)
+    _drift_ctl: Optional[DriftController] = None        # its controller in 'auto' mode
 
     def __init__(self, config: Config, acoustic_param=None, engine: Optional[Engine] = None, depth: int = 3, voice: int = 0,
                  measure_f0: bool = False, follow_f0: Optional[int] = None, formant: float = 0.0, denoise: Optional[float] = None,
                  noise_profile=None, learn_noise: Optional[float] = None, echo_cancel: bool = False, echo_taps: int = 32,
                  echo_delay_ms: float = 0.0, echo_suppression: float = 0.0, limiter: Optional[float] = None,
                  limiter_lookahead_ms: float = 5.0, limiter_hold_ms: float = 50.0, agc: Optional[float] = None,
-                 agc_max_gain_db: float = 20.0, agc_gate_db: float = -50.0):
+                 agc_max_gain_db: float = 20.0, agc_gate_db: float = -50.0, drift=None, drift_max_ppm: float = 500.0):
+        if drift is not None:
+            _check_drift(drift, float(drift_max_ppm))
         if agc is not None:
             _check_agc(float(agc), float(agc_max_gain_db), float(agc_gate_db))
         if limiter is not None:
@@ -222,6 +245,13 @@ class RealtimePipeline(object):
             self.engine.session_set_formant(self._sid, semitones=float(formant))
         self._scratch = numpy.empty(n_out_cap, dtype=numpy.float64)
         self._rid = self.engine.reblock_create(config.out_audio_chunk, n_out_cap, float(config.output_silent_threshold))
+        self._drift, self._drift_ctl = None, None
+        if drift is not None:           # the played stream's drift stage at the output rate: one out_audio_chunk per push
+            self._drift = self.engine.drift_create(int(config.out_audio_chunk), float(drift_max_ppm))
+            if drift == 'auto':
+                self._drift_ctl = DriftController(int(config.output_rate), int(config.out_audio_chunk), max_ppm=float(drift_max_ppm))
+            else:
+                self.engine.drift_set(self._drift, float(drift))
         self._inflight: Deque[Tuple[Item, int, int, float]] = deque()      # (item, session ticket, re-blocker ticket, host time of put)
         self._done: Deque[Item] = deque()
         # audio-loop state (run.py:155-157)
@@ -279,6 +309,43 @@ class RealtimePipeline(object):
     def agc_stats(self) -> Tuple[float, float, int]:
         """(level in dB, -inf before any active block; gain in dB; active blocks of the last chunk) of the chunks put (needs agc)."""
         return self.engine.session_agc_stats(self._sid)
+
+    def set_drift(self, ppm: float) -> None:
+        """A fixed trim of the drift stage from the next chunk on (needs drift); in 'auto' mode it stops the controller."""
+        self._need_drift()
+        self.engine.drift_set(self._drift, float(ppm))
+        self._drift_ctl = None
+
+    def update_drift(self, backlog_samples: float) -> Optional[float]:
+        """One reading of the output card's backlog in samples, taken after a chunk's write.  In 'auto' mode the controller turns it
+        into the trim of the next chunk, which is returned; otherwise nothing changes and the trim in force (None without drift) is
+        returned."""
+        if self._drift is None:
+            return None
+        if self._drift_ctl is None:
+            return self.engine.drift_get(self._drift)[0]
+        ppm = self._drift_ctl.update(backlog_samples)
+        self.engine.drift_set(self._drift, ppm)
+        return ppm
+
+    @property
+    def drift_auto(self) -> bool:
+        """whether a controller sets the drift stage's trim from the backlog readings update_drift gets"""
+        return self._drift_ctl is not None
+
+    def drift_stats(self) -> dict:
+        """ppm and inc of the next chunk, the samples the stage consumed and produced, and whether the controller sets the trim."""
+        self._need_drift()
+        ppm, inc = self.engine.drift_get(self._drift)
+        consumed, produced = self.engine.drift_stats(self._drift)
+        return {'ppm': ppm, 'inc': inc, 'consumed': consumed, 'produced': produced, 'auto': self.drift_auto}
+
+    def _need_drift(self) -> None:
+        if self._drift is None:
+            raise RuntimeError('the pipeline has no drift stage: create it with drift=PPM or drift=\'auto\'')
+
+    def _drift_push(self, wave: numpy.ndarray) -> numpy.ndarray:
+        return self.engine.drift_push(self._drift, wave).astype(numpy.float32)
 
     def measured_f0(self) -> Tuple[int, float, float]:
         """(voiced frames, mean, standard deviation) of the speaker's ln f0 over the chunks put so far (needs measure_f0)."""
@@ -362,6 +429,8 @@ class RealtimePipeline(object):
         out_wave = (out_wave * c.output_scale)[:c.out_audio_chunk].astype(numpy.float32)
         if self._echo:
             self._played = numpy.concatenate([self._played, out_wave])
+        if self._drift is not None:
+            out_wave = self._drift_push(out_wave)
         return out_wave
 
     def _next_output(self) -> Optional[numpy.ndarray]:
@@ -387,7 +456,8 @@ class RealtimePipeline(object):
 
     def drain(self) -> List[numpy.ndarray]:
         """End of a finite input (wav file): wait for everything in flight and return the output chunks not played yet, in
-        order (the reference's loop never ends; a file-driven run must not lose the tail that is still in the pipeline)."""
+        order (the reference's loop never ends; a file-driven run must not lose the tail that is still in the pipeline).  With drift the
+        chunks go through the drift stage and a last item flushes the 16 samples it holds: the played stream ends here."""
         c = self.config
         self.flush()
         outs: List[numpy.ndarray] = []
@@ -396,19 +466,24 @@ class RealtimePipeline(object):
             if w is None:
                 break
             outs.append((w * c.output_scale)[:c.out_audio_chunk].astype(numpy.float32))
+        if self._drift is not None:
+            outs = [self._drift_push(w) for w in outs] + [self._drift_push(numpy.zeros(DRIFT_HALF_WIDTH, numpy.float32))]
         return outs
 
     # ---- moving the stream (DESIGN.md §4k) ----------------------------------------------------------------------
     def snapshot(self) -> bytes:
         """The whole stream state as one blob: the session's, the re-blocker's and the pipeline's host state (the next item index,
-        the echo far-end queue, input_scale and output_scale).  Only a drained pipeline can be snapshotted: nothing in flight and
-        every finished item taken (`drain`)."""
+        the echo far-end queue, input_scale and output_scale; with drift the drift stage's blob and the controller's state).  Only a
+        drained pipeline can be snapshotted: nothing in flight and every finished item taken (`drain`)."""
         if self._inflight or self._done or self._popped or self._index_output != self._index_input:
             raise RuntimeError('the pipeline has chunks in flight or outputs not taken: drain() it before a snapshot')
-        return pack_pipeline(self.engine.session_snapshot(self._sid), self.engine.reblock_snapshot(self._rid),
-                             {'index': self._index_input, 'input_scale': float(self.config.input_scale),
-                              'output_scale': float(self.config.output_scale), 'echo': self._echo, 'limiter': self._limiter},
-                             self._played if self._echo else None)
+        host = {'index': self._index_input, 'input_scale': float(self.config.input_scale),
+                'output_scale': float(self.config.output_scale), 'echo': self._echo, 'limiter': self._limiter}
+        if self._drift is not None:
+            host['drift'] = {'controller': None if self._drift_ctl is None else self._drift_ctl.state()}
+        return pack_pipeline(self.engine.session_snapshot(self._sid), self.engine.reblock_snapshot(self._rid), host,
+                             self._played if self._echo else None,
+                             None if self._drift is None else self.engine.drift_snapshot(self._drift))
 
     @classmethod
     def restore(cls, blob: bytes, config: Config, engine: Optional[Engine] = None, voice: int = 0, depth: int = 3) -> 'RealtimePipeline':
@@ -435,6 +510,16 @@ class RealtimePipeline(object):
             self.engine.session_destroy(self._sid)
             raise
         host = parts['host']
+        self._drift, self._drift_ctl = None, None
+        if parts['drift'] is not None:
+            try:
+                self._drift = self.engine.drift_restore(parts['drift'])
+            except Exception:
+                self.engine.reblock_destroy(self._rid)
+                self.engine.session_destroy(self._sid)
+                raise
+            ctl = host['drift']['controller']
+            self._drift_ctl = None if ctl is None else DriftController.from_state(ctl)
         self._echo, self._limiter = bool(host['echo']), bool(host['limiter'])
         if self._echo:
             self._played = parts['played']
@@ -449,23 +534,29 @@ class RealtimePipeline(object):
         if self._sid is not None:
             self.flush()
             self.engine.reblock_destroy(self._rid)
+            if self._drift is not None:
+                self.engine.drift_destroy(self._drift)
+                self._drift = None
             self.engine.session_destroy(self._sid)
             self._sid = None
 
 
 # ---- the pipeline blob: the snapshot container (snapshot.py) of kind 'pipeline' ------------------------------------------------------
-# SESS: the session's blob, RBLK: the re-blocker's blob, PIPE: the pipeline's host state as JSON, FARQ: the echo far-end queue (float32).
-def pack_pipeline(session: bytes, reblock: bytes, host: dict, played: Optional[numpy.ndarray]) -> bytes:
+# SESS: the session's blob, RBLK: the re-blocker's blob, PIPE: the pipeline's host state as JSON, FARQ: the echo far-end queue (float32),
+# DRFT: the drift stage's blob.
+def pack_pipeline(session: bytes, reblock: bytes, host: dict, played: Optional[numpy.ndarray], drift: Optional[bytes] = None) -> bytes:
     from .snapshot import pack
     sections = [('SESS', session), ('RBLK', reblock), ('PIPE', json.dumps(host, sort_keys=True).encode('utf-8'))]
     if played is not None:
         sections.append(('FARQ', numpy.ascontiguousarray(played, dtype=numpy.float32).tobytes()))
+    if drift is not None:
+        sections.append(('DRFT', drift))
     return pack('pipeline', sections)
 
 
 def unpack_pipeline(blob: bytes) -> dict:
-    """{'session', 'reblock': blobs, 'host': dict, 'played': float32 array or None, 'session_config', 'reblock_config': the configurations
-    the two blobs record}; raises ValueError for a blob that is not a pipeline snapshot."""
+    """{'session', 'reblock': blobs, 'host': dict, 'played': float32 array or None, 'drift': blob or None, 'session_config',
+    'reblock_config': the configurations the two blobs record}; raises ValueError for a blob that is not a pipeline snapshot."""
     from .engine import RykError, describe_snapshot
     from .snapshot import unpack
     try:
@@ -474,15 +565,18 @@ def unpack_pipeline(blob: bytes) -> dict:
             raise ValueError('not a pipeline snapshot')
         host = json.loads(sec['PIPE'].decode('utf-8'))
         ds, dr = describe_snapshot(sec['SESS']), describe_snapshot(sec['RBLK'])
+        dd = describe_snapshot(sec['DRFT']) if 'DRFT' in sec else None
     except RykError as exc:
         raise ValueError(f'not a usable pipeline snapshot: {exc}') from exc
-    if ds['kind'] != 'session' or dr['kind'] != 'reblock':
+    if ds['kind'] != 'session' or dr['kind'] != 'reblock' or (dd is not None and dd['kind'] != 'drift'):
         raise ValueError('not a pipeline snapshot')
     played = numpy.frombuffer(sec['FARQ'], dtype=numpy.float32).copy() if 'FARQ' in sec else None
     if bool(host.get('echo')) != (played is not None):
         raise ValueError('malformed pipeline snapshot: the echo far-end queue')
-    return {'session': sec['SESS'], 'reblock': sec['RBLK'], 'host': host, 'played': played, 'session_config': ds['config'],
-            'reblock_config': dr['config']}
+    if ('drift' in host) != (dd is not None):
+        raise ValueError('malformed pipeline snapshot: the drift stage')
+    return {'session': sec['SESS'], 'reblock': sec['RBLK'], 'host': host, 'played': played, 'drift': sec.get('DRFT'),
+            'session_config': ds['config'], 'reblock_config': dr['config']}
 
 
 def check_pipeline_config(parts: dict, config: Config) -> None:
