@@ -973,6 +973,11 @@ int ryk_session_voice(ryk_engine* h, int id) {
 // Everything a session allocates and captures; on failure the caller frees the partly built session.
 static int session_build(Engine* e, Session* s, const ryk_session_config* cfg, int f0_method) {
   s->cfg = *cfg;
+  // the stream's times become frame counts at 1000 / frame_period frames per second; any other period rounds that rate, and the
+  // frame counts drift from the samples they stand for (6 ms: 167 or 166 frames a second for the true 166.67)
+  const double frames_per_second = 1000.0 / cfg->frame_period_ms;
+  RYK_CHECK(cfg->frame_period_ms > 0 && frames_per_second == floor(frames_per_second),
+            "the frame period must divide 1000 ms into a whole number of frames per second, such as 1, 2, 4, 5, 8 or 10 ms");
   s->hop = (int)(cfg->fs * cfg->frame_period_ms / 1000.0);
   s->rate = (int)lround(1000.0 / cfg->frame_period_ms);
   s->n_wave = (int)lrint(cfg->buffer_time * cfg->fs);

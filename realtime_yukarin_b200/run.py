@@ -142,7 +142,8 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
         stage1_model_path=config.stage1_model_path, stage1_config_path=config.stage1_config_path,
         stage2_model_path=config.stage2_model_path, stage2_config_path=config.stage2_config_path)
     if load_state is not None:
-        pipeline = RealtimePipeline.restore(state, config, engine=engine, depth=depth)
+        pipeline = RealtimePipeline.restore(state, config, engine=engine, depth=depth,
+                                            acoustic_param=converter.acoustic_converter.config.dataset.acoustic_param)
     else:
         pipeline = RealtimePipeline(config, acoustic_param=converter.acoustic_converter.config.dataset.acoustic_param, engine=engine, depth=depth,
                                 measure_f0=measure_input_statistics is not None, follow_f0=follow_input_f0, formant=formant,

@@ -82,6 +82,13 @@ class OutputReblocker(object):
             self._rid = None
 
 
+def model_frame_period(acoustic_param) -> float:
+    """The stream's frame period in ms: the stage-1 model's acoustic_param.frame_period (5 without one), as the reference builds its
+    vocoder and its three streams from it (run.py:41, encode_stream.py:21, convert_stream.py:19, decode_stream.py:17).  Config's
+    frame_period is read and not used, in the reference too."""
+    return float(getattr(acoustic_param, 'frame_period', 5))
+
+
 def _check_limiter(ceiling_db: float, output_scale: float, lookahead_ms: float, hold_ms: float) -> None:
     """the limiter's settings as Engine.session_limiter / session_set_limiter accept them, checked before a session exists"""
     lo, hi = LIMITER_CEILING_DB
@@ -169,10 +176,12 @@ class RealtimePipeline(object):
         self.config = config
         self.engine = engine or default_engine()
         p = acoustic_param
-        # analysis, the U-Nets and synthesis run at the models' rate; the sound card's rates are the session's device rates
+        # analysis, the U-Nets and synthesis run at the models' rate and frame period; the sound card's rates are the session's device
+        # rates
         fs = int(getattr(p, 'sampling_rate', 24000))
+        frame_period = model_frame_period(p)
         cfg = SessionConfig(
-            fs=fs, frame_period_ms=float(config.frame_period),
+            fs=fs, frame_period_ms=frame_period,
             f0_floor=float(getattr(p, 'f0_floor', 71.0)), f0_ceil=float(getattr(p, 'f0_ceil', 800.0)),
             fft_length=int(getattr(p, 'fft_length', 1024)), order=int(getattr(p, 'order', 8)), alpha=float(getattr(p, 'alpha', 0.466)),
             buffer_time=float(config.buffer_time), encode_extra_time=float(config.encode_extra_time),
@@ -213,8 +222,8 @@ class RealtimePipeline(object):
             n_out_cap = self.engine.session_io_geometry(self._sid)['max_out']
         else:
             # capacity of one step's synthesizer output, as the session sizes it: (decode-window samples // block + 4) blocks
-            rate = round(1000 / float(config.frame_period))
-            hop = round(fs * float(config.frame_period) / 1000)
+            rate = round(1000 / frame_period)
+            hop = round(fs * frame_period / 1000)
             td = round(config.buffer_time * rate) + 2 * round(config.decode_extra_time * rate)
             n_out_cap = (td * hop // config.vocoder_buffer_size + 4) * config.vocoder_buffer_size
         if denoise is not None:
@@ -486,12 +495,13 @@ class RealtimePipeline(object):
                              None if self._drift is None else self.engine.drift_snapshot(self._drift))
 
     @classmethod
-    def restore(cls, blob: bytes, config: Config, engine: Optional[Engine] = None, voice: int = 0, depth: int = 3) -> 'RealtimePipeline':
+    def restore(cls, blob: bytes, config: Config, engine: Optional[Engine] = None, voice: int = 0, depth: int = 3,
+                acoustic_param=None) -> 'RealtimePipeline':
         """The pipeline a snapshot was taken of, continued on `engine` (another engine or GPU too) and converting into `voice`: the same
         items give the same outputs bit for bit.  The models of `voice` must be loaded into `engine`.  Refused (ValueError) when the
-        blob's recorded configuration does not match `config`."""
+        blob's recorded configuration does not match `config` and the frame period of `acoustic_param`, as the constructor takes them."""
         parts = unpack_pipeline(blob)
-        check_pipeline_config(parts, config)
+        check_pipeline_config(parts, config, acoustic_param)
         self = cls.__new__(cls)
         self.config = config
         self.engine = engine or default_engine()
@@ -579,14 +589,15 @@ def unpack_pipeline(blob: bytes) -> dict:
             'session_config': ds['config'], 'reblock_config': dr['config']}
 
 
-def check_pipeline_config(parts: dict, config: Config) -> None:
-    """Refuse (ValueError, listing every difference) a pipeline snapshot whose recorded configuration is not what `config` makes."""
+def check_pipeline_config(parts: dict, config: Config, acoustic_param=None) -> None:
+    """Refuse (ValueError, listing every difference) a pipeline snapshot whose recorded configuration is not what `config` and the
+    model's `acoustic_param` make."""
     sc, rc, host = parts['session_config'], parts['reblock_config'], parts['host']
     cfg = sc['cfg']
     fs = int(cfg['fs'])
     crepe = VocodeMode(config.extract_f0_mode) is VocodeMode.CREPE
     want = [
-        ('frame_period', cfg['frame_period_ms'], float(config.frame_period)),
+        ('model frame_period', cfg['frame_period_ms'], model_frame_period(acoustic_param)),
         ('buffer_time', cfg['buffer_time'], float(config.buffer_time)),
         ('encode_extra_time', cfg['encode_extra_time'], float(config.encode_extra_time)),
         ('convert_extra_time', cfg['convert_extra_time'], float(config.convert_extra_time)),

@@ -102,7 +102,7 @@ class OracleEngine:
         self.sessions = getattr(self, 'sessions', {})
         sid = len(self.sessions)
         stats = self.stats if self.stats is not None else (float(np.log(150.0)), 0.2, float(np.log(250.0)), 0.2)
-        pc = opipe.PathConfig(threshold_db=cfg.threshold_db)
+        pc = opipe.PathConfig(frame_period=cfg.frame_period_ms, threshold_db=cfg.threshold_db)
         orc = opipe.StreamOracle(pc, self.p1, self.p2, stats, buffer_time=cfg.buffer_time,
                                  extra=(cfg.encode_extra_time, cfg.convert_extra_time, cfg.decode_extra_time), backend=self.backend)
         self.sessions[sid] = dict(orc=orc, out={}, step=0, last=None)

@@ -20,7 +20,7 @@ STATS = (float(np.log(150.0)), 0.2, float(np.log(250.0)), 0.2)
 def test_the_table_reaches_its_shapes():
     g = sg.BY_ID
     assert all(0 < x.Tw < x.Tp and x.Tp % 128 == 0 and x.Tp - x.Tw <= 128 and x.buckets <= sg.MAX_BUCKETS for x in sg.GEOMETRIES)
-    assert all(x.n_wave == x.n_feat * sg.HOP and x.e_wave == x.e_enc * sg.HOP for x in sg.GEOMETRIES)
+    assert all(x.n_wave == x.n_feat * x.hop and x.e_wave == x.e_enc * x.hop for x in sg.GEOMETRIES)
     assert g['G1'].n_feat == 1 and g['G1'].n_wave + 2 * g['G1'].e_wave == 120 and (g['G1'].Tw, g['G1'].Tp) == (21, 128)
     assert min(g['G2'].e_enc, g['G2'].e_conv, g['G2'].e_dec) > 0 and g['G2'].Td > g['G2'].n_feat and (g['G2'].Tw, g['G2'].Tp) == (50, 128)
     assert (g['G3'].Tw, g['G3'].Tp) == (128, 256) and g['G3'].Tw % 128 == 0
@@ -54,7 +54,7 @@ def test_oracle_stream_and_its_device_rows_hook(small_models, geo):
         # whole blocks, as many as end before the last pulse placed so far, which lies within fft_size samples of the end of the
         # (k + 1) Td frames handed to the synthesizer
         pulses = orc.synth.pulses()[0]
-        end = (k + 1) * geo.Td * sg.HOP
+        end = (k + 1) * geo.Td * geo.hop
         total += len(y)
         assert len(y) % B == 0, k
         if len(pulses):
