@@ -128,7 +128,6 @@ int agc_run(const AgcWork& w, const AgcState* st, AgcState* st_next, const float
 }  // namespace ryk
 
 using namespace ryk;
-struct ryk_engine { Engine impl; };
 
 extern "C" {
 

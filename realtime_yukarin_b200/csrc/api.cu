@@ -165,7 +165,6 @@ static int voice_for_update(Engine* e, int id, Voice** out) {
 
 using namespace ryk;
 
-struct ryk_engine { Engine impl; };
 static Engine* E(ryk_engine* e) { return &e->impl; }
 
 extern "C" {

@@ -175,7 +175,6 @@ int denoise_check(double reduction_db, const double* phi) {
 }  // namespace ryk
 
 using namespace ryk;
-struct ryk_engine { Engine impl; };
 
 extern "C" {
 

@@ -118,7 +118,6 @@ static Drift* get_drift(Engine* e, int id) { return (id >= 0 && id < (int)e->dri
 }  // namespace ryk
 
 using namespace ryk;
-struct ryk_engine { Engine impl; };
 
 extern "C" {
 

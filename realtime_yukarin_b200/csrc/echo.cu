@@ -113,7 +113,6 @@ int echo_check(int taps, int delay_frames, double suppression_db) {
 }  // namespace ryk
 
 using namespace ryk;
-struct ryk_engine { Engine impl; };
 
 extern "C" {
 

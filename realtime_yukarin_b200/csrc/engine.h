@@ -179,3 +179,6 @@ int gate_mask_run(Engine* e, const float* d_wave, int n, int frame_length, int h
                   double* d_mse_scratch, uint8_t* d_mask, int* d_index /*compacted frame ids*/, int* d_count, cudaStream_t st);
 
 }  // namespace ryk
+
+// The engine behind the public handle (include/ryk.h declares it opaque).
+struct ryk_engine { ryk::Engine impl; };

@@ -154,7 +154,6 @@ int limiter_run(const LimWork& w, const LimHist& cur, const LimHist& next, const
 }  // namespace ryk
 
 using namespace ryk;
-struct ryk_engine { Engine impl; };
 
 extern "C" {
 

@@ -65,7 +65,6 @@ static Reblock* get_reblock(Engine* e, int id) { return (id >= 0 && id < (int)e-
 }  // namespace ryk
 
 using namespace ryk;
-struct ryk_engine { Engine impl; };
 
 extern "C" {
 

@@ -21,7 +21,7 @@ namespace ryk {
 
 constexpr uint64_t kSnapMagic = 0x0050414e534b5952ull;     // "RYKSNAP\0"
 constexpr uint32_t kSnapVersion = 1;
-// The payloads are these structs as they lie in memory (and SnapHost in session.cu, ReblockState in reblock.cu, DriftSnap in drift.cu).  A change to any of them
+// The payloads are these structs as they lie in memory (and SnapHost in session_snapshot.cu, ReblockState in reblock.cu, DriftSnap in drift.cu).  A change to any of them
 // changes what a blob means: bump kSnapVersion with it, so that an older blob is refused before anything is allocated, and the sizes here.
 static_assert(sizeof(ryk_snapshot_session) == 224 && sizeof(ryk_snapshot_reblock) == 32, "snapshot layout: bump kSnapVersion");
 static_assert(sizeof(F0Map) == 64 && sizeof(F0Stats) == 24 && sizeof(ResampleState) == 16, "snapshot layout: bump kSnapVersion");
