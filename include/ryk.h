@@ -466,6 +466,40 @@ int ryk_session_get_agc(ryk_engine* e, int session_id, double* target_db, double
 int ryk_session_agc_stats(ryk_engine* e, int session_id, double* level_db, double* gain_db, int* active);
 int ryk_agc(ryk_engine* e, const float* x, int n, int fs, double target_db, double max_gain_db, double gate_db, float* z);
 
+/* Pitch correction (DESIGN.md §4m, DECIDE P1-P4): pulls each converted note toward the nearest pitch of a musical scale, with a retune
+ * time.  It runs on the converted f0 the synthesizer is given, one value per frame (0: unvoiced), in stream order, in FP64:
+ *   a voiced frame (0 < f0 < inf) sits at s = 69 + 12 (log2 f0 - log2 a4_hz) semitones; its target n is the nearest note whose pitch class
+ *   (n - key) mod 12 is set in scale_mask (bit j: pitch class key + j; ties to the lower note), except that the previous voiced frame's
+ *   target is kept while it is in the scale and |s - n_prev| < 0.65 (hysteresis: a note sung between two scale notes does not flap);
+ *   d = n - s;  c = d on the first voiced frame after an unvoiced one (no glide across a gap), else c += beta (d - c),
+ *   beta = -expm1(-frame_period / retune_ms), 1 for retune_ms = 0 (a hard snap);
+ *   f0' = f0 exp2(amount c / 12).  Any other frame is returned as it is and keeps c and the previous target.
+ * amount = 0 returns every frame bit for bit, so the correction can be faded out and in mid-stream.  The correction reaches 1 - 1/e of a
+ * note change retune_ms after it.
+ * ryk_session_pitch_correct: fresh session only (no chunk pushed), once.  The correction starts at amount 0 (key 0, the chromatic
+ *   scale 0xfff, a4_hz 440, retune_ms 50), so it changes nothing until ryk_session_set_pitch_correct.  It corrects the frames each step
+ *   appends to the decode window, once each and in stream order, so with a decode extra the synthesizer reads every frame of its window
+ *   corrected exactly once.  One more kernel per step on the decode stream; latency, geometry and capacities are unchanged.  A session
+ *   without it runs exactly the kernels it ran before.  With constant settings the synthesizer is given ryk_pitch_correct of the f0 the
+ *   session gives it without the correction, bitwise (as float).  A voice switch and group membership keep its state.
+ * ryk_session_set_pitch_correct: key in [0, 11], scale_mask a nonzero 12-bit mask, a4_hz in [400, 480], retune_ms in [0, 1000],
+ *   amount in [0, 1]; from the next submitted step on (chunks in flight keep theirs); allowed with chunks in flight and on a group
+ *   member; no device wait, no kernel.
+ * ryk_session_get_pitch_correct: the settings of the next submitted step.  Any pointer may be NULL.
+ * ryk_session_pitch_stats: waits for the decode stream of the submitted steps, then writes the voiced frames the last step corrected
+ *   and the mean and largest |amount c| over them in cents (0 when none).  Any pointer may be NULL.
+ * ryk_pitch_correct: the same correction over n frames of a whole signal on the same kernel from a fresh state (fs positive, frame_period
+ *   the stream's frame period in ms, which sets beta).
+ * Refused, changing nothing: an unknown session, enabling on a session that ran a step or twice, settings out of range or not finite,
+ * an empty scale mask, set / get / stats calls on a session without the correction. */
+int ryk_session_pitch_correct(ryk_engine* e, int session_id);
+int ryk_session_set_pitch_correct(ryk_engine* e, int session_id, int key, int scale_mask, double a4_hz, double retune_ms, double amount);
+int ryk_session_get_pitch_correct(ryk_engine* e, int session_id, int* key, int* scale_mask, double* a4_hz, double* retune_ms,
+                                  double* amount);
+int ryk_session_pitch_stats(ryk_engine* e, int session_id, long long* voiced, double* mean_cents, double* max_cents);
+int ryk_pitch_correct(ryk_engine* e, const double* f0, int n, int fs, double frame_period, int key, int scale_mask, double a4_hz,
+                      double retune_ms, double amount, double* out);
+
 /* Moving a session (DESIGN.md §4k): a snapshot of a quiescent session's stream state, restored bit for bit as a new session on the same
  * engine, another engine of the same device or an engine of another device.  After k steps of session A, a snapshot restored as B, the
  * next chunks fed to A and B give the same outputs bit for bit: windows, resampler positions, the learned noise profile, the echo
@@ -477,7 +511,7 @@ int ryk_agc(ryk_engine* e, const float* x, int n, int fs, double target_db, doub
  *   keeps running as if no snapshot had been taken.  A group member can be snapshotted: its stream state does not depend on the group.
  * ryk_session_restore: creates a session on engine e converting into voice_id, with the configuration the blob records (session
  *   config, device rates and their taps, f0 method, noise suppression, echo cancellation with its taps and delay, limiter with its
- *   look-ahead and hold, AGC, f0 measuring), through the same code ryk_session_create and the enabling calls run, copies the state
+ *   look-ahead and hold, AGC, f0 measuring, pitch correction), through the same code ryk_session_create and the enabling calls run, copies the state
  *   into the new session's buffers and sets its step count to the source's.  *id receives the new session.  To restore a group,
  *   restore its members and group them again (ryk_group_create / ryk_group_add).
  *   voice_id names the source's voice as loaded on engine e: the stream continues, so the f0 map (both sides, a pitch offset or a

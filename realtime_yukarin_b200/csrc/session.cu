@@ -599,8 +599,10 @@ static int session_back(Engine* e, Session* s) {
   if (stage_time(s, 4, 0, r, s->sD)) return -1;
   if (synth_host_advance(e, s->synth, s->Td, s->sD)) return -1;
   const int max_blocks = s->max_blocks;
-  // the limiter's settings: its pinned slot was last read by a copy of step k - kRing, ahead of that step's decode slides
+  // the limiter's and the pitch correction's settings: their pinned slots were last read by copies of step k - kRing, ahead of that
+  // step's decode slides
   if (host_block_sync(s->lim.block, s->lim.w.params, k, ev.dslide, s->sD)) return -1;
+  if (host_block_sync(s->pitch.block, s->pitch.w.params, k, ev.dslide, s->sD)) return -1;
   if (run_handoff_graph(e, s, k, &HandoffGraphs::dec_slide, s->sD, [&](int h) -> int {
         const HandoffSlot& o = s->ho[h];
         SlideBatch sb; sb.n = 0;
@@ -608,6 +610,8 @@ static int session_back(Engine* e, Session* s) {
         slide_add<float>(sb, p.dw_ap, o.ap_out + (size_t)pc * s->nb, q.dw_ap, s->Td, s->n_feat, s->nb);
         slide_add<float>(sb, p.dw_sp, o.sp_out + (size_t)pc * s->nb, q.dw_sp, s->Td, s->n_feat, s->nb);
         if (slide_batch(sb, s->sD)) return -1;
+        // P4: the rows this step appended, corrected once each in stream order; older rows were corrected when they were appended
+        if (s->pitch.on && pitch_run(s->pitch.w, q.dw_f0 + (s->Td - s->n_feat), s->n_feat, s->sD)) return -1;
         k_f32_to_f64<<<(s->Td + 127) / 128, 128, 0, s->sD>>>(q.dw_f0, s->dec_f0_f64, s->Td);
         RYK_CUDA(cudaGetLastError());
         return 0;

@@ -9,6 +9,7 @@
 #include "engine.h"
 #include "features.h"
 #include "limiter.h"
+#include "pitch.h"
 
 namespace ryk {
 
@@ -116,7 +117,7 @@ struct Stage2Lane {
   StageGraph s2_layers;            // alone: stage-2 layers 1..14
 };
 
-// The optional stages of a session, one member each (DESIGN.md §4a, §4f-§4j): `on`, the host block whose device copy is the `params` of
+// The optional stages of a session, one member each (DESIGN.md §4a, §4f-§4j, §4m): `on`, the host block whose device copy is the `params` of
 // the work struct the kernels read, the settings as the user gave them, and the stage's buffers.  Per-parity state stays in ParitySet.
 struct F0Control {                 // the f0 map, formant ratio and speaker statistics
   static constexpr const char* refusal = "f0 measurement is not enabled for this session";
@@ -157,6 +158,12 @@ struct AgcStage {
   AgcWork w;
   double db[3] = {};               // target, max gain and gate
   float* d_chunk = nullptr;        // the step's gain-controlled chunk
+};
+struct PitchStage {
+  static constexpr const char* refusal = "pitch correction is not enabled for this session (ryk_session_pitch_correct)";
+  bool on = false;
+  HostBlock<PitchParams> block;
+  PitchWork w;
 };
 
 struct Group;
@@ -202,6 +209,7 @@ struct Session {
   EchoStage aec;
   LimiterStage lim;
   AgcStage agc;
+  PitchStage pitch;
   BufferSet mem;                   // every device and pinned buffer above
 };
 

@@ -1,4 +1,4 @@
-// session_controls.cu -- the host API of a session's optional stages (DESIGN.md §4a, §4f-§4j).  The setters change host state only;
+// session_controls.cu -- the host API of a session's optional stages (DESIGN.md §4a, §4f-§4j, §4m).  The setters change host state only;
 // host_block_sync carries it to the device in front of the stage's readers of the next submitted step, alone or in a group.
 #include <math.h>
 #include <string.h>
@@ -399,6 +399,57 @@ int ryk_session_agc_stats(ryk_engine* h, int id, double* level_db, double* gain_
   if (level_db) *level_db = mt.started ? 10.0 * log10(mt.level) : -HUGE_VAL;
   if (gain_db) *gain_db = 20.0 * log10(mt.gain);
   if (active) *active = mt.active;
+  return 0;
+}
+
+// ---- pitch correction (DESIGN.md §4m) ----
+int ryk_session_pitch_correct(ryk_engine* h, int id) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Session* s = fresh_session(e, id, "pitch correction can only be enabled on a fresh session (no chunk pushed): the decode slides are captured at the first steps");
+  if (!s) return -2;
+  RYK_CHECK(!s->pitch.on, "pitch correction is already enabled for this session");
+  PitchWork& w = s->pitch.w;
+  // amount 0 changes nothing until the caller sets the correction
+  const PitchParams first = pitch_params(s->cfg.frame_period_ms, 0, 0xfff, 440.0, 50.0, 0.0);
+  if (host_block_alloc(s->mem, s->pitch.block, &w.params, first) || s->mem.device(&w.state, 1)) return -1;
+  PitchState st;
+  pitch_state_init(&st);
+  if (upload_wait(e, w.state, &st)) return -1;
+  s->pitch.on = true;
+  return 0;
+}
+
+int ryk_session_set_pitch_correct(ryk_engine* h, int id, int key, int scale_mask, double a4_hz, double retune_ms, double amount) {
+  Session* s = stage_session(&h->impl, id, &Session::pitch);
+  if (!s) return -2;
+  if (int rc = pitch_check(key, scale_mask, a4_hz, retune_ms, amount)) return rc;
+  s->pitch.block.edit() = pitch_params(s->cfg.frame_period_ms, key, scale_mask, a4_hz, retune_ms, amount);
+  return 0;
+}
+
+int ryk_session_get_pitch_correct(ryk_engine* h, int id, int* key, int* scale_mask, double* a4_hz, double* retune_ms, double* amount) {
+  Session* s = stage_session(&h->impl, id, &Session::pitch);
+  if (!s) return -2;
+  const PitchParams& P = s->pitch.block.next;
+  if (key) *key = P.key;
+  if (scale_mask) *scale_mask = P.scale;
+  if (a4_hz) *a4_hz = P.a4;
+  if (retune_ms) *retune_ms = P.retune_ms;
+  if (amount) *amount = P.amount;
+  return 0;
+}
+
+int ryk_session_pitch_stats(ryk_engine* h, int id, long long* voiced, double* mean_cents, double* max_cents) {
+  Engine* e = &h->impl;
+  RYK_CUDA(cudaSetDevice(e->device));
+  Session* s = stage_session(e, id, &Session::pitch);
+  if (!s) return -2;
+  PitchState st;
+  if (read_back(e, s->pitch.w.state, s->sD, &st)) return -1;      // behind the decode slides of every submitted step
+  if (voiced) *voiced = st.voiced;
+  if (mean_cents) *mean_cents = st.voiced ? st.sum_cents / (double)st.voiced : 0.0;
+  if (max_cents) *max_cents = st.max_cents;
   return 0;
 }
 

@@ -35,6 +35,14 @@ static void snap_host(Session* s, SnapHost& h, bool save) {
   x(s->synth->host_noise_slot, h.host_noise_slot);
 }
 
+// The host side of the pitch correction, in a section of its own that only a session with the correction writes (PTCH), so that
+// SnapHost and the blobs of every other session stay as they were.
+struct SnapPitch {
+  PitchParams next;
+  long long dirty;
+};
+static_assert(sizeof(SnapPitch) == 56, "snapshot layout: bump kSnapVersion (snapshot.h)");
+
 // One section's payload: its tag, where it lies and its size.
 struct SnapRegion { uint32_t tag; void* p; size_t bytes; };
 
@@ -93,6 +101,10 @@ static std::vector<SnapRegion> session_regions(const Session* s) {
     add("AGCP", s->agc.w.params, sizeof(AgcParams));
     add("AGCM", s->agc.w.meter, sizeof(AgcMeter));
   }
+  if (s->pitch.on) {
+    add("PTCP", s->pitch.w.params, sizeof(PitchParams));
+    add("PTCS", s->pitch.w.state, sizeof(PitchState));
+  }
   const SynthDev& D = s->synth->dev;
   const size_t sb = D.fft_size / 2 + 1;
   add("SYST", D.state, sizeof(SynthState));
@@ -111,11 +123,13 @@ static std::vector<SnapRegion> session_regions(const Session* s) {
 static void unet_channels(const UNet* n, int* c) { c[0] = n->in_ch; c[1] = n->out_ch; c[2] = n->base; }
 
 // What a session's blob records, in order: CONF (ryk_snapshot_session), TAPI / TAPO (the device rates' taps, when set), HOST (SnapHost),
-// FARN (the far end of the next step, with echo cancellation), all in host memory, then the device regions of session_regions.
+// FARN (the far end of the next step, with echo cancellation), PTCH (SnapPitch, with pitch correction), all in host memory, then the
+// device regions of session_regions.
 struct SessionBlob {
   ryk_snapshot_session conf;
   std::vector<double> taps_in, taps_out;
   SnapHost host;
+  SnapPitch pitch;
   std::vector<SnapRegion> head, regions;
   std::vector<size_t> payloads() const {
     std::vector<size_t> p;
@@ -159,6 +173,12 @@ static int session_blob(Engine* e, int id, Session** out, SessionBlob* b) {
   if (c.out_rate) b->head.push_back({snap_tag("TAPO"), b->taps_out.data(), sizeof(double) * c.out_taps});
   b->head.push_back({snap_tag("HOST"), &b->host, sizeof(b->host)});
   if (c.echo) b->head.push_back({snap_tag("FARN"), s->aec.far_next.data(), sizeof(float) * s->n_in});
+  if (s->pitch.on) {
+    memset(&b->pitch, 0, sizeof(b->pitch));
+    b->pitch.next = s->pitch.block.next;
+    b->pitch.dirty = s->pitch.block.dirty;
+    b->head.push_back({snap_tag("PTCH"), &b->pitch, sizeof(b->pitch)});
+  }
   b->regions = session_regions(s);
   *out = s;
   return 0;
@@ -170,6 +190,7 @@ static double ms_since(Clock::time_point t) { return std::chrono::duration<doubl
 // The sections of a session blob in front of its device regions, as restore_check found them.
 struct BlobSections {
   const SnapSection *taps_in = nullptr, *taps_out = nullptr, *host = nullptr, *far = nullptr;
+  const SnapSection* pitch = nullptr;    // present when the session had pitch correction
   size_t regions = 0;              // index of the first device region
 };
 
@@ -196,7 +217,7 @@ static int restore_check(Engine* e, int voice_id, const void* buf, size_t bytes,
     const char* refusal = crepe_plan_refusal(c->cfg.fs);
     if (refusal) { set_error(refusal); return -2; }
   }
-  // CONF, then TAPI / TAPO as the configuration says, HOST and FARN
+  // CONF, then TAPI / TAPO as the configuration says, HOST and FARN, and PTCH when present
   size_t i = 1;
   auto next = [&](const char (&t)[5]) { return i < sec->size() && (*sec)[i].tag == snap_tag(t) ? &(*sec)[i++] : nullptr; };
   auto sized = [&](const char (&t)[5], size_t n) { const SnapSection* x = next(t); return x && x->bytes == n ? x : nullptr; };
@@ -204,6 +225,8 @@ static int restore_check(Engine* e, int voice_id, const void* buf, size_t bytes,
   RYK_CHECK(!c->out_rate || (w->taps_out = sized("TAPO", sizeof(double) * c->out_taps)), "malformed session snapshot: output resampler taps");
   RYK_CHECK((w->host = sized("HOST", sizeof(SnapHost))), "malformed session snapshot: host state");
   RYK_CHECK(!c->echo || (w->far = next("FARN")), "malformed session snapshot: far end");   // its size is checked against the session
+  if (i < sec->size() && (*sec)[i].tag == snap_tag("PTCH"))
+    RYK_CHECK((w->pitch = sized("PTCH", sizeof(SnapPitch))), "malformed session snapshot: pitch correction");
   w->regions = i;
   return 0;
 }
@@ -217,6 +240,7 @@ static int restore_enable(ryk_engine* h, int id, const ryk_snapshot_session& c, 
   if (c.limiter && ryk_session_limiter(h, id, c.limiter_lookahead_ms, c.limiter_hold_ms)) return -1;
   if (c.agc && ryk_session_agc(h, id, -26.0, 20.0, -50.0)) return -1;
   if (c.f0_measure && ryk_session_f0_measure(h, id, 1)) return -1;
+  if (w.pitch && ryk_session_pitch_correct(h, id)) return -1;
   return 0;
 }
 
@@ -250,6 +274,12 @@ static int restore_state(Engine* e, Session* s, const std::vector<SnapSection>& 
   snap_host(s, hs, false);
   s->collected = s->step;
   if (w.far) memcpy(s->aec.far_next.data(), w.far->data, w.far->bytes);
+  if (w.pitch) {
+    SnapPitch sp;
+    memcpy(&sp, w.pitch->data, sizeof(sp));
+    s->pitch.block.next = sp.next;
+    s->pitch.block.dirty = sp.dirty != 0;
+  }
   return 0;
 }
 

@@ -15,6 +15,7 @@
 #include "echo.h"
 #include "features.h"
 #include "limiter.h"
+#include "pitch.h"
 #include "synth.h"
 
 namespace ryk {
@@ -29,6 +30,7 @@ static_assert(sizeof(DenoiseParams) == 2088 && sizeof(DenoiseLearn) == 4144 && s
 static_assert(sizeof(EchoParams) == 8 && sizeof(EchoFilter) == 541776, "snapshot layout: bump kSnapVersion");
 static_assert(sizeof(LimParams) == 16 && sizeof(LimState) == 8 && sizeof(LimMeter) == 16, "snapshot layout: bump kSnapVersion");
 static_assert(sizeof(AgcParams) == 56 && sizeof(AgcState) == 1064 && sizeof(AgcMeter) == 24, "snapshot layout: bump kSnapVersion");
+static_assert(sizeof(PitchParams) == 48 && sizeof(PitchState) == 40, "snapshot layout: bump kSnapVersion");
 static_assert(sizeof(SynthState) == 136, "snapshot layout: bump kSnapVersion");
 enum : uint32_t { kSnapSession = 1, kSnapReblock = 2, kSnapPipeline = 3, kSnapDrift = 4 };   // kinds (a pipeline blob is written by worker.py)
 

@@ -10,6 +10,7 @@ _os.environ.setdefault('CUDA_DEVICE_MAX_CONNECTIONS', '32')
 import ctypes
 import math
 import os
+import struct
 import threading
 from pathlib import Path
 from typing import Any, Dict, List, Optional, Sequence, Tuple
@@ -80,8 +81,8 @@ def _struct_dict(x) -> Dict[str, Any]:
 def describe_snapshot(blob: bytes) -> Dict[str, Any]:
     """ryk_snapshot_describe: verify a snapshot blob (header, size, FNV-1a-64 checksum, section walk) without an engine or a device.
     Returns kind ('session' / 'reblock' / 'pipeline' / 'drift'), version, config (the recorded configuration of a session, re-blocker or
-    drift stage, as a dict; None for a pipeline) and sections [(tag, payload bytes)] in blob order; raises RykError for a blob it
-    refuses."""
+    drift stage, as a dict; None for a pipeline), pitch_correct (a session's pitch correction settings for its next step, from its PTCH
+    section; None without the stage) and sections [(tag, payload bytes)] in blob order; raises RykError for a blob it refuses."""
     lib = load_library()
     blob = bytes(blob)
     kind, version = ctypes.c_int(), ctypes.c_int()
@@ -98,7 +99,13 @@ def describe_snapshot(blob: bytes) -> Dict[str, Any]:
     config = _struct_dict(ss) if k == 'session' else _struct_dict(sr) if k == 'reblock' else None
     if k == 'drift' and names[0] == 'DCNF' and sizes[0] >= ctypes.sizeof(SnapshotDrift):
         config = _struct_dict(SnapshotDrift.from_buffer_copy(blob, 48))     # after the header and the DCNF section header
-    return {'kind': k, 'version': version.value, 'config': config, 'sections': list(zip(names, (int(x) for x in sizes)))}
+    sections = list(zip(names, (int(x) for x in sizes)))
+    pitch = None
+    if k == 'session' and 'PTCH' in names:
+        at = 32 + sum(16 + (n + 7) // 8 * 8 for _, n in sections[:names.index('PTCH')]) + 16
+        a4, _, retune_ms, amount, _, key, scale = struct.unpack_from('<5d2i', blob, at)
+        pitch = {'key': key, 'scale': scale, 'a4_hz': a4, 'retune_ms': retune_ms, 'amount': amount}
+    return {'kind': k, 'version': version.value, 'config': config, 'pitch_correct': pitch, 'sections': sections}
 
 
 def _first_int(blob: bytes) -> int:
@@ -143,7 +150,8 @@ EXPORTED_SYMBOLS = [
     'ryk_session_noise_profile', 'ryk_denoise', 'ryk_session_echo_cancel', 'ryk_session_echo_reference', 'ryk_session_set_echo_suppression',
     'ryk_session_echo_stats', 'ryk_echo_cancel', 'ryk_session_limiter', 'ryk_session_set_limiter', 'ryk_session_get_limiter',
     'ryk_session_limiter_stats', 'ryk_limit', 'ryk_session_agc', 'ryk_session_set_agc', 'ryk_session_get_agc', 'ryk_session_agc_stats',
-    'ryk_agc', 'ryk_session_snapshot_size', 'ryk_session_snapshot', 'ryk_session_restore', 'ryk_reblock_snapshot_size',
+    'ryk_agc', 'ryk_session_pitch_correct', 'ryk_session_set_pitch_correct', 'ryk_session_get_pitch_correct', 'ryk_session_pitch_stats',
+    'ryk_pitch_correct', 'ryk_session_snapshot_size', 'ryk_session_snapshot', 'ryk_session_restore', 'ryk_reblock_snapshot_size',
     'ryk_reblock_snapshot', 'ryk_reblock_restore', 'ryk_snapshot_describe', 'ryk_snapshot_seal',
     'ryk_snapshot_last_times', 'ryk_drift_create', 'ryk_drift_destroy', 'ryk_drift_set', 'ryk_drift_get', 'ryk_drift_push',
     'ryk_drift_stats', 'ryk_drift_resample', 'ryk_drift_snapshot_size', 'ryk_drift_snapshot', 'ryk_drift_restore',
@@ -163,6 +171,11 @@ AGC_TARGET_DB = (-40.0, -6.0)            # automatic gain control: target levels
 AGC_MAX_GAIN_DB = (0.0, 30.0)            # ... largest gain either way
 AGC_GATE_DB = (-80.0, -20.0)             # ... and gates: blocks at or under the gate leave level and gain as they are
 AGC_LINEAR = ('target', 'gate', 'gmax', 'ginv', 'a', 's_up', 's_dn')     # ryk_session_get_agc's linear values, in order
+PITCH_A4_HZ = (400.0, 480.0)             # pitch correction: reference pitches of A4 it accepts
+PITCH_RETUNE_MS = (0.0, 1000.0)          # ... retune times (0: a hard snap)
+PITCH_SCALES = {'chromatic': 0xfff, 'major': 0b101010110101, 'minor': 0b010110101101}    # bit j: pitch class key + j
+PITCH_NOTE_NAMES = ('C', 'C#', 'D', 'D#', 'E', 'F', 'F#', 'G', 'G#', 'A', 'A#', 'B')
+_PITCH_FLATS = {'DB': 'C#', 'EB': 'D#', 'GB': 'F#', 'AB': 'G#', 'BB': 'A#'}
 DRIFT_MAX_PPM = 2000.0                   # clock drift stage: the largest max_ppm a drift object accepts
 
 
@@ -189,6 +202,26 @@ def formant_ratio(ratio=None, semitones=None) -> float:
     if (ratio is None) == (semitones is None):
         raise ValueError('give exactly one of ratio and semitones')
     return float(ratio) if ratio is not None else 2.0 ** (float(semitones) / 12.0)
+
+
+def pitch_key(key) -> int:
+    """A key as a pitch class 0-11 (0 is C): an int or its digits, or a note name such as 'A', 'F#' or 'Bb'."""
+    if isinstance(key, str) and not key.strip().isdigit():
+        name = key.strip().upper()
+        name = _PITCH_FLATS.get(name, name)
+        if name not in PITCH_NOTE_NAMES:
+            raise ValueError(f'unknown key {key!r}: use 0-11 or one of {", ".join(PITCH_NOTE_NAMES)} (or a flat such as Bb)')
+        return PITCH_NOTE_NAMES.index(name)
+    return int(key)
+
+
+def pitch_scale(scale) -> int:
+    """A scale as a 12-bit mask of pitch classes relative to the key: an int, or 'chromatic', 'major' or 'minor'."""
+    if isinstance(scale, str):
+        if scale.lower() not in PITCH_SCALES:
+            raise ValueError(f'unknown scale {scale!r}: use a 12-bit mask or one of {", ".join(PITCH_SCALES)}')
+        return PITCH_SCALES[scale.lower()]
+    return int(scale)
 
 
 def stage2_row_bands(Tp: int, W: int, keep_begin: int, keep_len: int) -> numpy.ndarray:
@@ -896,6 +929,50 @@ class Engine(object):
         self._check(self.lib.ryk_agc(self._h, _fp(x), len(x), int(fs), ctypes.c_double(target_db), ctypes.c_double(max_gain_db),
                                      ctypes.c_double(gate_db), _fp(z)))
         return z
+
+    # ---- pitch correction ----
+    def session_pitch_correct(self, sid: int):
+        """Fresh session only: pull each converted note toward the nearest note of a scale on the device.  Starts at amount 0 (no
+        change) until session_set_pitch_correct; one more kernel per step, no delay."""
+        self._check(self.lib.ryk_session_pitch_correct(self._h, int(sid)))
+
+    def session_set_pitch_correct(self, sid: int, key=None, scale=None, a4_hz: Optional[float] = None, retune_ms: Optional[float] = None,
+                                  amount: Optional[float] = None):
+        """New settings from the next submitted step on (chunks in flight keep theirs); a None keeps that setting.  key: 0-11 or a
+        note name; scale: a 12-bit mask or 'chromatic' / 'major' / 'minor'; a4_hz 400-480; retune_ms 0-1000 (0: a hard snap); amount
+        0-1."""
+        cur = self.session_get_pitch_correct(sid)
+        key = cur['key'] if key is None else pitch_key(key)
+        scale = cur['scale'] if scale is None else pitch_scale(scale)
+        a4_hz = cur['a4_hz'] if a4_hz is None else a4_hz
+        retune_ms = cur['retune_ms'] if retune_ms is None else retune_ms
+        amount = cur['amount'] if amount is None else amount
+        self._check(self.lib.ryk_session_set_pitch_correct(self._h, int(sid), int(key), int(scale), ctypes.c_double(a4_hz),
+                                                           ctypes.c_double(retune_ms), ctypes.c_double(amount)))
+
+    def session_get_pitch_correct(self, sid: int) -> Dict[str, Any]:
+        """key, scale (mask), a4_hz, retune_ms and amount of the next submitted step."""
+        k, m, a4, rt, am = ctypes.c_int(), ctypes.c_int(), ctypes.c_double(), ctypes.c_double(), ctypes.c_double()
+        self._check(self.lib.ryk_session_get_pitch_correct(self._h, int(sid), ctypes.byref(k), ctypes.byref(m), ctypes.byref(a4),
+                                                           ctypes.byref(rt), ctypes.byref(am)))
+        return {'key': k.value, 'scale': m.value, 'a4_hz': a4.value, 'retune_ms': rt.value, 'amount': am.value}
+
+    def session_pitch_stats(self, sid: int) -> Tuple[int, float, float]:
+        """(voiced frames, mean and largest applied correction in cents) over the frames the last submitted step corrected; waits for
+        the submitted steps' decode slides."""
+        n, mean, mx = ctypes.c_longlong(), ctypes.c_double(), ctypes.c_double()
+        self._check(self.lib.ryk_session_pitch_stats(self._h, int(sid), ctypes.byref(n), ctypes.byref(mean), ctypes.byref(mx)))
+        return n.value, mean.value, mx.value
+
+    def pitch_correct(self, f0, fs: int = 24000, frame_period: float = 5.0, key=0, scale='chromatic', a4_hz: float = 440.0,
+                      retune_ms: float = 50.0, amount: float = 1.0) -> numpy.ndarray:
+        """The session's pitch correction over a whole f0 contour (0: unvoiced) at `frame_period` ms: a fresh state, float64 out."""
+        f0 = numpy.ascontiguousarray(f0, dtype=numpy.float64).ravel()
+        out = numpy.empty_like(f0)
+        self._check(self.lib.ryk_pitch_correct(self._h, _dp(f0), len(f0), int(fs), ctypes.c_double(frame_period), pitch_key(key),
+                                               pitch_scale(scale), ctypes.c_double(a4_hz), ctypes.c_double(retune_ms),
+                                               ctypes.c_double(amount), _dp(out)))
+        return out
 
     # ---- moving a session (DESIGN.md §4k) ----
     def session_snapshot(self, sid: int) -> bytes:

@@ -19,8 +19,9 @@ import numpy
 from . import wave_io
 from .config import Config
 from .converter import YukarinConverter
+from .engine import pitch_key, pitch_scale
 from .models import write_f0_statistics
-from .worker import RealtimePipeline, unpack_pipeline
+from .worker import RealtimePipeline, pitch_settings, unpack_pipeline
 
 
 def audio_loop(pipeline: RealtimePipeline, read_chunk: Callable[[], Optional[numpy.ndarray]],
@@ -83,7 +84,21 @@ def save_state_file(pipeline: RealtimePipeline, path: Path) -> None:
 # options that set up the stream's stages, with the values that leave them off: a state file brings its own stages
 _STAGE_OPTIONS = {'follow_input_f0': None, 'pitch': 0.0, 'formant': 0.0, 'denoise': None, 'noise_profile': None, 'learn_noise': None,
                   'echo_cancel': None, 'echo_delay': 0.0, 'echo_suppression': 0.0, 'limit': None, 'limit_lookahead': None,
-                  'limit_hold': None, 'agc': None, 'agc_max_gain': None, 'agc_gate': None, 'drift_ppm': None, 'drift': None}
+                  'limit_hold': None, 'agc': None, 'agc_max_gain': None, 'agc_gate': None, 'drift_ppm': None, 'drift': None,
+                  'autotune': None, 'retune_ms': None, 'autotune_amount': None}
+
+
+def autotune_settings(autotune: str, retune_ms: Optional[float] = None, amount: Optional[float] = None) -> dict:
+    """--autotune KEY[:SCALE] (SCALE: major when missing, minor, chromatic or a 12-bit mask such as 0xab5) with --retune_ms (50 when
+    None) and --autotune_amount (1 when None), as RealtimePipeline(pitch_correct=...) takes them."""
+    key, _, scale = str(autotune).partition(':')
+    scale = scale.strip() or 'major'
+    try:
+        scale = int(scale, 0)
+    except ValueError:
+        pass
+    return dict(key=pitch_key(key), scale=pitch_scale(scale), retune_ms=50.0 if retune_ms is None else float(retune_ms),
+                amount=1.0 if amount is None else float(amount))
 
 
 def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path] = None, max_chunks: Optional[int] = None,
@@ -93,7 +108,8 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
         echo_delay: float = 0.0, echo_suppression: float = 0.0, limit: Optional[float] = None,
         limit_lookahead: Optional[float] = None, limit_hold: Optional[float] = None, agc: Optional[float] = None,
         agc_max_gain: Optional[float] = None, agc_gate: Optional[float] = None, save_state: Optional[Path] = None,
-        load_state: Optional[Path] = None, drift_ppm: Optional[float] = None, drift: Optional[float] = None) -> int:
+        load_state: Optional[Path] = None, drift_ppm: Optional[float] = None, drift: Optional[float] = None,
+        autotune: Optional[str] = None, retune_ms: Optional[float] = None, autotune_amount: Optional[float] = None) -> int:
     """`measure_input_statistics`: measure the speaker's log-f0 statistics during the run and write them to this file at the end;
     `follow_input_f0`: convert with the measured statistics once this many voiced frames are counted; `pitch`: semitones added to
     the target voice's mean f0; `formant`: semitones by which the converted spectral envelope moves; `denoise`: filter the input's
@@ -109,7 +125,9 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
     configuration and with the options that set up stages, which the file brings; --save_noise_profile and --measure_input_statistics
     then need the stage in the file; `drift_ppm`: play the output (1 + drift_ppm 1e-6) times as long through the drift stage, a fixed trim
     for an output sound card whose clock runs that much fast; `drift`: let a controller find the trim, up to +-drift ppm, from the output
-    card's backlog (live audio only: with wav files there is no second clock)."""
+    card's backlog (live audio only: with wav files there is no second clock); `autotune`: 'KEY[:SCALE]', pull each converted note
+    toward the nearest note of that scale (major when no SCALE is given) with a retune time of `retune_ms` (50 when None; 0 snaps) and
+    `autotune_amount` of the correction (1 when None)."""
     state = None
     if load_state is not None:
         values = locals()
@@ -126,6 +144,9 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
         raise ValueError('--drift and --drift_ppm exclude each other: the controller sets the trim, or --drift_ppm fixes it')
     if drift is not None and wav_in is not None:
         raise ValueError('--drift needs live audio: with --wav_in there is no second clock to follow (--drift_ppm sets a fixed trim)')
+    if autotune is None and (retune_ms is not None or autotune_amount is not None):
+        raise ValueError('--retune_ms and --autotune_amount need --autotune')
+    pitch_correct = None if autotune is None else pitch_settings(autotune_settings(autotune, retune_ms, autotune_amount))
     if agc is None and (agc_max_gain is not None or agc_gate is not None):
         raise ValueError('--agc_max_gain and --agc_gate need --agc')
     if limit is None and (limit_lookahead is not None or limit_hold is not None):
@@ -156,7 +177,8 @@ def run(config_path: Path, wav_in: Optional[Path] = None, wav_out: Optional[Path
                                 agc_max_gain_db=20.0 if agc_max_gain is None else agc_max_gain,
                                 agc_gate_db=-50.0 if agc_gate is None else agc_gate,
                                 drift='auto' if drift is not None else drift_ppm,
-                                drift_max_ppm=drift if drift is not None else max(500.0, abs(drift_ppm or 0.0)))
+                                drift_max_ppm=drift if drift is not None else max(500.0, abs(drift_ppm or 0.0)),
+                                pitch_correct=pitch_correct)
     try:
         if pitch:
             pipeline.set_f0_map(semitones=pitch)
@@ -260,6 +282,13 @@ def make_parser() -> argparse.ArgumentParser:
                         help='follow the clock difference of the input and output sound cards: a controller trims the played stream '
                              'by up to MAX_PPM (default 500, at most 2000) from the output card\'s backlog, so a long session neither '
                              'underruns nor falls behind (live audio only)')
+    parser.add_argument('--autotune', type=str, default=None, metavar='KEY[:SCALE]',
+                        help='pull each converted note toward the nearest note of a scale on the GPU: KEY is a note name (C, F#, Bb) '
+                             'or 0-11, SCALE major (default), minor, chromatic or a 12-bit mask of pitch classes above the key')
+    parser.add_argument('--retune_ms', type=float, default=None, metavar='MS',
+                        help='with --autotune: how fast a note is pulled to the scale, in ms (0-1000, default 50; 0 snaps at once)')
+    parser.add_argument('--autotune_amount', type=float, default=None, metavar='A',
+                        help='with --autotune: the share of the correction applied (0-1, default 1)')
     parser.add_argument('--save_state', type=Path, default=None, metavar='OUT.state',
                         help='when the audio loop ends, write the stream state (learned noise profile, echo path, AGC level, f0 '
                              'statistics, settings) to this file for --load_state')
@@ -277,7 +306,8 @@ def main(argv: Optional[Iterable[str]] = None) -> None:
         save_noise_profile=args.save_noise_profile, echo_cancel=args.echo_cancel, echo_delay=args.echo_delay,
         echo_suppression=args.echo_suppression, limit=args.limit, limit_lookahead=args.limit_lookahead, limit_hold=args.limit_hold,
         agc=args.agc, agc_max_gain=args.agc_max_gain, agc_gate=args.agc_gate, save_state=args.save_state, load_state=args.load_state,
-        drift_ppm=args.drift_ppm, drift=args.drift)
+        drift_ppm=args.drift_ppm, drift=args.drift, autotune=args.autotune, retune_ms=args.retune_ms,
+        autotune_amount=args.autotune_amount)
 
 
 if __name__ == '__main__':

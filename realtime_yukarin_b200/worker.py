@@ -28,7 +28,7 @@ import numpy
 from .config import Config, VocodeMode
 from .drift import DriftController
 from .engine import (AGC_GATE_DB, AGC_MAX_GAIN_DB, AGC_TARGET_DB, DRIFT_MAX_PPM, LIMITER_CEILING_DB, LIMITER_HOLD_MS, LIMITER_LOOKAHEAD_MS,
-                     Engine, SessionConfig, default_engine)
+                     PITCH_A4_HZ, PITCH_RETUNE_MS, Engine, SessionConfig, default_engine, pitch_key, pitch_scale)
 from .wave_io import DRIFT_HALF_WIDTH
 
 
@@ -112,6 +112,29 @@ def _check_agc(target_db: float, max_gain_db: float, gate_db: float) -> None:
             raise ValueError(f'the AGC {name} must be within [{lo}, {hi}] dB')
 
 
+PITCH_CORRECT_KEYS = ('key', 'scale', 'a4_hz', 'retune_ms', 'amount')
+
+
+def pitch_settings(settings: dict) -> dict:
+    """pitch correction settings as Engine.session_set_pitch_correct accepts them (key as 0-11, scale as a mask), checked before a
+    session exists"""
+    unknown = set(settings) - set(PITCH_CORRECT_KEYS)
+    if unknown:
+        raise ValueError(f'unknown pitch correction settings {sorted(unknown)}: use {", ".join(PITCH_CORRECT_KEYS)}')
+    out = dict(key=0, scale='chromatic', a4_hz=440.0, retune_ms=50.0, amount=1.0)
+    out.update(settings)
+    out['key'], out['scale'] = pitch_key(out['key']), pitch_scale(out['scale'])
+    if not 0 <= out['key'] <= 11:
+        raise ValueError('the pitch correction key must be a pitch class within [0, 11]')
+    if not 1 <= out['scale'] <= 0xfff:
+        raise ValueError('the pitch correction scale must be a nonzero 12-bit mask')
+    for name, (lo, hi) in (('a4_hz', PITCH_A4_HZ), ('retune_ms', PITCH_RETUNE_MS), ('amount', (0.0, 1.0))):
+        out[name] = float(out[name])
+        if not lo <= out[name] <= hi:
+            raise ValueError(f'the pitch correction {name} must be within [{lo:g}, {hi:g}]')
+    return out
+
+
 def _check_drift(drift, max_ppm: float) -> None:
     """the drift stage's settings as Engine.drift_create / drift_set accept them, checked before a session exists"""
     if not (math.isfinite(max_ppm) and 0 < max_ppm <= DRIFT_MAX_PPM):
@@ -154,7 +177,11 @@ class RealtimePipeline(object):
     `update_drift` derives from the output card's backlog; |ppm| <= `drift_max_ppm` (at most 2000).  `process` then returns the stage's
     output for the chunk it would have played: float32, one or two samples more or less than out_audio_chunk, 16 samples later.  The
     echo canceller's far end stays the chunk before the stage: the microphone hears the played sound in the input card's clock, which
-    the nominal-rate stream is in.  `set_drift` fixes the trim, `drift_stats` reads it with the stage's totals."""
+    the nominal-rate stream is in.  `set_drift` fixes the trim, `drift_stats` reads it with the stage's totals.  `pitch_correct=dict(
+    key=, scale=, a4_hz=, retune_ms=, amount=)` pulls each converted note toward the nearest note of a scale on the device (DESIGN.md
+    §4m): key 0-11 or a note name ('C' when missing), scale a 12-bit mask or 'chromatic' (default) / 'major' / 'minor', a4_hz 400-480
+    (440), retune_ms 0-1000 (50; 0 is a hard snap) and amount 0-1 (1); no delay.  `set_pitch_correct` changes the settings between
+    chunks and `pitch_stats` reads how much the last chunk was corrected."""
 
     _drift: Optional[int] = None                        # the drift stage's id on the engine (None: no drift stage)
     _drift_ctl: Optional[DriftController] = None        # its controller in 'auto' mode
@@ -164,7 +191,10 @@ class RealtimePipeline(object):
                  noise_profile=None, learn_noise: Optional[float] = None, echo_cancel: bool = False, echo_taps: int = 32,
                  echo_delay_ms: float = 0.0, echo_suppression: float = 0.0, limiter: Optional[float] = None,
                  limiter_lookahead_ms: float = 5.0, limiter_hold_ms: float = 50.0, agc: Optional[float] = None,
-                 agc_max_gain_db: float = 20.0, agc_gate_db: float = -50.0, drift=None, drift_max_ppm: float = 500.0):
+                 agc_max_gain_db: float = 20.0, agc_gate_db: float = -50.0, drift=None, drift_max_ppm: float = 500.0,
+                 pitch_correct: Optional[dict] = None):
+        if pitch_correct is not None:
+            pitch_correct = pitch_settings(pitch_correct)
         if drift is not None:
             _check_drift(drift, float(drift_max_ppm))
         if agc is not None:
@@ -246,6 +276,9 @@ class RealtimePipeline(object):
             self.engine.session_set_limiter(self._sid, float(limiter), gain=float(config.output_scale))
         if agc is not None:
             self.engine.session_agc(self._sid, float(agc), float(agc_max_gain_db), float(agc_gate_db))
+        if pitch_correct is not None:
+            self.engine.session_pitch_correct(self._sid)
+            self.engine.session_set_pitch_correct(self._sid, **pitch_correct)
         if measure_f0 or follow_f0 is not None:
             self.engine.session_f0_measure(self._sid)
         if follow_f0 is not None:
@@ -314,6 +347,18 @@ class RealtimePipeline(object):
     def set_agc(self, target_db: Optional[float] = None, max_gain_db: Optional[float] = None, gate_db: Optional[float] = None) -> None:
         """Engine.session_set_agc for this stream: from the next chunk on; a None keeps that setting (needs agc)."""
         self.engine.session_set_agc(self._sid, target_db, max_gain_db, gate_db)
+
+    def set_pitch_correct(self, **settings) -> None:
+        """Engine.session_set_pitch_correct for this stream: key, scale, a4_hz, retune_ms and amount from the next chunk on; a missing
+        one keeps its setting (needs pitch_correct)."""
+        unknown = set(settings) - set(PITCH_CORRECT_KEYS)
+        if unknown:
+            raise ValueError(f'unknown pitch correction settings {sorted(unknown)}: use {", ".join(PITCH_CORRECT_KEYS)}')
+        self.engine.session_set_pitch_correct(self._sid, **settings)
+
+    def pitch_stats(self) -> Tuple[int, float, float]:
+        """(voiced frames, mean and largest correction in cents) of the last chunk put (needs pitch_correct)."""
+        return self.engine.session_pitch_stats(self._sid)
 
     def agc_stats(self) -> Tuple[float, float, int]:
         """(level in dB, -inf before any active block; gain in dB; active blocks of the last chunk) of the chunks put (needs agc)."""
