@@ -139,26 +139,22 @@ int ryk_agc(ryk_engine* h, const float* x, int n, int fs, double target_db, doub
   RYK_CHECK(x && z && n > 0, "null argument or empty signal");
   RYK_CHECK(fs > 0, "fs must be positive");
   if (int rc = agc_check(target_db, max_gain_db, gate_db)) return rc;
-  auto align = [](size_t b) { return (b + 255) / 256 * 256; };
-  const size_t b_par = align(sizeof(AgcParams)), b_meter = align(sizeof(AgcMeter)), b_st = align(sizeof(AgcState));
-  const size_t b_x = align(sizeof(float) * n);
-  void* buf = nullptr;
-  if (engine_scratch(e, b_par + b_meter + 2 * b_st + 2 * b_x, &buf)) return -1;
-  char* p = (char*)buf;
   AgcWork w;
-  w.params = (AgcParams*)p; p += b_par;
-  w.meter = (AgcMeter*)p; p += b_meter;
   AgcState* st[2];
-  st[0] = (AgcState*)p; p += b_st;
-  st[1] = (AgcState*)p; p += b_st;
-  float* d_x = (float*)p; p += b_x;
-  float* d_z = (float*)p;
+  float *d_x, *d_z;
+  if (engine_scratch(e, [&](Arena& a) {
+        w.params = a.take<AgcParams>(1);
+        w.meter = a.take<AgcMeter>(1);
+        st[0] = a.take<AgcState>(1);
+        st[1] = a.take<AgcState>(1);
+        d_x = a.take<float>(n);
+        d_z = a.take<float>(n);
+      })) return -1;
   // host staging: the settings, a fresh state and x
-  void* hp = nullptr;
-  if (engine_pinned(e, sizeof(AgcParams) + sizeof(AgcState) + sizeof(float) * n, &hp)) return -1;
-  AgcParams* h_par = (AgcParams*)hp;
-  AgcState* h_st = (AgcState*)(h_par + 1);
-  float* h_x = (float*)(h_st + 1);
+  AgcParams* h_par;
+  AgcState* h_st;
+  float* h_x;
+  if (engine_pinned_layout(e, [&](Arena& a) { h_par = a.take<AgcParams>(1); h_st = a.take<AgcState>(1); h_x = a.take<float>(n); })) return -1;
   *h_par = agc_params(fs, target_db, max_gain_db, gate_db);
   agc_state_init(h_st);
   memcpy(h_x, x, sizeof(float) * n);

@@ -27,7 +27,7 @@ void fft_fill_twiddles(double2* t) {
   for (int k = 0; k < kTwiddleN / 2; ++k) t[k] = make_double2(cos(2.0 * kPi * k / kTwiddleN), -sin(2.0 * kPi * k / kTwiddleN));
 }
 
-int engine_scratch(Engine* e, size_t bytes, void** out) {
+static int device_scratch(Engine* e, size_t bytes, void** out) {
   if (bytes > e->scratch_bytes) {
     RYK_CUDA(cudaStreamSynchronize(e->stream));
     if (e->d_scratch) RYK_CUDA(cudaFree(e->d_scratch));
@@ -51,21 +51,17 @@ int engine_pinned(Engine* e, size_t bytes, void** out) {
   return 0;
 }
 
-struct Arena {
-  char* base; size_t off = 0;
-  explicit Arena(void* b) : base((char*)b) {}
-  template <typename T> T* take(size_t count) {
-    off = (off + 255) & ~(size_t)255;
-    T* p = (T*)(base + off);
-    off += count * sizeof(T);
-    return p;
-  }
-};
-static size_t arena_need(std::initializer_list<size_t> sizes) {
-  size_t t = 0;
-  for (size_t s : sizes) t = ((t + 255) & ~(size_t)255) + s;
-  return t + 256;
+static int layout(Engine* e, const std::function<void(Arena&)>& carve, int (*buffer)(Engine*, size_t, void**)) {
+  Arena size(nullptr);
+  carve(size);
+  void* base = nullptr;
+  if (buffer(e, size.off, &base)) return -1;
+  Arena a(base);
+  carve(a);
+  return 0;
 }
+int engine_scratch(Engine* e, const std::function<void(Arena&)>& carve) { return layout(e, carve, device_scratch); }
+int engine_pinned_layout(Engine* e, const std::function<void(Arena&)>& carve) { return layout(e, carve, engine_pinned); }
 
 int dio_get_plan(Engine* e, int n, int fs, double frame_period, double f0_floor, double f0_ceil, DioPlan** out) {
   // the f0 method is part of the key: switching it never reuses a plan built for the other extractor
@@ -305,9 +301,8 @@ int ryk_world_f0(ryk_engine* h, const float* wave, int n, int fs, double fp, dou
   RYK_CHECK(e->f0_method != 2, "f0 method 2 (CREPE) runs in sessions only: use the CREPE front-end (ryk_crepe_predict) for a single signal");
   DioPlan* plan = nullptr;
   if (dio_get_plan(e, n, fs, fp, f0_floor, f0_ceil, &plan)) return -1;
-  void* scratch = nullptr;
-  if (engine_scratch(e, sizeof(float) * n + 256, &scratch)) return -1;
-  float* d_x = (float*)scratch;
+  float* d_x;
+  if (engine_scratch(e, [&](Arena& a) { d_x = a.take<float>(n); })) return -1;
   RYK_CUDA(cudaMemcpyAsync(d_x, wave, sizeof(float) * n, cudaMemcpyHostToDevice, e->stream));
   if (dio_stonemask_run(e, plan, d_x, e->stream)) return -1;
   int nf = dio_plan_frames(plan);
@@ -331,17 +326,16 @@ int ryk_world_analyze(ryk_engine* h, const float* wave, int n, int fs, double fp
   if (sptk_prepare(e, order, alpha, fft_length, &mats)) return -1;
   DioPlan* plan = nullptr;
   if (dio_get_plan(e, n, fs, fp, f0_floor, f0_ceil, &plan)) return -1;
-  void* scratch = nullptr;
-  size_t need = arena_need({sizeof(float) * n, sizeof(float) * n_out, sizeof(float) * n_out * nb, sizeof(float) * n_out * nb,
-                            sizeof(float) * n_out * (order + 1), (size_t)n_out});
-  if (engine_scratch(e, need, &scratch)) return -1;
-  Arena A(scratch);
-  float* d_x = A.take<float>(n);
-  float* d_f0 = A.take<float>(n_out);
-  float* d_sp = A.take<float>((size_t)n_out * nb);
-  float* d_ap = A.take<float>((size_t)n_out * nb);
-  float* d_mc = A.take<float>((size_t)n_out * (order + 1));
-  uint8_t* d_v = A.take<uint8_t>(n_out);
+  float *d_x, *d_f0, *d_sp, *d_ap, *d_mc;
+  uint8_t* d_v;
+  if (engine_scratch(e, [&](Arena& a) {
+        d_x = a.take<float>(n);
+        d_f0 = a.take<float>(n_out);
+        d_sp = a.take<float>((size_t)n_out * nb);
+        d_ap = a.take<float>((size_t)n_out * nb);
+        d_mc = a.take<float>((size_t)n_out * (order + 1));
+        d_v = a.take<uint8_t>(n_out);
+      })) return -1;
   RYK_CUDA(cudaMemcpyAsync(d_x, wave, sizeof(float) * n, cudaMemcpyHostToDevice, e->stream));
   if (f0_override) {
     RYK_CUDA(cudaMemcpyAsync(dio_plan_f0_mut(plan), f0_override, sizeof(double) * dio_plan_frames(plan), cudaMemcpyHostToDevice, e->stream));
@@ -363,15 +357,17 @@ int ryk_silence_mask(ryk_engine* h, const float* wave, int n, int frame_length, 
   Engine* e = E(h);
   RYK_CUDA(cudaSetDevice(e->device));
   if (n_frames <= 0) return 0;
-  void* scratch = nullptr;
-  size_t need = arena_need({sizeof(float) * (size_t)(n > 0 ? n : 1), sizeof(double) * n_frames, (size_t)n_frames, sizeof(int) * n_frames, sizeof(int) * 2});
-  if (engine_scratch(e, need, &scratch)) return -1;
-  Arena A(scratch);
-  float* d_x = A.take<float>(n > 0 ? n : 1);
-  double* d_mse = A.take<double>(n_frames);
-  uint8_t* d_mask = A.take<uint8_t>(n_frames);
-  int* d_index = A.take<int>(n_frames);
-  int* d_count = A.take<int>(2);
+  float* d_x;
+  double* d_mse;
+  uint8_t* d_mask;
+  int *d_index, *d_count;
+  if (engine_scratch(e, [&](Arena& a) {
+        d_x = a.take<float>(n > 0 ? n : 1);
+        d_mse = a.take<double>(n_frames);
+        d_mask = a.take<uint8_t>(n_frames);
+        d_index = a.take<int>(n_frames);
+        d_count = a.take<int>(2);
+      })) return -1;
   if (n > 0) RYK_CUDA(cudaMemcpyAsync(d_x, wave, sizeof(float) * n, cudaMemcpyHostToDevice, e->stream));
   if (gate_mask_run(e, d_x, n, frame_length, hop, threshold_db, n_frames, d_mse, d_mask, d_index, d_count, e->stream)) return -1;
   RYK_CUDA(cudaMemcpyAsync(mask, d_mask, n_frames, cudaMemcpyDeviceToHost, e->stream));
@@ -472,12 +468,13 @@ int ryk_stage1_convert(ryk_engine* h, const float* x, int T, float* y) {
   const int Tp = T + (128 - T % 128);
   UNetPlan* plan = nullptr;
   if (stage1_plan_for(e, Tp, &plan)) return -1;
-  void* scratch = nullptr;
-  if (engine_scratch(e, arena_need({sizeof(float) * T * C, sizeof(float) * T * Co, sizeof(int) * 2}), &scratch)) return -1;
-  Arena A(scratch);
-  float* d_x = A.take<float>((size_t)T * C);
-  float* d_y = A.take<float>((size_t)T * Co);
-  int* d_count = A.take<int>(2);
+  float *d_x, *d_y;
+  int* d_count;
+  if (engine_scratch(e, [&](Arena& a) {
+        d_x = a.take<float>((size_t)T * C);
+        d_y = a.take<float>((size_t)T * Co);
+        d_count = a.take<int>(2);
+      })) return -1;
   int cnt[2] = {T, Tp};
   RYK_CUDA(cudaMemcpyAsync(d_x, x, sizeof(float) * T * C, cudaMemcpyHostToDevice, e->stream));
   RYK_CUDA(cudaMemcpyAsync(d_count, cnt, sizeof(cnt), cudaMemcpyHostToDevice, e->stream));
@@ -493,10 +490,9 @@ int ryk_f0_convert(ryk_engine* h, const float* f0, const uint8_t* voiced, int T,
   Engine* e = E(h);
   RYK_CUDA(cudaSetDevice(e->device));
   if (T <= 0) return 0;
-  void* scratch = nullptr;
-  if (engine_scratch(e, arena_need({sizeof(float) * T, (size_t)T, sizeof(float) * T}), &scratch)) return -1;
-  Arena A(scratch);
-  float* d_f0 = A.take<float>(T); uint8_t* d_v = A.take<uint8_t>(T); float* d_o = A.take<float>(T);
+  float *d_f0, *d_o;
+  uint8_t* d_v;
+  if (engine_scratch(e, [&](Arena& a) { d_f0 = a.take<float>(T); d_v = a.take<uint8_t>(T); d_o = a.take<float>(T); })) return -1;
   RYK_CUDA(cudaMemcpyAsync(d_f0, f0, sizeof(float) * T, cudaMemcpyHostToDevice, e->stream));
   RYK_CUDA(cudaMemcpyAsync(d_v, voiced, T, cudaMemcpyHostToDevice, e->stream));
   const Voice* v = e->voices[0];
@@ -514,11 +510,9 @@ int ryk_mc2sp(ryk_engine* h, const float* mc, int T, int order, double alpha, in
   SptkMats mats;
   if (sptk_prepare(e, order, alpha, fftlen, &mats)) return -1;
   int nb = fftlen / 2 + 1;
-  void* scratch = nullptr;
-  if (engine_scratch(e, arena_need({sizeof(float) * T * (order + 1), sizeof(double) * T * nb}), &scratch)) return -1;
-  Arena A(scratch);
-  float* d_mc = A.take<float>((size_t)T * (order + 1));
-  double* d_sp = A.take<double>((size_t)T * nb);
+  float* d_mc;
+  double* d_sp;
+  if (engine_scratch(e, [&](Arena& a) { d_mc = a.take<float>((size_t)T * (order + 1)); d_sp = a.take<double>((size_t)T * nb); })) return -1;
   RYK_CUDA(cudaMemcpyAsync(d_mc, mc, sizeof(float) * T * (order + 1), cudaMemcpyHostToDevice, e->stream));
   if (mc2sp_run(e, mats.d_H, d_mc, T, order, fftlen, 0.0, nullptr, d_sp, e->stream)) return -1;
   RYK_CUDA(cudaMemcpyAsync(sp, d_sp, sizeof(double) * T * nb, cudaMemcpyDeviceToHost, e->stream));
@@ -535,11 +529,8 @@ static int stage2_convert(ryk_engine* h, const float* sp, int T, double formant,
   const int Tp = T + (128 - T % 128);
   UNetPlan* plan = nullptr;
   if (stage2_plan_for(e, Tp, &plan)) return -1;
-  void* scratch = nullptr;
-  if (engine_scratch(e, arena_need({sizeof(float) * T * nb, sizeof(float) * T * nb}), &scratch)) return -1;
-  Arena A(scratch);
-  float* d_sp = A.take<float>((size_t)T * nb);
-  float* d_out = A.take<float>((size_t)T * nb);
+  float *d_sp, *d_out;
+  if (engine_scratch(e, [&](Arena& a) { d_sp = a.take<float>((size_t)T * nb); d_out = a.take<float>((size_t)T * nb); })) return -1;
   RYK_CUDA(cudaMemcpyAsync(d_sp, sp, sizeof(float) * T * nb, cudaMemcpyHostToDevice, e->stream));
   if (sr_prologue_run(e, d_sp, T, Tp, nb, (float*)plan->d_in, e->stream)) return -1;
   if (unet_forward(e, plan, e->stream)) return -1;
@@ -614,12 +605,10 @@ int ryk_synth_destroy(ryk_engine* h, int id) {
 static int synth_upload(Engine* e, Synth* s, const double* f0, int n, const float* sp, const float* ap, double** d_f0, float** d_sp, float** d_ap,
                         double** d_out, int max_blocks) {
   int nb = s->dev.fft_size / 2 + 1;
-  void* scratch = nullptr;
-  size_t need = arena_need({sizeof(double) * n, sizeof(float) * n * nb, sizeof(float) * n * nb, sizeof(double) * (size_t)max_blocks * s->dev.buffer_size});
-  if (engine_scratch(e, need, &scratch)) return -1;
-  Arena A(scratch);
-  *d_f0 = A.take<double>(n); *d_sp = A.take<float>((size_t)n * nb); *d_ap = A.take<float>((size_t)n * nb);
-  *d_out = A.take<double>((size_t)max_blocks * s->dev.buffer_size);
+  if (engine_scratch(e, [&](Arena& a) {
+        *d_f0 = a.take<double>(n); *d_sp = a.take<float>((size_t)n * nb); *d_ap = a.take<float>((size_t)n * nb);
+        *d_out = a.take<double>((size_t)max_blocks * s->dev.buffer_size);
+      })) return -1;
   if (n > 0) {
     RYK_CUDA(cudaMemcpyAsync(*d_f0, f0, sizeof(double) * n, cudaMemcpyHostToDevice, e->stream));
     RYK_CUDA(cudaMemcpyAsync(*d_sp, sp, sizeof(float) * n * nb, cudaMemcpyHostToDevice, e->stream));
@@ -650,9 +639,8 @@ int ryk_synth_synthesis2(ryk_engine* h, int id, double* buffer) {
   RYK_CUDA(cudaSetDevice(e->device));
   Synth* s = get_synth(e, id);
   RYK_CHECK(s != nullptr, "no such synthesizer");
-  void* scratch = nullptr;
-  if (engine_scratch(e, sizeof(double) * s->dev.buffer_size + 256, &scratch)) return -1;
-  double* d_out = (double*)scratch;
+  double* d_out;
+  if (engine_scratch(e, [&](Arena& a) { d_out = a.take<double>(s->dev.buffer_size); })) return -1;
   if (synth_drain_async(e, s, d_out, 1, e->stream)) return -1;
   int blocks = 0;
   RYK_CUDA(cudaMemcpyAsync(&blocks, (char*)s->dev.state + offsetof(SynthState, blocks_out), sizeof(int), cudaMemcpyDeviceToHost, e->stream));
@@ -708,12 +696,11 @@ int ryk_output_gate(ryk_engine* h, const double* wave, int n, int n_fft, int hop
   RYK_CUDA(cudaSetDevice(e->device));
   RYK_CHECK(wave != nullptr && n > 0, "empty chunk");
   const size_t scratch = output_gate_scratch_doubles(n, n_fft, hop);
-  void* buf = nullptr;
-  if (engine_scratch(e, sizeof(double) * (n + scratch + 2) + 64, &buf)) return -1;
-  double* d_wave = (double*)buf;
-  double* d_scr = d_wave + n;
-  double* d_power = d_scr + scratch;
-  int* d_status = (int*)(d_power + 1);
+  double *d_wave, *d_scr, *d_power;
+  int* d_status;
+  if (engine_scratch(e, [&](Arena& a) {
+        d_wave = a.take<double>(n); d_scr = a.take<double>(scratch); d_power = a.take<double>(1); d_status = a.take<int>(1);
+      })) return -1;
   RYK_CUDA(cudaMemcpyAsync(d_wave, wave, sizeof(double) * n, cudaMemcpyHostToDevice, e->stream));
   if (output_gate_async(e, d_wave, nullptr, n, n_fft, hop, threshold_db, d_scr, d_power, d_status, e->stream)) return -1;
   double pw = 0.0; int st = 0;
@@ -738,10 +725,9 @@ int ryk_resample_poly(ryk_engine* h, const float* x, int n, int up, int down, co
   RYK_CHECK(x && taps && y && n > 0 && up > 0 && down > 0 && n_taps > 0 && (n_taps & 1), "bad resampler arguments (the filter must have an odd number of taps)");
   const int no = ryk_resample_length(n, up, down);
   RYK_CHECK(no <= y_capacity, "output buffer too small: ryk_resample_length samples are written");
-  void* buf = nullptr;
-  const size_t bx = ((sizeof(float) * (size_t)n + 255) / 256) * 256, bh = ((sizeof(double) * (size_t)n_taps + 255) / 256) * 256;
-  if (engine_scratch(e, bx + bh + sizeof(float) * (size_t)no + 256, &buf)) return -1;
-  float* d_x = (float*)buf; double* d_h = (double*)((char*)buf + bx); float* d_y = (float*)((char*)buf + bx + bh);
+  float *d_x, *d_y;
+  double* d_h;
+  if (engine_scratch(e, [&](Arena& a) { d_x = a.take<float>(n); d_h = a.take<double>(n_taps); d_y = a.take<float>(no); })) return -1;
   RYK_CUDA(cudaMemcpyAsync(d_x, x, sizeof(float) * n, cudaMemcpyHostToDevice, e->stream));
   RYK_CUDA(cudaMemcpyAsync(d_h, taps, sizeof(double) * n_taps, cudaMemcpyHostToDevice, e->stream));
   if (resample_poly_run(e, d_x, n, up, down, d_h, n_taps, d_y, no, e->stream)) return -1;

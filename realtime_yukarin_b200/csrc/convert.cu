@@ -9,21 +9,14 @@
 namespace ryk {
 
 int convert_buffers_get(Engine* e, int T, int n_wave, int nb, int C, ConvertBuffers* cb) {
-  size_t sizes[] = {sizeof(float) * (size_t)n_wave, sizeof(float) * T, sizeof(float) * (size_t)T * nb, sizeof(float) * (size_t)T * C, (size_t)T,
-                    sizeof(double) * T, (size_t)T, sizeof(int) * T, sizeof(int) * 2,
-                    sizeof(float) * (size_t)T * C, sizeof(float) * T, sizeof(float) * (size_t)T * nb, sizeof(float) * (size_t)T * nb,
-                    sizeof(float) * (size_t)T * nb, (size_t)T};
-  size_t total = 0;
-  for (size_t s : sizes) total = ((total + 255) & ~(size_t)255) + s;
-  void* base = nullptr;
-  if (engine_scratch(e, total + 512, &base)) return -1;
-  char* p = (char*)base; size_t off = 0; int i = 0;
-  auto take = [&]() { off = (off + 255) & ~(size_t)255; void* r = p + off; off += sizes[i++]; return r; };
-  cb->d_wave = (float*)take(); cb->d_f0 = (float*)take(); cb->d_ap = (float*)take(); cb->d_mc = (float*)take(); cb->d_voiced = (uint8_t*)take();
-  cb->d_mse = (double*)take(); cb->d_mask = (uint8_t*)take(); cb->d_index = (int*)take(); cb->d_count = (int*)take();
-  cb->d_mc_out = (float*)take(); cb->d_f0_out = (float*)take(); cb->d_ap_out = (float*)take(); cb->d_sp_mid = (float*)take();
-  cb->d_sp_out = (float*)take(); cb->d_voiced_out = (uint8_t*)take();
-  return 0;
+  const size_t TC = (size_t)T * C, Tnb = (size_t)T * nb;
+  return engine_scratch(e, [&](Arena& a) {
+    cb->d_wave = a.take<float>(n_wave); cb->d_f0 = a.take<float>(T); cb->d_ap = a.take<float>(Tnb); cb->d_mc = a.take<float>(TC);
+    cb->d_voiced = a.take<uint8_t>(T);
+    cb->d_mse = a.take<double>(T); cb->d_mask = a.take<uint8_t>(T); cb->d_index = a.take<int>(T); cb->d_count = a.take<int>(2);
+    cb->d_mc_out = a.take<float>(TC); cb->d_f0_out = a.take<float>(T); cb->d_ap_out = a.take<float>(Tnb); cb->d_sp_mid = a.take<float>(Tnb);
+    cb->d_sp_out = a.take<float>(Tnb); cb->d_voiced_out = a.take<uint8_t>(T);
+  });
 }
 
 int convert_window_device(Engine* e, const ConvertBuffers& cb, int T, int n_wave, int frame_length, int hop, double threshold_db,

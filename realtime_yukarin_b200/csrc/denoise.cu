@@ -187,28 +187,25 @@ int ryk_denoise(ryk_engine* h, const float* x, int n, double reduction_db, const
   const int len = n + kDnDelay;
   DenoiseWork w;
   w.max_frames = denoise_max_frames(len);
-  auto align = [](size_t b) { return (b + 255) / 256 * 256; };
-  const size_t b_par = align(sizeof(DenoiseParams)), b_learn = align(sizeof(DenoiseLearn)), b_st = align(sizeof(DenoiseState));
-  const size_t b_spec = align(sizeof(double2) * kDnBins * w.max_frames), b_frames = align(sizeof(double) * kDnN * w.max_frames);
-  const size_t b_x = align(sizeof(float) * len);
-  void* buf = nullptr;
-  if (engine_scratch(e, b_par + b_learn + 2 * b_st + b_spec + b_frames + 2 * b_x + 256, &buf)) return -1;
-  char* p = (char*)buf;
-  w.params = (DenoiseParams*)p; p += b_par;
-  w.learn = (DenoiseLearn*)p; p += b_learn;
-  DenoiseState* st = (DenoiseState*)p; p += b_st;
-  DenoiseState* st_next = (DenoiseState*)p; p += b_st;
-  w.spec = (double2*)p; p += b_spec;
-  w.frames = (double*)p; p += b_frames;
-  float* d_x = (float*)p; p += b_x;
-  float* d_z = (float*)p; p += b_x;
-  w.done = (unsigned*)p;
+  DenoiseState *st, *st_next;
+  float *d_x, *d_z;
+  if (engine_scratch(e, [&](Arena& a) {
+        w.params = a.take<DenoiseParams>(1);
+        w.learn = a.take<DenoiseLearn>(1);
+        st = a.take<DenoiseState>(1);
+        st_next = a.take<DenoiseState>(1);
+        w.spec = a.take<double2>((size_t)kDnBins * w.max_frames);
+        w.frames = a.take<double>((size_t)kDnN * w.max_frames);
+        d_x = a.take<float>(len);
+        d_z = a.take<float>(len);
+        w.done = a.take<unsigned>(1);
+      })) return -1;
   // host staging: the parameter block (a profile set, no learning), the fresh state and x followed by zeros
-  void* hp = nullptr;
-  if (engine_pinned(e, sizeof(DenoiseParams) + sizeof(DenoiseState) + sizeof(float) * len, &hp)) return -1;
-  DenoiseParams* h_par = (DenoiseParams*)hp;
-  DenoiseState* h_st = (DenoiseState*)(h_par + 1);
-  float* h_x = (float*)(h_st + 1);
+  DenoiseParams* h_par;
+  DenoiseState* h_st;
+  float* h_x;
+  if (engine_pinned_layout(e, [&](Arena& a) { h_par = a.take<DenoiseParams>(1); h_st = a.take<DenoiseState>(1); h_x = a.take<float>(len); }))
+    return -1;
   memset(h_par, 0, sizeof(DenoiseParams));
   h_par->gain_floor = pow(10.0, -reduction_db / 20.0);
   h_par->profile_serial = 1;

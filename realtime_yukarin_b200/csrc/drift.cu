@@ -226,28 +226,30 @@ int ryk_drift_resample(ryk_engine* h, const double* x, int n, double ppm, const 
   const long long cap = drift_capacity(len, fabs(ppm));
   RYK_CHECK(y_capacity >= cap, "the output buffer must hold len + ceil(len |ppm| 1e-6) + 2 samples, len = n + 16");
   RYK_CUDA(cudaSetDevice(e->device));
-  auto align = [](size_t b) { return (b + 255) / 256 * 256; };
-  const size_t b_st = align(2 * sizeof(DriftState)), b_hist = align(2 * kDriftTaps * sizeof(double));
-  const size_t b_table = align(sizeof(double) * kDriftTable), b_x = align(sizeof(double) * len), b_y = align(sizeof(double) * cap);
-  void* buf = nullptr;
-  if (engine_scratch(e, b_st + b_hist + b_table + b_x + b_y, &buf)) return -1;
-  char* p = (char*)buf;
-  DriftState* d_st = (DriftState*)p; p += b_st;
-  double* d_hist = (double*)p; p += b_hist;
-  double* d_table = (double*)p; p += b_table;
-  double* d_x = (double*)p; p += b_x;
-  double* d_y = (double*)p;
-  void* hp = nullptr;
-  if (engine_pinned(e, sizeof(double) * (kDriftTable + len + cap) + sizeof(DriftState), &hp)) return -1;
-  double* h_table = (double*)hp;
-  double* h_x = h_table + kDriftTable;
-  double* h_y = h_x + len;
-  DriftState* h_st = (DriftState*)(h_y + cap);
+  DriftState* d_st;
+  double *d_hist, *d_table, *d_x, *d_y;
+  if (engine_scratch(e, [&](Arena& a) {
+        d_st = a.take<DriftState>(2);
+        d_hist = a.take<double>(2 * kDriftTaps);
+        d_table = a.take<double>(kDriftTable);
+        d_x = a.take<double>(len);
+        d_y = a.take<double>(cap);
+      })) return -1;
+  double *h_table, *h_x, *h_y;
+  DriftState* h_st;
+  if (engine_pinned_layout(e, [&](Arena& a) {
+        h_table = a.take<double>(kDriftTable);
+        h_x = a.take<double>(len);
+        h_y = a.take<double>(cap);
+        h_st = a.take<DriftState>(1);
+      })) return -1;
   memcpy(h_table, table, sizeof(double) * kDriftTable);
   memcpy(h_x, x, sizeof(double) * n);
   memset(h_x + n, 0, sizeof(double) * kDriftHalfWidth);
   cudaStream_t st = e->stream;
-  RYK_CUDA(cudaMemsetAsync(d_st, 0, b_st + b_hist, st));          // a fresh state: position 0, zeros before the signal
+  // a fresh state: position 0, zeros before the signal
+  RYK_CUDA(cudaMemsetAsync(d_st, 0, 2 * sizeof(DriftState), st));
+  RYK_CUDA(cudaMemsetAsync(d_hist, 0, 2 * kDriftTaps * sizeof(double), st));
   RYK_CUDA(cudaMemcpyAsync(d_table, h_table, sizeof(double) * kDriftTable, cudaMemcpyHostToDevice, st));
   RYK_CUDA(cudaMemcpyAsync(d_x, h_x, sizeof(double) * len, cudaMemcpyHostToDevice, st));
   if (drift_launch(d_st, d_st + 1, d_hist, d_hist + kDriftTaps, d_x, len, drift_inc(ppm), d_table, d_y, cap, st)) return -1;
@@ -277,10 +279,9 @@ int ryk_drift_snapshot(ryk_engine* h, int id, void* buf, size_t bytes) {
   RYK_CHECK(bytes == drift_blob_size(), "the buffer must be exactly ryk_drift_snapshot_size bytes");
   RYK_CUDA(cudaSetDevice(e->device));
   const int p = (int)(D->pushed & 1);
-  void* hp = nullptr;
-  if (engine_pinned(e, sizeof(DriftState) + sizeof(double) * kDriftTaps, &hp)) return -1;
-  DriftState* st = (DriftState*)hp;
-  double* hist = (double*)(st + 1);
+  DriftState* st;
+  double* hist;
+  if (engine_pinned_layout(e, [&](Arena& a) { st = a.take<DriftState>(1); hist = a.take<double>(kDriftTaps); })) return -1;
   RYK_CUDA(cudaMemcpyAsync(st, D->d_state + p, sizeof(DriftState), cudaMemcpyDeviceToHost, e->stream));
   RYK_CUDA(cudaMemcpyAsync(hist, D->d_hist[p], sizeof(double) * kDriftTaps, cudaMemcpyDeviceToHost, e->stream));
   RYK_CUDA(cudaStreamSynchronize(e->stream));

@@ -129,38 +129,38 @@ int ryk_echo_cancel(ryk_engine* h, const float* mic, const float* far, int n, in
   EchoWork a;
   w.max_frames = denoise_max_frames(len);
   a.taps = taps; a.delay = delay_frames;
-  auto align = [](size_t b) { return (b + 255) / 256 * 256; };
-  const size_t b_par = align(sizeof(DenoiseParams)), b_learn = align(sizeof(DenoiseLearn)), b_st = align(sizeof(DenoiseState));
-  const size_t b_spec = align(sizeof(double2) * kDnBins * w.max_frames), b_frames = align(sizeof(double) * kDnN * w.max_frames);
-  const size_t b_x = align(sizeof(float) * len), b_epar = align(sizeof(EchoParams)), b_flt = align(sizeof(EchoFilter));
-  const size_t b_ring = align(sizeof(double2) * kDnBins * (taps + delay_frames));
-  void* buf = nullptr;
-  if (engine_scratch(e, b_par + b_learn + 4 * b_st + 2 * b_spec + b_frames + 3 * b_x + b_epar + b_flt + b_ring + 256, &buf)) return -1;
-  char* p = (char*)buf;
-  w.params = (DenoiseParams*)p; p += b_par;
-  w.learn = (DenoiseLearn*)p; p += b_learn;
-  DenoiseState* st = (DenoiseState*)p; p += b_st;
-  DenoiseState* st_next = (DenoiseState*)p; p += b_st;
-  DenoiseState* fst = (DenoiseState*)p; p += b_st;
-  DenoiseState* fst_next = (DenoiseState*)p; p += b_st;
-  w.spec = (double2*)p; p += b_spec;
-  a.far_spec = (double2*)p; p += b_spec;
-  w.frames = (double*)p; p += b_frames;
-  float* d_mic = (float*)p; p += b_x;
-  float* d_far = (float*)p; p += b_x;
-  float* d_z = (float*)p; p += b_x;
-  a.params = (EchoParams*)p; p += b_epar;
-  a.filter = (EchoFilter*)p; p += b_flt;
-  a.ring = (double2*)p; p += b_ring;
-  w.done = (unsigned*)p;
+  DenoiseState *st, *st_next, *fst, *fst_next;
+  float *d_mic, *d_far, *d_z;
+  if (engine_scratch(e, [&](Arena& ar) {
+        w.params = ar.take<DenoiseParams>(1);
+        w.learn = ar.take<DenoiseLearn>(1);
+        st = ar.take<DenoiseState>(1);
+        st_next = ar.take<DenoiseState>(1);
+        fst = ar.take<DenoiseState>(1);
+        fst_next = ar.take<DenoiseState>(1);
+        w.spec = ar.take<double2>((size_t)kDnBins * w.max_frames);
+        a.far_spec = ar.take<double2>((size_t)kDnBins * w.max_frames);
+        w.frames = ar.take<double>((size_t)kDnN * w.max_frames);
+        d_mic = ar.take<float>(len);
+        d_far = ar.take<float>(len);
+        d_z = ar.take<float>(len);
+        a.params = ar.take<EchoParams>(1);
+        a.filter = ar.take<EchoFilter>(1);
+        a.ring = ar.take<double2>((size_t)kDnBins * (taps + delay_frames));
+        w.done = ar.take<unsigned>(1);
+      })) return -1;
   // host staging: both parameter blocks, the fresh state, and mic / far followed by zeros
-  void* hp = nullptr;
-  if (engine_pinned(e, sizeof(DenoiseParams) + sizeof(DenoiseState) + sizeof(EchoParams) + 2 * sizeof(float) * len, &hp)) return -1;
-  DenoiseParams* h_par = (DenoiseParams*)hp;
-  DenoiseState* h_st = (DenoiseState*)(h_par + 1);
-  EchoParams* h_epar = (EchoParams*)(h_st + 1);
-  float* h_mic = (float*)(h_epar + 1);
-  float* h_far = h_mic + len;
+  DenoiseParams* h_par;
+  DenoiseState* h_st;
+  EchoParams* h_epar;
+  float *h_mic, *h_far;
+  if (engine_pinned_layout(e, [&](Arena& ar) {
+        h_par = ar.take<DenoiseParams>(1);
+        h_st = ar.take<DenoiseState>(1);
+        h_epar = ar.take<EchoParams>(1);
+        h_mic = ar.take<float>(len);
+        h_far = ar.take<float>(len);
+      })) return -1;
   memset(h_par, 0, sizeof(DenoiseParams));
   h_par->gain_floor = pow(10.0, -reduction_db / 20.0);
   h_par->profile_serial = 1;

@@ -2,6 +2,7 @@
 #pragma once
 #include <string.h>
 #include <algorithm>
+#include <functional>
 #include <map>
 #include <memory>
 #include <string>
@@ -108,13 +109,31 @@ struct Engine {
   double snap_device_ms = 0.0, snap_host_ms = 0.0;
 };
 
-int engine_scratch(Engine* e, size_t bytes, void** out);
+// The sub-buffers of one engine buffer, each at the next 256-byte boundary in the order they are taken.  Over a null base it only adds
+// up the size.
+struct Arena {
+  char* base;
+  size_t off = 0;
+  explicit Arena(void* b) : base((char*)b) {}
+  template <typename T> T* take(size_t count) {
+    off = (off + 255) & ~(size_t)255;
+    T* p = base ? (T*)(base + off) : nullptr;
+    off += count * sizeof(T);
+    return p;
+  }
+};
+// Lay out the device scratch (engine_scratch) or the pinned staging (engine_pinned_layout) of a call: `carve` runs over a null arena,
+// which adds up the size, then over the buffer grown to that size.  It runs twice, so it may only take buffers.  Both buffers are the
+// engine's, reused by the next call: a call is done with them when it returns.
+int engine_scratch(Engine* e, const std::function<void(Arena&)>& carve);
+int engine_pinned_layout(Engine* e, const std::function<void(Arena&)>& carve);
+// the pinned staging as one block of `bytes`
+int engine_pinned(Engine* e, size_t bytes, void** out);
 inline Voice* engine_voice(Engine* e, int id) { return id >= 0 && id < (int)e->voices.size() ? e->voices[id] : nullptr; }
 // identity stage-1 statistics of C channels unless statistics of C channels are loaded
 int voice_default_stage1_stats(Voice* v, int C);
 // both U-Nets created and every layer loaded
 bool voice_models_loaded(const Voice* v);
-int engine_pinned(Engine* e, size_t bytes, void** out);
 
 // world_analysis.cu
 int analysis_kernels_init();

@@ -172,38 +172,30 @@ int ryk_limit(ryk_engine* h, const double* y, int n, int rate, double lookahead_
   w.max_n = len;
   size_t n_g0, n_t32, n_t1k, n_m;
   limiter_scratch_sizes(w, &n_g0, &n_t32, &n_t1k, &n_m);
-  auto align = [](size_t b) { return (b + 255) / 256 * 256; };
-  const size_t b_par = align(sizeof(LimParams)), b_meter = align(sizeof(LimMeter)), b_st = align(sizeof(LimState));
-  const size_t b_hg = align(sizeof(double) * H), b_hy = align(sizeof(double) * w.L), b_x = align(sizeof(double) * len);
-  const size_t b_g0 = align(sizeof(double) * n_g0), b_t32 = align(sizeof(double) * n_t32), b_t1k = align(sizeof(double) * n_t1k);
-  const size_t b_m = align(sizeof(double) * n_m), b_n = align(sizeof(int));
-  const size_t b_cur = b_st + b_hg + b_hy;
-  void* buf = nullptr;
-  if (engine_scratch(e, b_par + b_meter + 2 * b_cur + 2 * b_x + b_g0 + b_t32 + b_t1k + b_m + b_n + 256, &buf)) return -1;
-  char* p = (char*)buf;
   LimHist cur, next;
-  w.params = (LimParams*)p; p += b_par;
-  w.meter = (LimMeter*)p; p += b_meter;
-  char* cur_base = p;
-  cur.st = (LimState*)p; p += b_st;
-  cur.g0 = (double*)p; p += b_hg;
-  cur.y = (double*)p; p += b_hy;
-  next.st = (LimState*)p; p += b_st;
-  next.g0 = (double*)p; p += b_hg;
-  next.y = (double*)p; p += b_hy;
-  double* d_y = (double*)p; p += b_x;
-  double* d_z = (double*)p; p += b_x;
-  w.g0 = (double*)p; p += b_g0;
-  w.t32 = (double*)p; p += b_t32;
-  w.t1k = (double*)p; p += b_t1k;
-  w.m = (double*)p; p += b_m;
-  int* d_n = (int*)p;
+  double *d_y, *d_z;
+  int* d_n;
+  if (engine_scratch(e, [&](Arena& a) {
+        w.params = a.take<LimParams>(1);
+        w.meter = a.take<LimMeter>(1);
+        for (LimHist* hist : {&cur, &next}) {
+          hist->st = a.take<LimState>(1);
+          hist->g0 = a.take<double>(H);
+          hist->y = a.take<double>(w.L);
+        }
+        d_y = a.take<double>(len);
+        d_z = a.take<double>(len);
+        w.g0 = a.take<double>(n_g0);
+        w.t32 = a.take<double>(n_t32);
+        w.t1k = a.take<double>(n_t1k);
+        w.m = a.take<double>(n_m);
+        d_n = a.take<int>(1);
+      })) return -1;
   // host staging: the settings, the sample count, and y followed by L zeros
-  void* hp = nullptr;
-  if (engine_pinned(e, sizeof(LimParams) + sizeof(double) * len + 2 * sizeof(int), &hp)) return -1;
-  LimParams* h_par = (LimParams*)hp;
-  double* h_y = (double*)(h_par + 1);
-  int* h_n = (int*)(h_y + len);
+  LimParams* h_par;
+  double* h_y;
+  int* h_n;
+  if (engine_pinned_layout(e, [&](Arena& a) { h_par = a.take<LimParams>(1); h_y = a.take<double>(len); h_n = a.take<int>(1); })) return -1;
   *h_par = limiter_params(ceiling_db, gain);
   memcpy(h_y, y, sizeof(double) * n);
   memset(h_y + n, 0, sizeof(double) * w.L);
@@ -212,7 +204,10 @@ int ryk_limit(ryk_engine* h, const double* y, int n, int rate, double lookahead_
   RYK_CUDA(cudaMemcpyAsync(w.params, h_par, sizeof(LimParams), cudaMemcpyHostToDevice, s));
   RYK_CUDA(cudaMemcpyAsync(d_y, h_y, sizeof(double) * len, cudaMemcpyHostToDevice, s));
   RYK_CUDA(cudaMemcpyAsync(d_n, h_n, sizeof(int), cudaMemcpyHostToDevice, s));
-  RYK_CUDA(cudaMemsetAsync(cur_base, 0, b_cur, s));       // a fresh state: position 0 (the history is never read before 0)
+  // a fresh state: position 0 (the history is never read before 0)
+  RYK_CUDA(cudaMemsetAsync(cur.st, 0, sizeof(LimState), s));
+  RYK_CUDA(cudaMemsetAsync(cur.g0, 0, sizeof(double) * H, s));
+  RYK_CUDA(cudaMemsetAsync(cur.y, 0, sizeof(double) * w.L, s));
   if (limiter_run(w, cur, next, d_y, d_n, d_z, s)) return -1;
   RYK_CUDA(cudaMemcpyAsync(z, d_z + w.L, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
   RYK_CUDA(cudaStreamSynchronize(s));

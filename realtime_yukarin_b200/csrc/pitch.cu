@@ -138,19 +138,15 @@ int ryk_pitch_correct(ryk_engine* h, const double* f0, int n, int fs, double fra
   RYK_CHECK(fs > 0, "fs must be positive");
   RYK_CHECK(isfinite(frame_period) && frame_period > 0.0, "frame_period must be finite and positive");
   if (int rc = pitch_check(key, scale_mask, a4_hz, retune_ms, amount)) return rc;
-  auto align = [](size_t b) { return (b + 255) / 256 * 256; };
-  const size_t b_par = align(sizeof(PitchParams)), b_st = align(sizeof(PitchState)), b_f0 = align(sizeof(double) * n);
-  void* buf = nullptr;
-  if (engine_scratch(e, b_par + b_st + b_f0, &buf)) return -1;
   PitchWork w;
-  w.params = (PitchParams*)buf;
-  w.state = (PitchState*)((char*)buf + b_par);
-  double* d_f0 = (double*)((char*)buf + b_par + b_st);
-  void* hp = nullptr;
-  if (engine_pinned(e, sizeof(PitchParams) + sizeof(PitchState) + sizeof(double) * n, &hp)) return -1;
-  PitchParams* h_par = (PitchParams*)hp;
-  PitchState* h_st = (PitchState*)(h_par + 1);
-  double* h_f0 = (double*)(h_st + 1);
+  double* d_f0;
+  if (engine_scratch(e, [&](Arena& a) { w.params = a.take<PitchParams>(1); w.state = a.take<PitchState>(1); d_f0 = a.take<double>(n); }))
+    return -1;
+  PitchParams* h_par;
+  PitchState* h_st;
+  double* h_f0;
+  if (engine_pinned_layout(e, [&](Arena& a) { h_par = a.take<PitchParams>(1); h_st = a.take<PitchState>(1); h_f0 = a.take<double>(n); }))
+    return -1;
   *h_par = pitch_params(frame_period, key, scale_mask, a4_hz, retune_ms, amount);
   pitch_state_init(h_st);
   memcpy(h_f0, f0, sizeof(double) * n);

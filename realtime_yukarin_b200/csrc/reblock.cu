@@ -222,20 +222,21 @@ int ryk_reblock_snapshot(ryk_engine* h, int id, void* buf, size_t bytes) {
   RYK_CHECK(bytes == reblock_blob_size(R), "the buffer must be exactly ryk_reblock_snapshot_size bytes");
   if (R->pushed > 0) RYK_CUDA(cudaEventSynchronize(R->ev[(R->pushed - 1) % kRing]));     // pushes run in order on one stream each
   const size_t frag = sizeof(double) * R->cap;
-  void* hp = nullptr;
-  if (engine_pinned(e, sizeof(ReblockState) + 2 * frag, &hp)) return -1;
-  uint8_t* st = (uint8_t*)hp;
+  ReblockState* st;
+  double *fr0, *fr1;
+  if (engine_pinned_layout(e, [&](Arena& a) { st = a.take<ReblockState>(1); fr0 = a.take<double>(R->cap); fr1 = a.take<double>(R->cap); }))
+    return -1;
   RYK_CUDA(cudaMemcpyAsync(st, R->d_state, sizeof(ReblockState), cudaMemcpyDeviceToHost, e->stream));
-  RYK_CUDA(cudaMemcpyAsync(st + sizeof(ReblockState), R->d_frag[0], frag, cudaMemcpyDeviceToHost, e->stream));
-  RYK_CUDA(cudaMemcpyAsync(st + sizeof(ReblockState) + frag, R->d_frag[1], frag, cudaMemcpyDeviceToHost, e->stream));
+  RYK_CUDA(cudaMemcpyAsync(fr0, R->d_frag[0], frag, cudaMemcpyDeviceToHost, e->stream));
+  RYK_CUDA(cudaMemcpyAsync(fr1, R->d_frag[1], frag, cudaMemcpyDeviceToHost, e->stream));
   RYK_CUDA(cudaStreamSynchronize(e->stream));
   ryk_snapshot_reblock c;
   reblock_conf(R, &c);
   uint8_t* cur = snap_begin(buf, kSnapReblock);
   memcpy(snap_section(&cur, snap_tag("RCNF"), sizeof(c)), &c, sizeof(c));
   memcpy(snap_section(&cur, snap_tag("RSTA"), sizeof(ReblockState)), st, sizeof(ReblockState));
-  memcpy(snap_section(&cur, snap_tag("RFR0"), frag), st + sizeof(ReblockState), frag);
-  memcpy(snap_section(&cur, snap_tag("RFR1"), frag), st + sizeof(ReblockState) + frag, frag);
+  memcpy(snap_section(&cur, snap_tag("RFR0"), frag), fr0, frag);
+  memcpy(snap_section(&cur, snap_tag("RFR1"), frag), fr1, frag);
   snap_finish(buf, bytes);
   return 0;
 }
@@ -258,16 +259,16 @@ int ryk_reblock_restore(ryk_engine* h, const void* buf, size_t bytes, int* reblo
   int id = -1;
   if (int rc = ryk_reblock_create(h, c.out_audio_chunk, c.max_in, c.n_fft, c.hop, c.threshold_db, &id)) return rc;
   Reblock* R = e->reblocks[id];
-  void* hp = nullptr;
-  int rc = engine_pinned(e, sizeof(ReblockState) + 2 * frag, &hp);
+  ReblockState* st;
+  double *fr0, *fr1;
+  int rc = engine_pinned_layout(e, [&](Arena& a) { st = a.take<ReblockState>(1); fr0 = a.take<double>(R->cap); fr1 = a.take<double>(R->cap); });
   if (!rc) {
-    uint8_t* st = (uint8_t*)hp;
     memcpy(st, sec[1].data, sizeof(ReblockState));
-    memcpy(st + sizeof(ReblockState), sec[2].data, frag);
-    memcpy(st + sizeof(ReblockState) + frag, sec[3].data, frag);
+    memcpy(fr0, sec[2].data, frag);
+    memcpy(fr1, sec[3].data, frag);
     const cudaError_t err[4] = {cudaMemcpyAsync(R->d_state, st, sizeof(ReblockState), cudaMemcpyHostToDevice, e->stream),
-                                cudaMemcpyAsync(R->d_frag[0], st + sizeof(ReblockState), frag, cudaMemcpyHostToDevice, e->stream),
-                                cudaMemcpyAsync(R->d_frag[1], st + sizeof(ReblockState) + frag, frag, cudaMemcpyHostToDevice, e->stream),
+                                cudaMemcpyAsync(R->d_frag[0], fr0, frag, cudaMemcpyHostToDevice, e->stream),
+                                cudaMemcpyAsync(R->d_frag[1], fr1, frag, cudaMemcpyHostToDevice, e->stream),
                                 cudaStreamSynchronize(e->stream)};
     for (cudaError_t x : err) if (x != cudaSuccess && !rc) { set_error(std::string("re-blocker restore copy failed: ") + cudaGetErrorString(x)); rc = -1; }
   }

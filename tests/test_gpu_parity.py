@@ -135,6 +135,30 @@ def test_synthesizer_matches_oracle(engine):
     assert rmse < 1e-6 * max(1.0, float(np.abs(yr).max()) * 1e3)
 
 
+def test_synthesizer_add_and_synthesis2_equal_decode(engine):
+    # the world4py call pattern (AddParameters, then Synthesis2 until it has no block) is bitwise one decode of the same frames
+    x = _speech(1.2, 7)
+    f = opipe.extract_features(x, CFG)
+    fft = oworld.cheaptrick_fft_size(CFG.fs)
+    sid_dec = engine.synth_create(CFG.fs, CFG.frame_period, fft, 1024)
+    sid_blk = engine.synth_create(CFG.fs, CFG.frame_period, fft, 1024)
+    n_blocks = 0
+    for a in range(0, len(f['f0']), 60):
+        sl = slice(a, a + 60)
+        f0 = f['f0'][sl].ravel().astype(np.float64)
+        yd = engine.synth_decode(sid_dec, f0, f['sp'][sl], f['ap'][sl])
+        assert engine.synth_add_parameters(sid_blk, f0, f['sp'][sl], f['ap'][sl]) == 1
+        blocks = []
+        while (b := engine.synth_synthesis2(sid_blk)) is not None:
+            blocks.append(b)
+        yb = np.concatenate(blocks) if blocks else np.zeros(0)
+        assert np.array_equal(yd, yb), (a, len(yd), len(yb))
+        n_blocks += len(blocks)
+    assert n_blocks > 0
+    engine.synth_destroy(sid_dec)
+    engine.synth_destroy(sid_blk)
+
+
 def test_synthesizer_nan_on_silent_frames(engine):
     fft = oworld.cheaptrick_fft_size(CFG.fs)
     nb = fft // 2 + 1
