@@ -11,18 +11,17 @@ analysis window computed from the layer shapes.  Also the CREPE network's own de
     python bench_crepe.py --out DIR [--steps 200 --warmup 20 --rounds 3]
 
 Writes DIR/bench_crepe.json and prints it.  Needs a CUDA device; there is no CPU path."""
-import argparse
-import json
 import os
 import shutil
 import statistics
-import subprocess
 import tempfile
 from pathlib import Path
 
 import numpy as np
 
-T, EXTRA, FS = 0.3, (0.0, 0.5, 0.0), 24000
+from benchlib import (EXTRA, FS, T, bench_parser, card, device_chunks, device_pusher, emit, headline_config, require_cuda, stopwatch_ms,
+                      synthetic_builtin)
+
 FILTERS, WIDTHS = [32, 4, 4, 4, 8, 16], [512, 64, 64, 64, 64, 64]
 LEGS = [('dio', None, 'fp32'), ('dio', None, 'fp16'), ('crepe', 'tiny', 'fp32'), ('crepe', 'tiny', 'fp16'),
         ('crepe', 'full', 'fp32'), ('crepe', 'full', 'fp16')]
@@ -39,47 +38,27 @@ def crepe_flop_per_frame(capacity):
     return flop + 2 * 4 * cout[5] * 360
 
 
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'], capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else 'unknown (nvidia-smi unavailable)'
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--out', type=Path, required=True)
-    ap.add_argument('--steps', type=int, default=200)
-    ap.add_argument('--warmup', type=int, default=20)
-    ap.add_argument('--rounds', type=int, default=3)
-    args = ap.parse_args()
+    args = bench_parser(required_out=True, steps=200, warmup=20, rounds=3).parse_args()
+    require_cuda('bench_crepe.py')
     import torch
-    if not torch.cuda.is_available():
-        raise SystemExit('bench_crepe.py needs a CUDA device')
     os.environ['RYK_STAGE_TIMES'] = '1'
     from realtime_yukarin_b200 import crepe, synthetic
-    from realtime_yukarin_b200.engine import Engine, SessionConfig
-    from realtime_yukarin_b200.models import AcousticConverter, F0Converter, SuperResolution
-    from realtime_yukarin_b200.params import create_from_json, create_sr_from_json
+    from realtime_yukarin_b200.engine import Engine
 
     tmp = Path(tempfile.mkdtemp(prefix='bench_crepe_'))       # synthetic model files: never written into the tree
-    paths = synthetic.write_synthetic_models(tmp, seed=0)
+    eng = Engine()
+    synthetic_builtin(eng, tmp)
     weights = {}
     for c in ('tiny', 'full'):
         (tmp / c).mkdir()
         weights[c] = synthetic.write_crepe_model(tmp / c, seed=1, capacity=c)
-    eng = Engine()
-    f0c = F0Converter(paths['input_statistics_path'], paths['target_statistics_path'])
-    AcousticConverter(create_from_json(paths['stage1_config_path']), paths['stage1_model_path'], f0_converter=f0c, engine=eng)
-    SuperResolution(create_sr_from_json(paths['stage2_config_path']), paths['stage2_model_path'], engine=eng)
     n = round(T * FS)
     total = args.warmup + args.steps
     x = synthetic.synthetic_speech((total + 1) * T, stream=0)
-    d_in = torch.from_numpy(np.stack([x[k * n:(k + 1) * n] for k in range(total)])).cuda()
+    d_in = device_chunks(x, n, total)
     out_cap = (n // 1024 + 5) * 1024 + 8192
-    d_out = torch.empty((8, out_cap), dtype=torch.float64, device='cuda')
-    d_n = torch.zeros(8, dtype=torch.int32, device='cuda')
-    cfg = SessionConfig(fs=FS, frame_period_ms=5.0, f0_floor=71.0, f0_ceil=800.0, fft_length=1024, order=8, alpha=0.466, buffer_time=T,
-                        encode_extra_time=EXTRA[0], convert_extra_time=EXTRA[1], decode_extra_time=EXTRA[2], threshold_db=60.0,
-                        vocoder_buffer_size=1024)
+    cfg = headline_config()
 
     def leg(method, capacity, precision):
         if capacity is not None:
@@ -88,16 +67,8 @@ def main():
         eng.set_f0_method(method)
         sid = eng.session_create(cfg)
         eng.set_f0_method('dio')
-
-        def push(k):
-            eng.session_push_device(sid, d_in[k].data_ptr(), n, d_out[k % 8].data_ptr(), out_cap, d_n[k % 8:].data_ptr())
-        for k in range(args.warmup):
-            push(k)
-        eng.synchronize()
-        eng.timer_start()
-        for k in range(args.warmup, total):
-            push(k)
-        ms = eng.timer_stop()
+        push = device_pusher(eng, d_in, out_cap)
+        ms = stopwatch_ms(eng, lambda: push(sid), args.warmup, args.steps)
         st, en = eng.session_stage_times(sid)
         eng.session_destroy(sid)
         return ms / args.steps, float((en[:, 1] - st[:, 1]).mean())
@@ -143,9 +114,7 @@ def main():
                 note='CREPE convolutions: FP32 CUDA cores (conv_direct.cu) in precision 0, 3xTF32 tensor cores (crepe_tc.cu) in precision 1',
                 legs=rows, crepe_network=network, session_mib=footprint)
     shutil.rmtree(tmp, ignore_errors=True)
-    args.out.mkdir(parents=True, exist_ok=True)
-    (args.out / 'bench_crepe.json').write_text(json.dumps(line, indent=1))
-    print(json.dumps(line))
+    emit(args.out, 'bench_crepe', line)
 
 
 if __name__ == '__main__':

@@ -10,8 +10,6 @@ The card's name, power limit and SM clock are recorded with the numbers.
     python bench_drift.py [--out DIR] [--pushes 300 --warmup 20 --profile_pushes 50]
 
 Prints one JSON line (and writes it to DIR/bench_drift.json with --out).  Needs a CUDA device; there is no CPU path."""
-import argparse
-import json
 import shutil
 import statistics
 import tempfile
@@ -20,29 +18,16 @@ from pathlib import Path
 
 import numpy as np
 
-from bench_f0_control import card
+from benchlib import bench_parser, card, emit, kernel_durations, require_cuda
 
 RATES = (24000, 48000)
 CHUNKS_S = (0.3, 1.0)
 PPM = 250.0
 
 
-def make_parser():
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--out', type=Path, default=None)
-    ap.add_argument('--pushes', type=int, default=300)
-    ap.add_argument('--warmup', type=int, default=20)
-    ap.add_argument('--profile_pushes', type=int, default=50)
-    return ap
-
-
 def main(argv=None):
-    args = make_parser().parse_args(argv)
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit('bench_drift.py needs a CUDA device')
-    from torch.profiler import ProfilerActivity, profile
-
+    args = bench_parser(pushes=300, warmup=20, profile_pushes=50).parse_args(argv)
+    require_cuda('bench_drift.py')
     from realtime_yukarin_b200.engine import Engine
     eng = Engine(device=0)
     tmp = Path(tempfile.mkdtemp(prefix='bench_drift_'))
@@ -57,16 +42,11 @@ def main(argv=None):
                 eng.drift_set(did, PPM)
                 for _ in range(args.warmup):
                     eng.drift_push(did, x)
-                eng.synchronize()
-                with profile(activities=[ProfilerActivity.CUDA]) as prof:
+
+                def profiled_pushes():
                     for _ in range(args.profile_pushes):
                         eng.drift_push(did, x)
-                    eng.synchronize()
-                trace = tmp / f'trace_{rate}_{n}.json'
-                prof.export_chrome_trace(str(trace))
-                ev = json.loads(trace.read_text())
-                ev = ev['traceEvents'] if isinstance(ev, dict) else ev
-                kern = [e['dur'] for e in ev if e.get('cat') == 'kernel' and e.get('ph') == 'X' and 'k_drift' in e['name']]
+                kern = kernel_durations(eng, tmp, profiled_pushes, ['k_drift'])['k_drift']
                 host = []
                 for _ in range(args.pushes):
                     t0 = time.perf_counter()
@@ -82,10 +62,7 @@ def main(argv=None):
         shutil.rmtree(tmp, ignore_errors=True)
         eng.close()
     line = dict(card=card(), ppm=PPM, pushes=args.pushes, warmup=args.warmup, profile_pushes=args.profile_pushes, results=results)
-    if args.out is not None:
-        args.out.mkdir(parents=True, exist_ok=True)
-        (args.out / 'bench_drift.json').write_text(json.dumps(line, indent=1))
-    print(json.dumps(line))
+    emit(args.out, 'bench_drift', line)
 
 
 if __name__ == '__main__':

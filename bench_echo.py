@@ -15,8 +15,6 @@ with the numbers.
     python bench_echo.py [--out DIR] [--steps 1000 --block 100 --latency_steps 200 --group_steps 300 --warmup 30 --repeats 3]
 
 Prints one JSON line (and writes it to DIR/bench_echo.json with --out).  Needs a CUDA device; there is no CPU path."""
-import argparse
-import json
 import shutil
 import statistics
 import tempfile
@@ -25,50 +23,32 @@ from pathlib import Path
 
 import numpy as np
 
-from bench_f0_control import EXTRA, FS, T, card
+from benchlib import (EXTRA, FS, RING, T, bench_parser, card, device_chunks, emit, headline_config, kernel_durations, output_ring,
+                      require_cuda, synthetic_voice, throughput)
 
 VARIANTS = ('off', 16, 32, 64)
 GROUP = 8
 
 
-def make_parser():
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--out', type=Path, default=None)
-    ap.add_argument('--steps', type=int, default=1000)
-    ap.add_argument('--block', type=int, default=100)
-    ap.add_argument('--latency_steps', type=int, default=200)
-    ap.add_argument('--group_steps', type=int, default=300)
-    ap.add_argument('--warmup', type=int, default=30)
-    ap.add_argument('--repeats', type=int, default=3)
-    ap.add_argument('--profile_steps', type=int, default=20)
-    return ap
-
-
 def main(argv=None):
-    args = make_parser().parse_args(argv)
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit('bench_echo.py needs a CUDA device')
+    args = bench_parser(steps=1000, block=100, latency_steps=200, group_steps=300, warmup=30, repeats=3,
+                        profile_steps=20).parse_args(argv)
+    require_cuda('bench_echo.py')
     from realtime_yukarin_b200 import synthetic
-    from realtime_yukarin_b200.engine import Engine, SessionConfig
-    from realtime_yukarin_b200.models import load_voice
+    from realtime_yukarin_b200.engine import Engine
 
     tmp = Path(tempfile.mkdtemp(prefix='bench_echo_'))              # synthetic model files: never written into the tree
     eng = Engine()
     eng.set_precision('fp16')
-    paths = synthetic.write_synthetic_models(tmp / 'v0', seed=0)
-    voice = eng.voice_create()
-    load_voice(eng, voice, **{k: paths[k] for k in ('stage1_model_path', 'stage2_model_path', 'input_statistics_path', 'target_statistics_path')})
-    cfg = SessionConfig(fs=FS, frame_period_ms=5.0, f0_floor=71.0, f0_ceil=800.0, fft_length=1024, order=8, alpha=0.466, buffer_time=T,
-                        encode_extra_time=EXTRA[0], convert_extra_time=EXTRA[1], decode_extra_time=EXTRA[2], threshold_db=60.0,
-                        vocoder_buffer_size=1024)
+    voice = synthetic_voice(eng, tmp)
+    cfg = headline_config()
     n = round(T * FS)
     n_chunks = 64
-    x = synthetic.synthetic_speech((n_chunks + 1) * T, stream=0).astype(np.float32)
+    x = synthetic.synthetic_speech((n_chunks + 1) * T, stream=0)
     far = (0.5 * synthetic.synthetic_speech((n_chunks + 1) * T, stream=1)).astype(np.float32)
     mic_chunks = [np.ascontiguousarray(x[k * n:(k + 1) * n]) for k in range(n_chunks)]
     far_chunks = [np.ascontiguousarray(far[k * n:(k + 1) * n]) for k in range(n_chunks)]
-    d_in = torch.from_numpy(np.stack(mic_chunks)).cuda()
+    d_in = device_chunks(x, n, n_chunks)
 
     def make(v):
         sid = eng.session_create(cfg, voice=voice)
@@ -81,9 +61,7 @@ def main(argv=None):
         members = [make(v) for _ in range(GROUP)]
         groups[v] = (eng.group_create(members), members)
     cap = eng.session_io_geometry(alone['off'])['max_out']
-    ring = 8                                      # distinct output slots: consecutive steps are in flight together
-    d_out = torch.empty((ring, cap), dtype=torch.float64, device='cuda')
-    d_n = torch.zeros((ring, 1), dtype=torch.int32, device='cuda')
+    d_out, d_n = output_ring(cap)
     buf = np.empty(cap)
     gbufs = [np.empty(cap) for _ in range(GROUP)]
     step_no = {v: 0 for v in VARIANTS}
@@ -93,7 +71,7 @@ def main(argv=None):
         k = step_no[v]
         if v != 'off':
             eng.session_echo_reference(alone[v], far_chunks[k % n_chunks])
-        eng.session_push_device(alone[v], d_in[k % n_chunks].data_ptr(), n, d_out[k % ring].data_ptr(), cap, d_n[k % ring].data_ptr())
+        eng.session_push_device(alone[v], d_in[k % n_chunks].data_ptr(), n, d_out[k % RING, 0].data_ptr(), cap, d_n[k % RING, 0].data_ptr())
         step_no[v] = k + 1
 
     def push_host(v):
@@ -116,17 +94,6 @@ def main(argv=None):
         gstep_no[v] = k + 1
         return time.perf_counter() - t0
 
-    def leg_throughput(v, steps):
-        eng.synchronize()
-        t0 = time.perf_counter()
-        done = 0
-        while done < steps:
-            for _ in range(min(args.block, steps - done)):
-                push_device(v)
-            done += min(args.block, steps - done)
-            eng.synchronize()
-        return steps / (time.perf_counter() - t0)
-
     def leg_latency(fn, v, steps):
         eng.synchronize()
         t0 = time.perf_counter()
@@ -134,35 +101,26 @@ def main(argv=None):
         return steps / (time.perf_counter() - t0), lat
 
     for v in VARIANTS:
-        leg_throughput(v, args.warmup)
+        throughput(eng, lambda: push_device(v), args.warmup, args.block)
         leg_latency(push_host, v, args.warmup)
         leg_latency(push_group, v, args.warmup)
     res = {v: dict(alone_steps_per_s=[], alone_latency_ms=[], group_steps_per_s=[], group_latency_ms=[]) for v in VARIANTS}
     for _ in range(args.repeats):
         for v in VARIANTS:
             r = res[v]
-            r['alone_steps_per_s'].append(leg_throughput(v, args.steps))
+            r['alone_steps_per_s'].append(throughput(eng, lambda: push_device(v), args.steps, args.block))
             r['alone_latency_ms'].extend(1e3 * t for t in leg_latency(push_host, v, args.latency_steps)[1])
             rate, lat = leg_latency(push_group, v, args.group_steps)
             r['group_steps_per_s'].append(rate)
             r['group_latency_ms'].extend(1e3 * t for t in lat)
 
     # kernel times: one profiler window over the lone sessions, one variant after the other
-    from torch.profiler import ProfilerActivity, profile
-    eng.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    def profiled_steps():
         for v in VARIANTS:
             for _ in range(args.profile_steps):
                 push_host(v)
-        eng.synchronize()
-    trace = tmp / 'trace.json'
-    prof.export_chrome_trace(str(trace))
-    ev = json.loads(trace.read_text())
-    ev = ev['traceEvents'] if isinstance(ev, dict) else ev
-    kern = sorted((e for e in ev if e.get('cat') == 'kernel' and e.get('ph') == 'X'), key=lambda e: e['ts'])
-    scans = [e['dur'] for e in kern if 'k_aec_scan' in e['name']]
-    fwd = [e['dur'] for e in kern if 'k_dn_forward' in e['name']]
-    inv = [e['dur'] for e in kern if 'k_dn_inverse' in e['name']]
+    durations = kernel_durations(eng, tmp, profiled_steps, ('k_aec_scan', 'k_dn_forward', 'k_dn_inverse'))
+    scans, fwd, inv = durations['k_aec_scan'], durations['k_dn_forward'], durations['k_dn_inverse']
     tapped = [v for v in VARIANTS if v != 'off']
     kernels = {}
     for i, v in enumerate(tapped):
@@ -187,10 +145,7 @@ def main(argv=None):
     line = dict(card=card(), buffer_time=T, extras=EXTRA, group=GROUP, steps=args.steps, block=args.block,
                 latency_steps=args.latency_steps, group_steps=args.group_steps, warmup=args.warmup, repeats=args.repeats,
                 variants={str(v): summary(res[v]) for v in VARIANTS}, kernels=kernels)
-    if args.out is not None:
-        args.out.mkdir(parents=True, exist_ok=True)
-        (args.out / 'bench_echo.json').write_text(json.dumps(line, indent=1))
-    print(json.dumps(line))
+    emit(args.out, 'bench_echo', line)
 
 
 if __name__ == '__main__':

@@ -15,54 +15,32 @@ The card's name and power limit are recorded with the numbers.
     python bench_group_churn.py [--out DIR] [--repeats 7 --steps 100 --warmup 10 --rounds 3]
 
 Prints one JSON line (and writes it to DIR/bench_group_churn.json with --out).  Needs a CUDA device; there is no CPU path."""
-import argparse
-import json
 import shutil
 import statistics
-import subprocess
 import tempfile
 import time
 from pathlib import Path
 
-import numpy as np
+from benchlib import EXTRA, FS, T, bench_parser, card, device_chunks, emit, headline_config, require_cuda, synthetic_voice
 
-EXTRA, FS, T = (0.0, 0.5, 0.0), 24000, 0.3
 BS = list(range(1, 9))
 
 
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'], capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else 'unknown (nvidia-smi unavailable)'
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--out', type=Path, default=None)
-    ap.add_argument('--repeats', type=int, default=7)
-    ap.add_argument('--steps', type=int, default=100)
-    ap.add_argument('--warmup', type=int, default=10)
-    ap.add_argument('--rounds', type=int, default=3)
-    args = ap.parse_args()
+    args = bench_parser(repeats=7, steps=100, warmup=10, rounds=3).parse_args()
+    require_cuda('bench_group_churn.py')
     import torch
-    if not torch.cuda.is_available():
-        raise SystemExit('bench_group_churn.py needs a CUDA device')
     from realtime_yukarin_b200 import synthetic
-    from realtime_yukarin_b200.engine import Engine, SessionConfig
-    from realtime_yukarin_b200.models import load_voice
+    from realtime_yukarin_b200.engine import Engine
 
     tmp = Path(tempfile.mkdtemp(prefix='bench_group_churn_'))       # synthetic model files: never written into the tree
     eng = Engine()
     eng.set_precision('fp16')
-    paths = synthetic.write_synthetic_models(tmp / 'v0', seed=0)
-    voice = eng.voice_create()
-    load_voice(eng, voice, **{k: paths[k] for k in ('stage1_model_path', 'stage2_model_path', 'input_statistics_path', 'target_statistics_path')})
-    cfg = SessionConfig(fs=FS, frame_period_ms=5.0, f0_floor=71.0, f0_ceil=800.0, fft_length=1024, order=8, alpha=0.466, buffer_time=T,
-                        encode_extra_time=EXTRA[0], convert_extra_time=EXTRA[1], decode_extra_time=EXTRA[2], threshold_db=60.0,
-                        vocoder_buffer_size=1024)
+    voice = synthetic_voice(eng, tmp)
+    cfg = headline_config()
     n = round(T * FS)
     n_chunks = 64
-    x = synthetic.synthetic_speech((n_chunks + 1) * T, stream=0)
-    d_in = torch.from_numpy(np.stack([x[k * n:(k + 1) * n] for k in range(n_chunks)])).cuda()
+    d_in = device_chunks(synthetic.synthetic_speech((n_chunks + 1) * T, stream=0), n, n_chunks)
     sids = [eng.session_create(cfg, voice=voice) for _ in range(max(BS) + 1)]
     cap = eng.session_io_geometry(sids[0])['max_out']
     d_out = torch.empty((len(sids), cap), dtype=torch.float64, device='cuda')
@@ -147,10 +125,7 @@ def main():
                  fixed_chunks_per_s=statistics.median(rates['fixed']), churn_chunks_per_s=statistics.median(rates['churn']),
                  fixed_all=rates['fixed'], churn_all=rates['churn'])
     line = dict(card=card(), buffer_time=T, extras=EXTRA, repeats=args.repeats, changes=changes, churn=churn)
-    if args.out is not None:
-        args.out.mkdir(parents=True, exist_ok=True)
-        (args.out / 'bench_group_churn.json').write_text(json.dumps(line, indent=1))
-    print(json.dumps(line))
+    emit(args.out, 'bench_group_churn', line)
 
 
 if __name__ == '__main__':

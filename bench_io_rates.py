@@ -11,59 +11,35 @@ resampling), mean over the last 8 steps of the first session.  The card's name a
     python bench_io_rates.py --out DIR [--steps 200 --warmup 20 --rounds 3]
 
 Writes DIR/bench_io_rates.json and prints it.  Needs a CUDA device; there is no CPU path."""
-import argparse
-import json
 import os
 import shutil
 import statistics
-import subprocess
 import tempfile
 from pathlib import Path
 
-import numpy as np
+from benchlib import (EXTRA, FS, T, bench_parser, card, device_chunks, device_pusher, emit, headline_config, require_cuda, stopwatch_ms,
+                      synthetic_builtin)
 
-T, EXTRA, FS = 0.3, (0.0, 0.5, 0.0), 24000
 LEGS = [(24000, 24000, 1), (48000, 48000, 1), (44100, 44100, 1), (48000, 24000, 1), (48000, 48000, 4)]
 
 
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'], capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else 'unknown (nvidia-smi unavailable)'
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--out', type=Path, required=True)
-    ap.add_argument('--steps', type=int, default=200)
-    ap.add_argument('--warmup', type=int, default=20)
-    ap.add_argument('--rounds', type=int, default=3)
-    args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit('bench_io_rates.py needs a CUDA device')
+    args = bench_parser(required_out=True, steps=200, warmup=20, rounds=3).parse_args()
+    require_cuda('bench_io_rates.py')
     stage_times = os.environ.get('RYK_STAGE_TIMES', '0') not in ('', '0')
     from realtime_yukarin_b200 import synthetic, wave_io
-    from realtime_yukarin_b200.engine import Engine, SessionConfig
-    from realtime_yukarin_b200.models import AcousticConverter, F0Converter, SuperResolution
-    from realtime_yukarin_b200.params import create_from_json, create_sr_from_json
+    from realtime_yukarin_b200.engine import Engine
 
     tmp = Path(tempfile.mkdtemp(prefix='bench_io_rates_'))    # synthetic model files: never written into the tree
-    paths = synthetic.write_synthetic_models(tmp, seed=0)
     eng = Engine()
-    f0c = F0Converter(paths['input_statistics_path'], paths['target_statistics_path'])
-    AcousticConverter(create_from_json(paths['stage1_config_path']), paths['stage1_model_path'], f0_converter=f0c, engine=eng)
-    SuperResolution(create_sr_from_json(paths['stage2_config_path']), paths['stage2_model_path'], engine=eng)
+    synthetic_builtin(eng, tmp)
     eng.set_precision('fp16')
     total = args.warmup + args.steps
     x24 = synthetic.synthetic_speech((total + 1) * T, stream=0)
     inputs = {}                                       # device rate -> (total, n_in) chunks on the device
     for rate in sorted({leg[0] for leg in LEGS}):
-        n_in = round(T * rate)
-        x = wave_io.resample(x24, FS, rate, eng)
-        inputs[rate] = torch.from_numpy(np.stack([x[k * n_in:(k + 1) * n_in] for k in range(total)])).cuda()
-    cfg = SessionConfig(fs=FS, frame_period_ms=5.0, f0_floor=71.0, f0_ceil=800.0, fft_length=1024, order=8, alpha=0.466, buffer_time=T,
-                        encode_extra_time=EXTRA[0], convert_extra_time=EXTRA[1], decode_extra_time=EXTRA[2], threshold_db=60.0,
-                        vocoder_buffer_size=1024)
+        inputs[rate] = device_chunks(wave_io.resample(x24, FS, rate, eng), round(T * rate), total)
+    cfg = headline_config()
 
     def leg(rate_in, rate_out, members):
         sids = []
@@ -72,25 +48,9 @@ def main():
             eng.session_set_input_rate(sid, rate_in)
             eng.session_set_output_rate(sid, rate_out)
             sids.append(sid)
-        g = eng.session_io_geometry(sids[0])
-        d_in = inputs[rate_in]
-        d_out = torch.empty((members, 8, g['max_out']), dtype=torch.float64, device='cuda')
-        d_n = torch.zeros((members, 8), dtype=torch.int32, device='cuda')
+        push = device_pusher(eng, inputs[rate_in], eng.session_io_geometry(sids[0])['max_out'], members)
         gid = eng.group_create(sids) if members > 1 else None
-
-        def push(k):
-            if gid is None:
-                eng.session_push_device(sids[0], d_in[k].data_ptr(), g['n_in'], d_out[0, k % 8].data_ptr(), g['max_out'], d_n[0, k % 8:].data_ptr())
-            else:
-                eng.group_push_device(gid, [d_in[k].data_ptr()] * members, g['n_in'], [d_out[i, k % 8].data_ptr() for i in range(members)],
-                                      g['max_out'], [d_n[i, k % 8:].data_ptr() for i in range(members)])
-        for k in range(args.warmup):
-            push(k)
-        eng.synchronize()
-        eng.timer_start()
-        for k in range(args.warmup, total):
-            push(k)
-        ms = eng.timer_stop()
+        ms = stopwatch_ms(eng, (lambda: push(sids[0])) if gid is None else (lambda: push(gid, group=True)), args.warmup, args.steps)
         gate = synth = None
         if stage_times:
             st, en = eng.session_stage_times(sids[0])
@@ -117,9 +77,7 @@ def main():
     line = dict(card=card(), buffer_time=T, extras=EXTRA, steps=args.steps, warmup=args.warmup, rounds=args.rounds, stage_times=stage_times,
                 legs=rows)
     shutil.rmtree(tmp, ignore_errors=True)
-    args.out.mkdir(parents=True, exist_ok=True)
-    (args.out / 'bench_io_rates.json').write_text(json.dumps(line, indent=1))
-    print(json.dumps(line))
+    emit(args.out, 'bench_io_rates', line)
 
 
 if __name__ == '__main__':

@@ -10,17 +10,15 @@ other kernels.  The card's name and power limit are recorded with the numbers.
     python bench_limiter.py [--out DIR] [--steps 1000 --block 100 --warmup 30 --repeats 3 --profile_steps 20]
 
 Prints one JSON line (and writes it to DIR/bench_limiter.json with --out).  Needs a CUDA device; there is no CPU path."""
-import argparse
-import json
 import shutil
 import statistics
 import tempfile
-import time
 from pathlib import Path
 
 import numpy as np
 
-from bench_f0_control import EXTRA, FS, T, card
+from benchlib import (EXTRA, FS, T, alternate, bench_parser, card, device_chunks, device_pusher, emit, headline_config,
+                      kernel_durations, require_cuda, synthetic_voice, throughput)
 
 VARIANTS = [(rate, hold) for rate in (24000, 48000) for hold in (None, 50.0, 500.0)]
 LOOKAHEAD_MS = 5.0
@@ -32,40 +30,22 @@ def _name(v):
     return f'{rate // 1000}k_' + ('off' if hold is None else f'hold{int(hold)}')
 
 
-def make_parser():
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--out', type=Path, default=None)
-    ap.add_argument('--steps', type=int, default=1000)
-    ap.add_argument('--block', type=int, default=100)
-    ap.add_argument('--warmup', type=int, default=30)
-    ap.add_argument('--repeats', type=int, default=3)
-    ap.add_argument('--profile_steps', type=int, default=20)
-    return ap
-
-
 def main(argv=None):
-    args = make_parser().parse_args(argv)
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit('bench_limiter.py needs a CUDA device')
+    args = bench_parser(steps=1000, block=100, warmup=30, repeats=3, profile_steps=20).parse_args(argv)
+    require_cuda('bench_limiter.py')
     from realtime_yukarin_b200 import synthetic
-    from realtime_yukarin_b200.engine import Engine, SessionConfig
-    from realtime_yukarin_b200.models import load_voice
+    from realtime_yukarin_b200.engine import Engine
 
     tmp = Path(tempfile.mkdtemp(prefix='bench_limiter_'))           # synthetic model files: never written into the tree
     eng = Engine()
     eng.set_precision('fp16')
-    paths = synthetic.write_synthetic_models(tmp / 'v0', seed=0)
-    voice = eng.voice_create()
-    load_voice(eng, voice, **{k: paths[k] for k in ('stage1_model_path', 'stage2_model_path', 'input_statistics_path', 'target_statistics_path')})
-    cfg = SessionConfig(fs=FS, frame_period_ms=5.0, f0_floor=71.0, f0_ceil=800.0, fft_length=1024, order=8, alpha=0.466, buffer_time=T,
-                        encode_extra_time=EXTRA[0], convert_extra_time=EXTRA[1], decode_extra_time=EXTRA[2], threshold_db=60.0,
-                        vocoder_buffer_size=1024)
+    voice = synthetic_voice(eng, tmp)
+    cfg = headline_config()
     n = round(T * FS)
     n_chunks = 64
-    x = synthetic.synthetic_speech((n_chunks + 1) * T, stream=0).astype(np.float32)
+    x = synthetic.synthetic_speech((n_chunks + 1) * T, stream=0)
     chunks = [np.ascontiguousarray(x[k * n:(k + 1) * n]) for k in range(n_chunks)]
-    d_in = torch.from_numpy(np.stack(chunks)).cuda()
+    d_in = device_chunks(x, n, n_chunks)
 
     # the voice's peak level over the chunks sets the gain that drives the limiter
     probe = eng.session_create(cfg, voice=voice)
@@ -84,56 +64,27 @@ def main(argv=None):
             eng.session_set_limiter(sid, -1.0, gain)
         return sid
     sessions = {v: make(v) for v in VARIANTS}
-    cap = max(eng.session_io_geometry(s)['max_out'] for s in sessions.values())
-    ring = 8                                      # distinct output slots: consecutive steps are in flight together
-    d_out = torch.empty((ring, cap), dtype=torch.float64, device='cuda')
-    d_n = torch.zeros((ring, 1), dtype=torch.int32, device='cuda')
-    torch.cuda.synchronize()
-    step_no = {v: 0 for v in VARIANTS}
+    push = device_pusher(eng, d_in, max(eng.session_io_geometry(s)['max_out'] for s in sessions.values()))
 
-    def push_device(v):
-        k = step_no[v]
-        eng.session_push_device(sessions[v], d_in[k % n_chunks].data_ptr(), n, d_out[k % ring].data_ptr(), cap, d_n[k % ring].data_ptr())
-        step_no[v] = k + 1
-
-    def leg_throughput(v, steps):
-        eng.synchronize()
-        t0 = time.perf_counter()
-        done = 0
-        while done < steps:
-            for _ in range(min(args.block, steps - done)):
-                push_device(v)
-            done += min(args.block, steps - done)
-            eng.synchronize()
-        return steps / (time.perf_counter() - t0)
-
-    for v in VARIANTS:
-        leg_throughput(v, args.warmup)
-    res = {v: [] for v in VARIANTS}
-    for _ in range(args.repeats):
-        for v in VARIANTS:
-            res[v].append(leg_throughput(v, args.steps))
+    def leg(v, steps):
+        return throughput(eng, lambda: push(sessions[v]), steps, args.block)
+    res = alternate(VARIANTS, leg, args.steps, args.warmup, args.repeats)
     reductions = {_name(v): eng.session_limiter_stats(sessions[v]) for v in VARIANTS if v[1] is not None}
 
     # kernel times: one profiler window, one limited session after the other
-    from torch.profiler import ProfilerActivity, profile
     limited = [v for v in VARIANTS if v[1] is not None]
-    eng.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+
+    def profiled_steps():
         for v in limited:
             for _ in range(args.profile_steps):
-                push_device(v)
+                push(sessions[v])
             eng.synchronize()
-    trace = tmp / 'trace.json'
-    prof.export_chrome_trace(str(trace))
-    ev = json.loads(trace.read_text())
-    ev = ev['traceEvents'] if isinstance(ev, dict) else ev
-    kern = sorted((e for e in ev if e.get('cat') == 'kernel' and e.get('ph') == 'X'), key=lambda e: e['ts'])
+    durations = kernel_durations(eng, tmp, profiled_steps, KERNELS)
     kernels = {}
     for i, v in enumerate(limited):
         per = {}
         for name in KERNELS:
-            d = [e['dur'] for e in kern if name in e['name']][i * args.profile_steps:(i + 1) * args.profile_steps]
+            d = durations[name][i * args.profile_steps:(i + 1) * args.profile_steps]
             per[f'{name}_us_median'] = statistics.median(d) if d else None
         per['limiter_us_per_step_median'] = sum(per[f'{name}_us_median'] or 0.0 for name in KERNELS)
         kernels[_name(v)] = per
@@ -147,10 +98,7 @@ def main(argv=None):
                 warmup=args.warmup, repeats=args.repeats,
                 variants={_name(v): dict(steps_per_s=statistics.median(res[v]), steps_per_s_all=res[v]) for v in VARIANTS},
                 last_step_reduction=reductions, kernels=kernels)
-    if args.out is not None:
-        args.out.mkdir(parents=True, exist_ok=True)
-        (args.out / 'bench_limiter.json').write_text(json.dumps(line, indent=1))
-    print(json.dumps(line))
+    emit(args.out, 'bench_limiter', line)
 
 
 if __name__ == '__main__':

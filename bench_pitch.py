@@ -11,17 +11,13 @@ numbers.
     python bench_pitch.py [--out DIR] [--steps 1000 --block 100 --warmup 30 --repeats 3 --profile_steps 20]
 
 Prints one JSON line (and writes it to DIR/bench_pitch.json with --out).  Needs a CUDA device; there is no CPU path."""
-import argparse
-import json
 import shutil
 import statistics
 import tempfile
-import time
 from pathlib import Path
 
-import numpy as np
-
-from bench_f0_control import EXTRA, FS, T, card
+from benchlib import (EXTRA, FS, T, alternate, bench_parser, card, device_chunks, device_pusher, emit, headline_config,
+                      kernel_durations, require_cuda, synthetic_voice, throughput)
 
 VARIANTS = ('off', 'pitch')
 MEMBERS = 8
@@ -29,40 +25,19 @@ KERNEL = 'k_pitch'
 SETTINGS = dict(key='D', scale='major', a4_hz=440.0, retune_ms=30.0, amount=1.0)
 
 
-def make_parser():
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--out', type=Path, default=None)
-    ap.add_argument('--steps', type=int, default=1000)
-    ap.add_argument('--block', type=int, default=100)
-    ap.add_argument('--warmup', type=int, default=30)
-    ap.add_argument('--repeats', type=int, default=3)
-    ap.add_argument('--profile_steps', type=int, default=20)
-    return ap
-
-
 def main(argv=None):
-    args = make_parser().parse_args(argv)
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit('bench_pitch.py needs a CUDA device')
+    args = bench_parser(steps=1000, block=100, warmup=30, repeats=3, profile_steps=20).parse_args(argv)
+    require_cuda('bench_pitch.py')
     from realtime_yukarin_b200 import synthetic
-    from realtime_yukarin_b200.engine import Engine, SessionConfig
-    from realtime_yukarin_b200.models import load_voice
+    from realtime_yukarin_b200.engine import Engine
 
     tmp = Path(tempfile.mkdtemp(prefix='bench_pitch_'))               # synthetic model files: never written into the tree
     eng = Engine()
     eng.set_precision('fp16')
-    paths = synthetic.write_synthetic_models(tmp / 'v0', seed=0)
-    voice = eng.voice_create()
-    load_voice(eng, voice, **{k: paths[k] for k in ('stage1_model_path', 'stage2_model_path', 'input_statistics_path', 'target_statistics_path')})
-    cfg = SessionConfig(fs=FS, frame_period_ms=5.0, f0_floor=71.0, f0_ceil=800.0, fft_length=1024, order=8, alpha=0.466, buffer_time=T,
-                        encode_extra_time=EXTRA[0], convert_extra_time=EXTRA[1], decode_extra_time=EXTRA[2], threshold_db=60.0,
-                        vocoder_buffer_size=1024)
-    n = round(T * FS)
+    voice = synthetic_voice(eng, tmp)
+    cfg = headline_config()
     n_chunks = 64
-    x = synthetic.synthetic_speech((n_chunks + 1) * T, stream=0).astype(np.float32)
-    chunks = [np.ascontiguousarray(x[k * n:(k + 1) * n]) for k in range(n_chunks)]
-    d_in = torch.from_numpy(np.stack(chunks)).cuda()
+    d_in = device_chunks(synthetic.synthetic_speech((n_chunks + 1) * T, stream=0), round(T * FS), n_chunks)
 
     def make(v):
         sid = eng.session_create(cfg, voice=voice)
@@ -72,58 +47,25 @@ def main(argv=None):
         return sid
     sessions = {v: make(v) for v in VARIANTS}
     groups = {v: eng.group_create([make(v) for _ in range(MEMBERS)]) for v in VARIANTS}
-    cap = eng.session_io_geometry(sessions['off'])['max_out']
-    ring = 8                                      # distinct output slots: consecutive steps are in flight together
-    d_out = torch.empty((ring, MEMBERS, cap), dtype=torch.float64, device='cuda')
-    d_n = torch.zeros((ring, MEMBERS, 1), dtype=torch.int32, device='cuda')
-    torch.cuda.synchronize()
-    step_no = {}
-
-    def push_device(kind, v):
-        k = step_no.get((kind, v), 0)
-        src, r = d_in[k % n_chunks].data_ptr(), k % ring
-        if kind == 'single':
-            eng.session_push_device(sessions[v], src, n, d_out[r, 0].data_ptr(), cap, d_n[r, 0].data_ptr())
-        else:
-            eng.group_push_device(groups[v], [src] * MEMBERS, n, [d_out[r, j].data_ptr() for j in range(MEMBERS)], cap,
-                                  [d_n[r, j].data_ptr() for j in range(MEMBERS)])
-        step_no[(kind, v)] = k + 1
-
-    def leg_throughput(kind, v, steps):
-        eng.synchronize()
-        t0 = time.perf_counter()
-        done = 0
-        while done < steps:
-            for _ in range(min(args.block, steps - done)):
-                push_device(kind, v)
-            done += min(args.block, steps - done)
-            eng.synchronize()
-        return steps / (time.perf_counter() - t0)
-
+    push = device_pusher(eng, d_in, eng.session_io_geometry(sessions['off'])['max_out'], MEMBERS)
     legs = [(kind, v) for kind in ('single', 'group') for v in VARIANTS]
-    for leg in legs:
-        leg_throughput(*leg, args.warmup)
-    res = {leg: [] for leg in legs}
-    for _ in range(args.repeats):
-        for leg in legs:
-            res[leg].append(leg_throughput(*leg, args.steps))
+
+    def leg(kind_v, steps):
+        kind, v = kind_v
+        target = sessions[v] if kind == 'single' else groups[v]
+        return throughput(eng, lambda: push(target, group=kind == 'group'), steps, args.block)
+    res = alternate(legs, leg, args.steps, args.warmup, args.repeats)
     meters = {v: eng.session_pitch_stats(sessions[v]) for v in VARIANTS if v != 'off'}
 
     # kernel time: one profiler window over the session with the correction
-    from torch.profiler import ProfilerActivity, profile
     profiled = [v for v in VARIANTS if v != 'off']
-    eng.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+
+    def profiled_steps():
         for v in profiled:
             for _ in range(args.profile_steps):
-                push_device('single', v)
+                push(sessions[v])
             eng.synchronize()
-    trace = tmp / 'trace.json'
-    prof.export_chrome_trace(str(trace))
-    ev = json.loads(trace.read_text())
-    ev = ev['traceEvents'] if isinstance(ev, dict) else ev
-    kern = sorted((e for e in ev if e.get('cat') == 'kernel' and e.get('ph') == 'X'), key=lambda e: e['ts'])
-    pitch_us = [e['dur'] for e in kern if KERNEL in e['name']]
+    pitch_us = kernel_durations(eng, tmp, profiled_steps, [KERNEL])[KERNEL]
     kernels = {}
     for i, v in enumerate(profiled):
         d = pitch_us[i * args.profile_steps:(i + 1) * args.profile_steps]
@@ -141,13 +83,9 @@ def main(argv=None):
 
     line = dict(card=card(), buffer_time=T, extras=EXTRA, members=MEMBERS, settings=SETTINGS, steps=args.steps, block=args.block,
                 warmup=args.warmup, repeats=args.repeats,
-                legs={f'{kind}_{v}': dict(steps_per_s=statistics.median(res[(kind, v)]), steps_per_s_all=res[(kind, v)])
-                      for kind, v in legs},
+                legs={f'{kind}_{v}': dict(steps_per_s=statistics.median(r), steps_per_s_all=r) for (kind, v), r in res.items()},
                 last_step_meter={v: dict(voiced=m[0], mean_cents=m[1], max_cents=m[2]) for v, m in meters.items()}, kernels=kernels)
-    if args.out is not None:
-        args.out.mkdir(parents=True, exist_ok=True)
-        (args.out / 'bench_pitch.json').write_text(json.dumps(line, indent=1))
-    print(json.dumps(line))
+    emit(args.out, 'bench_pitch', line)
 
 
 if __name__ == '__main__':

@@ -11,8 +11,6 @@ as ryk_snapshot_last_times measures them, beside the 300 ms chunk period.  The c
     python bench_session_move.py [--out DIR] [--steps 20 --warmup 2 --repeats 10]
 
 Prints one JSON line (and writes it to DIR/bench_session_move.json with --out).  Needs a CUDA device; there is no CPU path."""
-import argparse
-import json
 import statistics
 import tempfile
 import time
@@ -21,16 +19,7 @@ from pathlib import Path
 
 import numpy as np
 
-from bench_f0_control import EXTRA, FS, T, card
-
-
-def make_parser():
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--out', type=Path, default=None)
-    ap.add_argument('--steps', type=int, default=20)
-    ap.add_argument('--warmup', type=int, default=2)
-    ap.add_argument('--repeats', type=int, default=10)
-    return ap
+from benchlib import FS, T, bench_parser, card, emit, headline_config, require_cuda, synthetic_voice
 
 
 def _stats(xs):
@@ -38,28 +27,19 @@ def _stats(xs):
 
 
 def main(argv=None):
-    args = make_parser().parse_args(argv)
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit('bench_session_move.py needs a CUDA device')
+    args = bench_parser(steps=20, warmup=2, repeats=10).parse_args(argv)
+    require_cuda('bench_session_move.py')
     from realtime_yukarin_b200 import synthetic
-    from realtime_yukarin_b200.engine import Engine, SessionConfig, describe_snapshot
-    from realtime_yukarin_b200.models import load_voice
+    from realtime_yukarin_b200.engine import Engine, describe_snapshot
 
     tmp = Path(tempfile.mkdtemp(prefix='bench_session_move_'))     # synthetic model files: never written into the tree
-    paths = synthetic.write_synthetic_models(tmp / 'v0', seed=0)
-    keys = ('stage1_model_path', 'stage2_model_path', 'input_statistics_path', 'target_statistics_path')
     engines = []
     for _ in range(2):
         e = Engine()
         e.set_precision('fp16')
-        v = e.voice_create()
-        load_voice(e, v, **{k: paths[k] for k in keys})
-        engines.append((e, v))
+        engines.append((e, synthetic_voice(e, tmp)))
     src, voice = engines[0]
-    cfg = SessionConfig(fs=FS, frame_period_ms=5.0, f0_floor=71.0, f0_ceil=800.0, fft_length=1024, order=8, alpha=0.466, buffer_time=T,
-                        encode_extra_time=EXTRA[0], convert_extra_time=EXTRA[1], decode_extra_time=EXTRA[2], threshold_db=60.0,
-                        vocoder_buffer_size=1024)
+    cfg = headline_config()
     n = round(T * FS)
     x = synthetic.synthetic_speech((args.steps + 1) * T, stream=3)
     far = synthetic.synthetic_speech((args.steps + 1) * T, stream=4) * 0.5
@@ -101,11 +81,7 @@ def main(argv=None):
                     t[k].append(v)
         result[name] = {k: _stats(v) for k, v in t.items()}
         result[name]['move_over_chunk'] = (statistics.median(t['snapshot_wall']) + statistics.median(t['restore_wall'])) / (T * 1000)
-    line = json.dumps(result)
-    print(line)
-    if args.out:
-        args.out.mkdir(parents=True, exist_ok=True)
-        (args.out / 'bench_session_move.json').write_text(line + '\n')
+    emit(args.out, 'bench_session_move', result)
 
 
 if __name__ == '__main__':

@@ -15,11 +15,9 @@ it) and the Cout = 1 kernel is the last layer.  The card's name, power limit and
 
 Writes DIR/bench_stages.json, DIR/bench_stages.md and the profiler traces, and prints the markdown.  Needs a CUDA device.  RYK_LIB
 selects another build of the library (engine.py), so two builds can be profiled by the same script."""
-import argparse
 import json
 import os
 import re
-import subprocess
 import tempfile
 from collections import defaultdict
 from pathlib import Path
@@ -29,7 +27,10 @@ os.environ.setdefault('CUDA_DEVICE_MAX_CONNECTIONS', '32')
 
 import numpy as np  # noqa: E402
 
-T, EXTRA, FS = 0.3, (0.0, 0.5, 0.0), 24000
+from benchlib import (FS, T, bench_parser, card, device_chunks, device_pusher, headline_config, kernel_events,  # noqa: E402
+                      require_cuda, stopwatch_ms, synthetic_builtin)
+
+CARD_FIELDS = 'name,power.limit,clocks.max.sm,clocks.sm'      # the SM clock too, read before and after the run
 STAGES = ['gate_slides', 'world_analysis', 'stage1', 'stage2', 'synthesis']
 # a stream's stage = the first of these whose kernel-name pattern occurs on it
 STREAM_ROLES = [
@@ -42,27 +43,16 @@ STREAM_ROLES = [
 REPORTED = ('gate_slides', 'world_analysis', 'stage1')
 
 
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm,clocks.sm', '--format=csv,noheader'],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else 'unknown (nvidia-smi unavailable)'
-
-
 def short_name(name):
     n = name.split('(')[0] if '(' in name else name
     n = re.sub(r'^void\s+', '', n).replace('ryk::', '').replace('(anonymous namespace)::', '')
     return n.strip()
 
 
-def kernels_of(trace_path):
-    """[(stream, name, ts_us, dur_us)] of the CUDA kernels in a chrome trace written by torch.profiler."""
-    ev = json.loads(Path(trace_path).read_text())
-    ev = ev['traceEvents'] if isinstance(ev, dict) else ev
-    out = []
-    for e in ev:
-        if e.get('cat') == 'kernel' and e.get('ph') == 'X':
-            out.append((e.get('args', {}).get('stream', e.get('tid')), short_name(e['name']), float(e['ts']), float(e['dur'])))
-    return out
+def kernels_of(prof, trace_path):
+    """[(stream, name, ts_us, dur_us)] of the CUDA kernels of a torch.profiler window, through the chrome trace written to trace_path."""
+    return [(e.get('args', {}).get('stream', e.get('tid')), short_name(e['name']), float(e['ts']), float(e['dur']))
+            for e in kernel_events(prof, trace_path)]
 
 
 def stream_roles(kernels):
@@ -125,66 +115,48 @@ def spans(kernels):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--out', type=Path, required=True)
-    ap.add_argument('--steps', type=int, default=40)
-    ap.add_argument('--warmup', type=int, default=10)
-    ap.add_argument('--isolated', type=int, default=8)
+    ap = bench_parser(required_out=True, steps=40, warmup=10, isolated=8)
     ap.add_argument('--f0', default='dio', choices=['dio', 'harvest'])
     args = ap.parse_args()
+    require_cuda('bench_stages.py')
     import torch
     from torch.profiler import ProfilerActivity, profile
-    if not torch.cuda.is_available():
-        raise SystemExit('bench_stages.py needs a CUDA device')
     from realtime_yukarin_b200 import synthetic
-    from realtime_yukarin_b200.engine import Engine, SessionConfig
-    from realtime_yukarin_b200.models import AcousticConverter, F0Converter, SuperResolution
-    from realtime_yukarin_b200.params import create_from_json, create_sr_from_json
+    from realtime_yukarin_b200.engine import Engine
 
     args.out.mkdir(parents=True, exist_ok=True)
     tmp = Path(tempfile.mkdtemp(prefix='bench_stages_'))       # synthetic model files: never written into the tree
-    paths = synthetic.write_synthetic_models(tmp, seed=0)
     eng = Engine()
-    f0c = F0Converter(paths['input_statistics_path'], paths['target_statistics_path'])
-    AcousticConverter(create_from_json(paths['stage1_config_path']), paths['stage1_model_path'], f0_converter=f0c, engine=eng)
-    SuperResolution(create_sr_from_json(paths['stage2_config_path']), paths['stage2_model_path'], engine=eng)
+    synthetic_builtin(eng, tmp)
     eng.set_precision('fp16')
     eng.set_f0_method(args.f0)
-    cfg = SessionConfig(fs=FS, frame_period_ms=5.0, f0_floor=71.0, f0_ceil=800.0, fft_length=1024, order=8, alpha=0.466, buffer_time=T,
-                        encode_extra_time=EXTRA[0], convert_extra_time=EXTRA[1], decode_extra_time=EXTRA[2], threshold_db=60.0,
-                        vocoder_buffer_size=1024)
+    cfg = headline_config()
     n = round(T * FS)
     total = args.warmup + max(args.steps, args.isolated)
-    x = synthetic.synthetic_speech((total + 1) * T, stream=0)
-    d_in = torch.from_numpy(np.stack([x[k * n:(k + 1) * n] for k in range(total)]).astype(np.float32)).cuda()
+    d_in = device_chunks(synthetic.synthetic_speech((total + 1) * T, stream=0), n, total)
     out_cap = (n // 1024 + 5) * 1024 + 8192
-    d_out = torch.empty((8, out_cap), dtype=torch.float64, device='cuda')
-    d_n = torch.zeros(8, dtype=torch.int32, device='cuda')
-    card_before = card()
+    card_before = card(CARD_FIELDS)
 
     def fresh_session():
+        """a new session after --warmup steps, and the call that queues its next step"""
         sid = eng.session_create(cfg)
-        for k in range(args.warmup):
-            eng.session_push_device(sid, d_in[k].data_ptr(), n, d_out[k % 8].data_ptr(), out_cap, d_n[k % 8:].data_ptr())
+        push = device_pusher(eng, d_in, out_cap)
+        for _ in range(args.warmup):
+            push(sid)
         eng.synchronize()
         torch.cuda.synchronize()
-        return sid
-
-    def push(sid, k):
-        eng.session_push_device(sid, d_in[k].data_ptr(), n, d_out[k % 8].data_ptr(), out_cap, d_n[k % 8:].data_ptr())
+        return sid, lambda: push(sid)
 
     acts = [ProfilerActivity.CPU, ProfilerActivity.CUDA]
     # ---- isolated steps ----
-    sid = fresh_session()
+    sid, step = fresh_session()
     iso_kernels, iso_spans = [], defaultdict(list)
     for i in range(args.isolated):
         with profile(activities=acts) as prof:
-            push(sid, args.warmup + i)
+            step()
             eng.synchronize()
             torch.cuda.synchronize()
-        tp = args.out / f'trace_isolated_{i}.json'
-        prof.export_chrome_trace(str(tp))
-        ks = kernels_of(tp)
+        ks = kernels_of(prof, args.out / f'trace_isolated_{i}.json')
         iso_kernels += ks
         for r, v in spans(ks).items():
             iso_spans[r].append(v)
@@ -193,31 +165,26 @@ def main():
     iso_layers = per_layer(iso_kernels, args.isolated)
 
     # ---- pipelined steps ----
-    sid = fresh_session()
+    sid, step = fresh_session()
     with profile(activities=acts) as prof:
-        for k in range(args.warmup, args.warmup + args.steps):
-            push(sid, k)
+        for _ in range(args.steps):
+            step()
         eng.synchronize()
         torch.cuda.synchronize()
-    tp = args.out / 'trace_pipelined.json'
-    prof.export_chrome_trace(str(tp))
-    pipe_kernels = kernels_of(tp)
+    pipe_kernels = kernels_of(prof, args.out / 'trace_pipelined.json')
     pipe_table, pipe_totals = per_kernel(pipe_kernels, args.steps)
     pipe_layers = per_layer(pipe_kernels, args.steps)
     eng.session_destroy(sid)
 
     # ---- stage timeline, profiler off ----
-    sid = fresh_session()
-    eng.timer_start()
-    for k in range(args.warmup, args.warmup + args.steps):
-        push(sid, k)
-    ms = eng.timer_stop()
+    sid, step = fresh_session()
+    ms = stopwatch_ms(eng, step, 0, args.steps)
     st, en = eng.session_stage_times(sid)
     eng.session_destroy(sid)
     # gate of step k against the end of stage 1 of step k-2 (> 0: the gate started after it)
     gate_vs_s1 = [float(st[i, 0] - en[i - 2, 2]) for i in range(2, len(st))]
 
-    res = dict(card=card_before, card_after=card(), f0=args.f0, steps=args.steps, warmup=args.warmup, isolated=args.isolated,
+    res = dict(card=card_before, card_after=card(CARD_FIELDS), f0=args.f0, steps=args.steps, warmup=args.warmup, isolated=args.isolated,
                lib=os.environ.get('RYK_LIB', 'realtime_yukarin_b200/csrc/libryk.so'),
                isolated_us=iso_table, isolated_stage_us=iso_totals,
                isolated_stage_span_us={r: float(np.mean(v)) for r, v in iso_spans.items()},

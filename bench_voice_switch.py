@@ -13,8 +13,6 @@ extras 0 / 0.5 / 0, full-width (base 64) synthetic voices.
     python bench_voice_switch.py [--out DIR] [--switches 24 --steps 400 --repeats 3]
 
 Prints one JSON line (and writes it to DIR/bench_voice_switch.json with --out).  Needs a CUDA device; there is no CPU path."""
-import argparse
-import json
 import shutil
 import statistics
 import tempfile
@@ -23,16 +21,8 @@ from pathlib import Path
 
 import numpy as np
 
-from bench_f0_control import EXTRA, FS, T, card
-
-
-def make_parser():
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--out', type=Path, default=None)
-    ap.add_argument('--switches', type=int, default=24)
-    ap.add_argument('--steps', type=int, default=400)
-    ap.add_argument('--repeats', type=int, default=3)
-    return ap
+from benchlib import (EXTRA, FS, RING, T, alternate, bench_parser, card, device_chunks, emit, headline_config, output_ring,
+                      require_cuda, synthetic_voice)
 
 
 def _ms(xs):
@@ -40,32 +30,22 @@ def _ms(xs):
 
 
 def main(argv=None):
-    args = make_parser().parse_args(argv)
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit('bench_voice_switch.py needs a CUDA device')
+    args = bench_parser(switches=24, steps=400, repeats=3).parse_args(argv)
+    require_cuda('bench_voice_switch.py')
     from realtime_yukarin_b200 import synthetic
-    from realtime_yukarin_b200.engine import Engine, SessionConfig
-    from realtime_yukarin_b200.models import load_voice
+    from realtime_yukarin_b200.engine import Engine
 
     tmp = Path(tempfile.mkdtemp(prefix='bench_voice_switch_'))      # synthetic model files: never written into the tree
     eng = Engine()
     eng.set_precision('fp16')
-    voices = []
-    for seed in (0, 1, 2):
-        paths = synthetic.write_synthetic_models(tmp / f'v{seed}', seed=seed)
-        voices.append(eng.voice_create())
-        load_voice(eng, voices[-1], **{k: paths[k] for k in ('stage1_model_path', 'stage2_model_path', 'input_statistics_path',
-                                                              'target_statistics_path')})
+    voices = [synthetic_voice(eng, tmp, seed) for seed in (0, 1, 2)]
     va, vb, vc = voices
-    cfg = SessionConfig(fs=FS, frame_period_ms=5.0, f0_floor=71.0, f0_ceil=800.0, fft_length=1024, order=8, alpha=0.466, buffer_time=T,
-                        encode_extra_time=EXTRA[0], convert_extra_time=EXTRA[1], decode_extra_time=EXTRA[2], threshold_db=60.0,
-                        vocoder_buffer_size=1024)
+    cfg = headline_config()
     n = round(T * FS)
     n_chunks = 64
     x = synthetic.synthetic_speech((n_chunks + 1) * T, stream=0)
     chunks = [np.ascontiguousarray(x[k * n:(k + 1) * n], np.float32) for k in range(n_chunks)]
-    d_in = torch.from_numpy(np.stack(chunks)).cuda()
+    d_in = device_chunks(x, n, n_chunks)
 
     # ---- call: alone and as a group member ----
     sid = eng.session_create(cfg, voice=va)
@@ -94,9 +74,7 @@ def main(argv=None):
     # ---- stream: switching every 10 steps vs never ----
     sids = {'never': eng.session_create(cfg, voice=va), 'every_10': eng.session_create(cfg, voice=va)}
     cap = eng.session_io_geometry(sids['never'])['max_out']
-    ring = 8
-    d_out = torch.empty((ring, cap), dtype=torch.float64, device='cuda')
-    d_n = torch.zeros((ring, 1), dtype=torch.int32, device='cuda')
+    d_out, d_n = output_ring(cap)
     step_no = {v: 0 for v in sids}
 
     def leg(v, steps):
@@ -107,18 +85,12 @@ def main(argv=None):
             k = step_no[v]
             if v == 'every_10' and k % 10 == 0 and k:
                 eng.session_set_voice(sids[v], vb if (k // 10) % 2 else va)
-            eng.session_push_device(sids[v], d_in[k % n_chunks].data_ptr(), n, d_out[k % ring].data_ptr(), cap, d_n[k % ring].data_ptr())
+            eng.session_push_device(sids[v], d_in[k % n_chunks].data_ptr(), n, d_out[k % RING, 0].data_ptr(), cap,
+                                    d_n[k % RING, 0].data_ptr())
             step_no[v] = k + 1
         eng.synchronize()
         return steps / (time.perf_counter() - t0), (eng.launch_count - launches0) / steps
-    for v in sids:
-        leg(v, 40)
-    rates = {v: [] for v in sids}
-    kernels = {}
-    for _ in range(args.repeats):
-        for v in sids:
-            r, kernels[v] = leg(v, args.steps)
-            rates[v].append(r)
+    res = alternate(list(sids), leg, args.steps, 40, args.repeats)
     for s in sids.values():
         eng.session_destroy(s)
 
@@ -138,15 +110,13 @@ def main(argv=None):
         eng.voice_destroy(v)
     shutil.rmtree(tmp, ignore_errors=True)
     steady = [t for i in range(5, 20) for t in after[i]]
+    rates = {v: [r for r, _ in res[v]] for v in sids}
     line = dict(card=card(), buffer_time=T, extras=EXTRA, switches=args.switches, steps=args.steps, repeats=args.repeats,
                 call=dict(alone=_ms(alone), group_member_of_8=_ms(grouped)),
-                stream={v: dict(steps_per_s=statistics.median(rates[v]), steps_per_s_all=rates[v], kernels_per_step=kernels[v])
+                stream={v: dict(steps_per_s=statistics.median(rates[v]), steps_per_s_all=rates[v], kernels_per_step=res[v][-1][1])
                         for v in sids},
                 latency=dict(**{f'step_{i}_after': _ms(after[i]) for i in range(3)}, steady=_ms(steady)))
-    if args.out is not None:
-        args.out.mkdir(parents=True, exist_ok=True)
-        (args.out / 'bench_voice_switch.json').write_text(json.dumps(line, indent=1))
-    print(json.dumps(line))
+    emit(args.out, 'bench_voice_switch', line)
 
 
 if __name__ == '__main__':

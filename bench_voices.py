@@ -11,24 +11,16 @@ the stage-2 weight bytes one forward streams at FP16 for V voices.  The card's n
     python bench_voices.py [--out DIR] [--steps 60 --warmup 10 --rounds 3]
 
 Prints one JSON line (and writes it to DIR/bench_voices.json with --out).  Needs a CUDA device; there is no CPU path."""
-import argparse
-import json
 import shutil
 import statistics
-import subprocess
 import tempfile
 from pathlib import Path
 
-import numpy as np
+from benchlib import (EXTRA, FS, bench_parser, card, device_chunks, device_pusher, emit, headline_config, require_cuda, stopwatch_ms,
+                      synthetic_voice)
 
-EXTRA, FS = (0.0, 0.5, 0.0), 24000
 GROUPS = [(8, 1.0), (4, 0.3)]
 VOICES = [1, 2, 4, 8]
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'], capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else 'unknown (nvidia-smi unavailable)'
 
 
 def stage2_weight_bytes(base=64):
@@ -38,60 +30,29 @@ def stage2_weight_bytes(base=64):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--out', type=Path, default=None)
-    ap.add_argument('--steps', type=int, default=60)
-    ap.add_argument('--warmup', type=int, default=10)
-    ap.add_argument('--rounds', type=int, default=3)
-    args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit('bench_voices.py needs a CUDA device')
+    args = bench_parser(steps=60, warmup=10, rounds=3).parse_args()
+    require_cuda('bench_voices.py')
     from realtime_yukarin_b200 import synthetic
-    from realtime_yukarin_b200.engine import Engine, SessionConfig
-    from realtime_yukarin_b200.models import load_voice
+    from realtime_yukarin_b200.engine import Engine
 
     tmp = Path(tempfile.mkdtemp(prefix='bench_voices_'))       # synthetic model files: never written into the tree
     eng = Engine()
     eng.set_precision('fp16')
-    voices = []
-    for seed in range(max(VOICES)):
-        paths = synthetic.write_synthetic_models(tmp / f'v{seed}', seed=seed)
-        v = eng.voice_create()
-        load_voice(eng, v, **{k: paths[k] for k in ('stage1_model_path', 'stage2_model_path', 'input_statistics_path', 'target_statistics_path')})
-        voices.append(v)
+    voices = [synthetic_voice(eng, tmp, seed) for seed in range(max(VOICES))]
     total = args.warmup + 2 * args.steps
     chunks = {}
     for _, T in GROUPS:
-        n = round(T * FS)
-        x = synthetic.synthetic_speech((total + 1) * T, stream=0)
-        chunks[T] = torch.from_numpy(np.stack([x[k * n:(k + 1) * n] for k in range(total)])).cuda()
+        chunks[T] = device_chunks(synthetic.synthetic_speech((total + 1) * T, stream=0), round(T * FS), total)
 
     def leg(members, T, n_voices):
-        cfg = SessionConfig(fs=FS, frame_period_ms=5.0, f0_floor=71.0, f0_ceil=800.0, fft_length=1024, order=8, alpha=0.466, buffer_time=T,
-                            encode_extra_time=EXTRA[0], convert_extra_time=EXTRA[1], decode_extra_time=EXTRA[2], threshold_db=60.0,
-                            vocoder_buffer_size=1024)
-        sids = [eng.session_create(cfg, voice=voices[i % n_voices]) for i in range(members)]
+        sids = [eng.session_create(headline_config(buffer_time=T), voice=voices[i % n_voices]) for i in range(members)]
         gid = eng.group_create(sids)
-        g = eng.session_io_geometry(sids[0])
-        d_in = chunks[T]
-        d_out = torch.empty((members, 8, g['max_out']), dtype=torch.float64, device='cuda')
-        d_n = torch.zeros((members, 8), dtype=torch.int32, device='cuda')
-
-        def push(k):
-            eng.group_push_device(gid, [d_in[k].data_ptr()] * members, g['n_in'], [d_out[i, k % 8].data_ptr() for i in range(members)],
-                                  g['max_out'], [d_n[i, k % 8:].data_ptr() for i in range(members)])
-        for k in range(args.warmup):
-            push(k)
-        eng.synchronize()
-        eng.timer_start()
-        for k in range(args.warmup, args.warmup + args.steps):
-            push(k)
-        ms = eng.timer_stop()
+        push = device_pusher(eng, chunks[T], eng.session_io_geometry(sids[0])['max_out'], members)
+        ms = stopwatch_ms(eng, lambda: push(gid, group=True), args.warmup, args.steps)
         eng.profile_read2()                       # drop events of earlier forwards
         eng.profile(True)
-        for k in range(args.warmup + args.steps, total):
-            push(k)
+        for _ in range(args.steps):
+            push(gid, group=True)
         s2_total, _, runs = eng.profile_read2()
         eng.profile(False)
         eng.group_destroy(gid)
@@ -118,10 +79,7 @@ def main():
     for v in voices:
         eng.voice_destroy(v)
     shutil.rmtree(tmp, ignore_errors=True)
-    if args.out is not None:
-        args.out.mkdir(parents=True, exist_ok=True)
-        (args.out / 'bench_voices.json').write_text(json.dumps(line, indent=1))
-    print(json.dumps(line))
+    emit(args.out, 'bench_voices', line)
 
 
 if __name__ == '__main__':

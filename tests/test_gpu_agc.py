@@ -23,7 +23,7 @@ from . import denoise_oracle as DO
 from . import echo_oracle as E
 from .test_gpu_f0_control import (EXTRA, FS, N, T, _cfg, _new_voice, _push, _same, made,  # noqa: F401
                                   second_voice_files)
-from .test_gpu_launch_count import _window
+from .test_gpu_launch_count import _run_child, _window
 from .test_gpu_parity import _load
 
 pytestmark = pytest.mark.gpu
@@ -239,12 +239,10 @@ def test_group_members_and_voice_switches_keep_the_agc(engine, made, full_models
 
 # ---- 6 ------------------------------------------------------------------------------------------------------------------------
 def _launch_windows(out_dir):
-    """Child process of the launch-count test: (kernels the profiler saw, change of engine.launch_count) over 12 steps of a plain session
-    fed the whole-signal output (the same kernels downstream), of a session with the AGC fed the input, and of a plain one after it,
-    written to out_dir / counts.json."""
-    import json
+    """Child process of the launch-count test: returns (kernels the profiler saw, change of engine.launch_count) over 12 steps of a
+    plain session fed the whole-signal output (the same kernels downstream), of a session with the AGC fed the input, and of a plain
+    one after it."""
     from realtime_yukarin_b200.engine import default_engine
-    out_dir = Path(out_dir)
     engine = default_engine()
     _load(engine, synthetic.write_synthetic_models(out_dir / 'models', seed=0))
     engine.set_precision('fp16')
@@ -258,21 +256,11 @@ def _launch_windows(out_dir):
             engine.session_agc(sid)
         counts[name] = _window(engine, out_dir, lambda: _push(engine, sid, chunks))
         engine.session_destroy(sid)
-    (out_dir / 'counts.json').write_text(json.dumps(counts))
+    return counts
 
 
 def test_one_kernel_per_step_and_none_for_other_sessions(tmp_path):
-    # torch.profiler runs in a process of its own, as in tests/test_gpu_denoise.py
-    import json
-    import os
-    import subprocess
-    import sys
-    root = Path(__file__).resolve().parent.parent
-    flags = ['-s'] if sys.flags.no_user_site else []
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([str(root)] + [p for p in [os.environ.get('PYTHONPATH')] if p]))
-    subprocess.run([sys.executable, *flags, '-c', f'from tests.test_gpu_agc import _launch_windows; _launch_windows({str(tmp_path)!r})'],
-                   cwd=root, env=env, check=True, timeout=900)
-    counts = json.loads((tmp_path / 'counts.json').read_text())
+    counts = _run_child(tmp_path, 'test_gpu_agc', '_launch_windows')
     for name, (seen, counted) in counts.items():
         print(f'{name}: {counted} kernels counted over 12 steps, {seen} seen by the profiler')
         assert seen == counted, name

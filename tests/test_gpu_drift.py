@@ -8,11 +8,6 @@
   * one kernel per push; refusals change nothing; create / destroy cycles return memory.
 """
 import functools
-import json
-import os
-import subprocess
-import sys
-from pathlib import Path
 
 import numpy as np
 import pytest
@@ -22,6 +17,7 @@ from realtime_yukarin_b200.engine import Engine, RykError, describe_snapshot
 
 from . import drift_oracle as D
 from .test_gpu_f0_control import EXTRA, FS, T
+from .test_gpu_launch_count import _kernel_events, _run_child
 
 pytestmark = pytest.mark.gpu
 
@@ -223,10 +219,9 @@ def _other_engine_with_models(full_models):
 
 # ---- 5 --------------------------------------------------------------------------------------------------------------------------
 def _launch_window(out_dir):
-    """Child process of the launch test: the kernels the profiler saw over 12 pushes, written to out_dir / kernels.json."""
+    """Child process of the launch test: returns the names of the kernels the profiler saw over 12 pushes."""
     from torch.profiler import ProfilerActivity, profile
     from realtime_yukarin_b200.engine import default_engine
-    out_dir = Path(out_dir)
     engine = default_engine()
     did = engine.drift_create(14400, 500.0)
     engine.drift_set(did, 250.0)
@@ -237,22 +232,11 @@ def _launch_window(out_dir):
         for k in range(1, 13):
             engine.drift_push(did, x[k * 14400:(k + 1) * 14400])
         engine.synchronize()
-    path = out_dir / 'trace.json'
-    prof.export_chrome_trace(str(path))
-    ev = json.loads(path.read_text())
-    ev = ev['traceEvents'] if isinstance(ev, dict) else ev
-    names = [e['name'] for e in ev if e.get('cat') == 'kernel' and e.get('ph') == 'X']
-    (out_dir / 'kernels.json').write_text(json.dumps(names))
+    return [e['name'] for e in _kernel_events(prof, out_dir / 'trace.json')]
 
 
 def test_one_kernel_per_push(tmp_path):
-    # torch.profiler runs in a process of its own, as in tests/test_gpu_limiter.py
-    root = Path(__file__).resolve().parent.parent
-    flags = ['-s'] if sys.flags.no_user_site else []
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([str(root)] + [p for p in [os.environ.get('PYTHONPATH')] if p]))
-    subprocess.run([sys.executable, *flags, '-c', f'from tests.test_gpu_drift import _launch_window; _launch_window({str(tmp_path)!r})'],
-                   cwd=root, env=env, check=True, timeout=900)
-    names = json.loads((tmp_path / 'kernels.json').read_text())
+    names = _run_child(tmp_path, 'test_gpu_drift', '_launch_window')
     print(f'kernels over 12 pushes: {len(names)}')
     assert len(names) == 12 and all('k_drift' in s for s in names)
 

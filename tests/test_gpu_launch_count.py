@@ -3,6 +3,10 @@ run, which include the kernels inside the stage graphs and the stage-1 SWITCH bo
 covers the first (capturing) launch of every stage graph and the synthesizer's noise top-up.  No torch CUDA work runs inside a window:
 every kernel in it belongs to the steps."""
 import json
+import os
+import subprocess
+import sys
+from pathlib import Path
 
 import numpy as np
 import pytest
@@ -29,6 +33,14 @@ def _speech(steps, stream, rate=FS):
     return [np.ascontiguousarray(x[k * n:(k + 1) * n]) for k in range(steps)]
 
 
+def _kernel_events(prof, path):
+    """the CUDA kernel events of a finished torch.profiler window, read back from the chrome trace it writes to path"""
+    prof.export_chrome_trace(str(path))
+    ev = json.loads(path.read_text())
+    ev = ev['traceEvents'] if isinstance(ev, dict) else ev
+    return [e for e in ev if e.get('cat') == 'kernel' and e.get('ph') == 'X']
+
+
 def _window(engine, tmp_path, run):
     """(CUDA kernels the profiler saw, change of engine.launch_count) over run()"""
     from torch.profiler import ProfilerActivity, profile
@@ -37,12 +49,23 @@ def _window(engine, tmp_path, run):
         run()
         engine.synchronize()
     counted = engine.launch_count - before
-    path = tmp_path / 'trace.json'
-    prof.export_chrome_trace(str(path))
-    ev = json.loads(path.read_text())
-    ev = ev['traceEvents'] if isinstance(ev, dict) else ev
-    seen = sum(1 for e in ev if e.get('cat') == 'kernel' and e.get('ph') == 'X')
-    return seen, counted
+    return len(_kernel_events(prof, tmp_path / 'trace.json')), counted
+
+
+def _run_child(tmp_path, module, function):
+    """function(tmp_path) of tests/<module>.py run in a Python process of its own; returns what it returned, through JSON.
+
+    Tests that profile outside this module do it this way: CUPTI's teardown and re-initialisation between profiling sessions is not
+    reliable in a process that runs CUDA graphs (torch's profiler says as much), and this module's tests expect to be the first
+    profiling in their process."""
+    root = Path(__file__).resolve().parent.parent
+    flags = ['-s'] if sys.flags.no_user_site else []
+    env = dict(os.environ, PYTHONPATH=os.pathsep.join([str(root)] + [p for p in [os.environ.get('PYTHONPATH')] if p]))
+    out = tmp_path / 'result.json'
+    code = (f'import json, pathlib; from tests.{module} import {function}; '
+            f'pathlib.Path({str(out)!r}).write_text(json.dumps({function}(pathlib.Path({str(tmp_path)!r}))))')
+    subprocess.run([sys.executable, *flags, '-c', code], cwd=root, env=env, check=True, timeout=900)
+    return json.loads(out.read_text())
 
 
 def _session_window(engine, tmp_path, chunks, in_rate=None, out_rate=None, f0_method='dio'):

@@ -20,7 +20,7 @@ from realtime_yukarin_b200.engine import RykError
 from . import limiter_oracle as LO
 from .test_gpu_f0_control import (EXTRA, FS, N, T, _cfg, _new_voice, _push, _same, _speech, made,  # noqa: F401
                                   second_voice_files)
-from .test_gpu_launch_count import _window
+from .test_gpu_launch_count import _run_child, _window
 from .test_gpu_parity import _load
 
 pytestmark = pytest.mark.gpu
@@ -231,11 +231,9 @@ def test_group_members_and_voice_switches_keep_the_limiter(engine, made, full_mo
 
 # ---- 5 ------------------------------------------------------------------------------------------------------------------------
 def _launch_windows(out_dir):
-    """Child process of the launch-count test: (kernels the profiler saw, change of engine.launch_count) over 12 steps of a plain
-    session, a limited one, and a plain one after the limited one ran on the same engine, written to out_dir / counts.json."""
-    import json
+    """Child process of the launch-count test: returns (kernels the profiler saw, change of engine.launch_count) over 12 steps of a plain
+    session, a limited one, and a plain one after the limited one ran on the same engine."""
     from realtime_yukarin_b200.engine import default_engine
-    out_dir = Path(out_dir)
     engine = default_engine()
     _load(engine, synthetic.write_synthetic_models(out_dir / 'models', seed=0))
     engine.set_precision('fp16')
@@ -251,21 +249,11 @@ def _launch_windows(out_dir):
             engine.session_set_limiter(sid, -1.0, 50.0)
         counts[name] = _window(engine, out_dir, lambda: _push(engine, sid, chunks))
         engine.session_destroy(sid)
-    (out_dir / 'counts.json').write_text(json.dumps(counts))
+    return counts
 
 
 def test_three_kernels_per_step_and_none_for_other_sessions(tmp_path):
-    # torch.profiler runs in a process of its own, as in tests/test_gpu_echo.py
-    import json
-    import os
-    import subprocess
-    import sys
-    root = Path(__file__).resolve().parent.parent
-    flags = ['-s'] if sys.flags.no_user_site else []
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([str(root)] + [p for p in [os.environ.get('PYTHONPATH')] if p]))
-    subprocess.run([sys.executable, *flags, '-c', f'from tests.test_gpu_limiter import _launch_windows; _launch_windows({str(tmp_path)!r})'],
-                   cwd=root, env=env, check=True, timeout=900)
-    counts = json.loads((tmp_path / 'counts.json').read_text())
+    counts = _run_child(tmp_path, 'test_gpu_limiter', '_launch_windows')
     for name, (seen, counted) in counts.items():
         print(f'{name}: {counted} kernels counted over 12 steps, {seen} seen by the profiler')
         assert seen == counted, name
